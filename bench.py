@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — the hot path of BASELINE.json on B200: rows/s and fraction of HBM roofline, filter AND aggregate.
+"""bench.py — the hot path of BASELINE.json on H100: rows/s and fraction of HBM roofline, filter AND aggregate.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--rows R]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--rows R] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Headline workload (BASELINE.json configs[1], "C2"): SELECT a FROM t WHERE a > 0.5 over 1e8 synthetic Float64
@@ -18,14 +18,23 @@ next to it (`roofline_c4`, `e2e_c4`, `cpu_baseline_c4`); C3 and C5 are in `extra
                 by row-range chunk inside the library
   roofline      algorithmic bytes of the dominant kernel (8*N read + 8*N_sel written) / its average duration
                 measured with CUDA events recorded around the launch on the launching stream
-  sustained     the same resident step repeated back to back for >= 0.5 s (the K timed steps of C2 last a few ms)
   roofline_c4   the same for k_hash_agg (16*N bytes read), e2e_c4 through dfgpu_aggregate_update_host
   extra         C3 (fused expr+filter) and C5 (1e6 keys, MIN/MAX/SUM, 1.25e8 rows per GPU = 1e9 rows on 8 GPUs;
                 with N>1 C4 and C5 include the NCCL partial-aggregate merge), same timing rules
-  checks        every aggregate result (also the merged multi-GPU one, on every rank) is compared with numpy /
-                torch on the same rows: key set, COUNT, MIN, MAX bit-exact, SUM within 1e-9; a mismatch fails the run
+  checks        every aggregate result of the last timed step (also the merged multi-GPU one, on every rank) is
+                compared with numpy / torch on the same rows: key set, COUNT, MIN, MAX bit-exact, SUM within 1e-9;
+                a mismatch fails the run
   cpu_baseline  the CPU oracle (C++ restatement of the reference's single-threaded operators) on a bounded
                 sample of the same workload, on this box's host cores (rank 0, N=1 only)
+
+Every timed leg runs exactly W untimed warm-up steps and then exactly K timed steps.
+
+--dump-outputs DIR writes (rank 0) what the last timed step of each leg returned, as DIR/<name>.npy:
+  c2_a, c3_sum, c3_prod   a fixed sample (seed 7, at most 2^20 rows, ascending row order) of the filter
+                          outputs, float64; c2_nrows / c3_nrows hold the full output row counts
+  c4_sum, c4_count        dense over the raw key index 0 .. nkeys-1 (float64; NaN / 0 where a key is absent)
+  c5_min, c5_max, c5_sum  the same for C5
+Inputs are seeded, so two builds given the same arguments can be compared output for output.
 
 --impl reference times that CPU restatement alone (the reference is Rust; no toolchain here) on the SAME
 config: one full 1e8-row C2 batch per step.
@@ -42,35 +51,18 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+sys.dont_write_bytecode = True  # the tree may be read-only: nothing is written there
 
 METRIC = "rows/s filter+agg over 1e8-row Arrow batch (C2: SELECT a FROM t WHERE a>0.5, Float64)"
 SUM_RTOL = 1e-9
+DUMP_SAMPLE_ROWS = 1 << 20
 
 
 def c2_config(n):
     """The `config` object of both arms (the reference arm must describe exactly what ours measures)."""
     return {"workload": "C2: SELECT a FROM t WHERE a > 0.5; a~U[0,1) Float64, %d rows per GPU, seed 42+rank" % n,
             "rows_per_gpu": n, "partitioning": "row-range, one batch per rank, no collective",
-            "l2": "inputs (%.1f GB per step) larger than L2 (126 MB); no explicit flush" % (8.0 * n / 1e9)}
-
-
-def ncu_traffic(key):
-    """DRAM bytes per launch of the dominant kernel, from the committed ncu capture (profiles/)."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json"))).get(key)
-    except Exception:
-        return None
-
-
-def scatter_ceiling(kernel_ms, n):
-    """C4's second bound: the measured time of its bare scattered-access pattern (profiles/scatter_peak.json)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "scatter_peak.json")) as f:
-            j = json.load(f)
-        floor_ms = j["ldg_red_f64_red_u64_ms_per_1e8_rows"] * n / 1e8
-        return {"bound": "lsu/l2-atomic", "floor_ms": floor_ms, "frac": floor_ms / kernel_ms, "source": j["source"]}
-    except Exception:
-        return None
+            "l2": "inputs (%.1f GB per step) larger than L2 (50 MB); no explicit flush" % (8.0 * n / 1e9)}
 
 
 def hbm_peak():
@@ -80,7 +72,41 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
+
+
+def gpu_info(local):
+    """Name and power limit of the card the numbers were measured on (they belong beside every number)."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(local), "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        name, power, clock = [x.strip() for x in out.split(",")]
+        return {"name": name, "power_limit": power, "sm_max_clock": clock}
+    except Exception:
+        return None
+
+
+def dump_sample(columns, names, out_dir, prefix):
+    """A fixed, seeded sample of equally long filter-output columns (ascending row order) plus the row count."""
+    n = len(columns[0])
+    idx = np.unique(np.random.default_rng(7).integers(0, n, DUMP_SAMPLE_ROWS)) if n > DUMP_SAMPLE_ROWS else np.arange(n)
+    for c, name in zip(columns, names):
+        np.save(os.path.join(out_dir, "%s_%s.npy" % (prefix, name)), np.asarray(c[idx], dtype=np.float64))
+    np.save(os.path.join(out_dir, "%s_nrows.npy" % prefix), np.array([n], dtype=np.float64))
+
+
+def dump_groupby(got, nkeys, want, out_dir, prefix):
+    """A GROUP BY result made dense over the raw key index (the keys are a bijective scramble of 0 .. nkeys-1)."""
+    from datafusion_archive_b200 import workloads
+    mixed = workloads.mix_keys(np.arange(nkeys, dtype=np.int64))
+    order = np.argsort(mixed)
+    pos = np.searchsorted(mixed[order], got[0])
+    raw = order[np.minimum(pos, nkeys - 1)]
+    assert np.array_equal(mixed[raw], got[0]), prefix + ": a result key is not one of the generated keys"
+    for j, name in enumerate(want):
+        dense = np.zeros(nkeys) if name == "count" else np.full(nkeys, np.nan)
+        dense[raw] = got[1 + j]
+        np.save(os.path.join(out_dir, "%s_%s.npy" % (prefix, name)), dense)
 
 
 class ClockSampler:
@@ -151,7 +177,7 @@ class ClockSampler:
             reasons = sorted({nm for _, rs, _ in self.samples for nm, b in bits.items() if rs & b})
             sm = [x[0] for x in self.samples]
             return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": mx, "power_w_max": max([x[2] for x in self.samples], default=None),
-                    "samples": len(sm), "reasons": reasons, "source": "nvml, ~2 ms period, warm-up + timed steps + sustained loop"}
+                    "samples": len(sm), "reasons": reasons, "source": "nvml, ~2 ms period, C2 warm-up + timed steps"}
         if not self.proc:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
@@ -281,6 +307,15 @@ def check_groupby(torch, got, k_raw, v, nkeys, want, what):
             + ("; per-rank partials all-reduced with torch.distributed" if torch is not None else "")}
 
 
+def hold_last(state, key, r):
+    """Keep the result of the latest step and free its predecessor: after the loop, state[key] is what the
+    last timed step returned."""
+    old = state.get(key)
+    if old is not None:
+        old.free()
+    state[key] = r
+
+
 def run_ours(args):
     from datafusion_archive_b200 import engine, workloads
     rank, world, local, torch = dist_setup(args.gpus)
@@ -289,7 +324,10 @@ def run_ours(args):
     ctx = engine.GpuContext(local)
     peak, peak_src = hbm_peak()
     n = args.rows
-    steps, warmup = (args.steps or 2000), max(3, args.warmup)
+    steps, warmup = args.steps, args.warmup
+    dump = args.dump_outputs if rank == 0 else None
+    if dump:
+        os.makedirs(dump, exist_ok=True)
 
     # ---- C2 (headline) -----------------------------------------------------------------------
     pin_in = engine.PinnedBuffer((n,), np.float64)
@@ -300,9 +338,7 @@ def run_ours(args):
     state = {}
 
     def step_resident():
-        r = ctx.filter_project(batch, pred, proj)
-        state["nrows"] = r.nrows
-        r.free()
+        hold_last(state, "r2", ctx.filter_project(batch, pred, proj))
 
     def step_e2e():
         # the call a user of the engine makes for a host-resident batch: host buffers in, host buffers
@@ -315,18 +351,19 @@ def run_ours(args):
     sampler = ClockSampler(local)
     sampler.start()
     ms, kms, kn, launches = time_steps(ctx, torch, step_resident, steps, warmup)
-    assert state["nrows"] == n_sel, "GPU row count %d != expected %d" % (state["nrows"], n_sel)
-    # sustained: the same step back to back for >= 0.5 s (same kernel, clocks sampled throughout)
-    sus_steps = steps if args.no_sustained else max(steps, int(np.ceil(600.0 / max(ms / steps, 1e-3))))
-    sms, skms, skn, _ = time_steps(ctx, torch, step_resident, sus_steps, 0)
     clocks = sampler.stop()
+    r2 = state.pop("r2")
+    assert r2.nrows == n_sel, "GPU row count %d != expected %d" % (r2.nrows, n_sel)
+    if dump:
+        dump_sample(r2.columns(), ["a"], dump, "c2")
+    r2.free()
     total_rows = sum_over_ranks(torch, float(n))
     value = total_rows * steps / (ms / 1e3)
     kernel_ms = kms / steps  # device time of the dominant kernel per step (1 launch per step here)
     alg_bytes = 8.0 * n + 8.0 * n_sel
     achieved = alg_bytes / (kernel_ms / 1e3) / 1e9
-    e2e_steps = max(3, min(steps, 10))
-    ems, _, _, _ = time_steps(ctx, torch, step_e2e, e2e_steps, 3)
+    e2e_steps = steps
+    ems, _, _, _ = time_steps(ctx, torch, step_e2e, e2e_steps, warmup)
     assert state["nrows"] == n_sel and np.array_equal(state["e2e_out"], a[a > 0.5][:1000])
     e2e_value = total_rows * e2e_steps / (ems / 1e3)
     batch.free()
@@ -336,32 +373,31 @@ def run_ours(args):
     out = {
         "metric": METRIC, "value": value, "unit": "rows/s", "n_gpus": world, "steps": steps, "warmup": warmup,
         "ms_per_step": ms / steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f64",
-        "data": "synthetic", "config": cfg, "clocks": clocks,
+        "data": "synthetic", "config": cfg, "gpu": gpu_info(local), "clocks": clocks,
         "e2e": {"value": e2e_value, "unit": "rows/s", "h2d_bytes_per_step": 8 * n, "d2h_bytes_per_step": 8 * n_sel + 32,
                 "steps": e2e_steps, "ms_per_step": ems / e2e_steps,
                 "path": "dfgpu_filter_project_host: pinned host batch -> chunked H2D | kernel | D2H pipeline -> pinned host result"},
         "gpu_launches": launches,
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": ncu_traffic("k_filter_project:c2") if n == 100_000_000 else None, "kernel": "k_filter_project_tma", "kernel_ms": kernel_ms,
-                     "algorithmic_bytes": alg_bytes, "peak_source": peak_src},
-        "sustained": {"steps": sus_steps, "seconds": sms / 1e3, "ms_per_step": sms / sus_steps, "kernel_ms": skms / sus_steps,
-                      "value": total_rows * sus_steps / (sms / 1e3), "roofline_frac": alg_bytes / (skms / sus_steps / 1e3) / 1e9 / peak},
+                     "kernel": "k_filter_project_tma", "kernel_ms": kernel_ms, "algorithmic_bytes": alg_bytes, "peak_source": peak_src},
     }
 
     # ---- C3 (extra) ---------------------------------------------------------------------------------
     extra = {}
-    xs = max(3, min(steps, 10))
+    xs = steps
     try:
         arrays3, pred3, proj3 = workloads.c3(n, seed=142 + 10 * rank)
         b3 = ctx.upload(arrays3[:2])  # c, d are never referenced: not uploaded (the host layer prunes them the same way)
         sel3 = int(np.count_nonzero(arrays3[1] < arrays3[0]))
 
         def step3():
-            r = ctx.filter_project(b3, pred3, proj3)
-            state["n3"] = r.nrows
-            r.free()
-        ms3, kms3, kn3, _ = time_steps(ctx, torch, step3, xs, 3)
-        assert state["n3"] == sel3
+            hold_last(state, "r3", ctx.filter_project(b3, pred3, proj3))
+        ms3, kms3, kn3, _ = time_steps(ctx, torch, step3, xs, warmup)
+        r3 = state.pop("r3")
+        assert r3.nrows == sel3
+        if dump:
+            dump_sample(r3.columns(), ["sum", "prod"], dump, "c3")
+        r3.free()
         k3 = kms3 / xs
         bytes3 = 16.0 * n + 16.0 * sel3
         extra["c3"] = {"workload": "C3: SELECT a+b, a*b FROM t WHERE b<a; 4 Float64 cols", "value": total_rows * xs / (ms3 / 1e3),
@@ -370,6 +406,8 @@ def run_ours(args):
                                     "frac": bytes3 / (k3 / 1e3) / 1e9 / peak, "algorithmic_bytes": bytes3}}
         b3.free()
         del arrays3
+    except AssertionError:
+        raise
     except Exception as e:  # pragma: no cover
         extra["c3"] = {"error": repr(e)}
 
@@ -389,32 +427,29 @@ def run_ours(args):
     b4 = ctx.upload(arrays4)
 
     def step4():
-        r = ctx.aggregate(b4, keys4, aggs4)
-        state["g4"] = r.nrows
-        if "keep4" in state:
-            state["cols4"] = r.columns()
-        r.free()
+        hold_last(state, "r4", ctx.aggregate(b4, keys4, aggs4))
 
     def step4_e2e():
         r = ctx.aggregate_host(arrays4, keys4, aggs4)
         state["g4e"] = r.nrows
         state["cols4e"] = r.columns()  # D2H of the (small) result is part of the step
         r.free()
-    ms4, kms4, kn4, _ = time_steps(ctx, torch, step4, xs, 3)
-    state["keep4"] = True
-    step4()
-    del state["keep4"]
-    chk4 = check_groupby(torch, state["cols4"], kraw4, arrays4[1], 100_000, ["sum", "count"], "C4")
+    ms4, kms4, kn4, _ = time_steps(ctx, torch, step4, xs, warmup)
+    r4 = state.pop("r4")
+    cols4 = r4.columns()
+    r4.free()
+    chk4 = check_groupby(torch, cols4, kraw4, arrays4[1], 100_000, ["sum", "count"], "C4")
+    if dump:
+        dump_groupby(cols4, 100_000, ["sum", "count"], dump, "c4")
     k4 = kms4 / xs  # scan kernel time per step (a first batch runs two launches: 1 Mi-row sampled prefix + the rest)
     bytes4 = 16.0 * n
     out["roofline_c4"] = {"bound": "hbm", "achieved": bytes4 / (k4 / 1e3) / 1e9, "peak": peak, "unit": "GB/s",
                           "frac": bytes4 / (k4 / 1e3) / 1e9 / peak, "algorithmic_bytes": bytes4, "kernel": "k_hash_agg_lean", "kernel_ms": k4,
-                          "traffic": ncu_traffic("k_hash_agg:c4") if n == 100_000_000 else None, "peak_source": peak_src,
-                          "scatter_ceiling": scatter_ceiling(k4, n)}
+                          "peak_source": peak_src}
     out["c4"] = {"workload": "C4: SELECT k, SUM(v), COUNT(v) FROM t GROUP BY k; 1e5 Int64 keys, %d rows per GPU%s" % (n, merge),
                  "value": total_rows * xs / (ms4 / 1e3), "unit": "rows/s", "ms_per_step": ms4 / xs, "steps": xs, "result_check": chk4}
     try:
-        ems4, _, _, _ = time_steps(ctx, torch, step4_e2e, xs, 3)
+        ems4, _, _, _ = time_steps(ctx, torch, step4_e2e, xs, warmup)
         check_groupby(torch, state["cols4e"], kraw4, arrays4[1], 100_000, ["sum", "count"], "C4 e2e")
         out["e2e_c4"] = {"value": total_rows * xs / (ems4 / 1e3), "unit": "rows/s", "h2d_bytes_per_step": 16 * n,
                          "d2h_bytes_per_step": 24 * state["g4e"], "steps": xs, "ms_per_step": ems4 / xs,
@@ -429,21 +464,20 @@ def run_ours(args):
         b5 = ctx.upload(arrays5)
 
         def step5():
-            r = ctx.aggregate(b5, keys5, aggs5)
-            state["g5"] = r.nrows
-            if "keep5" in state:
-                state["cols5"] = r.columns()
-            r.free()
-        ms5, kms5, kn5, _ = time_steps(ctx, torch, step5, xs, 3)
-        state["keep5"] = True
-        step5()
-        chk5 = check_groupby(torch, state["cols5"], kraw5, arrays5[1], 1_000_000, ["min", "max", "sum"], "C5")
+            hold_last(state, "r5", ctx.aggregate(b5, keys5, aggs5))
+        ms5, kms5, kn5, _ = time_steps(ctx, torch, step5, xs, warmup)
+        r5 = state.pop("r5")
+        cols5 = r5.columns()
+        r5.free()
+        chk5 = check_groupby(torch, cols5, kraw5, arrays5[1], 1_000_000, ["min", "max", "sum"], "C5")
+        if dump:
+            dump_groupby(cols5, 1_000_000, ["min", "max", "sum"], dump, "c5")
         k5 = kms5 / xs
         bytes5 = 16.0 * n5
         total5 = sum_over_ranks(torch, float(n5))
         extra["c5"] = {"workload": "C5: SELECT k, MIN(v), MAX(v), SUM(v) FROM t GROUP BY k; 1e6 Int64 keys, %d rows per GPU (%.3g rows in all)%s"
                                    % (n5, total5, merge),
-                       "groups": state["g5"], "value": total5 * xs / (ms5 / 1e3), "unit": "rows/s", "ms_per_step": ms5 / xs, "kernel_ms": k5,
+                       "groups": len(cols5[0]), "value": total5 * xs / (ms5 / 1e3), "unit": "rows/s", "ms_per_step": ms5 / xs, "kernel_ms": k5,
                        "roofline": {"bound": "hbm", "achieved": bytes5 / (k5 / 1e3) / 1e9, "peak": peak, "unit": "GB/s",
                                     "frac": bytes5 / (k5 / 1e3) / 1e9 / peak, "algorithmic_bytes": bytes5, "kernel": "k_hash_agg_lean"},
                        "result_check": chk5}
@@ -511,7 +545,7 @@ def run_reference(args):
     from datafusion_archive_b200 import workloads
     n = args.rows
     arrays, pred, proj = workloads.c2(n, seed=42)
-    steps, warmup = (args.steps or 5), max(3, args.warmup)
+    steps, warmup = args.steps, args.warmup
     state = {}
     for _ in range(warmup):
         state["out"] = O.filter_project(arrays, pred, proj)
@@ -539,14 +573,18 @@ def run_reference(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=None, help="timed steps (default: 2000 resident steps = ~0.6 s; reference arm: 5)")
-    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=None, help="timed steps of every leg (default: 100; reference arm: 5)")
+    ap.add_argument("--warmup", type=int, default=3, help="untimed warm-up steps before every timed leg")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--rows", type=int, default=100_000_000, help="rows per GPU")
     ap.add_argument("--rows5", type=int, default=0, help="rows per GPU of the C5 extra (default 1.25 x --rows)")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline legs")
-    ap.add_argument("--no-sustained", action="store_true", help="keep the sustained loop as short as the timed steps (for ncu launch lists)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps is not None and args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    if args.steps is None:
+        args.steps = 5 if args.impl == "reference" else 100
     if args.impl == "reference":
         run_reference(args)
     else:

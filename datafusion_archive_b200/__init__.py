@@ -1,4 +1,4 @@
-"""dfgpu — B200-native (sm_100a) engine for DataFusion 0.6.0's Arrow-batch hot path:
+"""dfgpu — H100-native (sm_90a) engine for DataFusion 0.6.0's Arrow-batch hot path:
 FilterRelation / ProjectRelation / AggregateRelation behind the reference's operator API.
 
 Layout: csrc/ (CUDA kernels + C ABI of include/dfgpu.h + the C++ host mirror of the reference's

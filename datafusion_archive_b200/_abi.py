@@ -1,4 +1,4 @@
-"""ctypes mirror of include/dfgpu.h (the C ABI of the sm_100a engine).
+"""ctypes mirror of include/dfgpu.h (the C ABI of the sm_90a engine).
 
 Only plain-old-data definitions live here so that the test-only CPU checker under
 tests/ can share them.  Nothing in this module touches a GPU.

@@ -19,7 +19,7 @@ void shift_copy_i32(dfgpu_ctx* ctx, int* dst, const int* src, long long n, int a
 void gather_utf8_multi(dfgpu_ctx* ctx, const Utf8Source* d_srcs, const unsigned long long* d_idx, long long nsel, DevColumn* out);
 
 constexpr int AG_THREADS = 256;
-constexpr int AG_R = 2;  // rows per thread per tile: 2 measured best on B200 (1.65 vs 1.74 ms at 4, 1.94 at 8: the kernel is bound by scattered L2 reductions, not by loads in flight)
+constexpr int AG_R = 2;  // rows per thread per tile: the kernel is bound by scattered L2 reductions, not by loads in flight, so more rows per thread only add registers
 constexpr int AG_TILE = AG_THREADS * AG_R;
 constexpr int kMaxAggs = 8;
 constexpr int kMaxKeys = 4;
@@ -36,19 +36,18 @@ struct AggDesc {
 
 // Table addressing.  A slot is a LINE of lw 64-bit words (lw a power of two; word 0 = the packed key) plus
 // one word in each of n_add separate arrays.  loc[a] says where accumulator a lives: >= 1 = that word of
-// the line, < 0 = additive array ~loc[a].  Three layouts fall out of it (measured on B200,
-// profiles/r02a_scatter_ops2.txt and profiles/r01m_microbench_agg.txt):
+// the line, < 0 = additive array ~loc[a].  Three layouts fall out of it:
 //   SoA     lw = 1, every accumulator in its own array.  A row's probe and reductions go to different L2
 //           slices in parallel; reductions that hit the SAME 32-byte sector as the probe serialise in the
-//           slice (LDG + 2 RED on one sector: 2.04 ms per 1e8 rows against 1.38 ms on three arrays).
+//           slice.
 //   hybrid  MIN / MAX accumulators share the line with the key, SUM / COUNT stay in arrays.  The probe is
-//           one 128/256-bit load that also returns the current MIN / MAX, and a MIN / MAX reduction is only
+//           one or two 128-bit loads that also return the current MIN / MAX, and a MIN / MAX reduction is only
 //           issued when the row improves on the value just read (monotone accumulators: a stale read can
 //           only cause a redundant reduction, never a missed one).  After a group's first few rows almost
 //           no row does, so MIN + MAX + SUM costs one load and one reduction per row instead of one load
 //           and three reductions.
 //   line    every accumulator in the line (lw >= 1 + naggs): one sector per group; wins once the table no
-//           longer fits L2 and every touched sector is an HBM transaction (1e7 groups: 7.1 vs 11.2 ms).
+//           longer fits L2 and every touched sector is an HBM transaction.
 struct TableLayout {
   unsigned long long* base;  // (cap + 1) lines of lw words
   unsigned long long* add;   // n_add arrays of (cap + 1) words
@@ -247,14 +246,24 @@ __device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
 struct Line {
   unsigned long long w[4];
 };
+// A 4-word line as two 128-bit loads (sm_90 has no 256-bit global load); both land in the same 32-byte
+// sector.  The halves are not read atomically together, which the protocol tolerates: a key seen in word 0
+// is final, and the accumulators are monotone, so an older or newer word 1..3 can only cause a redundant
+// MIN / MAX reduction, never a missed one.
+__device__ __forceinline__ void load_line4(const unsigned long long* q, Line& ln, unsigned long long pol = 0ull) {
+  if (pol) {
+    asm volatile("ld.global.cg.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(ln.w[0]), "=l"(ln.w[1]) : "l"(q), "l"(pol) : "memory");
+    asm volatile("ld.global.cg.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(ln.w[2]), "=l"(ln.w[3]) : "l"(q + 2), "l"(pol) : "memory");
+  } else {
+    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln.w[0]), "=l"(ln.w[1]) : "l"(q) : "memory");
+    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln.w[2]), "=l"(ln.w[3]) : "l"(q + 2) : "memory");
+  }
+}
 template <bool WITH_VALS>
 __device__ __forceinline__ void load_line(const TableLayout& t, long long slot, Line& ln, unsigned long long pol = 0ull) {
   const unsigned long long* q = t.key(slot);
-  if (WITH_VALS && t.lw >= 4) {  // 256-bit load (LDG.E.ENL2.256): lines are 32-byte aligned
-    if (pol)
-      asm volatile("ld.global.cg.L2::cache_hint.v4.u64 {%0, %1, %2, %3}, [%4], %5;" : "=l"(ln.w[0]), "=l"(ln.w[1]), "=l"(ln.w[2]), "=l"(ln.w[3]) : "l"(q), "l"(pol) : "memory");
-    else
-      asm volatile("ld.global.cg.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(ln.w[0]), "=l"(ln.w[1]), "=l"(ln.w[2]), "=l"(ln.w[3]) : "l"(q) : "memory");
+  if (WITH_VALS && t.lw >= 4) {  // lines are 32-byte aligned
+    load_line4(q, ln, pol);
   } else if (WITH_VALS && t.lw == 2) {
     if (pol)
       asm volatile("ld.global.cg.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(ln.w[0]), "=l"(ln.w[1]) : "l"(q), "l"(pol) : "memory");
@@ -519,13 +528,12 @@ struct PlainSrc {
   __device__ __forceinline__ unsigned rowid(int r) const { return (unsigned)(row0 + r); }
 };
 
-// K5 scan.  Per row: key -> mix64 -> linear probing over table lines (ld.global.cg, 64/128/256 bits: the
+// K5 scan.  Per row: key -> mix64 -> linear probing over table lines (ld.global.cg, 64/128 bits or 2 x 128: the
 // probe also brings the in-line MIN / MAX accumulators) -> atomicCAS to claim an empty slot -> one
 // fire-and-forget L2 reduction per additive accumulator and per MIN / MAX that the row improves.
 // FRONT: a per-CTA open-addressed table in shared memory absorbs the updates (shared-memory atomics),
 // and is merged into the global table once, when the CTA is done.  Used when the sampled prefix shows
-// few groups: with a handful of hot keys every global reduction would serialise on the same L2 sector
-// (measured: 10 groups, 1e8 rows: 21 ms through L2 atomics).
+// few groups: with a handful of hot keys every global reduction would serialise on the same L2 sector.
 template <class Src, bool FRONT, bool NULLS>
 __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long long* s_front) {
   constexpr int R = Src::R;
@@ -701,7 +709,7 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
   const long long tstep = (long long)gridDim.x * TILE;
   // software pipeline: the two 128-bit loads of the NEXT tile are in flight while this tile's probes and
   // reductions are issued (HBM latency of the stream and L2 latency of the probe chain overlap per thread)
-  // (measured: a gain for SUM / COUNT shapes, a loss where the 256-bit line of MIN / MAX needs the registers)
+  // (only for the 1-word line of SUM / COUNT shapes: the 4-word line of MIN / MAX needs the registers)
   constexpr bool PF = LW == 1;
   unsigned long long nk[2] = {0ull, 0ull}, nv[2] = {0ull, 0ull};
   if (PF) {
@@ -740,7 +748,7 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
       act[r] = (r == 0 ? any : both) && (p.npass == 1 || (k[r] == EMPTY_KEY ? p.pass_id == 0 : (int)(hs >> p.pass_shift) == p.pass_id));
       if (act[r] && k[r] != EMPTY_KEY) {
         const unsigned long long* q = base + slot[r] * LW;
-        if (LW == 4) asm volatile("ld.global.cg.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(ln[r].w[0]), "=l"(ln[r].w[1]), "=l"(ln[r].w[2]), "=l"(ln[r].w[3]) : "l"(q) : "memory");
+        if (LW == 4) load_line4(q, ln[r]);
         else if (LW == 2) asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln[r].w[0]), "=l"(ln[r].w[1]) : "l"(q) : "memory");
         else asm volatile("ld.global.cg.u64 %0, [%1];" : "=l"(ln[r].w[0]) : "l"(q) : "memory");
       }
@@ -766,7 +774,7 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
           }
           slot[r] = (slot[r] + 1ull) & smask;
           const unsigned long long* q = base + slot[r] * LW;
-          if (LW == 4) asm volatile("ld.global.cg.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(ln[r].w[0]), "=l"(ln[r].w[1]), "=l"(ln[r].w[2]), "=l"(ln[r].w[3]) : "l"(q) : "memory");
+          if (LW == 4) load_line4(q, ln[r]);
           else if (LW == 2) asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln[r].w[0]), "=l"(ln[r].w[1]) : "l"(q) : "memory");
           else asm volatile("ld.global.cg.u64 %0, [%1];" : "=l"(ln[r].w[0]) : "l"(q) : "memory");
         }
@@ -1441,8 +1449,8 @@ long long next_pow2(long long x) {
 int grid_for(dfgpu_ctx* ctx, long long work_items, int per_block, int blocks_per_sm);
 
 // groups x (1 + naggs) sectors is what the SoA layout keeps hot in L2; beyond this many bytes the
-// table is built AoS (one sector per group).  B200 L2 = 126 MB, shared with the streaming input.
-constexpr long long AG_SOA_L2_BUDGET = 64ll << 20;
+// table is built AoS (one sector per group).  H100 L2 = 50 MB, shared with the streaming input.
+constexpr long long AG_SOA_L2_BUDGET = 24ll << 20;
 
 // Cardinality estimate from a prefix sample: `d` distinct keys among the first `s` rows.  Under a
 // uniform model E[d] = G (1 - exp(-s / G)); solved for G by bisection and capped by the rows of the
@@ -1464,7 +1472,7 @@ long long estimate_groups(long long d, long long s, long long total_rows) {
 // every sector of each additive array once a quarter of its slots is in use.  Beyond the budget the table
 // is built in "line" form (one sector per group, whatever the number of aggregates).
 bool hybrid_enabled() {
-  static const bool off = getenv("DFGPU_AGG_HYBRID") && atoi(getenv("DFGPU_AGG_HYBRID")) == 0;  // A/B switch: 0 = plain SoA (round-1 layout)
+  static const bool off = getenv("DFGPU_AGG_HYBRID") && atoi(getenv("DFGPU_AGG_HYBRID")) == 0;  // A/B switch: 0 = plain SoA
   return !off;
 }
 void layout_shape(const std::vector<AggDesc>& descs, int naggs, int nkeys, bool line_mode, long long* lw, int* n_add, signed char* loc, int kw = 0) {
@@ -1498,7 +1506,7 @@ bool want_aos(long long groups, const std::vector<AggDesc>& descs, int naggs) {
   const long long cap = std::max(AG_MIN_CAP, next_pow2(2 * groups));
   const long long line_hot = std::min(cap * 8 * lw, groups * std::max<long long>(32, 8 * lw));
   const long long arr_hot = std::min(cap * 8, groups * 32);
-  static const long long budget = std::max<long long>(AG_SOA_L2_BUDGET, (long long)env_int("DFGPU_AGG_PASS_MB", 32) * env_int("DFGPU_AGG_MAX_PASSES", 1) << 20);
+  static const long long budget = std::max<long long>(AG_SOA_L2_BUDGET, (long long)env_int("DFGPU_AGG_PASS_MB", 16) * env_int("DFGPU_AGG_MAX_PASSES", 1) << 20);
   return line_hot + n_add * arr_hot > budget;
 }
 
@@ -1602,8 +1610,8 @@ long long hybrid_hot_bytes(long long groups, const std::vector<AggDesc>& descs, 
 }
 int passes_for(long long groups, const std::vector<AggDesc>& descs, int naggs) {
   static const int forced = env_int("DFGPU_AGG_PASSES", 0);          // A/B switch: 1 | 2 | 4 | 8
-  static const int pass_mb = env_int("DFGPU_AGG_PASS_MB", 32);       // hot megabytes one pass may touch
-  static const int max_passes = env_int("DFGPU_AGG_MAX_PASSES", 1);  // measured (profiles/r02d_microbench_agg.txt): a second pass over the input costs what the L2 hits save; off by default
+  static const int pass_mb = env_int("DFGPU_AGG_PASS_MB", 16);       // hot megabytes one pass may touch
+  static const int max_passes = env_int("DFGPU_AGG_MAX_PASSES", 1);  // a second pass over the input costs about what the L2 hits save; off by default
   if (forced > 0) return forced;
   const long long hot = hybrid_hot_bytes(groups, descs, naggs);
   int np = 1;
@@ -2223,8 +2231,8 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
           static const bool no_hint = getenv("DFGPU_AGG_STREAM_HINT") && atoi(getenv("DFGPU_AGG_STREAM_HINT")) == 0;  // A/B switch
           p.stream_hint = no_hint ? 0 : 1;
         }
-        // (A persisting-L2 access-policy window over the table was measured in round 2 and removed: the scan
-        // went from 1.57 to 7.8 ms at 1e5 groups and from 3.4 to 15 ms at 1e6, profiles/r02a_l2persist.txt.)
+        // (A persisting-L2 access-policy window over the table was tried and removed: it slowed the scan
+        // several-fold at 1e5 and 1e6 groups.)
         // tables that outgrow L2: several passes over the rows, each confined to one contiguous part of the table
         const int npass = (list || front || ranges[ri].second < (4ll << 20) || st->aos) ? 1 : st->npass;
         p.npass = npass;

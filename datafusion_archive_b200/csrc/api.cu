@@ -61,7 +61,7 @@ void dfgpu_ctx::use() { DF_CUDA(cudaSetDevice(device)); }
 // buffers, hash tables, overflow lists: hundreds of MB each) are kept in a per-ctx cache by size class
 // (8 classes per power of two, <= 12.5 % padding) and handed out again without a driver call: the
 // stream-ordered pool splits and re-merges big blocks, and a request it cannot serve from a cached
-// block maps new physical memory, which was measured at 15-45 ms for a 1 GB table (DESIGN 4.3).
+// block maps new physical memory, which takes milliseconds for a table of a few hundred MB.
 // Every consumer of these blocks is ordered on ctx->stream (or synchronises its side stream before
 // freeing), so immediate reuse is safe.
 static size_t big_class(size_t bytes) {
@@ -228,9 +228,9 @@ extern "C" int dfgpu_device_count(int* out) {
 }
 
 // One process (host thread) per GPU: keep that thread and the memory it allocates next — numpy / Arrow buffers,
-// cudaMallocHost staging — on the NUMA node the GPU hangs off.  On the 2-socket B200 hosts GPUs 0-3 sit on node 0
-// and 4-7 on node 1; round 1 measured the 8-rank end-to-end step at 25.6 ms against 15.9 ms for one rank, with
-// ranks and their pinned buffers placed by the OS.  Opt out with DFGPU_NUMA=0.  Best effort: silently does
+// cudaMallocHost staging — on the NUMA node the GPU hangs off.  On 2-socket hosts with 8 GPUs, half the GPUs sit
+// on each node, and ranks whose pinned buffers the OS places on the far node pay for it in every H2D / D2H
+// copy.  Opt out with DFGPU_NUMA=0.  Best effort: silently does
 // nothing when sysfs does not expose the topology.
 static void bind_to_gpu_numa_node(int device) {
   if (const char* e = getenv("DFGPU_NUMA")) if (atoi(e) == 0) return;
@@ -291,9 +291,9 @@ extern "C" int dfgpu_init(int device, dfgpu_ctx** out) {
     bind_to_gpu_numa_node(device);
     cudaDeviceProp prop;
     DF_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10)
+    if (prop.major != 9 || prop.minor != 0)
       fail(DFGPU_ERR_CUDA, std::string("device '") + prop.name + "' is sm_" + std::to_string(prop.major * 10 + prop.minor) +
-                               "; this library is built for sm_100a (B200) only");
+                               "; this library is built for sm_90a (H100) only");
     ctx->sm_count = prop.multiProcessorCount;
     ctx->device_mem_bytes = prop.totalGlobalMem;
     if (const char* e = getenv("DFGPU_FP_KERNEL")) ctx->force_direct_kernel = std::string(e) == "direct";
@@ -378,7 +378,7 @@ extern "C" int dfgpu_flush_l2(dfgpu_ctx* ctx) {
   return guarded([&] {
     ctx->use();
     if (!ctx->flush_buf) {
-      ctx->flush_bytes = size_t(256) << 20;  // 2x the 126 MB L2
+      ctx->flush_bytes = size_t(128) << 20;  // > 2x the 50 MB L2
       DF_CUDA(cudaMalloc(&ctx->flush_buf, ctx->flush_bytes));
     }
     DF_CUDA(cudaMemsetAsync(ctx->flush_buf, 0x5a, ctx->flush_bytes, ctx->stream));

@@ -1,4 +1,4 @@
-// common.cuh — internals shared by the sm_100a engine's translation units.
+// common.cuh — internals shared by the sm_90a engine's translation units.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -63,7 +63,7 @@ inline bool is_numeric(int dt) { return dt >= DFGPU_INT8 && dt <= DFGPU_FLOAT64;
 // ---------------------------------------------------------------------------------------------
 struct dfgpu_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   size_t device_mem_bytes = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev_start = nullptr, ev_stop = nullptr;

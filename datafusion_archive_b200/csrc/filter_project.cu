@@ -601,7 +601,8 @@ extern "C" int dfgpu_filter_project_host(dfgpu_ctx* ctx, const dfgpu_col* cols, 
       return;
     }
 
-    // default chunk: measured on C2 (profiles/r02y_e2e_chunks.txt): 16 / 8 / 4 / 2 / 1 Mi rows -> 16.59 / 15.96 / 15.45 / 15.47 / 15.99 ms per step
+    // default chunk: big enough that per-chunk launch and copy overheads stay small, small enough that the
+    // first upload and the last download, which nothing overlaps, stay short (profiles/e2e_chunks.py sweeps it)
     if (chunk_rows <= 0) chunk_rows = 4ll << 20;
     const long long nchunks = n > 0 ? (n + chunk_rows - 1) / chunk_rows : 1;
     struct Chunk {

@@ -7,7 +7,7 @@
 //   producer A (1 warp) : one elected lane streams the PREDICATE columns of tile it into ring A with
 //                         cp.async.bulk (SASS UBLKCP), completion tracked by mbarrier tx counts
 //   producer B (1 warp) : streams the PROJECTION columns of tile it-LAG into ring B the same way —
-//                         a re-read of bytes fetched LAG tiles earlier, served by the 126 MB L2
+//                         a re-read of bytes fetched LAG tiles earlier, served by the 50 MB L2
 //   16 consumer warps   : phase 1 = predicate of tile it over ring A -> K flag bits per lane, kept in
 //                         a 64-bit shift register; phase 2 = projections of tile it-LAG over ring B,
 //                         selected rows stored at their compacted global position
@@ -37,17 +37,17 @@
 namespace dfgpu {
 
 constexpr int TM_CWARPS = 16;  // consumer warps
-constexpr int TM_SWARPS = 2;   // scan warps (2 x TM_BATCH gathers in flight; 20 warps = 5 per SM sub-partition leave 96 registers per thread; a third scan warp was measured: 6 warps on one sub-partition cap the kernel at 80 registers and C2 went from 0.260 to 0.278 ms, profiles/r02_history.md)
+constexpr int TM_SWARPS = 2;   // scan warps (2 x TM_BATCH gathers in flight; 20 warps = 5 per SM sub-partition leave 96 registers per thread; a third scan warp would put 6 warps on one sub-partition and cap the kernel at 80 registers)
 #ifndef DF_TM_BATCH
 #define DF_TM_BATCH 4
 #endif
-constexpr int TM_BATCH = DF_TM_BATCH;  // waves per scan-warp batch.  Measured with the lean consumer loop (profiles/r02x_sweep_fp_scan_variants.txt): 2 -> C2 0.298 ms, 3 -> 0.260, 4 -> 0.239; issuing a wave's gather right behind its own publish: 0.33-0.41; one wave per step with the gather consumed a step later (profiles/r02z_sweep_fp_scan_pipe2.txt): 0.38 at every lag (statuses read right after the publish are stale and the re-poll is serial)
+constexpr int TM_BATCH = DF_TM_BATCH;  // waves per scan-warp batch: more waves per batch put more gathers in flight; issuing a wave's gather right behind its own publish is slower (statuses read right after the publish are stale and the re-poll is serial)
 constexpr int TM_WARPS = TM_CWARPS + 2 + TM_SWARPS;
 constexpr int TM_THREADS = TM_WARPS * 32;
 constexpr int TM_MAX_STAGES = 8;
 constexpr int TM_RING = 32;       // slots of the count/offset hand-off rings (> max lag + 1)
 constexpr int TM_MAX_LAG = 24;
-constexpr int TM_MAX_GRID = 160;  // CTAs (= SMs) the wave gather is written for (B200: 148)
+constexpr int TM_MAX_GRID = 160;  // CTAs (= SMs) the wave gather is written for (H100 SXM: 132)
 constexpr int TM_HDR_BYTES = 8192;
 constexpr int TM_SMEM_BUDGET = 200 * 1024;
 // upper bound of one hardware suspension in mbarrier.try_wait: a waiting warp sleeps until the phase
@@ -240,12 +240,10 @@ __device__ __forceinline__ void arith_term_t(const FastOp& t, const unsigned cha
 // ---- lean consumer loop ---------------------------------------------------------------------------
 // The shapes the headline configurations have (C2: SELECT a WHERE a > c; C3: SELECT a+b, a*b WHERE b < a): ONE
 // Float64 comparison as the predicate and one or two projections that copy an 8-byte column or combine Float64
-// operands.  ncu on the generic FAST loop (profiles/r02_c2.lines.txt, SASS view in profiles/r02_history.md): 383
-// instructions per warp-tile of which ~120 touch rows; the rest re-derives per-tile invariants — indexed
+// operands.  In the generic FAST loop most instructions per warp-tile re-derive per-tile invariants — indexed
 // constant-bank loads of the column offsets behind the term's column index, a jump table on the comparison
-// operator, generic -> shared address conversions in front of every mbarrier operation — and its dependent
-// latencies (short scoreboard 19 %, no-instruction 7 %, branch resolving 5 % of the consumer samples) are what the
-// 4 consumer warps per scheduler cannot hide.  Here the comparison operator and the operand kind are template
+// operator, generic -> shared address conversions in front of every mbarrier operation — and their dependent
+// latencies are what the 4 consumer warps per scheduler cannot hide.  Here the comparison operator and the operand kind are template
 // parameters, every offset, pointer and barrier address is computed once before the loop, and the loop body is
 // waits + loads + compares + the ballot-compacted store.  Protocol (barriers, rings, scan warps) unchanged.
 template <int CMP, class T>
@@ -971,7 +969,7 @@ bool launch_fp_tma(dfgpu_ctx* ctx, FPParams& p) {
   p.slab_slots = 0;
   p.noscan = getenv("DFGPU_FP_NOSCAN") && atoi(getenv("DFGPU_FP_NOSCAN")) != 0;
   // stash mode: every program a fast shape over 8-byte columns with 8-byte results
-  // (opt-in, DFGPU_FP_MODE=stash: measured slower than the dual ring at 50 % selectivity, equal at 1 %: profiles/r02m_sweep_fp.txt)
+  // (opt-in, DFGPU_FP_MODE=stash: slower than the dual ring at 50 % selectivity, equal at 1 %, where it was measured)
   bool stash = p.has_pred && p.pred_fast.nterms > 0 && mode && std::string(mode) == "stash";
   for (int q = 0; stash && q < p.nproj; q++) {
     const FastOp& fo = p.proj_fast[q];
@@ -1002,7 +1000,7 @@ bool launch_fp_tma(dfgpu_ctx* ctx, FPParams& p) {
     // lag: the slab slots the grid keeps live (lag x grid x nproj x tile x 8 bytes, about half of it touched at
     // 50 % selectivity) should stay L2 resident
     const long long slot_bytes = grid * p.nproj * (long long)tile * 8;
-    p.lag = (int)std::min<long long>(TM_MAX_LAG, std::max<long long>(TM_BATCH, (96ll << 20) / slot_bytes));
+    p.lag = (int)std::min<long long>(TM_MAX_LAG, std::max<long long>(TM_BATCH, (32ll << 20) / slot_bytes));
     if (const char* e = getenv("DFGPU_FP_LAG")) {
       const int l = atoi(e);
       if (l >= TM_BATCH - 1 && l <= TM_MAX_LAG) p.lag = l;
@@ -1018,7 +1016,7 @@ bool launch_fp_tma(dfgpu_ctx* ctx, FPParams& p) {
     ctx->free(p.slab);  // stream ordered: the block is only handed out again to work queued behind this kernel
     return true;
   }
-  if (p.has_pred && mode && std::string(mode) == "single") {  // measured slower than dual on B200 (profiles/r01_history.md): opt-in only
+  if (p.has_pred && mode && std::string(mode) == "single") {  // slower than dual where it was measured: opt-in only
     for (int k : {8, 4, 2}) {
       if (k == 8 && p.ps.max_depth > 2) continue;
       const long long tile = (long long)TM_CWARPS * 32 * k;
@@ -1026,9 +1024,9 @@ bool launch_fp_tma(dfgpu_ctx* ctx, FPParams& p) {
     }
   }
   if (!p.single_ring) {
-    // rows per lane K in {8,4,2}: the biggest tile that still gives both rings 3 stages.  Measured on
-    // B200 (profiles/r01_microbench_fp.txt): per-tile fixed costs (barrier hand-offs, offset gather)
-    // outweigh deeper prefetch, so bigger tiles with few stages beat smaller tiles with many.
+    // rows per lane K in {8,4,2}: the biggest tile that still gives both rings 3 stages.  Per-tile fixed
+    // costs (barrier hand-offs, offset gather) outweigh deeper prefetch, so bigger tiles with few stages
+    // beat smaller tiles with many.
     for (int k : {8, 4, 2}) {
       if (k == 8 && p.ps.max_depth > 2) continue;  // deep register stacks spill at 8 rows per lane
       const long long tile = (long long)TM_CWARPS * 32 * k;
@@ -1078,11 +1076,13 @@ bool launch_fp_tma(dfgpu_ctx* ctx, FPParams& p) {
     }
     // lag: as large as the flag shift register allows (K bits per tile in 64 bits), but the bytes the
     // projection stream will re-read (lag x grid x stage B) must still be in L2 when it gets there
+    // On H100 (132 SMs, 50 MB L2) the shortest lag the scan warps allow was fastest for C2 and C3, whose
+    // projection stages re-read about 4 MB per wave (profiles/microbench_fp.py under DFGPU_FP_LAG=3..12).
     p.lag = 0;
     if (p.has_pred) {
-      const long long l2_budget = 40ll << 20;
+      const long long l2_budget = 12ll << 20;  // a quarter of the 50 MB L2
       const long long per_tile = (long long)std::min(ctx->sm_count, TM_MAX_GRID) * offB;
-      p.lag = (int)std::min<long long>(std::min(TM_MAX_LAG, 128 / K - 1), std::max<long long>(4, l2_budget / per_tile));
+      p.lag = (int)std::min<long long>(std::min(TM_MAX_LAG, 128 / K - 1), std::max<long long>(TM_BATCH - 1, l2_budget / per_tile));
     }
     if (const char* e = getenv("DFGPU_FP_LAG")) {  // experiment knob
       const int l = atoi(e);

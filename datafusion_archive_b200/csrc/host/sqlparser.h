@@ -1,5 +1,5 @@
 // sqlparser.h — SQL subset front-end.  The reference delegates parsing to crate sqlparser 0.2.1
-// (Cargo.toml:34, wrapped by src/dfparser.rs:74); that crate is not under /root/reference, so this
+// (Cargo.toml:34, wrapped by src/dfparser.rs:74); that crate is not in the reference repository, so this
 // is a restatement of the grammar subset the planner consumes (src/sqlplanner.rs:46-375): one
 // SELECT [list] [FROM ident] [WHERE e] [GROUP BY e,..] [HAVING e] [ORDER BY e [ASC|DESC],..] [LIMIT n].
 #pragma once

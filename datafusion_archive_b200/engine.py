@@ -1,8 +1,8 @@
-"""ctypes binding of libdfgpu.so (the sm_100a engine behind include/dfgpu.h).
+"""ctypes binding of libdfgpu.so (the sm_90a engine behind include/dfgpu.h).
 
 This is the harness-side view of the C ABI: tests and bench.py drive the kernels through it with
 host (numpy / pyarrow) buffers, exactly as the Rust shim of INTEGRATION.md would.  There is no CPU
-fallback: if the shared library is missing or no B200 is present, calls raise.
+fallback: if the shared library is missing or no H100 is present, calls raise.
 """
 import ctypes as C
 import os
@@ -27,7 +27,7 @@ def lib_path():
 
 
 def build(force=False):
-    """Compile csrc/*.cu for sm_100a into libdfgpu.so (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/*.cu for sm_90a into libdfgpu.so (nvcc cross-compiles without a GPU)."""
     here = os.path.dirname(os.path.abspath(__file__))
     csrc = os.path.join(here, "csrc")
     so = lib_path()
@@ -231,7 +231,7 @@ class Batch:
 
 
 class GpuContext:
-    """One dfgpu_ctx = one B200 + stream + memory pool."""
+    """One dfgpu_ctx = one H100 + stream + memory pool."""
 
     def __init__(self, device=0):
         self.h = C.c_void_p()

@@ -6,7 +6,7 @@ This module is a numpy MODEL of that protocol (row ranges, owner function, per-o
 that the world_size>1 host logic can be exercised on CPU over gloo.  It is not the product's merge: on
 GPUs the exchange runs inside libdfgpu.so (aggregate.cu agg_exchange_groups: k_owner_count /
 k_owner_scatter -> grouped ncclSend/ncclRecv -> k_merge -> k_compact -> grouped ncclBroadcast), which is
-tested under NCCL on two B200s (tests/test_multiprocess.py) and checked against numpy inside bench.py at
+tested under NCCL on two GPUs (tests/test_multiprocess.py) and checked against numpy inside bench.py at
 every N."""
 import numpy as np
 

@@ -1,5 +1,5 @@
 /*
- * dfgpu.h — C ABI of the B200-native (sm_100a) engine for DataFusion 0.6.0's Arrow-batch hot path.
+ * dfgpu.h — C ABI of the H100-native (sm_90a) engine for DataFusion 0.6.0's Arrow-batch hot path.
  *
  * This is the drop-in boundary.  The reference (andygrove/datafusion-archive, Rust) has no FFI; its
  * operator "plugin API" is the `Relation` trait plus the `Expr`/`LogicalPlan` IR.  Each entry point

@@ -5,7 +5,7 @@
 //                   then the same update with slot = HIGH bits of the hash, so that the rows of one
 //                   partition touch one contiguous 1/256th of the table (L2 resident while it is hot)
 // Prints the time of every pass and checks that A and B produce the same table contents.
-//   build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o profiles/bin/partition_agg profiles/src/partition_agg.cu
+//   build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o profiles/bin/partition_agg profiles/src/partition_agg.cu
 //   usage: partition_agg [rows=1e8] [groups=1e7]
 #include <cstdio>
 #include <cstdlib>

@@ -9,9 +9,9 @@
 //   M5  the 16-byte TMA reduction only
 //   M6  RED.v2.f32 only (vector reduction, for the rate of a 2-element RED)
 //   M7  LDG.128 only (probe of a 16-byte {key, aux})
-//   M8  LDG.256 of a 32-byte line {key, min, max, -} + RED.f64 on a separate array (the hybrid layout's row)
-//   M9  LDG.256 only          M10  RED.u32 only          M11  LDG + RED.f64 + RED.u32 (32-bit COUNT)
-//   build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o profiles/bin/scatter_ops2 profiles/src/scatter_ops2.cu
+//   M8  2 x LDG.128 of a 32-byte line {key, min, max, -} + RED.f64 on a separate array (the hybrid layout's row)
+//   M9  2 x LDG.128 only         M10  RED.u32 only          M11  LDG + RED.f64 + RED.u32 (32-bit COUNT)
+//   build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o profiles/bin/scatter_ops2 profiles/src/scatter_ops2.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -63,7 +63,8 @@ __global__ void __launch_bounds__(256) k_ops(unsigned long long* tab, unsigned l
       acc += v.x + v.y;
     } else if (MODE == 8 || MODE == 9) {
       unsigned long long a, b, c, d;
-      asm volatile("ld.global.cg.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(&tab[h * 4]));
+      asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "l"(&tab[h * 4]));
+      asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(c), "=l"(d) : "l"(&tab[h * 4 + 2]));
       acc += a + b + c + d;
       if (MODE == 8) atomicAdd((double*)&soa1[h], 1.0);
     } else if (MODE == 10) {
@@ -113,8 +114,8 @@ int main(int argc, char** argv) {
     run<5>("M5 TMA reduce 16B add.f64", 1, n, slots, tab, s1, s2, sink, sms);
     run<6>("M6 RED.v2.f32", 1, n, slots, tab, s1, s2, sink, sms);
     run<7>("M7 LDG.128", 1, n, slots, tab, s1, s2, sink, sms);
-    run<8>("M8 LDG.256 (AoS line) + RED.f64 (array)", 2, n, slots, tab, s1, s2, sink, sms);
-    run<9>("M9 LDG.256", 1, n, slots, tab, s1, s2, sink, sms);
+    run<8>("M8 2xLDG.128 (AoS line) + RED.f64 (array)", 2, n, slots, tab, s1, s2, sink, sms);
+    run<9>("M9 2xLDG.128", 1, n, slots, tab, s1, s2, sink, sms);
     run<10>("M10 RED.u32", 1, n, slots, tab, s1, s2, sink, sms);
     run<11>("M11 LDG + RED.f64 + RED.u32 (SoA)", 3, n, slots, tab, s1, s2, sink, sms);
     cudaFree(tab); cudaFree(s1); cudaFree(s2); cudaFree(sink);

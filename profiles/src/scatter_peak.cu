@@ -1,7 +1,7 @@
 // Measures the machine's rate for scattered (one distinct address per lane) global-memory operations:
 // the ceiling for an open-addressed hash aggregate whose table lives in L2 / HBM.  No input stream is
 // read (addresses come from a hash of the row number), so the result is the pure LSU / L2-atomic rate.
-//   build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o profiles/bin/scatter_peak profiles/src/scatter_peak.cu
+//   build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o profiles/bin/scatter_peak profiles/src/scatter_peak.cu
 //   usage: scatter_peak [rows=1e8]
 #include <cstdio>
 #include <cstdlib>

@@ -1,4 +1,4 @@
-// build.rs — link the B200 engine.  DFGPU_LIB_DIR = directory holding libdfgpu.so
+// build.rs — link the H100 engine.  DFGPU_LIB_DIR = directory holding libdfgpu.so
 // (built by `make -C datafusion_archive_b200/csrc`).
 fn main() {
     if let Ok(dir) = std::env::var("DFGPU_LIB_DIR") {

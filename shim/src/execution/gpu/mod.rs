@@ -1,4 +1,4 @@
-//! B200 (sm_100a) execution of the Arrow-batch hot path: FilterRelation, ProjectRelation and
+//! H100 (sm_90a) execution of the Arrow-batch hot path: FilterRelation, ProjectRelation and
 //! AggregateRelation behind the `Relation` trait, calling libdfgpu.so (include/dfgpu.h).
 pub mod ffi;
 pub mod lower;

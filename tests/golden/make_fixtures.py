@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Generate tests/golden/reference_vectors.json from the reference checkout (run in the build
-container only: /root/reference does not exist on the GPU box).
+"""Generate tests/golden/reference_vectors.json from a checkout of the reference
+(usage: make_fixtures.py <reference checkout>; the tests only read what it writes).
 
 Inputs are the reference's own test fixtures (test/data/*.csv) and the golden strings / values its
 tests assert (tests/sql.rs, src/execution/aggregate.rs).  The expected strings are extracted from
@@ -12,7 +12,7 @@ import os
 import re
 import sys
 
-REF = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+REF = sys.argv[1]
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_vectors.json")
 
 
@@ -40,7 +40,7 @@ def main():
     agg1 = read_csv(os.path.join(REF, "test/data/aggregate_test_1.csv"), True)
     agg2 = read_csv(os.path.join(REF, "test/data/aggregate_test_2.csv"), True)
     out = {
-        "_generated_by": "tests/golden/make_fixtures.py from /root/reference (andygrove/datafusion-archive)",
+        "_generated_by": "tests/golden/make_fixtures.py from andygrove/datafusion-archive",
         "uk_cities": {  # schema tests/sql.rs:79-87
             "city": [r[0] for r in cities], "lat": [float(r[1]) for r in cities], "lng": [float(r[2]) for r in cities],
         },
@@ -75,7 +75,7 @@ def main():
         json.dump(out, f, indent=1)
     print("wrote", OUT)
     # byte-for-byte copies of the three CSV data files the hot-path tests open (test DATA, not source),
-    # so CsvDataSource can be exercised on the GPU box where /root/reference does not exist
+    # so CsvDataSource can be exercised without the reference checkout
     import shutil
     data = os.path.join(os.path.dirname(OUT), "data")
     os.makedirs(data, exist_ok=True)

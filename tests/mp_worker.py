@@ -5,7 +5,7 @@
               the keys it owns, the owned segments are gathered, and the result is checked against the
               oracle on the full data.  Exercises row ranges, the owner function and the merge algebra
               without a GPU; likewise a model of the regroup merge used for Utf8 / wide keys.
-  mode nccl : GPUs.  Each rank drives its own B200 through the C ABI with a communicator attached;
+  mode nccl : GPUs.  Each rank drives its own H100 through the C ABI with a communicator attached;
               every rank must end with the SAME global result (dfgpu_aggregate_finish: owner-partitioned
               exchange over NCCL), also when one rank saw no rows at all.
 """

@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a path through the C ABI vs the CPU oracle on the same seeded inputs
+"""GPU parity tests: the sm_90a path through the C ABI vs the CPU oracle on the same seeded inputs
 (bit-exact for integer/index/ordering work and every non-reduced f64, 1e-9 relative for f64 SUM),
 the reference's golden vectors, edge cases, and size-independent properties at BASELINE sizes."""
 import numpy as np
