@@ -102,15 +102,9 @@ struct AggParams {
   // private table per warp, so that shared-memory atomics only contend inside a warp
   int front_slots;     // power of two
   int front_per_warp;  // 0 / 1
-  int stream_hint;     // 1: input columns are loaded with an L2 evict-first policy
   // fused WHERE (Aggregate{input: Selection}, context.rs:126-139,162-192): program 0 is the predicate and
   // the key / argument programs follow; rows that fail it are skipped before the probe
   int has_pred;
-  int cond_mm;         // 1: MIN / MAX reductions are skipped when the value read with the probe already covers the row
-  int table_hint;      // 1: table loads / reductions carry an L2 evict-last policy
-  // multi-pass scan (tables that outgrow L2): launch `pass_id` of `npass` takes the rows whose hash's top
-  // log2(npass) bits equal pass_id, i.e. whose home slot lies in one contiguous 1/npass of the table
-  int npass, pass_id, pass_shift;
   // wide keys (k_hash_agg_wide): composite keys of more than 64 bits and keys with Utf8 parts.  Line word 0 is a
   // TAG (the 64-bit hash of the key tuple, low bit = ready), words 1..kw the key parts: the 64-bit value of a
   // fixed-width part, or for a Utf8 part a reference (source << 40 | row) to the string of the row that created
@@ -224,9 +218,7 @@ __device__ __forceinline__ void acc_fold_global(int func, int mt, unsigned long 
   }
 }
 
-// Home slot of a key = the TOP log2(cap) bits of its hash.  The top bits of the slot index are then the top
-// bits of the hash whatever the capacity, which is what the multi-pass scan selects rows by (a pass touches
-// one contiguous 1/P of the table, and the assignment of rows to passes survives a table growth).
+// Home slot of a key = the TOP log2(cap) bits of its hash.
 __host__ __device__ __forceinline__ int hash_shift(long long cap) {
   int lg = 0;
   while ((1ll << lg) < cap) lg++;
@@ -241,8 +233,6 @@ __device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
 }
 
 // One table line as read by a probe: word 0 = key, words 1..3 = the accumulators that share the line.
-// `pol` != 0: an L2 evict-last policy word — the table competes for L2 with a 1.6 GB input stream that is
-// read once (marked evict-first), so its lines should be the last to go.
 struct Line {
   unsigned long long w[4];
 };
@@ -250,49 +240,22 @@ struct Line {
 // sector.  The halves are not read atomically together, which the protocol tolerates: a key seen in word 0
 // is final, and the accumulators are monotone, so an older or newer word 1..3 can only cause a redundant
 // MIN / MAX reduction, never a missed one.
-__device__ __forceinline__ void load_line4(const unsigned long long* q, Line& ln, unsigned long long pol = 0ull) {
-  if (pol) {
-    asm volatile("ld.global.cg.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(ln.w[0]), "=l"(ln.w[1]) : "l"(q), "l"(pol) : "memory");
-    asm volatile("ld.global.cg.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(ln.w[2]), "=l"(ln.w[3]) : "l"(q + 2), "l"(pol) : "memory");
-  } else {
-    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln.w[0]), "=l"(ln.w[1]) : "l"(q) : "memory");
-    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln.w[2]), "=l"(ln.w[3]) : "l"(q + 2) : "memory");
-  }
+__device__ __forceinline__ void load_line4(const unsigned long long* q, Line& ln) {
+  asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln.w[0]), "=l"(ln.w[1]) : "l"(q) : "memory");
+  asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln.w[2]), "=l"(ln.w[3]) : "l"(q + 2) : "memory");
 }
 template <bool WITH_VALS>
-__device__ __forceinline__ void load_line(const TableLayout& t, long long slot, Line& ln, unsigned long long pol = 0ull) {
+__device__ __forceinline__ void load_line(const TableLayout& t, long long slot, Line& ln) {
   const unsigned long long* q = t.key(slot);
   if (WITH_VALS && t.lw >= 4) {  // lines are 32-byte aligned
-    load_line4(q, ln, pol);
+    load_line4(q, ln);
   } else if (WITH_VALS && t.lw == 2) {
-    if (pol)
-      asm volatile("ld.global.cg.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(ln.w[0]), "=l"(ln.w[1]) : "l"(q), "l"(pol) : "memory");
-    else
-      asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln.w[0]), "=l"(ln.w[1]) : "l"(q) : "memory");
+    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln.w[0]), "=l"(ln.w[1]) : "l"(q) : "memory");
     ln.w[2] = ln.w[3] = 0ull;
   } else {
-    if (pol)
-      asm volatile("ld.global.cg.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(ln.w[0]) : "l"(q), "l"(pol) : "memory");
-    else
-      asm volatile("ld.global.cg.u64 %0, [%1];" : "=l"(ln.w[0]) : "l"(q) : "memory");
+    asm volatile("ld.global.cg.u64 %0, [%1];" : "=l"(ln.w[0]) : "l"(q) : "memory");
     ln.w[1] = ln.w[2] = ln.w[3] = 0ull;
   }
-}
-// fire-and-forget reductions with an L2 cache-policy operand
-__device__ __forceinline__ void red_add_f64(unsigned long long* p, double v, unsigned long long pol) {
-  asm volatile("red.global.add.L2::cache_hint.f64 [%0], %1, %2;" ::"l"(p), "d"(v), "l"(pol) : "memory");
-}
-__device__ __forceinline__ void red_add_f32(unsigned long long* p, float v, unsigned long long pol) {
-  asm volatile("red.global.add.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(p), "f"(v), "l"(pol) : "memory");
-}
-__device__ __forceinline__ void red_add_u64(unsigned long long* p, unsigned long long v, unsigned long long pol) {
-  asm volatile("red.global.add.L2::cache_hint.u64 [%0], %1, %2;" ::"l"(p), "l"(v), "l"(pol) : "memory");
-}
-__device__ __forceinline__ void red_min_u64(unsigned long long* p, unsigned long long v, unsigned long long pol) {
-  asm volatile("red.global.min.L2::cache_hint.u64 [%0], %1, %2;" ::"l"(p), "l"(v), "l"(pol) : "memory");
-}
-__device__ __forceinline__ void red_max_u64(unsigned long long* p, unsigned long long v, unsigned long long pol) {
-  asm volatile("red.global.max.L2::cache_hint.u64 [%0], %1, %2;" ::"l"(p), "l"(v), "l"(pol) : "memory");
 }
 __device__ __forceinline__ unsigned long long line_word(const Line& ln, int l) {
   return l == 1 ? ln.w[1] : (l == 2 ? ln.w[2] : ln.w[3]);
@@ -305,7 +268,7 @@ __device__ __forceinline__ unsigned long long line_word(const Line& ln, int l) {
 // probe limit): the row goes to the overflow list.
 template <bool WITH_VALS>
 __device__ __forceinline__ long long probe_insert(const TableLayout& t, long long cap, unsigned long long key, Line& ln,
-                                                  unsigned long long h, bool full, unsigned& new_groups, unsigned long long pol = 0ull) {
+                                                  unsigned long long h, bool full, unsigned& new_groups) {
   const unsigned long long mask = (unsigned long long)cap - 1ull;
   for (int probes = 0; probes < AG_MAX_PROBE; ++probes) {
     if (ln.w[0] == key) return (long long)h;
@@ -316,7 +279,7 @@ __device__ __forceinline__ long long probe_insert(const TableLayout& t, long lon
       if (old == key) return (long long)h;
     }
     h = (h + 1ull) & mask;
-    load_line<WITH_VALS>(t, (long long)h, ln, pol);
+    load_line<WITH_VALS>(t, (long long)h, ln);
   }
   return -1;
 }
@@ -324,25 +287,17 @@ __device__ __forceinline__ long long probe_insert(const TableLayout& t, long lon
 // fold one raw value into global memory; `cur` = the accumulator as read with the probe (have_cur): a
 // MIN / MAX that the row does not improve needs no reduction (the stored value only moves towards it)
 __device__ __forceinline__ void acc_fold_global_cond(int func, int mt, unsigned long long* p, unsigned long long v, bool have_cur,
-                                                     unsigned long long cur, unsigned long long pol) {
+                                                     unsigned long long cur) {
   if (func == DFGPU_AGG_MIN) {
     if (is_nan_val(v, mt)) return;
     const unsigned long long e = ord_enc(v, mt);
-    if (!have_cur || e < cur) { if (pol) red_min_u64(p, e, pol); else atomicMin(p, e); }
+    if (!have_cur || e < cur) atomicMin(p, e);
   } else if (func == DFGPU_AGG_MAX) {
     if (is_nan_val(v, mt)) return;
     const unsigned long long e = ord_enc(v, mt);
-    if (!have_cur || e > cur) { if (pol) red_max_u64(p, e, pol); else atomicMax(p, e); }
-  } else if (!pol) {
-    acc_fold_global(func, mt, p, v);
-  } else if (func == DFGPU_AGG_COUNT) {
-    red_add_u64(p, 1ull, pol);
-  } else if (mt == MT_F64) {
-    red_add_f64(p, u2d(v), pol);
-  } else if (mt == MT_F32) {
-    red_add_f32(p, u2f(v), pol);
+    if (!have_cur || e > cur) atomicMax(p, e);
   } else {
-    red_add_u64(p, v, pol);
+    acc_fold_global(func, mt, p, v);
   }
 }
 
@@ -378,7 +333,6 @@ constexpr int AG_FRONT_MAX_GROUPS = 1024;
 template <int DEPTH, bool NULLS>
 struct InterpSrc {
   static constexpr int R = AG_R;
-  static constexpr bool PREFETCH = false;
   GlobalRows<R> g;
   unsigned mask;  // rows to aggregate: in range and passing the predicate
   unsigned bad = 0;
@@ -468,12 +422,10 @@ __device__ __forceinline__ unsigned cmp_bits2(int op, int mt, const unsigned lon
   return f;
 }
 // NC: column slots the instantiation holds (2 = the common key + value shape: fewer registers, more CTAs
-// per SM); PF: the loads of the NEXT tile are issued before the current tile's probes, so the HBM latency of
-// the input stream and the L2 latency of the probe chain overlap instead of adding up per thread.
-template <int NC, bool PF>
+// per SM).
+template <int NC>
 struct PlainSrc {
   static constexpr int R = 2;
-  static constexpr bool PREFETCH = PF;
   unsigned long long cv[NC][2];
   long long row0;
   unsigned mask;
@@ -552,22 +504,18 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
   const long long n = p.row_list ? p.nlist : p.nrows;
   const int hshift = hash_shift(p.cap);
   // the input is read exactly once: mark its lines evict-first so that they do not displace the table
-  const unsigned long long stream_policy = p.stream_hint ? l2_evict_first_policy() : 0ull;
-  const unsigned long long tpol = p.table_hint ? l2_evict_last_policy() : 0ull;
+  const unsigned long long stream_policy = l2_evict_first_policy();
   bool bad = false;
   constexpr int TILE = AG_THREADS * R;
   const long long tstep = (long long)gridDim.x * TILE;
-  Src src, nxt;
-  bool first = true;
+  Src src;
   for (long long tb = (long long)blockIdx.x * TILE; tb < n; tb += tstep) {
     // fill limit, once per warp per tile (no CTA-wide barrier in the steady state)
     unsigned long long filled = 0;
     if (lane == 0) filled = __ldcg(&p.counters[0]);
     filled = __shfl_sync(0xffffffffu, filled, 0);
     const bool full = (long long)filled >= p.max_groups;
-    if (!Src::PREFETCH || first) src.load(p, tb, n, tid, stream_policy);
-    first = false;
-    if (Src::PREFETCH && tb + tstep < n) nxt.load(p, tb + tstep, n, tid, stream_policy);
+    src.load(p, tb, n, tid, stream_policy);
     src.prepare(p);
     // group key: one packed 64-bit word (GroupByScalar vector of aggregate.rs:807-852)
     unsigned long long key[R];
@@ -602,11 +550,9 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
     for (int r = 0; r < R; r++) {
       const unsigned long long hs = mix64(key[r]);
       h[r] = home_slot(hs, hshift);
-      // multi-pass scan: this launch only takes the rows whose home slot lies in its 1/npass of the table
-      if (p.npass > 1 && (key[r] == EMPTY_KEY ? p.pass_id != 0 : (int)(hs >> p.pass_shift) != p.pass_id)) src.mask &= ~(1u << r);
       probing[r] = ((src.mask >> r) & 1u) && key[r] != EMPTY_KEY && fslot[r] < 0;
       ln[r].w[0] = ln[r].w[1] = ln[r].w[2] = ln[r].w[3] = 0ull;
-      if (probing[r]) load_line<true>(p.t, (long long)h[r], ln[r], tpol);
+      if (probing[r]) load_line<true>(p.t, (long long)h[r], ln[r]);
     }
     long long slot[R];
     unsigned new_groups = 0;
@@ -619,7 +565,7 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
         slot[r] = p.cap;
         continue;
       }
-      slot[r] = probe_insert<true>(p.t, p.cap, key[r], ln[r], h[r], full, new_groups, tpol);
+      slot[r] = probe_insert<true>(p.t, p.cap, key[r], ln[r], h[r], full, new_groups);
       if (slot[r] < 0) {
         const unsigned long long at = atomicAdd(&p.counters[1], 1ull);
         p.ovf_rows[at] = src.rowid(r);
@@ -633,7 +579,7 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
       for (int a = 0; a < p.naggs; a++) {
         if (p.agg_arg[a] != g) continue;
         const int func = p.aggs[a].func, mt = p.aggs[a].mtype, l = p.t.loc[a];
-        const bool cond = p.cond_mm && l >= 1 && l <= 3 && (func == DFGPU_AGG_MIN || func == DFGPU_AGG_MAX);
+        const bool cond = l >= 1 && l <= 3 && (func == DFGPU_AGG_MIN || func == DFGPU_AGG_MAX);
 #pragma unroll
         for (int r = 0; r < R; r++) {
           if (NULLS && func == DFGPU_AGG_COUNT && !((av >> r) & 1u)) continue;  // COUNT counts non-null values
@@ -641,7 +587,7 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
             acc_fold_shared(func, mt, &ftab[(1 + a) * FS + fslot[r]], v[r]);
             if ((b >> r) & 1u) bad = true;
           } else if (slot[r] >= 0) {
-            acc_fold_global_cond(func, mt, p.t.val(slot[r], a), v[r], cond && probing[r], cond ? line_word(ln[r], l) : 0ull, tpol);
+            acc_fold_global_cond(func, mt, p.t.val(slot[r], a), v[r], cond && probing[r], cond ? line_word(ln[r], l) : 0ull);
             if ((b >> r) & 1u) bad = true;
           }
         }
@@ -652,7 +598,6 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) new_groups += __shfl_xor_sync(0xffffffffu, new_groups, o);
     if (lane == 0 && new_groups) atomicAdd(&p.counters[0], (unsigned long long)new_groups);
-    if (Src::PREFETCH) src = nxt;
   }
   if (FRONT) {
     // merge this CTA's front table into the global table.  New keys are always admitted here; the host
@@ -677,15 +622,17 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
   if (bad) p.counters[3] = 1ull;
 }
 
+// Occupancy target (H100): the global-table scan wants its interpreter stack in registers more than a fourth
+// CTA per SM (3: up to 80 registers, no spills), the front-table scan wants the fourth CTA (4: 64 registers).
 template <int DEPTH, bool FRONT, bool NULLS>
-__global__ void __launch_bounds__(AG_THREADS) k_hash_agg(const __grid_constant__ AggParams p) {
+__global__ void __launch_bounds__(AG_THREADS, FRONT ? 4 : 3) k_hash_agg(const __grid_constant__ AggParams p) {
   extern __shared__ unsigned long long s_front[];  // FRONT: keys[AG_FRONT_SLOTS] then vals[naggs][AG_FRONT_SLOTS]
   hash_agg_body<InterpSrc<DEPTH, NULLS>, FRONT, NULLS>(p, s_front);
 }
-template <int NC, bool PF, bool FRONT>
+template <int NC, bool FRONT>
 __global__ void __launch_bounds__(AG_THREADS, 4) k_hash_agg_plain(const __grid_constant__ AggParams p) {
   extern __shared__ unsigned long long s_front[];
-  hash_agg_body<PlainSrc<NC, PF>, FRONT, false>(p, s_front);
+  hash_agg_body<PlainSrc<NC>, FRONT, false>(p, s_front);
 }
 
 // K5, lean form: the canonical GROUP BY shape — one 8-byte integer key column, one 8-byte argument column, any
@@ -704,7 +651,7 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
   unsigned long long* const base = p.t.base;
   const int hshift = hash_shift(p.cap);
   const unsigned long long smask = (unsigned long long)p.cap - 1ull;
-  const unsigned long long policy = p.stream_hint ? l2_evict_first_policy() : 0ull;
+  const unsigned long long policy = l2_evict_first_policy();
   constexpr int TILE = AG_THREADS * 2;
   const long long tstep = (long long)gridDim.x * TILE;
   // software pipeline: the two 128-bit loads of the NEXT tile are in flight while this tile's probes and
@@ -743,9 +690,8 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
     bool act[2];
 #pragma unroll
     for (int r = 0; r < 2; r++) {
-      const unsigned long long hs = mix64(k[r]);
-      slot[r] = home_slot(hs, hshift);
-      act[r] = (r == 0 ? any : both) && (p.npass == 1 || (k[r] == EMPTY_KEY ? p.pass_id == 0 : (int)(hs >> p.pass_shift) == p.pass_id));
+      slot[r] = home_slot(mix64(k[r]), hshift);
+      act[r] = r == 0 ? any : both;
       if (act[r] && k[r] != EMPTY_KEY) {
         const unsigned long long* q = base + slot[r] * LW;
         if (LW == 4) load_line4(q, ln[r]);
@@ -788,8 +734,8 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
       if (HAS_MIN || HAS_MAX) {
         if (!is_nan_val(v[r], MT)) {  // f64::min / f64::max ignore NaN (aggregate.rs:139-140, 208-209)
           const unsigned long long e = ord_enc(v[r], MT);
-          if (HAS_MIN && (!have_line || !p.cond_mm || e < line_word(ln[r], p.lean.min_w))) atomicMin(line + p.lean.min_w, e);
-          if (HAS_MAX && (!have_line || !p.cond_mm || e > line_word(ln[r], p.lean.max_w))) atomicMax(line + p.lean.max_w, e);
+          if (HAS_MIN && (!have_line || e < line_word(ln[r], p.lean.min_w))) atomicMin(line + p.lean.min_w, e);
+          if (HAS_MAX && (!have_line || e > line_word(ln[r], p.lean.max_w))) atomicMax(line + p.lean.max_w, e);
         }
       }
       if (HAS_SUM) {
@@ -977,7 +923,7 @@ __global__ void __launch_bounds__(AG_THREADS) k_reduce(const __grid_constant__ A
   unsigned nn[kMaxAggs];
 #pragma unroll
   for (int a = 0; a < kMaxAggs; a++) nn[a] = 0;
-  unsigned npass = 0;  // rows that passed the fused predicate (counters[6]: an aggregate over zero rows is null)
+  unsigned passed = 0;  // rows that passed the fused predicate (counters[6]: an aggregate over zero rows is null)
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int a = 0; a < p.naggs; a++) s_acc[a][tid] = agg_identity(p.aggs[a].func);
   bool bad = false;
@@ -1002,7 +948,7 @@ __global__ void __launch_bounds__(AG_THREADS) k_reduce(const __grid_constant__ A
       for (int r = 0; r < RD_R; r++) keep |= (unsigned)(v[r] & 1ull) << r;
       rmask &= keep;
     }
-    if (p.has_pred) npass += __popc(rmask);
+    if (p.has_pred) passed += __popc(rmask);
     for (int g = 0; g < p.nargs; g++) {
       unsigned long long v[RD_R];
       unsigned av;
@@ -1047,8 +993,8 @@ __global__ void __launch_bounds__(AG_THREADS) k_reduce(const __grid_constant__ A
   }
   if (p.has_pred) {
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) npass += __shfl_xor_sync(0xffffffffu, npass, o);
-    if (lane == 0 && npass) atomicAdd(&p.counters[6], (unsigned long long)npass);
+    for (int o = 16; o > 0; o >>= 1) passed += __shfl_xor_sync(0xffffffffu, passed, o);
+    if (lane == 0 && passed) atomicAdd(&p.counters[6], (unsigned long long)passed);
   }
   if (bad) p.counters[3] = 1ull;
 }
@@ -1387,7 +1333,6 @@ struct dfgpu_aggstate {
   bool aos = false;        // "line" layout: every accumulator shares the line with the key (tables beyond L2)
   std::vector<dfgpu_insn> pred_prog;  // fused WHERE predicate (dfgpu_aggregate_set_predicate); empty = none
   bool use_front = false;  // route rows through the per-CTA shared-memory front table
-  int npass = 1;           // scan passes per big batch (tables that outgrow L2, see AggParams)
   // wide keys: composite keys of more than 64 bits or with Utf8 parts (k_hash_agg_wide)
   bool wide = false;
   std::vector<int> key_is_utf8;
@@ -1468,13 +1413,6 @@ long long estimate_groups(long long d, long long s, long long total_rows) {
   return g > double(total_rows) ? total_rows : (long long)g;
 }
 
-// Bytes the scan keeps hot in L2 with the hybrid layout: one sector (or lw/4) per group for the line, and
-// every sector of each additive array once a quarter of its slots is in use.  Beyond the budget the table
-// is built in "line" form (one sector per group, whatever the number of aggregates).
-bool hybrid_enabled() {
-  static const bool off = getenv("DFGPU_AGG_HYBRID") && atoi(getenv("DFGPU_AGG_HYBRID")) == 0;  // A/B switch: 0 = plain SoA
-  return !off;
-}
 void layout_shape(const std::vector<AggDesc>& descs, int naggs, int nkeys, bool line_mode, long long* lw, int* n_add, signed char* loc, int kw = 0) {
   *lw = 1;
   *n_add = 0;
@@ -1486,15 +1424,14 @@ void layout_shape(const std::vector<AggDesc>& descs, int naggs, int nkeys, bool 
   int nmm = 0;
   for (int a = 0; a < naggs; a++) {
     const bool mm = descs[size_t(a)].func == DFGPU_AGG_MIN || descs[size_t(a)].func == DFGPU_AGG_MAX;
-    if (nkeys > 0 && mm && hybrid_enabled()) loc[a] = (signed char)(1 + nmm++);
+    if (nkeys > 0 && mm) loc[a] = (signed char)(1 + nmm++);
     else loc[a] = (signed char)~((*n_add)++);
   }
   while (*lw < 1 + nmm) *lw <<= 1;
 }
-int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : dflt;
-}
+// Bytes the scan keeps hot in L2 with the hybrid layout: one sector (or lw/4) per group for the line, and
+// every sector of each additive array once a quarter of its slots is in use.  Beyond the budget the table
+// is built in "line" form (one sector per group, whatever the number of aggregates).
 bool want_aos(long long groups, const std::vector<AggDesc>& descs, int naggs) {
   static const char* force = getenv("DFGPU_AGG_LAYOUT");  // A/B switch: "line" | "hybrid"
   if (force && std::string(force) == "line") return true;
@@ -1506,8 +1443,7 @@ bool want_aos(long long groups, const std::vector<AggDesc>& descs, int naggs) {
   const long long cap = std::max(AG_MIN_CAP, next_pow2(2 * groups));
   const long long line_hot = std::min(cap * 8 * lw, groups * std::max<long long>(32, 8 * lw));
   const long long arr_hot = std::min(cap * 8, groups * 32);
-  static const long long budget = std::max<long long>(AG_SOA_L2_BUDGET, (long long)env_int("DFGPU_AGG_PASS_MB", 16) * env_int("DFGPU_AGG_MAX_PASSES", 1) << 20);
-  return line_hot + n_add * arr_hot > budget;
+  return line_hot + n_add * arr_hot > AG_SOA_L2_BUDGET;
 }
 
 TableLayout table_alloc(dfgpu_ctx* ctx, int naggs, int nkeys, const std::vector<AggDesc>& descs, long long cap, bool aos, int kw = 0) {
@@ -1596,27 +1532,6 @@ void table_grow(dfgpu_aggstate* st, long long new_cap) {
   st->t = nt;
   st->aos = aos;
   st->cap = new_cap;
-}
-
-// Hot bytes of the hybrid layout for `groups` groups (see want_aos) and the number of scan passes that
-// keeps the part of the table one pass touches L2 resident.
-long long hybrid_hot_bytes(long long groups, const std::vector<AggDesc>& descs, int naggs) {
-  long long lw;
-  int n_add;
-  signed char loc[kMaxAggs];
-  layout_shape(descs, naggs, 1, false, &lw, &n_add, loc);
-  const long long cap = std::max(AG_MIN_CAP, next_pow2(2 * groups));
-  return std::min(cap * 8 * lw, groups * std::max<long long>(32, 8 * lw)) + n_add * std::min(cap * 8, groups * 32);
-}
-int passes_for(long long groups, const std::vector<AggDesc>& descs, int naggs) {
-  static const int forced = env_int("DFGPU_AGG_PASSES", 0);          // A/B switch: 1 | 2 | 4 | 8
-  static const int pass_mb = env_int("DFGPU_AGG_PASS_MB", 16);       // hot megabytes one pass may touch
-  static const int max_passes = env_int("DFGPU_AGG_MAX_PASSES", 1);  // a second pass over the input costs about what the L2 hits save; off by default
-  if (forced > 0) return forced;
-  const long long hot = hybrid_hot_bytes(groups, descs, naggs);
-  int np = 1;
-  while (np < max_passes && hot / np > ((long long)pass_mb << 20)) np <<= 1;
-  return hot / np > ((long long)pass_mb << 20) ? 1 : np;  // beyond max_passes x pass_mb: one pass over the line layout
 }
 
 // Launch one scan kernel.  FRONT launches admit the keys of every CTA's front table unconditionally when
@@ -1941,7 +1856,6 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
         st->t = table_alloc(ctx, st->naggs, st->nkeys, st->descs, st->cap, true, st->nkeys);
       } else {
       st->aos = st->nkeys > 0 && want_aos(st->expected, st->descs, st->naggs);
-      st->npass = (st->nkeys > 0 && !st->aos && st->expected > 0) ? passes_for(st->expected, st->descs, st->naggs) : 1;
       st->t = table_alloc(ctx, st->naggs, st->nkeys, st->descs, st->cap, st->aos);
       }
     } else {
@@ -1972,12 +1886,6 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
     p.nrows = batch->nrows;
     p.counters = st->d_counters;
     p.has_pred = has_pred;
-    {
-      static const bool no_cond = getenv("DFGPU_AGG_COND_MM") && atoi(getenv("DFGPU_AGG_COND_MM")) == 0;  // A/B switch
-      p.cond_mm = no_cond ? 0 : 1;
-      static const bool hint = getenv("DFGPU_AGG_TABLE_HINT") && atoi(getenv("DFGPU_AGG_TABLE_HINT")) != 0;  // A/B switch (default off until measured)
-      p.table_hint = hint ? 1 : 0;
-    }
     const int d = p.ps.max_depth;
 
     if (st->nkeys == 0) {
@@ -2086,7 +1994,6 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
         p.row_list = list;
         p.nlist = nlist;
         p.ovf_rows = wovf[cur];
-        p.npass = 1;
         DF_CUDA(cudaMemsetAsync(st->d_counters + 1, 0, 8, ctx->stream));
         DF_CUDA(cudaMemsetAsync(st->d_counters + 5, 0, 8, ctx->stream));
         const long long n = list ? nlist : p.nrows;
@@ -2227,60 +2134,42 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
         // CTA-wide 2048-slot table); otherwise one table per CTA
         p.front_per_warp = st->ngroups <= 64 ? 1 : 0;
         p.front_slots = p.front_per_warp ? AG_FRONT_SLOTS / (AG_THREADS / 32) : AG_FRONT_SLOTS;
-        {
-          static const bool no_hint = getenv("DFGPU_AGG_STREAM_HINT") && atoi(getenv("DFGPU_AGG_STREAM_HINT")) == 0;  // A/B switch
-          p.stream_hint = no_hint ? 0 : 1;
-        }
         // (A persisting-L2 access-policy window over the table was tried and removed: it slowed the scan
         // several-fold at 1e5 and 1e6 groups.)
-        // tables that outgrow L2: several passes over the rows, each confined to one contiguous part of the table
-        const int npass = (list || front || ranges[ri].second < (4ll << 20) || st->aos) ? 1 : st->npass;
-        p.npass = npass;
-        p.pass_shift = 64;
-        for (int q = 1; q < npass; q <<= 1) p.pass_shift--;
-        const long long max_groups = p.max_groups;
-        for (int pass = 0; pass < npass; pass++) {
-          p.pass_id = pass;
-          p.max_groups = max_groups;
-          if (p.ps.has_nulls) launch_scan(ctx, k_hash_agg<8, false, true>, p, n, false);
-          else if (lean_mask && !list && !front && !st->aos && (p.row_begin & 1) == 0) {
-            // the lean kernel addresses the hybrid layout directly
-            p.lean.key_col = (const unsigned long long*)p.ps.cols[p.plain.key_slot[0]].ptr;
-            p.lean.arg_col = (const unsigned long long*)p.ps.cols[p.plain.arg_slot[0]].ptr;
-            p.lean.min_w = p.lean.max_w = 0;
-            p.lean.sum_arr = p.lean.cnt_arr = nullptr;
-            for (int a = 0; a < st->naggs; a++) {
-              const int f = st->descs[size_t(a)].func, l = st->t.loc[a];
-              if (f == DFGPU_AGG_MIN) p.lean.min_w = l;
-              else if (f == DFGPU_AGG_MAX) p.lean.max_w = l;
-              else if (f == DFGPU_AGG_SUM) p.lean.sum_arr = st->t.add + (long long)(~l) * st->t.astride;
-              else p.lean.cnt_arr = st->t.add + (long long)(~l) * st->t.astride;
-            }
-            bool layout_ok = st->t.lw == (((lean_mask & 3) == 3) ? 4 : ((lean_mask & 3) ? 2 : 1));
-            for (int a = 0; a < st->naggs; a++) {
-              const int f = st->descs[size_t(a)].func;
-              layout_ok = layout_ok && ((f == DFGPU_AGG_MIN || f == DFGPU_AGG_MAX) ? st->t.loc[a] >= 1 : st->t.loc[a] < 0);
-            }
-            if (layout_ok) launch_lean(ctx, p, n, lean_mask, lean_mt);
-            else launch_scan(ctx, k_hash_agg_plain<2, false, false>, p, n, false);
-          } else if (use_plain && !list && (p.row_begin & 1) == 0) {
-            static const bool pf = getenv("DFGPU_AGG_PREFETCH") && atoi(getenv("DFGPU_AGG_PREFETCH")) != 0;  // A/B switch (measured: no gain)
-            const bool two = p.plain.ncols <= 2;
-            if (front) {
-              if (two) launch_scan(ctx, k_hash_agg_plain<2, false, true>, p, n, true);
-              else launch_scan(ctx, k_hash_agg_plain<4, false, true>, p, n, true);
-            } else if (!pf) {
-              if (two) launch_scan(ctx, k_hash_agg_plain<2, false, false>, p, n, false);
-              else launch_scan(ctx, k_hash_agg_plain<4, false, false>, p, n, false);
-            } else {
-              if (two) launch_scan(ctx, k_hash_agg_plain<2, true, false>, p, n, false);
-              else launch_scan(ctx, k_hash_agg_plain<4, true, false>, p, n, false);
-            }
-          } else if (d <= 1) launch_hash_agg<1>(ctx, p, n, front);
-          else if (d <= 2) launch_hash_agg<2>(ctx, p, n, front);
-          else if (d <= 4) launch_hash_agg<4>(ctx, p, n, front);
-          else launch_hash_agg<8>(ctx, p, n, front);
-        }
+        if (p.ps.has_nulls) launch_scan(ctx, k_hash_agg<8, false, true>, p, n, false);
+        else if (lean_mask && !list && !front && !st->aos && (p.row_begin & 1) == 0) {
+          // the lean kernel addresses the hybrid layout directly
+          p.lean.key_col = (const unsigned long long*)p.ps.cols[p.plain.key_slot[0]].ptr;
+          p.lean.arg_col = (const unsigned long long*)p.ps.cols[p.plain.arg_slot[0]].ptr;
+          p.lean.min_w = p.lean.max_w = 0;
+          p.lean.sum_arr = p.lean.cnt_arr = nullptr;
+          for (int a = 0; a < st->naggs; a++) {
+            const int f = st->descs[size_t(a)].func, l = st->t.loc[a];
+            if (f == DFGPU_AGG_MIN) p.lean.min_w = l;
+            else if (f == DFGPU_AGG_MAX) p.lean.max_w = l;
+            else if (f == DFGPU_AGG_SUM) p.lean.sum_arr = st->t.add + (long long)(~l) * st->t.astride;
+            else p.lean.cnt_arr = st->t.add + (long long)(~l) * st->t.astride;
+          }
+          bool layout_ok = st->t.lw == (((lean_mask & 3) == 3) ? 4 : ((lean_mask & 3) ? 2 : 1));
+          for (int a = 0; a < st->naggs; a++) {
+            const int f = st->descs[size_t(a)].func;
+            layout_ok = layout_ok && ((f == DFGPU_AGG_MIN || f == DFGPU_AGG_MAX) ? st->t.loc[a] >= 1 : st->t.loc[a] < 0);
+          }
+          if (layout_ok) launch_lean(ctx, p, n, lean_mask, lean_mt);
+          else launch_scan(ctx, k_hash_agg_plain<2, false>, p, n, false);
+        } else if (use_plain && !list && (p.row_begin & 1) == 0) {
+          const bool two = p.plain.ncols <= 2;
+          if (front) {
+            if (two) launch_scan(ctx, k_hash_agg_plain<2, true>, p, n, true);
+            else launch_scan(ctx, k_hash_agg_plain<4, true>, p, n, true);
+          } else {
+            if (two) launch_scan(ctx, k_hash_agg_plain<2, false>, p, n, false);
+            else launch_scan(ctx, k_hash_agg_plain<4, false>, p, n, false);
+          }
+        } else if (d <= 1) launch_hash_agg<1>(ctx, p, n, front);
+        else if (d <= 2) launch_hash_agg<2>(ctx, p, n, front);
+        else if (d <= 4) launch_hash_agg<4>(ctx, p, n, front);
+        else launch_hash_agg<8>(ctx, p, n, front);
         unsigned long long c[8];
         read_counters(st, c);
         if (c[3] == 2) fail(DFGPU_ERR_INTERNAL, "front-table merge could not find a slot");
@@ -2309,7 +2198,6 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
         long long want_cap = std::max(AG_MIN_CAP, next_pow2(est * 2));
         while (want_cap > st->cap && want_cap > afford) want_cap >>= 1;
         const bool to_aos = !st->aos && want_aos(est, st->descs, st->naggs);
-        st->npass = (st->aos || to_aos) ? 1 : passes_for(est, st->descs, st->naggs);
         if (to_aos || want_cap > st->cap) {
           st->aos = st->aos || to_aos;
           table_grow(st, std::max(st->cap, want_cap));

@@ -160,11 +160,6 @@ __device__ __forceinline__ unsigned long long l2_evict_first_policy() {
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
   return pol;
 }
-__device__ __forceinline__ unsigned long long l2_evict_last_policy() {
-  unsigned long long pol;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
 
 template <int R>
 struct GlobalRows {

@@ -52,15 +52,6 @@ struct FPParams {
   int stage_bytesA, stage_bytesB;
   int nstagesA, nstagesB;
   int lag;  // tiles between the predicate pass and the projection pass
-  int count_ballot; // 1: per-tile counts via K ballots (A/B switch); 0: one REDUX per warp
-  int single_ring;  // 1: one ring holds the union of the columns; the projection pass reads the SAME staged tile
-  // "stash" mode (STASH instantiations): one ring for the HBM stream; the predicate pass also evaluates the
-  // projections and compacts the selected values of the tile into a slab in global memory (L2 resident: it is a
-  // ring that is rewritten every slab_slots tiles), the second pass copies slab -> final position once the tile's
-  // output offset is known.  Nothing is read twice and nothing but selected values moves after the first pass.
-  unsigned long long* slab;  // [grid][slab_slots][nproj][tile] 8-byte values
-  int slab_slots;
-  int noscan;  // TIMING EXPERIMENT ONLY (DFGPU_FP_NOSCAN=1, stash mode): skip the cross-CTA scan and the second pass; results are garbage
   // "fast shapes": single-operation programs over 4- and 8-byte numeric columns are recognised on the host and executed by
   // straight-line code instead of the interpreter (same arithmetic, no decode in the inner loop).
   //   predicate : chain of (COL cmp COL | COL cmp IMM) joined by AND / OR

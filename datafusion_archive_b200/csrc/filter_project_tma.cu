@@ -321,7 +321,6 @@ __device__ __forceinline__ void consumer_lean(const FPParams& p, int warp, int l
   const int first = blockIdx.x, step = gridDim.x;
   const int nloc = first < p.ntiles ? (p.ntiles - first + step - 1) / step : 0;
   const int SA = p.nstagesA, SB = p.nstagesB, LAG = p.lag;
-  const bool single = p.single_ring != 0;
   const int last_it = (p.ntiles - 1 - first) % step == 0 ? (p.ntiles - 1 - first) / step : -1;  // the only ragged tile, if this CTA owns it
   unsigned sh0 = smem_u32(smem_raw);
   asm volatile("" : "+r"(sh0));  // one register for every barrier address: do not re-derive the shared-window base at every use
@@ -333,8 +332,7 @@ __device__ __forceinline__ void consumer_lean(const FPParams& p, int warp, int l
   const FastOp& pt = p.pred_fast.term[0];
   const unsigned long long pimm = pt.imm;
   const int ringA_off = TM_HDR_BYTES, stageA = p.stage_bytesA;
-  const int ring2_off = single ? TM_HDR_BYTES : TM_HDR_BYTES + SA * stageA;
-  const int stage2 = single ? stageA : p.stage_bytesB;
+  const int ringB_off = TM_HDR_BYTES + SA * stageA, stageB = p.stage_bytesB;
   const unsigned a1 = sh0 + (unsigned)(ringA_off + p.col_offA[pt.a] + lrow0 * 8);  // shared-window addresses: LDS [R + imm], nothing to derive per tile
   const unsigned b1 = PB ? sh0 + (unsigned)(ringA_off + p.col_offA[pt.b] + lrow0 * 8) : a1;
   unsigned a2[NP], b2[NP];
@@ -347,8 +345,8 @@ __device__ __forceinline__ void consumer_lean(const FPParams& p, int warp, int l
     // -1 copy; op (+0x100: the right operand is the immediate; +0x200: 64-bit integer arithmetic, two's complement wrap-around)
     kop2[q] = fo.kind == 1 ? -1 : ((fo.kind == 2 ? fo.op : fo.op | 0x100) | (fo.ty == DFGPU_FLOAT64 ? 0 : 0x200));
     imm2[q] = fo.imm;
-    a2[q] = sh0 + (unsigned)(ring2_off + p.col_offB[fo.a] + lrow0 * 8);
-    b2[q] = fo.kind == 2 ? sh0 + (unsigned)(ring2_off + p.col_offB[fo.b] + lrow0 * 8) : a2[q];
+    a2[q] = sh0 + (unsigned)(ringB_off + p.col_offB[fo.a] + lrow0 * 8);
+    b2[q] = fo.kind == 2 ? sh0 + (unsigned)(ringB_off + p.col_offB[fo.b] + lrow0 * 8) : a2[q];
     out2[q] = (unsigned long long*)p.out[q];
   }
   bool bad = false;
@@ -378,7 +376,7 @@ __device__ __forceinline__ void consumer_lean(const FPParams& p, int warp, int l
       }
       const unsigned cnt = __reduce_add_sync(0xffffffffu, (unsigned)__popc(f0));
       if (lane == 0) {
-        if (!single) mbar_arrive_a(sh0 + b_emptyA + 8u * sa);  // this warp is done reading the stage
+        mbar_arrive_a(sh0 + b_emptyA + 8u * sa);  // this warp is done reading the stage
         sh.s_cnt[it % TM_RING][warp] = cnt;
         mbar_arrive_a(sh0 + b_cnt + 8u * (it % TM_RING));
       }
@@ -391,20 +389,20 @@ __device__ __forceinline__ void consumer_lean(const FPParams& p, int warp, int l
       const unsigned flags = (unsigned)(fl >> (K * LAG)) & KMASK;
       mbar_wait_a(sh0 + b_pfx + 8u * (j % TM_RING), (j / TM_RING) & 1);
       const unsigned long long base = sh.s_off[j % TM_RING][warp];
-      if (!single) mbar_wait_a(sh0 + b_fullB + 8u * sb, phb);
+      mbar_wait_a(sh0 + b_fullB + 8u * sb, phb);
       // projection values of the K rows of this lane, then the ballot compaction: the rank of a selected row inside the
       // warp's slice (row order: k major, lane minor) is computed while the first projection is stored
       unsigned pos[K];
 #pragma unroll
       for (int q = 0; q < NP; q++) {
-        const unsigned A = a2[q] + (unsigned)(sb * stage2);
+        const unsigned A = a2[q] + (unsigned)(sb * stageB);
         unsigned long long* o = out2[q] + base;
         unsigned long long v[K];
         if (kop2[q] < 0) {
 #pragma unroll
           for (int k = 0; k < K; k++) v[k] = lds64(A + k * 256);
         } else {
-          const unsigned B = b2[q] + (unsigned)(sb * stage2);
+          const unsigned B = b2[q] + (unsigned)(sb * stageB);
           const bool rimm = (kop2[q] & 0x100) != 0;
           const int op = kop2[q] & 0xff;
           unsigned long long y[K];
@@ -450,7 +448,7 @@ __device__ __forceinline__ void consumer_lean(const FPParams& p, int warp, int l
         }
       }
       __syncwarp();
-      if (lane == 0) mbar_arrive_a(sh0 + (single ? b_emptyA : b_emptyB) + 8u * sb);
+      if (lane == 0) mbar_arrive_a(sh0 + b_emptyB + 8u * sb);
       if (++sb == SB) { sb = 0; phb ^= 1u; }
     }
   }
@@ -490,7 +488,7 @@ __device__ __forceinline__ void consumer_lean_dispatch(const FPParams& p, int wa
 // FAST: every program of the query is a fast shape, so the interpreter is not even compiled into
 // this instantiation (fewer registers, smaller code).  FAST + F64ONLY: additionally every operand is
 // Float64, and the per-type dispatch of the fast shapes disappears too (the C2 / C3 kernels).
-template <int DEPTH, int K, bool F64ONLY, bool FAST, bool STASH = false, int LEAN = 0>  // LEAN = number of projections of a lean shape
+template <int DEPTH, int K, bool F64ONLY, bool FAST, int LEAN = 0>  // LEAN = number of projections of a lean shape
 __global__ void __launch_bounds__(TM_THREADS, 1) k_filter_project_tma(const __grid_constant__ FPParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   constexpr int TILE = TM_CWARPS * 32 * K;
@@ -523,16 +521,15 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_filter_project_tma(const __gr
 
   if (warp == TM_CWARPS) {
     // ================================ producer A: predicate columns ============================
-    if (p.has_pred) producer_loop(p, TILE, p.col_offA, STASH ? nullptr : p.col_offB, ringA, SA, p.stage_bytesA, sh.fullA, sh.emptyA, lane);
+    if (p.has_pred) producer_loop(p, TILE, p.col_offA, p.col_offB, ringA, SA, p.stage_bytesA, sh.fullA, sh.emptyA, lane);
   } else if (warp == TM_CWARPS + 1) {
     // ================================ producer B: projection columns ===========================
     // Runs as far ahead as ring B allows; the consumers reach these tiles LAG iterations after the
     // predicate pass touched the same rows, so the bytes are L2 hits.
-    if (!STASH && !p.single_ring) producer_loop(p, TILE, p.col_offB, nullptr, ringB, SB, p.stage_bytesB, sh.fullB, sh.emptyB, lane);
+    producer_loop(p, TILE, p.col_offB, nullptr, ringB, SB, p.stage_bytesB, sh.fullB, sh.emptyB, lane);
   } else if (warp >= TM_CWARPS + 2) {
     // ================================ scan warps ================================================
     if (!p.has_pred) return;  // nothing is dropped: output positions are the row numbers
-    if (STASH && p.noscan) return;
     const int sw = warp - (TM_CWARPS + 2);
     int nloc = 0;
     for (int tile = first; tile < p.ntiles; tile += step) nloc++;
@@ -660,16 +657,9 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_filter_project_tma(const __gr
       }
       flags &= src.valid;
       // rows this warp selected in the tile: one population count per lane, one warp reduction (REDUX)
-      unsigned cnt = 0;
-      if (p.count_ballot) {  // A/B switch (DFGPU_FP_COUNT=ballot): the pre-REDUX form
-#pragma unroll
-        for (int k = 0; k < K; k++) cnt += __popc(__ballot_sync(0xffffffffu, (flags >> k) & 1u));
-        __syncwarp();
-      } else {
-        cnt = __reduce_add_sync(0xffffffffu, (unsigned)__popc(flags));
-      }
+      const unsigned cnt = __reduce_add_sync(0xffffffffu, (unsigned)__popc(flags));
       if (lane == 0) {
-        if (!p.single_ring) mbar_arrive(&sh.emptyA[s]);  // this warp is done reading the stage
+        mbar_arrive(&sh.emptyA[s]);  // this warp is done reading the stage
         sh.s_cnt[it % TM_RING][warp] = cnt;
         mbar_arrive(&sh.cnt_ready[it % TM_RING]);
       }
@@ -686,13 +676,8 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_filter_project_tma(const __gr
         base = (unsigned long long)tile * TILE + (unsigned long long)warp * 32 * K;
       }
       StagedTile<K> src;
-      if (p.single_ring) {
-        // the tile is still resident in ring A (held since the predicate pass): no second load
-        src.stage = ringA + (size_t)s * p.stage_bytesA;
-      } else {
-        mbar_wait(&sh.fullB[s], ph);
-        src.stage = ringB + (size_t)s * p.stage_bytesB;
-      }
+      mbar_wait(&sh.fullB[s], ph);
+      src.stage = ringB + (size_t)s * p.stage_bytesB;
       src.col_off = p.col_offB;
       src.lrow0 = warp * 32 * K + lane;
       src.row0 = (long long)tile * TILE + src.lrow0;
@@ -762,104 +747,14 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_filter_project_tma(const __gr
 #undef DF_STORE_LOOP
       }
       __syncwarp();
-      if (lane == 0) mbar_arrive(p.single_ring ? &sh.emptyA[s] : &sh.emptyB[s]);
-    };
-
-    // ---- stash mode (FAST shapes over 8-byte columns) -----------------------------------------------------
-    // pass 1 of local iteration `it`: predicate, projections, compaction of the selected values into this
-    // tile's slab slot at WARP-LOCAL positions (no global offset needed), stage released at once
-    auto stash1 = [&](int it, int tile, int s, unsigned ph) {
-      mbar_wait(&sh.fullA[s], ph);
-      const unsigned char* stage = ringA + (size_t)s * p.stage_bytesA;
-      const int lrow0 = warp * 32 * K + lane;
-      unsigned valid = KMASK;
-      if (tile == p.ntiles - 1) {  // only the last tile can be ragged
-        const long long row0 = (long long)tile * TILE + lrow0;
-        valid = 0;
-#pragma unroll
-        for (int k = 0; k < K; k++)
-          if (row0 + k * 32 < p.nrows) valid |= 1u << k;
-      }
-      unsigned flags = cmp_term<K, FAST && F64ONLY>(p.pred_fast.term[0], stage, p.col_offA, lrow0);
-      for (int t = 1; t < p.pred_fast.nterms; t++) {
-        const unsigned ft = cmp_term<K, FAST && F64ONLY>(p.pred_fast.term[t], stage, p.col_offA, lrow0);
-        flags = p.pred_fast.conn[t] ? (flags | ft) : (flags & ft);
-      }
-      flags &= valid;
-      // ranks of this lane's selected rows inside the warp's slice of the tile (row order: k major, lane minor)
-      unsigned pos[K];
-      unsigned run = 0;
-#pragma unroll
-      for (int k = 0; k < K; k++) {
-        const unsigned m = __ballot_sync(0xffffffffu, (flags >> k) & 1u);
-        pos[k] = run + __popc(m & lt_mask);
-        run += __popc(m);
-      }
-      unsigned long long* slab_w = p.slab + (((size_t)blockIdx.x * p.slab_slots + (size_t)(it % p.slab_slots)) * p.nproj) * TILE + (size_t)warp * 32 * K;
-      for (int q = 0; q < p.nproj; q++) {
-        const FastOp& fo = p.proj_fast[q];
-        unsigned long long v[K];
-        if (fo.kind < 2) {
-          const unsigned long long* A = (const unsigned long long*)(stage + p.col_offA[fo.a]) + lrow0;
-#pragma unroll
-          for (int k = 0; k < K; k++) v[k] = A[k * 32];
-        } else if (F64ONLY || fo.ty == DFGPU_FLOAT64) {
-          double o[K];
-          arith_term_t<K, double>(fo, stage, p.col_offA, lrow0, u2d(fo.imm), flags, bad, o);
-#pragma unroll
-          for (int k = 0; k < K; k++) v[k] = d2u(o[k]);
-        } else {  // Int64 / UInt64: two's complement wrap-around is the natural 64-bit result
-          unsigned long long o[K];
-          arith_term_t<K, unsigned long long>(fo, stage, p.col_offA, lrow0, fo.imm, flags, bad, o);
-#pragma unroll
-          for (int k = 0; k < K; k++) v[k] = o[k];
-        }
-        unsigned long long* dst = slab_w + (size_t)q * TILE;
-#pragma unroll
-        for (int k = 0; k < K; k++)
-          if ((flags >> k) & 1u) dst[pos[k]] = v[k];
-      }
-      __syncwarp();  // the warp's slab writes are ordered before its later reads (pass 2 runs lanes over other lanes' values)
-      if (lane == 0) {
-        mbar_arrive(&sh.emptyA[s]);
-        sh.s_cnt[it % TM_RING][warp] = run;
-        mbar_arrive(&sh.cnt_ready[it % TM_RING]);
-      }
-      return run;
-    };
-    // pass 2: the warp's `cnt` stashed values go to their final place; coalesced both ways
-    auto stash2 = [&](int it, unsigned cnt) {
-      mbar_wait(&sh.pfx_ready[it % TM_RING], (it / TM_RING) & 1);
-      const unsigned long long base = sh.s_off[it % TM_RING][warp];
-      const unsigned long long* slab_w = p.slab + (((size_t)blockIdx.x * p.slab_slots + (size_t)(it % p.slab_slots)) * p.nproj) * TILE + (size_t)warp * 32 * K;
-      for (int q = 0; q < p.nproj; q++) {
-        const unsigned long long* src = slab_w + (size_t)q * TILE;
-        unsigned long long* dst = (unsigned long long*)p.out[q] + base;
-        unsigned long long v[K];
-#pragma unroll
-        for (int k = 0; k < K; k++)
-          if ((unsigned)(k * 32 + lane) < cnt) v[k] = __ldcg(src + k * 32 + lane);
-#pragma unroll
-        for (int k = 0; k < K; k++)
-          if ((unsigned)(k * 32 + lane) < cnt) dst[k * 32 + lane] = v[k];
-      }
+      if (lane == 0) mbar_arrive(&sh.emptyB[s]);
     };
 
     int nloc = 0;
     for (int tile = first; tile < p.ntiles; tile += step) nloc++;
     int sb = 0;
     unsigned phb = 0;
-    if (STASH) {
-      int sa = 0;
-      unsigned pha = 0;
-      for (int it = 0; it < nloc + LAG; it++) {
-        if (it < nloc) {
-          stash1(it, first + it * step, sa, pha);
-          if (++sa == SA) { sa = 0; pha ^= 1u; }
-        }
-        if (it >= LAG && !p.noscan) stash2(it - LAG, sh.s_cnt[(it - LAG) % TM_RING][warp]);  // the warp's own count, published LAG tiles ago
-      }
-    } else if (!p.has_pred) {
+    if (!p.has_pred) {
       // pure projection: no predicate pass, no lag
       for (int it = 0; it < nloc; it++) {
         const int tile = first + it * step;
@@ -897,9 +792,9 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_filter_project_tma(const __gr
   }
 }
 
-template <int DEPTH, int K, bool F64ONLY, bool FAST, bool STASH = false, int LEAN = 0>
+template <int DEPTH, int K, bool F64ONLY, bool FAST, int LEAN = 0>
 static void launch_one(dfgpu_ctx* ctx, const FPParams& p, size_t smem) {
-  auto kern = k_filter_project_tma<DEPTH, K, F64ONLY, FAST, STASH, LEAN>;
+  auto kern = k_filter_project_tma<DEPTH, K, F64ONLY, FAST, LEAN>;
   if (ctx->first_use((const void*)kern))
     DF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TM_SMEM_BUDGET + 16384 + TM_HDR_BYTES));
   long long grid = std::min(ctx->sm_count, TM_MAX_GRID);  // one persistent CTA per SM
@@ -920,13 +815,11 @@ static void launch_k(dfgpu_ctx* ctx, const FPParams& p, size_t smem) {
   for (int c = 0; c < p.ps.ncols; c++) all_f64 = all_f64 && p.ps.cols[c].dtype == DFGPU_FLOAT64;
   // lean shapes: one comparison over 8-byte operands (Float64 / Int64 / UInt64), one or two copy / arithmetic projections over 8-byte columns (DFGPU_FP_LEAN=0: A/B switch)
   auto w8 = [](int dt) { return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64; };
-  bool lean = fast && p.has_pred && p.pred_fast.nterms == 1 && w8(p.pred_fast.term[0].ty) && p.nproj >= 1 && p.nproj <= LEAN_MAX_PROJ && !p.slab && !p.count_ballot;
+  bool lean = fast && p.has_pred && p.pred_fast.nterms == 1 && w8(p.pred_fast.term[0].ty) && p.nproj >= 1 && p.nproj <= LEAN_MAX_PROJ;
   for (int q = 0; lean && q < p.nproj; q++) lean = w8(p.proj_fast[q].ty);  // copies and arithmetic over 8-byte columns only
   if (const char* e = getenv("DFGPU_FP_LEAN")) lean = lean && atoi(e) != 0;
-  if (lean && p.nproj == 1) launch_one<1, K, true, true, false, 1>(ctx, p, smem);
-  else if (lean) launch_one<1, K, true, true, false, 2>(ctx, p, smem);
-  else if (p.slab && all_f64) launch_one<1, K, true, true, true>(ctx, p, smem);
-  else if (p.slab) launch_one<1, K, false, true, true>(ctx, p, smem);
+  if (lean && p.nproj == 1) launch_one<1, K, true, true, 1>(ctx, p, smem);
+  else if (lean) launch_one<1, K, true, true, 2>(ctx, p, smem);
   else if (fast && all_f64) launch_one<1, K, true, true>(ctx, p, smem);
   else if (fast) launch_one<1, K, false, true>(ctx, p, smem);
   else if (p.ps.f64_only) launch_one<DEPTH, K, true, false>(ctx, p, smem);
@@ -953,94 +846,24 @@ bool launch_fp_tma(dfgpu_ctx* ctx, FPParams& p) {
   }
   // projections of literals only, or a predicate over literals only: leave to the direct kernel
   if (rowB == 0 || (p.has_pred && rowA == 0)) return false;
-  // Two layouts.
-  //  single ring: one ring holds the UNION of the referenced columns; a tile stays staged from its
-  //    predicate pass until its projection pass LAG tiles later (no second load).  Needs LAG + 2 stages,
-  //    so it is used when the union is narrow enough for >= 6 stages of a >= 1024-row tile.
-  //  dual ring: ring A = predicate columns, ring B = projection columns re-read LAG tiles later from
-  //    L2 (evict_last / evict_first hints).  Any width; the lag can be long.
-  int rowU = 0;
-  for (int c = 0; c < p.ps.ncols; c++)
-    if (inA[c] || inB[c]) rowU += p.col_w[c];
-  const char* mode = getenv("DFGPU_FP_MODE");  // experiment knob: single | dual | stash
+  // Layout: ring A holds the predicate's columns, ring B the projections' columns.  A column in both rings is
+  // loaded evict_last by producer A and re-read from L2 by producer B LAG tiles later; every other load is
+  // evict_first.  Any width; the lag can be long.
+  // Rows per lane K in {8,4,2}: the biggest tile that still gives both rings 3 stages.  Per-tile fixed
+  // costs (barrier hand-offs, offset gather) outweigh deeper prefetch, so bigger tiles with few stages
+  // beat smaller tiles with many.
   int K = 0;
-  p.single_ring = 0;
-  p.slab = nullptr;
-  p.slab_slots = 0;
-  p.noscan = getenv("DFGPU_FP_NOSCAN") && atoi(getenv("DFGPU_FP_NOSCAN")) != 0;
-  // stash mode: every program a fast shape over 8-byte columns with 8-byte results
-  // (opt-in, DFGPU_FP_MODE=stash: slower than the dual ring at 50 % selectivity, equal at 1 %, where it was measured)
-  bool stash = p.has_pred && p.pred_fast.nterms > 0 && mode && std::string(mode) == "stash";
-  for (int q = 0; stash && q < p.nproj; q++) {
-    const FastOp& fo = p.proj_fast[q];
-    stash = fo.kind > 0 && dtype_width(p.ps.out_dtype[q + p.has_pred]) == 8 &&
-            (fo.kind < 2 || fo.ty == DFGPU_FLOAT64 || fo.ty == DFGPU_INT64 || fo.ty == DFGPU_UINT64);
-  }
-  for (int c = 0; stash && c < p.ps.ncols; c++) stash = !(inA[c] || inB[c]) || p.col_w[c] == 8;
-  if (stash) {
-    for (int k : {8, 4, 2}) {
-      const long long tile = (long long)TM_CWARPS * 32 * k;
-      if (tile * rowU * 3 <= TM_SMEM_BUDGET) { K = k; break; }
-    }
-    if (!K) stash = false;
-  }
-  if (stash) {
-    const int tile = TM_CWARPS * 32 * K;
-    int off = 0;
-    for (int c = 0; c < p.ps.ncols; c++) {
-      p.col_offA[c] = (inA[c] || inB[c]) ? off : -1;
-      p.col_offB[c] = -1;
-      if (inA[c] || inB[c]) off += tile * p.col_w[c];
-    }
-    p.stage_bytesA = off;
-    p.stage_bytesB = 0;
-    p.nstagesA = std::min(TM_MAX_STAGES, TM_SMEM_BUDGET / off);
-    p.nstagesB = 0;
-    const long long grid = std::min(ctx->sm_count, TM_MAX_GRID);
-    // lag: the slab slots the grid keeps live (lag x grid x nproj x tile x 8 bytes, about half of it touched at
-    // 50 % selectivity) should stay L2 resident
-    const long long slot_bytes = grid * p.nproj * (long long)tile * 8;
-    p.lag = (int)std::min<long long>(TM_MAX_LAG, std::max<long long>(TM_BATCH, (32ll << 20) / slot_bytes));
-    if (const char* e = getenv("DFGPU_FP_LAG")) {
-      const int l = atoi(e);
-      if (l >= TM_BATCH - 1 && l <= TM_MAX_LAG) p.lag = l;
-    }
-    p.slab_slots = p.lag + 2;
-    p.slab = (unsigned long long*)ctx->alloc(size_t(grid) * size_t(p.slab_slots) * size_t(slot_bytes / grid));
-    p.ntiles = int((p.nrows + tile - 1) / tile);
-    p.count_ballot = 0;
-    const size_t smem = TM_HDR_BYTES + (size_t)p.nstagesA * p.stage_bytesA;
-    if (K == 8) launch_k<2, 8>(ctx, p, smem);
-    else if (K == 4) launch_k<2, 4>(ctx, p, smem);
-    else launch_k<2, 2>(ctx, p, smem);
-    ctx->free(p.slab);  // stream ordered: the block is only handed out again to work queued behind this kernel
-    return true;
-  }
-  if (p.has_pred && mode && std::string(mode) == "single") {  // slower than dual where it was measured: opt-in only
-    for (int k : {8, 4, 2}) {
-      if (k == 8 && p.ps.max_depth > 2) continue;
-      const long long tile = (long long)TM_CWARPS * 32 * k;
-      if (tile * rowU * 6 <= TM_SMEM_BUDGET + 16384) { K = k; p.single_ring = 1; break; }
-    }
-  }
-  if (!p.single_ring) {
-    // rows per lane K in {8,4,2}: the biggest tile that still gives both rings 3 stages.  Per-tile fixed
-    // costs (barrier hand-offs, offset gather) outweigh deeper prefetch, so bigger tiles with few stages
-    // beat smaller tiles with many.
-    for (int k : {8, 4, 2}) {
-      if (k == 8 && p.ps.max_depth > 2) continue;  // deep register stacks spill at 8 rows per lane
-      const long long tile = (long long)TM_CWARPS * 32 * k;
-      if (tile * (rowA + rowB) * 3 <= TM_SMEM_BUDGET) { K = k; break; }
-    }
+  for (int k : {8, 4, 2}) {
+    if (k == 8 && p.ps.max_depth > 2) continue;  // deep register stacks spill at 8 rows per lane
+    const long long tile = (long long)TM_CWARPS * 32 * k;
+    if (tile * (rowA + rowB) * 3 <= TM_SMEM_BUDGET) { K = k; break; }
   }
   if (const char* e = getenv("DFGPU_FP_K")) {  // experiment knob
     const int k = atoi(e);
-    if (!p.single_ring && (k == 8 || k == 4 || k == 2) && (long long)TM_CWARPS * 32 * k * (rowA + rowB) * 2 <= TM_SMEM_BUDGET && !(k == 8 && p.ps.max_depth > 2)) K = k;
+    if ((k == 8 || k == 4 || k == 2) && (long long)TM_CWARPS * 32 * k * (rowA + rowB) * 2 <= TM_SMEM_BUDGET && !(k == 8 && p.ps.max_depth > 2)) K = k;
   }
   if (!K) return false;
   const int tile = TM_CWARPS * 32 * K;
-  if (p.single_ring)
-    for (int c = 0; c < p.ps.ncols; c++) inA[c] = inB[c] = inA[c] || inB[c];
   int offA = 0, offB = 0;
   for (int c = 0; c < p.ps.ncols; c++) {
     // tile is a multiple of 512 rows: every column slice stays 128-B aligned
@@ -1051,49 +874,33 @@ bool launch_fp_tma(dfgpu_ctx* ctx, FPParams& p) {
   }
   p.stage_bytesA = offA;
   p.stage_bytesB = offB;
-  if (p.single_ring) {
-    p.nstagesA = std::min(TM_MAX_STAGES, (TM_SMEM_BUDGET + 16384) / offA);
-    p.nstagesB = p.nstagesA;  // the projection pass walks the same ring
-    p.stage_bytesB = 0;
-    p.lag = p.nstagesA - 3;  // LAG+1 stages are held by the consumers, 2 are prefetch depth
-    if (p.lag < TM_BATCH - 1) return false;
-    if (const char* e = getenv("DFGPU_FP_LAG")) {
-      const int l = atoi(e);
-      if (l >= TM_BATCH - 1 && l <= p.nstagesA - 2) p.lag = l;
+  const int S = std::min(TM_MAX_STAGES, TM_SMEM_BUDGET / (offA + offB));
+  p.nstagesA = offA ? S : 0;
+  p.nstagesB = S;
+  if (!p.has_pred) p.nstagesB = std::min(TM_MAX_STAGES, TM_SMEM_BUDGET / offB);
+  if (const char* e = getenv("DFGPU_FP_STAGES")) {  // experiment knob: "A,B"
+    int sa = 0, sb = 0;
+    if (sscanf(e, "%d,%d", &sa, &sb) == 2 && sa >= 1 && sb >= 1 && sa <= TM_MAX_STAGES && sb <= TM_MAX_STAGES &&
+        (long long)sa * offA + (long long)sb * offB <= TM_SMEM_BUDGET + 16384 && p.has_pred) {
+      p.nstagesA = sa;
+      p.nstagesB = sb;
     }
-  } else {
-    const int S = std::min(TM_MAX_STAGES, TM_SMEM_BUDGET / (offA + offB));
-    p.nstagesA = offA ? S : 0;
-    p.nstagesB = S;
-    if (!p.has_pred) p.nstagesB = std::min(TM_MAX_STAGES, TM_SMEM_BUDGET / offB);
-    if (const char* e = getenv("DFGPU_FP_STAGES")) {  // experiment knob: "A,B"
-      int sa = 0, sb = 0;
-      if (sscanf(e, "%d,%d", &sa, &sb) == 2 && sa >= 1 && sb >= 1 && sa <= TM_MAX_STAGES && sb <= TM_MAX_STAGES &&
-          (long long)sa * offA + (long long)sb * offB <= TM_SMEM_BUDGET + 16384 && p.has_pred) {
-        p.nstagesA = sa;
-        p.nstagesB = sb;
-      }
-    }
-    // lag: as large as the flag shift register allows (K bits per tile in 64 bits), but the bytes the
-    // projection stream will re-read (lag x grid x stage B) must still be in L2 when it gets there
-    // On H100 (132 SMs, 50 MB L2) the shortest lag the scan warps allow was fastest for C2 and C3, whose
-    // projection stages re-read about 4 MB per wave (profiles/microbench_fp.py under DFGPU_FP_LAG=3..12).
-    p.lag = 0;
-    if (p.has_pred) {
-      const long long l2_budget = 12ll << 20;  // a quarter of the 50 MB L2
-      const long long per_tile = (long long)std::min(ctx->sm_count, TM_MAX_GRID) * offB;
-      p.lag = (int)std::min<long long>(std::min(TM_MAX_LAG, 128 / K - 1), std::max<long long>(TM_BATCH - 1, l2_budget / per_tile));
-    }
-    if (const char* e = getenv("DFGPU_FP_LAG")) {  // experiment knob
-      const int l = atoi(e);
-      if (p.has_pred && l >= TM_BATCH - 1 && l <= std::min(TM_MAX_LAG, 128 / K - 1)) p.lag = l;
-    }
+  }
+  // lag: as large as the flag shift register allows (K bits per tile in 64 bits), but the bytes the
+  // projection stream will re-read (lag x grid x stage B) must still be in L2 when it gets there
+  // On H100 (132 SMs, 50 MB L2) the shortest lag the scan warps allow was fastest for C2 and C3, whose
+  // projection stages re-read about 4 MB per wave (profiles/microbench_fp.py under DFGPU_FP_LAG=3..12).
+  p.lag = 0;
+  if (p.has_pred) {
+    const long long l2_budget = 12ll << 20;  // a quarter of the 50 MB L2
+    const long long per_tile = (long long)std::min(ctx->sm_count, TM_MAX_GRID) * offB;
+    p.lag = (int)std::min<long long>(std::min(TM_MAX_LAG, 128 / K - 1), std::max<long long>(TM_BATCH - 1, l2_budget / per_tile));
+  }
+  if (const char* e = getenv("DFGPU_FP_LAG")) {  // experiment knob
+    const int l = atoi(e);
+    if (p.has_pred && l >= TM_BATCH - 1 && l <= std::min(TM_MAX_LAG, 128 / K - 1)) p.lag = l;
   }
   p.ntiles = int((p.nrows + tile - 1) / tile);
-  {
-    const char* e = getenv("DFGPU_FP_COUNT");
-    p.count_ballot = (e && std::string(e) == "ballot") ? 1 : 0;
-  }
   const size_t smem = TM_HDR_BYTES + (size_t)p.nstagesA * p.stage_bytesA + (size_t)p.nstagesB * p.stage_bytesB;
   const int d = p.ps.max_depth;
   if (K == 8) launch_k<2, 8>(ctx, p, smem);
