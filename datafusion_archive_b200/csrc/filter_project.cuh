@@ -51,7 +51,8 @@ struct FPParams {
   int col_w[kMaxCols];  // element width of column slot s
   int stage_bytesA, stage_bytesB;
   int nstagesA, nstagesB;
-  int lag;  // tiles between the predicate pass and the projection pass
+  int lag;    // tiles between the predicate pass and the projection pass
+  int delay;  // waves between publishing a tile's count and resolving the offsets of its wave (1 <= delay <= lag)
   // "fast shapes": single-operation programs over 4- and 8-byte numeric columns are recognised on the host and executed by
   // straight-line code instead of the interpreter (same arithmetic, no decode in the inner loop).
   //   predicate : chain of (COL cmp COL | COL cmp IMM) joined by AND / OR

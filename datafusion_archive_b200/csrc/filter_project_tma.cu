@@ -11,8 +11,8 @@
 //   16 consumer warps   : phase 1 = predicate of tile it over ring A -> K flag bits per lane, kept in
 //                         a 64-bit shift register; phase 2 = projections of tile it-LAG over ring B,
 //                         selected rows stored at their compacted global position
-//   2 scan warps        : turn the per-warp counts of a tile into global output offsets, 4 waves per
-//                         warp at a time (8 cross-CTA gathers in flight per SM)
+//   1 scan warp         : turns the per-warp counts of a tile into global output offsets, one wave per
+//                         step, a fixed delay behind publishing the counts
 //
 // Why the lag: order-preserving compaction needs, per tile, the number of selected rows in ALL
 // earlier tiles.  Under a bandwidth-saturating stream every dependent global round trip costs
@@ -21,14 +21,15 @@
 // only produces 1 bit per row, runs LAG tiles ahead; by the time the projection pass reaches a
 // tile its offset has long been resolved, and the tile's bytes come back from L2, not HBM.
 //
-// The lag must be >= TM_BATCH - 1: a scan warp waits for the counts of a whole batch of waves, and the
-// consumers only reach the projection pass of wave w after the predicate pass of wave w + LAG.
-//
-// Offsets: every scan warp publishes its tile's count, then GATHERS the counts of all G tiles of
-// its wave with one batch of parallel loads: offset = base + sum(counts of lower CTAs); base
-// advances by the wave total, computed redundantly by every CTA (nothing is forwarded between
-// waves through memory).  The scan warps take batches of waves round-robin; the
-// running base is handed from wave to wave through shared memory.
+// Offsets: in step w the scan warp publishes the count of its tile of wave w to tile_status, then
+// RESOLVES wave w - D: it gathers the counts of all G tiles of that wave (offset = base + sum(counts
+// of lower CTAs) + the warp's offset inside the tile); base advances by the wave total, computed
+// redundantly by every CTA (nothing is forwarded between waves through memory).  The status loads
+// of wave w - D are issued before the step waits for the counts of wave w, so their L2 round trip
+// overlaps the predicate pass; every CTA published wave w - D about D waves earlier, so a re-poll
+// of a status not yet written is rare.  The offsets of wave j are ready right after the counts of
+// wave j + D, so the lag must be >= D (the consumers reach the projection pass of wave j right
+// after the predicate pass of wave j + LAG), and every wave gets the same slack.
 //
 // Nothing in the CTA executes __syncthreads in the steady state; all hand-offs are mbarriers.
 // Reference path replaced: src/execution/filter.rs:46-110 + src/execution/projection.rs:46-66.
@@ -37,16 +38,18 @@
 namespace dfgpu {
 
 constexpr int TM_CWARPS = 16;  // consumer warps
-constexpr int TM_SWARPS = 2;   // scan warps (2 x TM_BATCH gathers in flight; 20 warps = 5 per SM sub-partition leave 96 registers per thread; a third scan warp would put 6 warps on one sub-partition and cap the kernel at 80 registers)
-#ifndef DF_TM_BATCH
-#define DF_TM_BATCH 4
-#endif
-constexpr int TM_BATCH = DF_TM_BATCH;  // waves per scan-warp batch: more waves per batch put more gathers in flight; issuing a wave's gather right behind its own publish is slower (statuses read right after the publish are stale and the re-poll is serial)
-constexpr int TM_WARPS = TM_CWARPS + 2 + TM_SWARPS;
+// one scan warp: its status loads fly while it waits for the next tile's counts, so a second warp taking every
+// other wave was 2-8 % slower on H100 (C2, C3).  19 warps leave 96 registers per thread, as 20 did.
+constexpr int TM_WARPS = TM_CWARPS + 2 + 1;
 constexpr int TM_THREADS = TM_WARPS * 32;
 constexpr int TM_MAX_STAGES = 8;
-constexpr int TM_RING = 32;       // slots of the count/offset hand-off rings (> max lag + 1)
 constexpr int TM_MAX_LAG = 24;
+constexpr int TM_MAX_DELAY = 8;
+// slots of the count/offset hand-off rings.  The slot of wave w is reused by wave w + TM_RING, whose publish
+// rewrites s_off; that publish waits for the counts of wave w + TM_RING, which the consumers only report after
+// reading the offsets of wave w + TM_RING - 1 - lag.  So TM_RING >= lag + 1 keeps every slot alive until read.
+constexpr int TM_RING = 32;
+static_assert(TM_RING >= TM_MAX_LAG + 1, "hand-off ring too short for the longest lag");
 constexpr int TM_MAX_GRID = 160;  // CTAs (= SMs) the wave gather is written for (H100 SXM: 132)
 constexpr int TM_HDR_BYTES = 8192;
 constexpr int TM_SMEM_BUDGET = 200 * 1024;
@@ -122,8 +125,6 @@ struct TmaShared {
   unsigned long long fullB[TM_MAX_STAGES], emptyB[TM_MAX_STAGES];  // ring B (projection columns)
   unsigned long long cnt_ready[TM_RING];   // consumers -> scan warp: per-warp counts of a tile are in s_cnt
   unsigned long long pfx_ready[TM_RING];   // scan warp -> consumers: global offsets of a tile are in s_off
-  unsigned long long base_ready[TM_RING];  // scan warp of wave it-1 -> scan warp of wave it
-  unsigned long long s_base[TM_RING];
   unsigned long long s_off[TM_RING][TM_CWARPS];
   unsigned s_cnt[TM_RING][TM_CWARPS];
 };
@@ -245,7 +246,7 @@ __device__ __forceinline__ void arith_term_t(const FastOp& t, const unsigned cha
 // operator, generic -> shared address conversions in front of every mbarrier operation — and their dependent
 // latencies are what the 4 consumer warps per scheduler cannot hide.  Here the comparison operator and the operand kind are template
 // parameters, every offset, pointer and barrier address is computed once before the loop, and the loop body is
-// waits + loads + compares + the ballot-compacted store.  Protocol (barriers, rings, scan warps) unchanged.
+// waits + loads + compares + the ballot-compacted store.  Protocol (barriers, rings, scan warp) unchanged.
 template <int CMP, class T>
 __device__ __forceinline__ bool lean_cmp_t(T a, T b) {
   if (CMP == V_EQ) return a == b;
@@ -509,11 +510,8 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_filter_project_tma(const __gr
     for (int i = 0; i < TM_RING; i++) {
       mbar_init(&sh.cnt_ready[i], TM_CWARPS);
       mbar_init(&sh.pfx_ready[i], 1);
-      mbar_init(&sh.base_ready[i], 1);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    sh.s_base[0] = 0;  // wave 0 starts from offset 0: its hand-off is pre-completed here
-    mbar_arrive(&sh.base_ready[0]);
   }
   __syncthreads();
 
@@ -527,92 +525,69 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_filter_project_tma(const __gr
     // Runs as far ahead as ring B allows; the consumers reach these tiles LAG iterations after the
     // predicate pass touched the same rows, so the bytes are L2 hits.
     producer_loop(p, TILE, p.col_offB, nullptr, ringB, SB, p.stage_bytesB, sh.fullB, sh.emptyB, lane);
-  } else if (warp >= TM_CWARPS + 2) {
-    // ================================ scan warps ================================================
+  } else if (warp == TM_CWARPS + 2) {
+    // ================================ scan warp =================================================
     if (!p.has_pred) return;  // nothing is dropped: output positions are the row numbers
-    const int sw = warp - (TM_CWARPS + 2);
+    const int D = p.delay;
     int nloc = 0;
     for (int tile = first; tile < p.ntiles; tile += step) nloc++;
-    // Each scan warp owns batches of TM_BATCH consecutive waves (batch j -> warp j % TM_SWARPS), so
-    // TM_SWARPS * TM_BATCH gathers are in flight per CTA: one gather is a full L2 round trip under
-    // load, several times longer than a tile.
-    for (int w0 = sw * TM_BATCH; w0 < nloc; w0 += TM_SWARPS * TM_BATCH) {
-      const int nb = min(TM_BATCH, nloc - w0);
-      unsigned excl[TM_BATCH];
-      unsigned long long total[TM_BATCH];
-      // 1. per-tile counts -> exclusive per-warp offsets, publish the tile totals
-      unsigned long long sv[TM_BATCH][TM_MAX_GRID / 32];
+    unsigned long long base = 0;  // selected rows in all waves before the one being resolved
+    // Step w publishes wave w and resolves wave w - D; the last D steps only resolve.
+    for (int w = 0; w < nloc + D; w++) {
+      const int v = w - D;  // the wave this step resolves
+      const long long wave0 = (long long)v * step;
+      // 1. the statuses of every tile of wave v, all loads issued before this step waits for its own counts:
+      //    the L2 round trip overlaps the predicate pass of wave w
+      unsigned long long sv[TM_MAX_GRID / 32];
 #pragma unroll
-      for (int i = 0; i < TM_BATCH; i++) {
-        excl[i] = 0;
-        total[i] = 0;
-        if (i < nb) {
-          const int it = w0 + i, b = it % TM_RING;
-          mbar_wait(&sh.cnt_ready[b], (it / TM_RING) & 1);
-          const unsigned c = lane < TM_CWARPS ? sh.s_cnt[b][lane] : 0u;
-          unsigned incl = c;
-#pragma unroll
-          for (int o = 1; o < 32; o <<= 1) {
-            const unsigned t = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += t;
-          }
-          excl[i] = incl - c;
-          total[i] = __shfl_sync(0xffffffffu, incl, 31);
-          if (lane == 0) st_relaxed(&p.tile_status[first + it * step], ST_AGG | total[i]);
-        }
+      for (int g = 0; g < TM_MAX_GRID / 32; g++) {
+        const int j = g * 32 + lane;
+        sv[g] = (v >= 0 && j < step && wave0 + j < p.ntiles) ? ld_relaxed(&p.tile_status[wave0 + j]) : ST_AGG;
       }
-      // 2. gather the counts of every tile of these waves: all loads issued before any is used
+      // 2. publish wave w: per-warp counts -> exclusive offsets inside the tile, parked in s_off until the wave is
+      //    resolved; the tile total goes to tile_status
+      if (w < nloc) {
+        const int b = w % TM_RING;
+        mbar_wait(&sh.cnt_ready[b], (w / TM_RING) & 1);
+        const unsigned c = lane < TM_CWARPS ? sh.s_cnt[b][lane] : 0u;
+        unsigned incl = c;
 #pragma unroll
-      for (int i = 0; i < TM_BATCH; i++) {
-        const long long wave0 = (long long)(w0 + i) * step;
-#pragma unroll
-        for (int w = 0; w < TM_MAX_GRID / 32; w++) {
-          const int j = w * 32 + lane;
-          const long long idx = wave0 + j;
-          sv[i][w] = (i < nb && w * 32 < step && j < step && idx < p.ntiles) ? ld_relaxed(&p.tile_status[idx]) : ST_AGG;
+        for (int o = 1; o < 32; o <<= 1) {
+          const unsigned t = __shfl_up_sync(0xffffffffu, incl, o);
+          if (lane >= o) incl += t;
         }
+        const unsigned total = __shfl_sync(0xffffffffu, incl, 31);
+        if (lane == 0) st_relaxed(&p.tile_status[first + w * step], ST_AGG | total);
+        if (lane < TM_CWARPS) sh.s_off[b][lane] = incl - c;
       }
-      unsigned long long before[TM_BATCH], wave_total[TM_BATCH];
+      if (v < 0) continue;
+      // 3. resolve wave v: re-poll only the statuses that were still unpublished, all of them at once
+      for (;;) {
+        bool missing = false;
 #pragma unroll
-      for (int i = 0; i < TM_BATCH; i++) {
-        const long long wave0 = (long long)(w0 + i) * step;
-        unsigned long long bf = 0, wt = 0;
-#pragma unroll
-        for (int w = 0; w < TM_MAX_GRID / 32; w++) {
-          if (i < nb && w * 32 < step) {
-            const int j = w * 32 + lane;
-            const long long idx = wave0 + j;
-            while (__any_sync(0xffffffffu, (sv[i][w] >> 62) == 0)) {
-              if ((sv[i][w] >> 62) == 0) sv[i][w] = ld_relaxed(&p.tile_status[idx]);
-            }
-            const unsigned long long v = sv[i][w] & ST_MASK;
-            wt += v;
-            if (j < (int)blockIdx.x) bf += v;
+        for (int g = 0; g < TM_MAX_GRID / 32; g++) {
+          if ((sv[g] >> 62) == 0) {
+            missing = true;
+            sv[g] = ld_relaxed(&p.tile_status[wave0 + g * 32 + lane]);
           }
         }
-        before[i] = warp_sum64(bf);
-        wave_total[i] = warp_sum64(wt);
+        if (!__any_sync(0xffffffffu, missing)) break;
       }
-      // 3. running base: handed from the scan warp of the previous batch through shared memory
-      const int hb = (w0 / TM_BATCH) % TM_RING;
-      mbar_wait(&sh.base_ready[hb], ((w0 / TM_BATCH) / TM_RING) & 1);
-      unsigned long long base = sh.s_base[hb];
+      unsigned long long bf = 0, wt = 0;
 #pragma unroll
-      for (int i = 0; i < TM_BATCH; i++) {
-        if (i < nb) {
-          const int it = w0 + i, b = it % TM_RING;
-          if (lane < TM_CWARPS) sh.s_off[b][lane] = base + before[i] + excl[i];
-          if (lane == 0 && first + it * step == p.ntiles - 1) *p.out_count = base + before[i] + total[i];
-          base += wave_total[i];
-        }
+      for (int g = 0; g < TM_MAX_GRID / 32; g++) {
+        const unsigned long long c = sv[g] & ST_MASK;
+        wt += c;
+        if (g * 32 + lane < (int)blockIdx.x) bf += c;
       }
+      const unsigned long long before = warp_sum64(bf), wave_total = warp_sum64(wt);
+      const int b = v % TM_RING;
+      if (lane < TM_CWARPS) sh.s_off[b][lane] += base + before;
+      base += wave_total;
+      // the last tile is the highest of its wave: everything up to and including it is the new base
+      if (lane == 0 && first + v * step == p.ntiles - 1) *p.out_count = base;
       __syncwarp();
-      if (lane == 0) {
-        const int nh = (w0 / TM_BATCH + 1) % TM_RING;
-        sh.s_base[nh] = base;
-        mbar_arrive(&sh.base_ready[nh]);
-        for (int i = 0; i < nb; i++) mbar_arrive(&sh.pfx_ready[(w0 + i) % TM_RING]);
-      }
+      if (lane == 0) mbar_arrive(&sh.pfx_ready[b]);
     }
   } else if constexpr (LEAN > 0) {
     // ================================ consumer warps, lean shapes ================================
@@ -886,19 +861,30 @@ bool launch_fp_tma(dfgpu_ctx* ctx, FPParams& p) {
       p.nstagesB = sb;
     }
   }
-  // lag: as large as the flag shift register allows (K bits per tile in 64 bits), but the bytes the
-  // projection stream will re-read (lag x grid x stage B) must still be in L2 when it gets there
-  // On H100 (132 SMs, 50 MB L2) the shortest lag the scan warps allow was fastest for C2 and C3, whose
-  // projection stages re-read about 4 MB per wave (profiles/microbench_fp.py under DFGPU_FP_LAG=3..12).
+  // delay: the scan warp resolves wave w - delay right after publishing wave w.  Its status loads are issued one
+  // wave-time after the wave was published locally, so at delay 2 the other CTAs have published it too and the
+  // re-poll is rare; delay 1 reads statuses the slower CTAs have not written yet (C3: 0.90 -> 0.86 ms at 2).
+  // lag: at least the delay (the consumers wait for the offsets of tile it - lag right after reporting the
+  // counts of tile it, and those are resolved in the scan step of tile it - lag + delay), as large as the flag
+  // shift register allows (K bits per tile in 128 bits), but the bytes the projection stream will re-read
+  // (lag x grid x stage B) must still be in L2 when it gets there.  On H100 (132 SMs, 50 MB L2) lag = delay = 2
+  // was fastest for C2 and C3, whose projection stages re-read about 4.3 MB per wave; every extra wave of lag
+  // cost 5-15 % (profiles/sweep_fp_lean.sh).
   p.lag = 0;
+  p.delay = 2;
+  if (const char* e = getenv("DFGPU_FP_DELAY")) {  // experiment knob
+    const int d = atoi(e);
+    if (d >= 1 && d <= TM_MAX_DELAY) p.delay = d;
+  }
+  const int max_lag = std::min(TM_MAX_LAG, 128 / K - 1);
   if (p.has_pred) {
     const long long l2_budget = 12ll << 20;  // a quarter of the 50 MB L2
     const long long per_tile = (long long)std::min(ctx->sm_count, TM_MAX_GRID) * offB;
-    p.lag = (int)std::min<long long>(std::min(TM_MAX_LAG, 128 / K - 1), std::max<long long>(TM_BATCH - 1, l2_budget / per_tile));
+    p.lag = (int)std::min<long long>(max_lag, std::max<long long>(p.delay, l2_budget / per_tile));
   }
   if (const char* e = getenv("DFGPU_FP_LAG")) {  // experiment knob
     const int l = atoi(e);
-    if (p.has_pred && l >= TM_BATCH - 1 && l <= std::min(TM_MAX_LAG, 128 / K - 1)) p.lag = l;
+    if (p.has_pred && l >= p.delay && l <= max_lag) p.lag = l;
   }
   p.ntiles = int((p.nrows + tile - 1) / tile);
   const size_t smem = TM_HDR_BYTES + (size_t)p.nstagesA * p.stage_bytesA + (size_t)p.nstagesB * p.stage_bytesB;
