@@ -1385,6 +1385,12 @@ struct Trace {
   }
 };
 
+// DFGPU_TRACE: name each scan, reduce and re-layout kernel as it is launched, template arguments included, so
+// that a run shows which instantiation the dispatch chose (the GROUP BY kernel tests assert it)
+void trace_launch(const char* kernel) {
+  if (getenv("DFGPU_TRACE")) fprintf(stderr, "[dfgpu trace] launch %s\n", kernel);
+}
+
 long long next_pow2(long long x) {
   long long p = 1;
   while (p < x) p <<= 1;
@@ -1506,6 +1512,7 @@ void table_grow(dfgpu_aggstate* st, long long new_cap) {
   cp.counter = st->d_counters + 4;
   k_compact<<<grid_for(ctx, st->cap + 1, 256, 8), 256, 0, ctx->stream>>>(cp);
   DF_CUDA(cudaGetLastError());
+  trace_launch("k_compact");
   ctx->launches++;
   MergeParams mp;
   memset(&mp, 0, sizeof(mp));
@@ -1523,6 +1530,7 @@ void table_grow(dfgpu_aggstate* st, long long new_cap) {
   if (mp.n > 0) {
     k_merge<<<grid_for(ctx, mp.n, 256, 8), 256, 0, ctx->stream>>>(mp);
     DF_CUDA(cudaGetLastError());
+    trace_launch("k_merge");
     ctx->launches++;
   }
   DF_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1538,7 +1546,7 @@ void table_grow(dfgpu_aggstate* st, long long new_cap) {
 // the CTA retires, so the fill limit of the global path is lowered by what they can add (grid x front
 // slots): the table stays at most half full and the front merge always finds a slot.
 template <class Kern>
-void launch_scan(dfgpu_ctx* ctx, Kern kern, AggParams& p, long long n, bool front) {
+void launch_scan(dfgpu_ctx* ctx, Kern kern, const char* name, AggParams& p, long long n, bool front) {
   const size_t smem = front ? size_t(AG_FRONT_SLOTS) * 8 * size_t(1 + p.naggs) : 0;
   if (front && ctx->first_use((const void*)kern))
     DF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, AG_FRONT_SLOTS * 8 * (1 + kMaxAggs)));
@@ -1550,19 +1558,25 @@ void launch_scan(dfgpu_ctx* ctx, Kern kern, AggParams& p, long long n, bool fron
   const int ps = ctx->prof_begin();
   kern<<<grid, AG_THREADS, smem, ctx->stream>>>(p);
   DF_CUDA(cudaGetLastError());
+  trace_launch(name);
   ctx->prof_end(ps);
   ctx->launches++;
 }
 template <int DEPTH>
 void launch_hash_agg(dfgpu_ctx* ctx, AggParams& p, long long n, bool front) {
-  if (front) launch_scan(ctx, k_hash_agg<DEPTH, true, false>, p, n, true);
-  else launch_scan(ctx, k_hash_agg<DEPTH, false, false>, p, n, false);
+  static const std::string with_front = "k_hash_agg<" + std::to_string(DEPTH) + ", true, false>";
+  static const std::string without = "k_hash_agg<" + std::to_string(DEPTH) + ", false, false>";
+  if (front) launch_scan(ctx, k_hash_agg<DEPTH, true, false>, with_front.c_str(), p, n, true);
+  else launch_scan(ctx, k_hash_agg<DEPTH, false, false>, without.c_str(), p, n, false);
 }
 template <int M>
 void launch_lean_m(dfgpu_ctx* ctx, AggParams& p, long long n, int mt) {
-  if (mt == MT_F64) launch_scan(ctx, k_hash_agg_lean<M, MT_F64>, p, n, false);
-  else if (mt == MT_I) launch_scan(ctx, k_hash_agg_lean<M, MT_I>, p, n, false);
-  else launch_scan(ctx, k_hash_agg_lean<M, MT_U>, p, n, false);
+  static const std::string name[3] = {"k_hash_agg_lean<" + std::to_string(M) + ", " + std::to_string(int(MT_F64)) + ">",
+                                      "k_hash_agg_lean<" + std::to_string(M) + ", " + std::to_string(int(MT_I)) + ">",
+                                      "k_hash_agg_lean<" + std::to_string(M) + ", " + std::to_string(int(MT_U)) + ">"};
+  if (mt == MT_F64) launch_scan(ctx, k_hash_agg_lean<M, MT_F64>, name[0].c_str(), p, n, false);
+  else if (mt == MT_I) launch_scan(ctx, k_hash_agg_lean<M, MT_I>, name[1].c_str(), p, n, false);
+  else launch_scan(ctx, k_hash_agg_lean<M, MT_U>, name[2].c_str(), p, n, false);
 }
 void launch_lean(dfgpu_ctx* ctx, AggParams& p, long long n, int mask, int mt) {
   switch (mask) {
@@ -1581,6 +1595,8 @@ void launch_reduce(dfgpu_ctx* ctx, const AggParams& p, long long n) {
   const int ps = ctx->prof_begin();
   k_reduce<DEPTH, NULLS><<<grid_for(ctx, n, RD_TILE, per_sm), AG_THREADS, 0, ctx->stream>>>(p);
   DF_CUDA(cudaGetLastError());
+  static const std::string name = "k_reduce<" + std::to_string(DEPTH) + (NULLS ? ", true>" : ", false>");
+  trace_launch(name.c_str());
   ctx->prof_end(ps);
   ctx->launches++;
 }
@@ -1917,6 +1933,7 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
           const int ps = ctx->prof_begin();
           k_reduce_f64<<<grid_for(ctx, p.nrows, 256 * 8, 8), 256, 0, ctx->stream>>>(rp);
           DF_CUDA(cudaGetLastError());
+          trace_launch("k_reduce_f64");
           ctx->prof_end(ps);
           ctx->launches++;
         } else if (d <= 1) launch_reduce<1>(ctx, p, p.nrows);
@@ -1975,6 +1992,7 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
         mp.naggs = st->naggs;
         k_wide_move<<<grid_for(ctx, st->cap, 256, 8), 256, 0, ctx->stream>>>(mp);
         DF_CUDA(cudaGetLastError());
+        trace_launch("k_wide_move");
         ctx->launches++;
         DF_CUDA(cudaStreamSynchronize(ctx->stream));
         ctx->free(st->t.base);
@@ -1997,8 +2015,8 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
         DF_CUDA(cudaMemsetAsync(st->d_counters + 1, 0, 8, ctx->stream));
         DF_CUDA(cudaMemsetAsync(st->d_counters + 5, 0, 8, ctx->stream));
         const long long n = list ? nlist : p.nrows;
-        if (p.ps.has_nulls) launch_scan(ctx, k_hash_agg_wide<8, true>, p, n, false);
-        else launch_scan(ctx, k_hash_agg_wide<8, false>, p, n, false);
+        if (p.ps.has_nulls) launch_scan(ctx, k_hash_agg_wide<8, true>, "k_hash_agg_wide<8, true>", p, n, false);
+        else launch_scan(ctx, k_hash_agg_wide<8, false>, "k_hash_agg_wide<8, false>", p, n, false);
         unsigned long long c[8];
         read_counters(st, c);
         if (c[3]) fail(DFGPU_ERR_ARROW, "DivideByZero");
@@ -2136,7 +2154,7 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
         p.front_slots = p.front_per_warp ? AG_FRONT_SLOTS / (AG_THREADS / 32) : AG_FRONT_SLOTS;
         // (A persisting-L2 access-policy window over the table was tried and removed: it slowed the scan
         // several-fold at 1e5 and 1e6 groups.)
-        if (p.ps.has_nulls) launch_scan(ctx, k_hash_agg<8, false, true>, p, n, false);
+        if (p.ps.has_nulls) launch_scan(ctx, k_hash_agg<8, false, true>, "k_hash_agg<8, false, true>", p, n, false);
         else if (lean_mask && !list && !front && !st->aos && (p.row_begin & 1) == 0) {
           // the lean kernel addresses the hybrid layout directly
           p.lean.key_col = (const unsigned long long*)p.ps.cols[p.plain.key_slot[0]].ptr;
@@ -2156,15 +2174,15 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
             layout_ok = layout_ok && ((f == DFGPU_AGG_MIN || f == DFGPU_AGG_MAX) ? st->t.loc[a] >= 1 : st->t.loc[a] < 0);
           }
           if (layout_ok) launch_lean(ctx, p, n, lean_mask, lean_mt);
-          else launch_scan(ctx, k_hash_agg_plain<2, false>, p, n, false);
+          else launch_scan(ctx, k_hash_agg_plain<2, false>, "k_hash_agg_plain<2, false>", p, n, false);
         } else if (use_plain && !list && (p.row_begin & 1) == 0) {
           const bool two = p.plain.ncols <= 2;
           if (front) {
-            if (two) launch_scan(ctx, k_hash_agg_plain<2, true>, p, n, true);
-            else launch_scan(ctx, k_hash_agg_plain<4, true>, p, n, true);
+            if (two) launch_scan(ctx, k_hash_agg_plain<2, true>, "k_hash_agg_plain<2, true>", p, n, true);
+            else launch_scan(ctx, k_hash_agg_plain<4, true>, "k_hash_agg_plain<4, true>", p, n, true);
           } else {
-            if (two) launch_scan(ctx, k_hash_agg_plain<2, false>, p, n, false);
-            else launch_scan(ctx, k_hash_agg_plain<4, false>, p, n, false);
+            if (two) launch_scan(ctx, k_hash_agg_plain<2, false>, "k_hash_agg_plain<2, false>", p, n, false);
+            else launch_scan(ctx, k_hash_agg_plain<4, false>, "k_hash_agg_plain<4, false>", p, n, false);
           }
         } else if (d <= 1) launch_hash_agg<1>(ctx, p, n, front);
         else if (d <= 2) launch_hash_agg<2>(ctx, p, n, front);
