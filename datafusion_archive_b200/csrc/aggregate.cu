@@ -78,6 +78,18 @@ struct PlainSpec {
   PlainTerm term[4];
 };
 
+// Slots of the operator's device counters (AggParams::counters, dfgpu_aggstate::d_counters).
+constexpr int CTR_GROUPS = 0;    // groups in the table
+constexpr int CTR_OVERFLOW = 1;  // rows appended to the overflow list
+constexpr int CTR_SENTINEL = 2;  // nonzero: the key that equals EMPTY_KEY holds slot cap
+constexpr int CTR_ERROR = 3;     // 1: an expression raised DivideByZero, 2: a merge into the table found no slot
+constexpr int CTR_COMPACT = 4;   // entries written by k_compact
+constexpr int CTR_DEFERRED = 5;  // wide scan: overflow rows that only met a slot still being published; Utf8 verify: its flag
+constexpr int CTR_PASSED = 6;    // reduce with WHERE: rows that passed the predicate
+constexpr int CTR_ROWS = 7;      // multi-GPU reduce: rows seen on every rank
+constexpr int CTR_NONNULL = 8;   // [8, 8 + kMaxAggs): reduce: non-null inputs per aggregate
+constexpr int CTR_SLOTS = CTR_NONNULL + kMaxAggs;
+
 struct AggParams {
   ProgramSet ps;  // programs [0,nkeys) = group keys, then the distinct aggregate-argument programs
   AggDesc aggs[kMaxAggs];
@@ -96,7 +108,7 @@ struct AggParams {
   TableLayout t;
   long long cap;             // power of two
   long long max_groups;      // new keys are refused (-> overflow list) beyond this fill
-  unsigned long long* counters;  // [0] ngroups [1] overflow count [2] sentinel-key used [3] error
+  unsigned long long* counters;  // CTR_SLOTS words, see CTR_*
   unsigned* ovf_rows;
   // front table (FRONT kernels): one table of front_slots per CTA, or — for very few groups — one
   // private table per warp, so that shared-memory atomics only contend inside a warp
@@ -512,7 +524,7 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
   for (long long tb = (long long)blockIdx.x * TILE; tb < n; tb += tstep) {
     // fill limit, once per warp per tile (no CTA-wide barrier in the steady state)
     unsigned long long filled = 0;
-    if (lane == 0) filled = __ldcg(&p.counters[0]);
+    if (lane == 0) filled = __ldcg(&p.counters[CTR_GROUPS]);
     filled = __shfl_sync(0xffffffffu, filled, 0);
     const bool full = (long long)filled >= p.max_groups;
     src.load(p, tb, n, tid, stream_policy);
@@ -561,13 +573,13 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
       slot[r] = -1;
       if (!((src.mask >> r) & 1u) || fslot[r] >= 0) continue;
       if (key[r] == EMPTY_KEY) {  // the one key value that collides with the empty marker
-        if (__ldcg(&p.counters[2]) == 0ull) p.counters[2] = 1ull;
+        if (__ldcg(&p.counters[CTR_SENTINEL]) == 0ull) p.counters[CTR_SENTINEL] = 1ull;
         slot[r] = p.cap;
         continue;
       }
       slot[r] = probe_insert<true>(p.t, p.cap, key[r], ln[r], h[r], full, new_groups);
       if (slot[r] < 0) {
-        const unsigned long long at = atomicAdd(&p.counters[1], 1ull);
+        const unsigned long long at = atomicAdd(&p.counters[CTR_OVERFLOW], 1ull);
         p.ovf_rows[at] = src.rowid(r);
       }
     }
@@ -597,7 +609,7 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
     // one counter update per warp
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) new_groups += __shfl_xor_sync(0xffffffffu, new_groups, o);
-    if (lane == 0 && new_groups) atomicAdd(&p.counters[0], (unsigned long long)new_groups);
+    if (lane == 0 && new_groups) atomicAdd(&p.counters[CTR_GROUPS], (unsigned long long)new_groups);
   }
   if (FRONT) {
     // merge this CTA's front table into the global table.  New keys are always admitted here; the host
@@ -613,13 +625,13 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
       Line ln;
       load_line<false>(p.t, (long long)h, ln);
       const long long slot = probe_insert<false>(p.t, p.cap, key, ln, h, false, new_groups);
-      if (slot < 0) { p.counters[3] = 2ull; continue; }
+      if (slot < 0) { p.counters[CTR_ERROR] = 2ull; continue; }
       for (int a = 0; a < p.naggs; a++)
         acc_merge_global(p.aggs[a].func, p.aggs[a].mtype, p.t.val(slot, a), tb[(1 + a) * FS + j]);
     }
-    if (new_groups) atomicAdd(&p.counters[0], (unsigned long long)new_groups);
+    if (new_groups) atomicAdd(&p.counters[CTR_GROUPS], (unsigned long long)new_groups);
   }
-  if (bad) p.counters[3] = 1ull;
+  if (bad) p.counters[CTR_ERROR] = 1ull;
 }
 
 // Occupancy target (H100): the global-table scan wants its interpreter stack in registers more than a fourth
@@ -668,7 +680,7 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
   }
   for (long long tb = (long long)blockIdx.x * TILE; tb < n; tb += tstep) {
     unsigned long long filled = 0;
-    if (lane == 0) filled = __ldcg(&p.counters[0]);
+    if (lane == 0) filled = __ldcg(&p.counters[CTR_GROUPS]);
     filled = __shfl_sync(0xffffffffu, filled, 0);
     const bool full = (long long)filled >= p.max_groups;
     const long long i = tb + 2ll * tid;
@@ -705,7 +717,7 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
       if (!act[r]) continue;
       bool have_line = true;
       if (k[r] == EMPTY_KEY) {  // the one key value that collides with the empty marker
-        if (__ldcg(&p.counters[2]) == 0ull) p.counters[2] = 1ull;
+        if (__ldcg(&p.counters[CTR_SENTINEL]) == 0ull) p.counters[CTR_SENTINEL] = 1ull;
         slot[r] = (unsigned long long)p.cap;
         have_line = false;
       } else {
@@ -725,7 +737,7 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
           else asm volatile("ld.global.cg.u64 %0, [%1];" : "=l"(ln[r].w[0]) : "l"(q) : "memory");
         }
         if (!found) {  // table refuses new keys: the row is replayed after the table has grown
-          const unsigned long long at = atomicAdd(&p.counters[1], 1ull);
+          const unsigned long long at = atomicAdd(&p.counters[CTR_OVERFLOW], 1ull);
           p.ovf_rows[at] = (unsigned)(p.row_begin + i + r);
           continue;
         }
@@ -746,7 +758,7 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) new_groups += __shfl_xor_sync(0xffffffffu, new_groups, o);
-    if (lane == 0 && new_groups) atomicAdd(&p.counters[0], (unsigned long long)new_groups);
+    if (lane == 0 && new_groups) atomicAdd(&p.counters[CTR_GROUPS], (unsigned long long)new_groups);
   }
 }
 
@@ -771,7 +783,7 @@ __device__ __forceinline__ unsigned long long ld_volatile_u64(const unsigned lon
 
 // K5 for wide keys.  Claim protocol of a slot: CAS the tag word EMPTY -> tag & ~1 (busy), store the key parts,
 // fence, store tag | 1 (ready).  A row that meets a busy slot with its own tag polls briefly and otherwise
-// defers itself to the replay list (counters[5] counts those: they need no table growth, the slot is
+// defers itself to the replay list (counter CTR_DEFERRED counts those: they need no table growth, the slot is
 // ready by the time the replay runs), so no thread ever waits on another one indefinitely.
 template <int DEPTH, bool NULLS>
 __global__ void __launch_bounds__(AG_THREADS) k_hash_agg_wide(const __grid_constant__ AggParams p) {
@@ -786,7 +798,7 @@ __global__ void __launch_bounds__(AG_THREADS) k_hash_agg_wide(const __grid_const
   constexpr int TILE = AG_THREADS * R;
   for (long long tb = (long long)blockIdx.x * TILE; tb < n; tb += (long long)gridDim.x * TILE) {
     unsigned long long filled = 0;
-    if (lane == 0) filled = __ldcg(&p.counters[0]);
+    if (lane == 0) filled = __ldcg(&p.counters[CTR_GROUPS]);
     filled = __shfl_sync(0xffffffffu, filled, 0);
     const bool full = (long long)filled >= p.max_groups;
     Src src;
@@ -851,9 +863,9 @@ __global__ void __launch_bounds__(AG_THREADS) k_hash_agg_wide(const __grid_const
         h = (h + 1ull) & smask;
       }
       if (slot[r] < 0) {
-        const unsigned long long at = atomicAdd(&p.counters[1], 1ull);
+        const unsigned long long at = atomicAdd(&p.counters[CTR_OVERFLOW], 1ull);
         p.ovf_rows[at] = (unsigned)row;
-        if (deferred) atomicAdd(&p.counters[5], 1ull);
+        if (deferred) atomicAdd(&p.counters[CTR_DEFERRED], 1ull);
       }
     }
     for (int g = 0; g < p.nargs; g++) {
@@ -876,9 +888,9 @@ __global__ void __launch_bounds__(AG_THREADS) k_hash_agg_wide(const __grid_const
     bad = bad || src.bad != 0;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) new_groups += __shfl_xor_sync(0xffffffffu, new_groups, o);
-    if (lane == 0 && new_groups) atomicAdd(&p.counters[0], (unsigned long long)new_groups);
+    if (lane == 0 && new_groups) atomicAdd(&p.counters[CTR_GROUPS], (unsigned long long)new_groups);
   }
-  if (bad) p.counters[3] = 1ull;
+  if (bad) p.counters[CTR_ERROR] = 1ull;
 }
 
 // Re-insertion of the (distinct) groups of a wide-key table into a bigger one: every entry goes to the first
@@ -915,7 +927,7 @@ constexpr int RD_TILE = AG_THREADS * RD_R;
 
 // NULLS: array_ops::{min,max,sum} skip nulls and report None when nothing was non-null
 // (restated from arrow 0.12; call sites aggregate.rs:347-541): the number of non-null inputs per
-// aggregate is accumulated in counters[8 + a] so finish can emit a null.
+// aggregate is accumulated in counter CTR_NONNULL + a so finish can emit a null.
 template <int DEPTH, bool NULLS>
 __global__ void __launch_bounds__(AG_THREADS) k_reduce(const __grid_constant__ AggParams p) {
   __shared__ unsigned long long s_acc[kMaxAggs][AG_THREADS];
@@ -923,7 +935,7 @@ __global__ void __launch_bounds__(AG_THREADS) k_reduce(const __grid_constant__ A
   unsigned nn[kMaxAggs];
 #pragma unroll
   for (int a = 0; a < kMaxAggs; a++) nn[a] = 0;
-  unsigned passed = 0;  // rows that passed the fused predicate (counters[6]: an aggregate over zero rows is null)
+  unsigned passed = 0;  // rows that passed the fused predicate (counter CTR_PASSED: an aggregate over zero rows is null)
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int a = 0; a < p.naggs; a++) s_acc[a][tid] = agg_identity(p.aggs[a].func);
   bool bad = false;
@@ -988,15 +1000,15 @@ __global__ void __launch_bounds__(AG_THREADS) k_reduce(const __grid_constant__ A
       unsigned c = nn[a];
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-      if (lane == 0 && c && a < p.naggs) atomicAdd(&p.counters[8 + a], (unsigned long long)c);
+      if (lane == 0 && c && a < p.naggs) atomicAdd(&p.counters[CTR_NONNULL + a], (unsigned long long)c);
     }
   }
   if (p.has_pred) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) passed += __shfl_xor_sync(0xffffffffu, passed, o);
-    if (lane == 0 && passed) atomicAdd(&p.counters[6], (unsigned long long)passed);
+    if (lane == 0 && passed) atomicAdd(&p.counters[CTR_PASSED], (unsigned long long)passed);
   }
-  if (bad) p.counters[3] = 1ull;
+  if (bad) p.counters[CTR_ERROR] = 1ull;
 }
 
 // K4 fast path: every aggregate argument is a plain, null-free Float64 column.  One pass per distinct
@@ -1160,19 +1172,19 @@ __global__ void __launch_bounds__(256) k_merge(const __grid_constant__ MergePara
     const unsigned long long key = p.in_keys[at];
     long long slot;
     if (key == EMPTY_KEY) {
-      p.counters[2] = 1ull;
+      p.counters[CTR_SENTINEL] = 1ull;
       slot = p.cap;
     } else {
       const unsigned long long h = home_slot(mix64(key), hshift);
       Line ln;
       load_line<false>(p.t, (long long)h, ln);
       slot = probe_insert<false>(p.t, p.cap, key, ln, h, false, new_groups);
-      if (slot < 0) { p.counters[3] = 2ull; continue; }  // cannot happen: caller sizes the table
+      if (slot < 0) { p.counters[CTR_ERROR] = 2ull; continue; }  // cannot happen: caller sizes the table
     }
     for (int a = 0; a < p.naggs; a++)
       acc_merge_global(p.aggs[a].func, p.aggs[a].mtype, p.t.val(slot, a), p.in_vals[a][at]);
   }
-  if (new_groups) atomicAdd(&p.counters[0], (unsigned long long)new_groups);
+  if (new_groups) atomicAdd(&p.counters[CTR_GROUPS], (unsigned long long)new_groups);
 }
 
 // ---- owner-partitioned exchange of partial aggregates (multi-GPU merge, SURVEY.md §8e) -----------------
@@ -1345,7 +1357,7 @@ struct dfgpu_aggstate {
   Utf8Source* d_utf8_srcs = nullptr;
   bool saw_nulls = false;  // some batch went through the null-aware reduce: per-aggregate non-null counts are on the device
   std::vector<long long> nonnull_host = std::vector<long long>(8, 0);
-  unsigned long long* d_counters = nullptr;  // 8 x u64
+  unsigned long long* d_counters = nullptr;  // CTR_SLOTS words, see CTR_*
   long long ngroups = 0;
   bool sentinel_used = false;
   long long rows_seen = 0;
@@ -1385,11 +1397,35 @@ struct Trace {
   }
 };
 
-// DFGPU_TRACE: name each scan, reduce and re-layout kernel as it is launched, template arguments included, so
-// that a run shows which instantiation the dispatch chose (the GROUP BY kernel tests assert it)
+// DFGPU_TRACE: name each kernel as it is launched, template arguments included, so that a run shows which
+// instantiation the dispatch chose (the GROUP BY kernel tests assert it)
 void trace_launch(const char* kernel) {
   if (getenv("DFGPU_TRACE")) fprintf(stderr, "[dfgpu trace] launch %s\n", kernel);
 }
+
+// Words of the pinned ctx->h_scratch that the operator stages through.
+constexpr int HS_COUNTERS = 8;  // counter slots [0, CTR_NONNULL)
+constexpr int HS_HEADER = 16;   // multi-GPU header record (up to 16 words)
+constexpr int HS_NONNULL = 40;  // the CTR_NONNULL block (kMaxAggs words)
+constexpr int HS_ROWS = 48;     // CTR_ROWS
+
+// Device blocks that go back to the ctx pool at scope exit.
+struct DevBufs {
+  dfgpu_ctx* ctx;
+  std::vector<void*> blocks;
+  explicit DevBufs(dfgpu_ctx* c) : ctx(c) {}
+  DevBufs(const DevBufs&) = delete;
+  DevBufs& operator=(const DevBufs&) = delete;
+  ~DevBufs() {
+    for (void* q : blocks) ctx->free(q);
+  }
+  template <class T = unsigned long long>
+  T* alloc(size_t bytes) {
+    void* q = ctx->alloc(bytes);
+    blocks.push_back(q);
+    return static_cast<T*>(q);
+  }
+};
 
 long long next_pow2(long long x) {
   long long p = 1;
@@ -1397,7 +1433,88 @@ long long next_pow2(long long x) {
   return p;
 }
 
-int grid_for(dfgpu_ctx* ctx, long long work_items, int per_block, int blocks_per_sm);
+int grid_for(dfgpu_ctx* ctx, long long work_items, int per_block, int blocks_per_sm) {
+  long long g = (work_items + per_block - 1) / per_block;
+  long long cap = (long long)ctx->sm_count * blocks_per_sm;
+  if (g > cap) g = cap;
+  if (g < 1) g = 1;
+  return int(g);
+}
+
+// Launch one of the kernels that are neither a scan nor a reduce: 256 threads per CTA, one CTA per `per_block` work
+// items, at most blocks_per_sm CTAs per SM.
+template <class P>
+void launch_kernel(dfgpu_ctx* ctx, void (*kern)(P), const char* name, const P& p, long long work_items, int per_block, int blocks_per_sm) {
+  kern<<<grid_for(ctx, work_items, per_block, blocks_per_sm), 256, 0, ctx->stream>>>(p);
+  DF_CUDA(cudaGetLastError());
+  trace_launch(name);
+  ctx->launches++;
+}
+
+// One scan kernel instantiation.  FRONT kernels route rows through the shared-memory front table.
+struct ScanKernel {
+  void (*fn)(AggParams);
+  const char* name;
+  bool front;
+};
+
+// Launch one scan kernel.  FRONT launches admit the keys of every CTA's front table unconditionally when
+// the CTA retires, so the fill limit of the global path is lowered by what they can add (grid x front
+// slots): the table stays at most half full and the front merge always finds a slot.
+void launch_scan(dfgpu_ctx* ctx, const ScanKernel& k, AggParams& p, long long n) {
+  const size_t smem = k.front ? size_t(AG_FRONT_SLOTS) * 8 * size_t(1 + p.naggs) : 0;
+  if (k.front && ctx->first_use((const void*)k.fn))
+    DF_CUDA(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, AG_FRONT_SLOTS * 8 * (1 + kMaxAggs)));
+  int per_sm = 0;
+  DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k.fn, AG_THREADS, smem));
+  if (per_sm < 1) per_sm = 1;
+  const int grid = grid_for(ctx, n, AG_TILE, per_sm);
+  if (k.front) p.max_groups = std::max<long long>(0, p.max_groups - (long long)grid * AG_FRONT_SLOTS);
+  const int ps = ctx->prof_begin();
+  k.fn<<<grid, AG_THREADS, smem, ctx->stream>>>(p);
+  DF_CUDA(cudaGetLastError());
+  trace_launch(k.name);
+  ctx->prof_end(ps);
+  ctx->launches++;
+}
+template <int DEPTH>
+ScanKernel hash_agg_kernel(bool front) {
+  static const std::string with_front = "k_hash_agg<" + std::to_string(DEPTH) + ", true, false>";
+  static const std::string without = "k_hash_agg<" + std::to_string(DEPTH) + ", false, false>";
+  if (front) return {k_hash_agg<DEPTH, true, false>, with_front.c_str(), true};
+  return {k_hash_agg<DEPTH, false, false>, without.c_str(), false};
+}
+template <int M>
+ScanKernel lean_kernel_m(int mt) {
+  static const std::string name[3] = {"k_hash_agg_lean<" + std::to_string(M) + ", " + std::to_string(int(MT_F64)) + ">",
+                                      "k_hash_agg_lean<" + std::to_string(M) + ", " + std::to_string(int(MT_I)) + ">",
+                                      "k_hash_agg_lean<" + std::to_string(M) + ", " + std::to_string(int(MT_U)) + ">"};
+  if (mt == MT_F64) return {k_hash_agg_lean<M, MT_F64>, name[0].c_str(), false};
+  if (mt == MT_I) return {k_hash_agg_lean<M, MT_I>, name[1].c_str(), false};
+  return {k_hash_agg_lean<M, MT_U>, name[2].c_str(), false};
+}
+ScanKernel lean_kernel(int mask, int mt) {
+  switch (mask) {
+#define DF_LEAN(M) case M: return lean_kernel_m<M>(mt);
+    DF_LEAN(1) DF_LEAN(2) DF_LEAN(3) DF_LEAN(4) DF_LEAN(5) DF_LEAN(6) DF_LEAN(7) DF_LEAN(8)
+    DF_LEAN(9) DF_LEAN(10) DF_LEAN(11) DF_LEAN(12) DF_LEAN(13) DF_LEAN(14) DF_LEAN(15)
+#undef DF_LEAN
+    default: fail(DFGPU_ERR_INTERNAL, "lean kernel: bad aggregate mask");
+  }
+}
+template <int DEPTH, bool NULLS = false>
+void launch_reduce(dfgpu_ctx* ctx, const AggParams& p, long long n) {
+  int per_sm = 0;
+  DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_reduce<DEPTH, NULLS>, AG_THREADS, 0));
+  if (per_sm < 1) per_sm = 1;
+  const int ps = ctx->prof_begin();
+  k_reduce<DEPTH, NULLS><<<grid_for(ctx, n, RD_TILE, per_sm), AG_THREADS, 0, ctx->stream>>>(p);
+  DF_CUDA(cudaGetLastError());
+  static const std::string name = "k_reduce<" + std::to_string(DEPTH) + (NULLS ? ", true>" : ", false>");
+  trace_launch(name.c_str());
+  ctx->prof_end(ps);
+  ctx->launches++;
+}
 
 // groups x (1 + naggs) sectors is what the SoA layout keeps hot in L2; beyond this many bytes the
 // table is built AoS (one sector per group).  H100 L2 = 50 MB, shared with the streaming input.
@@ -1465,140 +1582,93 @@ TableLayout table_alloc(dfgpu_ctx* ctx, int naggs, int nkeys, const std::vector<
   ip.nslots = cap + 1;
   ip.naggs = naggs;
   for (int a = 0; a < naggs; a++) ip.ident[a] = agg_identity(descs[size_t(a)].func);
-  k_table_init<<<grid_for(ctx, ip.nslots, 256 * 4, 16), 256, 0, ctx->stream>>>(ip);
-  DF_CUDA(cudaGetLastError());
-  ctx->launches++;
+  launch_kernel(ctx, k_table_init, "k_table_init", ip, ip.nslots, 256 * 4, 16);
   return ip.t;
 }
 
+// counter slots [0, CTR_NONNULL) -> host8 (synchronises the stream)
 void read_counters(dfgpu_aggstate* st, unsigned long long* host8) {
   dfgpu_ctx* ctx = st->ctx;
-  DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 8, st->d_counters, 64, cudaMemcpyDeviceToHost, ctx->stream));
+  DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + HS_COUNTERS, st->d_counters, CTR_NONNULL * 8, cudaMemcpyDeviceToHost, ctx->stream));
   DF_CUDA(cudaStreamSynchronize(ctx->stream));
-  for (int i = 0; i < 8; i++) host8[i] = ctx->h_scratch[8 + i];
+  for (int i = 0; i < CTR_NONNULL; i++) host8[i] = ctx->h_scratch[HS_COUNTERS + i];
 }
-
-int grid_for(dfgpu_ctx* ctx, long long work_items, int per_block, int blocks_per_sm) {
-  long long g = (work_items + per_block - 1) / per_block;
-  long long cap = (long long)ctx->sm_count * blocks_per_sm;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return int(g);
-}
-
-// grow the table to new_cap, re-inserting every occupied slot
-void table_grow(dfgpu_aggstate* st, long long new_cap) {
+// one counter slot (synchronises the stream)
+unsigned long long read_counter(dfgpu_aggstate* st, int slot) {
   dfgpu_ctx* ctx = st->ctx;
-  const bool aos = st->aos || want_aos(std::max(st->ngroups, new_cap / 8), st->descs, st->naggs);
-  TableLayout nt = table_alloc(ctx, st->naggs, st->nkeys, st->descs, new_cap, aos);
-  // compact raw, then merge into the new table
-  const size_t cnt = size_t(st->ngroups + 1);
-  unsigned long long* ck = (unsigned long long*)ctx->alloc(cnt * 8);
-  unsigned long long* cv = (unsigned long long*)ctx->alloc(cnt * 8 * size_t(st->naggs > 0 ? st->naggs : 1));
+  DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + HS_COUNTERS + slot, st->d_counters + slot, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  DF_CUDA(cudaStreamSynchronize(ctx->stream));
+  return ctx->h_scratch[HS_COUNTERS + slot];
+}
+
+// Raw compaction (k_compact, raw = 1) of table t: the occupied slots as (packed key, accumulators) entries.  Entry i's
+// key goes to keys[i * stride] and accumulator a to vals[a * val_step + i * stride] (stride 0 = 1); the number of
+// entries to counter CTR_COMPACT.
+void compact_raw(dfgpu_aggstate* st, const TableLayout& t, long long cap, int sentinel_used, const unsigned long long* sentinel_flag,
+                 unsigned long long* keys, unsigned long long* vals, size_t val_step, long long stride) {
+  dfgpu_ctx* ctx = st->ctx;
   CompactParams cp;
   memset(&cp, 0, sizeof(cp));
-  cp.t = st->t;
-  cp.cap = st->cap;
-  cp.sentinel_used = st->sentinel_used;
+  cp.t = t;
+  cp.cap = cap;
+  cp.sentinel_used = sentinel_used;
+  cp.sentinel_flag = sentinel_flag;
   cp.nkeys = st->nkeys;
   cp.naggs = st->naggs;
   cp.raw = 1;
-  cp.out_keys[0] = ck;
+  cp.raw_stride = stride;
+  cp.out_keys[0] = keys;
   for (int a = 0; a < st->naggs; a++) {
     cp.aggs[a] = st->descs[size_t(a)];
-    cp.out_vals[a] = cv + size_t(a) * cnt;
+    cp.out_vals[a] = vals + size_t(a) * val_step;
   }
-  DF_CUDA(cudaMemsetAsync(st->d_counters + 4, 0, 8, ctx->stream));
-  cp.counter = st->d_counters + 4;
-  k_compact<<<grid_for(ctx, st->cap + 1, 256, 8), 256, 0, ctx->stream>>>(cp);
-  DF_CUDA(cudaGetLastError());
-  trace_launch("k_compact");
-  ctx->launches++;
-  MergeParams mp;
-  memset(&mp, 0, sizeof(mp));
-  mp.in_keys = ck;
-  for (int a = 0; a < st->naggs; a++) {
-    mp.in_vals[a] = cv + size_t(a) * cnt;
-    mp.aggs[a] = st->descs[size_t(a)];
-  }
-  mp.n = st->ngroups + (st->sentinel_used ? 1 : 0);
-  mp.t = nt;
-  mp.cap = new_cap;
-  mp.naggs = st->naggs;
-  DF_CUDA(cudaMemsetAsync(st->d_counters, 0, 8, ctx->stream));  // ngroups is recounted by the merge
-  mp.counters = st->d_counters;
-  if (mp.n > 0) {
-    k_merge<<<grid_for(ctx, mp.n, 256, 8), 256, 0, ctx->stream>>>(mp);
-    DF_CUDA(cudaGetLastError());
-    trace_launch("k_merge");
-    ctx->launches++;
+  DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_COMPACT, 0, 8, ctx->stream));
+  cp.counter = st->d_counters + CTR_COMPACT;
+  launch_kernel(ctx, k_compact, "k_compact", cp, cap + 1, 256, 8);
+}
+
+// Grow the table to new_cap.  Wide tables move their slots (k_wide_move: every entry is distinct); the others are
+// raw-compacted and merged into the new table (k_merge), which may also change their layout.
+void table_grow(dfgpu_aggstate* st, long long new_cap) {
+  dfgpu_ctx* ctx = st->ctx;
+  const bool aos = st->aos || want_aos(std::max(st->ngroups, new_cap / 8), st->descs, st->naggs);
+  TableLayout nt = table_alloc(ctx, st->naggs, st->nkeys, st->descs, new_cap, aos, st->wide ? st->nkeys : 0);
+  DevBufs tmp(ctx);
+  if (st->wide) {
+    WideMoveParams mp;
+    memset(&mp, 0, sizeof(mp));
+    mp.from = st->t;
+    mp.to = nt;
+    mp.from_cap = st->cap;
+    mp.to_cap = new_cap;
+    mp.kw = st->nkeys;
+    mp.naggs = st->naggs;
+    launch_kernel(ctx, k_wide_move, "k_wide_move", mp, st->cap, 256, 8);
+  } else {
+    const size_t cnt = size_t(st->ngroups + 1);
+    unsigned long long* ck = tmp.alloc(cnt * 8);
+    unsigned long long* cv = tmp.alloc(cnt * 8 * size_t(st->naggs > 0 ? st->naggs : 1));
+    compact_raw(st, st->t, st->cap, st->sentinel_used, nullptr, ck, cv, cnt, 0);
+    MergeParams mp;
+    memset(&mp, 0, sizeof(mp));
+    mp.in_keys = ck;
+    for (int a = 0; a < st->naggs; a++) {
+      mp.in_vals[a] = cv + size_t(a) * cnt;
+      mp.aggs[a] = st->descs[size_t(a)];
+    }
+    mp.n = st->ngroups + (st->sentinel_used ? 1 : 0);
+    mp.t = nt;
+    mp.cap = new_cap;
+    mp.naggs = st->naggs;
+    DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_GROUPS, 0, 8, ctx->stream));  // ngroups is recounted by the merge
+    mp.counters = st->d_counters;
+    if (mp.n > 0) launch_kernel(ctx, k_merge, "k_merge", mp, mp.n, 256, 8);
   }
   DF_CUDA(cudaStreamSynchronize(ctx->stream));
-  ctx->free(ck);
-  ctx->free(cv);
   ctx->free(st->t.base);
   st->t = nt;
   st->aos = aos;
   st->cap = new_cap;
-}
-
-// Launch one scan kernel.  FRONT launches admit the keys of every CTA's front table unconditionally when
-// the CTA retires, so the fill limit of the global path is lowered by what they can add (grid x front
-// slots): the table stays at most half full and the front merge always finds a slot.
-template <class Kern>
-void launch_scan(dfgpu_ctx* ctx, Kern kern, const char* name, AggParams& p, long long n, bool front) {
-  const size_t smem = front ? size_t(AG_FRONT_SLOTS) * 8 * size_t(1 + p.naggs) : 0;
-  if (front && ctx->first_use((const void*)kern))
-    DF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, AG_FRONT_SLOTS * 8 * (1 + kMaxAggs)));
-  int per_sm = 0;
-  DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, AG_THREADS, smem));
-  if (per_sm < 1) per_sm = 1;
-  const int grid = grid_for(ctx, n, AG_TILE, per_sm);
-  if (front) p.max_groups = std::max<long long>(0, p.max_groups - (long long)grid * AG_FRONT_SLOTS);
-  const int ps = ctx->prof_begin();
-  kern<<<grid, AG_THREADS, smem, ctx->stream>>>(p);
-  DF_CUDA(cudaGetLastError());
-  trace_launch(name);
-  ctx->prof_end(ps);
-  ctx->launches++;
-}
-template <int DEPTH>
-void launch_hash_agg(dfgpu_ctx* ctx, AggParams& p, long long n, bool front) {
-  static const std::string with_front = "k_hash_agg<" + std::to_string(DEPTH) + ", true, false>";
-  static const std::string without = "k_hash_agg<" + std::to_string(DEPTH) + ", false, false>";
-  if (front) launch_scan(ctx, k_hash_agg<DEPTH, true, false>, with_front.c_str(), p, n, true);
-  else launch_scan(ctx, k_hash_agg<DEPTH, false, false>, without.c_str(), p, n, false);
-}
-template <int M>
-void launch_lean_m(dfgpu_ctx* ctx, AggParams& p, long long n, int mt) {
-  static const std::string name[3] = {"k_hash_agg_lean<" + std::to_string(M) + ", " + std::to_string(int(MT_F64)) + ">",
-                                      "k_hash_agg_lean<" + std::to_string(M) + ", " + std::to_string(int(MT_I)) + ">",
-                                      "k_hash_agg_lean<" + std::to_string(M) + ", " + std::to_string(int(MT_U)) + ">"};
-  if (mt == MT_F64) launch_scan(ctx, k_hash_agg_lean<M, MT_F64>, name[0].c_str(), p, n, false);
-  else if (mt == MT_I) launch_scan(ctx, k_hash_agg_lean<M, MT_I>, name[1].c_str(), p, n, false);
-  else launch_scan(ctx, k_hash_agg_lean<M, MT_U>, name[2].c_str(), p, n, false);
-}
-void launch_lean(dfgpu_ctx* ctx, AggParams& p, long long n, int mask, int mt) {
-  switch (mask) {
-#define DF_LEAN(M) case M: launch_lean_m<M>(ctx, p, n, mt); break;
-    DF_LEAN(1) DF_LEAN(2) DF_LEAN(3) DF_LEAN(4) DF_LEAN(5) DF_LEAN(6) DF_LEAN(7) DF_LEAN(8)
-    DF_LEAN(9) DF_LEAN(10) DF_LEAN(11) DF_LEAN(12) DF_LEAN(13) DF_LEAN(14) DF_LEAN(15)
-#undef DF_LEAN
-    default: fail(DFGPU_ERR_INTERNAL, "lean kernel: bad aggregate mask");
-  }
-}
-template <int DEPTH, bool NULLS = false>
-void launch_reduce(dfgpu_ctx* ctx, const AggParams& p, long long n) {
-  int per_sm = 0;
-  DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_reduce<DEPTH, NULLS>, AG_THREADS, 0));
-  if (per_sm < 1) per_sm = 1;
-  const int ps = ctx->prof_begin();
-  k_reduce<DEPTH, NULLS><<<grid_for(ctx, n, RD_TILE, per_sm), AG_THREADS, 0, ctx->stream>>>(p);
-  DF_CUDA(cudaGetLastError());
-  static const std::string name = "k_reduce<" + std::to_string(DEPTH) + (NULLS ? ", true>" : ", false>");
-  trace_launch(name.c_str());
-  ctx->prof_end(ps);
-  ctx->launches++;
 }
 
 }  // namespace
@@ -1626,8 +1696,8 @@ extern "C" int dfgpu_aggregate_create(dfgpu_ctx* ctx, const dfgpu_insn* const* k
       st->funcs.push_back(aggs[a].func);
       st->out_dtypes.push_back(aggs[a].out_dtype);
     }
-    st->d_counters = (unsigned long long*)ctx->alloc(128);  // [0..7] see AggParams, [8..15] non-null inputs per aggregate
-    DF_CUDA(cudaMemsetAsync(st->d_counters, 0, 128, ctx->stream));
+    st->d_counters = (unsigned long long*)ctx->alloc(CTR_SLOTS * 8);
+    DF_CUDA(cudaMemsetAsync(st->d_counters, 0, CTR_SLOTS * 8, ctx->stream));
     *out = st.release();
   });
 }
@@ -1677,18 +1747,17 @@ extern "C" int dfgpu_aggregate_update_host(dfgpu_aggstate* st, const dfgpu_col* 
       return;
     }
     const int nchunks = int((n + chunk_rows - 1) / chunk_rows);
-    std::vector<void*> dev(size_t(ncols), nullptr);
+    DevBufs dev(ctx);  // freed after the Cleanup below has drained both streams
     std::vector<cudaEvent_t> evs(size_t(nchunks), nullptr);
     struct Cleanup {
-      dfgpu_ctx* c; std::vector<void*>* d; std::vector<cudaEvent_t>* e;
+      dfgpu_ctx* c; std::vector<cudaEvent_t>* e;
       ~Cleanup() {
         cudaStreamSynchronize(c->stream_in);
         cudaStreamSynchronize(c->stream);
-        for (void* q : *d) c->free(q);
         for (cudaEvent_t x : *e) if (x) cudaEventDestroy(x);
       }
-    } cleanup{ctx, &dev, &evs};
-    for (int i = 0; i < ncols; i++) dev[size_t(i)] = ctx->alloc(size_t(n) * size_t(dtype_width(cols[i].dtype)));
+    } cleanup{ctx, &evs};
+    for (int i = 0; i < ncols; i++) dev.alloc<void>(size_t(n) * size_t(dtype_width(cols[i].dtype)));
     // the device buffers may have been used on ctx->stream before (cached blocks): order the copies after it
     cudaEvent_t ready;
     DF_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
@@ -1699,7 +1768,7 @@ extern "C" int dfgpu_aggregate_update_host(dfgpu_aggstate* st, const dfgpu_col* 
       const int64_t lo = int64_t(c) * chunk_rows, cnt = std::min<int64_t>(chunk_rows, n - lo);
       for (int i = 0; i < ncols; i++) {
         const size_t w = size_t(dtype_width(cols[i].dtype));
-        DF_CUDA(cudaMemcpyAsync(static_cast<uint8_t*>(dev[size_t(i)]) + size_t(lo) * w,
+        DF_CUDA(cudaMemcpyAsync(static_cast<uint8_t*>(dev.blocks[size_t(i)]) + size_t(lo) * w,
                                 static_cast<const uint8_t*>(cols[i].values) + size_t(cols[i].offset + lo) * w, size_t(cnt) * w,
                                 cudaMemcpyHostToDevice, ctx->stream_in));
       }
@@ -1717,7 +1786,7 @@ extern "C" int dfgpu_aggregate_update_host(dfgpu_aggstate* st, const dfgpu_col* 
         DevColumn d;
         d.dtype = cols[i].dtype;
         const size_t w = size_t(dtype_width(cols[i].dtype));
-        d.values = static_cast<uint8_t*>(dev[size_t(i)]) + size_t(lo) * w;
+        d.values = static_cast<uint8_t*>(dev.blocks[size_t(i)]) + size_t(lo) * w;
         d.values_bytes = size_t(cnt) * w;
         view.cols.push_back(d);
       }
@@ -1727,524 +1796,504 @@ extern "C" int dfgpu_aggregate_update_host(dfgpu_aggstate* st, const dfgpu_col* 
 }
 
 namespace {
-void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
-  {
-    if (st->finished) fail(DFGPU_ERR_GENERAL, "aggregate already finished");
-    dfgpu_ctx* ctx = st->ctx;
-    ctx->use();
-    if (batch->nrows >= (1ll << 32)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "batches of 2^32 rows or more");
 
-    Trace tr(ctx);
-    AggParams p;
-    memset(&p, 0, sizeof(p));
-    ProgramBuilder pb(batch);
-    std::vector<int> kdt;
-    // fused WHERE: program 0 (FilterRelation under the aggregate, context.rs:126-139)
-    const int has_pred = st->pred_prog.empty() ? 0 : 1;
-    if (has_pred) {
-      const int pi = pb.add(st->pred_prog.data(), int(st->pred_prog.size()), "filter expression");
-      if (pb.out_dtype(pi) != DFGPU_BOOL) fail(DFGPU_ERR_EXECUTION, "Filter expression did not evaluate to boolean");  // filter.rs:62-67
-    }
-    // a single plain Utf8 column as the key: group by a 64-bit hash of the strings (see dfgpu_aggstate)
-    const DevColumn* ukey = nullptr;
-    if (st->nkeys == 1 && st->key_progs[0].size() == 1 && st->key_progs[0][0].op == DFGPU_OP_COL && st->key_progs[0][0].col >= 0 &&
-        size_t(st->key_progs[0][0].col) < batch->cols.size() && batch->cols[size_t(st->key_progs[0][0].col)].dtype == DFGPU_UTF8)
-      ukey = &batch->cols[size_t(st->key_progs[0][0].col)];
-    unsigned long long* d_hash = nullptr;
-    struct HashFree { dfgpu_ctx* c; unsigned long long** p; ~HashFree() { c->free(*p); } } hash_free{ctx, &d_hash};
-    std::vector<const DevColumn*> wide_ucols;    // per key part: its Utf8 column in this batch (or null)
-    std::vector<unsigned long long*> wide_hashes;  // string hashes of the Utf8 parts
-    struct HashesFree { dfgpu_ctx* c; std::vector<unsigned long long*>* v; ~HashesFree() { for (auto* q : *v) c->free(q); } } hashes_free{ctx, &wide_hashes};
-    if (ukey) {
-      if (st->typed && !st->utf8_key) fail(DFGPU_ERR_GENERAL, "GROUP BY key types changed between batches");
-      if (!st->typed && st->naggs >= kMaxAggs) fail(DFGPU_ERR_NOT_IMPLEMENTED, "Utf8 GROUP BY key with " + std::to_string(kMaxAggs) + " aggregates");
-      if (st->utf8_srcs.size() >= (1u << 20)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "more than 2^20 batches with a Utf8 GROUP BY key");
-      d_hash = (unsigned long long*)ctx->alloc(size_t(batch->nrows > 0 ? batch->nrows : 1) * 8);
-      utf8_hash(ctx, *ukey, batch->nrows, d_hash);
-      pb.add_synthetic_column(d_hash, DFGPU_UINT64);
-      kdt.push_back(DFGPU_UINT64);
-    } else {
-      // key parts: integer expressions, and plain Utf8 columns (hashed here; the scan reads the hash as a column)
-      for (int k = 0; k < st->nkeys; k++) {
-        const auto& kp = st->key_progs[size_t(k)];
-        const DevColumn* uc = nullptr;
-        if (kp.size() == 1 && kp[0].op == DFGPU_OP_COL && kp[0].col >= 0 && size_t(kp[0].col) < batch->cols.size() &&
-            batch->cols[size_t(kp[0].col)].dtype == DFGPU_UTF8)
-          uc = &batch->cols[size_t(kp[0].col)];
-        wide_ucols.push_back(uc);
-        if (uc) {
-          unsigned long long* dh = (unsigned long long*)ctx->alloc(size_t(batch->nrows > 0 ? batch->nrows : 1) * 8);
-          wide_hashes.push_back(dh);
-          utf8_hash(ctx, *uc, batch->nrows, dh);
-          pb.add_synthetic_column(dh, DFGPU_UINT64);
-          kdt.push_back(DFGPU_UTF8);
-          continue;
-        }
-        int pi = pb.add(kp.data(), int(kp.size()), "GROUP BY expression");
-        int dt = pb.out_dtype(pi);
-        if (dt == DFGPU_UTF8) fail(DFGPU_ERR_NOT_IMPLEMENTED, "Utf8 GROUP BY keys must be plain columns");
-        if (!is_int(dt)) fail(DFGPU_ERR_EXECUTION, "Unsupported GROUP BY data type");  // aggregate.rs:848-850
-        kdt.push_back(dt);
-      }
-    }
-    const int user_aggs = st->utf8_key ? st->naggs - 1 : st->naggs;  // the hidden representative is appended below
-    std::vector<AggDesc> descs;
-    std::vector<int> agg_arg(size_t(user_aggs), 0);
-    int nargs = 0;
-    for (int a = 0; a < user_aggs; a++) {
-      // identical argument expressions are compiled (and evaluated) once
-      int same = -1;
-      for (int b = 0; b < a && same < 0; b++) {
-        const auto &x = st->arg_progs[size_t(a)], &y = st->arg_progs[size_t(b)];
-        if (x.size() == y.size() && memcmp(x.data(), y.data(), x.size() * sizeof(dfgpu_insn)) == 0) same = b;
-      }
-      int pi;
-      if (same >= 0) {
-        agg_arg[size_t(a)] = agg_arg[size_t(same)];
-        pi = has_pred + st->nkeys + agg_arg[size_t(a)];
-      } else {
-        pi = pb.add(st->arg_progs[size_t(a)].data(), int(st->arg_progs[size_t(a)].size()), "aggregate argument");
-        agg_arg[size_t(a)] = nargs++;
-      }
-      int dt = pb.out_dtype(pi);
-      if (!is_numeric(dt)) fail(DFGPU_ERR_EXECUTION, std::string("Unsupported data type for aggregate: ") + dtype_name(dt));
-      AggDesc d;
-      d.func = uint8_t(st->funcs[size_t(a)]);
-      d.mtype = mtype_of(dt);
-      d.dtype = uint8_t(dt);
-      int want = d.func == DFGPU_AGG_COUNT ? DFGPU_UINT64 : dt;
-      int odt = st->out_dtypes[size_t(a)];
-      if (odt == 0) odt = want;
-      if (odt != want)  // the reference would hit "unexpected type when creating array from aggregate map" (aggregate.rs:683-695)
-        fail(DFGPU_ERR_EXECUTION, "unexpected type when creating array from aggregate map");
-      d.out_dtype = uint8_t(odt);
-      descs.push_back(d);
-    }
-    if (ukey) {
-      // hidden accumulator: MIN(source << 40 | row)
-      pb.add_rowid_plus((unsigned long long)st->utf8_srcs.size() << UTF8_SRC_SHIFT);
-      agg_arg.push_back(nargs++);
-      AggDesc d;
-      d.func = DFGPU_AGG_MIN;
-      d.mtype = MT_U;
-      d.dtype = DFGPU_UINT64;
-      d.out_dtype = DFGPU_UINT64;
-      descs.push_back(d);
-      if (!st->typed) {
-        st->utf8_key = true;
-        st->naggs += 1;
-      }
-      // retain this batch's key column: representatives are gathered from it at finish
-      const size_t ob = size_t(batch->nrows + 1) * 4, vb = ukey->values_bytes ? ukey->values_bytes : 1;
-      int* off = (int*)ctx->alloc(ob);
-      unsigned char* bytes = (unsigned char*)ctx->alloc(vb);
-      DF_CUDA(cudaMemcpyAsync(off, ukey->offsets, ob, cudaMemcpyDeviceToDevice, ctx->stream));
-      if (ukey->values_bytes) DF_CUDA(cudaMemcpyAsync(bytes, ukey->values, ukey->values_bytes, cudaMemcpyDeviceToDevice, ctx->stream));
-      st->utf8_owned.push_back(off);
-      st->utf8_owned.push_back(bytes);
-      st->utf8_srcs.push_back(Utf8Source{off, bytes});
-      ctx->free(st->d_utf8_srcs);
-      st->d_utf8_srcs = (Utf8Source*)ctx->alloc(st->utf8_srcs.size() * sizeof(Utf8Source));
-      DF_CUDA(cudaMemcpyAsync(st->d_utf8_srcs, st->utf8_srcs.data(), st->utf8_srcs.size() * sizeof(Utf8Source), cudaMemcpyHostToDevice, ctx->stream));
-      DF_CUDA(cudaStreamSynchronize(ctx->stream));  // utf8_srcs may reallocate on the next batch
-    }
-    if (!st->typed) {
-      st->key_dtypes = kdt;
-      st->descs = descs;
-      int bits = 0;
-      bool any_utf8 = false;
-      for (int k = st->nkeys - 1; k >= 0; k--) {  // last key in the low bits
-        const bool u = !ukey && kdt[size_t(k)] == DFGPU_UTF8;
-        any_utf8 = any_utf8 || u;
-        int w = u ? 64 : dtype_width(kdt[size_t(k)]) * 8;
-        st->key_shift.insert(st->key_shift.begin(), bits > 63 ? 0 : bits);
-        st->key_mask.insert(st->key_mask.begin(), w == 64 ? ~0ull : ((1ull << w) - 1ull));
-        st->key_is_utf8.insert(st->key_is_utf8.begin(), u ? 1 : 0);
-        bits += w;
-      }
-      // more than 64 key bits, or Utf8 parts next to other parts: tagged slots with full key comparison
-      st->wide = !ukey && (bits > 64 || any_utf8);
-      if (st->nkeys == 1) st->key_mask[0] = ~0ull;  // single key: keep the sign-extended 64-bit value
-      st->typed = true;
-      st->cap = st->nkeys == 0 ? 0 : std::max(AG_MIN_CAP, next_pow2(2 * st->expected));
-      if (st->wide) {
-        st->aos = true;
-        st->t = table_alloc(ctx, st->naggs, st->nkeys, st->descs, st->cap, true, st->nkeys);
-      } else {
-      st->aos = st->nkeys > 0 && want_aos(st->expected, st->descs, st->naggs);
-      st->t = table_alloc(ctx, st->naggs, st->nkeys, st->descs, st->cap, st->aos);
-      }
-    } else {
-      if (kdt != st->key_dtypes) fail(DFGPU_ERR_GENERAL, "GROUP BY key types changed between batches");
-      for (int a = 0; a < st->naggs; a++)
-        if (descs[size_t(a)].dtype != st->descs[size_t(a)].dtype) fail(DFGPU_ERR_GENERAL, "aggregate argument types changed between batches");
-    }
-    tr.mark("programs + table alloc");
-    pb.finish(&p.ps);
-    for (int s = 0; s < p.ps.ncols; s++)
-      if (!is_numeric(p.ps.cols[s].dtype) && p.ps.cols[s].dtype != DFGPU_BOOL)  // Boolean columns: WHERE operands (boolean_ops!)
-        fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string("expressions over ") + dtype_name(p.ps.cols[s].dtype) + " columns are not supported on the GPU path yet");
-    if (p.ps.max_depth > 8) fail(DFGPU_ERR_NOT_IMPLEMENTED, "expression too deep (register stack depth > 8)");
-    st->rows_seen += batch->nrows;
-    if (batch->nrows == 0) return;
+// The batch's column that a key program reads when the program is one plain Utf8 column, else null.
+const DevColumn* plain_utf8_col(const std::vector<dfgpu_insn>& kp, const dfgpu_batch* batch) {
+  if (kp.size() != 1 || kp[0].op != DFGPU_OP_COL || kp[0].col < 0 || size_t(kp[0].col) >= batch->cols.size()) return nullptr;
+  const DevColumn& c = batch->cols[size_t(kp[0].col)];
+  return c.dtype == DFGPU_UTF8 ? &c : nullptr;
+}
 
-    p.nkeys = st->nkeys;
-    p.naggs = st->naggs;
-    for (int a = 0; a < st->naggs; a++) {
-      p.aggs[a] = st->descs[size_t(a)];
-      p.agg_arg[a] = agg_arg[size_t(a)];
-    }
-    p.nargs = nargs;
-    for (int k = 0; k < st->nkeys; k++) {
-      p.key_mask[k] = st->key_mask[size_t(k)];
-      p.key_shift[k] = st->key_shift[size_t(k)];
-    }
-    p.nrows = batch->nrows;
-    p.counters = st->d_counters;
-    p.has_pred = has_pred;
-    const int d = p.ps.max_depth;
+// Keep a copy of a batch's Utf8 key column: a group refers to its string as (source << UTF8_SRC_SHIFT | row), and the
+// strings are gathered at finish.  Returns the column's source index; upload_utf8_srcs makes it visible to kernels.
+unsigned long long retain_utf8(dfgpu_aggstate* st, const DevColumn& c, long long nrows) {
+  dfgpu_ctx* ctx = st->ctx;
+  const size_t ob = size_t(nrows + 1) * 4, vb = c.values_bytes ? c.values_bytes : 1;
+  int* off = (int*)ctx->alloc(ob);
+  unsigned char* bytes = (unsigned char*)ctx->alloc(vb);
+  DF_CUDA(cudaMemcpyAsync(off, c.offsets, ob, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (c.values_bytes) DF_CUDA(cudaMemcpyAsync(bytes, c.values, c.values_bytes, cudaMemcpyDeviceToDevice, ctx->stream));
+  st->utf8_owned.push_back(off);
+  st->utf8_owned.push_back(bytes);
+  st->utf8_srcs.push_back(Utf8Source{off, bytes});
+  return st->utf8_srcs.size() - 1;
+}
+void upload_utf8_srcs(dfgpu_aggstate* st) {
+  dfgpu_ctx* ctx = st->ctx;
+  ctx->free(st->d_utf8_srcs);
+  st->d_utf8_srcs = (Utf8Source*)ctx->alloc(st->utf8_srcs.size() * sizeof(Utf8Source));
+  DF_CUDA(cudaMemcpyAsync(st->d_utf8_srcs, st->utf8_srcs.data(), st->utf8_srcs.size() * sizeof(Utf8Source), cudaMemcpyHostToDevice, ctx->stream));
+  DF_CUDA(cudaStreamSynchronize(ctx->stream));  // utf8_srcs may reallocate on the next batch
+}
 
-    if (st->nkeys == 0) {
-      p.t = st->t;
-      p.cap = 0;
-      if (has_pred) DF_CUDA(cudaMemsetAsync(st->d_counters + 6, 0, 8, ctx->stream));  // rows passing the predicate
-      if (p.ps.has_nulls) {
-        st->saw_nulls = true;
-        launch_reduce<8, true>(ctx, p, p.nrows);
-      } else {
-        if (!has_pred)
-          for (int a = 0; a < st->naggs; a++) st->nonnull_host[size_t(a)] += batch->nrows;
-        // fast path: every distinct argument is a plain Float64 column
-        bool plain = !has_pred;
-        ReduceF64Params rp;
-        memset(&rp, 0, sizeof(rp));
-        for (int g = 0; g < nargs && plain; g++) {
-          const CompiledProgram& cpg = pb.prog(g);
-          plain = cpg.is_plain_column && p.ps.cols[cpg.plain_slot].dtype == DFGPU_FLOAT64 &&
-                  (reinterpret_cast<uintptr_t>(p.ps.cols[cpg.plain_slot].ptr) & 15) == 0;
-          if (plain) rp.col[g] = (const double*)p.ps.cols[cpg.plain_slot].ptr;
-        }
-        if (plain) {
-          rp.ncols = nargs;
-          rp.nrows = p.nrows;
-          rp.naggs = st->naggs;
-          for (int a = 0; a < st->naggs; a++) { rp.aggs[a] = p.aggs[a]; rp.agg_arg[a] = p.agg_arg[a]; }
-          rp.t = st->t;
-          const int ps = ctx->prof_begin();
-          k_reduce_f64<<<grid_for(ctx, p.nrows, 256 * 8, 8), 256, 0, ctx->stream>>>(rp);
-          DF_CUDA(cudaGetLastError());
-          trace_launch("k_reduce_f64");
-          ctx->prof_end(ps);
-          ctx->launches++;
-        } else if (d <= 1) launch_reduce<1>(ctx, p, p.nrows);
-        else if (d <= 2) launch_reduce<2>(ctx, p, p.nrows);
-        else if (d <= 4) launch_reduce<4>(ctx, p, p.nrows);
-        else launch_reduce<8>(ctx, p, p.nrows);
-      }
-      unsigned long long c[8];
-      read_counters(st, c);
-      if (c[3]) fail(DFGPU_ERR_ARROW, "DivideByZero");
-      if (has_pred && !p.ps.has_nulls)  // null-free inputs: every row that passed the predicate is a non-null input
-        for (int a = 0; a < st->naggs; a++) st->nonnull_host[size_t(a)] += (long long)c[6];
-      return;
-    }
+// Pack the key parts into one 64-bit word, the last key in the low bits; a Utf8 part (wide keys) takes a whole word.
+// Returns whether the keys need the wide table: more than 64 key bits, or a Utf8 part next to other parts.
+bool pack_keys(dfgpu_aggstate* st) {
+  const size_t nk = size_t(st->nkeys);
+  st->key_shift.assign(nk, 0);
+  st->key_mask.assign(nk, 0);
+  st->key_is_utf8.assign(nk, 0);
+  int bits = 0;
+  bool any_utf8 = false;
+  for (int k = st->nkeys - 1; k >= 0; k--) {
+    const bool u = st->key_dtypes[size_t(k)] == DFGPU_UTF8;
+    const int w = u ? 64 : dtype_width(st->key_dtypes[size_t(k)]) * 8;
+    st->key_shift[size_t(k)] = bits > 63 ? 0 : bits;
+    st->key_mask[size_t(k)] = w == 64 ? ~0ull : ((1ull << w) - 1ull);
+    st->key_is_utf8[size_t(k)] = u ? 1 : 0;
+    any_utf8 = any_utf8 || u;
+    bits += w;
+  }
+  if (st->nkeys == 1) st->key_mask[0] = ~0ull;  // single key: keep the sign-extended 64-bit value
+  return bits > 64 || any_utf8;
+}
 
-    if (st->wide) {
-      // retain this batch's Utf8 key columns: a group's string lives in the batch whose row created it
-      p.wide.kw = st->nkeys;
-      bool new_src = false;
-      for (int k = 0; k < st->nkeys; k++) {
-        p.wide.is_utf8[k] = st->key_is_utf8[size_t(k)];
-        const DevColumn* uc = wide_ucols[size_t(k)];
-        if (!uc) continue;
-        if (st->utf8_srcs.size() >= (1u << 20)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "more than 2^20 retained Utf8 GROUP BY key columns");
-        const size_t ob = size_t(batch->nrows + 1) * 4, vb = uc->values_bytes ? uc->values_bytes : 1;
-        int* off = (int*)ctx->alloc(ob);
-        unsigned char* bytes = (unsigned char*)ctx->alloc(vb);
-        DF_CUDA(cudaMemcpyAsync(off, uc->offsets, ob, cudaMemcpyDeviceToDevice, ctx->stream));
-        if (uc->values_bytes) DF_CUDA(cudaMemcpyAsync(bytes, uc->values, uc->values_bytes, cudaMemcpyDeviceToDevice, ctx->stream));
-        p.wide.off[k] = off;
-        p.wide.bytes[k] = bytes;
-        p.wide.ref_base[k] = (unsigned long long)st->utf8_srcs.size() << UTF8_SRC_SHIFT;
-        st->utf8_owned.push_back(off);
-        st->utf8_owned.push_back(bytes);
-        st->utf8_srcs.push_back(Utf8Source{off, bytes});
-        new_src = true;
-      }
-      if (new_src) {
-        ctx->free(st->d_utf8_srcs);
-        st->d_utf8_srcs = (Utf8Source*)ctx->alloc(st->utf8_srcs.size() * sizeof(Utf8Source));
-        DF_CUDA(cudaMemcpyAsync(st->d_utf8_srcs, st->utf8_srcs.data(), st->utf8_srcs.size() * sizeof(Utf8Source), cudaMemcpyHostToDevice, ctx->stream));
-        DF_CUDA(cudaStreamSynchronize(ctx->stream));  // utf8_srcs may reallocate on the next batch
-      }
-      p.wide.srcs = st->d_utf8_srcs;
-      unsigned* wovf[2] = {(unsigned*)ctx->alloc(size_t(batch->nrows) * 4), nullptr};
-      struct WFreer { dfgpu_ctx* c; unsigned** o; ~WFreer() { c->free(o[0]); c->free(o[1]); } } wfreer{ctx, wovf};
-      auto wide_grow = [&](long long new_cap) {
-        TableLayout nt = table_alloc(ctx, st->naggs, st->nkeys, st->descs, new_cap, true, st->nkeys);
-        WideMoveParams mp;
-        memset(&mp, 0, sizeof(mp));
-        mp.from = st->t;
-        mp.to = nt;
-        mp.from_cap = st->cap;
-        mp.to_cap = new_cap;
-        mp.kw = st->nkeys;
-        mp.naggs = st->naggs;
-        k_wide_move<<<grid_for(ctx, st->cap, 256, 8), 256, 0, ctx->stream>>>(mp);
-        DF_CUDA(cudaGetLastError());
-        trace_launch("k_wide_move");
-        ctx->launches++;
-        DF_CUDA(cudaStreamSynchronize(ctx->stream));
-        ctx->free(st->t.base);
-        st->t = nt;
-        st->cap = new_cap;
-      };
-      int cur = 0;
-      const unsigned* list = nullptr;
-      long long nlist = 0;
-      for (int round = 0;; round++) {
-        if (round > 60) fail(DFGPU_ERR_INTERNAL, "hash table growth did not converge");
-        p.t = st->t;
-        p.cap = st->cap;
-        p.max_groups = st->cap / 2;
-        p.row_begin = 0;
-        p.nrows = batch->nrows;
-        p.row_list = list;
-        p.nlist = nlist;
-        p.ovf_rows = wovf[cur];
-        DF_CUDA(cudaMemsetAsync(st->d_counters + 1, 0, 8, ctx->stream));
-        DF_CUDA(cudaMemsetAsync(st->d_counters + 5, 0, 8, ctx->stream));
-        const long long n = list ? nlist : p.nrows;
-        if (p.ps.has_nulls) launch_scan(ctx, k_hash_agg_wide<8, true>, "k_hash_agg_wide<8, true>", p, n, false);
-        else launch_scan(ctx, k_hash_agg_wide<8, false>, "k_hash_agg_wide<8, false>", p, n, false);
-        unsigned long long c[8];
-        read_counters(st, c);
-        if (c[3]) fail(DFGPU_ERR_ARROW, "DivideByZero");
-        st->ngroups = (long long)c[0];
-        const long long novf = (long long)c[1], deferred = (long long)c[5];
-        tr.mark("scan kernel (wide keys)");
-        if (novf == 0) {
-          if (st->ngroups > st->cap / 2) wide_grow(st->cap * 4);
-          break;
-        }
-        // rows that only met a slot still being published need no bigger table: replay them as they are
-        if (!(novf == deferred && st->ngroups <= st->cap / 2)) wide_grow(st->cap * 4);
-        list = wovf[cur];
-        nlist = novf;
-        cur ^= 1;
-        if (!wovf[cur]) wovf[cur] = (unsigned*)ctx->alloc(size_t(batch->nrows) * 4);
-      }
-      return;
-    }
+// The programs of one batch: the fused WHERE (program 0, FilterRelation under the aggregate, context.rs:126-139), the
+// GROUP BY keys, the distinct aggregate arguments and, for a single Utf8 key, the hidden representative.  A Utf8 key
+// column is read as a column of its 64-bit string hashes.
+struct BatchPrograms {
+  ProgramBuilder pb;
+  DevBufs hashes;  // the string hashes of the Utf8 key columns
+  int has_pred = 0;
+  std::vector<int> key_dtypes;  // a Utf8 part of a wide key is Utf8, the single Utf8 key UInt64 (its hash)
+  std::vector<AggDesc> descs;
+  std::vector<int> agg_arg;
+  int nargs = 0;
+  const DevColumn* ukey = nullptr;  // the single Utf8 key column (grouped by hash, then verified)
+  const unsigned long long* ukey_hash = nullptr;
+  std::vector<const DevColumn*> key_utf8;  // per key part (not the single Utf8 key): its Utf8 column, or null
+  BatchPrograms(const dfgpu_batch* batch, dfgpu_ctx* ctx) : pb(batch), hashes(ctx) {}
+};
 
-    // Plain-column fast path: keys and arguments are plain 4/8-byte columns, the WHERE clause (if any) a
-    // chain of column comparisons -> the interpreter-free kernel with 128-bit loads.
-    bool use_plain = false;
-    {
-      static const bool off = getenv("DFGPU_AGG_PLAIN") && atoi(getenv("DFGPU_AGG_PLAIN")) == 0;  // A/B switch
-      PlainSpec sp;
-      memset(&sp, 0, sizeof(sp));
-      auto wide = [](int dt) {
-        return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64 || dt == DFGPU_FLOAT32 || dt == DFGPU_INT32 || dt == DFGPU_UINT32;
-      };
-      bool ok = !off && !p.ps.has_nulls && p.ps.ncols <= 4;
-      for (int c = 0; ok && c < p.ps.ncols; c++)
-        ok = wide(p.ps.cols[c].dtype) && (reinterpret_cast<uintptr_t>(p.ps.cols[c].ptr) & 15) == 0;
-      for (int k = 0; ok && k < st->nkeys; k++) {
-        const CompiledProgram& cpk = pb.prog(has_pred + k);
-        ok = cpk.is_plain_column;
-        sp.key_slot[k] = cpk.plain_slot;
+// Compile a batch's programs and type its aggregates.  The single Utf8 key column is retained here, because the
+// representative program refers to the source index it is retained under.
+void compile_batch(dfgpu_aggstate* st, const dfgpu_batch* batch, BatchPrograms& bp) {
+  dfgpu_ctx* ctx = st->ctx;
+  ProgramBuilder& pb = bp.pb;
+  bp.has_pred = st->pred_prog.empty() ? 0 : 1;
+  if (bp.has_pred) {
+    const int pi = pb.add(st->pred_prog.data(), int(st->pred_prog.size()), "filter expression");
+    if (pb.out_dtype(pi) != DFGPU_BOOL) fail(DFGPU_ERR_EXECUTION, "Filter expression did not evaluate to boolean");  // filter.rs:62-67
+  }
+  auto hash_key = [&](const DevColumn& c) {
+    unsigned long long* h = bp.hashes.alloc(size_t(batch->nrows > 0 ? batch->nrows : 1) * 8);
+    utf8_hash(ctx, c, batch->nrows, h);
+    pb.add_synthetic_column(h, DFGPU_UINT64);
+    return h;
+  };
+  bp.ukey = st->nkeys == 1 ? plain_utf8_col(st->key_progs[0], batch) : nullptr;
+  if (bp.ukey) {
+    if (st->typed && !st->utf8_key) fail(DFGPU_ERR_GENERAL, "GROUP BY key types changed between batches");
+    if (!st->typed && st->naggs >= kMaxAggs) fail(DFGPU_ERR_NOT_IMPLEMENTED, "Utf8 GROUP BY key with " + std::to_string(kMaxAggs) + " aggregates");
+    if (st->utf8_srcs.size() >= (1u << 20)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "more than 2^20 batches with a Utf8 GROUP BY key");
+    bp.ukey_hash = hash_key(*bp.ukey);
+    bp.key_dtypes.push_back(DFGPU_UINT64);
+  } else {
+    for (int k = 0; k < st->nkeys; k++) {  // key parts: integer expressions and plain Utf8 columns
+      const auto& kp = st->key_progs[size_t(k)];
+      const DevColumn* uc = plain_utf8_col(kp, batch);
+      bp.key_utf8.push_back(uc);
+      if (uc) {
+        hash_key(*uc);
+        bp.key_dtypes.push_back(DFGPU_UTF8);
+        continue;
       }
-      for (int g = 0; ok && g < nargs; g++) {
-        const CompiledProgram& cpa = pb.prog(has_pred + st->nkeys + g);
-        ok = cpa.is_plain_column;
-        sp.arg_slot[g] = cpa.plain_slot;
-      }
-      if (ok && has_pred) {
-        // t0 [t1 AND|OR [t2 AND|OR ...]] in lowered form: (PUSH_COL, CMP leaf) {(PUSH_COL, CMP leaf), AND|OR stack}*
-        const int b = p.ps.start[0], e = p.ps.start[1];
-        const DevInsn* in = &p.ps.insn[b];
-        auto term_at = [&](int i, PlainTerm* out) {
-          if (i + 1 >= e - b) return false;
-          const DevInsn &c = in[i], &o = in[i + 1];
-          if (c.op != V_PUSH_COL) return false;
-          if (o.op < V_EQ || o.op > V_GE || o.mode == RHS_STACK) return false;
-          if (o.mode == RHS_COL && p.ps.cols[o.slot].dtype != p.ps.cols[c.slot].dtype) return false;
-          memset(out, 0, sizeof(*out));
-          out->kind = o.mode == RHS_COL ? 2 : 3;
-          out->op = o.op;
-          out->a = c.slot;
-          out->b = o.mode == RHS_COL ? o.slot : 0;
-          out->mt = mtype_of(p.ps.cols[c.slot].dtype);
-          out->imm = o.imm;
-          return true;
-        };
-        ok = term_at(0, &sp.term[0]);
-        sp.nterms = ok ? 1 : 0;
-        int i = 2;
-        while (ok && i < e - b) {
-          if (sp.nterms >= 4 || !term_at(i, &sp.term[sp.nterms]) || i + 2 >= e - b) { ok = false; break; }
-          const DevInsn& j = in[i + 2];
-          if ((j.op != V_AND && j.op != V_OR) || j.mode != RHS_STACK) { ok = false; break; }
-          sp.term[sp.nterms].conn = j.op == V_OR ? 1 : 0;
-          sp.nterms++;
-          i += 3;
-        }
-      }
-      sp.ncols = p.ps.ncols;
-      if (ok) p.plain = sp;
-      use_plain = ok;
-    }
-    // lean kernel: one 8-byte integer key column, one 8-byte argument column, distinct MIN/MAX/SUM/COUNT, no WHERE
-    int lean_mask = 0, lean_mt = 0;
-    {
-      static const bool off = getenv("DFGPU_AGG_LEAN") && atoi(getenv("DFGPU_AGG_LEAN")) == 0;  // A/B switch
-      auto w8 = [](int dt) { return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64; };
-      bool ok = !off && use_plain && !has_pred && st->nkeys == 1 && nargs == 1 && w8(p.ps.cols[p.plain.key_slot[0]].dtype) &&
-                w8(p.ps.cols[p.plain.arg_slot[0]].dtype);
-      for (int a = 0; ok && a < st->naggs; a++) {
-        const int bit = 1 << (st->descs[size_t(a)].func - 1);  // MIN 1, MAX 2, SUM 4, COUNT 8
-        ok = !(lean_mask & bit);
-        lean_mask |= bit;
-      }
-      if (ok) lean_mt = mtype_of(p.ps.cols[p.plain.arg_slot[0]].dtype);
-      else lean_mask = 0;
-    }
-
-    // GROUP BY: run, then replay rows that could not get a slot after growing the table.
-    // First big batch with no cardinality hint: a 1 Mi-row prefix is aggregated first; the number of
-    // groups it produces decides the table layout (SoA while the hot sectors fit L2, AoS beyond) before
-    // the bulk of the batch is touched.
-    unsigned* ovf[2] = {(unsigned*)ctx->alloc(size_t(batch->nrows) * 4), nullptr};
-    tr.mark("overflow list alloc");
-    struct Freer {
-      dfgpu_ctx* c;
-      unsigned** o;
-      ~Freer() { c->free(o[0]); c->free(o[1]); }
-    } freer{ctx, ovf};
-    const long long kPrefix = 1ll << 20;
-    const bool sample = st->rows_seen == batch->nrows && st->expected == 0 && !st->aos && batch->nrows >= 4 * kPrefix;
-    std::vector<std::pair<long long, long long>> ranges;  // (begin, count)
-    if (sample) {
-      ranges.push_back({0, kPrefix});
-      ranges.push_back({kPrefix, batch->nrows - kPrefix});
-    } else {
-      ranges.push_back({0, batch->nrows});
-    }
-    for (size_t ri = 0; ri < ranges.size(); ri++) {
-      int cur = 0;
-      const unsigned* list = nullptr;
-      long long nlist = 0;
-      for (int round = 0;; round++) {
-        if (round > 40) fail(DFGPU_ERR_INTERNAL, "hash table growth did not converge");
-        p.t = st->t;
-        p.cap = st->cap;
-        p.max_groups = st->cap / 2;
-        p.row_begin = ranges[ri].first;
-        p.nrows = ranges[ri].second;
-        p.row_list = list;
-        p.nlist = nlist;
-        p.ovf_rows = ovf[cur];
-        DF_CUDA(cudaMemsetAsync(st->d_counters + 1, 0, 8, ctx->stream));
-        const long long n = list ? nlist : p.nrows;
-        const bool front = st->use_front && !list;
-        // <= 64 groups: one private 256-slot table per warp (same shared-memory footprint as the
-        // CTA-wide 2048-slot table); otherwise one table per CTA
-        p.front_per_warp = st->ngroups <= 64 ? 1 : 0;
-        p.front_slots = p.front_per_warp ? AG_FRONT_SLOTS / (AG_THREADS / 32) : AG_FRONT_SLOTS;
-        // (A persisting-L2 access-policy window over the table was tried and removed: it slowed the scan
-        // several-fold at 1e5 and 1e6 groups.)
-        if (p.ps.has_nulls) launch_scan(ctx, k_hash_agg<8, false, true>, "k_hash_agg<8, false, true>", p, n, false);
-        else if (lean_mask && !list && !front && !st->aos && (p.row_begin & 1) == 0) {
-          // the lean kernel addresses the hybrid layout directly
-          p.lean.key_col = (const unsigned long long*)p.ps.cols[p.plain.key_slot[0]].ptr;
-          p.lean.arg_col = (const unsigned long long*)p.ps.cols[p.plain.arg_slot[0]].ptr;
-          p.lean.min_w = p.lean.max_w = 0;
-          p.lean.sum_arr = p.lean.cnt_arr = nullptr;
-          for (int a = 0; a < st->naggs; a++) {
-            const int f = st->descs[size_t(a)].func, l = st->t.loc[a];
-            if (f == DFGPU_AGG_MIN) p.lean.min_w = l;
-            else if (f == DFGPU_AGG_MAX) p.lean.max_w = l;
-            else if (f == DFGPU_AGG_SUM) p.lean.sum_arr = st->t.add + (long long)(~l) * st->t.astride;
-            else p.lean.cnt_arr = st->t.add + (long long)(~l) * st->t.astride;
-          }
-          bool layout_ok = st->t.lw == (((lean_mask & 3) == 3) ? 4 : ((lean_mask & 3) ? 2 : 1));
-          for (int a = 0; a < st->naggs; a++) {
-            const int f = st->descs[size_t(a)].func;
-            layout_ok = layout_ok && ((f == DFGPU_AGG_MIN || f == DFGPU_AGG_MAX) ? st->t.loc[a] >= 1 : st->t.loc[a] < 0);
-          }
-          if (layout_ok) launch_lean(ctx, p, n, lean_mask, lean_mt);
-          else launch_scan(ctx, k_hash_agg_plain<2, false>, "k_hash_agg_plain<2, false>", p, n, false);
-        } else if (use_plain && !list && (p.row_begin & 1) == 0) {
-          const bool two = p.plain.ncols <= 2;
-          if (front) {
-            if (two) launch_scan(ctx, k_hash_agg_plain<2, true>, "k_hash_agg_plain<2, true>", p, n, true);
-            else launch_scan(ctx, k_hash_agg_plain<4, true>, "k_hash_agg_plain<4, true>", p, n, true);
-          } else {
-            if (two) launch_scan(ctx, k_hash_agg_plain<2, false>, "k_hash_agg_plain<2, false>", p, n, false);
-            else launch_scan(ctx, k_hash_agg_plain<4, false>, "k_hash_agg_plain<4, false>", p, n, false);
-          }
-        } else if (d <= 1) launch_hash_agg<1>(ctx, p, n, front);
-        else if (d <= 2) launch_hash_agg<2>(ctx, p, n, front);
-        else if (d <= 4) launch_hash_agg<4>(ctx, p, n, front);
-        else launch_hash_agg<8>(ctx, p, n, front);
-        unsigned long long c[8];
-        read_counters(st, c);
-        if (c[3] == 2) fail(DFGPU_ERR_INTERNAL, "front-table merge could not find a slot");
-        if (c[3]) fail(DFGPU_ERR_ARROW, "DivideByZero");
-        st->ngroups = (long long)c[0];
-        st->sentinel_used = c[2] != 0;
-        const long long novf = (long long)c[1];
-        tr.mark(ri == 0 && ranges.size() > 1 ? "scan kernel (prefix)" : "scan kernel");
-        if (novf == 0) {
-          if (st->ngroups > st->cap / 2) { table_grow(st, st->cap * 4); tr.mark("table_grow (load factor)"); }
-          break;
-        }
-        table_grow(st, st->cap * 4);
-        list = ovf[cur];
-        nlist = novf;
-        cur ^= 1;
-        if (!ovf[cur]) ovf[cur] = (unsigned*)ctx->alloc(size_t(batch->nrows) * 4);
-      }
-      // few groups so far: later rows of this stream go through the shared-memory front table
-      st->use_front = st->ngroups <= AG_FRONT_MAX_GROUPS && st->rows_seen >= (1ll << 20);
-      if (sample && ri == 0) {
-        // size (and lay out) the table for the estimated number of groups before the bulk of the batch
-        // is touched: one rebuild of a ~1 Mi-entry table instead of repeated 4x growth + replays
-        long long est = std::max(estimate_groups(st->ngroups, kPrefix, batch->nrows), st->ngroups);
-        const long long afford = (long long)(ctx->device_mem_bytes / 8) / (32 * (1 + st->naggs));  // slots that fit in 1/8 of device memory
-        long long want_cap = std::max(AG_MIN_CAP, next_pow2(est * 2));
-        while (want_cap > st->cap && want_cap > afford) want_cap >>= 1;
-        const bool to_aos = !st->aos && want_aos(est, st->descs, st->naggs);
-        if (to_aos || want_cap > st->cap) {
-          st->aos = st->aos || to_aos;
-          table_grow(st, std::max(st->cap, want_cap));
-          tr.mark("table_grow (prefix estimate)");
-        }
-      }
-    }
-    if (ukey) {
-      VerifyParams vp;
-      memset(&vp, 0, sizeof(vp));
-      vp.hashes = d_hash;
-      vp.n = batch->nrows;
-      vp.t = st->t;
-      vp.cap = st->cap;
-      vp.rep_agg = st->naggs - 1;
-      vp.off = ukey->offsets;
-      vp.bytes = (const unsigned char*)ukey->values;
-      vp.srcs = st->d_utf8_srcs;
-      vp.flag = st->d_counters + 5;
-      DF_CUDA(cudaMemsetAsync(st->d_counters + 5, 0, 8, ctx->stream));
-      k_utf8_group_verify<<<grid_for(ctx, batch->nrows, 256, 8), 256, 0, ctx->stream>>>(vp);
-      DF_CUDA(cudaGetLastError());
-      ctx->launches++;
-      DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 12, st->d_counters + 5, 8, cudaMemcpyDeviceToHost, ctx->stream));
-      DF_CUDA(cudaStreamSynchronize(ctx->stream));
-      if (ctx->h_scratch[12] == 1ull) fail(DFGPU_ERR_INTERNAL, "two different Utf8 GROUP BY keys share a 64-bit hash (p < 1e-7 per 1e6 distinct keys)");
-      if (ctx->h_scratch[12]) fail(DFGPU_ERR_INTERNAL, "Utf8 GROUP BY verification could not find a group");
+      const int dt = pb.out_dtype(pb.add(kp.data(), int(kp.size()), "GROUP BY expression"));
+      if (dt == DFGPU_UTF8) fail(DFGPU_ERR_NOT_IMPLEMENTED, "Utf8 GROUP BY keys must be plain columns");
+      if (!is_int(dt)) fail(DFGPU_ERR_EXECUTION, "Unsupported GROUP BY data type");  // aggregate.rs:848-850
+      bp.key_dtypes.push_back(dt);
     }
   }
+  const int user_aggs = st->utf8_key ? st->naggs - 1 : st->naggs;  // the hidden representative is appended below
+  bp.agg_arg.assign(size_t(user_aggs), 0);
+  for (int a = 0; a < user_aggs; a++) {
+    // identical argument expressions are compiled (and evaluated) once
+    int same = -1;
+    for (int b = 0; b < a && same < 0; b++) {
+      const auto &x = st->arg_progs[size_t(a)], &y = st->arg_progs[size_t(b)];
+      if (x.size() == y.size() && memcmp(x.data(), y.data(), x.size() * sizeof(dfgpu_insn)) == 0) same = b;
+    }
+    int pi;
+    if (same >= 0) {
+      bp.agg_arg[size_t(a)] = bp.agg_arg[size_t(same)];
+      pi = bp.has_pred + st->nkeys + bp.agg_arg[size_t(a)];
+    } else {
+      pi = pb.add(st->arg_progs[size_t(a)].data(), int(st->arg_progs[size_t(a)].size()), "aggregate argument");
+      bp.agg_arg[size_t(a)] = bp.nargs++;
+    }
+    int dt = pb.out_dtype(pi);
+    if (!is_numeric(dt)) fail(DFGPU_ERR_EXECUTION, std::string("Unsupported data type for aggregate: ") + dtype_name(dt));
+    AggDesc d;
+    d.func = uint8_t(st->funcs[size_t(a)]);
+    d.mtype = mtype_of(dt);
+    d.dtype = uint8_t(dt);
+    int want = d.func == DFGPU_AGG_COUNT ? DFGPU_UINT64 : dt;
+    int odt = st->out_dtypes[size_t(a)];
+    if (odt == 0) odt = want;
+    if (odt != want)  // the reference would hit "unexpected type when creating array from aggregate map" (aggregate.rs:683-695)
+      fail(DFGPU_ERR_EXECUTION, "unexpected type when creating array from aggregate map");
+    d.out_dtype = uint8_t(odt);
+    bp.descs.push_back(d);
+  }
+  if (bp.ukey) {
+    // hidden accumulator: MIN(source << 40 | row)
+    pb.add_rowid_plus((unsigned long long)st->utf8_srcs.size() << UTF8_SRC_SHIFT);
+    bp.agg_arg.push_back(bp.nargs++);
+    bp.descs.push_back(AggDesc{DFGPU_AGG_MIN, MT_U, DFGPU_UINT64, DFGPU_UINT64});
+    if (!st->typed) {
+      st->utf8_key = true;
+      st->naggs += 1;
+    }
+    retain_utf8(st, *bp.ukey, batch->nrows);
+    upload_utf8_srcs(st);
+  }
+}
+
+// The first batch types the operator: key packing, table form and capacity.  Later batches must bring the same types.
+void type_batch(dfgpu_aggstate* st, const BatchPrograms& bp) {
+  if (st->typed) {
+    if (bp.key_dtypes != st->key_dtypes) fail(DFGPU_ERR_GENERAL, "GROUP BY key types changed between batches");
+    for (int a = 0; a < st->naggs; a++)
+      if (bp.descs[size_t(a)].dtype != st->descs[size_t(a)].dtype) fail(DFGPU_ERR_GENERAL, "aggregate argument types changed between batches");
+    return;
+  }
+  st->key_dtypes = bp.key_dtypes;
+  st->descs = bp.descs;
+  st->wide = pack_keys(st);
+  st->typed = true;
+  st->cap = st->nkeys == 0 ? 0 : std::max(AG_MIN_CAP, next_pow2(2 * st->expected));
+  st->aos = st->wide || (st->nkeys > 0 && want_aos(st->expected, st->descs, st->naggs));
+  st->t = table_alloc(st->ctx, st->naggs, st->nkeys, st->descs, st->cap, st->aos, st->wide ? st->nkeys : 0);
+}
+
+// No GROUP BY: one reduce over the batch.
+void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
+  dfgpu_ctx* ctx = st->ctx;
+  p.t = st->t;
+  p.cap = 0;
+  if (bp.has_pred) DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_PASSED, 0, 8, ctx->stream));
+  const int d = p.ps.max_depth;
+  if (p.ps.has_nulls) {
+    st->saw_nulls = true;
+    launch_reduce<8, true>(ctx, p, p.nrows);
+  } else {
+    if (!bp.has_pred)
+      for (int a = 0; a < st->naggs; a++) st->nonnull_host[size_t(a)] += p.nrows;
+    // fast path: every distinct argument is a plain Float64 column
+    bool plain = !bp.has_pred;
+    ReduceF64Params rp;
+    memset(&rp, 0, sizeof(rp));
+    for (int g = 0; g < bp.nargs && plain; g++) {
+      const CompiledProgram& cpg = bp.pb.prog(g);
+      plain = cpg.is_plain_column && p.ps.cols[cpg.plain_slot].dtype == DFGPU_FLOAT64 &&
+              (reinterpret_cast<uintptr_t>(p.ps.cols[cpg.plain_slot].ptr) & 15) == 0;
+      if (plain) rp.col[g] = (const double*)p.ps.cols[cpg.plain_slot].ptr;
+    }
+    if (plain) {
+      rp.ncols = bp.nargs;
+      rp.nrows = p.nrows;
+      rp.naggs = st->naggs;
+      for (int a = 0; a < st->naggs; a++) { rp.aggs[a] = p.aggs[a]; rp.agg_arg[a] = p.agg_arg[a]; }
+      rp.t = st->t;
+      const int ps = ctx->prof_begin();
+      launch_kernel(ctx, k_reduce_f64, "k_reduce_f64", rp, p.nrows, 256 * 8, 8);
+      ctx->prof_end(ps);
+    } else if (d <= 1) launch_reduce<1>(ctx, p, p.nrows);
+    else if (d <= 2) launch_reduce<2>(ctx, p, p.nrows);
+    else if (d <= 4) launch_reduce<4>(ctx, p, p.nrows);
+    else launch_reduce<8>(ctx, p, p.nrows);
+  }
+  unsigned long long c[CTR_NONNULL];
+  read_counters(st, c);
+  if (c[CTR_ERROR]) fail(DFGPU_ERR_ARROW, "DivideByZero");
+  if (bp.has_pred && !p.ps.has_nulls)  // null-free inputs: every row that passed the predicate is a non-null input
+    for (int a = 0; a < st->naggs; a++) st->nonnull_host[size_t(a)] += (long long)c[CTR_PASSED];
+}
+
+// What the interpreter-free scan kernels can do with a batch (once per batch; narrow keys only).
+struct ScanPlan {
+  bool plain = false;  // keys and arguments are plain 4/8-byte columns and the WHERE clause, if any, a chain of column
+                       // comparisons: p.plain describes them for k_hash_agg_plain
+  int lean_mask = 0;   // nonzero: k_hash_agg_lean applies, with this aggregate set (MIN 1, MAX 2, SUM 4, COUNT 8)
+  int lean_mt = 0;     // and this machine type of the argument
+};
+ScanPlan plan_scan(const dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
+  ScanPlan plan;
+  static const bool plain_off = getenv("DFGPU_AGG_PLAIN") && atoi(getenv("DFGPU_AGG_PLAIN")) == 0;  // A/B switch
+  PlainSpec sp;
+  memset(&sp, 0, sizeof(sp));
+  auto wide = [](int dt) {
+    return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64 || dt == DFGPU_FLOAT32 || dt == DFGPU_INT32 || dt == DFGPU_UINT32;
+  };
+  bool ok = !plain_off && !p.ps.has_nulls && p.ps.ncols <= 4;
+  for (int c = 0; ok && c < p.ps.ncols; c++)
+    ok = wide(p.ps.cols[c].dtype) && (reinterpret_cast<uintptr_t>(p.ps.cols[c].ptr) & 15) == 0;
+  for (int k = 0; ok && k < st->nkeys; k++) {
+    const CompiledProgram& cpk = bp.pb.prog(bp.has_pred + k);
+    ok = cpk.is_plain_column;
+    sp.key_slot[k] = cpk.plain_slot;
+  }
+  for (int g = 0; ok && g < bp.nargs; g++) {
+    const CompiledProgram& cpa = bp.pb.prog(bp.has_pred + st->nkeys + g);
+    ok = cpa.is_plain_column;
+    sp.arg_slot[g] = cpa.plain_slot;
+  }
+  if (ok && bp.has_pred) {
+    // t0 [t1 AND|OR [t2 AND|OR ...]] in lowered form: (PUSH_COL, CMP leaf) {(PUSH_COL, CMP leaf), AND|OR stack}*
+    const int b = p.ps.start[0], e = p.ps.start[1];
+    const DevInsn* in = &p.ps.insn[b];
+    auto term_at = [&](int i, PlainTerm* out) {
+      if (i + 1 >= e - b) return false;
+      const DevInsn &c = in[i], &o = in[i + 1];
+      if (c.op != V_PUSH_COL) return false;
+      if (o.op < V_EQ || o.op > V_GE || o.mode == RHS_STACK) return false;
+      if (o.mode == RHS_COL && p.ps.cols[o.slot].dtype != p.ps.cols[c.slot].dtype) return false;
+      memset(out, 0, sizeof(*out));
+      out->kind = o.mode == RHS_COL ? 2 : 3;
+      out->op = o.op;
+      out->a = c.slot;
+      out->b = o.mode == RHS_COL ? o.slot : 0;
+      out->mt = mtype_of(p.ps.cols[c.slot].dtype);
+      out->imm = o.imm;
+      return true;
+    };
+    ok = term_at(0, &sp.term[0]);
+    sp.nterms = ok ? 1 : 0;
+    int i = 2;
+    while (ok && i < e - b) {
+      if (sp.nterms >= 4 || !term_at(i, &sp.term[sp.nterms]) || i + 2 >= e - b) { ok = false; break; }
+      const DevInsn& j = in[i + 2];
+      if ((j.op != V_AND && j.op != V_OR) || j.mode != RHS_STACK) { ok = false; break; }
+      sp.term[sp.nterms].conn = j.op == V_OR ? 1 : 0;
+      sp.nterms++;
+      i += 3;
+    }
+  }
+  sp.ncols = p.ps.ncols;
+  if (ok) p.plain = sp;
+  plan.plain = ok;
+  // lean kernel: one 8-byte integer key column, one 8-byte argument column, distinct MIN/MAX/SUM/COUNT, no WHERE
+  static const bool lean_off = getenv("DFGPU_AGG_LEAN") && atoi(getenv("DFGPU_AGG_LEAN")) == 0;  // A/B switch
+  auto w8 = [](int dt) { return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64; };
+  ok = !lean_off && plan.plain && !bp.has_pred && st->nkeys == 1 && bp.nargs == 1 && w8(p.ps.cols[p.plain.key_slot[0]].dtype) &&
+       w8(p.ps.cols[p.plain.arg_slot[0]].dtype);
+  int mask = 0;
+  for (int a = 0; ok && a < st->naggs; a++) {
+    const int bit = 1 << (st->descs[size_t(a)].func - 1);  // MIN 1, MAX 2, SUM 4, COUNT 8
+    ok = !(mask & bit);
+    mask |= bit;
+  }
+  if (ok) {
+    plan.lean_mask = mask;
+    plan.lean_mt = mtype_of(p.ps.cols[p.plain.arg_slot[0]].dtype);
+  }
+  return plan;
+}
+
+// The scan kernel of one round.  Replays read a row list and the plain and lean kernels start on an even row, so both
+// take the interpreter; FRONT routes rows through the shared-memory front table.  A lean launch gets its table
+// addresses in p.lean.
+ScanKernel choose_scan(const dfgpu_aggstate* st, AggParams& p, const ScanPlan& plan, bool replay, bool front) {
+  if (st->wide) {
+    if (p.ps.has_nulls) return {k_hash_agg_wide<8, true>, "k_hash_agg_wide<8, true>", false};
+    return {k_hash_agg_wide<8, false>, "k_hash_agg_wide<8, false>", false};
+  }
+  if (p.ps.has_nulls) return {k_hash_agg<8, false, true>, "k_hash_agg<8, false, true>", false};
+  const bool even = (p.row_begin & 1) == 0;
+  if (plan.lean_mask && !replay && !front && !st->aos && even) {
+    // the lean kernel addresses the hybrid layout directly
+    p.lean.key_col = (const unsigned long long*)p.ps.cols[p.plain.key_slot[0]].ptr;
+    p.lean.arg_col = (const unsigned long long*)p.ps.cols[p.plain.arg_slot[0]].ptr;
+    p.lean.min_w = p.lean.max_w = 0;
+    p.lean.sum_arr = p.lean.cnt_arr = nullptr;
+    for (int a = 0; a < st->naggs; a++) {
+      const int f = st->descs[size_t(a)].func, l = st->t.loc[a];
+      if (f == DFGPU_AGG_MIN) p.lean.min_w = l;
+      else if (f == DFGPU_AGG_MAX) p.lean.max_w = l;
+      else if (f == DFGPU_AGG_SUM) p.lean.sum_arr = st->t.add + (long long)(~l) * st->t.astride;
+      else p.lean.cnt_arr = st->t.add + (long long)(~l) * st->t.astride;
+    }
+    bool layout_ok = st->t.lw == (((plan.lean_mask & 3) == 3) ? 4 : ((plan.lean_mask & 3) ? 2 : 1));
+    for (int a = 0; a < st->naggs; a++) {
+      const int f = st->descs[size_t(a)].func;
+      layout_ok = layout_ok && ((f == DFGPU_AGG_MIN || f == DFGPU_AGG_MAX) ? st->t.loc[a] >= 1 : st->t.loc[a] < 0);
+    }
+    if (layout_ok) return lean_kernel(plan.lean_mask, plan.lean_mt);
+    return {k_hash_agg_plain<2, false>, "k_hash_agg_plain<2, false>", false};
+  }
+  if (plan.plain && !replay && even) {
+    const bool two = p.plain.ncols <= 2;
+    if (front) {
+      if (two) return {k_hash_agg_plain<2, true>, "k_hash_agg_plain<2, true>", true};
+      return {k_hash_agg_plain<4, true>, "k_hash_agg_plain<4, true>", true};
+    }
+    if (two) return {k_hash_agg_plain<2, false>, "k_hash_agg_plain<2, false>", false};
+    return {k_hash_agg_plain<4, false>, "k_hash_agg_plain<4, false>", false};
+  }
+  const int d = p.ps.max_depth;
+  if (d <= 1) return hash_agg_kernel<1>(front);
+  if (d <= 2) return hash_agg_kernel<2>(front);
+  if (d <= 4) return hash_agg_kernel<4>(front);
+  return hash_agg_kernel<8>(front);
+}
+
+// Single Utf8 key: every row's string must equal its group's representative string, or two strings share a hash.
+void verify_utf8_groups(dfgpu_aggstate* st, const BatchPrograms& bp, long long nrows) {
+  dfgpu_ctx* ctx = st->ctx;
+  VerifyParams vp;
+  memset(&vp, 0, sizeof(vp));
+  vp.hashes = bp.ukey_hash;
+  vp.n = nrows;
+  vp.t = st->t;
+  vp.cap = st->cap;
+  vp.rep_agg = st->naggs - 1;
+  vp.off = bp.ukey->offsets;
+  vp.bytes = (const unsigned char*)bp.ukey->values;
+  vp.srcs = st->d_utf8_srcs;
+  vp.flag = st->d_counters + CTR_DEFERRED;
+  DF_CUDA(cudaMemsetAsync(vp.flag, 0, 8, ctx->stream));
+  launch_kernel(ctx, k_utf8_group_verify, "k_utf8_group_verify", vp, nrows, 256, 8);
+  const unsigned long long flag = read_counter(st, CTR_DEFERRED);
+  if (flag == 1ull) fail(DFGPU_ERR_INTERNAL, "two different Utf8 GROUP BY keys share a 64-bit hash (p < 1e-7 per 1e6 distinct keys)");
+  if (flag) fail(DFGPU_ERR_INTERNAL, "Utf8 GROUP BY verification could not find a group");
+}
+
+// GROUP BY: scan the batch into the table.  Rows that find no slot go to an overflow list and are replayed in the next
+// round, after the table grew x4 -- or as they are, when each of them only met a slot that was still being published
+// (counter CTR_DEFERRED, which only wide scans set).
+void group_by_update(dfgpu_aggstate* st, const dfgpu_batch* batch, const BatchPrograms& bp, AggParams& p, Trace& tr) {
+  dfgpu_ctx* ctx = st->ctx;
+  if (st->wide) {
+    // retain this batch's Utf8 key columns: a group's string lives in the batch whose row created it
+    p.wide.kw = st->nkeys;
+    bool new_src = false;
+    for (int k = 0; k < st->nkeys; k++) {
+      p.wide.is_utf8[k] = st->key_is_utf8[size_t(k)];
+      const DevColumn* uc = bp.key_utf8[size_t(k)];
+      if (!uc) continue;
+      if (st->utf8_srcs.size() >= (1u << 20)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "more than 2^20 retained Utf8 GROUP BY key columns");
+      p.wide.ref_base[k] = retain_utf8(st, *uc, batch->nrows) << UTF8_SRC_SHIFT;
+      p.wide.off[k] = st->utf8_srcs.back().off;
+      p.wide.bytes[k] = st->utf8_srcs.back().bytes;
+      new_src = true;
+    }
+    if (new_src) upload_utf8_srcs(st);
+    p.wide.srcs = st->d_utf8_srcs;
+  }
+  const ScanPlan plan = st->wide ? ScanPlan{} : plan_scan(st, bp, p);
+  DevBufs lists(ctx);
+  unsigned* ovf[2] = {lists.alloc<unsigned>(size_t(batch->nrows) * 4), nullptr};
+  tr.mark("overflow list alloc");
+  // First big batch with no cardinality hint: a 1 Mi-row prefix is aggregated first; the number of groups it
+  // produces decides the table layout (SoA while the hot sectors fit L2, AoS beyond) before the bulk of the batch
+  // is touched.  Wide tables are AoS from the start.
+  const long long kPrefix = 1ll << 20;
+  const bool sample = st->rows_seen == batch->nrows && st->expected == 0 && !st->aos && batch->nrows >= 4 * kPrefix;
+  std::vector<std::pair<long long, long long>> ranges;  // (begin, count)
+  if (sample) {
+    ranges.push_back({0, kPrefix});
+    ranges.push_back({kPrefix, batch->nrows - kPrefix});
+  } else {
+    ranges.push_back({0, batch->nrows});
+  }
+  for (size_t ri = 0; ri < ranges.size(); ri++) {
+    int cur = 0;
+    const unsigned* list = nullptr;
+    long long nlist = 0;
+    for (int round = 0;; round++) {
+      if (round > 60) fail(DFGPU_ERR_INTERNAL, "hash table growth did not converge");
+      p.t = st->t;
+      p.cap = st->cap;
+      p.max_groups = st->cap / 2;
+      p.row_begin = ranges[ri].first;
+      p.nrows = ranges[ri].second;
+      p.row_list = list;
+      p.nlist = nlist;
+      p.ovf_rows = ovf[cur];
+      DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_OVERFLOW, 0, 8, ctx->stream));
+      // <= 64 groups: one private 256-slot table per warp (same shared-memory footprint as the
+      // CTA-wide 2048-slot table); otherwise one table per CTA
+      p.front_per_warp = st->ngroups <= 64 ? 1 : 0;
+      p.front_slots = p.front_per_warp ? AG_FRONT_SLOTS / (AG_THREADS / 32) : AG_FRONT_SLOTS;
+      // (A persisting-L2 access-policy window over the table was tried and removed: it slowed the scan
+      // several-fold at 1e5 and 1e6 groups.)
+      launch_scan(ctx, choose_scan(st, p, plan, list != nullptr, st->use_front && !list), p, list ? nlist : p.nrows);
+      unsigned long long c[CTR_NONNULL];
+      read_counters(st, c);
+      if (c[CTR_ERROR] == 2) fail(DFGPU_ERR_INTERNAL, "front-table merge could not find a slot");
+      if (c[CTR_ERROR]) fail(DFGPU_ERR_ARROW, "DivideByZero");
+      st->ngroups = (long long)c[CTR_GROUPS];
+      st->sentinel_used = c[CTR_SENTINEL] != 0;
+      const long long novf = (long long)c[CTR_OVERFLOW], deferred = (long long)c[CTR_DEFERRED];
+      if (deferred) DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_DEFERRED, 0, 8, ctx->stream));
+      tr.mark(ri == 0 && ranges.size() > 1 ? "scan kernel (prefix)" : "scan kernel");
+      if (novf == 0) {
+        if (st->ngroups > st->cap / 2) { table_grow(st, st->cap * 4); tr.mark("table_grow (load factor)"); }
+        break;
+      }
+      // rows that only met a slot still being published need no bigger table: replay them as they are
+      if (!(novf == deferred && st->ngroups <= st->cap / 2)) table_grow(st, st->cap * 4);
+      list = ovf[cur];
+      nlist = novf;
+      cur ^= 1;
+      if (!ovf[cur]) ovf[cur] = lists.alloc<unsigned>(size_t(batch->nrows) * 4);
+    }
+    // few groups so far: later rows of this stream go through the shared-memory front table
+    st->use_front = st->ngroups <= AG_FRONT_MAX_GROUPS && st->rows_seen >= (1ll << 20);
+    if (sample && ri == 0) {
+      // size (and lay out) the table for the estimated number of groups before the bulk of the batch
+      // is touched: one rebuild of a ~1 Mi-entry table instead of repeated 4x growth + replays
+      long long est = std::max(estimate_groups(st->ngroups, kPrefix, batch->nrows), st->ngroups);
+      const long long afford = (long long)(ctx->device_mem_bytes / 8) / (32 * (1 + st->naggs));  // slots that fit in 1/8 of device memory
+      long long want_cap = std::max(AG_MIN_CAP, next_pow2(est * 2));
+      while (want_cap > st->cap && want_cap > afford) want_cap >>= 1;
+      const bool to_aos = !st->aos && want_aos(est, st->descs, st->naggs);
+      if (to_aos || want_cap > st->cap) {
+        st->aos = st->aos || to_aos;
+        table_grow(st, std::max(st->cap, want_cap));
+        tr.mark("table_grow (prefix estimate)");
+      }
+    }
+  }
+  if (bp.ukey) verify_utf8_groups(st, bp, batch->nrows);
+}
+
+void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
+  if (st->finished) fail(DFGPU_ERR_GENERAL, "aggregate already finished");
+  dfgpu_ctx* ctx = st->ctx;
+  ctx->use();
+  if (batch->nrows >= (1ll << 32)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "batches of 2^32 rows or more");
+  Trace tr(ctx);
+  BatchPrograms bp(batch, ctx);
+  compile_batch(st, batch, bp);
+  type_batch(st, bp);
+  tr.mark("programs + table alloc");
+  AggParams p;
+  memset(&p, 0, sizeof(p));
+  bp.pb.finish(&p.ps);
+  for (int s = 0; s < p.ps.ncols; s++)
+    if (!is_numeric(p.ps.cols[s].dtype) && p.ps.cols[s].dtype != DFGPU_BOOL)  // Boolean columns: WHERE operands (boolean_ops!)
+      fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string("expressions over ") + dtype_name(p.ps.cols[s].dtype) + " columns are not supported on the GPU path yet");
+  if (p.ps.max_depth > 8) fail(DFGPU_ERR_NOT_IMPLEMENTED, "expression too deep (register stack depth > 8)");
+  st->rows_seen += batch->nrows;
+  if (batch->nrows == 0) return;
+
+  p.nkeys = st->nkeys;
+  p.naggs = st->naggs;
+  for (int a = 0; a < st->naggs; a++) {
+    p.aggs[a] = st->descs[size_t(a)];
+    p.agg_arg[a] = bp.agg_arg[size_t(a)];
+  }
+  p.nargs = bp.nargs;
+  for (int k = 0; k < st->nkeys; k++) {
+    p.key_mask[k] = st->key_mask[size_t(k)];
+    p.key_shift[k] = st->key_shift[size_t(k)];
+  }
+  p.nrows = batch->nrows;
+  p.counters = st->d_counters;
+  p.has_pred = bp.has_pred;
+  if (st->nkeys == 0) reduce_update(st, bp, p);
+  else group_by_update(st, batch, bp, p, tr);
 }
 }  // namespace
 
@@ -2263,30 +2312,12 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
 // ---------------------------------------------------------------------------------------------
 namespace {
 
-void agg_export_raw(dfgpu_aggstate* st, unsigned long long** keys, unsigned long long** vals, long long* n) {
-  dfgpu_ctx* ctx = st->ctx;
+void agg_export_raw(dfgpu_aggstate* st, DevBufs& bufs, unsigned long long** keys, unsigned long long** vals, long long* n) {
   const long long cnt = st->nkeys == 0 ? 1 : st->ngroups + (st->sentinel_used ? 1 : 0);
   const size_t alloc_n = size_t(cnt > 0 ? cnt : 1);
-  *keys = (unsigned long long*)ctx->alloc(alloc_n * 8);
-  *vals = (unsigned long long*)ctx->alloc(alloc_n * 8 * size_t(st->naggs));
-  CompactParams cp;
-  memset(&cp, 0, sizeof(cp));
-  cp.t = st->t;
-  cp.cap = st->cap;
-  cp.sentinel_used = st->nkeys == 0 ? 1 : (st->sentinel_used ? 1 : 0);
-  cp.nkeys = st->nkeys;
-  cp.naggs = st->naggs;
-  cp.raw = 1;
-  cp.out_keys[0] = *keys;
-  for (int a = 0; a < st->naggs; a++) {
-    cp.aggs[a] = st->descs[size_t(a)];
-    cp.out_vals[a] = *vals + size_t(a) * alloc_n;
-  }
-  DF_CUDA(cudaMemsetAsync(st->d_counters + 4, 0, 8, ctx->stream));
-  cp.counter = st->d_counters + 4;
-  k_compact<<<grid_for(ctx, st->cap + 1, 256, 8), 256, 0, ctx->stream>>>(cp);
-  DF_CUDA(cudaGetLastError());
-  ctx->launches++;
+  *keys = bufs.alloc(alloc_n * 8);
+  *vals = bufs.alloc(alloc_n * 8 * size_t(st->naggs));
+  compact_raw(st, st->t, st->cap, st->nkeys == 0 ? 1 : (st->sentinel_used ? 1 : 0), nullptr, *keys, *vals, alloc_n, 0);
   *n = cnt;
 }
 
@@ -2299,21 +2330,19 @@ void agg_exchange_scalars(dfgpu_ctx* ctx, dfgpu_aggstate* st) {
   }
   // per-aggregate non-null input counts travel with the accumulators: fold the host-side counts of the
   // null-free batches into the device counters, which the exchange sums over ranks
-  DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 40, st->d_counters + 8, 64, cudaMemcpyDeviceToHost, ctx->stream));
+  DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + HS_NONNULL, st->d_counters + CTR_NONNULL, kMaxAggs * 8, cudaMemcpyDeviceToHost, ctx->stream));
   DF_CUDA(cudaStreamSynchronize(ctx->stream));
   for (int a = 0; a < kMaxAggs; a++) {
-    if (a < st->naggs) ctx->h_scratch[40 + a] += (unsigned long long)st->nonnull_host[size_t(a)];
+    if (a < st->naggs) ctx->h_scratch[HS_NONNULL + a] += (unsigned long long)st->nonnull_host[size_t(a)];
     if (a < st->naggs) st->nonnull_host[size_t(a)] = 0;
   }
-  ctx->h_scratch[48] = (unsigned long long)st->rows_seen;
-  DF_CUDA(cudaMemcpyAsync(st->d_counters + 8, ctx->h_scratch + 40, 64, cudaMemcpyHostToDevice, ctx->stream));
-  DF_CUDA(cudaMemcpyAsync(st->d_counters + 7, ctx->h_scratch + 48, 8, cudaMemcpyHostToDevice, ctx->stream));
+  ctx->h_scratch[HS_ROWS] = (unsigned long long)st->rows_seen;
+  DF_CUDA(cudaMemcpyAsync(st->d_counters + CTR_NONNULL, ctx->h_scratch + HS_NONNULL, kMaxAggs * 8, cudaMemcpyHostToDevice, ctx->stream));
+  DF_CUDA(cudaMemcpyAsync(st->d_counters + CTR_ROWS, ctx->h_scratch + HS_ROWS, 8, cudaMemcpyHostToDevice, ctx->stream));
   st->saw_nulls = true;
   // slot 0's accumulators (cap = 0: every accumulator in its own one-word array, contiguous)
-  comm_allreduce_aggs(ctx, st->naggs, funcs, mtypes, st->t.val(0, 0), st->d_counters + 8, st->d_counters + 7);
-  DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 48, st->d_counters + 7, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  DF_CUDA(cudaStreamSynchronize(ctx->stream));
-  st->rows_seen = (long long)ctx->h_scratch[48];
+  comm_allreduce_aggs(ctx, st->naggs, funcs, mtypes, st->t.val(0, 0), st->d_counters + CTR_NONNULL, st->d_counters + CTR_ROWS);
+  st->rows_seen = (long long)read_counter(st, CTR_ROWS);
 }
 
 // GROUP BY.  Returns the global result as raw rows of (1 + naggs) words in *rows (caller frees) and their number.
@@ -2323,24 +2352,20 @@ struct GatheredSegments {
   long long stride = 0;
   long long n[AG_MAX_WORLD] = {0};
 };
-void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, unsigned long long** rows_out, long long* n_out, GatheredSegments* seg, bool* regroup) {
+void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, DevBufs& rows_buf, unsigned long long** rows_out, long long* n_out, GatheredSegments* seg,
+                         bool* regroup) {
   const int W = ctx->world, me = ctx->rank;
   if (W > AG_MAX_WORLD) fail(DFGPU_ERR_NOT_IMPLEMENTED, "more than " + std::to_string(AG_MAX_WORLD) + " ranks");
   Trace tr(ctx);
-  std::vector<void*> owned;
-  struct Freer { dfgpu_ctx* c; std::vector<void*>* v; ~Freer() { for (void* q : *v) c->free(q); } } freer{ctx, &owned};
-  auto dalloc = [&](size_t words) { void* q = ctx->alloc((words ? words : 1) * 8); owned.push_back(q); return (unsigned long long*)q; };
+  DevBufs tmp(ctx);
+  auto dalloc = [&](size_t words) { return tmp.alloc((words ? words : 1) * 8); };
   // 1. local entries, counted per owner
   unsigned long long *keys = nullptr, *vals = nullptr;
   long long n_local = 0;
   // Utf8 and wide keys do not fit the (packed key, accumulators) rows of this exchange: if any rank has them, every
   // rank leaves through the regroup merge (finish_regroup) right after the header round
   const bool special = st->typed && (st->wide || st->utf8_key);
-  if (st->typed && !special) {
-    agg_export_raw(st, &keys, &vals, &n_local);
-    owned.push_back(keys);
-    owned.push_back(vals);
-  }
+  if (st->typed && !special) agg_export_raw(st, tmp, &keys, &vals, &n_local);
   unsigned long long* d_rec = dalloc(size_t(HDR + W));
   DF_CUDA(cudaMemsetAsync(d_rec, 0, size_t(HDR + W) * 8, ctx->stream));
   OwnerParams op;
@@ -2352,12 +2377,8 @@ void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, unsigned long long*
   op.world = W;
   op.naggs = st->naggs;
   op.counts = d_rec + HDR;
-  if (n_local > 0) {
-    k_owner_count<<<grid_for(ctx, n_local, 256 * 4, 8), 256, 0, ctx->stream>>>(op);
-    DF_CUDA(cudaGetLastError());
-    ctx->launches++;
-  }
-  unsigned long long* hh = ctx->h_scratch + 16;  // pinned
+  if (n_local > 0) launch_kernel(ctx, k_owner_count, "k_owner_count", op, n_local, 256 * 4, 8);
+  unsigned long long* hh = ctx->h_scratch + HS_HEADER;  // pinned
   memset(hh, 0, HDR * 8);
   hh[0] = st->typed ? 1 : 0;
   hh[1] = (unsigned long long)st->nkeys;
@@ -2407,16 +2428,7 @@ void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, unsigned long long*
       d.out_dtype = uint8_t(d.func == DFGPU_AGG_COUNT ? DFGPU_UINT64 : dt);
       st->descs.push_back(d);
     }
-    st->key_shift.clear();
-    st->key_mask.clear();
-    int bits = 0;
-    for (int k = st->nkeys - 1; k >= 0 && !*regroup; k--) {  // (the regroup merge never packs keys)
-      const int w = dtype_width(st->key_dtypes[size_t(k)]) * 8;
-      st->key_shift.insert(st->key_shift.begin(), bits);
-      st->key_mask.insert(st->key_mask.begin(), w == 64 ? ~0ull : ((1ull << w) - 1ull));
-      bits += w;
-    }
-    if (st->nkeys == 1 && !*regroup) st->key_mask[0] = ~0ull;
+    if (!*regroup) pack_keys(st);  // (the regroup merge never packs keys)
     st->typed = true;
   }
   if (*regroup) {
@@ -2450,9 +2462,7 @@ void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, unsigned long long*
     op.cursor = d_cursor;
     op.rows = d_send;
     for (int r = 0; r < W; r++) op.seg_off[r] = s_off[size_t(r)] / E;
-    k_owner_scatter<<<grid_for(ctx, n_local, 256 * 4, 8), 256, 0, ctx->stream>>>(op);
-    DF_CUDA(cudaGetLastError());
-    ctx->launches++;
+    launch_kernel(ctx, k_owner_scatter, "k_owner_scatter", op, n_local, 256 * 4, 8);
   }
   // 5. all-to-all: every entry goes to its owner
   unsigned long long* d_recv = dalloc(total_recv * E);
@@ -2465,7 +2475,7 @@ void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, unsigned long long*
     const long long ocap = std::max<long long>(1024, next_pow2(2 * (long long)total_recv));
     const bool oaos = want_aos((long long)total_recv, st->descs, st->naggs);
     TableLayout ot = table_alloc(ctx, st->naggs, st->nkeys, st->descs, ocap, oaos);
-    owned.push_back(ot.base);
+    tmp.blocks.push_back(ot.base);
     MergeParams mp;
     memset(&mp, 0, sizeof(mp));
     mp.in_keys = d_recv;
@@ -2478,42 +2488,21 @@ void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, unsigned long long*
     mp.t = ot;
     mp.cap = ocap;
     mp.naggs = st->naggs;
-    DF_CUDA(cudaMemsetAsync(st->d_counters, 0, 32, ctx->stream));
+    DF_CUDA(cudaMemsetAsync(st->d_counters, 0, (CTR_ERROR + 1) * 8, ctx->stream));  // slots CTR_GROUPS .. CTR_ERROR
     mp.counters = st->d_counters;
-    k_merge<<<grid_for(ctx, mp.n, 256, 8), 256, 0, ctx->stream>>>(mp);
-    DF_CUDA(cudaGetLastError());
-    ctx->launches++;
+    launch_kernel(ctx, k_merge, "k_merge", mp, mp.n, 256, 8);
     // compact what this rank owns without a host round trip in between: the buffer has room for the largest
     // number of entries any rank receives (known to all from the count matrix), which also makes it a valid send
     // buffer of the padded all-gather below; the sentinel slot's use and the count stay on the device
     d_owned = dalloc(max_recv * E);
-    CompactParams cp;
-    memset(&cp, 0, sizeof(cp));
-    cp.t = ot;
-    cp.cap = ocap;
-    cp.sentinel_used = 0;
-    cp.sentinel_flag = st->d_counters + 2;
-    cp.nkeys = st->nkeys;
-    cp.naggs = st->naggs;
-    cp.raw = 1;
-    cp.raw_stride = (long long)E;
-    cp.out_keys[0] = d_owned;
-    for (int a = 0; a < st->naggs; a++) {
-      cp.aggs[a] = st->descs[size_t(a)];
-      cp.out_vals[a] = d_owned + 1 + a;
-    }
-    DF_CUDA(cudaMemsetAsync(st->d_counters + 4, 0, 8, ctx->stream));
-    cp.counter = st->d_counters + 4;
-    k_compact<<<grid_for(ctx, ocap + 1, 256, 8), 256, 0, ctx->stream>>>(cp);
-    DF_CUDA(cudaGetLastError());
-    ctx->launches++;
+    compact_raw(st, ot, ocap, 0, st->d_counters + CTR_SENTINEL, d_owned, d_owned + 1, 1, (long long)E);
   } else {
-    DF_CUDA(cudaMemsetAsync(st->d_counters, 0, 64, ctx->stream));
+    DF_CUDA(cudaMemsetAsync(st->d_counters, 0, CTR_NONNULL * 8, ctx->stream));  // no entries, no merge error
   }
   // 7. every rank gathers the owned segments: sizes first ([owned entries, merge error flag] per rank)
   unsigned long long* d_n = dalloc(size_t(2 + 2 * W));
-  DF_CUDA(cudaMemcpyAsync(d_n, st->d_counters + 4, 8, cudaMemcpyDeviceToDevice, ctx->stream));
-  DF_CUDA(cudaMemcpyAsync(d_n + 1, st->d_counters + 3, 8, cudaMemcpyDeviceToDevice, ctx->stream));
+  DF_CUDA(cudaMemcpyAsync(d_n, st->d_counters + CTR_COMPACT, 8, cudaMemcpyDeviceToDevice, ctx->stream));
+  DF_CUDA(cudaMemcpyAsync(d_n + 1, st->d_counters + CTR_ERROR, 8, cudaMemcpyDeviceToDevice, ctx->stream));
   comm_allgather_u64(ctx, d_n, d_n + 2, 2);
   std::vector<unsigned long long> owned_n2(size_t(2 * W), 0);
   DF_CUDA(cudaMemcpyAsync(owned_n2.data(), d_n + 2, size_t(2 * W) * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2532,7 +2521,7 @@ void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, unsigned long long*
     G += size_t(owned_n[size_t(r)]);
   }
   if (max_owned > max_recv) fail(DFGPU_ERR_INTERNAL, "owned groups exceed the received entries");
-  unsigned long long* d_final = (unsigned long long*)ctx->alloc((max_owned ? size_t(W) * max_owned * E : 1) * 8);
+  unsigned long long* d_final = rows_buf.alloc((max_owned ? size_t(W) * max_owned * E : 1) * 8);
   if (max_owned > 0) {
     if (!d_owned) d_owned = dalloc(max_recv * E);  // a rank that owns nothing still contributes its (empty) segment
     comm_allgather_u64(ctx, d_owned, d_final, max_owned * E);
@@ -2563,7 +2552,7 @@ struct WorldGuard {  // run a stretch of the operator as if no communicator were
 };
 
 std::unique_ptr<dfgpu_result> finish_regroup(dfgpu_ctx* ctx, dfgpu_aggstate* st) {
-  const int W = ctx->world, me = ctx->rank;
+  const int W = ctx->world;
   const int user_aggs = st->utf8_key ? st->naggs - 1 : st->naggs;
   const int ncols = st->nkeys + user_aggs;
   // 1. this rank's own result (an empty one when it saw no batch: types were adopted from the header)
@@ -2596,11 +2585,9 @@ std::unique_ptr<dfgpu_result> finish_regroup(dfgpu_ctx* ctx, dfgpu_aggstate* st)
   if (int(local->cols.size()) != ncols) fail(DFGPU_ERR_INTERNAL, "regroup merge: unexpected local result shape");
   // 2. sizes: [rows, bytes of every Utf8 column] per rank
   const int NH = 1 + kMaxKeys;
-  std::vector<void*> tmp;
-  struct Freer { dfgpu_ctx* c; std::vector<void*>* v; ~Freer() { for (void* q : *v) c->free(q); } } freer{ctx, &tmp};
-  auto dalloc = [&](size_t bytes) { void* q = ctx->alloc(bytes ? bytes : 8); tmp.push_back(q); return q; };
-  unsigned long long* d_h = (unsigned long long*)dalloc(size_t(NH) * 8 * size_t(W + 1));
-  unsigned long long* hh = ctx->h_scratch + 16;
+  DevBufs tmp(ctx);
+  unsigned long long* d_h = tmp.alloc(size_t(NH) * 8 * size_t(W + 1));
+  unsigned long long* hh = ctx->h_scratch + HS_HEADER;
   memset(hh, 0, size_t(NH) * 8);
   hh[0] = (unsigned long long)local->nrows;
   for (int k = 0; k < st->nkeys; k++)
@@ -2641,7 +2628,7 @@ std::unique_ptr<dfgpu_result> finish_regroup(dfgpu_ctx* ctx, dfgpu_aggstate* st)
       gc.values = ctx->alloc(total_b ? total_b : 1);
       comm_allgather_bytes_v(ctx, lc.values, gc.values, off.data(), cnt.data());
       // offsets: every rank's (rows + 1) array, spliced with its byte base
-      int* raw = (int*)dalloc(size_t(N + W) * 4);
+      int* raw = tmp.alloc<int>(size_t(N + W) * 4);
       for (int r = 0; r < W; r++) {
         off[size_t(r)] = size_t(row_base[size_t(r)] + r) * 4;
         cnt[size_t(r)] = size_t(all[size_t(r) * NH] + 1) * 4;
@@ -2666,7 +2653,6 @@ std::unique_ptr<dfgpu_result> finish_regroup(dfgpu_ctx* ctx, dfgpu_aggstate* st)
     gathered->cols.push_back(gc);
   }
   DF_CUDA(cudaStreamSynchronize(ctx->stream));
-  (void)me;
   // 4. aggregate the partial results once more, with each aggregate's merge function
   const size_t nk = size_t(st->nkeys), na = size_t(user_aggs);
   std::vector<dfgpu_insn> kprog(nk), aprog(na);
@@ -2742,10 +2728,10 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
     long long xn = -1;
     GatheredSegments xseg;
     bool regroup = false;
-    struct XFree { dfgpu_ctx* c; unsigned long long** p; ~XFree() { c->free(*p); } } xfree{ctx, &xrows};
+    DevBufs xbuf(ctx);
     if (ctx->world > 1) {
       if (st->nkeys == 0) agg_exchange_scalars(ctx, st);
-      else agg_exchange_groups(ctx, st, &xrows, &xn, &xseg, &regroup);
+      else agg_exchange_groups(ctx, st, xbuf, &xrows, &xn, &xseg, &regroup);
       if (regroup) {
         *out = finish_regroup(ctx, st).release();
         st->finished = true;
@@ -2832,21 +2818,13 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
         dp.aggs[a] = cp.aggs[a];
         dp.out_vals[a] = cp.out_vals[a];
       }
-      if (xn > 0) {
-        k_decode_rows<<<grid_for(ctx, xn, 256, 8), 256, 0, ctx->stream>>>(dp);
-        DF_CUDA(cudaGetLastError());
-        ctx->launches++;
-      }
+      if (xn > 0) launch_kernel(ctx, k_decode_rows, "k_decode_rows", dp, xn, 256, 8);
       DF_CUDA(cudaStreamSynchronize(ctx->stream));
     } else {
-      DF_CUDA(cudaMemsetAsync(st->d_counters + 4, 0, 8, ctx->stream));
-      cp.counter = st->d_counters + 4;
-      k_compact<<<grid_for(ctx, st->cap + 1, 256, 8), 256, 0, ctx->stream>>>(cp);
-      DF_CUDA(cudaGetLastError());
-      ctx->launches++;
-      DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 8, st->d_counters + 4, 8, cudaMemcpyDeviceToHost, ctx->stream));
-      DF_CUDA(cudaStreamSynchronize(ctx->stream));
-      if ((long long)ctx->h_scratch[8] != cnt) fail(DFGPU_ERR_INTERNAL, "table compaction count mismatch");
+      DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_COMPACT, 0, 8, ctx->stream));
+      cp.counter = st->d_counters + CTR_COMPACT;
+      launch_kernel(ctx, k_compact, "k_compact", cp, st->cap + 1, 256, 8);
+      if ((long long)read_counter(st, CTR_COMPACT) != cnt) fail(DFGPU_ERR_INTERNAL, "table compaction count mismatch");
     }
     res->nrows = cnt;
     for (auto& wr : wide_refs)  // wide keys: the Utf8 parts' strings, in output order
@@ -2857,9 +2835,9 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
       // an aggregate that saw no non-null input is null (array_from_scalar!, aggregate.rs:641-643)
       std::vector<long long> nonnull = st->nonnull_host;
       if (st->saw_nulls) {
-        DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 40, st->d_counters + 8, 64, cudaMemcpyDeviceToHost, ctx->stream));
+        DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + HS_NONNULL, st->d_counters + CTR_NONNULL, kMaxAggs * 8, cudaMemcpyDeviceToHost, ctx->stream));
         DF_CUDA(cudaStreamSynchronize(ctx->stream));
-        for (int a = 0; a < st->naggs; a++) nonnull[size_t(a)] += (long long)ctx->h_scratch[40 + a];
+        for (int a = 0; a < st->naggs; a++) nonnull[size_t(a)] += (long long)ctx->h_scratch[HS_NONNULL + a];
       }
       for (int a = 0; a < st->naggs; a++) {
         if (nonnull[size_t(a)] > 0 || (st->rows_seen > 0 && st->descs[size_t(a)].func == DFGPU_AGG_COUNT)) continue;

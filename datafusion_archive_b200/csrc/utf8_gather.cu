@@ -97,20 +97,6 @@ __global__ void k_utf8_hash(const int* __restrict__ off, const unsigned char* __
   }
 }
 
-// every row's string must equal the string of its group's representative (rep[i] = source|row):
-// a mismatch means two different strings share a 64-bit hash
-__global__ void k_utf8_verify(const int* __restrict__ off, const unsigned char* __restrict__ bytes, long long n,
-                              const unsigned long long* __restrict__ rep, const Utf8Source* __restrict__ srcs, unsigned long long* flag) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    long long r;
-    const Utf8Source& sc = src_of(srcs, rep[i], &r);
-    const int s = off[i], len = off[i + 1] - s, s2 = sc.off[r], len2 = sc.off[r + 1] - s2;
-    bool same = len == len2;
-    for (int b = 0; same && b < len; b++) same = bytes[s + b] == sc.bytes[s2 + b];
-    if (!same) *flag = 1ull;
-  }
-}
-
 void gather_utf8_multi(dfgpu_ctx* ctx, const Utf8Source* d_srcs, const unsigned long long* d_idx, long long nsel, DevColumn* out);
 
 // gather `src` (Utf8) by `d_idx[0..nsel)` into `out`.  Synchronises the stream (byte count).
@@ -153,15 +139,6 @@ void utf8_hash(dfgpu_ctx* ctx, const DevColumn& src, long long n, unsigned long 
   if (n <= 0) return;
   const int grid = (int)std::min<long long>((n + 255) / 256, (long long)ctx->sm_count * 16);
   k_utf8_hash<<<grid, 256, 0, ctx->stream>>>(src.offsets, (const unsigned char*)src.values, n, d_out);
-  DF_CUDA(cudaGetLastError());
-  ctx->launches++;
-}
-
-void utf8_verify(dfgpu_ctx* ctx, const DevColumn& src, long long n, const unsigned long long* d_rep, const Utf8Source* d_srcs,
-                 unsigned long long* d_flag) {
-  if (n <= 0) return;
-  const int grid = (int)std::min<long long>((n + 255) / 256, (long long)ctx->sm_count * 16);
-  k_utf8_verify<<<grid, 256, 0, ctx->stream>>>(src.offsets, (const unsigned char*)src.values, n, d_rep, d_srcs, d_flag);
   DF_CUDA(cudaGetLastError());
   ctx->launches++;
 }
