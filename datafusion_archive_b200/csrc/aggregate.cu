@@ -26,6 +26,8 @@ constexpr int kMaxKeys = 4;
 constexpr unsigned long long EMPTY_KEY = ~0ull;
 constexpr int AG_MAX_PROBE = 1 << 14;
 constexpr long long AG_MIN_CAP = 1ll << 22;
+constexpr long long AG_SET_MIN_CAP = 1ll << 20;  // COUNT(DISTINCT) pair sets: 16-byte slots
+constexpr long long AG_PREFIX_ROWS = 1ll << 20;  // prefix sample that sizes the tables of a first big batch
 
 struct AggDesc {
   uint8_t func;   // DFGPU_AGG_*
@@ -1319,6 +1321,200 @@ __global__ void __launch_bounds__(256) k_table_init(const __grid_constant__ Init
   }
 }
 
+// ---- COUNT(DISTINCT x): pair sets ----------------------------------------------------------------------------
+// One open-addressed set per distinct argument program.  A slot is 16 bytes, (packed group key, normalised value),
+// both words EMPTY_KEY when empty.  A slot is only ever written by the 128-bit CAS that claims it, so it changes
+// once, from empty to its pair.  The one pair equal to the empty marker is kept in a flag counter instead.
+constexpr int DCTR_OVERFLOW = 0;  // rows appended to the overflow list
+constexpr int DCTR_ERROR = 1;     // 1: an expression raised DivideByZero, 2: a pair found no slot, or no group
+constexpr int DCTR_SET = 2;       // [DCTR_SET + 2s]: pairs in set s, [DCTR_SET + 2s + 1]: nonzero when set s holds the empty-marker pair
+constexpr int DCTR_SLOTS = DCTR_SET + 2 * kMaxAggs;
+
+struct SetParams {
+  unsigned long long* slots[kMaxAggs];  // two words per slot
+  long long cap[kMaxAggs];              // power of two
+  long long max_fill[kMaxAggs];         // new pairs are refused (-> overflow list) beyond this fill
+  int mt[kMaxAggs];                     // machine type of the argument
+};
+
+// 128-bit atomicCAS (ATOMG.E.CAS.128 on sm_90); returns the slot as it was, read atomically
+__device__ __forceinline__ void cas128(unsigned long long* q, unsigned long long cmp_lo, unsigned long long cmp_hi, unsigned long long new_lo,
+                                       unsigned long long new_hi, unsigned long long& old_lo, unsigned long long& old_hi) {
+  asm volatile(
+      "{\n\t.reg .b128 d, c, s;\n\t"
+      "mov.b128 c, {%2, %3};\n\t"
+      "mov.b128 s, {%4, %5};\n\t"
+      "atom.global.cas.b128 d, [%6], c, s;\n\t"
+      "mov.b128 {%0, %1}, d;\n\t}"
+      : "=l"(old_lo), "=l"(old_hi)
+      : "l"(cmp_lo), "l"(cmp_hi), "l"(new_lo), "l"(new_hi), "l"(q)
+      : "memory");
+}
+
+// The word distinctness is decided on: SQL `=` for floats (+0.0 equals -0.0), except that every NaN is one value.
+__device__ __forceinline__ unsigned long long distinct_norm(unsigned long long v, int mt) {
+  if (mt == MT_F64) {
+    const double d = u2d(v);
+    return d != d ? 0x7ff8000000000000ull : (d == 0.0 ? 0ull : v);
+  }
+  if (mt == MT_F32) {
+    const float f = u2f(v);
+    return f != f ? 0x7fc00000ull : (f == 0.0f ? 0ull : (v & 0xffffffffull));
+  }
+  return v;
+}
+
+// Insert (key, val): 1 = inserted, 0 = already there, -1 = not inserted (full: the set refuses new pairs; or probe limit).
+__device__ __forceinline__ int set_insert(unsigned long long* slots, long long cap, int hshift, unsigned long long key, unsigned long long val,
+                                          bool full) {
+  const unsigned long long mask = (unsigned long long)cap - 1ull;
+  unsigned long long h = home_slot(mix64(val ^ mix64(key)), hshift);
+  for (int probes = 0; probes < AG_MAX_PROBE; ++probes) {
+    unsigned long long* q = slots + 2 * h;
+    unsigned long long a, b;
+    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "l"(q) : "memory");
+    // the halves of a plain load may straddle a claim: only a view without an EMPTY_KEY half is certainly a
+    // published pair; otherwise the CAS (a no-op when full) reads the slot atomically, claiming it when empty
+    if (a == EMPTY_KEY || b == EMPTY_KEY) {
+      cas128(q, EMPTY_KEY, EMPTY_KEY, full ? EMPTY_KEY : key, full ? EMPTY_KEY : val, a, b);
+      if (a == EMPTY_KEY && b == EMPTY_KEY) return full ? -1 : 1;
+    }
+    if (a == key && b == val) return 0;
+    h = (h + 1ull) & mask;
+  }
+  return -1;
+}
+
+// Insert the (group key, argument) pairs of a batch into the sets, one set per argument program p.ps[has_pred +
+// nkeys + s].  Runs after the group scan over the same rows: every key it packs (exactly as the scan packs it) is
+// already in the group table.  Rows that fail the WHERE clause and null arguments are skipped.  A row that some set
+// refused goes to the overflow list and is replayed into every set after growth (inserting a pair twice is harmless).
+template <class Src, bool NULLS>
+__device__ __forceinline__ void distinct_insert_body(const AggParams& p, const SetParams& sp) {
+  constexpr int R = Src::R;
+  constexpr int TILE = AG_THREADS * R;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const long long n = p.row_list ? p.nlist : p.nrows;
+  const unsigned long long stream_policy = l2_evict_first_policy();
+  bool bad = false;
+  Src src;
+  for (long long tb = (long long)blockIdx.x * TILE; tb < n; tb += (long long)gridDim.x * TILE) {
+    unsigned full = 0;  // bit s: set s refuses new pairs (fill limit, once per warp per tile)
+    if (lane == 0)
+      for (int s = 0; s < p.nargs; s++)
+        if ((long long)__ldcg(&p.counters[DCTR_SET + 2 * s]) >= sp.max_fill[s]) full |= 1u << s;
+    full = __shfl_sync(0xffffffffu, full, 0);
+    src.load(p, tb, n, tid, stream_policy);
+    src.prepare(p);
+    unsigned long long key[R];
+#pragma unroll
+    for (int r = 0; r < R; r++) key[r] = 0;
+    for (int k = 0; k < p.nkeys; k++) {
+      unsigned long long v[R];
+      src.key(p, k, v);
+#pragma unroll
+      for (int r = 0; r < R; r++) key[r] |= (v[r] & p.key_mask[k]) << p.key_shift[k];
+    }
+    unsigned refused = 0;
+    for (int s = 0; s < p.nargs; s++) {
+      unsigned long long v[R];
+      unsigned av;
+      const unsigned b = src.arg(p, s, v, av);
+      const int hshift = hash_shift(sp.cap[s]);
+      unsigned added = 0;
+#pragma unroll
+      for (int r = 0; r < R; r++) {
+        if (!((src.mask >> r) & 1u) || (NULLS && !((av >> r) & 1u))) continue;
+        if ((b >> r) & 1u) bad = true;
+        const unsigned long long val = distinct_norm(v[r], sp.mt[s]);
+        if (key[r] == EMPTY_KEY && val == EMPTY_KEY) {
+          if (__ldcg(&p.counters[DCTR_SET + 2 * s + 1]) == 0ull) p.counters[DCTR_SET + 2 * s + 1] = 1ull;
+          continue;
+        }
+        const int rc = set_insert(sp.slots[s], sp.cap[s], hshift, key[r], val, ((full >> s) & 1u) != 0);
+        if (rc > 0) added++;
+        else if (rc < 0) refused |= 1u << r;
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) added += __shfl_xor_sync(0xffffffffu, added, o);
+      if (lane == 0 && added) atomicAdd(&p.counters[DCTR_SET + 2 * s], (unsigned long long)added);
+    }
+#pragma unroll
+    for (int r = 0; r < R; r++) {
+      if (!((refused >> r) & 1u)) continue;
+      const unsigned long long at = atomicAdd(&p.counters[DCTR_OVERFLOW], 1ull);
+      p.ovf_rows[at] = src.rowid(r);
+    }
+    bad = bad || src.bad != 0;
+  }
+  if (bad) p.counters[DCTR_ERROR] = 1ull;
+}
+template <int DEPTH, bool NULLS>
+__global__ void __launch_bounds__(AG_THREADS, 3) k_distinct_insert(const __grid_constant__ AggParams p, const __grid_constant__ SetParams sp) {
+  distinct_insert_body<InterpSrc<DEPTH, NULLS>, NULLS>(p, sp);
+}
+template <int NC>
+__global__ void __launch_bounds__(AG_THREADS) k_distinct_insert_plain(const __grid_constant__ AggParams p, const __grid_constant__ SetParams sp) {
+  distinct_insert_body<PlainSrc<NC>, false>(p, sp);
+}
+
+// Re-insertion of a set's pairs into a bigger set (growth).
+struct SetMoveParams {
+  const unsigned long long* from;
+  long long from_cap;
+  unsigned long long* to;
+  long long to_cap;
+  unsigned long long* error;
+};
+__global__ void __launch_bounds__(256) k_set_move(const __grid_constant__ SetMoveParams p) {
+  const int hshift = hash_shift(p.to_cap);
+  for (long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x; s < p.from_cap; s += (long long)gridDim.x * blockDim.x) {
+    const unsigned long long key = p.from[2 * s], val = p.from[2 * s + 1];
+    if (key == EMPTY_KEY && val == EMPTY_KEY) continue;
+    if (set_insert(p.to, p.to_cap, hshift, key, val, false) < 0) *p.error = 2ull;
+  }
+}
+
+// Count a set's pairs into the group table: +1 on the accumulator words `words` of the pair's group.  Index `cap` is the
+// empty-marker pair (flag `marker`), whose group is the sentinel slot.  A pair whose group is missing sets `error`.
+struct DistinctCountParams {
+  const unsigned long long* slots;
+  long long cap;
+  const unsigned long long* marker;
+  TableLayout t;
+  long long tcap;
+  int sentinel_used;
+  int nwords;
+  int words[kMaxAggs];
+  unsigned long long* error;
+};
+__global__ void __launch_bounds__(256) k_distinct_count(const __grid_constant__ DistinctCountParams p) {
+  const unsigned long long hmask = (unsigned long long)p.tcap - 1ull;
+  const int hshift = hash_shift(p.tcap);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i <= p.cap; i += (long long)gridDim.x * blockDim.x) {
+    unsigned long long key = EMPTY_KEY;
+    if (i < p.cap) {
+      key = p.slots[2 * i];
+      if (key == EMPTY_KEY && p.slots[2 * i + 1] == EMPTY_KEY) continue;
+    } else if (*p.marker == 0ull) {
+      continue;
+    }
+    long long slot = p.sentinel_used ? p.tcap : -1;
+    if (key != EMPTY_KEY) {
+      unsigned long long h = home_slot(mix64(key), hshift);
+      slot = -1;
+      for (long long probes = 0; probes < p.tcap; probes++) {  // bounded: a missing key is an error, never a hang
+        const unsigned long long cur = *p.t.key((long long)h);
+        if (cur == key) { slot = (long long)h; break; }
+        if (cur == EMPTY_KEY) break;
+        h = (h + 1ull) & hmask;
+      }
+    }
+    if (slot < 0) { *p.error = 2ull; continue; }
+    for (int w = 0; w < p.nwords; w++) atomicAdd(p.t.val(slot, p.words[w]), 1ull);
+  }
+}
+
 }  // namespace dfgpu
 
 using namespace dfgpu;
@@ -1362,6 +1558,17 @@ struct dfgpu_aggstate {
   bool sentinel_used = false;
   long long rows_seen = 0;
   bool finished = false;
+  // COUNT(DISTINCT): key_progs / arg_progs / funcs / out_dtypes above describe the accumulators the scan kernels
+  // update, table words [0, nscan).  Word nscan + j belongs to the j-th COUNT(DISTINCT), which counts the pairs of set
+  // dist_set[j]; set s holds the (packed key, value) pairs of argument program dist_progs[s].
+  int nscan = 0;
+  std::vector<std::vector<dfgpu_insn>> dist_progs;
+  std::vector<int> dist_set;
+  std::vector<int> out_word;        // user aggregate -> table word
+  std::vector<int> dist_dtypes;     // argument dtype per set, typed at the first batch
+  std::vector<unsigned long long*> set_slots;
+  std::vector<long long> set_cap;
+  unsigned long long* d_dctr = nullptr;  // DCTR_SLOTS words, see DCTR_*
 
   ~dfgpu_aggstate() {
     if (ctx) {
@@ -1369,6 +1576,8 @@ struct dfgpu_aggstate {
       ctx->free(d_counters);
       for (void* p : utf8_owned) ctx->free(p);
       ctx->free(d_utf8_srcs);
+      for (void* p : set_slots) ctx->free(p);
+      ctx->free(d_dctr);
     }
   }
 };
@@ -1687,17 +1896,43 @@ extern "C" int dfgpu_aggregate_create(dfgpu_ctx* ctx, const dfgpu_insn* const* k
     st->naggs = naggs;
     st->expected = expected_groups;
     for (int k = 0; k < nkeys; k++) st->key_progs.emplace_back(keys[k], keys[k] + key_len[k]);
+    std::vector<int> dist_user;  // user aggregates that are COUNT(DISTINCT)
     for (int a = 0; a < naggs; a++) {
-      // compile_expr accepts min/max/count/sum (expression.rs:98-107); anything else is
-      // General("Unsupported aggregate function ...")
-      if (aggs[a].func < DFGPU_AGG_MIN || aggs[a].func > DFGPU_AGG_COUNT)
+      // compile_expr accepts min/max/count/sum (expression.rs:98-107), this engine also COUNT(DISTINCT); anything
+      // else is General("Unsupported aggregate function ...")
+      if (aggs[a].func < DFGPU_AGG_MIN || aggs[a].func > DFGPU_AGG_COUNT_DISTINCT)
         fail(DFGPU_ERR_GENERAL, "Unsupported aggregate function '" + std::to_string(aggs[a].func) + "'");
-      st->arg_progs.emplace_back(aggs[a].arg, aggs[a].arg + aggs[a].arg_len);
+      std::vector<dfgpu_insn> prog(aggs[a].arg, aggs[a].arg + aggs[a].arg_len);
+      if (aggs[a].func == DFGPU_AGG_COUNT_DISTINCT) {
+        if (aggs[a].out_dtype != 0 && aggs[a].out_dtype != DFGPU_UINT64)
+          fail(DFGPU_ERR_EXECUTION, "unexpected type when creating array from aggregate map");
+        // COUNT(DISTINCT) over the same argument program share one set
+        int s = 0;
+        while (s < int(st->dist_progs.size()) && !(st->dist_progs[size_t(s)].size() == prog.size() &&
+                                                   memcmp(st->dist_progs[size_t(s)].data(), prog.data(), prog.size() * sizeof(dfgpu_insn)) == 0))
+          s++;
+        if (s == int(st->dist_progs.size())) st->dist_progs.push_back(prog);
+        st->dist_set.push_back(s);
+        dist_user.push_back(a);
+        st->out_word.push_back(-1);
+        continue;
+      }
+      st->out_word.push_back(int(st->funcs.size()));
+      st->arg_progs.push_back(prog);
       st->funcs.push_back(aggs[a].func);
       st->out_dtypes.push_back(aggs[a].out_dtype);
     }
+    // the pair exchange across ranks is not built: refuse where the communicator is known (and again at finish, for
+    // one attached after create)
+    if (!dist_user.empty() && ctx->world > 1) fail(DFGPU_ERR_NOT_IMPLEMENTED, "COUNT(DISTINCT) with a communicator attached");
+    st->nscan = int(st->funcs.size());
+    for (size_t j = 0; j < dist_user.size(); j++) st->out_word[size_t(dist_user[j])] = st->nscan + int(j);
     st->d_counters = (unsigned long long*)ctx->alloc(CTR_SLOTS * 8);
     DF_CUDA(cudaMemsetAsync(st->d_counters, 0, CTR_SLOTS * 8, ctx->stream));
+    if (!dist_user.empty()) {
+      st->d_dctr = (unsigned long long*)ctx->alloc(DCTR_SLOTS * 8);
+      DF_CUDA(cudaMemsetAsync(st->d_dctr, 0, DCTR_SLOTS * 8, ctx->stream));
+    }
     *out = st.release();
   });
 }
@@ -1862,7 +2097,10 @@ struct BatchPrograms {
   const DevColumn* ukey = nullptr;  // the single Utf8 key column (grouped by hash, then verified)
   const unsigned long long* ukey_hash = nullptr;
   std::vector<const DevColumn*> key_utf8;  // per key part (not the single Utf8 key): its Utf8 column, or null
-  BatchPrograms(const dfgpu_batch* batch, dfgpu_ctx* ctx) : pb(batch), hashes(ctx) {}
+  // COUNT(DISTINCT): the WHERE clause, the keys and the argument of each set, for k_distinct_insert
+  ProgramBuilder dpb;
+  std::vector<int> dist_dtypes;
+  BatchPrograms(const dfgpu_batch* batch, dfgpu_ctx* ctx) : pb(batch), hashes(ctx), dpb(batch) {}
 };
 
 // Compile a batch's programs and type its aggregates.  The single Utf8 key column is retained here, because the
@@ -1881,7 +2119,9 @@ void compile_batch(dfgpu_aggstate* st, const dfgpu_batch* batch, BatchPrograms& 
     pb.add_synthetic_column(h, DFGPU_UINT64);
     return h;
   };
+  const bool distinct = !st->dist_progs.empty();
   bp.ukey = st->nkeys == 1 ? plain_utf8_col(st->key_progs[0], batch) : nullptr;
+  if (bp.ukey && distinct) fail(DFGPU_ERR_NOT_IMPLEMENTED, "COUNT(DISTINCT) with a Utf8 GROUP BY key");
   if (bp.ukey) {
     if (st->typed && !st->utf8_key) fail(DFGPU_ERR_GENERAL, "GROUP BY key types changed between batches");
     if (!st->typed && st->naggs >= kMaxAggs) fail(DFGPU_ERR_NOT_IMPLEMENTED, "Utf8 GROUP BY key with " + std::to_string(kMaxAggs) + " aggregates");
@@ -1893,6 +2133,7 @@ void compile_batch(dfgpu_aggstate* st, const dfgpu_batch* batch, BatchPrograms& 
       const auto& kp = st->key_progs[size_t(k)];
       const DevColumn* uc = plain_utf8_col(kp, batch);
       bp.key_utf8.push_back(uc);
+      if (uc && distinct) fail(DFGPU_ERR_NOT_IMPLEMENTED, "COUNT(DISTINCT) with a Utf8 GROUP BY key part");
       if (uc) {
         hash_key(*uc);
         bp.key_dtypes.push_back(DFGPU_UTF8);
@@ -1904,7 +2145,7 @@ void compile_batch(dfgpu_aggstate* st, const dfgpu_batch* batch, BatchPrograms& 
       bp.key_dtypes.push_back(dt);
     }
   }
-  const int user_aggs = st->utf8_key ? st->naggs - 1 : st->naggs;  // the hidden representative is appended below
+  const int user_aggs = int(st->funcs.size());  // the hidden representative is appended below
   bp.agg_arg.assign(size_t(user_aggs), 0);
   for (int a = 0; a < user_aggs; a++) {
     // identical argument expressions are compiled (and evaluated) once
@@ -1935,6 +2176,18 @@ void compile_batch(dfgpu_aggstate* st, const dfgpu_batch* batch, BatchPrograms& 
     d.out_dtype = uint8_t(odt);
     bp.descs.push_back(d);
   }
+  if (distinct) {
+    // the words COUNT(DISTINCT) counts into at finish: a COUNT for growth, exchange and compaction
+    for (size_t j = 0; j < st->dist_set.size(); j++) bp.descs.push_back(AggDesc{DFGPU_AGG_COUNT, MT_U, DFGPU_UINT64, DFGPU_UINT64});
+    if (bp.has_pred) bp.dpb.add(st->pred_prog.data(), int(st->pred_prog.size()), "filter expression");
+    for (int k = 0; k < st->nkeys; k++) bp.dpb.add(st->key_progs[size_t(k)].data(), int(st->key_progs[size_t(k)].size()), "GROUP BY expression");
+    for (const auto& prog : st->dist_progs) {
+      const int dt = bp.dpb.out_dtype(bp.dpb.add(prog.data(), int(prog.size()), "aggregate argument"));
+      if (dt == DFGPU_UTF8) fail(DFGPU_ERR_NOT_IMPLEMENTED, "COUNT(DISTINCT) of a Utf8 argument");
+      if (!is_numeric(dt)) fail(DFGPU_ERR_EXECUTION, std::string("Unsupported data type for aggregate: ") + dtype_name(dt));
+      bp.dist_dtypes.push_back(dt);
+    }
+  }
   if (bp.ukey) {
     // hidden accumulator: MIN(source << 40 | row)
     pb.add_rowid_plus((unsigned long long)st->utf8_srcs.size() << UTF8_SRC_SHIFT);
@@ -1949,21 +2202,249 @@ void compile_batch(dfgpu_aggstate* st, const dfgpu_batch* batch, BatchPrograms& 
   }
 }
 
+// Whether programs [has_pred] + nkeys keys + nargs arguments of `pb` fit the interpreter-free PlainSrc: every key and argument
+// a plain 4/8-byte column and the WHERE clause, if any, a chain of column comparisons.  If so, *out describes them.
+bool plain_spec(const ProgramBuilder& pb, const ProgramSet& ps, int has_pred, int nkeys, int nargs, PlainSpec* out) {
+  PlainSpec sp;
+  memset(&sp, 0, sizeof(sp));
+  auto wide = [](int dt) {
+    return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64 || dt == DFGPU_FLOAT32 || dt == DFGPU_INT32 || dt == DFGPU_UINT32;
+  };
+  bool ok = !ps.has_nulls && ps.ncols <= 4;
+  for (int c = 0; ok && c < ps.ncols; c++)
+    ok = wide(ps.cols[c].dtype) && (reinterpret_cast<uintptr_t>(ps.cols[c].ptr) & 15) == 0;
+  for (int k = 0; ok && k < nkeys; k++) {
+    const CompiledProgram& cpk = pb.prog(has_pred + k);
+    ok = cpk.is_plain_column;
+    sp.key_slot[k] = cpk.plain_slot;
+  }
+  for (int g = 0; ok && g < nargs; g++) {
+    const CompiledProgram& cpa = pb.prog(has_pred + nkeys + g);
+    ok = cpa.is_plain_column;
+    sp.arg_slot[g] = cpa.plain_slot;
+  }
+  if (ok && has_pred) {
+    // t0 [t1 AND|OR [t2 AND|OR ...]] in lowered form: (PUSH_COL, CMP leaf) {(PUSH_COL, CMP leaf), AND|OR stack}*
+    const int b = ps.start[0], e = ps.start[1];
+    const DevInsn* in = &ps.insn[b];
+    auto term_at = [&](int i, PlainTerm* out) {
+      if (i + 1 >= e - b) return false;
+      const DevInsn &c = in[i], &o = in[i + 1];
+      if (c.op != V_PUSH_COL) return false;
+      if (o.op < V_EQ || o.op > V_GE || o.mode == RHS_STACK) return false;
+      if (o.mode == RHS_COL && ps.cols[o.slot].dtype != ps.cols[c.slot].dtype) return false;
+      memset(out, 0, sizeof(*out));
+      out->kind = o.mode == RHS_COL ? 2 : 3;
+      out->op = o.op;
+      out->a = c.slot;
+      out->b = o.mode == RHS_COL ? o.slot : 0;
+      out->mt = mtype_of(ps.cols[c.slot].dtype);
+      out->imm = o.imm;
+      return true;
+    };
+    ok = term_at(0, &sp.term[0]);
+    sp.nterms = ok ? 1 : 0;
+    int i = 2;
+    while (ok && i < e - b) {
+      if (sp.nterms >= 4 || !term_at(i, &sp.term[sp.nterms]) || i + 2 >= e - b) { ok = false; break; }
+      const DevInsn& j = in[i + 2];
+      if ((j.op != V_AND && j.op != V_OR) || j.mode != RHS_STACK) { ok = false; break; }
+      sp.term[sp.nterms].conn = j.op == V_OR ? 1 : 0;
+      sp.nterms++;
+      i += 3;
+    }
+  }
+  sp.ncols = ps.ncols;
+  if (ok) *out = sp;
+  return ok;
+}
+
+unsigned long long* set_alloc(dfgpu_ctx* ctx, long long cap);
+
 // The first batch types the operator: key packing, table form and capacity.  Later batches must bring the same types.
 void type_batch(dfgpu_aggstate* st, const BatchPrograms& bp) {
   if (st->typed) {
     if (bp.key_dtypes != st->key_dtypes) fail(DFGPU_ERR_GENERAL, "GROUP BY key types changed between batches");
     for (int a = 0; a < st->naggs; a++)
       if (bp.descs[size_t(a)].dtype != st->descs[size_t(a)].dtype) fail(DFGPU_ERR_GENERAL, "aggregate argument types changed between batches");
+    if (bp.dist_dtypes != st->dist_dtypes) fail(DFGPU_ERR_GENERAL, "aggregate argument types changed between batches");
     return;
   }
   st->key_dtypes = bp.key_dtypes;
   st->descs = bp.descs;
   st->wide = pack_keys(st);
+  if (st->wide && !st->dist_progs.empty()) fail(DFGPU_ERR_NOT_IMPLEMENTED, "COUNT(DISTINCT) with GROUP BY keys wider than 64 bits");
+  st->dist_dtypes = bp.dist_dtypes;
   st->typed = true;
   st->cap = st->nkeys == 0 ? 0 : std::max(AG_MIN_CAP, next_pow2(2 * st->expected));
   st->aos = st->wide || (st->nkeys > 0 && want_aos(st->expected, st->descs, st->naggs));
   st->t = table_alloc(st->ctx, st->naggs, st->nkeys, st->descs, st->cap, st->aos, st->wide ? st->nkeys : 0);
+  for (size_t s = 0; s < st->dist_progs.size(); s++) {
+    st->set_cap.push_back(std::max(AG_SET_MIN_CAP, next_pow2(2 * st->expected)));
+    st->set_slots.push_back(set_alloc(st->ctx, st->set_cap.back()));
+  }
+}
+
+// ---- COUNT(DISTINCT) ----------------------------------------------------------------------------------------
+unsigned long long* set_alloc(dfgpu_ctx* ctx, long long cap) {
+  unsigned long long* q = (unsigned long long*)ctx->alloc(size_t(cap) * 16);
+  DF_CUDA(cudaMemsetAsync(q, 0xff, size_t(cap) * 16, ctx->stream));  // every word EMPTY_KEY
+  return q;
+}
+
+// DCTR_* slots -> host (synchronises the stream)
+void read_dctr(dfgpu_aggstate* st, unsigned long long* host) {
+  dfgpu_ctx* ctx = st->ctx;
+  DF_CUDA(cudaMemcpyAsync(host, st->d_dctr, DCTR_SLOTS * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  DF_CUDA(cudaStreamSynchronize(ctx->stream));
+}
+
+// Grow set s to new_cap by re-inserting its pairs (their number does not change).
+void set_grow(dfgpu_aggstate* st, int s, long long new_cap) {
+  dfgpu_ctx* ctx = st->ctx;
+  SetMoveParams mp;
+  mp.from = st->set_slots[size_t(s)];
+  mp.from_cap = st->set_cap[size_t(s)];
+  mp.to = set_alloc(ctx, new_cap);
+  mp.to_cap = new_cap;
+  mp.error = st->d_dctr + DCTR_ERROR;
+  launch_kernel(ctx, k_set_move, "k_set_move", mp, mp.from_cap, 256 * 4, 8);
+  unsigned long long c[DCTR_SLOTS];
+  read_dctr(st, c);
+  if (c[DCTR_ERROR] == 2) fail(DFGPU_ERR_INTERNAL, "COUNT(DISTINCT) set growth could not place a pair");
+  ctx->free(st->set_slots[size_t(s)]);
+  st->set_slots[size_t(s)] = mp.to;
+  st->set_cap[size_t(s)] = new_cap;
+}
+
+// Insert the pairs of rows [begin, begin + count) of the batch into every set: after the group scan of the same rows.
+// Rows that a full set refused are replayed after the sets that reached their fill limit grew x4, like
+// group_by_update's loop.  `prefix_of` > 0: these rows are the prefix sample of a first batch of that many rows, and
+// each set is then sized for the number of pairs estimated from it.
+void distinct_update(dfgpu_aggstate* st, const BatchPrograms& bp, const AggParams& scan, long long begin, long long count, long long prefix_of) {
+  dfgpu_ctx* ctx = st->ctx;
+  const int nsets = int(st->dist_progs.size());
+  AggParams p;
+  memset(&p, 0, sizeof(p));
+  bp.dpb.finish(&p.ps);
+  if (p.ps.max_depth > 8) fail(DFGPU_ERR_NOT_IMPLEMENTED, "expression too deep (register stack depth > 8)");
+  p.has_pred = bp.has_pred;
+  p.nkeys = st->nkeys;
+  p.nargs = nsets;
+  for (int k = 0; k < st->nkeys; k++) {
+    p.key_mask[k] = scan.key_mask[k];
+    p.key_shift[k] = scan.key_shift[k];
+  }
+  p.counters = st->d_dctr;
+  const bool plain = plain_spec(bp.dpb, p.ps, bp.has_pred, st->nkeys, nsets, &p.plain);
+  DevBufs lists(ctx);
+  unsigned* ovf[2] = {lists.alloc<unsigned>(size_t(count) * 4), nullptr};
+  int cur = 0;
+  const unsigned* list = nullptr;
+  long long nlist = 0;
+  for (int round = 0;; round++) {
+    if (round > 60) fail(DFGPU_ERR_INTERNAL, "COUNT(DISTINCT) set growth did not converge");
+    p.row_begin = begin;
+    p.nrows = count;
+    p.row_list = list;
+    p.nlist = nlist;
+    p.ovf_rows = ovf[cur];
+    DF_CUDA(cudaMemsetAsync(st->d_dctr + DCTR_OVERFLOW, 0, 8, ctx->stream));
+    void (*fn)(AggParams, SetParams);
+    const char* name;
+    const int d = p.ps.max_depth;
+    if (p.ps.has_nulls) fn = k_distinct_insert<8, true>, name = "k_distinct_insert<8, true>";
+    else if (plain && !list && (begin & 1) == 0 && p.plain.ncols <= 2) fn = k_distinct_insert_plain<2>, name = "k_distinct_insert_plain<2>";
+    else if (plain && !list && (begin & 1) == 0) fn = k_distinct_insert_plain<4>, name = "k_distinct_insert_plain<4>";
+    else if (d <= 2) fn = k_distinct_insert<2, false>, name = "k_distinct_insert<2, false>";
+    else fn = k_distinct_insert<8, false>, name = "k_distinct_insert<8, false>";
+    int per_sm = 0;
+    DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, AG_THREADS, 0));
+    const int grid = grid_for(ctx, list ? nlist : count, AG_TILE, std::max(per_sm, 1));
+    // A warp reads the fill once per tile and adds its tile's pairs after it, so up to one tile per warp of the grid
+    // (grid x AG_TILE pairs per set) is inserted past what the others read: the fill limit is lowered by that much,
+    // which keeps every set at most half full.
+    SetParams sp;
+    memset(&sp, 0, sizeof(sp));
+    for (int s = 0; s < nsets; s++) {
+      sp.slots[s] = st->set_slots[size_t(s)];
+      sp.cap[s] = st->set_cap[size_t(s)];
+      sp.max_fill[s] = std::max<long long>(0, sp.cap[s] / 2 - (long long)grid * AG_TILE);
+      sp.mt[s] = mtype_of(st->dist_dtypes[size_t(s)]);
+    }
+    const int ps = ctx->prof_begin();
+    fn<<<grid, AG_THREADS, 0, ctx->stream>>>(p, sp);
+    DF_CUDA(cudaGetLastError());
+    trace_launch(name);
+    ctx->prof_end(ps);
+    ctx->launches++;
+    unsigned long long c[DCTR_SLOTS];
+    read_dctr(st, c);
+    if (c[DCTR_ERROR]) fail(DFGPU_ERR_ARROW, "DivideByZero");
+    const long long novf = (long long)c[DCTR_OVERFLOW];
+    bool grew = false;
+    for (int s = 0; s < nsets; s++) {
+      const long long n = (long long)c[DCTR_SET + 2 * s];
+      const bool refused = novf > 0 && n >= sp.max_fill[s];  // at the fill limit: this set refused new pairs
+      if (!refused && n <= sp.cap[s] / 2) continue;
+      set_grow(st, s, sp.cap[s] * 4);
+      grew = true;
+    }
+    if (novf == 0) break;
+    if (!grew)  // refused at the probe limit below the fill limit: grow every set
+      for (int s = 0; s < nsets; s++) set_grow(st, s, sp.cap[s] * 4);
+    list = ovf[cur];
+    nlist = novf;
+    cur ^= 1;
+    if (!ovf[cur]) ovf[cur] = lists.alloc<unsigned>(size_t(count) * 4);
+  }
+  if (prefix_of > 0) {
+    unsigned long long c[DCTR_SLOTS];
+    read_dctr(st, c);
+    const long long afford = (long long)(ctx->device_mem_bytes / 8) / 16;  // slots that fit in 1/8 of device memory
+    for (int s = 0; s < nsets; s++) {
+      const long long n = (long long)c[DCTR_SET + 2 * s];
+      long long want = std::max(AG_SET_MIN_CAP, next_pow2(2 * std::max(estimate_groups(n, count, prefix_of), n)));
+      while (want > st->set_cap[size_t(s)] && want > afford) want >>= 1;
+      if (want > st->set_cap[size_t(s)]) set_grow(st, s, want);
+    }
+  }
+}
+
+// GROUP BY at finish: add each set's pairs to the COUNT(DISTINCT) words of their groups.
+void distinct_count(dfgpu_aggstate* st, const TableLayout& t, long long cap, int sentinel_used) {
+  dfgpu_ctx* ctx = st->ctx;
+  DF_CUDA(cudaMemsetAsync(st->d_dctr + DCTR_ERROR, 0, 8, ctx->stream));
+  for (size_t s = 0; s < st->dist_progs.size(); s++) {
+    DistinctCountParams cp;
+    memset(&cp, 0, sizeof(cp));
+    cp.slots = st->set_slots[s];
+    cp.cap = st->set_cap[s];
+    cp.marker = st->d_dctr + DCTR_SET + 2 * s + 1;
+    cp.t = t;
+    cp.tcap = cap;
+    cp.sentinel_used = sentinel_used;
+    for (size_t j = 0; j < st->dist_set.size(); j++)
+      if (st->dist_set[j] == int(s)) cp.words[cp.nwords++] = st->nscan + int(j);
+    cp.error = st->d_dctr + DCTR_ERROR;
+    launch_kernel(ctx, k_distinct_count, "k_distinct_count", cp, cp.cap + 1, 256 * 4, 8);
+  }
+  unsigned long long c[DCTR_SLOTS];
+  read_dctr(st, c);
+  if (c[DCTR_ERROR]) fail(DFGPU_ERR_INTERNAL, "COUNT(DISTINCT) found a pair whose group is not in the table");
+}
+
+// No GROUP BY at finish: each COUNT(DISTINCT) is the number of pairs in its set.
+void distinct_count_scalar(dfgpu_aggstate* st) {
+  dfgpu_ctx* ctx = st->ctx;
+  unsigned long long c[DCTR_SLOTS], n[kMaxAggs];
+  read_dctr(st, c);
+  for (size_t j = 0; j < st->dist_set.size(); j++) {
+    const int s = st->dist_set[j];
+    n[j] = c[DCTR_SET + 2 * s] + (c[DCTR_SET + 2 * s + 1] ? 1ull : 0ull);
+    DF_CUDA(cudaMemcpyAsync(st->t.val(0, st->nscan + int(j)), &n[j], 8, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  DF_CUDA(cudaStreamSynchronize(ctx->stream));  // `n` is a stack array
 }
 
 // No GROUP BY: one reduce over the batch.
@@ -1971,6 +2452,7 @@ void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
   dfgpu_ctx* ctx = st->ctx;
   p.t = st->t;
   p.cap = 0;
+  if (p.naggs == 0) return;  // COUNT(DISTINCT) alone: nothing for the reduce kernels to do
   if (bp.has_pred) DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_PASSED, 0, 8, ctx->stream));
   const int d = p.ps.max_depth;
   if (p.ps.has_nulls) {
@@ -1992,8 +2474,8 @@ void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
     if (plain) {
       rp.ncols = bp.nargs;
       rp.nrows = p.nrows;
-      rp.naggs = st->naggs;
-      for (int a = 0; a < st->naggs; a++) { rp.aggs[a] = p.aggs[a]; rp.agg_arg[a] = p.agg_arg[a]; }
+      rp.naggs = p.naggs;
+      for (int a = 0; a < p.naggs; a++) { rp.aggs[a] = p.aggs[a]; rp.agg_arg[a] = p.agg_arg[a]; }
       rp.t = st->t;
       const int ps = ctx->prof_begin();
       launch_kernel(ctx, k_reduce_f64, "k_reduce_f64", rp, p.nrows, 256 * 8, 8);
@@ -2020,65 +2502,14 @@ struct ScanPlan {
 ScanPlan plan_scan(const dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
   ScanPlan plan;
   static const bool plain_off = getenv("DFGPU_AGG_PLAIN") && atoi(getenv("DFGPU_AGG_PLAIN")) == 0;  // A/B switch
-  PlainSpec sp;
-  memset(&sp, 0, sizeof(sp));
-  auto wide = [](int dt) {
-    return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64 || dt == DFGPU_FLOAT32 || dt == DFGPU_INT32 || dt == DFGPU_UINT32;
-  };
-  bool ok = !plain_off && !p.ps.has_nulls && p.ps.ncols <= 4;
-  for (int c = 0; ok && c < p.ps.ncols; c++)
-    ok = wide(p.ps.cols[c].dtype) && (reinterpret_cast<uintptr_t>(p.ps.cols[c].ptr) & 15) == 0;
-  for (int k = 0; ok && k < st->nkeys; k++) {
-    const CompiledProgram& cpk = bp.pb.prog(bp.has_pred + k);
-    ok = cpk.is_plain_column;
-    sp.key_slot[k] = cpk.plain_slot;
-  }
-  for (int g = 0; ok && g < bp.nargs; g++) {
-    const CompiledProgram& cpa = bp.pb.prog(bp.has_pred + st->nkeys + g);
-    ok = cpa.is_plain_column;
-    sp.arg_slot[g] = cpa.plain_slot;
-  }
-  if (ok && bp.has_pred) {
-    // t0 [t1 AND|OR [t2 AND|OR ...]] in lowered form: (PUSH_COL, CMP leaf) {(PUSH_COL, CMP leaf), AND|OR stack}*
-    const int b = p.ps.start[0], e = p.ps.start[1];
-    const DevInsn* in = &p.ps.insn[b];
-    auto term_at = [&](int i, PlainTerm* out) {
-      if (i + 1 >= e - b) return false;
-      const DevInsn &c = in[i], &o = in[i + 1];
-      if (c.op != V_PUSH_COL) return false;
-      if (o.op < V_EQ || o.op > V_GE || o.mode == RHS_STACK) return false;
-      if (o.mode == RHS_COL && p.ps.cols[o.slot].dtype != p.ps.cols[c.slot].dtype) return false;
-      memset(out, 0, sizeof(*out));
-      out->kind = o.mode == RHS_COL ? 2 : 3;
-      out->op = o.op;
-      out->a = c.slot;
-      out->b = o.mode == RHS_COL ? o.slot : 0;
-      out->mt = mtype_of(p.ps.cols[c.slot].dtype);
-      out->imm = o.imm;
-      return true;
-    };
-    ok = term_at(0, &sp.term[0]);
-    sp.nterms = ok ? 1 : 0;
-    int i = 2;
-    while (ok && i < e - b) {
-      if (sp.nterms >= 4 || !term_at(i, &sp.term[sp.nterms]) || i + 2 >= e - b) { ok = false; break; }
-      const DevInsn& j = in[i + 2];
-      if ((j.op != V_AND && j.op != V_OR) || j.mode != RHS_STACK) { ok = false; break; }
-      sp.term[sp.nterms].conn = j.op == V_OR ? 1 : 0;
-      sp.nterms++;
-      i += 3;
-    }
-  }
-  sp.ncols = p.ps.ncols;
-  if (ok) p.plain = sp;
-  plan.plain = ok;
+  plan.plain = !plain_off && plain_spec(bp.pb, p.ps, bp.has_pred, st->nkeys, bp.nargs, &p.plain);
   // lean kernel: one 8-byte integer key column, one 8-byte argument column, distinct MIN/MAX/SUM/COUNT, no WHERE
   static const bool lean_off = getenv("DFGPU_AGG_LEAN") && atoi(getenv("DFGPU_AGG_LEAN")) == 0;  // A/B switch
   auto w8 = [](int dt) { return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64; };
-  ok = !lean_off && plan.plain && !bp.has_pred && st->nkeys == 1 && bp.nargs == 1 && w8(p.ps.cols[p.plain.key_slot[0]].dtype) &&
+  bool ok = !lean_off && plan.plain && !bp.has_pred && st->nkeys == 1 && bp.nargs == 1 && w8(p.ps.cols[p.plain.key_slot[0]].dtype) &&
        w8(p.ps.cols[p.plain.arg_slot[0]].dtype);
   int mask = 0;
-  for (int a = 0; ok && a < st->naggs; a++) {
+  for (int a = 0; ok && a < p.naggs; a++) {
     const int bit = 1 << (st->descs[size_t(a)].func - 1);  // MIN 1, MAX 2, SUM 4, COUNT 8
     ok = !(mask & bit);
     mask |= bit;
@@ -2106,7 +2537,7 @@ ScanKernel choose_scan(const dfgpu_aggstate* st, AggParams& p, const ScanPlan& p
     p.lean.arg_col = (const unsigned long long*)p.ps.cols[p.plain.arg_slot[0]].ptr;
     p.lean.min_w = p.lean.max_w = 0;
     p.lean.sum_arr = p.lean.cnt_arr = nullptr;
-    for (int a = 0; a < st->naggs; a++) {
+    for (int a = 0; a < p.naggs; a++) {
       const int f = st->descs[size_t(a)].func, l = st->t.loc[a];
       if (f == DFGPU_AGG_MIN) p.lean.min_w = l;
       else if (f == DFGPU_AGG_MAX) p.lean.max_w = l;
@@ -2114,7 +2545,7 @@ ScanKernel choose_scan(const dfgpu_aggstate* st, AggParams& p, const ScanPlan& p
       else p.lean.cnt_arr = st->t.add + (long long)(~l) * st->t.astride;
     }
     bool layout_ok = st->t.lw == (((plan.lean_mask & 3) == 3) ? 4 : ((plan.lean_mask & 3) ? 2 : 1));
-    for (int a = 0; a < st->naggs; a++) {
+    for (int a = 0; a < p.naggs; a++) {
       const int f = st->descs[size_t(a)].func;
       layout_ok = layout_ok && ((f == DFGPU_AGG_MIN || f == DFGPU_AGG_MAX) ? st->t.loc[a] >= 1 : st->t.loc[a] < 0);
     }
@@ -2187,7 +2618,7 @@ void group_by_update(dfgpu_aggstate* st, const dfgpu_batch* batch, const BatchPr
   // First big batch with no cardinality hint: a 1 Mi-row prefix is aggregated first; the number of groups it
   // produces decides the table layout (SoA while the hot sectors fit L2, AoS beyond) before the bulk of the batch
   // is touched.  Wide tables are AoS from the start.
-  const long long kPrefix = 1ll << 20;
+  const long long kPrefix = AG_PREFIX_ROWS;
   const bool sample = st->rows_seen == batch->nrows && st->expected == 0 && !st->aos && batch->nrows >= 4 * kPrefix;
   std::vector<std::pair<long long, long long>> ranges;  // (begin, count)
   if (sample) {
@@ -2238,6 +2669,7 @@ void group_by_update(dfgpu_aggstate* st, const dfgpu_batch* batch, const BatchPr
       cur ^= 1;
       if (!ovf[cur]) ovf[cur] = lists.alloc<unsigned>(size_t(batch->nrows) * 4);
     }
+    if (!st->dist_progs.empty()) distinct_update(st, bp, p, ranges[ri].first, ranges[ri].second, sample && ri == 0 ? batch->nrows : 0);
     // few groups so far: later rows of this stream go through the shared-memory front table
     st->use_front = st->ngroups <= AG_FRONT_MAX_GROUPS && st->rows_seen >= (1ll << 20);
     if (sample && ri == 0) {
@@ -2279,8 +2711,8 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
   if (batch->nrows == 0) return;
 
   p.nkeys = st->nkeys;
-  p.naggs = st->naggs;
-  for (int a = 0; a < st->naggs; a++) {
+  p.naggs = st->naggs - int(st->dist_set.size());  // the scan kernels never see the COUNT(DISTINCT) words
+  for (int a = 0; a < p.naggs; a++) {
     p.aggs[a] = st->descs[size_t(a)];
     p.agg_arg[a] = bp.agg_arg[size_t(a)];
   }
@@ -2292,8 +2724,18 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
   p.nrows = batch->nrows;
   p.counters = st->d_counters;
   p.has_pred = bp.has_pred;
-  if (st->nkeys == 0) reduce_update(st, bp, p);
-  else group_by_update(st, batch, bp, p, tr);
+  if (st->nkeys > 0) {
+    group_by_update(st, batch, bp, p, tr);
+    return;
+  }
+  reduce_update(st, bp, p);
+  if (st->dist_progs.empty()) return;
+  if (st->rows_seen == batch->nrows && st->expected == 0 && batch->nrows >= 4 * AG_PREFIX_ROWS) {  // size the sets from a prefix
+    distinct_update(st, bp, p, 0, AG_PREFIX_ROWS, batch->nrows);
+    distinct_update(st, bp, p, AG_PREFIX_ROWS, batch->nrows - AG_PREFIX_ROWS, 0);
+  } else {
+    distinct_update(st, bp, p, 0, batch->nrows, 0);
+  }
 }
 }  // namespace
 
@@ -2703,13 +3145,14 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
     dfgpu_ctx* ctx = st->ctx;
     ctx->use();
     Trace tr(ctx);
+    if (ctx->world > 1 && !st->dist_progs.empty()) fail(DFGPU_ERR_NOT_IMPLEMENTED, "COUNT(DISTINCT) with a communicator attached");
     if (!st->typed && !(st->nkeys > 0 && ctx->world > 1)) {
       // no batch was ever seen: resolve types from the declared output types
       if (st->nkeys > 0) {
         // an empty GROUP BY input yields an empty batch; key types are unknown -> need a batch
         fail(DFGPU_ERR_GENERAL, "aggregate finished before any input batch was provided");
       }
-      for (int a = 0; a < st->naggs; a++) {
+      for (int a = 0; a < st->nscan; a++) {
         AggDesc d;
         int odt = st->out_dtypes[size_t(a)];
         if (!is_numeric(odt)) fail(DFGPU_ERR_GENERAL, "aggregate output type must be given when there is no input");
@@ -2719,6 +3162,7 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
         d.out_dtype = uint8_t(odt);
         st->descs.push_back(d);
       }
+      for (size_t j = 0; j < st->dist_set.size(); j++) st->descs.push_back(AggDesc{DFGPU_AGG_COUNT, MT_U, DFGPU_UINT64, DFGPU_UINT64});
       st->typed = true;
       st->cap = 0;
       st->t = table_alloc(ctx, st->naggs, st->nkeys, st->descs, 0, false);
@@ -2737,6 +3181,10 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
         st->finished = true;
         return;
       }
+    }
+    if (!st->dist_progs.empty()) {  // the COUNT(DISTINCT) words (single GPU: the exchange is refused above)
+      if (st->nkeys == 0) distinct_count_scalar(st);
+      else distinct_count(st, st->t, st->cap, st->sentinel_used ? 1 : 0);
     }
     auto res = std::make_unique<dfgpu_result>();
     res->ctx = ctx;
@@ -2848,6 +3296,9 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
       }
       DF_CUDA(cudaStreamSynchronize(ctx->stream));
     }
+    // aggregate columns in the caller's order: the COUNT(DISTINCT) words follow the scan's accumulators in the table
+    const std::vector<DevColumn> words(res->cols.begin() + st->nkeys, res->cols.end());
+    for (size_t i = 0; i < st->out_word.size(); i++) res->cols[size_t(st->nkeys) + i] = words[size_t(st->out_word[i])];
     tr.mark("finish (compact + outputs)");
     st->finished = true;
     *out = res.release();

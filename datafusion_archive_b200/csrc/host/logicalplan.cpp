@@ -140,8 +140,8 @@ ExprRef Expr::binary(ExprRef l, Operator op, ExprRef r) {
   auto e = std::make_shared<Expr>(); e->kind = BinaryExpr; e->left = std::move(l); e->op = op; e->right = std::move(r); return e;
 }
 ExprRef Expr::cast(ExprRef x, DataType dt) { auto e = std::make_shared<Expr>(); e->kind = Cast; e->left = std::move(x); e->data_type = dt; return e; }
-ExprRef Expr::aggregate(const std::string& name, std::vector<ExprRef> args, DataType rt) {
-  auto e = std::make_shared<Expr>(); e->kind = AggregateFunction; e->name = name; e->args = std::move(args); e->data_type = rt; return e;
+ExprRef Expr::aggregate(const std::string& name, std::vector<ExprRef> args, DataType rt, bool distinct) {
+  auto e = std::make_shared<Expr>(); e->kind = AggregateFunction; e->name = name; e->args = std::move(args); e->data_type = rt; e->distinct = distinct; return e;
 }
 ExprRef Expr::scalar_fn(const std::string& name, std::vector<ExprRef> args, DataType rt) {
   auto e = std::make_shared<Expr>(); e->kind = ScalarFunction; e->name = name; e->args = std::move(args); e->data_type = rt; return e;
@@ -194,7 +194,7 @@ std::string Expr::debug() const {
     case BinaryExpr: return left->debug() + " " + operator_debug(op) + " " + right->debug();
     case Sort: return left->debug() + (asc ? " ASC" : " DESC");
     case ScalarFunction: case AggregateFunction: {
-      std::string s = name + "(";
+      std::string s = name + (distinct ? "(DISTINCT " : "(");
       for (size_t i = 0; i < args.size(); i++) {
         if (i) s += ", ";
         s += args[i]->debug();

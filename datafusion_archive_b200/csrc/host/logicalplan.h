@@ -67,12 +67,13 @@ struct Expr {
   bool asc = true;          // Sort
   std::string name;         // functions
   std::vector<ExprRef> args;
+  bool distinct = false;    // AggregateFunction: COUNT(DISTINCT ..)
 
   static ExprRef column(size_t i);
   static ExprRef literal(const ScalarValue& v);
   static ExprRef binary(ExprRef l, Operator op, ExprRef r);
   static ExprRef cast(ExprRef e, DataType dt);
-  static ExprRef aggregate(const std::string& name, std::vector<ExprRef> args, DataType rt);
+  static ExprRef aggregate(const std::string& name, std::vector<ExprRef> args, DataType rt, bool distinct = false);
   static ExprRef scalar_fn(const std::string& name, std::vector<ExprRef> args, DataType rt);
   static ExprRef sort(ExprRef e, bool asc);
   static ExprRef is_null(ExprRef e, bool negated);

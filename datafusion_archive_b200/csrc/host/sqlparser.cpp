@@ -179,6 +179,13 @@ struct Parser {
         if (accept_sym("(")) {  // function call
           n->kind = ASTNode::SQLFunction;
           n->id = t.text;
+          // COUNT(DISTINCT expr); a column named "distinct" still reads as COUNT(distinct)
+          if (is_kw("DISTINCT") && !(toks[pos + 1].kind == Token::Sym && toks[pos + 1].text == ")")) {
+            pos++;
+            if (upper(t.text) != "COUNT") perr("DISTINCT is only supported in COUNT(DISTINCT expr), not in " + t.text + "()");
+            if (peek().kind == Token::Sym && peek().text == "*") perr("COUNT(DISTINCT *) is not supported");
+            n->distinct = true;
+          }
           if (!accept_sym(")")) {
             do { n->args.push_back(parse_expr()); } while (accept_sym(","));
             expect_sym(")");

@@ -25,6 +25,7 @@ struct ASTNode {
   SQLOperator op = SQLOperator::Eq;
   SQLType sql_type = SQLType::Other;
   std::vector<ASTRef> args;
+  bool distinct = false;  // SQLFunction: COUNT(DISTINCT expr)
   // SQLSelect
   std::vector<ASTRef> projection;
   ASTRef relation, selection, having, limit;

@@ -196,6 +196,12 @@ ExprRef SqlToRel::sql_to_rex(const ASTRef& sql, const Schema& schema) const {
         // return type is same as the argument type for these aggregate functions
         return Expr::aggregate(sql->id, rex_args, rex_args[0]->get_type(schema));
       }
+      if (lid == "count" && sql->distinct) {
+        std::vector<ExprRef> rex_args;
+        for (auto& a : sql->args) rex_args.push_back(sql_to_rex(a, schema));
+        if (rex_args.size() != 1) fail(DFGPU_ERR_GENERAL, "COUNT(DISTINCT) takes exactly one argument");
+        return Expr::aggregate(sql->id, rex_args, DFGPU_UINT64, true);
+      }
       if (lid == "count") {
         std::vector<ExprRef> rex_args;
         for (auto& a : sql->args) {

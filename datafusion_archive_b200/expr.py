@@ -133,14 +133,17 @@ class AggregateFunction:
 
     _F = {"min": A.AGG_MIN, "max": A.AGG_MAX, "sum": A.AGG_SUM, "count": A.AGG_COUNT}
 
-    def __init__(self, name, arg, return_type=None):
-        self.name, self.arg, self.return_type = name, _wrap(arg), return_type
+    def __init__(self, name, arg, return_type=None, distinct=False):
+        """distinct=True: COUNT(DISTINCT arg), the number of distinct non-null values (count only)."""
+        if distinct and name.lower() != "count":
+            raise ValueError("DISTINCT is only supported in COUNT(DISTINCT expr)")
+        self.name, self.arg, self.return_type, self.distinct = name, _wrap(arg), return_type, distinct
 
     def lower(self, schema):
-        func = self._F[self.name.lower()]
+        func = A.AGG_COUNT_DISTINCT if self.distinct else self._F[self.name.lower()]
         rt = self.return_type
         if rt is None:
-            rt = A.UINT64 if func == A.AGG_COUNT else self.arg.get_type(schema)
+            rt = A.UINT64 if func in (A.AGG_COUNT, A.AGG_COUNT_DISTINCT) else self.arg.get_type(schema)
         return (func, self.arg.program(schema), rt)
 
 

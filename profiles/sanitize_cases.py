@@ -119,5 +119,15 @@ r = ctx.aggregate_host([kh, a], [col(0)], [AggregateFunction("sum", col(1))], ch
 assert r.nrows == 1000
 r.free()
 print("host pipelines ok", flush=True)
+
+# 7. COUNT(DISTINCT): 128-bit CAS pair sets, their growth with overflow replay, and the count at finish
+kd = rng.integers(-1, 300, 1_500_000).astype(np.int64)
+vd = rng.integers(-1, 5000, 1_500_000).astype(np.int64)
+got = agg([kd, vd], [col(0)], [AggregateFunction("count", col(1), distinct=True)], nb=2)
+pairs = np.unique(np.stack([kd, vd], 1), axis=0)
+assert int(got[1].sum()) == len(pairs) and len(got[0]) == len(np.unique(kd))
+got = agg([vd], [], [AggregateFunction("count", col(0), distinct=True)])
+assert int(got[0][0]) == len(np.unique(vd))
+print("count distinct ok", flush=True)
 ctx.close()
 print("SANITIZE_CASES_OK")

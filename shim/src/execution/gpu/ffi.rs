@@ -47,6 +47,9 @@ pub const AGG_MIN: i32 = 1;
 pub const AGG_MAX: i32 = 2;
 pub const AGG_SUM: i32 = 3;
 pub const AGG_COUNT: i32 = 4;
+/// AggregateType::CountDistinct; the reference's parser (sqlparser 0.2.1) cannot express it, so the shim only
+/// carries the constant.
+pub const AGG_COUNT_DISTINCT: i32 = 5;
 
 /// Borrowed view of one Arrow array (dfgpu_col).
 #[repr(C)]
