@@ -62,22 +62,12 @@ struct TableLayout {
   }
 };
 
-// plain-column fast path (k_hash_agg_plain): every key and aggregate argument is a plain column and the
-// WHERE clause, if any, is a chain of column comparisons: no interpreter in the kernel
-struct PlainTerm {
-  int a, b;      // column slots (b: right-hand column when kind == 2)
-  int kind;      // 2 = col cmp col, 3 = col cmp imm
-  int op;        // VOp (V_EQ .. V_GE)
-  int mt;        // machine type of the operands
-  int conn;      // joins the running result with this term: 0 = AND, 1 = OR
-  unsigned long long imm;
-};
+// plain-column fast path (k_hash_agg_plain): every key and aggregate argument is a plain column of the (at most 4)
+// column slots and the WHERE clause, if any, is a chain of column comparisons: no interpreter in the kernel
 struct PlainSpec {
-  int ncols;                  // distinct column slots referenced (<= 4): ps.cols[0 .. ncols)
   int key_slot[kMaxKeys];
-  int arg_slot[kMaxAggs];     // per distinct argument program
-  int nterms;                 // predicate terms (0 = no predicate)
-  PlainTerm term[4];
+  int arg_slot[kMaxAggs];  // per distinct argument program
+  LeafChain pred;          // the WHERE clause (nterms = 0: none)
 };
 
 // Slots of the operator's device counters (AggParams::counters, dfgpu_aggstate::d_counters).
@@ -463,7 +453,7 @@ struct PlainSrc {
 #pragma unroll
     for (int c = 0; c < NC; c++) {
       cv[c][0] = cv[c][1] = 0ull;
-      if (c < p.plain.ncols && mask) {
+      if (c < p.ps.ncols && mask) {
         const int dt = p.ps.cols[c].dtype;  // warp-uniform
         if (dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64) ld_pair64(p.ps.cols[c].ptr, row0, both, policy, cv[c]);
         else ld_pair32(p.ps.cols[c].ptr, row0, both, dt == DFGPU_INT32, cv[c]);
@@ -471,15 +461,15 @@ struct PlainSrc {
     }
   }
   __device__ __forceinline__ void prepare(const AggParams& p) {
-    if (p.plain.nterms > 0) {
+    if (p.plain.pred.nterms > 0) {
       unsigned keep = 0;
-      for (int t = 0; t < p.plain.nterms; t++) {
-        const PlainTerm& pt = p.plain.term[t];
+      for (int t = 0; t < p.plain.pred.nterms; t++) {
+        const Leaf& pt = p.plain.pred.term[t];
         unsigned long long x[2], y[2];
         col(pt.a, x);
         if (pt.kind == 2) col(pt.b, y);
         else y[0] = y[1] = pt.imm;
-        const unsigned f = cmp_bits2(pt.op, pt.mt, x, y);
+        const unsigned f = cmp_bits2(pt.op, pt.mtype, x, y);
         keep = t == 0 ? f : (pt.conn ? (keep | f) : (keep & f));
       }
       mask &= keep;
@@ -1584,34 +1574,6 @@ struct dfgpu_aggstate {
 
 namespace {
 
-// DFGPU_TRACE=1: print host-side phase timings of the aggregate operator (each phase synchronised)
-struct Trace {
-  bool on;
-  dfgpu_ctx* ctx;
-  double t0;
-  static double now() {
-    timespec ts;
-    clock_gettime(CLOCK_MONOTONIC, &ts);
-    return ts.tv_sec * 1e3 + ts.tv_nsec * 1e-6;
-  }
-  explicit Trace(dfgpu_ctx* c) : on(getenv("DFGPU_TRACE") != nullptr), ctx(c), t0(0) {
-    if (on) { cudaStreamSynchronize(ctx->stream); t0 = now(); }
-  }
-  void mark(const char* what) {
-    if (!on) return;
-    cudaStreamSynchronize(ctx->stream);
-    const double t = now();
-    fprintf(stderr, "[dfgpu trace] %-28s %8.3f ms\n", what, t - t0);
-    t0 = t;
-  }
-};
-
-// DFGPU_TRACE: name each kernel as it is launched, template arguments included, so that a run shows which
-// instantiation the dispatch chose (the GROUP BY kernel tests assert it)
-void trace_launch(const char* kernel) {
-  if (getenv("DFGPU_TRACE")) fprintf(stderr, "[dfgpu trace] launch %s\n", kernel);
-}
-
 // Words of the pinned ctx->h_scratch that the operator stages through.
 constexpr int HS_COUNTERS = 8;  // counter slots [0, CTR_NONNULL)
 constexpr int HS_HEADER = 16;   // multi-GPU header record (up to 16 words)
@@ -2202,59 +2164,27 @@ void compile_batch(dfgpu_aggstate* st, const dfgpu_batch* batch, BatchPrograms& 
   }
 }
 
-// Whether programs [has_pred] + nkeys keys + nargs arguments of `pb` fit the interpreter-free PlainSrc: every key and argument
-// a plain 4/8-byte column and the WHERE clause, if any, a chain of column comparisons.  If so, *out describes them.
+// Whether programs [has_pred] + nkeys keys + nargs arguments of `pb` fit the interpreter-free PlainSrc: at most 4 column
+// slots, all 4/8-byte, null-free and 16-byte aligned, every key and argument a plain column and the WHERE clause, if
+// any, a comparison chain.  If so, *out describes them.
 bool plain_spec(const ProgramBuilder& pb, const ProgramSet& ps, int has_pred, int nkeys, int nargs, PlainSpec* out) {
   PlainSpec sp;
   memset(&sp, 0, sizeof(sp));
-  auto wide = [](int dt) {
-    return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64 || dt == DFGPU_FLOAT32 || dt == DFGPU_INT32 || dt == DFGPU_UINT32;
-  };
   bool ok = !ps.has_nulls && ps.ncols <= 4;
   for (int c = 0; ok && c < ps.ncols; c++)
-    ok = wide(ps.cols[c].dtype) && (reinterpret_cast<uintptr_t>(ps.cols[c].ptr) & 15) == 0;
+    ok = is_numeric4or8(ps.cols[c].dtype) && (reinterpret_cast<uintptr_t>(ps.cols[c].ptr) & 15) == 0;
   for (int k = 0; ok && k < nkeys; k++) {
-    const CompiledProgram& cpk = pb.prog(has_pred + k);
-    ok = cpk.is_plain_column;
-    sp.key_slot[k] = cpk.plain_slot;
+    ok = pb.prog(has_pred + k).leaf.kind == 1;
+    sp.key_slot[k] = pb.prog(has_pred + k).leaf.a;
   }
   for (int g = 0; ok && g < nargs; g++) {
-    const CompiledProgram& cpa = pb.prog(has_pred + nkeys + g);
-    ok = cpa.is_plain_column;
-    sp.arg_slot[g] = cpa.plain_slot;
+    ok = pb.prog(has_pred + nkeys + g).leaf.kind == 1;
+    sp.arg_slot[g] = pb.prog(has_pred + nkeys + g).leaf.a;
   }
   if (ok && has_pred) {
-    // t0 [t1 AND|OR [t2 AND|OR ...]] in lowered form: (PUSH_COL, CMP leaf) {(PUSH_COL, CMP leaf), AND|OR stack}*
-    const int b = ps.start[0], e = ps.start[1];
-    const DevInsn* in = &ps.insn[b];
-    auto term_at = [&](int i, PlainTerm* out) {
-      if (i + 1 >= e - b) return false;
-      const DevInsn &c = in[i], &o = in[i + 1];
-      if (c.op != V_PUSH_COL) return false;
-      if (o.op < V_EQ || o.op > V_GE || o.mode == RHS_STACK) return false;
-      if (o.mode == RHS_COL && ps.cols[o.slot].dtype != ps.cols[c.slot].dtype) return false;
-      memset(out, 0, sizeof(*out));
-      out->kind = o.mode == RHS_COL ? 2 : 3;
-      out->op = o.op;
-      out->a = c.slot;
-      out->b = o.mode == RHS_COL ? o.slot : 0;
-      out->mt = mtype_of(ps.cols[c.slot].dtype);
-      out->imm = o.imm;
-      return true;
-    };
-    ok = term_at(0, &sp.term[0]);
-    sp.nterms = ok ? 1 : 0;
-    int i = 2;
-    while (ok && i < e - b) {
-      if (sp.nterms >= 4 || !term_at(i, &sp.term[sp.nterms]) || i + 2 >= e - b) { ok = false; break; }
-      const DevInsn& j = in[i + 2];
-      if ((j.op != V_AND && j.op != V_OR) || j.mode != RHS_STACK) { ok = false; break; }
-      sp.term[sp.nterms].conn = j.op == V_OR ? 1 : 0;
-      sp.nterms++;
-      i += 3;
-    }
+    sp.pred = pb.prog(0).chain;
+    ok = sp.pred.nterms > 0;
   }
-  sp.ncols = ps.ncols;
   if (ok) *out = sp;
   return ok;
 }
@@ -2354,7 +2284,7 @@ void distinct_update(dfgpu_aggstate* st, const BatchPrograms& bp, const AggParam
     const char* name;
     const int d = p.ps.max_depth;
     if (p.ps.has_nulls) fn = k_distinct_insert<8, true>, name = "k_distinct_insert<8, true>";
-    else if (plain && !list && (begin & 1) == 0 && p.plain.ncols <= 2) fn = k_distinct_insert_plain<2>, name = "k_distinct_insert_plain<2>";
+    else if (plain && !list && (begin & 1) == 0 && p.ps.ncols <= 2) fn = k_distinct_insert_plain<2>, name = "k_distinct_insert_plain<2>";
     else if (plain && !list && (begin & 1) == 0) fn = k_distinct_insert_plain<4>, name = "k_distinct_insert_plain<4>";
     else if (d <= 2) fn = k_distinct_insert<2, false>, name = "k_distinct_insert<2, false>";
     else fn = k_distinct_insert<8, false>, name = "k_distinct_insert<8, false>";
@@ -2466,10 +2396,9 @@ void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
     ReduceF64Params rp;
     memset(&rp, 0, sizeof(rp));
     for (int g = 0; g < bp.nargs && plain; g++) {
-      const CompiledProgram& cpg = bp.pb.prog(g);
-      plain = cpg.is_plain_column && p.ps.cols[cpg.plain_slot].dtype == DFGPU_FLOAT64 &&
-              (reinterpret_cast<uintptr_t>(p.ps.cols[cpg.plain_slot].ptr) & 15) == 0;
-      if (plain) rp.col[g] = (const double*)p.ps.cols[cpg.plain_slot].ptr;
+      const Leaf& f = bp.pb.prog(g).leaf;
+      plain = f.kind == 1 && f.dtype == DFGPU_FLOAT64 && (reinterpret_cast<uintptr_t>(p.ps.cols[f.a].ptr) & 15) == 0;
+      if (plain) rp.col[g] = (const double*)p.ps.cols[f.a].ptr;
     }
     if (plain) {
       rp.ncols = bp.nargs;
@@ -2505,9 +2434,8 @@ ScanPlan plan_scan(const dfgpu_aggstate* st, const BatchPrograms& bp, AggParams&
   plan.plain = !plain_off && plain_spec(bp.pb, p.ps, bp.has_pred, st->nkeys, bp.nargs, &p.plain);
   // lean kernel: one 8-byte integer key column, one 8-byte argument column, distinct MIN/MAX/SUM/COUNT, no WHERE
   static const bool lean_off = getenv("DFGPU_AGG_LEAN") && atoi(getenv("DFGPU_AGG_LEAN")) == 0;  // A/B switch
-  auto w8 = [](int dt) { return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64; };
-  bool ok = !lean_off && plan.plain && !bp.has_pred && st->nkeys == 1 && bp.nargs == 1 && w8(p.ps.cols[p.plain.key_slot[0]].dtype) &&
-       w8(p.ps.cols[p.plain.arg_slot[0]].dtype);
+  bool ok = !lean_off && plan.plain && !bp.has_pred && st->nkeys == 1 && bp.nargs == 1 && is_numeric8(p.ps.cols[p.plain.key_slot[0]].dtype) &&
+       is_numeric8(p.ps.cols[p.plain.arg_slot[0]].dtype);
   int mask = 0;
   for (int a = 0; ok && a < p.naggs; a++) {
     const int bit = 1 << (st->descs[size_t(a)].func - 1);  // MIN 1, MAX 2, SUM 4, COUNT 8
@@ -2553,7 +2481,7 @@ ScanKernel choose_scan(const dfgpu_aggstate* st, AggParams& p, const ScanPlan& p
     return {k_hash_agg_plain<2, false>, "k_hash_agg_plain<2, false>", false};
   }
   if (plan.plain && !replay && even) {
-    const bool two = p.plain.ncols <= 2;
+    const bool two = p.ps.ncols <= 2;
     if (front) {
       if (two) return {k_hash_agg_plain<2, true>, "k_hash_agg_plain<2, true>", true};
       return {k_hash_agg_plain<4, true>, "k_hash_agg_plain<4, true>", true};

@@ -44,6 +44,28 @@ int dtype_width(int dt) {
   return 0;
 }
 
+static double now_ms() {
+  timespec ts;
+  clock_gettime(CLOCK_MONOTONIC, &ts);
+  return ts.tv_sec * 1e3 + ts.tv_nsec * 1e-6;
+}
+
+Trace::Trace(dfgpu_ctx* c) : on(getenv("DFGPU_TRACE") != nullptr), ctx(c), t0(0) {
+  if (on) { cudaStreamSynchronize(ctx->stream); t0 = now_ms(); }
+}
+
+void Trace::mark(const char* what) {
+  if (!on) return;
+  cudaStreamSynchronize(ctx->stream);
+  const double t = now_ms();
+  fprintf(stderr, "[dfgpu trace] %-28s %8.3f ms\n", what, t - t0);
+  t0 = t;
+}
+
+void trace_launch(const char* kernel) {
+  if (getenv("DFGPU_TRACE")) fprintf(stderr, "[dfgpu trace] launch %s\n", kernel);
+}
+
 }  // namespace dfgpu
 
 using namespace dfgpu;

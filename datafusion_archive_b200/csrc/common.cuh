@@ -55,6 +55,9 @@ inline bool is_unsigned_int(int dt) { return dt >= DFGPU_UINT8 && dt <= DFGPU_UI
 inline bool is_int(int dt) { return dt >= DFGPU_INT8 && dt <= DFGPU_UINT64; }
 inline bool is_float(int dt) { return dt == DFGPU_FLOAT32 || dt == DFGPU_FLOAT64; }
 inline bool is_numeric(int dt) { return dt >= DFGPU_INT8 && dt <= DFGPU_FLOAT64; }
+// operand types of the interpreter-free kernels: 8-byte numeric, and 4- or 8-byte numeric
+inline bool is_numeric8(int dt) { return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64; }
+inline bool is_numeric4or8(int dt) { return is_numeric8(dt) || dt == DFGPU_FLOAT32 || dt == DFGPU_INT32 || dt == DFGPU_UINT32; }
 
 }  // namespace dfgpu
 
@@ -144,6 +147,18 @@ struct Utf8Source {
   const unsigned char* bytes;
 };
 constexpr int UTF8_SRC_SHIFT = 40;  // gather index = (source << 40) | row
+
+// DFGPU_TRACE=1: print host-side phase timings of an operator (each phase synchronised)
+struct Trace {
+  bool on;
+  dfgpu_ctx* ctx;
+  double t0;
+  explicit Trace(dfgpu_ctx* c);
+  void mark(const char* what);
+};
+// DFGPU_TRACE: name each kernel as it is launched, template arguments included, so that a run shows which
+// instantiation the dispatch chose (the kernel tests assert it)
+void trace_launch(const char* kernel);
 }  // namespace dfgpu
 
 struct dfgpu_batch {

@@ -62,6 +62,41 @@ VOp vop_of(int op) {
   }
 }
 
+// COL op COL | COL op LIT over 4- or 8-byte numeric operands (the type check gave both sides one dtype), else kind 0.
+// Called after lowering: every column already has its slot.
+Leaf leaf_of(ProgramBuilder* pb, const Node* nd) {
+  Leaf f;
+  memset(&f, 0, sizeof(f));
+  if (nd->kind != Node::BIN || nd->l->kind != Node::COL || (nd->r->kind != Node::COL && nd->r->kind != Node::LIT)) return f;
+  const int dt = nd->l->dtype;
+  if (!is_numeric4or8(dt) || nd->r->dtype != dt) return f;
+  const bool rcol = nd->r->kind == Node::COL;
+  f.kind = rcol ? 2 : 3;
+  f.op = vop_of(nd->op);
+  f.a = pb->slot_of_column(nd->l->col);
+  f.b = rcol ? pb->slot_of_column(nd->r->col) : 0;
+  f.dtype = dt;
+  f.mtype = mtype_of(dt);
+  f.imm = rcol ? 0 : nd->r->imm;
+  return f;
+}
+
+// Appends the comparison leaves of a left-deep AND / OR chain to *c; false when `nd` is not one of at most 4 terms.
+bool chain_of(ProgramBuilder* pb, const Node* nd, LeafChain* c) {
+  const Node* leaf = nd;
+  int conn = 0;
+  if (nd->kind == Node::BIN && (nd->op == DFGPU_OP_AND || nd->op == DFGPU_OP_OR)) {
+    if (!chain_of(pb, nd->l.get(), c)) return false;
+    leaf = nd->r.get();
+    conn = nd->op == DFGPU_OP_OR ? 1 : 0;
+  }
+  const Leaf t = leaf_of(pb, leaf);
+  if (c->nterms == 4 || !t.kind || t.op < V_EQ || t.op > V_GE) return false;
+  c->term[c->nterms] = t;
+  c->term[c->nterms++].conn = uint8_t(conn);
+  return true;
+}
+
 }  // namespace
 
 int ProgramBuilder::slot_of_column(int col) {
@@ -248,10 +283,20 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
   } em{this, &cp, &depth};
   em.go(st[0].get());
   cp.out_dtype = st[0]->dtype;
-  if (st[0]->kind == Node::COL) {
-    cp.is_plain_column = true;
-    cp.plain_slot = cp.code[0].slot;
+
+  // 3. interpreter-free shapes
+  const Node* root = st[0].get();
+  if (root->kind == Node::COL) {
+    cp.leaf.kind = 1;
+    cp.leaf.a = cp.code[0].slot;
+    cp.leaf.dtype = root->dtype;
+    cp.leaf.mtype = mtype_of(root->dtype);
+  } else {
+    const Leaf f = leaf_of(this, root);
+    const bool arith = f.op >= V_ADD && f.op <= V_DIV;
+    if (f.kind && arith && (is_float(f.dtype) || (is_numeric8(f.dtype) && f.op != V_DIV))) cp.leaf = f;
   }
+  if (!chain_of(this, root, &cp.chain)) cp.chain = LeafChain{};
   progs_.push_back(std::move(cp));
   return int(progs_.size()) - 1;
 }

@@ -57,14 +57,35 @@ struct ProgramSet {
   uint8_t nullable[kMaxProgs];  // program result can be null (arrow 0.12 array_ops semantics)
 };
 
+// Interpreter-free shapes.  ProgramBuilder::add recognises them; the operators pass them to kernels that evaluate them
+// with straight-line code (same arithmetic as the interpreter, no decode in the inner loop).
+// One leaf: a column copy, or one operation whose left operand is a column and whose right operand is a column or an
+// immediate, both of one 4- or 8-byte numeric dtype.
+struct Leaf {
+  int kind;       // 0 = none (use the interpreter), 1 = copy column a, 2 = a op column b, 3 = a op imm
+  int op;         // VOp
+  int a, b;       // column slots (b: kind 2 only, else 0)
+  int dtype;      // Arrow dtype of the operands (of the column, for a copy: any fixed width)
+  uint8_t mtype;  // machine type of the operands
+  uint8_t conn;   // in a chain: joins the running result with this leaf, 0 = AND, 1 = OR
+  unsigned long long imm;  // kind 3: raw bits, widened like DevInsn::imm
+};
+// Up to 4 comparison leaves evaluated left to right: term[0] [conn term[1] [conn term[2] [conn term[3]]]]
+struct LeafChain {
+  int nterms;  // 0 = not a chain
+  Leaf term[4];
+};
+static_assert(sizeof(Leaf) == 32 && sizeof(LeafChain) == 136, "FPParams and AggParams carry chains and leaves: keep them compact");
+
 // ---- host side ----------------------------------------------------------------------------
 struct CompiledProgram {
   std::vector<DevInsn> code;
   bool nullable = false;
   int out_dtype = 0;
   int max_depth = 0;
-  bool is_plain_column = false;  // program is exactly [PUSH_COL]
-  int plain_slot = -1;
+  Leaf leaf{};        // kind 1: the program is exactly one column; 2 / 3: one + - * / (no integer division, no
+                      // arithmetic on integers narrower than 64 bits); else kind 0
+  LeafChain chain{};  // nterms > 0: the program is a chain of comparisons joined by AND / OR
 };
 
 class ProgramBuilder {

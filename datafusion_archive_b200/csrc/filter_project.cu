@@ -198,6 +198,8 @@ static void launch_fp(dfgpu_ctx* ctx, const FPParams& p) {
   const int ps = ctx->prof_begin();
   k_filter_project<DEPTH, NULLS><<<(unsigned)grid, FP_THREADS, 0, ctx->stream>>>(p);
   DF_CUDA(cudaGetLastError());
+  static const std::string name = "k_filter_project<" + std::to_string(DEPTH) + (NULLS ? ", true>" : ", false>");
+  trace_launch(name.c_str());
   ctx->prof_end(ps);
   ctx->launches++;
 }
@@ -388,74 +390,8 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
         }
       }
     }
-    // fast shapes (see FPParams): straight from the lowered bytecode
-    auto fast_type = [&](int dt) {
-      return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64 || dt == DFGPU_FLOAT32 || dt == DFGPU_INT32 || dt == DFGPU_UINT32;
-    };
-    auto fast_of = [&](int prog, bool is_pred) {
-      FastOp f;
-      memset(&f, 0, sizeof(f));
-      const int b = p.ps.start[prog], e = p.ps.start[prog + 1];
-      const DevInsn* in = &p.ps.insn[b];
-      if (in[0].op != V_PUSH_COL) return f;
-      const int dt = p.ps.cols[in[0].slot].dtype;
-      if (e - b == 1 && !is_pred) {  // plain column copy: any fixed width
-        f.kind = 1;
-        f.a = in[0].slot;
-        f.ty = dt;
-        return f;
-      }
-      if (e - b != 2 || in[1].mode == RHS_STACK || !fast_type(dt)) return f;
-      const bool cmp = in[1].op >= V_EQ && in[1].op <= V_GE, arith = in[1].op >= V_ADD && in[1].op <= V_DIV;
-      if (is_pred ? !cmp : !arith) return f;
-      if (arith && (dt == DFGPU_INT32 || dt == DFGPU_UINT32)) return f;               // narrow wrap-around: interpreter
-      if (arith && in[1].op == V_DIV && !(dt == DFGPU_FLOAT64 || dt == DFGPU_FLOAT32)) return f;  // integer division: interpreter
-      if (in[1].mode == RHS_COL && p.ps.cols[in[1].slot].dtype != dt) return f;
-      f.kind = in[1].mode == RHS_COL ? 2 : 3;
-      f.op = in[1].op;
-      f.a = in[0].slot;
-      f.b = in[1].slot;
-      f.ty = dt;
-      f.imm = in[1].imm;
-      return f;
-    };
-    memset(&p.pred_fast, 0, sizeof(p.pred_fast));
-    if (has_pred) {
-      // t0 [t1 AND|OR [t2 AND|OR ...]] in lowered form: (PUSH_COL, CMP leaf) {(PUSH_COL, CMP leaf), AND|OR stack}*
-      const int b = p.ps.start[0], e = p.ps.start[1];
-      const DevInsn* in = &p.ps.insn[b];
-      auto term_at = [&](int i, FastOp* out) {
-        if (i + 1 >= e - b) return false;
-        const DevInsn &c = in[i], &o = in[i + 1];
-        if (c.op != V_PUSH_COL || !fast_type(p.ps.cols[c.slot].dtype)) return false;
-        if (o.op < V_EQ || o.op > V_GE || o.mode == RHS_STACK) return false;
-        if (o.mode == RHS_COL && p.ps.cols[o.slot].dtype != p.ps.cols[c.slot].dtype) return false;
-        memset(out, 0, sizeof(*out));
-        out->kind = o.mode == RHS_COL ? 2 : 3;
-        out->op = o.op;
-        out->a = c.slot;
-        out->b = o.slot;
-        out->ty = p.ps.cols[c.slot].dtype;
-        out->imm = o.imm;
-        return true;
-      };
-      FastPred fp;
-      memset(&fp, 0, sizeof(fp));
-      int i = 0;
-      bool ok = term_at(0, &fp.term[0]);
-      fp.nterms = ok ? 1 : 0;
-      i = 2;
-      while (ok && i < e - b) {
-        if (fp.nterms >= 4 || !term_at(i, &fp.term[fp.nterms]) || i + 2 >= e - b) { ok = false; break; }
-        const DevInsn& j = in[i + 2];
-        if ((j.op != V_AND && j.op != V_OR) || j.mode != RHS_STACK) { ok = false; break; }
-        fp.conn[fp.nterms] = j.op == V_OR ? 1 : 0;
-        fp.nterms++;
-        i += 3;
-      }
-      if (ok) p.pred_fast = fp;
-    }
-    for (int i = 0; i < nkern; i++) p.proj_fast[i] = fast_of(i + has_pred, false);
+    p.pred_fast = has_pred ? pb.prog(0).chain : LeafChain{};
+    for (int i = 0; i < nkern; i++) p.proj_fast[i] = pb.prog(i + has_pred).leaf;
     if (p.ps.has_nulls) {
       p.ntiles = int((n + FP_TILE - 1) / FP_TILE);
       launch_fp<8, true>(ctx, p);  // the null-aware evaluator lives in the direct kernel only

@@ -12,23 +12,6 @@ constexpr int FP_CHUNKS = 2;  // interpreter passes per tile
 constexpr int FP_ITEMS = FP_R * FP_CHUNKS;
 constexpr int FP_TILE = FP_THREADS * FP_ITEMS;
 
-struct FastOp {
-  int kind;  // 0 = use the interpreter, 1 = copy column a, 2 = a op column b, 3 = a op imm
-  int op;    // VOp
-  int a, b;  // column slots
-  int ty;    // operand dtype: Float64 / Int64 / UInt64 / Float32 / Int32 / UInt32
-  int _pad;
-  unsigned long long imm;  // raw bits, widened like DevInsn::imm
-};
-
-// predicate fast shape: up to 4 Float64 comparisons chained left to right with AND / OR
-//   t0 [conn1 t1 [conn2 t2 [conn3 t3]]]   (each term: COL cmp COL | COL cmp IMM)
-struct FastPred {
-  int nterms;  // 0 = use the interpreter
-  int conn[4]; // conn[i] joins the running result with term i: 0 = AND, 1 = OR
-  FastOp term[4];
-};
-
 struct FPParams {
   ProgramSet ps;  // program 0 = predicate when has_pred, projections follow
   void* out[kMaxProgs];
@@ -53,12 +36,9 @@ struct FPParams {
   int nstagesA, nstagesB;
   int lag;    // tiles between the predicate pass and the projection pass
   int delay;  // waves between publishing a tile's count and resolving the offsets of its wave (1 <= delay <= lag)
-  // "fast shapes": single-operation programs over 4- and 8-byte numeric columns are recognised on the host and executed by
-  // straight-line code instead of the interpreter (same arithmetic, no decode in the inner loop).
-  //   predicate : chain of (COL cmp COL | COL cmp IMM) joined by AND / OR
-  //   projection: COL | COL op COL | COL op IMM          (op in + - * /)
-  FastPred pred_fast;
-  FastOp proj_fast[kMaxProgs];
+  // "fast shapes" (Leaf, as ProgramBuilder::add recognised them): the TMA kernel runs them without the interpreter
+  LeafChain pred_fast;  // the predicate as a comparison chain
+  Leaf proj_fast[kMaxProgs];
 };
 
 constexpr unsigned long long ST_AGG = 1ull << 62, ST_INCL = 2ull << 62, ST_MASK = (1ull << 62) - 1;

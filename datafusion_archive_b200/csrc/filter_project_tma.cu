@@ -170,7 +170,7 @@ __device__ __forceinline__ void producer_loop(const FPParams& p, int tile_rows, 
 
 // one comparison over the K rows of this lane -> K flag bits (operands straight from the staged tile)
 template <int K, class T>
-__device__ __forceinline__ unsigned cmp_term_t(const FastOp& t, const unsigned char* stage, const int* col_off, int lrow0, T imm) {
+__device__ __forceinline__ unsigned cmp_term_t(const Leaf& t, const unsigned char* stage, const int* col_off, int lrow0, T imm) {
   const T* A = (const T*)(stage + col_off[t.a]) + lrow0;
   const bool bcol = t.kind == 2;
   const T* B = bcol ? (const T*)(stage + col_off[t.b]) + lrow0 : A;
@@ -193,9 +193,9 @@ __device__ __forceinline__ unsigned cmp_term_t(const FastOp& t, const unsigned c
   return flags;
 }
 template <int K, bool F64>
-__device__ __forceinline__ unsigned cmp_term(const FastOp& t, const unsigned char* stage, const int* col_off, int lrow0) {
+__device__ __forceinline__ unsigned cmp_term(const Leaf& t, const unsigned char* stage, const int* col_off, int lrow0) {
   if (F64) return cmp_term_t<K, double>(t, stage, col_off, lrow0, u2d(t.imm));
-  switch (t.ty) {
+  switch (t.dtype) {
     case DFGPU_FLOAT64: return cmp_term_t<K, double>(t, stage, col_off, lrow0, u2d(t.imm));
     case DFGPU_INT64: return cmp_term_t<K, long long>(t, stage, col_off, lrow0, (long long)t.imm);
     case DFGPU_UINT64: return cmp_term_t<K, unsigned long long>(t, stage, col_off, lrow0, t.imm);
@@ -207,7 +207,7 @@ __device__ __forceinline__ unsigned cmp_term(const FastOp& t, const unsigned cha
 
 // one arithmetic operation over the K rows of this lane (Float64 / Float32 / 64-bit integers)
 template <int K, class T>
-__device__ __forceinline__ void arith_term_t(const FastOp& t, const unsigned char* stage, const int* col_off, int lrow0, T imm, unsigned flags,
+__device__ __forceinline__ void arith_term_t(const Leaf& t, const unsigned char* stage, const int* col_off, int lrow0, T imm, unsigned flags,
                                              bool& bad, T (&out)[K]) {
   const T* A = (const T*)(stage + col_off[t.a]) + lrow0;
   const bool bcol = t.kind == 2;
@@ -330,7 +330,7 @@ __device__ __forceinline__ void consumer_lean(const FPParams& p, int warp, int l
   constexpr unsigned b_cnt = (unsigned)offsetof(TmaShared, cnt_ready), b_pfx = (unsigned)offsetof(TmaShared, pfx_ready);
   // operand offsets (bytes from the start of shared memory) in stage 0
   const int lrow0 = warp * 32 * K + lane;
-  const FastOp& pt = p.pred_fast.term[0];
+  const Leaf& pt = p.pred_fast.term[0];
   const unsigned long long pimm = pt.imm;
   const int ringA_off = TM_HDR_BYTES, stageA = p.stage_bytesA;
   const int ringB_off = TM_HDR_BYTES + SA * stageA, stageB = p.stage_bytesB;
@@ -342,9 +342,9 @@ __device__ __forceinline__ void consumer_lean(const FPParams& p, int warp, int l
   unsigned long long* out2[NP];
 #pragma unroll
   for (int q = 0; q < NP; q++) {
-    const FastOp& fo = p.proj_fast[q];
+    const Leaf& fo = p.proj_fast[q];
     // -1 copy; op (+0x100: the right operand is the immediate; +0x200: 64-bit integer arithmetic, two's complement wrap-around)
-    kop2[q] = fo.kind == 1 ? -1 : ((fo.kind == 2 ? fo.op : fo.op | 0x100) | (fo.ty == DFGPU_FLOAT64 ? 0 : 0x200));
+    kop2[q] = fo.kind == 1 ? -1 : ((fo.kind == 2 ? fo.op : fo.op | 0x100) | (fo.dtype == DFGPU_FLOAT64 ? 0 : 0x200));
     imm2[q] = fo.imm;
     a2[q] = sh0 + (unsigned)(ringB_off + p.col_offB[fo.a] + lrow0 * 8);
     b2[q] = fo.kind == 2 ? sh0 + (unsigned)(ringB_off + p.col_offB[fo.b] + lrow0 * 8) : a2[q];
@@ -480,7 +480,7 @@ __device__ __forceinline__ void consumer_lean_ops(const FPParams& p, int warp, i
 }
 template <int K, int NP>
 __device__ __forceinline__ void consumer_lean_dispatch(const FPParams& p, int warp, int lane) {
-  const int ty = p.pred_fast.term[0].ty;
+  const int ty = p.pred_fast.term[0].dtype;
   if (ty == DFGPU_FLOAT64) consumer_lean_ops<K, NP, 0>(p, warp, lane);
   else if (ty == DFGPU_INT64) consumer_lean_ops<K, NP, 1>(p, warp, lane);
   else consumer_lean_ops<K, NP, 2>(p, warp, lane);
@@ -620,7 +620,7 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_filter_project_tma(const __gr
         flags = cmp_term<K, FAST && F64ONLY>(p.pred_fast.term[0], src.stage, p.col_offA, src.lrow0);
         for (int t = 1; t < p.pred_fast.nterms; t++) {
           const unsigned ft = cmp_term<K, FAST && F64ONLY>(p.pred_fast.term[t], src.stage, p.col_offA, src.lrow0);
-          flags = p.pred_fast.conn[t] ? (flags | ft) : (flags & ft);
+          flags = p.pred_fast.term[t].conn ? (flags | ft) : (flags & ft);
         }
       } else if constexpr (!FAST) {
         unsigned long long v[K];
@@ -660,7 +660,7 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_filter_project_tma(const __gr
       for (int q = 0; q < p.nproj; q++) {
         const int prog = q + p.has_pred;
         unsigned long long v[K];
-        const FastOp& fo = p.proj_fast[q];
+        const Leaf& fo = p.proj_fast[q];
         if (fo.kind == 1 || (FAST && fo.kind < 2)) {
           if (FAST && F64ONLY) {
             const unsigned long long* A = (const unsigned long long*)(src.stage + p.col_offB[fo.a]) + src.lrow0;
@@ -670,7 +670,7 @@ __global__ void __launch_bounds__(TM_THREADS, 1) k_filter_project_tma(const __gr
             src.load_rows(p.ps, fo.a, v);
           }
         } else if (fo.kind >= 2) {
-          switch ((FAST && F64ONLY) ? (int)DFGPU_FLOAT64 : fo.ty) {
+          switch ((FAST && F64ONLY) ? (int)DFGPU_FLOAT64 : fo.dtype) {
             case DFGPU_FLOAT64: {
               double o[K];
               arith_term_t<K, double>(fo, src.stage, p.col_offB, src.lrow0, u2d(fo.imm), flags, bad, o);
@@ -778,6 +778,9 @@ static void launch_one(dfgpu_ctx* ctx, const FPParams& p, size_t smem) {
   // cooperative launch: the wave-synchronous scan needs every CTA of the grid resident at once
   void* args[] = {(void*)&p};
   DF_CUDA(cudaLaunchCooperativeKernel((const void*)kern, dim3((unsigned)grid), dim3(TM_THREADS), args, smem, ctx->stream));
+  static const std::string name = "k_filter_project_tma<" + std::to_string(DEPTH) + ", " + std::to_string(K) + (F64ONLY ? ", true" : ", false") +
+                                  (FAST ? ", true, " : ", false, ") + std::to_string(LEAN) + ">";
+  trace_launch(name.c_str());
   ctx->prof_end(ps);
   ctx->launches++;
 }
@@ -789,9 +792,8 @@ static void launch_k(dfgpu_ctx* ctx, const FPParams& p, size_t smem) {
   bool all_f64 = true;
   for (int c = 0; c < p.ps.ncols; c++) all_f64 = all_f64 && p.ps.cols[c].dtype == DFGPU_FLOAT64;
   // lean shapes: one comparison over 8-byte operands (Float64 / Int64 / UInt64), one or two copy / arithmetic projections over 8-byte columns (DFGPU_FP_LEAN=0: A/B switch)
-  auto w8 = [](int dt) { return dt == DFGPU_FLOAT64 || dt == DFGPU_INT64 || dt == DFGPU_UINT64; };
-  bool lean = fast && p.has_pred && p.pred_fast.nterms == 1 && w8(p.pred_fast.term[0].ty) && p.nproj >= 1 && p.nproj <= LEAN_MAX_PROJ;
-  for (int q = 0; lean && q < p.nproj; q++) lean = w8(p.proj_fast[q].ty);  // copies and arithmetic over 8-byte columns only
+  bool lean = fast && p.has_pred && p.pred_fast.nterms == 1 && is_numeric8(p.pred_fast.term[0].dtype) && p.nproj >= 1 && p.nproj <= LEAN_MAX_PROJ;
+  for (int q = 0; lean && q < p.nproj; q++) lean = is_numeric8(p.proj_fast[q].dtype);  // copies and arithmetic over 8-byte columns only
   if (const char* e = getenv("DFGPU_FP_LEAN")) lean = lean && atoi(e) != 0;
   if (lean && p.nproj == 1) launch_one<1, K, true, true, 1>(ctx, p, smem);
   else if (lean) launch_one<1, K, true, true, 2>(ctx, p, smem);
