@@ -32,7 +32,7 @@ OP_ADD, OP_SUB, OP_MUL, OP_DIV = 10, 11, 12, 13
 OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE = 20, 21, 22, 23, 24, 25
 OP_AND, OP_OR = 30, 31
 
-AGG_MIN, AGG_MAX, AGG_SUM, AGG_COUNT, AGG_COUNT_DISTINCT = 1, 2, 3, 4, 5
+AGG_MIN, AGG_MAX, AGG_SUM, AGG_COUNT, AGG_COUNT_DISTINCT, AGG_AVG = 1, 2, 3, 4, 5, 6
 
 
 class Col(C.Structure):

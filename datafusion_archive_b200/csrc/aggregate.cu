@@ -29,6 +29,12 @@ constexpr long long AG_MIN_CAP = 1ll << 22;
 constexpr long long AG_SET_MIN_CAP = 1ll << 20;  // COUNT(DISTINCT) pair sets: 16-byte slots
 constexpr long long AG_PREFIX_ROWS = 1ll << 20;  // prefix sample that sizes the tables of a first big batch
 
+// Internal function code (not part of the C ABI) of the sum word of an AVG: every AVG(x) is two table words, this one
+// and a COUNT of the same argument.  Only the per-row fold sees the argument's type: it widens the value to f64 and
+// adds it, and it skips nulls also under GROUP BY.  Everything else -- merges, growth, the exchanges, compaction and
+// decoding -- treats the word as an f64 SUM.
+constexpr int AGG_AVG_SUM = 16;
+
 struct AggDesc {
   uint8_t func;   // DFGPU_AGG_*
   uint8_t mtype;  // machine type of the argument
@@ -159,6 +165,17 @@ __host__ __device__ __forceinline__ unsigned long long agg_identity(int func) {
   return func == DFGPU_AGG_MIN ? ~0ull : 0ull;
 }
 
+// an argument value in the widened 64-bit machine representation, as f64 (AVG): exact for Float32, rounded to nearest
+// for integers beyond 2^53
+__device__ __forceinline__ double widen_f64(unsigned long long v, int mt) {
+  switch (mt) {
+    case MT_F64: return u2d(v);
+    case MT_F32: return (double)u2f(v);
+    case MT_I: return (double)(long long)v;
+    default: return (double)v;
+  }
+}
+
 // fold one value into an accumulator held in a register / shared memory
 __device__ __forceinline__ unsigned long long acc_fold(int func, int mt, unsigned long long acc, unsigned long long v) {
   switch (func) {
@@ -166,6 +183,7 @@ __device__ __forceinline__ unsigned long long acc_fold(int func, int mt, unsigne
       if (mt == MT_F64) return d2u(u2d(acc) + u2d(v));
       if (mt == MT_F32) return f2u(u2f(acc) + u2f(v));
       return acc + v;
+    case AGG_AVG_SUM: return d2u(u2d(acc) + widen_f64(v, mt));
     case DFGPU_AGG_COUNT: return acc + 1ull;
     case DFGPU_AGG_MIN: {
       if (is_nan_val(v, mt)) return acc;  // f64::min ignores NaN (aggregate.rs:139-140)
@@ -186,6 +204,7 @@ __device__ __forceinline__ unsigned long long acc_merge(int func, int mt, unsign
       if (mt == MT_F64) return d2u(u2d(a) + u2d(b));
       if (mt == MT_F32) return f2u(u2f(a) + u2f(b));
       return a + b;
+    case AGG_AVG_SUM: return d2u(u2d(a) + u2d(b));
     case DFGPU_AGG_COUNT: return a + b;
     case DFGPU_AGG_MIN: return a < b ? a : b;
     default: return a > b ? a : b;
@@ -199,6 +218,7 @@ __device__ __forceinline__ void acc_merge_global(int func, int mt, unsigned long
       else if (mt == MT_F32) atomicAdd((float*)p, u2f(b));
       else atomicAdd(p, b);
       break;
+    case AGG_AVG_SUM: atomicAdd((double*)p, u2d(b)); break;
     case DFGPU_AGG_COUNT: atomicAdd(p, b); break;
     case DFGPU_AGG_MIN: atomicMin(p, b); break;
     default: atomicMax(p, b); break;
@@ -332,7 +352,7 @@ constexpr int AG_FRONT_MAX_GROUPS = 1024;
 // expr_vm.cuh, AG_R rows per thread.
 // NULLS: like the reference, keys and MIN/MAX/SUM arguments are read ignoring the validity bitmap
 // (`array.value(row)`, aggregate.rs:561-601, 807-852; a null produced by arithmetic reads as the
-// builder's default 0); only COUNT (an extension, §DESIGN) honours nulls.  A predicate that evaluates to
+// builder's default 0); only COUNT and AVG (extensions, §DESIGN) honour nulls.  A predicate that evaluates to
 // null reads as its value false (filter.rs:86 `filter.value(i)`).
 template <int DEPTH, bool NULLS>
 struct InterpSrc {
@@ -582,16 +602,19 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
       const unsigned b = src.arg(p, g, v, av);
       for (int a = 0; a < p.naggs; a++) {
         if (p.agg_arg[a] != g) continue;
-        const int func = p.aggs[a].func, mt = p.aggs[a].mtype, l = p.t.loc[a];
+        // AVG's sum word: the value is widened to f64 here and folded as an f64 SUM
+        const bool avg = p.aggs[a].func == AGG_AVG_SUM;
+        const int func = avg ? int(DFGPU_AGG_SUM) : p.aggs[a].func, mt = avg ? int(MT_F64) : p.aggs[a].mtype, l = p.t.loc[a];
         const bool cond = l >= 1 && l <= 3 && (func == DFGPU_AGG_MIN || func == DFGPU_AGG_MAX);
 #pragma unroll
         for (int r = 0; r < R; r++) {
-          if (NULLS && func == DFGPU_AGG_COUNT && !((av >> r) & 1u)) continue;  // COUNT counts non-null values
+          if (NULLS && (func == DFGPU_AGG_COUNT || avg) && !((av >> r) & 1u)) continue;  // COUNT and AVG skip nulls
+          const unsigned long long x = avg ? d2u(widen_f64(v[r], p.aggs[a].mtype)) : v[r];
           if (FRONT && fslot[r] >= 0 && ((src.mask >> r) & 1u)) {
-            acc_fold_shared(func, mt, &ftab[(1 + a) * FS + fslot[r]], v[r]);
+            acc_fold_shared(func, mt, &ftab[(1 + a) * FS + fslot[r]], x);
             if ((b >> r) & 1u) bad = true;
           } else if (slot[r] >= 0) {
-            acc_fold_global_cond(func, mt, p.t.val(slot[r], a), v[r], cond && probing[r], cond ? line_word(ln[r], l) : 0ull);
+            acc_fold_global_cond(func, mt, p.t.val(slot[r], a), x, cond && probing[r], cond ? line_word(ln[r], l) : 0ull);
             if ((b >> r) & 1u) bad = true;
           }
         }
@@ -866,12 +889,13 @@ __global__ void __launch_bounds__(AG_THREADS) k_hash_agg_wide(const __grid_const
       const unsigned b = src.arg(p, g, v, av);
       for (int a = 0; a < p.naggs; a++) {
         if (p.agg_arg[a] != g) continue;
-        const int func = p.aggs[a].func, mt = p.aggs[a].mtype;
+        const bool avg = p.aggs[a].func == AGG_AVG_SUM;  // widened here, folded as an f64 SUM
+        const int func = avg ? int(DFGPU_AGG_SUM) : p.aggs[a].func, mt = avg ? int(MT_F64) : p.aggs[a].mtype;
 #pragma unroll
         for (int r = 0; r < R; r++) {
-          if (NULLS && func == DFGPU_AGG_COUNT && !((av >> r) & 1u)) continue;
+          if (NULLS && (func == DFGPU_AGG_COUNT || avg) && !((av >> r) & 1u)) continue;
           if (slot[r] >= 0) {
-            acc_fold_global(func, mt, p.t.val(slot[r], a), v[r]);
+            acc_fold_global(func, mt, p.t.val(slot[r], a), avg ? d2u(widen_f64(v[r], p.aggs[a].mtype)) : v[r]);
             if ((b >> r) & 1u) bad = true;
           }
         }
@@ -1064,7 +1088,7 @@ __global__ void __launch_bounds__(256) k_reduce_f64(const __grid_constant__ Redu
         for (int a = 0; a < p.naggs; a++) {
           if (p.agg_arg[a] != g) continue;
           const int f = p.aggs[a].func;
-          if (f == DFGPU_AGG_SUM) atomicAdd((double*)p.t.val(0, a), u2d(sum));
+          if (f == DFGPU_AGG_SUM || f == AGG_AVG_SUM) atomicAdd((double*)p.t.val(0, a), u2d(sum));
           else if (f == DFGPU_AGG_MIN) atomicMin(p.t.val(0, a), mn);
           else if (f == DFGPU_AGG_MAX) atomicMax(p.t.val(0, a), mx);
           else if (blockIdx.x == 0) atomicAdd(p.t.val(0, a), (unsigned long long)p.nrows);  // COUNT of a null-free column
@@ -1255,6 +1279,34 @@ __global__ void __launch_bounds__(256) k_decode_rows(const __grid_constant__ Dec
       store_elem(p.out_vals[a], p.aggs[a].out_dtype, i, v);
     }
   }
+}
+
+// AVG output: from the sum and count columns of an AVG's two words (compacted or decoded), the Float64 means, a
+// bit-packed validity bitmap (a group, or the scalar row, with no non-null value is null) and the number of nulls.
+struct AvgFinishParams {
+  const double* sum;
+  const unsigned long long* cnt;
+  long long n;
+  double* out;
+  unsigned* validity;  // (n + 31) / 32 words: bit j of word w is row 32 w + j (arrow's LSB-first bytes)
+  unsigned long long* nulls;
+};
+__global__ void __launch_bounds__(256) k_avg_finish(const __grid_constant__ AvgFinishParams p) {
+  const int lane = threadIdx.x & 31;
+  unsigned nulls = 0;
+  // the loop bound is a multiple of the block for every thread, so ballots stay converged
+  for (long long i0 = (long long)blockIdx.x * blockDim.x; i0 < p.n; i0 += (long long)gridDim.x * blockDim.x) {
+    const long long i = i0 + threadIdx.x;
+    const bool in = i < p.n;
+    const unsigned long long c = in ? p.cnt[i] : 0ull;
+    if (in) p.out[i] = c ? p.sum[i] / (double)c : 0.0;
+    const unsigned valid = __ballot_sync(0xffffffffu, c != 0ull), rows = __ballot_sync(0xffffffffu, in);
+    if (lane == 0 && rows) {
+      p.validity[i >> 5] = valid;
+      nulls += (unsigned)__popc(rows & ~valid);
+    }
+  }
+  if (lane == 0 && nulls) atomicAdd(p.nulls, (unsigned long long)nulls);
 }
 
 // Utf8 GROUP BY keys are grouped by a 64-bit hash of the string; accumulator `rep_agg` holds the
@@ -1554,7 +1606,11 @@ struct dfgpu_aggstate {
   int nscan = 0;
   std::vector<std::vector<dfgpu_insn>> dist_progs;
   std::vector<int> dist_set;
+  // AVG: each one is two scan words, an AGG_AVG_SUM word and the COUNT word right after it; out_word points at the sum
+  // word and out_is_avg says that the output is computed from the pair (k_avg_finish)
   std::vector<int> out_word;        // user aggregate -> table word
+  std::vector<char> out_is_avg;
+  bool emit_words = false;          // finish returns one column per table word (the regroup merge across ranks)
   std::vector<int> dist_dtypes;     // argument dtype per set, typed at the first batch
   std::vector<unsigned long long*> set_slots;
   std::vector<long long> set_cap;
@@ -1860,11 +1916,25 @@ extern "C" int dfgpu_aggregate_create(dfgpu_ctx* ctx, const dfgpu_insn* const* k
     for (int k = 0; k < nkeys; k++) st->key_progs.emplace_back(keys[k], keys[k] + key_len[k]);
     std::vector<int> dist_user;  // user aggregates that are COUNT(DISTINCT)
     for (int a = 0; a < naggs; a++) {
-      // compile_expr accepts min/max/count/sum (expression.rs:98-107), this engine also COUNT(DISTINCT); anything
-      // else is General("Unsupported aggregate function ...")
-      if (aggs[a].func < DFGPU_AGG_MIN || aggs[a].func > DFGPU_AGG_COUNT_DISTINCT)
+      // compile_expr accepts min/max/count/sum (expression.rs:98-107), this engine also COUNT(DISTINCT) and AVG;
+      // anything else is General("Unsupported aggregate function ...")
+      if (aggs[a].func < DFGPU_AGG_MIN || aggs[a].func > DFGPU_AGG_AVG)
         fail(DFGPU_ERR_GENERAL, "Unsupported aggregate function '" + std::to_string(aggs[a].func) + "'");
       std::vector<dfgpu_insn> prog(aggs[a].arg, aggs[a].arg + aggs[a].arg_len);
+      st->out_is_avg.push_back(aggs[a].func == DFGPU_AGG_AVG ? 1 : 0);
+      if (aggs[a].func == DFGPU_AGG_AVG) {
+        if (aggs[a].out_dtype != 0 && aggs[a].out_dtype != DFGPU_FLOAT64)
+          fail(DFGPU_ERR_EXECUTION, "unexpected type when creating array from aggregate map");
+        // two scan words of its own, never shared with a SUM(x) / COUNT(x) of the query: under GROUP BY those read
+        // null rows, AVG skips them
+        st->out_word.push_back(int(st->funcs.size()));
+        for (int f : {AGG_AVG_SUM, int(DFGPU_AGG_COUNT)}) {
+          st->arg_progs.push_back(prog);
+          st->funcs.push_back(f);
+          st->out_dtypes.push_back(f == AGG_AVG_SUM ? DFGPU_FLOAT64 : DFGPU_UINT64);
+        }
+        continue;
+      }
       if (aggs[a].func == DFGPU_AGG_COUNT_DISTINCT) {
         if (aggs[a].out_dtype != 0 && aggs[a].out_dtype != DFGPU_UINT64)
           fail(DFGPU_ERR_EXECUTION, "unexpected type when creating array from aggregate map");
@@ -1888,6 +1958,9 @@ extern "C" int dfgpu_aggregate_create(dfgpu_ctx* ctx, const dfgpu_insn* const* k
     // one attached after create)
     if (!dist_user.empty() && ctx->world > 1) fail(DFGPU_ERR_NOT_IMPLEMENTED, "COUNT(DISTINCT) with a communicator attached");
     st->nscan = int(st->funcs.size());
+    st->naggs = st->nscan + int(dist_user.size());  // table words
+    if (st->naggs > kMaxAggs)
+      fail(DFGPU_ERR_NOT_IMPLEMENTED, "aggregates that need more than " + std::to_string(kMaxAggs) + " accumulator words (each AVG takes two)");
     for (size_t j = 0; j < dist_user.size(); j++) st->out_word[size_t(dist_user[j])] = st->nscan + int(j);
     st->d_counters = (unsigned long long*)ctx->alloc(CTR_SLOTS * 8);
     DF_CUDA(cudaMemsetAsync(st->d_counters, 0, CTR_SLOTS * 8, ctx->stream));
@@ -2130,7 +2203,7 @@ void compile_batch(dfgpu_aggstate* st, const dfgpu_batch* batch, BatchPrograms& 
     d.func = uint8_t(st->funcs[size_t(a)]);
     d.mtype = mtype_of(dt);
     d.dtype = uint8_t(dt);
-    int want = d.func == DFGPU_AGG_COUNT ? DFGPU_UINT64 : dt;
+    int want = d.func == DFGPU_AGG_COUNT ? DFGPU_UINT64 : (d.func == AGG_AVG_SUM ? DFGPU_FLOAT64 : dt);
     int odt = st->out_dtypes[size_t(a)];
     if (odt == 0) odt = want;
     if (odt != want)  // the reference would hit "unexpected type when creating array from aggregate map" (aggregate.rs:683-695)
@@ -2438,8 +2511,13 @@ ScanPlan plan_scan(const dfgpu_aggstate* st, const BatchPrograms& bp, AggParams&
        is_numeric8(p.ps.cols[p.plain.arg_slot[0]].dtype);
   int mask = 0;
   for (int a = 0; ok && a < p.naggs; a++) {
-    const int bit = 1 << (st->descs[size_t(a)].func - 1);  // MIN 1, MAX 2, SUM 4, COUNT 8
-    ok = !(mask & bit);
+    int f = st->descs[size_t(a)].func;
+    if (f == AGG_AVG_SUM) {  // the lean SUM adds the argument as it is: that is AVG's f64 sum for a Float64 argument only
+      ok = st->descs[size_t(a)].mtype == MT_F64;
+      f = DFGPU_AGG_SUM;
+    }
+    const int bit = 1 << (f - 1);  // MIN 1, MAX 2, SUM 4, COUNT 8
+    ok = ok && !(mask & bit);
     mask |= bit;
   }
   if (ok) {
@@ -2469,7 +2547,7 @@ ScanKernel choose_scan(const dfgpu_aggstate* st, AggParams& p, const ScanPlan& p
       const int f = st->descs[size_t(a)].func, l = st->t.loc[a];
       if (f == DFGPU_AGG_MIN) p.lean.min_w = l;
       else if (f == DFGPU_AGG_MAX) p.lean.max_w = l;
-      else if (f == DFGPU_AGG_SUM) p.lean.sum_arr = st->t.add + (long long)(~l) * st->t.astride;
+      else if (f == DFGPU_AGG_SUM || f == AGG_AVG_SUM) p.lean.sum_arr = st->t.add + (long long)(~l) * st->t.astride;
       else p.lean.cnt_arr = st->t.add + (long long)(~l) * st->t.astride;
     }
     bool layout_ok = st->t.lw == (((plan.lean_mask & 3) == 3) ? 4 : ((plan.lean_mask & 3) ? 2 : 1));
@@ -2695,8 +2773,9 @@ void agg_export_raw(dfgpu_aggstate* st, DevBufs& bufs, unsigned long long** keys
 void agg_exchange_scalars(dfgpu_ctx* ctx, dfgpu_aggstate* st) {
   int funcs[kMaxAggs], mtypes[kMaxAggs];
   for (int a = 0; a < st->naggs; a++) {
-    funcs[a] = st->descs[size_t(a)].func;
-    mtypes[a] = st->descs[size_t(a)].mtype;
+    const bool avg = st->descs[size_t(a)].func == AGG_AVG_SUM;  // merged as the f64 SUM it is
+    funcs[a] = avg ? DFGPU_AGG_SUM : st->descs[size_t(a)].func;
+    mtypes[a] = avg ? MT_F64 : st->descs[size_t(a)].mtype;
   }
   // per-aggregate non-null input counts travel with the accumulators: fold the host-side counts of the
   // null-free batches into the device counters, which the exchange sums over ranks
@@ -2795,7 +2874,7 @@ void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, DevBufs& rows_buf, 
       d.func = uint8_t(st->funcs[size_t(a)]);
       d.dtype = uint8_t(dt);
       d.mtype = mtype_of(dt);
-      d.out_dtype = uint8_t(d.func == DFGPU_AGG_COUNT ? DFGPU_UINT64 : dt);
+      d.out_dtype = uint8_t(d.func == DFGPU_AGG_COUNT ? DFGPU_UINT64 : (d.func == AGG_AVG_SUM ? DFGPU_FLOAT64 : dt));
       st->descs.push_back(d);
     }
     if (!*regroup) pack_keys(st);  // (the regroup merge never packs keys)
@@ -2908,9 +2987,10 @@ void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, DevBufs& rows_buf, 
 }  // namespace
 
 // Multi-GPU merge for key shapes whose groups cannot travel as (packed key, accumulators) rows — Utf8 keys and
-// wide composite keys: every rank finishes locally, the ranks all-gather their LOCAL RESULT columns (strings
-// included), and every rank aggregates the concatenation once more with the merge function of each aggregate
-// (SUM -> SUM, COUNT -> SUM of counts, MIN -> MIN, MAX -> MAX) through the same single-GPU operator.  O(W x G) work
+// wide composite keys: every rank finishes locally, the ranks all-gather their LOCAL key and table-word columns
+// (strings included), and every rank aggregates the concatenation once more with the merge function of each word
+// (SUM -> SUM, COUNT -> SUM of counts, AVG's sum -> SUM, MIN -> MIN, MAX -> MAX) through the same single-GPU
+// operator.  O(W x G) work
 // per rank instead of the owner-partitioned O(G): accepted for these shapes.  Results agree across ranks bit for
 // bit except Float64 SUMs (order of the second aggregation's reductions: <= 1e-9 relative).
 namespace {
@@ -2921,15 +3001,18 @@ struct WorldGuard {  // run a stretch of the operator as if no communicator were
   ~WorldGuard() { c->world = world; }
 };
 
+// The merge works on table words, not on the caller's columns: an AVG travels as its sum and count words, which are
+// merged with SUM and divided only after the merge (k_avg_finish, in finish).  Returns keys + one column per word.
 std::unique_ptr<dfgpu_result> finish_regroup(dfgpu_ctx* ctx, dfgpu_aggstate* st) {
   const int W = ctx->world;
-  const int user_aggs = st->utf8_key ? st->naggs - 1 : st->naggs;
-  const int ncols = st->nkeys + user_aggs;
-  // 1. this rank's own result (an empty one when it saw no batch: types were adopted from the header)
+  const int nwords = st->utf8_key ? st->naggs - 1 : st->naggs;
+  const int ncols = st->nkeys + nwords;
+  // 1. this rank's own words (an empty result when it saw no batch: types were adopted from the header)
   std::unique_ptr<dfgpu_result> local;
   if (st->t.base) {
     WorldGuard g(ctx);
     dfgpu_result* r = nullptr;
+    st->emit_words = true;
     const int rc = dfgpu_aggregate_finish(st, &r);
     if (rc != DFGPU_OK) fail(rc, dfgpu_last_error());
     local.reset(r);
@@ -2946,7 +3029,7 @@ std::unique_ptr<dfgpu_result> finish_regroup(dfgpu_ctx* ctx, dfgpu_aggstate* st)
       }
       local->cols.push_back(c);
     }
-    for (int a = 0; a < user_aggs; a++) {
+    for (int a = 0; a < nwords; a++) {
       DevColumn c;
       c.dtype = st->descs[size_t(a)].out_dtype;
       local->cols.push_back(c);
@@ -3024,7 +3107,7 @@ std::unique_ptr<dfgpu_result> finish_regroup(dfgpu_ctx* ctx, dfgpu_aggstate* st)
   }
   DF_CUDA(cudaStreamSynchronize(ctx->stream));
   // 4. aggregate the partial results once more, with each aggregate's merge function
-  const size_t nk = size_t(st->nkeys), na = size_t(user_aggs);
+  const size_t nk = size_t(st->nkeys), na = size_t(nwords);
   std::vector<dfgpu_insn> kprog(nk), aprog(na);
   std::vector<const dfgpu_insn*> kptr;
   std::vector<int> klen;
@@ -3037,13 +3120,13 @@ std::unique_ptr<dfgpu_result> finish_regroup(dfgpu_ctx* ctx, dfgpu_aggstate* st)
     klen.push_back(1);
   }
   std::vector<dfgpu_agg> aggs(na);
-  for (int a = 0; a < user_aggs; a++) {
+  for (int a = 0; a < nwords; a++) {
     memset(&aprog[size_t(a)], 0, sizeof(dfgpu_insn));
     aprog[size_t(a)].op = DFGPU_OP_COL;
     aprog[size_t(a)].col = st->nkeys + a;
     aprog[size_t(a)].dtype = gathered->cols[size_t(st->nkeys + a)].dtype;
     const int f = st->descs[size_t(a)].func;
-    aggs[size_t(a)].func = f == DFGPU_AGG_COUNT ? DFGPU_AGG_SUM : f;
+    aggs[size_t(a)].func = f == DFGPU_AGG_COUNT || f == AGG_AVG_SUM ? DFGPU_AGG_SUM : f;  // AVG's sum word: a Float64 column
     aggs[size_t(a)].arg = &aprog[size_t(a)];
     aggs[size_t(a)].arg_len = 1;
     aggs[size_t(a)].out_dtype = gathered->cols[size_t(st->nkeys + a)].dtype;
@@ -3051,7 +3134,7 @@ std::unique_ptr<dfgpu_result> finish_regroup(dfgpu_ctx* ctx, dfgpu_aggstate* st)
   }
   WorldGuard g(ctx);
   dfgpu_aggstate* st2 = nullptr;
-  int rc = dfgpu_aggregate_create(ctx, kptr.data(), klen.data(), st->nkeys, aggs.data(), user_aggs, N / W + 1, &st2);
+  int rc = dfgpu_aggregate_create(ctx, kptr.data(), klen.data(), st->nkeys, aggs.data(), nwords, N / W + 1, &st2);
   if (rc != DFGPU_OK) fail(rc, dfgpu_last_error());
   struct StFree { dfgpu_aggstate* s; ~StFree() { dfgpu_aggregate_free(s); } } stfree{st2};
   dfgpu_result* res = nullptr;
@@ -3064,6 +3147,66 @@ std::unique_ptr<dfgpu_result> finish_regroup(dfgpu_ctx* ctx, dfgpu_aggstate* st)
   }
   return local;  // nobody had a group: the (empty) local result has the right columns
 }
+
+// The caller's aggregate columns from a result that holds the key columns and then one column per table word: the
+// COUNT(DISTINCT) words are put in the caller's order, and each AVG is computed from its sum and count words, which
+// are then freed like every word no output uses.
+void assemble_outputs(dfgpu_aggstate* st, dfgpu_result* res) {
+  dfgpu_ctx* ctx = st->ctx;
+  const size_t nk = size_t(st->nkeys);
+  const long long n = res->nrows;
+  dfgpu_result spare;  // RAII: the word columns that are not outputs
+  spare.ctx = ctx;
+  spare.cols.assign(res->cols.begin() + nk, res->cols.end());
+  res->cols.resize(nk);
+  bool any_avg = false;
+  for (char a : st->out_is_avg) any_avg = any_avg || a;
+  if (!any_avg) {  // a reordering only: no device work, no synchronisation
+    for (int w : st->out_word) {
+      res->cols.push_back(spare.cols[size_t(w)]);
+      spare.cols[size_t(w)] = DevColumn{};
+    }
+    return;
+  }
+  DevBufs tmp(ctx);
+  unsigned long long* d_nulls = tmp.alloc(kMaxAggs * 8);
+  DF_CUDA(cudaMemsetAsync(d_nulls, 0, kMaxAggs * 8, ctx->stream));
+  for (size_t i = 0; i < st->out_word.size(); i++) {
+    const size_t w = size_t(st->out_word[i]);
+    if (!st->out_is_avg[i]) {
+      res->cols.push_back(spare.cols[w]);
+      spare.cols[w] = DevColumn{};
+      continue;
+    }
+    DevColumn c;
+    c.dtype = DFGPU_FLOAT64;
+    c.values_bytes = size_t(n) * 8;
+    c.values = ctx->alloc(size_t(n > 0 ? n : 1) * 8);
+    res->cols.push_back(c);
+    if (n == 0) continue;
+    res->cols.back().validity = (uint8_t*)ctx->alloc(size_t((n + 31) / 32) * 4);
+    AvgFinishParams ap;
+    ap.sum = (const double*)spare.cols[w].values;
+    ap.cnt = (const unsigned long long*)spare.cols[w + 1].values;
+    ap.n = n;
+    ap.out = (double*)res->cols.back().values;
+    ap.validity = (unsigned*)res->cols.back().validity;
+    ap.nulls = d_nulls + i;
+    launch_kernel(ctx, k_avg_finish, "k_avg_finish", ap, n, 256 * 4, 8);
+  }
+  unsigned long long* h = ctx->h_scratch + HS_NONNULL;  // pinned
+  DF_CUDA(cudaMemcpyAsync(h, d_nulls, kMaxAggs * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  DF_CUDA(cudaStreamSynchronize(ctx->stream));
+  for (size_t i = 0; i < st->out_word.size(); i++) {
+    DevColumn& c = res->cols[nk + i];
+    if (!st->out_is_avg[i]) continue;
+    c.null_count = (int64_t)h[i];
+    if (c.null_count == 0) {  // no null: no bitmap, like every other aggregate column
+      ctx->free(c.validity);
+      c.validity = nullptr;
+    }
+  }
+}
 }  // namespace
 
 extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
@@ -3075,7 +3218,7 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
     Trace tr(ctx);
     if (ctx->world > 1 && !st->dist_progs.empty()) fail(DFGPU_ERR_NOT_IMPLEMENTED, "COUNT(DISTINCT) with a communicator attached");
     if (!st->typed && !(st->nkeys > 0 && ctx->world > 1)) {
-      // no batch was ever seen: resolve types from the declared output types
+      // no batch was ever seen: resolve types from the declared output types (an AVG's words: Float64 and UInt64)
       if (st->nkeys > 0) {
         // an empty GROUP BY input yields an empty batch; key types are unknown -> need a batch
         fail(DFGPU_ERR_GENERAL, "aggregate finished before any input batch was provided");
@@ -3105,8 +3248,10 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
       if (st->nkeys == 0) agg_exchange_scalars(ctx, st);
       else agg_exchange_groups(ctx, st, xbuf, &xrows, &xn, &xseg, &regroup);
       if (regroup) {
-        *out = finish_regroup(ctx, st).release();
+        std::unique_ptr<dfgpu_result> res = finish_regroup(ctx, st);
+        assemble_outputs(st, res.get());
         st->finished = true;
+        *out = res.release();
         return;
       }
     }
@@ -3215,8 +3360,11 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
         DF_CUDA(cudaStreamSynchronize(ctx->stream));
         for (int a = 0; a < st->naggs; a++) nonnull[size_t(a)] += (long long)ctx->h_scratch[HS_NONNULL + a];
       }
+      std::vector<char> avg_word(size_t(st->naggs), 0);  // an AVG's validity comes from its count word (k_avg_finish)
+      for (size_t i = 0; i < st->out_word.size(); i++)
+        if (st->out_is_avg[i]) avg_word[size_t(st->out_word[i])] = avg_word[size_t(st->out_word[i]) + 1] = 1;
       for (int a = 0; a < st->naggs; a++) {
-        if (nonnull[size_t(a)] > 0 || (st->rows_seen > 0 && st->descs[size_t(a)].func == DFGPU_AGG_COUNT)) continue;
+        if (avg_word[size_t(a)] || nonnull[size_t(a)] > 0 || (st->rows_seen > 0 && st->descs[size_t(a)].func == DFGPU_AGG_COUNT)) continue;
         DevColumn& c = res->cols[size_t(a)];
         c.validity = (uint8_t*)ctx->alloc(1);
         DF_CUDA(cudaMemsetAsync(c.validity, 0, 1, ctx->stream));
@@ -3224,9 +3372,7 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
       }
       DF_CUDA(cudaStreamSynchronize(ctx->stream));
     }
-    // aggregate columns in the caller's order: the COUNT(DISTINCT) words follow the scan's accumulators in the table
-    const std::vector<DevColumn> words(res->cols.begin() + st->nkeys, res->cols.end());
-    for (size_t i = 0; i < st->out_word.size(); i++) res->cols[size_t(st->nkeys) + i] = words[size_t(st->out_word[i])];
+    if (!st->emit_words) assemble_outputs(st, res.get());
     tr.mark("finish (compact + outputs)");
     st->finished = true;
     *out = res.release();

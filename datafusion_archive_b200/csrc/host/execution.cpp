@@ -508,6 +508,7 @@ std::optional<RecordBatch> GpuAggregateRelation::next() {
     std::string n = a->name;
     for (auto& c : n) c = char(tolower((unsigned char)c));
     int f = n == "min" ? DFGPU_AGG_MIN : n == "max" ? DFGPU_AGG_MAX : n == "sum" ? DFGPU_AGG_SUM : n == "count" ? DFGPU_AGG_COUNT : 0;
+    if (n == "avg") f = DFGPU_AGG_AVG;
     if (a->distinct) f = f == DFGPU_AGG_COUNT ? DFGPU_AGG_COUNT_DISTINCT : 0;
     if (!f) fail(DFGPU_ERR_GENERAL, "Unsupported aggregate function '" + a->name + "'");  // expression.rs:103-106
     funcs.push_back(f);

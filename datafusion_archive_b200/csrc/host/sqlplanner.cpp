@@ -193,7 +193,9 @@ ExprRef SqlToRel::sql_to_rex(const ASTRef& sql, const Schema& schema) const {
         std::vector<ExprRef> rex_args;
         for (auto& a : sql->args) rex_args.push_back(sql_to_rex(a, schema));
         if (rex_args.empty()) fail(DFGPU_ERR_INTERNAL, "aggregate function without arguments (reference: index panic at sqlplanner.rs:320)");
-        // return type is same as the argument type for these aggregate functions
+        // return type is same as the argument type for MIN / MAX / SUM; AVG is Float64 (the reference types it as
+        // its argument too, but never executes it)
+        if (lid == "avg") return Expr::aggregate(sql->id, rex_args, DFGPU_FLOAT64);
         return Expr::aggregate(sql->id, rex_args, rex_args[0]->get_type(schema));
       }
       if (lid == "count" && sql->distinct) {

@@ -131,7 +131,7 @@ class BinaryExpr(Expr):
 class AggregateFunction:
     """Expr::AggregateFunction{name,args,return_type} (src/logicalplan.rs:162-166)."""
 
-    _F = {"min": A.AGG_MIN, "max": A.AGG_MAX, "sum": A.AGG_SUM, "count": A.AGG_COUNT}
+    _F = {"min": A.AGG_MIN, "max": A.AGG_MAX, "sum": A.AGG_SUM, "count": A.AGG_COUNT, "avg": A.AGG_AVG}
 
     def __init__(self, name, arg, return_type=None, distinct=False):
         """distinct=True: COUNT(DISTINCT arg), the number of distinct non-null values (count only)."""
@@ -143,7 +143,12 @@ class AggregateFunction:
         func = A.AGG_COUNT_DISTINCT if self.distinct else self._F[self.name.lower()]
         rt = self.return_type
         if rt is None:
-            rt = A.UINT64 if func in (A.AGG_COUNT, A.AGG_COUNT_DISTINCT) else self.arg.get_type(schema)
+            if func in (A.AGG_COUNT, A.AGG_COUNT_DISTINCT):
+                rt = A.UINT64
+            elif func == A.AGG_AVG:
+                rt = A.FLOAT64
+            else:
+                rt = self.arg.get_type(schema)
         return (func, self.arg.program(schema), rt)
 
 

@@ -117,12 +117,23 @@ typedef struct dfgpu_insn {
  * DFGPU_AGG_COUNT_DISTINCT is AggregateType::CountDistinct (expression.rs:32-39), which the reference
  * declares but never produces or executes (COUNT(DISTINCT) is a ROADMAP.md 0.6.x item): the number of
  * distinct non-null argument values per group.  Additive: libraries older than it reject code 5 with
- * "Unsupported aggregate function". */
-enum { DFGPU_AGG_MIN = 1, DFGPU_AGG_MAX = 2, DFGPU_AGG_SUM = 3, DFGPU_AGG_COUNT = 4, DFGPU_AGG_COUNT_DISTINCT = 5 };
+ * "Unsupported aggregate function".
+ * DFGPU_AGG_AVG is AggregateType::Avg, likewise declared but never executed by the reference: the mean of
+ * the non-null argument values as Float64 (sum in f64 / count, one IEEE division), null when there are
+ * none.  Additive like code 5. */
+enum {
+  DFGPU_AGG_MIN = 1,
+  DFGPU_AGG_MAX = 2,
+  DFGPU_AGG_SUM = 3,
+  DFGPU_AGG_COUNT = 4,
+  DFGPU_AGG_COUNT_DISTINCT = 5,
+  DFGPU_AGG_AVG = 6
+};
 
 /* One aggregate expression: func(arg).  `arg` is a postfix program (exactly one argument, as
  * compile_expr asserts: expression.rs:91).  `out_dtype` is Expr::AggregateFunction.return_type
- * (arg type for MIN/MAX/SUM, UInt64 for COUNT and COUNT(DISTINCT): src/sqlplanner.rs:320-341). */
+ * (arg type for MIN/MAX/SUM, UInt64 for COUNT and COUNT(DISTINCT): src/sqlplanner.rs:320-341;
+ * Float64 for AVG).  0 = the default for the function. */
 typedef struct dfgpu_agg {
   int32_t func;
   int32_t arg_len;

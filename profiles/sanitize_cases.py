@@ -129,5 +129,19 @@ assert int(got[1].sum()) == len(pairs) and len(got[0]) == len(np.unique(kd))
 got = agg([vd], [], [AggregateFunction("count", col(0), distinct=True)])
 assert int(got[0][0]) == len(np.unique(vd))
 print("count distinct ok", flush=True)
+
+# 8. AVG: the converting fold with nulls, the lean f64 scan, k_avg_finish's bitmap, and the scalar reduce
+import pyarrow as pa  # noqa: E402
+ka = rng.integers(0, 1000, 1_000_003).astype(np.int64)
+va = rng.integers(-100, 100, 1_000_003).astype(np.int32)
+ok = (rng.random(len(va)) < 0.5) & (ka != 3)
+got = agg([ka, pa.array(va, mask=~ok)], [col(0)], [AggregateFunction("avg", col(1))])
+vals, valid = got[1]
+assert len(got[0]) == len(np.unique(ka)) and not valid[np.asarray(got[0]) == 3].any()
+got = agg([ka, va.astype(np.float64)], [col(0)], [AggregateFunction("avg", col(1))])
+assert len(got[0]) == len(np.unique(ka))
+got = agg([va], [], [AggregateFunction("avg", col(0))])
+assert float(got[0][0]) == float(np.float64(va.astype(np.int64).sum()) / len(va))
+print("avg ok", flush=True)
 ctx.close()
 print("SANITIZE_CASES_OK")

@@ -50,6 +50,8 @@ pub const AGG_COUNT: i32 = 4;
 /// AggregateType::CountDistinct; the reference's parser (sqlparser 0.2.1) cannot express it, so the shim only
 /// carries the constant.
 pub const AGG_COUNT_DISTINCT: i32 = 5;
+/// AggregateType::Avg: the mean of the non-null values as Float64, null when there are none.
+pub const AGG_AVG: i32 = 6;
 
 /// Borrowed view of one Arrow array (dfgpu_col).
 #[repr(C)]

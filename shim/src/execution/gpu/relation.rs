@@ -225,6 +225,7 @@ fn agg_func(name: &str) -> Result<i32> {
         "max" => Ok(AGG_MAX),
         "sum" => Ok(AGG_SUM),
         "count" => Ok(AGG_COUNT),
+        "avg" => Ok(AGG_AVG),
         _ => Err(ExecutionError::General(format!("Unsupported aggregate function '{}'", name))), // expression.rs:103-106
     }
 }
