@@ -31,6 +31,19 @@ OP_COL, OP_LIT, OP_CAST = 1, 2, 3
 OP_ADD, OP_SUB, OP_MUL, OP_DIV = 10, 11, 12, 13
 OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE = 20, 21, 22, 23, 24, 25
 OP_AND, OP_OR = 30, 31
+OP_FN = 40
+
+# built-in scalar functions (DFGPU_OP_FN: `col` = code); all Float64 -> Float64
+FN_SQRT, FN_ABS, FN_FLOOR, FN_CEIL, FN_TRUNC, FN_ROUND, FN_SIGNUM = 1, 2, 3, 4, 5, 6, 7
+FN_EXP, FN_LN, FN_LOG2, FN_LOG10 = 8, 9, 10, 11
+FN_SIN, FN_COS, FN_TAN, FN_ASIN, FN_ACOS, FN_ATAN = 12, 13, 14, 15, 16, 17
+FN_POWER, FN_ATAN2 = 18, 19
+FN_CODES = {
+    "sqrt": FN_SQRT, "abs": FN_ABS, "floor": FN_FLOOR, "ceil": FN_CEIL, "trunc": FN_TRUNC, "round": FN_ROUND,
+    "signum": FN_SIGNUM, "exp": FN_EXP, "ln": FN_LN, "log2": FN_LOG2, "log10": FN_LOG10, "sin": FN_SIN, "cos": FN_COS,
+    "tan": FN_TAN, "asin": FN_ASIN, "acos": FN_ACOS, "atan": FN_ATAN, "power": FN_POWER, "atan2": FN_ATAN2,
+}
+FN_ARITY = {code: (2 if code in (FN_POWER, FN_ATAN2) else 1) for code in FN_CODES.values()}
 
 AGG_MIN, AGG_MAX, AGG_SUM, AGG_COUNT, AGG_COUNT_DISTINCT, AGG_AVG = 1, 2, 3, 4, 5, 6
 

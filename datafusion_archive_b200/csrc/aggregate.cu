@@ -1706,8 +1706,8 @@ void launch_scan(dfgpu_ctx* ctx, const ScanKernel& k, AggParams& p, long long n)
 }
 template <int DEPTH>
 ScanKernel hash_agg_kernel(bool front) {
-  static const std::string with_front = "k_hash_agg<" + std::to_string(DEPTH) + ", true, false>";
-  static const std::string without = "k_hash_agg<" + std::to_string(DEPTH) + ", false, false>";
+  static const std::string with_front = "k_hash_agg<" + depth_arg(DEPTH) + ", true, false>";
+  static const std::string without = "k_hash_agg<" + depth_arg(DEPTH) + ", false, false>";
   if (front) return {k_hash_agg<DEPTH, true, false>, with_front.c_str(), true};
   return {k_hash_agg<DEPTH, false, false>, without.c_str(), false};
 }
@@ -1737,7 +1737,7 @@ void launch_reduce(dfgpu_ctx* ctx, const AggParams& p, long long n) {
   const int ps = ctx->prof_begin();
   k_reduce<DEPTH, NULLS><<<grid_for(ctx, n, RD_TILE, per_sm), AG_THREADS, 0, ctx->stream>>>(p);
   DF_CUDA(cudaGetLastError());
-  static const std::string name = "k_reduce<" + std::to_string(DEPTH) + (NULLS ? ", true>" : ", false>");
+  static const std::string name = "k_reduce<" + depth_arg(DEPTH) + (NULLS ? ", true>" : ", false>");
   trace_launch(name.c_str());
   ctx->prof_end(ps);
   ctx->launches++;
@@ -2356,7 +2356,9 @@ void distinct_update(dfgpu_aggstate* st, const BatchPrograms& bp, const AggParam
     void (*fn)(AggParams, SetParams);
     const char* name;
     const int d = p.ps.max_depth;
-    if (p.ps.has_nulls) fn = k_distinct_insert<8, true>, name = "k_distinct_insert<8, true>";
+    if (has_fn(p.ps) && p.ps.has_nulls) fn = k_distinct_insert<kFnDepth, true>, name = "k_distinct_insert<kFnDepth, true>";
+    else if (has_fn(p.ps)) fn = k_distinct_insert<kFnDepth, false>, name = "k_distinct_insert<kFnDepth, false>";
+    else if (p.ps.has_nulls) fn = k_distinct_insert<8, true>, name = "k_distinct_insert<8, true>";
     else if (plain && !list && (begin & 1) == 0 && p.ps.ncols <= 2) fn = k_distinct_insert_plain<2>, name = "k_distinct_insert_plain<2>";
     else if (plain && !list && (begin & 1) == 0) fn = k_distinct_insert_plain<4>, name = "k_distinct_insert_plain<4>";
     else if (d <= 2) fn = k_distinct_insert<2, false>, name = "k_distinct_insert<2, false>";
@@ -2458,9 +2460,11 @@ void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
   if (p.naggs == 0) return;  // COUNT(DISTINCT) alone: nothing for the reduce kernels to do
   if (bp.has_pred) DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_PASSED, 0, 8, ctx->stream));
   const int d = p.ps.max_depth;
+  const bool fn = has_fn(p.ps);
   if (p.ps.has_nulls) {
     st->saw_nulls = true;
-    launch_reduce<8, true>(ctx, p, p.nrows);
+    if (fn) launch_reduce<kFnDepth, true>(ctx, p, p.nrows);
+    else launch_reduce<8, true>(ctx, p, p.nrows);
   } else {
     if (!bp.has_pred)
       for (int a = 0; a < st->naggs; a++) st->nonnull_host[size_t(a)] += p.nrows;
@@ -2482,7 +2486,8 @@ void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
       const int ps = ctx->prof_begin();
       launch_kernel(ctx, k_reduce_f64, "k_reduce_f64", rp, p.nrows, 256 * 8, 8);
       ctx->prof_end(ps);
-    } else if (d <= 1) launch_reduce<1>(ctx, p, p.nrows);
+    } else if (fn) launch_reduce<kFnDepth>(ctx, p, p.nrows);
+    else if (d <= 1) launch_reduce<1>(ctx, p, p.nrows);
     else if (d <= 2) launch_reduce<2>(ctx, p, p.nrows);
     else if (d <= 4) launch_reduce<4>(ctx, p, p.nrows);
     else launch_reduce<8>(ctx, p, p.nrows);
@@ -2531,10 +2536,14 @@ ScanPlan plan_scan(const dfgpu_aggstate* st, const BatchPrograms& bp, AggParams&
 // take the interpreter; FRONT routes rows through the shared-memory front table.  A lean launch gets its table
 // addresses in p.lean.
 ScanKernel choose_scan(const dfgpu_aggstate* st, AggParams& p, const ScanPlan& plan, bool replay, bool front) {
+  const bool fn = has_fn(p.ps);
   if (st->wide) {
+    if (fn && p.ps.has_nulls) return {k_hash_agg_wide<kFnDepth, true>, "k_hash_agg_wide<kFnDepth, true>", false};
+    if (fn) return {k_hash_agg_wide<kFnDepth, false>, "k_hash_agg_wide<kFnDepth, false>", false};
     if (p.ps.has_nulls) return {k_hash_agg_wide<8, true>, "k_hash_agg_wide<8, true>", false};
     return {k_hash_agg_wide<8, false>, "k_hash_agg_wide<8, false>", false};
   }
+  if (fn && p.ps.has_nulls) return {k_hash_agg<kFnDepth, false, true>, "k_hash_agg<kFnDepth, false, true>", false};
   if (p.ps.has_nulls) return {k_hash_agg<8, false, true>, "k_hash_agg<8, false, true>", false};
   const bool even = (p.row_begin & 1) == 0;
   if (plan.lean_mask && !replay && !front && !st->aos && even) {
@@ -2568,6 +2577,7 @@ ScanKernel choose_scan(const dfgpu_aggstate* st, AggParams& p, const ScanPlan& p
     return {k_hash_agg_plain<4, false>, "k_hash_agg_plain<4, false>", false};
   }
   const int d = p.ps.max_depth;
+  if (fn) return hash_agg_kernel<kFnDepth>(front);
   if (d <= 1) return hash_agg_kernel<1>(front);
   if (d <= 2) return hash_agg_kernel<2>(front);
   if (d <= 4) return hash_agg_kernel<4>(front);

@@ -21,12 +21,12 @@ MType mtype_of(int dt) {
 namespace {
 
 struct Node {
-  enum Kind { COL, LIT, CAST, BIN } kind = COL;
+  enum Kind { COL, LIT, CAST, BIN, FN } kind = COL;
   int col = 0;
   int dtype = 0;             // result dtype
   unsigned long long imm = 0;  // LIT payload, widened to the machine representation
-  int op = 0;                // DFGPU_OP_* for BIN
-  std::unique_ptr<Node> l, r;
+  int op = 0;                // DFGPU_OP_* for BIN, DFGPU_FN_* for FN
+  std::unique_ptr<Node> l, r;  // FN: the arguments (r: second argument of a two-argument function, else null)
 };
 
 const char* op_debug_name(int op) {
@@ -52,6 +52,14 @@ unsigned long long widen_literal(const dfgpu_insn& in) {
   }
   return 0;
 }
+
+// DFGPU_FN_* code -> name, nullptr for an unknown code; arity of a known code
+const char* fn_name(int code) {
+  static const char* const names[] = {nullptr, "sqrt", "abs", "floor", "ceil", "trunc", "round", "signum", "exp", "ln", "log2",
+                                      "log10", "sin", "cos", "tan", "asin", "acos", "atan", "power", "atan2"};
+  return code >= 1 && code <= DFGPU_FN_ATAN2 ? names[code] : nullptr;
+}
+int fn_arity(int code) { return code == DFGPU_FN_POWER || code == DFGPU_FN_ATAN2 ? 2 : 1; }
 
 VOp vop_of(int op) {
   switch (op) {
@@ -161,6 +169,27 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
         }
         break;
       }
+      case DFGPU_OP_FN: {  // Expr::ScalarFunction (logicalplan.rs:156-160), which the reference plans but never executes
+        const char* name = fn_name(in.col);
+        if (!name) fail(DFGPU_ERR_EXECUTION, "unknown scalar function code " + std::to_string(in.col));
+        const int arity = fn_arity(in.col);
+        if (int(st.size()) < arity)
+          fail(DFGPU_ERR_EXECUTION, std::string("function '") + name + "' takes " + std::to_string(arity) + (arity == 1 ? " argument" : " arguments"));
+        nd->kind = Node::FN;
+        nd->op = in.col;
+        nd->dtype = DFGPU_FLOAT64;
+        if (arity == 2) {
+          nd->r = std::move(st.back());
+          st.pop_back();
+        }
+        nd->l = std::move(st.back());
+        st.pop_back();
+        // monomorphic over Float64: the caller casts, as the planner does (sqlplanner.rs:343-365)
+        for (const Node* a : {nd->l.get(), nd->r.get()})
+          if (a && a->dtype != DFGPU_FLOAT64)
+            fail(DFGPU_ERR_EXECUTION, std::string("function '") + name + "' takes Float64 arguments, not " + dtype_name(a->dtype));
+        break;
+      }
       default: {
         int op = in.op;
         bool is_math = op >= DFGPU_OP_ADD && op <= DFGPU_OP_DIV;
@@ -202,6 +231,7 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
           case Node::COL: return b->cols[size_t(nd->col)].null_count > 0;
           case Node::LIT: return false;
           case Node::CAST: return go(nd->l.get());
+          case Node::FN: return go(nd->l.get()) || (nd->r && go(nd->r.get()));  // like arithmetic
           default: {
             const bool cmp = nd->op >= DFGPU_OP_EQ && nd->op <= DFGPU_OP_GE;
             return !cmp && (go(nd->l.get()) || go(nd->r.get()));
@@ -248,9 +278,25 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
           di.mtype = mtype_of(nd->l->dtype);
           cp->code.push_back(di);
           break;
+        case Node::FN:
+          if (!nd->r) {  // one argument: applied to the accumulator, like CAST
+            go(nd->l.get());
+            di.op = V_FN;
+            di.dtype = DFGPU_FLOAT64;
+            di.mtype = MT_F64;
+            di.aux = int16_t(nd->op);
+            cp->code.push_back(di);
+            break;
+          }
+          [[fallthrough]];
         case Node::BIN:
           go(nd->l.get());
-          di.op = vop_of(nd->op);
+          if (nd->kind == Node::FN) {
+            di.op = V_FN2;
+            di.aux = int16_t(nd->op);
+          } else {
+            di.op = vop_of(nd->op);
+          }
           di.dtype = uint8_t(nd->l->dtype);
           di.mtype = mtype_of(nd->l->dtype);
           if (nd->r->kind == Node::LIT) {
@@ -264,10 +310,11 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
             di.mode = RHS_STACK;
             // The evaluator keeps the TOP of the stack (here: the right operand) in its accumulator and
             // pops the operand below it as the second input, so a stack-mode instruction is emitted with
-            // its operands exchanged: reverse subtract / divide, mirrored comparisons.
+            // its operands exchanged: reverse subtract / divide / function, mirrored comparisons.
             switch (di.op) {
               case V_SUB: di.op = V_RSUB; break;
               case V_DIV: di.op = V_RDIV; break;
+              case V_FN2: di.op = V_RFN2; break;
               case V_LT: di.op = V_GT; break;
               case V_LE: di.op = V_GE; break;
               case V_GT: di.op = V_LT; break;

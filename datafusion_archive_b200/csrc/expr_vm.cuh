@@ -19,8 +19,16 @@ enum VOp : uint8_t {
   V_ADD, V_SUB, V_MUL, V_DIV,
   V_EQ, V_NE, V_LT, V_LE, V_GT, V_GE,
   V_AND, V_OR,
-  V_RSUB, V_RDIV  // operands exchanged (emitted for stack-mode instructions only, see expr_compile.cu)
+  V_RSUB, V_RDIV,  // operands exchanged (emitted for stack-mode instructions only, see expr_compile.cu)
+  // scalar functions (DFGPU_OP_FN), Float64 only, `aux` = DFGPU_FN_* code: V_FN applies a one-argument function to the
+  // accumulator like V_CAST, V_FN2 / V_RFN2 a two-argument one in any RhsMode (V_RFN2: operands exchanged)
+  V_FN, V_FN2, V_RFN2
 };
+// The interpreter kernels' DEPTH template argument is the register-stack depth (1, 2, 4 or 8), or kFnDepth for a program
+// set that contains V_FN* (has_fn below): depth 8 with the scalar functions compiled in.  Only kFnDepth
+// instantiations contain them, so the kernels that run function-free queries keep their code.
+constexpr int kFnDepth = 9;
+inline std::string depth_arg(int depth) { return depth == kFnDepth ? "kFnDepth" : std::to_string(depth); }
 enum RhsMode : uint8_t { RHS_STACK = 0, RHS_IMM = 1, RHS_COL = 2 };
 
 struct __align__(16) DevInsn {   // 16 bytes, lives in kernel parameter (constant) space
@@ -29,7 +37,7 @@ struct __align__(16) DevInsn {   // 16 bytes, lives in kernel parameter (constan
   uint8_t mtype;   // machine type of the operands (CAST: of the source)
   uint8_t dtype;   // Arrow dtype of the operands (int width for wrap-around); CAST: target dtype
   int16_t slot;    // column slot for PUSH_COL / RHS_COL
-  int16_t aux;     // CAST: source dtype
+  int16_t aux;     // CAST: source dtype; V_FN*: DFGPU_FN_* code
   unsigned long long imm;  // PUSH_IMM / RHS_IMM payload (raw bits, already widened)
 };
 
@@ -56,6 +64,13 @@ struct ProgramSet {
   int has_nulls; // some referenced column carries a validity bitmap: kernels use the NULLS evaluator
   uint8_t nullable[kMaxProgs];  // program result can be null (arrow 0.12 array_ops semantics)
 };
+// Some program of the set calls a scalar function (V_FN*): its kernels run with DEPTH = kFnDepth.  Read from the code rather
+// than stored, so that the kernel parameter blocks keep their layout.
+inline bool has_fn(const ProgramSet& ps) {
+  for (int pc = 0; pc < ps.start[ps.nprog]; pc++)
+    if (ps.insn[pc].op >= V_FN) return true;
+  return false;
+}
 
 // Interpreter-free shapes.  ProgramBuilder::add recognises them; the operators pass them to kernels that evaluate them
 // with straight-line code (same arithmetic as the interpreter, no decode in the inner loop).
@@ -341,6 +356,36 @@ __device__ __forceinline__ unsigned long long cast_value(unsigned long long v, i
   return norm_int(v, dst_dt);  // int -> int: truncate / extend (value already sign/zero extended)
 }
 
+// Built-in scalar function `fn` (DFGPU_FN_*) of x (and y), each the Rust f64 method of the same name.  Out of line, so the
+// code of the transcendentals, and the slow argument reduction of sin / cos / tan, is there once per module rather than
+// once per row at every call site.
+static __device__ __noinline__ double scalar_fn(int fn, double x, double y) {
+  switch (fn) {
+    case DFGPU_FN_SQRT: return sqrt(x);
+    case DFGPU_FN_ABS: return u2d(d2u(x) & 0x7fffffffffffffffull);  // clears the sign bit, NaN payloads included
+    case DFGPU_FN_FLOOR: return floor(x);
+    case DFGPU_FN_CEIL: return ceil(x);
+    case DFGPU_FN_TRUNC: return trunc(x);
+    case DFGPU_FN_ROUND: {  // half away from zero; x - trunc(x) is exact, so 0.49999999999999994 stays 0
+      const double t = trunc(x);
+      return fabs(x - t) >= 0.5 ? t + copysign(1.0, x) : t;
+    }
+    case DFGPU_FN_SIGNUM: return x != x ? x : copysign(1.0, x);  // by the sign bit: signum(-0.0) = -1.0
+    case DFGPU_FN_EXP: return exp(x);
+    case DFGPU_FN_LN: return log(x);
+    case DFGPU_FN_LOG2: return log2(x);
+    case DFGPU_FN_LOG10: return log10(x);
+    case DFGPU_FN_SIN: return sin(x);
+    case DFGPU_FN_COS: return cos(x);
+    case DFGPU_FN_TAN: return tan(x);
+    case DFGPU_FN_ASIN: return asin(x);
+    case DFGPU_FN_ACOS: return acos(x);
+    case DFGPU_FN_ATAN: return atan(x);
+    case DFGPU_FN_POWER: return pow(x, y);
+    default: return atan2(x, y);  // DFGPU_FN_ATAN2; the compiler accepts no other code
+  }
+}
+
 // Evaluate program `prog` of `ps` for the R rows described by `src` (GlobalRows / StagedTile).
 // Returns the value stack top in out[]; bit r of the return value is set when valid row r divided
 // by zero.  With F64ONLY every operand is Float64/Boolean (checked on the host): the machine-type
@@ -361,7 +406,9 @@ __device__ __forceinline__ unsigned eval_program_n(const ProgramSet& ps, int pro
   // stack-mode instruction R loads (its operands were exchanged at lowering so that the accumulator is
   // always the left input).
   constexpr unsigned ALL = (1u << R) - 1u;
-  constexpr int SPILL = DEPTH > 1 ? DEPTH - 1 : 1;
+  constexpr bool FN = DEPTH == kFnDepth;  // the scalar-function cases are compiled in
+  constexpr int D = FN ? 8 : DEPTH;
+  constexpr int SPILL = D > 1 ? D - 1 : 1;
   unsigned long long spill[SPILL][R];
   unsigned spillv[SPILL];
   unsigned accv = ALL;
@@ -379,8 +426,44 @@ __device__ __forceinline__ unsigned eval_program_n(const ProgramSet& ps, int pro
     const int dt = (raw.x >> 24) & 0xff;
     const int slot = (int)(short)(raw.y & 0xffff);
     const unsigned long long imm = ((unsigned long long)raw.w << 32) | raw.z;
+    if constexpr (FN) {  // discarded in every other instantiation, which therefore keeps its code
+      if (op >= V_FN) {
+        // scalar function: Float64 in, Float64 out; a row is null where an argument is, with value 0 (like arithmetic)
+        const int fn = (int)(short)(raw.y >> 16);
+        unsigned valid = accv;
+        if (op == V_FN) {  // one argument: the accumulator
+#pragma unroll
+          for (int r = 0; r < R; r++) out[r] = d2u(scalar_fn(fn, u2d(out[r]), 0.0));
+        } else {  // two arguments, right one as in the binary ops below; V_RFN2: the accumulator is the right argument
+          unsigned long long y[R];
+          if (mode == RHS_IMM) {
+#pragma unroll
+            for (int r = 0; r < R; r++) y[r] = imm;
+          } else if (mode == RHS_COL) {
+            src.load_rows(ps, slot, y);
+            if (NULLS) valid &= src.col_valid(ps, slot);
+          } else {
+            depth--;
+            const int d = depth - 1 >= 0 ? (depth - 1 < SPILL ? depth - 1 : SPILL - 1) : 0;
+#pragma unroll
+            for (int r = 0; r < R; r++) y[r] = spill[d][r];
+            if (NULLS) valid &= spillv[d];
+          }
+          const bool swap = op == V_RFN2;
+#pragma unroll
+          for (int r = 0; r < R; r++) out[r] = d2u(scalar_fn(fn, u2d(swap ? y[r] : out[r]), u2d(swap ? out[r] : y[r])));
+        }
+        if (NULLS) {
+#pragma unroll
+          for (int r = 0; r < R; r++)
+            if (!((valid >> r) & 1u)) out[r] = 0ull;
+          accv = valid;
+        }
+        continue;
+      }
+    }
     if (op <= V_PUSH_ROWID) {
-      if (DEPTH > 1 && depth > 0) {  // spill the current top
+      if (D > 1 && depth > 0) {  // spill the current top
         const int d = depth - 1 < SPILL ? depth - 1 : SPILL - 1;
 #pragma unroll
         for (int r = 0; r < R; r++) spill[d][r] = out[r];

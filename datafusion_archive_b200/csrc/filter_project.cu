@@ -198,7 +198,7 @@ static void launch_fp(dfgpu_ctx* ctx, const FPParams& p) {
   const int ps = ctx->prof_begin();
   k_filter_project<DEPTH, NULLS><<<(unsigned)grid, FP_THREADS, 0, ctx->stream>>>(p);
   DF_CUDA(cudaGetLastError());
-  static const std::string name = "k_filter_project<" + std::to_string(DEPTH) + (NULLS ? ", true>" : ", false>");
+  static const std::string name = "k_filter_project<" + depth_arg(DEPTH) + (NULLS ? ", true>" : ", false>");
   trace_launch(name.c_str());
   ctx->prof_end(ps);
   ctx->launches++;
@@ -392,13 +392,17 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
     }
     p.pred_fast = has_pred ? pb.prog(0).chain : LeafChain{};
     for (int i = 0; i < nkern; i++) p.proj_fast[i] = pb.prog(i + has_pred).leaf;
+    const bool fn = has_fn(p.ps);
     if (p.ps.has_nulls) {
       p.ntiles = int((n + FP_TILE - 1) / FP_TILE);
-      launch_fp<8, true>(ctx, p);  // the null-aware evaluator lives in the direct kernel only
+      // the null-aware evaluator lives in the direct kernel only
+      if (fn) launch_fp<kFnDepth, true>(ctx, p);
+      else launch_fp<8, true>(ctx, p);
     } else if (ctx->force_direct_kernel || !launch_fp_tma(ctx, p)) {
       p.ntiles = int((n + FP_TILE - 1) / FP_TILE);
       const int d = p.ps.max_depth;
-      if (d <= 1) launch_fp<1>(ctx, p);
+      if (fn) launch_fp<kFnDepth>(ctx, p);
+      else if (d <= 1) launch_fp<1>(ctx, p);
       else if (d <= 2) launch_fp<2>(ctx, p);
       else if (d <= 4) launch_fp<4>(ctx, p);
       else launch_fp<8>(ctx, p);

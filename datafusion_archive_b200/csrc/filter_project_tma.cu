@@ -778,7 +778,7 @@ static void launch_one(dfgpu_ctx* ctx, const FPParams& p, size_t smem) {
   // cooperative launch: the wave-synchronous scan needs every CTA of the grid resident at once
   void* args[] = {(void*)&p};
   DF_CUDA(cudaLaunchCooperativeKernel((const void*)kern, dim3((unsigned)grid), dim3(TM_THREADS), args, smem, ctx->stream));
-  static const std::string name = "k_filter_project_tma<" + std::to_string(DEPTH) + ", " + std::to_string(K) + (F64ONLY ? ", true" : ", false") +
+  static const std::string name = "k_filter_project_tma<" + depth_arg(DEPTH) + ", " + std::to_string(K) + (F64ONLY ? ", true" : ", false") +
                                   (FAST ? ", true, " : ", false, ") + std::to_string(LEAN) + ">";
   trace_launch(name.c_str());
   ctx->prof_end(ps);
@@ -839,7 +839,11 @@ bool launch_fp_tma(dfgpu_ctx* ctx, FPParams& p) {
     const int k = atoi(e);
     if ((k == 8 || k == 4 || k == 2) && (long long)TM_CWARPS * 32 * k * (rowA + rowB) * 2 <= TM_SMEM_BUDGET && !(k == 8 && p.ps.max_depth > 2)) K = k;
   }
-  if (!K) return false;
+  // program sets with scalar functions take one tile shape, 4 rows per lane: K = 8 holds too many live rows across the
+  // function calls, and a set whose columns leave room for 2 rows only takes the direct kernel
+  const bool fn = has_fn(p.ps);
+  if (fn && K == 8) K = 4;
+  if (!K || (fn && K != 4)) return false;
   const int tile = TM_CWARPS * 32 * K;
   int offA = 0, offB = 0;
   for (int c = 0; c < p.ps.ncols; c++) {
@@ -891,7 +895,10 @@ bool launch_fp_tma(dfgpu_ctx* ctx, FPParams& p) {
   p.ntiles = int((p.nrows + tile - 1) / tile);
   const size_t smem = TM_HDR_BYTES + (size_t)p.nstagesA * p.stage_bytesA + (size_t)p.nstagesB * p.stage_bytesB;
   const int d = p.ps.max_depth;
-  if (K == 8) launch_k<2, 8>(ctx, p, smem);
+  if (fn) {
+    if (p.ps.f64_only) launch_one<kFnDepth, 4, true, false>(ctx, p, smem);
+    else launch_one<kFnDepth, 4, false, false>(ctx, p, smem);
+  } else if (K == 8) launch_k<2, 8>(ctx, p, smem);
   else if (K == 4) { if (d <= 2) launch_k<2, 4>(ctx, p, smem); else launch_k<4, 4>(ctx, p, smem); }
   else { if (d <= 2) launch_k<2, 2>(ctx, p, smem); else launch_k<4, 2>(ctx, p, smem); }
   return true;

@@ -28,13 +28,15 @@ int guarded(Fn&& fn) {
 struct Catalog : SchemaProvider {
   std::map<std::string, SchemaRef> tables;
   std::map<std::string, std::shared_ptr<FunctionMeta>> functions;
+  bool builtins = false;  // dfhost_catalog_add_builtin_functions: ExecutionContext's catalogue, behind `functions`
   SchemaRef get_table_meta(const std::string& name) const override {
     auto it = tables.find(name);
     return it == tables.end() ? nullptr : it->second;
   }
   std::shared_ptr<FunctionMeta> get_function_meta(const std::string& name) const override {
     auto it = functions.find(name);
-    return it == functions.end() ? nullptr : it->second;
+    if (it != functions.end()) return it->second;
+    return builtins ? builtin_function_meta(name) : nullptr;
   }
 };
 
@@ -77,6 +79,7 @@ int dfhost_catalog_add_function(dfhost_catalog* c, const char* name, int nargs, 
     c->c->functions[name] = fm;
   });
 }
+int dfhost_catalog_add_builtin_functions(dfhost_catalog* c) { return guarded([&] { c->c->builtins = true; }); }
 // SQL -> `format!("{:?}", plan)` of the reference's LogicalPlan
 int dfhost_plan_sql(dfhost_catalog* c, const char* sql, char** out_debug) {
   return guarded([&] {

@@ -197,6 +197,41 @@ std::optional<RecordBatch> MemoryDataSource::next() {
   return b;
 }
 
+// ---- built-in scalar functions ---------------------------------------------------------------------------
+const std::vector<BuiltinFunction>& builtin_functions() {
+  static const std::vector<BuiltinFunction> table = {
+      {"sqrt", DFGPU_FN_SQRT, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},     {"abs", DFGPU_FN_ABS, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
+      {"floor", DFGPU_FN_FLOOR, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},   {"ceil", DFGPU_FN_CEIL, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
+      {"trunc", DFGPU_FN_TRUNC, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},   {"round", DFGPU_FN_ROUND, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
+      {"signum", DFGPU_FN_SIGNUM, 1, DFGPU_FLOAT64, DFGPU_FLOAT64}, {"exp", DFGPU_FN_EXP, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
+      {"ln", DFGPU_FN_LN, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},         {"log2", DFGPU_FN_LOG2, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
+      {"log10", DFGPU_FN_LOG10, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},   {"sin", DFGPU_FN_SIN, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
+      {"cos", DFGPU_FN_COS, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},       {"tan", DFGPU_FN_TAN, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
+      {"asin", DFGPU_FN_ASIN, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},     {"acos", DFGPU_FN_ACOS, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
+      {"atan", DFGPU_FN_ATAN, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},     {"power", DFGPU_FN_POWER, 2, DFGPU_FLOAT64, DFGPU_FLOAT64},
+      {"atan2", DFGPU_FN_ATAN2, 2, DFGPU_FLOAT64, DFGPU_FLOAT64},
+  };
+  return table;
+}
+
+const BuiltinFunction* find_builtin_function(const std::string& name) {
+  std::string n = name;
+  for (auto& c : n) c = char(tolower((unsigned char)c));
+  for (const auto& f : builtin_functions())
+    if (n == f.name) return &f;
+  return nullptr;
+}
+
+std::shared_ptr<FunctionMeta> builtin_function_meta(const std::string& name) {
+  const BuiltinFunction* f = find_builtin_function(name);
+  if (!f) return nullptr;
+  auto fm = std::make_shared<FunctionMeta>();
+  fm->name = f->name;
+  for (int i = 0; i < f->arity; i++) fm->args.push_back(Field{"n", f->arg_type, false});
+  fm->return_type = f->return_type;
+  return fm;
+}
+
 // ---- Expr -> postfix program of the C ABI -------------------------------------------------------------
 namespace {
 
@@ -262,6 +297,20 @@ void lower(const Expr& e, const Schema& schema, const std::map<size_t, int>& rem
         case Operator::Divide: in.op = DFGPU_OP_DIV; break;
         default: fail(DFGPU_ERR_EXECUTION, std::string("operator: ") + operator_debug(e.op));  // expression.rs:494-497
       }
+      out.push_back(in);
+      return;
+    }
+    case Expr::ScalarFunction: {
+      const BuiltinFunction* f = find_builtin_function(e.name);
+      if (!f) fail(DFGPU_ERR_GENERAL, "Invalid function '" + e.name + "'");
+      // the planner rejects extra arguments but not missing ones
+      if (e.args.size() != size_t(f->arity))
+        fail(DFGPU_ERR_EXECUTION, "function '" + e.name + "' takes " + std::to_string(f->arity) + (f->arity == 1 ? " argument" : " arguments") +
+                                      ", got " + std::to_string(e.args.size()));
+      for (auto& a : e.args) lower(*a, schema, remap, out);
+      in.op = DFGPU_OP_FN;
+      in.col = f->code;
+      in.dtype = f->return_type;
       out.push_back(in);
       return;
     }
@@ -616,9 +665,8 @@ struct ContextSchemaProvider : SchemaProvider {  // context.rs:244-258
     auto it = datasources->find(name);
     return it == datasources->end() ? nullptr : it->second->schema();
   }
-  std::shared_ptr<FunctionMeta> get_function_meta(const std::string&) const override {
-    fail(DFGPU_ERR_NOT_IMPLEMENTED, "scalar functions are not registered with ExecutionContext (reference: unimplemented!() at context.rs:255-257)");
-  }
+  // the built-in catalogue; the reference has unimplemented!() here (context.rs:255-257)
+  std::shared_ptr<FunctionMeta> get_function_meta(const std::string& name) const override { return builtin_function_meta(name); }
 };
 }  // namespace
 

@@ -159,6 +159,20 @@ class ExecutionContext {
   int rank_ = 0, world_ = 1;
 };
 
+// ---- built-in scalar functions ---------------------------------------------------------------------------
+// The catalogue of functions ExecutionContext plans and runs on the GPU (DFGPU_OP_FN of include/dfgpu.h).  The reference
+// only plans Expr::ScalarFunction; its console registers one `sqrt` UDF (src/bin/console/main.rs:123-125).  No function
+// can be registered by the user: the GPU cannot run an arbitrary closure.
+struct BuiltinFunction {
+  const char* name;  // lower case; SQL names match in any letter case
+  int code;          // DFGPU_FN_*
+  int arity;
+  DataType arg_type, return_type;
+};
+const std::vector<BuiltinFunction>& builtin_functions();
+const BuiltinFunction* find_builtin_function(const std::string& name);      // nullptr for an unknown name
+std::shared_ptr<FunctionMeta> builtin_function_meta(const std::string& name);  // FunctionMeta for the planner, or nullptr
+
 // Expr name as RuntimeExpr::get_name reports it (expression.rs:230,312,322,407)
 std::string runtime_expr_name(const Expr& e, const Schema& input_schema);
 

@@ -128,6 +128,28 @@ class BinaryExpr(Expr):
         return "%r %s %r" % (self.left, _OPNAME[self.op], self.right)
 
 
+class ScalarFunction(Expr):
+    """Expr::ScalarFunction{name,args,return_type} (src/logicalplan.rs:156-160) for a built-in function: Float64
+    arguments, Float64 result.  Like the C ABI, it casts nothing; cast integer arguments with `.cast(A.FLOAT64)`."""
+
+    def __init__(self, name, *args):
+        self.name, self.args = name, [_wrap(a) for a in args]
+        self.code = A.FN_CODES[name.lower()]
+
+    def get_type(self, schema):
+        return A.FLOAT64
+
+    def _emit(self, schema, out):
+        for a in self.args:
+            a._emit(schema, out)
+        i = A.Insn()
+        i.op, i.col, i.dtype = A.OP_FN, self.code, A.FLOAT64
+        out.append(i)
+
+    def __repr__(self):
+        return "%s(%s)" % (self.name, ", ".join(repr(a) for a in self.args))
+
+
 class AggregateFunction:
     """Expr::AggregateFunction{name,args,return_type} (src/logicalplan.rs:162-166)."""
 
@@ -162,6 +184,10 @@ def col(i):
 
 def lit(v, dtype=None):
     return Literal(v, dtype)
+
+
+def fn(name, *args):
+    return ScalarFunction(name, *args)
 
 
 def f64_bits(x):

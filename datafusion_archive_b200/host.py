@@ -47,6 +47,7 @@ def lib():
         L.dfhost_catalog_free.argtypes = [vp]
         L.dfhost_catalog_add_table.argtypes = [vp, cp, C.c_int, C.POINTER(cp), C.POINTER(C.c_int32)]
         L.dfhost_catalog_add_function.argtypes = [vp, cp, C.c_int, C.POINTER(C.c_int32), C.c_int32]
+        L.dfhost_catalog_add_builtin_functions.argtypes = [vp]
         L.dfhost_plan_sql.argtypes = [vp, cp, C.POINTER(vp)]
         L.dfhost_supertype.argtypes = [C.c_int32, C.c_int32, C.POINTER(C.c_int32)]
         L.dfhost_debug_f64.argtypes = [C.c_double, C.POINTER(vp)]
@@ -103,6 +104,10 @@ class Catalog:
     def add_function(self, name, arg_dtypes, return_dtype):
         args = (C.c_int32 * len(arg_dtypes))(*arg_dtypes)
         _check(lib().dfhost_catalog_add_function(self.h, name.encode(), len(arg_dtypes), args, return_dtype))
+
+    def add_builtin_functions(self):
+        """The built-in scalar functions ExecutionContext plans and runs (sqrt, abs, power, ...)."""
+        _check(lib().dfhost_catalog_add_builtin_functions(self.h))
 
     def plan(self, sql):
         """`format!("{:?}", plan)` of the logical plan for `sql`."""

@@ -97,7 +97,38 @@ enum {
   DFGPU_OP_GT = 24,  /* array_ops::gt      expression.rs:438 */
   DFGPU_OP_GE = 25,  /* array_ops::gt_eq   expression.rs:445 */
   DFGPU_OP_AND = 30, /* array_ops::and     expression.rs:452 */
-  DFGPU_OP_OR = 31   /* array_ops::or      expression.rs:459 */
+  DFGPU_OP_OR = 31,  /* array_ops::or      expression.rs:459 */
+  DFGPU_OP_FN = 40   /* Expr::ScalarFunction{name,args,return_type} logicalplan.rs:156-160: `col` = DFGPU_FN_* code,
+                        `dtype` = Float64; the arguments come first, in order.  Additive: libraries older than it
+                        reject it with "operator: 40". */
+};
+
+/* Built-in scalar functions (DFGPU_OP_FN).  The reference declares Expr::ScalarFunction and plans it
+ * (sqlplanner.rs:343-365: every argument cast to the declared type) but never executes it
+ * (context.rs:255-257 unimplemented!()).  Every function takes Float64 arguments and returns Float64; a
+ * caller of this ABI inserts the CASTs, as the planner does.  Each value follows the Rust f64 method named
+ * beside it, since a reference UDF is a Rust closure; a row is null where an argument is null.  No
+ * function raises an error: domain errors give NaN or +-inf. */
+enum {
+  DFGPU_FN_SQRT = 1,   /* f64::sqrt   */
+  DFGPU_FN_ABS = 2,    /* f64::abs    */
+  DFGPU_FN_FLOOR = 3,  /* f64::floor  */
+  DFGPU_FN_CEIL = 4,   /* f64::ceil   */
+  DFGPU_FN_TRUNC = 5,  /* f64::trunc  */
+  DFGPU_FN_ROUND = 6,  /* f64::round: half away from zero */
+  DFGPU_FN_SIGNUM = 7, /* f64::signum: +-1.0 by the sign bit, NaN for NaN */
+  DFGPU_FN_EXP = 8,    /* f64::exp    */
+  DFGPU_FN_LN = 9,     /* f64::ln     */
+  DFGPU_FN_LOG2 = 10,  /* f64::log2   */
+  DFGPU_FN_LOG10 = 11, /* f64::log10  */
+  DFGPU_FN_SIN = 12,   /* f64::sin    */
+  DFGPU_FN_COS = 13,   /* f64::cos    */
+  DFGPU_FN_TAN = 14,   /* f64::tan    */
+  DFGPU_FN_ASIN = 15,  /* f64::asin   */
+  DFGPU_FN_ACOS = 16,  /* f64::acos   */
+  DFGPU_FN_ATAN = 17,  /* f64::atan   */
+  DFGPU_FN_POWER = 18, /* f64::powf(x, y), two arguments */
+  DFGPU_FN_ATAN2 = 19  /* f64::atan2(y, x), two arguments */
 };
 
 typedef struct dfgpu_insn {
@@ -185,7 +216,8 @@ int dfgpu_batch_free(dfgpu_batch* b);
  * Type-check one expression program against a schema (`col_dtypes[i]` = dtype of column i) exactly as
  * dfgpu_filter_project / dfgpu_aggregate_update would before launching anything, without touching a
  * GPU: identical operand dtypes ("math_ops" / "comparison_ops"), Boolean operands for AND / OR, the CAST
- * rules, column indices.  `out_dtype` receives the result type.  Usable on a machine with no device. */
+ * rules, Float64 arguments and the arity of DFGPU_OP_FN, column indices.  `out_dtype` receives the result
+ * type.  Usable on a machine with no device. */
 int dfgpu_check_program(const int32_t* col_dtypes, int ncols, const dfgpu_insn* prog, int prog_len, int32_t* out_dtype);
 
 /* ---- FilterRelation + ProjectRelation fused (src/execution/filter.rs:46-110,

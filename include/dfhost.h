@@ -36,6 +36,9 @@ int dfhost_catalog_new(dfhost_catalog** out);
 void dfhost_catalog_free(dfhost_catalog* c);
 int dfhost_catalog_add_table(dfhost_catalog* c, const char* name, int ncols, const char* const* names, const int32_t* dtypes);
 int dfhost_catalog_add_function(dfhost_catalog* c, const char* name, int nargs, const int32_t* arg_dtypes, int32_t return_dtype);
+/* the built-in scalar functions ExecutionContext plans and runs (sqrt, abs, power, ...: DFGPU_FN_* of dfgpu.h), matched in
+ * any letter case; functions added by name take precedence */
+int dfhost_catalog_add_builtin_functions(dfhost_catalog* c);
 int dfhost_plan_sql(dfhost_catalog* c, const char* sql, char** out_debug);
 int dfhost_supertype(int32_t l, int32_t r, int32_t* out); /* get_supertype; *out = 0 when there is none */
 int dfhost_debug_f64(double x, char** out);               /* format!("{:?}", x) */

@@ -41,6 +41,29 @@ pub const OP_GT: i32 = 24;
 pub const OP_GE: i32 = 25;
 pub const OP_AND: i32 = 30;
 pub const OP_OR: i32 = 31;
+/// Expr::ScalarFunction of a built-in function: `col` = FN_* code, `dtype` = Float64, arguments first.
+pub const OP_FN: i32 = 40;
+
+// built-in scalar functions (DFGPU_FN_*): Float64 arguments, Float64 result, each the Rust f64 method of the same name
+pub const FN_SQRT: i32 = 1;
+pub const FN_ABS: i32 = 2;
+pub const FN_FLOOR: i32 = 3;
+pub const FN_CEIL: i32 = 4;
+pub const FN_TRUNC: i32 = 5;
+pub const FN_ROUND: i32 = 6;
+pub const FN_SIGNUM: i32 = 7;
+pub const FN_EXP: i32 = 8;
+pub const FN_LN: i32 = 9;
+pub const FN_LOG2: i32 = 10;
+pub const FN_LOG10: i32 = 11;
+pub const FN_SIN: i32 = 12;
+pub const FN_COS: i32 = 13;
+pub const FN_TAN: i32 = 14;
+pub const FN_ASIN: i32 = 15;
+pub const FN_ACOS: i32 = 16;
+pub const FN_ATAN: i32 = 17;
+pub const FN_POWER: i32 = 18;
+pub const FN_ATAN2: i32 = 19;
 
 // aggregate functions (src/execution/expression.rs:32-39 AggregateType)
 pub const AGG_MIN: i32 = 1;

@@ -65,6 +65,19 @@ fn op_code(op: &Operator) -> Result<i32> {
     })
 }
 
+/// The built-in scalar functions: (name, FN_* code, arity).  Names match in any letter case.
+pub const BUILTIN_FUNCTIONS: &[(&str, i32, usize)] = &[
+    ("sqrt", FN_SQRT, 1), ("abs", FN_ABS, 1), ("floor", FN_FLOOR, 1), ("ceil", FN_CEIL, 1), ("trunc", FN_TRUNC, 1),
+    ("round", FN_ROUND, 1), ("signum", FN_SIGNUM, 1), ("exp", FN_EXP, 1), ("ln", FN_LN, 1), ("log2", FN_LOG2, 1),
+    ("log10", FN_LOG10, 1), ("sin", FN_SIN, 1), ("cos", FN_COS, 1), ("tan", FN_TAN, 1), ("asin", FN_ASIN, 1),
+    ("acos", FN_ACOS, 1), ("atan", FN_ATAN, 1), ("power", FN_POWER, 2), ("atan2", FN_ATAN2, 2),
+];
+
+/// (FN_* code, arity) of a built-in function
+pub fn builtin_function(name: &str) -> Option<(i32, usize)> {
+    BUILTIN_FUNCTIONS.iter().find(|f| f.0.eq_ignore_ascii_case(name)).map(|f| (f.1, f.2))
+}
+
 /// `remap[i]` = index of input column i among the columns actually uploaded (pruned to the referenced ones).
 pub fn lower(e: &Expr, schema: &Schema, remap: &[Option<usize>], out: &mut Vec<dfgpu_insn>) -> Result<()> {
     match e {
@@ -85,6 +98,17 @@ pub fn lower(e: &Expr, schema: &Schema, remap: &[Option<usize>], out: &mut Vec<d
             lower(left, schema, remap, out)?;
             lower(right, schema, remap, out)?;
             out.push(insn(op_code(op)?, 0, dtype_code(&left.get_type(schema)).unwrap_or(0), 0));
+        }
+        Expr::ScalarFunction { name, args, .. } => {
+            let (code, arity) = builtin_function(name).ok_or_else(|| ExecutionError::General(format!("Invalid function '{}'", name)))?;
+            if args.len() != arity {
+                // the planner rejects extra arguments but not missing ones
+                return Err(ExecutionError::ExecutionError(format!("function '{}' takes {} argument(s), got {}", name, arity, args.len())));
+            }
+            for a in args {
+                lower(a, schema, remap, out)?;
+            }
+            out.push(insn(OP_FN, code, DT_FLOAT64, 0));
         }
         other => return Err(ExecutionError::ExecutionError(format!("expression {:?}", other))), // expression.rs:500-503
     }
