@@ -42,6 +42,29 @@ struct AggDesc {
   uint8_t out_dtype;
 };
 
+__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
+  x ^= x >> 33; x *= 0xff51afd7ed558ccdull;
+  x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull;
+  x ^= x >> 33;
+  return x;
+}
+
+// Capacity and probe sequence of the group table and of the COUNT(DISTINCT) pair sets: cap slots (a power of two), a
+// hash's home slot is its TOP log2(cap) bits, and probing steps linearly, wrapping at cap.  The host fills both fields
+// (set_cap); every kernel that places or looks up a key goes through home() and next().
+struct ProbeRule {
+  long long cap;
+  int hshift;  // 64 - log2(cap)
+  __host__ void set_cap(long long c) {
+    int lg = 0;
+    while ((1ll << lg) < c) lg++;
+    cap = c;
+    hshift = 64 - lg;
+  }
+  __device__ __forceinline__ unsigned long long home(unsigned long long hash) const { return hshift >= 64 ? 0ull : hash >> hshift; }
+  __device__ __forceinline__ unsigned long long next(unsigned long long slot) const { return (slot + 1ull) & ((unsigned long long)cap - 1ull); }
+};
+
 // Table addressing.  A slot is a LINE of lw 64-bit words (lw a power of two; word 0 = the packed key) plus
 // one word in each of n_add separate arrays.  loc[a] says where accumulator a lives: >= 1 = that word of
 // the line, < 0 = additive array ~loc[a].  Three layouts fall out of it:
@@ -56,7 +79,8 @@ struct AggDesc {
 //           and three reductions.
 //   line    every accumulator in the line (lw >= 1 + naggs): one sector per group; wins once the table no
 //           longer fits L2 and every touched sector is an HBM transaction.
-struct TableLayout {
+// cap + 1 slots: slot cap is reserved for the key that equals EMPTY_KEY.  The table without GROUP BY has cap = 0.
+struct TableLayout : ProbeRule {
   unsigned long long* base;  // (cap + 1) lines of lw words
   unsigned long long* add;   // n_add arrays of (cap + 1) words
   long long lw, astride;
@@ -66,6 +90,24 @@ struct TableLayout {
     const int l = loc[a];
     return l >= 0 ? base + slot * lw + l : add + (long long)(~l) * astride + slot;
   }
+  // The slot of key k, which is in the table unless the table is inconsistent: cap for EMPTY_KEY when the sentinel slot
+  // is in use, -1 when the key is missing.  At most cap probes.
+  __device__ __forceinline__ long long find(unsigned long long k, bool sentinel_used) const {
+    if (k == EMPTY_KEY) return sentinel_used ? cap : -1;
+    unsigned long long h = home(mix64(k));
+    for (long long probes = 0; probes < cap; probes++) {
+      const unsigned long long cur = __ldcg(key((long long)h));
+      if (cur == k) return (long long)h;
+      if (cur == EMPTY_KEY) return -1;
+      h = next(h);
+    }
+    return -1;
+  }
+};
+
+// A COUNT(DISTINCT) pair set: cap slots of two words.
+struct SetView : ProbeRule {
+  unsigned long long* slots;
 };
 
 // plain-column fast path (k_hash_agg_plain): every key and aggregate argument is a plain column of the (at most 4)
@@ -102,9 +144,7 @@ struct AggParams {
   long long row_begin;       // process rows [row_begin, row_begin + nrows) of the batch
   const unsigned* row_list;  // non-null: process rows row_list[0..nlist) (overflow replay)
   long long nlist;
-  // cap+1 slots; slot cap is reserved for the key that equals EMPTY_KEY
   TableLayout t;
-  long long cap;             // power of two
   long long max_groups;      // new keys are refused (-> overflow list) beyond this fill
   unsigned long long* counters;  // CTR_SLOTS words, see CTR_*
   unsigned* ovf_rows;
@@ -224,7 +264,7 @@ __device__ __forceinline__ void acc_merge_global(int func, int mt, unsigned long
     default: atomicMax(p, b); break;
   }
 }
-// fold one raw value into global memory
+// fold one raw value into global or shared memory
 __device__ __forceinline__ void acc_fold_global(int func, int mt, unsigned long long* p, unsigned long long v) {
   switch (func) {
     case DFGPU_AGG_SUM:
@@ -242,20 +282,6 @@ __device__ __forceinline__ void acc_fold_global(int func, int mt, unsigned long 
   }
 }
 
-// Home slot of a key = the TOP log2(cap) bits of its hash.
-__host__ __device__ __forceinline__ int hash_shift(long long cap) {
-  int lg = 0;
-  while ((1ll << lg) < cap) lg++;
-  return 64 - lg;
-}
-__device__ __forceinline__ unsigned long long home_slot(unsigned long long hash, int hshift) { return hshift >= 64 ? 0ull : hash >> hshift; }
-__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
-  x ^= x >> 33; x *= 0xff51afd7ed558ccdull;
-  x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull;
-  x ^= x >> 33;
-  return x;
-}
-
 // One table line as read by a probe: word 0 = key, words 1..3 = the accumulators that share the line.
 struct Line {
   unsigned long long w[4];
@@ -268,44 +294,52 @@ __device__ __forceinline__ void load_line4(const unsigned long long* q, Line& ln
   asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln.w[0]), "=l"(ln.w[1]) : "l"(q) : "memory");
   asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln.w[2]), "=l"(ln.w[3]) : "l"(q + 2) : "memory");
 }
-template <bool WITH_VALS>
-__device__ __forceinline__ void load_line(const TableLayout& t, long long slot, Line& ln) {
-  const unsigned long long* q = t.key(slot);
-  if (WITH_VALS && t.lw >= 4) {  // lines are 32-byte aligned
+// What a probe loads at a slot: LW > 0 = the first words of lines LW words apart, LW known at compile time (the lean
+// scan, whose words past the line are never read); LINE_RT = up to 4 words of the table's lw-word lines (the generic
+// scan: the probe also returns the in-line MIN / MAX); LINE_KEY = the key word alone (merges).
+constexpr int LINE_RT = 0, LINE_KEY = -1;
+template <int LW>
+__device__ __forceinline__ unsigned long long* line_at(const TableLayout& t, unsigned long long slot) {
+  return LW > 0 ? t.base + slot * LW : t.key((long long)slot);
+}
+template <int LW>
+__device__ __forceinline__ void load_line(const TableLayout& t, unsigned long long slot, Line& ln) {
+  const unsigned long long* q = line_at<LW>(t, slot);
+  const long long w = LW > 0 ? LW : (LW == LINE_RT ? t.lw : 1);
+  if (w >= 4) {  // lines are 32-byte aligned
     load_line4(q, ln);
-  } else if (WITH_VALS && t.lw == 2) {
+  } else if (w == 2) {
     asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln.w[0]), "=l"(ln.w[1]) : "l"(q) : "memory");
-    ln.w[2] = ln.w[3] = 0ull;
+    if (LW <= 0) ln.w[2] = ln.w[3] = 0ull;
   } else {
     asm volatile("ld.global.cg.u64 %0, [%1];" : "=l"(ln.w[0]) : "l"(q) : "memory");
-    ln.w[1] = ln.w[2] = ln.w[3] = 0ull;
+    if (LW <= 0) ln.w[1] = ln.w[2] = ln.w[3] = 0ull;
   }
 }
 __device__ __forceinline__ unsigned long long line_word(const Line& ln, int l) {
   return l == 1 ? ln.w[1] : (l == 2 ? ln.w[2] : ln.w[3]);
 }
 
-// Find the slot of `key`, claiming an empty one when the key is new.  `ln` is the line read at the home
-// slot h on entry and the line of the returned slot on exit (as it was when this thread read it: a slot
-// claimed meanwhile still shows its initial accumulator identities, which is what the conditional
-// MIN / MAX update needs).  Returns -1 when the key is new and the table refuses new keys (fill limit /
+// Find the slot of `key`, claiming an empty one when the key is new.  `h` is the home slot on entry and the key's slot
+// on exit; `ln` is the line read at h on entry and the line of the key's slot on exit (as it was when this thread read
+// it: a slot claimed meanwhile still shows its initial accumulator identities, which is what the conditional
+// MIN / MAX update needs).  Returns false when the key is new and the table refuses new keys (fill limit /
 // probe limit): the row goes to the overflow list.
-template <bool WITH_VALS>
-__device__ __forceinline__ long long probe_insert(const TableLayout& t, long long cap, unsigned long long key, Line& ln,
-                                                  unsigned long long h, bool full, unsigned& new_groups) {
-  const unsigned long long mask = (unsigned long long)cap - 1ull;
+template <int LW>
+__device__ __forceinline__ bool probe_insert(const TableLayout& t, unsigned long long key, Line& ln, unsigned long long& h, bool full,
+                                             unsigned& new_groups) {
   for (int probes = 0; probes < AG_MAX_PROBE; ++probes) {
-    if (ln.w[0] == key) return (long long)h;
+    if (ln.w[0] == key) return true;
     if (ln.w[0] == EMPTY_KEY) {
-      if (full) return -1;
-      const unsigned long long old = atomicCAS(t.key((long long)h), EMPTY_KEY, key);
-      if (old == EMPTY_KEY) { new_groups++; return (long long)h; }
-      if (old == key) return (long long)h;
+      if (full) return false;
+      const unsigned long long old = atomicCAS(line_at<LW>(t, h), EMPTY_KEY, key);
+      if (old == EMPTY_KEY) { new_groups++; return true; }
+      if (old == key) return true;
     }
-    h = (h + 1ull) & mask;
-    load_line<WITH_VALS>(t, (long long)h, ln);
+    h = t.next(h);
+    load_line<LW>(t, h, ln);
   }
-  return -1;
+  return false;
 }
 
 // fold one raw value into global memory; `cur` = the accumulator as read with the probe (have_cur): a
@@ -322,24 +356,6 @@ __device__ __forceinline__ void acc_fold_global_cond(int func, int mt, unsigned 
     if (!have_cur || e > cur) atomicMax(p, e);
   } else {
     acc_fold_global(func, mt, p, v);
-  }
-}
-
-// fold one raw value into a shared-memory accumulator (front table)
-__device__ __forceinline__ void acc_fold_shared(int func, int mt, unsigned long long* p, unsigned long long v) {
-  switch (func) {
-    case DFGPU_AGG_SUM:
-      if (mt == MT_F64) atomicAdd((double*)p, u2d(v));
-      else if (mt == MT_F32) atomicAdd((float*)p, u2f(v));
-      else atomicAdd(p, v);
-      break;
-    case DFGPU_AGG_COUNT: atomicAdd(p, 1ull); break;
-    case DFGPU_AGG_MIN:
-      if (!is_nan_val(v, mt)) atomicMin(p, ord_enc(v, mt));
-      break;
-    default:
-      if (!is_nan_val(v, mt)) atomicMax(p, ord_enc(v, mt));
-      break;
   }
 }
 
@@ -526,7 +542,6 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
   }
   const int tid = threadIdx.x, lane = tid & 31;
   const long long n = p.row_list ? p.nlist : p.nrows;
-  const int hshift = hash_shift(p.cap);
   // the input is read exactly once: mark its lines evict-first so that they do not displace the table
   const unsigned long long stream_policy = l2_evict_first_policy();
   bool bad = false;
@@ -573,10 +588,10 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
 #pragma unroll
     for (int r = 0; r < R; r++) {
       const unsigned long long hs = mix64(key[r]);
-      h[r] = home_slot(hs, hshift);
+      h[r] = p.t.home(hs);
       probing[r] = ((src.mask >> r) & 1u) && key[r] != EMPTY_KEY && fslot[r] < 0;
       ln[r].w[0] = ln[r].w[1] = ln[r].w[2] = ln[r].w[3] = 0ull;
-      if (probing[r]) load_line<true>(p.t, (long long)h[r], ln[r]);
+      if (probing[r]) load_line<LINE_RT>(p.t, h[r], ln[r]);
     }
     long long slot[R];
     unsigned new_groups = 0;
@@ -586,10 +601,10 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
       if (!((src.mask >> r) & 1u) || fslot[r] >= 0) continue;
       if (key[r] == EMPTY_KEY) {  // the one key value that collides with the empty marker
         if (__ldcg(&p.counters[CTR_SENTINEL]) == 0ull) p.counters[CTR_SENTINEL] = 1ull;
-        slot[r] = p.cap;
+        slot[r] = p.t.cap;
         continue;
       }
-      slot[r] = probe_insert<true>(p.t, p.cap, key[r], ln[r], h[r], full, new_groups);
+      slot[r] = probe_insert<LINE_RT>(p.t, key[r], ln[r], h[r], full, new_groups) ? (long long)h[r] : -1;
       if (slot[r] < 0) {
         const unsigned long long at = atomicAdd(&p.counters[CTR_OVERFLOW], 1ull);
         p.ovf_rows[at] = src.rowid(r);
@@ -611,7 +626,7 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
           if (NULLS && (func == DFGPU_AGG_COUNT || avg) && !((av >> r) & 1u)) continue;  // COUNT and AVG skip nulls
           const unsigned long long x = avg ? d2u(widen_f64(v[r], p.aggs[a].mtype)) : v[r];
           if (FRONT && fslot[r] >= 0 && ((src.mask >> r) & 1u)) {
-            acc_fold_shared(func, mt, &ftab[(1 + a) * FS + fslot[r]], x);
+            acc_fold_global(func, mt, &ftab[(1 + a) * FS + fslot[r]], x);
             if ((b >> r) & 1u) bad = true;
           } else if (slot[r] >= 0) {
             acc_fold_global_cond(func, mt, p.t.val(slot[r], a), x, cond && probing[r], cond ? line_word(ln[r], l) : 0ull);
@@ -636,13 +651,12 @@ __device__ __forceinline__ void hash_agg_body(const AggParams& p, unsigned long 
       const int j = i % FS;
       const unsigned long long key = tb[j];
       if (key == EMPTY_KEY) continue;
-      const unsigned long long h = home_slot(mix64(key), hshift);
+      unsigned long long h = p.t.home(mix64(key));
       Line ln;
-      load_line<false>(p.t, (long long)h, ln);
-      const long long slot = probe_insert<false>(p.t, p.cap, key, ln, h, false, new_groups);
-      if (slot < 0) { p.counters[CTR_ERROR] = 2ull; continue; }
+      load_line<LINE_KEY>(p.t, h, ln);
+      if (!probe_insert<LINE_KEY>(p.t, key, ln, h, false, new_groups)) { p.counters[CTR_ERROR] = 2ull; continue; }
       for (int a = 0; a < p.naggs; a++)
-        acc_merge_global(p.aggs[a].func, p.aggs[a].mtype, p.t.val(slot, a), tb[(1 + a) * FS + j]);
+        acc_merge_global(p.aggs[a].func, p.aggs[a].mtype, p.t.val((long long)h, a), tb[(1 + a) * FS + j]);
     }
     if (new_groups) atomicAdd(&p.counters[CTR_GROUPS], (unsigned long long)new_groups);
   }
@@ -676,8 +690,6 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
   const unsigned long long* __restrict__ kc = p.lean.key_col + p.row_begin;
   const unsigned long long* __restrict__ vc = p.lean.arg_col + p.row_begin;
   unsigned long long* const base = p.t.base;
-  const int hshift = hash_shift(p.cap);
-  const unsigned long long smask = (unsigned long long)p.cap - 1ull;
   const unsigned long long policy = l2_evict_first_policy();
   constexpr int TILE = AG_THREADS * 2;
   const long long tstep = (long long)gridDim.x * TILE;
@@ -717,14 +729,9 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
     bool act[2];
 #pragma unroll
     for (int r = 0; r < 2; r++) {
-      slot[r] = home_slot(mix64(k[r]), hshift);
+      slot[r] = p.t.home(mix64(k[r]));
       act[r] = r == 0 ? any : both;
-      if (act[r] && k[r] != EMPTY_KEY) {
-        const unsigned long long* q = base + slot[r] * LW;
-        if (LW == 4) load_line4(q, ln[r]);
-        else if (LW == 2) asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln[r].w[0]), "=l"(ln[r].w[1]) : "l"(q) : "memory");
-        else asm volatile("ld.global.cg.u64 %0, [%1];" : "=l"(ln[r].w[0]) : "l"(q) : "memory");
-      }
+      if (act[r] && k[r] != EMPTY_KEY) load_line<LW>(p.t, slot[r], ln[r]);
     }
     unsigned new_groups = 0;
 #pragma unroll
@@ -733,25 +740,10 @@ __global__ void __launch_bounds__(AG_THREADS, 5) k_hash_agg_lean(const __grid_co
       bool have_line = true;
       if (k[r] == EMPTY_KEY) {  // the one key value that collides with the empty marker
         if (__ldcg(&p.counters[CTR_SENTINEL]) == 0ull) p.counters[CTR_SENTINEL] = 1ull;
-        slot[r] = (unsigned long long)p.cap;
+        slot[r] = (unsigned long long)p.t.cap;
         have_line = false;
       } else {
-        bool found = false;
-        for (int probes = 0; probes < AG_MAX_PROBE; ++probes) {
-          if (ln[r].w[0] == k[r]) { found = true; break; }
-          if (ln[r].w[0] == EMPTY_KEY) {
-            if (full) break;
-            const unsigned long long old = atomicCAS(base + slot[r] * LW, EMPTY_KEY, k[r]);
-            if (old == EMPTY_KEY) { new_groups++; found = true; break; }
-            if (old == k[r]) { found = true; break; }
-          }
-          slot[r] = (slot[r] + 1ull) & smask;
-          const unsigned long long* q = base + slot[r] * LW;
-          if (LW == 4) load_line4(q, ln[r]);
-          else if (LW == 2) asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(ln[r].w[0]), "=l"(ln[r].w[1]) : "l"(q) : "memory");
-          else asm volatile("ld.global.cg.u64 %0, [%1];" : "=l"(ln[r].w[0]) : "l"(q) : "memory");
-        }
-        if (!found) {  // table refuses new keys: the row is replayed after the table has grown
+        if (!probe_insert<LW>(p.t, k[r], ln[r], slot[r], full, new_groups)) {  // table refuses new keys: the row is replayed after the table has grown
           const unsigned long long at = atomicAdd(&p.counters[CTR_OVERFLOW], 1ull);
           p.ovf_rows[at] = (unsigned)(p.row_begin + i + r);
           continue;
@@ -806,8 +798,6 @@ __global__ void __launch_bounds__(AG_THREADS) k_hash_agg_wide(const __grid_const
   constexpr int R = Src::R;
   const int tid = threadIdx.x, lane = tid & 31;
   const long long n = p.row_list ? p.nlist : p.nrows;
-  const int hshift = hash_shift(p.cap);
-  const unsigned long long smask = (unsigned long long)p.cap - 1ull;
   const int KW = p.wide.kw;
   bool bad = false;
   constexpr int TILE = AG_THREADS * R;
@@ -842,7 +832,7 @@ __global__ void __launch_bounds__(AG_THREADS) k_hash_agg_wide(const __grid_const
       if (!((src.mask >> r) & 1u)) continue;
       const long long row = src.g.rows[r];
       const unsigned long long ready = wide_tag(hsh[r]), busy = ready & ~1ull;
-      unsigned long long h = home_slot(hsh[r], hshift);
+      unsigned long long h = p.t.home(hsh[r]);
       bool deferred = false;
       for (int probes = 0; probes < AG_MAX_PROBE; ++probes) {
         unsigned long long* line = p.t.key((long long)h);
@@ -875,7 +865,7 @@ __global__ void __launch_bounds__(AG_THREADS) k_hash_agg_wide(const __grid_const
           }
           if (same) { slot[r] = (long long)h; break; }
         }
-        h = (h + 1ull) & smask;
+        h = p.t.next(h);
       }
       if (slot[r] < 0) {
         const unsigned long long at = atomicAdd(&p.counters[CTR_OVERFLOW], 1ull);
@@ -910,29 +900,30 @@ __global__ void __launch_bounds__(AG_THREADS) k_hash_agg_wide(const __grid_const
 }
 
 // Re-insertion of the (distinct) groups of a wide-key table into a bigger one: every entry goes to the first
-// empty slot after its home; no key comparison is needed because the source table holds each key once.
+// empty slot after its home; no key comparison is needed because the source table holds each key once.  An entry that
+// finds no empty slot in cap probes sets *error to 2.
 struct WideMoveParams {
   TableLayout from, to;
-  long long from_cap, to_cap;
   int kw, naggs;
+  unsigned long long* error;
 };
 __global__ void __launch_bounds__(256) k_wide_move(const __grid_constant__ WideMoveParams p) {
-  const int hshift = hash_shift(p.to_cap);
-  const unsigned long long smask = (unsigned long long)p.to_cap - 1ull;
-  for (long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x; s < p.from_cap; s += (long long)gridDim.x * blockDim.x) {
+  for (long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x; s < p.from.cap; s += (long long)gridDim.x * blockDim.x) {
     const unsigned long long* src = p.from.key(s);
     const unsigned long long tag = src[0];
     if (tag == EMPTY_KEY) continue;
-    unsigned long long h = home_slot(tag & ~1ull, hshift);  // the tag IS the hash (but for its low bit): same home rule as the scan
-    for (;;) {
+    unsigned long long h = p.to.home(tag & ~1ull);  // the tag IS the hash (but for its low bit): same home rule as the scan
+    long long probes = 0;
+    for (; probes < p.to.cap; probes++) {
       unsigned long long* dst = p.to.key((long long)h);
       if (atomicCAS(dst, EMPTY_KEY, tag) == EMPTY_KEY) {
         for (int k = 0; k < p.kw; k++) dst[1 + k] = src[1 + k];
         for (int a = 0; a < p.naggs; a++) *p.to.val((long long)h, a) = *p.from.val(s, a);
         break;
       }
-      h = (h + 1ull) & smask;
+      h = p.to.next(h);
     }
+    if (probes == p.to.cap) *p.error = 2ull;
   }
 }
 
@@ -1103,7 +1094,6 @@ __global__ void __launch_bounds__(256) k_reduce_f64(const __grid_constant__ Redu
 // accumulators (the exchange format of the multi-GPU merge).
 struct CompactParams {
   TableLayout t;
-  long long cap;
   int sentinel_used;
   int nkeys, naggs, raw;
   long long raw_stride;  // raw output: element idx of every raw array lives at idx * raw_stride (0 = 1: dense arrays)
@@ -1125,15 +1115,15 @@ struct CompactParams {
 
 __global__ void __launch_bounds__(256) k_compact(const __grid_constant__ CompactParams p) {
   const int lane = threadIdx.x & 31;
-  const long long total = p.cap + 1;
+  const long long total = p.t.cap + 1;
   const long long step = (long long)gridDim.x * blockDim.x;
   // round the loop bound up to a warp multiple so ballots stay converged
   for (long long s0 = (long long)blockIdx.x * blockDim.x; s0 < total; s0 += step) {
     const long long s = s0 + threadIdx.x;
     bool occ = false;
     unsigned long long key = 0;
-    if (s < p.cap) { key = *p.t.key(s); occ = key != EMPTY_KEY; }
-    else if (s == p.cap) { key = EMPTY_KEY; occ = p.sentinel_used != 0 || (p.sentinel_flag && *p.sentinel_flag != 0ull); }
+    if (s < p.t.cap) { key = *p.t.key(s); occ = key != EMPTY_KEY; }
+    else if (s == p.t.cap) { key = EMPTY_KEY; occ = p.sentinel_used != 0 || (p.sentinel_flag && *p.sentinel_flag != 0ull); }
     const unsigned m = __ballot_sync(0xffffffffu, occ);
     if (!m) continue;
     unsigned long long basei = 0;
@@ -1174,14 +1164,12 @@ struct MergeParams {
   long long in_stride;  // entry i of every input array lives at i * in_stride (0 = 1: dense arrays)
   long long n;
   TableLayout t;
-  long long cap;
   int naggs;
   AggDesc aggs[kMaxAggs];
   unsigned long long* counters;
 };
 
 __global__ void __launch_bounds__(256) k_merge(const __grid_constant__ MergeParams p) {
-  const int hshift = hash_shift(p.cap);
   unsigned new_groups = 0;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += (long long)gridDim.x * blockDim.x) {
     const long long at = p.in_stride ? i * p.in_stride : i;
@@ -1189,13 +1177,13 @@ __global__ void __launch_bounds__(256) k_merge(const __grid_constant__ MergePara
     long long slot;
     if (key == EMPTY_KEY) {
       p.counters[CTR_SENTINEL] = 1ull;
-      slot = p.cap;
+      slot = p.t.cap;
     } else {
-      const unsigned long long h = home_slot(mix64(key), hshift);
+      unsigned long long h = p.t.home(mix64(key));
       Line ln;
-      load_line<false>(p.t, (long long)h, ln);
-      slot = probe_insert<false>(p.t, p.cap, key, ln, h, false, new_groups);
-      if (slot < 0) { p.counters[CTR_ERROR] = 2ull; continue; }  // cannot happen: caller sizes the table
+      load_line<LINE_KEY>(p.t, h, ln);
+      if (!probe_insert<LINE_KEY>(p.t, key, ln, h, false, new_groups)) { p.counters[CTR_ERROR] = 2ull; continue; }  // cannot happen: caller sizes the table
+      slot = (long long)h;
     }
     for (int a = 0; a < p.naggs; a++)
       acc_merge_global(p.aggs[a].func, p.aggs[a].mtype, p.t.val(slot, a), p.in_vals[a][at]);
@@ -1316,7 +1304,6 @@ struct VerifyParams {
   const unsigned long long* hashes;
   long long n;
   TableLayout t;
-  long long cap;
   int rep_agg;
   const int* off;
   const unsigned char* bytes;
@@ -1324,20 +1311,8 @@ struct VerifyParams {
   unsigned long long* flag;
 };
 __global__ void __launch_bounds__(256) k_utf8_group_verify(const __grid_constant__ VerifyParams p) {
-  const unsigned long long hmask = (unsigned long long)p.cap - 1ull;
-  const int hshift = hash_shift(p.cap);
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += (long long)gridDim.x * blockDim.x) {
-    const unsigned long long key = p.hashes[i];
-    long long slot = p.cap;
-    if (key != EMPTY_KEY) {
-      unsigned long long h = home_slot(mix64(key), hshift);
-      for (;;) {
-        const unsigned long long cur = __ldcg(p.t.key((long long)h));
-        if (cur == key) { slot = (long long)h; break; }
-        if (cur == EMPTY_KEY) { slot = -1; break; }
-        h = (h + 1ull) & hmask;
-      }
-    }
+    const long long slot = p.t.find(p.hashes[i], true);
     if (slot < 0) { *p.flag = 2ull; continue; }
     const unsigned long long rep = *p.t.val(slot, p.rep_agg);
     const Utf8Source& sc = p.srcs[rep >> UTF8_SRC_SHIFT];
@@ -1373,8 +1348,7 @@ constexpr int DCTR_SET = 2;       // [DCTR_SET + 2s]: pairs in set s, [DCTR_SET 
 constexpr int DCTR_SLOTS = DCTR_SET + 2 * kMaxAggs;
 
 struct SetParams {
-  unsigned long long* slots[kMaxAggs];  // two words per slot
-  long long cap[kMaxAggs];              // power of two
+  SetView set[kMaxAggs];
   long long max_fill[kMaxAggs];         // new pairs are refused (-> overflow list) beyond this fill
   int mt[kMaxAggs];                     // machine type of the argument
 };
@@ -1407,12 +1381,10 @@ __device__ __forceinline__ unsigned long long distinct_norm(unsigned long long v
 }
 
 // Insert (key, val): 1 = inserted, 0 = already there, -1 = not inserted (full: the set refuses new pairs; or probe limit).
-__device__ __forceinline__ int set_insert(unsigned long long* slots, long long cap, int hshift, unsigned long long key, unsigned long long val,
-                                          bool full) {
-  const unsigned long long mask = (unsigned long long)cap - 1ull;
-  unsigned long long h = home_slot(mix64(val ^ mix64(key)), hshift);
+__device__ __forceinline__ int set_insert(const SetView& set, unsigned long long key, unsigned long long val, bool full) {
+  unsigned long long h = set.home(mix64(val ^ mix64(key)));
   for (int probes = 0; probes < AG_MAX_PROBE; ++probes) {
-    unsigned long long* q = slots + 2 * h;
+    unsigned long long* q = set.slots + 2 * h;
     unsigned long long a, b;
     asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "l"(q) : "memory");
     // the halves of a plain load may straddle a claim: only a view without an EMPTY_KEY half is certainly a
@@ -1422,7 +1394,7 @@ __device__ __forceinline__ int set_insert(unsigned long long* slots, long long c
       if (a == EMPTY_KEY && b == EMPTY_KEY) return full ? -1 : 1;
     }
     if (a == key && b == val) return 0;
-    h = (h + 1ull) & mask;
+    h = set.next(h);
   }
   return -1;
 }
@@ -1462,7 +1434,6 @@ __device__ __forceinline__ void distinct_insert_body(const AggParams& p, const S
       unsigned long long v[R];
       unsigned av;
       const unsigned b = src.arg(p, s, v, av);
-      const int hshift = hash_shift(sp.cap[s]);
       unsigned added = 0;
 #pragma unroll
       for (int r = 0; r < R; r++) {
@@ -1473,7 +1444,7 @@ __device__ __forceinline__ void distinct_insert_body(const AggParams& p, const S
           if (__ldcg(&p.counters[DCTR_SET + 2 * s + 1]) == 0ull) p.counters[DCTR_SET + 2 * s + 1] = 1ull;
           continue;
         }
-        const int rc = set_insert(sp.slots[s], sp.cap[s], hshift, key[r], val, ((full >> s) & 1u) != 0);
+        const int rc = set_insert(sp.set[s], key[r], val, ((full >> s) & 1u) != 0);
         if (rc > 0) added++;
         else if (rc < 0) refused |= 1u << r;
       }
@@ -1502,56 +1473,38 @@ __global__ void __launch_bounds__(AG_THREADS) k_distinct_insert_plain(const __gr
 
 // Re-insertion of a set's pairs into a bigger set (growth).
 struct SetMoveParams {
-  const unsigned long long* from;
-  long long from_cap;
-  unsigned long long* to;
-  long long to_cap;
+  SetView from, to;
   unsigned long long* error;
 };
 __global__ void __launch_bounds__(256) k_set_move(const __grid_constant__ SetMoveParams p) {
-  const int hshift = hash_shift(p.to_cap);
-  for (long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x; s < p.from_cap; s += (long long)gridDim.x * blockDim.x) {
-    const unsigned long long key = p.from[2 * s], val = p.from[2 * s + 1];
+  for (long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x; s < p.from.cap; s += (long long)gridDim.x * blockDim.x) {
+    const unsigned long long key = p.from.slots[2 * s], val = p.from.slots[2 * s + 1];
     if (key == EMPTY_KEY && val == EMPTY_KEY) continue;
-    if (set_insert(p.to, p.to_cap, hshift, key, val, false) < 0) *p.error = 2ull;
+    if (set_insert(p.to, key, val, false) < 0) *p.error = 2ull;
   }
 }
 
-// Count a set's pairs into the group table: +1 on the accumulator words `words` of the pair's group.  Index `cap` is the
-// empty-marker pair (flag `marker`), whose group is the sentinel slot.  A pair whose group is missing sets `error`.
+// Count a set's pairs into the group table: +1 on the accumulator words `words` of the pair's group.  Index `set.cap` is
+// the empty-marker pair (flag `marker`), whose group is the sentinel slot.  A pair whose group is missing sets `error`.
 struct DistinctCountParams {
-  const unsigned long long* slots;
-  long long cap;
+  SetView set;
   const unsigned long long* marker;
   TableLayout t;
-  long long tcap;
   int sentinel_used;
   int nwords;
   int words[kMaxAggs];
   unsigned long long* error;
 };
 __global__ void __launch_bounds__(256) k_distinct_count(const __grid_constant__ DistinctCountParams p) {
-  const unsigned long long hmask = (unsigned long long)p.tcap - 1ull;
-  const int hshift = hash_shift(p.tcap);
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i <= p.cap; i += (long long)gridDim.x * blockDim.x) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i <= p.set.cap; i += (long long)gridDim.x * blockDim.x) {
     unsigned long long key = EMPTY_KEY;
-    if (i < p.cap) {
-      key = p.slots[2 * i];
-      if (key == EMPTY_KEY && p.slots[2 * i + 1] == EMPTY_KEY) continue;
+    if (i < p.set.cap) {
+      key = p.set.slots[2 * i];
+      if (key == EMPTY_KEY && p.set.slots[2 * i + 1] == EMPTY_KEY) continue;
     } else if (*p.marker == 0ull) {
       continue;
     }
-    long long slot = p.sentinel_used ? p.tcap : -1;
-    if (key != EMPTY_KEY) {
-      unsigned long long h = home_slot(mix64(key), hshift);
-      slot = -1;
-      for (long long probes = 0; probes < p.tcap; probes++) {  // bounded: a missing key is an error, never a hang
-        const unsigned long long cur = *p.t.key((long long)h);
-        if (cur == key) { slot = (long long)h; break; }
-        if (cur == EMPTY_KEY) break;
-        h = (h + 1ull) & hmask;
-      }
-    }
+    const long long slot = p.t.find(key, p.sentinel_used != 0);
     if (slot < 0) { *p.error = 2ull; continue; }
     for (int w = 0; w < p.nwords; w++) atomicAdd(p.t.val(slot, p.words[w]), 1ull);
   }
@@ -1577,7 +1530,6 @@ struct dfgpu_aggstate {
   std::vector<unsigned long long> key_mask;
   std::vector<AggDesc> descs;
   // table
-  long long cap = 0;
   long long expected = 0;
   TableLayout t{};
   bool aos = false;        // "line" layout: every accumulator shares the line with the key (tables beyond L2)
@@ -1612,8 +1564,7 @@ struct dfgpu_aggstate {
   std::vector<char> out_is_avg;
   bool emit_words = false;          // finish returns one column per table word (the regroup merge across ranks)
   std::vector<int> dist_dtypes;     // argument dtype per set, typed at the first batch
-  std::vector<unsigned long long*> set_slots;
-  std::vector<long long> set_cap;
+  std::vector<SetView> sets;
   unsigned long long* d_dctr = nullptr;  // DCTR_SLOTS words, see DCTR_*
 
   ~dfgpu_aggstate() {
@@ -1622,7 +1573,7 @@ struct dfgpu_aggstate {
       ctx->free(d_counters);
       for (void* p : utf8_owned) ctx->free(p);
       ctx->free(d_utf8_srcs);
-      for (void* p : set_slots) ctx->free(p);
+      for (const SetView& s : sets) ctx->free(s.slots);
       ctx->free(d_dctr);
     }
   }
@@ -1659,6 +1610,12 @@ long long next_pow2(long long x) {
   while (p < x) p <<= 1;
   return p;
 }
+
+// Sizing policy of the group table and the pair sets: a table for n entries has at least min_cap slots and at least twice
+// n, rounded up to a power of two; it takes new entries up to half full and grows x4.
+long long table_cap(long long n, long long min_cap) { return std::max(min_cap, next_pow2(2 * n)); }
+long long fill_limit(long long cap) { return cap / 2; }
+long long grown_cap(long long cap) { return cap * 4; }
 
 int grid_for(dfgpu_ctx* ctx, long long work_items, int per_block, int blocks_per_sm) {
   long long g = (work_items + per_block - 1) / per_block;
@@ -1763,6 +1720,19 @@ long long estimate_groups(long long d, long long s, long long total_rows) {
   return g > double(total_rows) ? total_rows : (long long)g;
 }
 
+// Capacity for a table that holds `seen` distinct entries after the first `prefix_rows` rows of a batch of `batch_rows`:
+// sized for the estimated total (*est), but halved while it exceeds what 1/8 of device memory holds at `slot_bytes` per
+// slot; never below the current capacity `cur_cap`.
+long long prefix_cap(const dfgpu_ctx* ctx, long long seen, long long prefix_rows, long long batch_rows, long long slot_bytes,
+                     long long cur_cap, long long min_cap, long long* est = nullptr) {
+  const long long e = std::max(estimate_groups(seen, prefix_rows, batch_rows), seen);
+  if (est) *est = e;
+  const long long afford = (long long)(ctx->device_mem_bytes / 8) / slot_bytes;
+  long long want = table_cap(e, min_cap);
+  while (want > cur_cap && want > afford) want >>= 1;
+  return std::max(want, cur_cap);
+}
+
 void layout_shape(const std::vector<AggDesc>& descs, int naggs, int nkeys, bool line_mode, long long* lw, int* n_add, signed char* loc, int kw = 0) {
   *lw = 1;
   *n_add = 0;
@@ -1790,7 +1760,7 @@ bool want_aos(long long groups, const std::vector<AggDesc>& descs, int naggs) {
   int n_add;
   signed char loc[kMaxAggs];
   layout_shape(descs, naggs, 1, false, &lw, &n_add, loc);
-  const long long cap = std::max(AG_MIN_CAP, next_pow2(2 * groups));
+  const long long cap = table_cap(groups, AG_MIN_CAP);
   const long long line_hot = std::min(cap * 8 * lw, groups * std::max<long long>(32, 8 * lw));
   const long long arr_hot = std::min(cap * 8, groups * 32);
   return line_hot + n_add * arr_hot > AG_SOA_L2_BUDGET;
@@ -1800,6 +1770,7 @@ TableLayout table_alloc(dfgpu_ctx* ctx, int naggs, int nkeys, const std::vector<
   InitParams ip;
   memset(&ip, 0, sizeof(ip));
   int n_add = 0;
+  ip.t.set_cap(cap);
   layout_shape(descs, naggs, nkeys, aos, &ip.t.lw, &n_add, ip.t.loc, kw);
   const size_t line_words = size_t(cap + 1) * size_t(ip.t.lw);
   const size_t words = line_words + size_t(n_add) * size_t(cap + 1);
@@ -1831,13 +1802,12 @@ unsigned long long read_counter(dfgpu_aggstate* st, int slot) {
 // Raw compaction (k_compact, raw = 1) of table t: the occupied slots as (packed key, accumulators) entries.  Entry i's
 // key goes to keys[i * stride] and accumulator a to vals[a * val_step + i * stride] (stride 0 = 1); the number of
 // entries to counter CTR_COMPACT.
-void compact_raw(dfgpu_aggstate* st, const TableLayout& t, long long cap, int sentinel_used, const unsigned long long* sentinel_flag,
-                 unsigned long long* keys, unsigned long long* vals, size_t val_step, long long stride) {
+void compact_raw(dfgpu_aggstate* st, const TableLayout& t, int sentinel_used, const unsigned long long* sentinel_flag, unsigned long long* keys,
+                 unsigned long long* vals, size_t val_step, long long stride) {
   dfgpu_ctx* ctx = st->ctx;
   CompactParams cp;
   memset(&cp, 0, sizeof(cp));
   cp.t = t;
-  cp.cap = cap;
   cp.sentinel_used = sentinel_used;
   cp.sentinel_flag = sentinel_flag;
   cp.nkeys = st->nkeys;
@@ -1851,7 +1821,7 @@ void compact_raw(dfgpu_aggstate* st, const TableLayout& t, long long cap, int se
   }
   DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_COMPACT, 0, 8, ctx->stream));
   cp.counter = st->d_counters + CTR_COMPACT;
-  launch_kernel(ctx, k_compact, "k_compact", cp, cap + 1, 256, 8);
+  launch_kernel(ctx, k_compact, "k_compact", cp, t.cap + 1, 256, 8);
 }
 
 // Grow the table to new_cap.  Wide tables move their slots (k_wide_move: every entry is distinct); the others are
@@ -1866,16 +1836,15 @@ void table_grow(dfgpu_aggstate* st, long long new_cap) {
     memset(&mp, 0, sizeof(mp));
     mp.from = st->t;
     mp.to = nt;
-    mp.from_cap = st->cap;
-    mp.to_cap = new_cap;
     mp.kw = st->nkeys;
     mp.naggs = st->naggs;
-    launch_kernel(ctx, k_wide_move, "k_wide_move", mp, st->cap, 256, 8);
+    mp.error = st->d_counters + CTR_ERROR;
+    launch_kernel(ctx, k_wide_move, "k_wide_move", mp, st->t.cap, 256, 8);
   } else {
     const size_t cnt = size_t(st->ngroups + 1);
     unsigned long long* ck = tmp.alloc(cnt * 8);
     unsigned long long* cv = tmp.alloc(cnt * 8 * size_t(st->naggs > 0 ? st->naggs : 1));
-    compact_raw(st, st->t, st->cap, st->sentinel_used, nullptr, ck, cv, cnt, 0);
+    compact_raw(st, st->t, st->sentinel_used, nullptr, ck, cv, cnt, 0);
     MergeParams mp;
     memset(&mp, 0, sizeof(mp));
     mp.in_keys = ck;
@@ -1885,17 +1854,18 @@ void table_grow(dfgpu_aggstate* st, long long new_cap) {
     }
     mp.n = st->ngroups + (st->sentinel_used ? 1 : 0);
     mp.t = nt;
-    mp.cap = new_cap;
     mp.naggs = st->naggs;
     DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_GROUPS, 0, 8, ctx->stream));  // ngroups is recounted by the merge
     mp.counters = st->d_counters;
     if (mp.n > 0) launch_kernel(ctx, k_merge, "k_merge", mp, mp.n, 256, 8);
   }
-  DF_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (read_counter(st, CTR_ERROR) == 2) {
+    ctx->free(nt.base);
+    fail(DFGPU_ERR_INTERNAL, "table growth could not place a group");
+  }
   ctx->free(st->t.base);
   st->t = nt;
   st->aos = aos;
-  st->cap = new_cap;
 }
 
 }  // namespace
@@ -2262,7 +2232,7 @@ bool plain_spec(const ProgramBuilder& pb, const ProgramSet& ps, int has_pred, in
   return ok;
 }
 
-unsigned long long* set_alloc(dfgpu_ctx* ctx, long long cap);
+SetView set_alloc(dfgpu_ctx* ctx, long long cap);
 
 // The first batch types the operator: key packing, table form and capacity.  Later batches must bring the same types.
 void type_batch(dfgpu_aggstate* st, const BatchPrograms& bp) {
@@ -2279,20 +2249,19 @@ void type_batch(dfgpu_aggstate* st, const BatchPrograms& bp) {
   if (st->wide && !st->dist_progs.empty()) fail(DFGPU_ERR_NOT_IMPLEMENTED, "COUNT(DISTINCT) with GROUP BY keys wider than 64 bits");
   st->dist_dtypes = bp.dist_dtypes;
   st->typed = true;
-  st->cap = st->nkeys == 0 ? 0 : std::max(AG_MIN_CAP, next_pow2(2 * st->expected));
+  const long long cap = st->nkeys == 0 ? 0 : table_cap(st->expected, AG_MIN_CAP);
   st->aos = st->wide || (st->nkeys > 0 && want_aos(st->expected, st->descs, st->naggs));
-  st->t = table_alloc(st->ctx, st->naggs, st->nkeys, st->descs, st->cap, st->aos, st->wide ? st->nkeys : 0);
-  for (size_t s = 0; s < st->dist_progs.size(); s++) {
-    st->set_cap.push_back(std::max(AG_SET_MIN_CAP, next_pow2(2 * st->expected)));
-    st->set_slots.push_back(set_alloc(st->ctx, st->set_cap.back()));
-  }
+  st->t = table_alloc(st->ctx, st->naggs, st->nkeys, st->descs, cap, st->aos, st->wide ? st->nkeys : 0);
+  for (size_t s = 0; s < st->dist_progs.size(); s++) st->sets.push_back(set_alloc(st->ctx, table_cap(st->expected, AG_SET_MIN_CAP)));
 }
 
 // ---- COUNT(DISTINCT) ----------------------------------------------------------------------------------------
-unsigned long long* set_alloc(dfgpu_ctx* ctx, long long cap) {
-  unsigned long long* q = (unsigned long long*)ctx->alloc(size_t(cap) * 16);
-  DF_CUDA(cudaMemsetAsync(q, 0xff, size_t(cap) * 16, ctx->stream));  // every word EMPTY_KEY
-  return q;
+SetView set_alloc(dfgpu_ctx* ctx, long long cap) {
+  SetView set;
+  set.set_cap(cap);
+  set.slots = (unsigned long long*)ctx->alloc(size_t(cap) * 16);
+  DF_CUDA(cudaMemsetAsync(set.slots, 0xff, size_t(cap) * 16, ctx->stream));  // every word EMPTY_KEY
+  return set;
 }
 
 // DCTR_* slots -> host (synchronises the stream)
@@ -2306,18 +2275,15 @@ void read_dctr(dfgpu_aggstate* st, unsigned long long* host) {
 void set_grow(dfgpu_aggstate* st, int s, long long new_cap) {
   dfgpu_ctx* ctx = st->ctx;
   SetMoveParams mp;
-  mp.from = st->set_slots[size_t(s)];
-  mp.from_cap = st->set_cap[size_t(s)];
+  mp.from = st->sets[size_t(s)];
   mp.to = set_alloc(ctx, new_cap);
-  mp.to_cap = new_cap;
   mp.error = st->d_dctr + DCTR_ERROR;
-  launch_kernel(ctx, k_set_move, "k_set_move", mp, mp.from_cap, 256 * 4, 8);
+  launch_kernel(ctx, k_set_move, "k_set_move", mp, mp.from.cap, 256 * 4, 8);
   unsigned long long c[DCTR_SLOTS];
   read_dctr(st, c);
   if (c[DCTR_ERROR] == 2) fail(DFGPU_ERR_INTERNAL, "COUNT(DISTINCT) set growth could not place a pair");
-  ctx->free(st->set_slots[size_t(s)]);
-  st->set_slots[size_t(s)] = mp.to;
-  st->set_cap[size_t(s)] = new_cap;
+  ctx->free(mp.from.slots);
+  st->sets[size_t(s)] = mp.to;
 }
 
 // Insert the pairs of rows [begin, begin + count) of the batch into every set: after the group scan of the same rows.
@@ -2372,9 +2338,8 @@ void distinct_update(dfgpu_aggstate* st, const BatchPrograms& bp, const AggParam
     SetParams sp;
     memset(&sp, 0, sizeof(sp));
     for (int s = 0; s < nsets; s++) {
-      sp.slots[s] = st->set_slots[size_t(s)];
-      sp.cap[s] = st->set_cap[size_t(s)];
-      sp.max_fill[s] = std::max<long long>(0, sp.cap[s] / 2 - (long long)grid * AG_TILE);
+      sp.set[s] = st->sets[size_t(s)];
+      sp.max_fill[s] = std::max<long long>(0, fill_limit(sp.set[s].cap) - (long long)grid * AG_TILE);
       sp.mt[s] = mtype_of(st->dist_dtypes[size_t(s)]);
     }
     const int ps = ctx->prof_begin();
@@ -2391,13 +2356,13 @@ void distinct_update(dfgpu_aggstate* st, const BatchPrograms& bp, const AggParam
     for (int s = 0; s < nsets; s++) {
       const long long n = (long long)c[DCTR_SET + 2 * s];
       const bool refused = novf > 0 && n >= sp.max_fill[s];  // at the fill limit: this set refused new pairs
-      if (!refused && n <= sp.cap[s] / 2) continue;
-      set_grow(st, s, sp.cap[s] * 4);
+      if (!refused && n <= fill_limit(sp.set[s].cap)) continue;
+      set_grow(st, s, grown_cap(sp.set[s].cap));
       grew = true;
     }
     if (novf == 0) break;
     if (!grew)  // refused at the probe limit below the fill limit: grow every set
-      for (int s = 0; s < nsets; s++) set_grow(st, s, sp.cap[s] * 4);
+      for (int s = 0; s < nsets; s++) set_grow(st, s, grown_cap(sp.set[s].cap));
     list = ovf[cur];
     nlist = novf;
     cur ^= 1;
@@ -2406,33 +2371,29 @@ void distinct_update(dfgpu_aggstate* st, const BatchPrograms& bp, const AggParam
   if (prefix_of > 0) {
     unsigned long long c[DCTR_SLOTS];
     read_dctr(st, c);
-    const long long afford = (long long)(ctx->device_mem_bytes / 8) / 16;  // slots that fit in 1/8 of device memory
     for (int s = 0; s < nsets; s++) {
-      const long long n = (long long)c[DCTR_SET + 2 * s];
-      long long want = std::max(AG_SET_MIN_CAP, next_pow2(2 * std::max(estimate_groups(n, count, prefix_of), n)));
-      while (want > st->set_cap[size_t(s)] && want > afford) want >>= 1;
-      if (want > st->set_cap[size_t(s)]) set_grow(st, s, want);
+      const long long cur_cap = st->sets[size_t(s)].cap;
+      const long long want = prefix_cap(ctx, (long long)c[DCTR_SET + 2 * s], count, prefix_of, 16, cur_cap, AG_SET_MIN_CAP);
+      if (want > cur_cap) set_grow(st, s, want);
     }
   }
 }
 
 // GROUP BY at finish: add each set's pairs to the COUNT(DISTINCT) words of their groups.
-void distinct_count(dfgpu_aggstate* st, const TableLayout& t, long long cap, int sentinel_used) {
+void distinct_count(dfgpu_aggstate* st, const TableLayout& t, int sentinel_used) {
   dfgpu_ctx* ctx = st->ctx;
   DF_CUDA(cudaMemsetAsync(st->d_dctr + DCTR_ERROR, 0, 8, ctx->stream));
   for (size_t s = 0; s < st->dist_progs.size(); s++) {
     DistinctCountParams cp;
     memset(&cp, 0, sizeof(cp));
-    cp.slots = st->set_slots[s];
-    cp.cap = st->set_cap[s];
+    cp.set = st->sets[s];
     cp.marker = st->d_dctr + DCTR_SET + 2 * s + 1;
     cp.t = t;
-    cp.tcap = cap;
     cp.sentinel_used = sentinel_used;
     for (size_t j = 0; j < st->dist_set.size(); j++)
       if (st->dist_set[j] == int(s)) cp.words[cp.nwords++] = st->nscan + int(j);
     cp.error = st->d_dctr + DCTR_ERROR;
-    launch_kernel(ctx, k_distinct_count, "k_distinct_count", cp, cp.cap + 1, 256 * 4, 8);
+    launch_kernel(ctx, k_distinct_count, "k_distinct_count", cp, cp.set.cap + 1, 256 * 4, 8);
   }
   unsigned long long c[DCTR_SLOTS];
   read_dctr(st, c);
@@ -2456,7 +2417,6 @@ void distinct_count_scalar(dfgpu_aggstate* st) {
 void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
   dfgpu_ctx* ctx = st->ctx;
   p.t = st->t;
-  p.cap = 0;
   if (p.naggs == 0) return;  // COUNT(DISTINCT) alone: nothing for the reduce kernels to do
   if (bp.has_pred) DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_PASSED, 0, 8, ctx->stream));
   const int d = p.ps.max_depth;
@@ -2592,7 +2552,6 @@ void verify_utf8_groups(dfgpu_aggstate* st, const BatchPrograms& bp, long long n
   vp.hashes = bp.ukey_hash;
   vp.n = nrows;
   vp.t = st->t;
-  vp.cap = st->cap;
   vp.rep_agg = st->naggs - 1;
   vp.off = bp.ukey->offsets;
   vp.bytes = (const unsigned char*)bp.ukey->values;
@@ -2650,8 +2609,7 @@ void group_by_update(dfgpu_aggstate* st, const dfgpu_batch* batch, const BatchPr
     for (int round = 0;; round++) {
       if (round > 60) fail(DFGPU_ERR_INTERNAL, "hash table growth did not converge");
       p.t = st->t;
-      p.cap = st->cap;
-      p.max_groups = st->cap / 2;
+      p.max_groups = fill_limit(st->t.cap);
       p.row_begin = ranges[ri].first;
       p.nrows = ranges[ri].second;
       p.row_list = list;
@@ -2675,11 +2633,11 @@ void group_by_update(dfgpu_aggstate* st, const dfgpu_batch* batch, const BatchPr
       if (deferred) DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_DEFERRED, 0, 8, ctx->stream));
       tr.mark(ri == 0 && ranges.size() > 1 ? "scan kernel (prefix)" : "scan kernel");
       if (novf == 0) {
-        if (st->ngroups > st->cap / 2) { table_grow(st, st->cap * 4); tr.mark("table_grow (load factor)"); }
+        if (st->ngroups > fill_limit(st->t.cap)) { table_grow(st, grown_cap(st->t.cap)); tr.mark("table_grow (load factor)"); }
         break;
       }
       // rows that only met a slot still being published need no bigger table: replay them as they are
-      if (!(novf == deferred && st->ngroups <= st->cap / 2)) table_grow(st, st->cap * 4);
+      if (!(novf == deferred && st->ngroups <= fill_limit(st->t.cap))) table_grow(st, grown_cap(st->t.cap));
       list = ovf[cur];
       nlist = novf;
       cur ^= 1;
@@ -2691,14 +2649,12 @@ void group_by_update(dfgpu_aggstate* st, const dfgpu_batch* batch, const BatchPr
     if (sample && ri == 0) {
       // size (and lay out) the table for the estimated number of groups before the bulk of the batch
       // is touched: one rebuild of a ~1 Mi-entry table instead of repeated 4x growth + replays
-      long long est = std::max(estimate_groups(st->ngroups, kPrefix, batch->nrows), st->ngroups);
-      const long long afford = (long long)(ctx->device_mem_bytes / 8) / (32 * (1 + st->naggs));  // slots that fit in 1/8 of device memory
-      long long want_cap = std::max(AG_MIN_CAP, next_pow2(est * 2));
-      while (want_cap > st->cap && want_cap > afford) want_cap >>= 1;
+      long long est = 0;
+      const long long want_cap = prefix_cap(ctx, st->ngroups, kPrefix, batch->nrows, 32 * (1 + st->naggs), st->t.cap, AG_MIN_CAP, &est);
       const bool to_aos = !st->aos && want_aos(est, st->descs, st->naggs);
-      if (to_aos || want_cap > st->cap) {
+      if (to_aos || want_cap > st->t.cap) {
         st->aos = st->aos || to_aos;
-        table_grow(st, std::max(st->cap, want_cap));
+        table_grow(st, want_cap);
         tr.mark("table_grow (prefix estimate)");
       }
     }
@@ -2775,7 +2731,7 @@ void agg_export_raw(dfgpu_aggstate* st, DevBufs& bufs, unsigned long long** keys
   const size_t alloc_n = size_t(cnt > 0 ? cnt : 1);
   *keys = bufs.alloc(alloc_n * 8);
   *vals = bufs.alloc(alloc_n * 8 * size_t(st->naggs));
-  compact_raw(st, st->t, st->cap, st->nkeys == 0 ? 1 : (st->sentinel_used ? 1 : 0), nullptr, *keys, *vals, alloc_n, 0);
+  compact_raw(st, st->t, st->nkeys == 0 ? 1 : (st->sentinel_used ? 1 : 0), nullptr, *keys, *vals, alloc_n, 0);
   *n = cnt;
 }
 
@@ -2931,9 +2887,8 @@ void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, DevBufs& rows_buf, 
   long long n_owned = 0;
   unsigned long long* d_owned = nullptr;
   if (total_recv > 0) {
-    const long long ocap = std::max<long long>(1024, next_pow2(2 * (long long)total_recv));
     const bool oaos = want_aos((long long)total_recv, st->descs, st->naggs);
-    TableLayout ot = table_alloc(ctx, st->naggs, st->nkeys, st->descs, ocap, oaos);
+    TableLayout ot = table_alloc(ctx, st->naggs, st->nkeys, st->descs, table_cap((long long)total_recv, 1024), oaos);
     tmp.blocks.push_back(ot.base);
     MergeParams mp;
     memset(&mp, 0, sizeof(mp));
@@ -2945,7 +2900,6 @@ void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, DevBufs& rows_buf, 
     mp.in_stride = (long long)E;
     mp.n = (long long)total_recv;
     mp.t = ot;
-    mp.cap = ocap;
     mp.naggs = st->naggs;
     DF_CUDA(cudaMemsetAsync(st->d_counters, 0, (CTR_ERROR + 1) * 8, ctx->stream));  // slots CTR_GROUPS .. CTR_ERROR
     mp.counters = st->d_counters;
@@ -2954,7 +2908,7 @@ void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, DevBufs& rows_buf, 
     // number of entries any rank receives (known to all from the count matrix), which also makes it a valid send
     // buffer of the padded all-gather below; the sentinel slot's use and the count stay on the device
     d_owned = dalloc(max_recv * E);
-    compact_raw(st, ot, ocap, 0, st->d_counters + CTR_SENTINEL, d_owned, d_owned + 1, 1, (long long)E);
+    compact_raw(st, ot, 0, st->d_counters + CTR_SENTINEL, d_owned, d_owned + 1, 1, (long long)E);
   } else {
     DF_CUDA(cudaMemsetAsync(st->d_counters, 0, CTR_NONNULL * 8, ctx->stream));  // no entries, no merge error
   }
@@ -3245,7 +3199,6 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
       }
       for (size_t j = 0; j < st->dist_set.size(); j++) st->descs.push_back(AggDesc{DFGPU_AGG_COUNT, MT_U, DFGPU_UINT64, DFGPU_UINT64});
       st->typed = true;
-      st->cap = 0;
       st->t = table_alloc(ctx, st->naggs, st->nkeys, st->descs, 0, false);
     }
     // multi-GPU: every rank must take part (also one that saw no batch), and every rank gets the global result
@@ -3267,7 +3220,7 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
     }
     if (!st->dist_progs.empty()) {  // the COUNT(DISTINCT) words (single GPU: the exchange is refused above)
       if (st->nkeys == 0) distinct_count_scalar(st);
-      else distinct_count(st, st->t, st->cap, st->sentinel_used ? 1 : 0);
+      else distinct_count(st, st->t, st->sentinel_used ? 1 : 0);
     }
     auto res = std::make_unique<dfgpu_result>();
     res->ctx = ctx;
@@ -3276,7 +3229,6 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
     CompactParams cp;
     memset(&cp, 0, sizeof(cp));
     cp.t = st->t;
-    cp.cap = st->cap;
     cp.sentinel_used = st->nkeys == 0 ? 1 : (st->sentinel_used ? 1 : 0);
     cp.nkeys = st->nkeys;
     cp.naggs = st->naggs;
@@ -3354,7 +3306,7 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
     } else {
       DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_COMPACT, 0, 8, ctx->stream));
       cp.counter = st->d_counters + CTR_COMPACT;
-      launch_kernel(ctx, k_compact, "k_compact", cp, st->cap + 1, 256, 8);
+      launch_kernel(ctx, k_compact, "k_compact", cp, st->t.cap + 1, 256, 8);
       if ((long long)read_counter(st, CTR_COMPACT) != cnt) fail(DFGPU_ERR_INTERNAL, "table compaction count mismatch");
     }
     res->nrows = cnt;
