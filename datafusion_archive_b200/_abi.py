@@ -27,9 +27,11 @@ NP_OF = {
 DTYPE_OF_NP = {np.dtype(v): k for k, v in NP_OF.items()}
 
 # expression opcodes
-OP_COL, OP_LIT, OP_CAST = 1, 2, 3
+OP_COL, OP_LIT, OP_CAST, OP_LIT_UTF8 = 1, 2, 3, 4
 OP_ADD, OP_SUB, OP_MUL, OP_DIV = 10, 11, 12, 13
 OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE = 20, 21, 22, 23, 24, 25
+OP_LIKE, OP_NOT_LIKE = 26, 27
+UTF8_LITERAL_MAX = 4096  # longest Utf8 literal or LIKE pattern, in bytes
 OP_AND, OP_OR = 30, 31
 OP_FN = 40
 
@@ -56,7 +58,7 @@ class Col(C.Structure):
 
 
 class _Lit(C.Union):
-    _fields_ = [("f64", C.c_double), ("i64", C.c_int64), ("u64", C.c_uint64), ("f32", C.c_float)]
+    _fields_ = [("f64", C.c_double), ("i64", C.c_int64), ("u64", C.c_uint64), ("f32", C.c_float), ("str", C.c_void_p)]
 
 
 class Insn(C.Structure):

@@ -8,6 +8,7 @@
 // (linear probing, 64-bit packed keys claimed with atomicCAS) whose accumulators are updated with
 // fire-and-forget L2 reductions: RED.ADD.F64 for f64 SUM, RED.ADD.U64 for COUNT / integer SUM,
 // RED.MIN/MAX.U64 on an order-preserving encoding for MIN/MAX (bit-exact for every type).
+#include <deque>
 #include <memory>
 
 #include "expr_vm.cuh"
@@ -1309,11 +1310,15 @@ struct VerifyParams {
   const unsigned char* bytes;
   const Utf8Source* srcs;
   unsigned long long* flag;
+  int has_pred;  // a fused WHERE ran: a row it dropped may have no group
 };
 __global__ void __launch_bounds__(256) k_utf8_group_verify(const __grid_constant__ VerifyParams p) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += (long long)gridDim.x * blockDim.x) {
     const long long slot = p.t.find(p.hashes[i], true);
-    if (slot < 0) { *p.flag = 2ull; continue; }
+    if (slot < 0) {
+      if (!p.has_pred) *p.flag = 2ull;
+      continue;
+    }
     const unsigned long long rep = *p.t.val(slot, p.rep_agg);
     const Utf8Source& sc = p.srcs[rep >> UTF8_SRC_SHIFT];
     const long long r = (long long)(rep & ((1ull << UTF8_SRC_SHIFT) - 1ull));
@@ -1534,6 +1539,15 @@ struct dfgpu_aggstate {
   TableLayout t{};
   bool aos = false;        // "line" layout: every accumulator shares the line with the key (tables beyond L2)
   std::vector<dfgpu_insn> pred_prog;  // fused WHERE predicate (dfgpu_aggregate_set_predicate); empty = none
+  // the bytes of the DFGPU_OP_LIT_UTF8 literals of the kept programs: the caller's are borrowed for the call only
+  std::deque<std::string> utf8_lits;
+  void own_literals(std::vector<dfgpu_insn>& prog) {
+    for (dfgpu_insn& in : prog)
+      if (in.op == DFGPU_OP_LIT_UTF8 && in.col > 0 && in.lit.str) {  // malformed ones are refused when compiled
+        utf8_lits.emplace_back(in.lit.str, size_t(in.col));
+        in.lit.str = utf8_lits.back().data();
+      }
+  }
   bool use_front = false;  // route rows through the per-CTA shared-memory front table
   // wide keys: composite keys of more than 64 bits or with Utf8 parts (k_hash_agg_wide)
   bool wide = false;
@@ -1883,7 +1897,10 @@ extern "C" int dfgpu_aggregate_create(dfgpu_ctx* ctx, const dfgpu_insn* const* k
     st->nkeys = nkeys;
     st->naggs = naggs;
     st->expected = expected_groups;
-    for (int k = 0; k < nkeys; k++) st->key_progs.emplace_back(keys[k], keys[k] + key_len[k]);
+    for (int k = 0; k < nkeys; k++) {
+      st->key_progs.emplace_back(keys[k], keys[k] + key_len[k]);
+      st->own_literals(st->key_progs.back());
+    }
     std::vector<int> dist_user;  // user aggregates that are COUNT(DISTINCT)
     for (int a = 0; a < naggs; a++) {
       // compile_expr accepts min/max/count/sum (expression.rs:98-107), this engine also COUNT(DISTINCT) and AVG;
@@ -1891,6 +1908,7 @@ extern "C" int dfgpu_aggregate_create(dfgpu_ctx* ctx, const dfgpu_insn* const* k
       if (aggs[a].func < DFGPU_AGG_MIN || aggs[a].func > DFGPU_AGG_AVG)
         fail(DFGPU_ERR_GENERAL, "Unsupported aggregate function '" + std::to_string(aggs[a].func) + "'");
       std::vector<dfgpu_insn> prog(aggs[a].arg, aggs[a].arg + aggs[a].arg_len);
+      st->own_literals(prog);
       st->out_is_avg.push_back(aggs[a].func == DFGPU_AGG_AVG ? 1 : 0);
       if (aggs[a].func == DFGPU_AGG_AVG) {
         if (aggs[a].out_dtype != 0 && aggs[a].out_dtype != DFGPU_FLOAT64)
@@ -1947,6 +1965,7 @@ extern "C" int dfgpu_aggregate_set_predicate(dfgpu_aggstate* st, const dfgpu_ins
     if (!st || (pred_len > 0 && !pred)) fail(DFGPU_ERR_GENERAL, "dfgpu_aggregate_set_predicate: null argument");
     if (st->rows_seen > 0 || st->typed) fail(DFGPU_ERR_GENERAL, "the predicate must be set before the first batch");
     st->pred_prog.assign(pred, pred + (pred_len > 0 ? pred_len : 0));
+    st->own_literals(st->pred_prog);  // replayed on every update
   });
 }
 
@@ -2205,6 +2224,8 @@ void compile_batch(dfgpu_aggstate* st, const dfgpu_batch* batch, BatchPrograms& 
     retain_utf8(st, *bp.ukey, batch->nrows);
     upload_utf8_srcs(st);
   }
+  pb.eval_utf8_predicates(ctx);
+  bp.dpb.eval_utf8_predicates(ctx);
 }
 
 // Whether programs [has_pred] + nkeys keys + nargs arguments of `pb` fit the interpreter-free PlainSrc: at most 4 column
@@ -2557,6 +2578,7 @@ void verify_utf8_groups(dfgpu_aggstate* st, const BatchPrograms& bp, long long n
   vp.bytes = (const unsigned char*)bp.ukey->values;
   vp.srcs = st->d_utf8_srcs;
   vp.flag = st->d_counters + CTR_DEFERRED;
+  vp.has_pred = bp.has_pred;
   DF_CUDA(cudaMemsetAsync(vp.flag, 0, 8, ctx->stream));
   launch_kernel(ctx, k_utf8_group_verify, "k_utf8_group_verify", vp, nrows, 256, 8);
   const unsigned long long flag = read_counter(st, CTR_DEFERRED);

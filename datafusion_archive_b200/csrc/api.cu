@@ -521,7 +521,8 @@ extern "C" int dfgpu_batch_upload(dfgpu_ctx* ctx, const dfgpu_col* cols, int nco
         // only this batch's bytes [lo, hi) travel (a batch is often a slice of a long column: copying the
         // prefix [0, hi) for every batch is quadratic over a table); the device offsets are rebased by -lo
         d.values_bytes = size_t(hi - lo);
-        d.values = ctx->alloc(d.values_bytes);
+        // whole 16-byte words: the string predicates read aligned 16-byte words (utf8_predicate.cu)
+        d.values = ctx->alloc((d.values_bytes + 15) & ~size_t(15));
         if (hi > lo) h2d(ctx, d.values, static_cast<const uint8_t*>(c.values) + lo, size_t(hi - lo));
         rebase_offsets(ctx, d.offsets, c.len + 1, lo);
       } else {

@@ -22,12 +22,27 @@ namespace {
 
 struct Node {
   enum Kind { COL, LIT, CAST, BIN, FN } kind = COL;
-  int col = 0;
+  int col = 0;               // COL: batch column, or -1 - k for synthetic column k (a recognised Utf8 predicate)
   int dtype = 0;             // result dtype
   unsigned long long imm = 0;  // LIT payload, widened to the machine representation
   int op = 0;                // DFGPU_OP_* for BIN, DFGPU_FN_* for FN
+  std::string str;           // LIT of dtype Utf8: the bytes
   std::unique_ptr<Node> l, r;  // FN: the arguments (r: second argument of a two-argument function, else null)
 };
+
+bool is_utf8_lit(const Node* nd) { return nd->kind == Node::LIT && nd->dtype == DFGPU_UTF8; }
+
+// A Utf8 literal is an operand of a Utf8 comparison or LIKE only; anywhere else it keeps the reference's error
+// (expression.rs:306-309), spelled like ScalarValue's Debug
+void refuse_utf8_literal(const Node* nd) {
+  if (!nd || !is_utf8_lit(nd)) return;
+  std::string d = "Utf8(\"";
+  for (char ch : nd->str) {
+    if (ch == '"' || ch == '\\') d += '\\';
+    d += ch;
+  }
+  fail(DFGPU_ERR_EXECUTION, "No support for literal type " + d + "\")");
+}
 
 const char* op_debug_name(int op) {
   switch (op) {
@@ -140,10 +155,20 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
         nd->imm = widen_literal(in);
         break;
       }
+      case DFGPU_OP_LIT_UTF8: {  // Expr::Literal(ScalarValue::Utf8): the bytes are copied, the program's are borrowed
+        if (in.dtype != DFGPU_UTF8 || in.col < 0 || (!in.lit.str && in.col > 0)) fail(DFGPU_ERR_GENERAL, "malformed expression program");
+        if (in.col > DFGPU_UTF8_LITERAL_MAX)
+          fail(DFGPU_ERR_NOT_IMPLEMENTED, "Utf8 literal of " + std::to_string(in.col) + " bytes (at most " + std::to_string(DFGPU_UTF8_LITERAL_MAX) + ")");
+        nd->kind = Node::LIT;
+        nd->dtype = DFGPU_UTF8;
+        nd->str.assign(in.lit.str ? in.lit.str : "", size_t(in.col));
+        break;
+      }
       case DFGPU_OP_CAST: {  // Expr::Cast (expression.rs:316-378)
         if (st.empty()) fail(DFGPU_ERR_GENERAL, "malformed expression program");
         auto inner = std::move(st.back());
         st.pop_back();
+        refuse_utf8_literal(inner.get());
         if (inner->kind == Node::LIT) {
           // only Literal Int64 -> Float64 exists in the reference (expression.rs:345-373)
           if (inner->dtype != DFGPU_INT64)
@@ -184,6 +209,8 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
         }
         nd->l = std::move(st.back());
         st.pop_back();
+        refuse_utf8_literal(nd->l.get());
+        refuse_utf8_literal(nd->r.get());
         // monomorphic over Float64: the caller casts, as the planner does (sqlplanner.rs:343-365)
         for (const Node* a : {nd->l.get(), nd->r.get()})
           if (a && a->dtype != DFGPU_FLOAT64)
@@ -195,7 +222,8 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
         bool is_math = op >= DFGPU_OP_ADD && op <= DFGPU_OP_DIV;
         bool is_cmp = op >= DFGPU_OP_EQ && op <= DFGPU_OP_GE;
         bool is_bool = op == DFGPU_OP_AND || op == DFGPU_OP_OR;
-        if (!is_math && !is_cmp && !is_bool) fail(DFGPU_ERR_EXECUTION, "operator: " + std::to_string(op));
+        const bool is_like = op == DFGPU_OP_LIKE || op == DFGPU_OP_NOT_LIKE;
+        if (!is_math && !is_cmp && !is_bool && !is_like) fail(DFGPU_ERR_EXECUTION, "operator: " + std::to_string(op));
         if (st.size() < 2) fail(DFGPU_ERR_GENERAL, "malformed expression program");
         nd->kind = Node::BIN;
         nd->op = op;
@@ -204,6 +232,36 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
         nd->l = std::move(st.back());
         st.pop_back();
         int lt = nd->l->dtype, rt = nd->r->dtype;
+        if (!is_cmp && !is_like) {
+          refuse_utf8_literal(nd->l.get());
+          refuse_utf8_literal(nd->r.get());
+        }
+        // A maximal Utf8 comparison or LIKE (Utf8 operands are columns or literals: nothing else yields Utf8) becomes a
+        // Boolean synthetic column, filled by eval_utf8_predicates before the scan
+        if (is_like || (is_cmp && lt == DFGPU_UTF8 && rt == DFGPU_UTF8)) {
+          const char* name = op == DFGPU_OP_LIKE ? "Like" : op == DFGPU_OP_NOT_LIKE ? "NotLike" : op_debug_name(op);
+          if (lt != DFGPU_UTF8 || rt != DFGPU_UTF8)
+            fail(DFGPU_ERR_EXECUTION, std::string(name) + ": operands must be Utf8, not " + dtype_name(lt) + " and " + dtype_name(rt));
+          const bool llit = nd->l->kind == Node::LIT, rlit = nd->r->kind == Node::LIT;
+          if (llit && rlit) fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string(name) + " between two Utf8 literals");
+          if (is_like && !rlit) fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string(name) + " with a pattern that is not a literal");
+          Utf8Pred sp;
+          sp.op = op;
+          if (llit) {  // 'lit' op x  ==  x op' 'lit'
+            sp.op = op == DFGPU_OP_LT ? DFGPU_OP_GT : op == DFGPU_OP_LE ? DFGPU_OP_GE : op == DFGPU_OP_GT ? DFGPU_OP_LT : op == DFGPU_OP_GE ? DFGPU_OP_LE : op;
+            std::swap(nd->l, nd->r);
+          }
+          sp.a = nd->l->col;
+          sp.b = nd->r->kind == Node::COL ? nd->r->col : -1;
+          if (sp.b < 0) sp.lit = nd->r->str;
+          sp.synth = new_synth(nullptr, DFGPU_BOOL);
+          utf8_preds_.push_back(std::move(sp));
+          nd = std::make_unique<Node>();
+          nd->kind = Node::COL;
+          nd->col = -1 - utf8_preds_.back().synth;
+          nd->dtype = DFGPU_BOOL;
+          break;
+        }
         if (is_bool) {
           if (lt != DFGPU_BOOL || rt != DFGPU_BOOL)
             fail(DFGPU_ERR_INTERNAL, "boolean_ops: operand is not a BooleanArray (the reference panics here: expression.rs:217-221)");
@@ -218,6 +276,7 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
     st.push_back(std::move(nd));
   }
   if (st.size() != 1) fail(DFGPU_ERR_GENERAL, "malformed expression program");
+  refuse_utf8_literal(st[0].get());
 
   // 2. tree -> bytecode with right-hand leaf folding; track the live register-stack depth
   CompiledProgram cp;
@@ -228,7 +287,7 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
       const dfgpu_batch* b;
       bool go(const Node* nd) const {
         switch (nd->kind) {
-          case Node::COL: return b->cols[size_t(nd->col)].null_count > 0;
+          case Node::COL: return nd->col >= 0 && b->cols[size_t(nd->col)].null_count > 0;  // synthetic: never null
           case Node::LIT: return false;
           case Node::CAST: return go(nd->l.get());
           case Node::FN: return go(nd->l.get()) || (nd->r && go(nd->r.get()));  // like arithmetic
@@ -383,10 +442,15 @@ int ProgramBuilder::add_rowid_plus(unsigned long long bias) {
   return int(progs_.size()) - 1;
 }
 
-int ProgramBuilder::add_synthetic_column(const void* dptr, int dtype) {
+int ProgramBuilder::new_synth(const void* dptr, int dtype) {
   if (int(slots_.size()) >= kMaxCols) fail(DFGPU_ERR_NOT_IMPLEMENTED, "too many distinct columns");
   synth_.push_back(Synth{dptr, dtype});
   slots_.push_back(-int(synth_.size()));  // -1 - k
+  return int(synth_.size()) - 1;
+}
+
+int ProgramBuilder::add_synthetic_column(const void* dptr, int dtype) {
+  new_synth(dptr, dtype);
   CompiledProgram cp;
   DevInsn di;
   memset(&di, 0, sizeof(di));
@@ -403,6 +467,7 @@ int ProgramBuilder::add_synthetic_column(const void* dptr, int dtype) {
 
 void ProgramBuilder::finish(ProgramSet* out) const {
   memset(out, 0, sizeof(*out));
+  if (!utf8_preds_.empty() && !utf8_evaluated_ && batch_->ctx) fail(DFGPU_ERR_INTERNAL, "Utf8 predicates not evaluated before the scan");
   if (int(progs_.size()) > kMaxProgs)
     fail(DFGPU_ERR_NOT_IMPLEMENTED, "more than " + std::to_string(kMaxProgs) + " expressions in one operator");
   int pc = 0, maxd = 1;

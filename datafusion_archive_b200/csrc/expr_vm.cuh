@@ -103,9 +103,22 @@ struct CompiledProgram {
   LeafChain chain{};  // nterms > 0: the program is a chain of comparisons joined by AND / OR
 };
 
+// A Utf8 comparison or LIKE that ProgramBuilder::add recognised.  It is evaluated before the operator's scan, into a
+// bit-packed Boolean column without nulls (utf8_predicate.cu), and the program reads that column as synthetic column
+// `synth`.  No string code runs inside the scan kernels.
+struct Utf8Pred {
+  int op;           // DFGPU_OP_EQ .. DFGPU_OP_GE (a literal on the left already mirrored), DFGPU_OP_LIKE, DFGPU_OP_NOT_LIKE
+  int a, b;         // batch columns: a op b, or a op lit when b < 0
+  std::string lit;  // the literal, or the LIKE pattern (a copy: the program's bytes are borrowed)
+  int synth;        // synthetic column index
+};
+
 class ProgramBuilder {
  public:
   explicit ProgramBuilder(const dfgpu_batch* batch) : batch_(batch) {}
+  ProgramBuilder(const ProgramBuilder&) = delete;
+  ProgramBuilder& operator=(const ProgramBuilder&) = delete;
+  ~ProgramBuilder();  // returns the predicate bitmaps to the ctx pool
   // Type-check + lower one postfix program; appends to the set and returns its index.
   int add(const dfgpu_insn* p, int n, const char* what);
   // Program yielding the global row number (UInt64): the gather index for variable-width columns.
@@ -120,9 +133,18 @@ class ProgramBuilder {
   // Finalise into the POD passed to kernels.
   void finish(ProgramSet* out) const;
   int slot_of_column(int col);
+  // Evaluate the recognised Utf8 predicates over the batch on ctx->stream and point their synthetic columns at the
+  // bitmaps (utf8_predicate.cu).  Every operator calls it once per batch, after the last add() and before finish().
+  void eval_utf8_predicates(dfgpu_ctx* ctx);
+  const std::vector<Utf8Pred>& utf8_preds() const { return utf8_preds_; }
 
  private:
+  int new_synth(const void* dptr, int dtype);  // a synthetic column slot; returns the synthetic index
   const dfgpu_batch* batch_;
+  std::vector<Utf8Pred> utf8_preds_;
+  bool utf8_evaluated_ = false;
+  dfgpu_ctx* ctx_ = nullptr;  // of owned_
+  std::vector<void*> owned_;  // device bitmaps and literals of utf8_preds_
   std::vector<CompiledProgram> progs_;
   std::vector<int> slots_;  // slot -> batch column index, or -1 - k for synthetic column k
   struct Synth { const void* ptr; int dtype; };

@@ -224,7 +224,7 @@ extern "C" int dfgpu_check_program(const int32_t* col_dtypes, int ncols, const d
     }
     ProgramBuilder pb(&schema_only);
     const int pi = pb.add(prog, prog_len, "expression");
-    ProgramSet ps;
+    ProgramSet ps;  // Utf8 predicates are typed, not evaluated
     pb.finish(&ps);  // instruction / column-slot limits
     *out_dtype = pb.out_dtype(pi);
   });
@@ -286,6 +286,7 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
       pb.add_rowid();
       rowid_slot = nkern++;
     }
+    pb.eval_utf8_predicates(ctx);
     // columns referenced anywhere must be null-free and fixed width for now
     FPParams p;
     pb.finish(&p.ps);

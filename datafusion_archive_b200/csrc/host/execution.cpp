@@ -262,6 +262,14 @@ void lower(const Expr& e, const Schema& schema, const std::map<size_t, int>& rem
     }
     case Expr::Literal: {
       const ScalarValue& v = e.value;
+      if (v.dtype == DFGPU_UTF8) {  // an operand of a Utf8 comparison or LIKE; the engine refuses it anywhere else
+        in.op = DFGPU_OP_LIT_UTF8;
+        in.dtype = DFGPU_UTF8;
+        in.col = int(v.s.size());
+        in.lit.str = v.s.data();  // the plan's ScalarValue outlives the call
+        out.push_back(in);
+        return;
+      }
       if (!(v.dtype >= DFGPU_INT8 && v.dtype <= DFGPU_FLOAT64))
         fail(DFGPU_ERR_EXECUTION, "No support for literal type " + v.debug());  // expression.rs:306-309
       in.op = DFGPU_OP_LIT;
@@ -295,6 +303,8 @@ void lower(const Expr& e, const Schema& schema, const std::map<size_t, int>& rem
         case Operator::Minus: in.op = DFGPU_OP_SUB; break;
         case Operator::Multiply: in.op = DFGPU_OP_MUL; break;
         case Operator::Divide: in.op = DFGPU_OP_DIV; break;
+        case Operator::Like: in.op = DFGPU_OP_LIKE; break;
+        case Operator::NotLike: in.op = DFGPU_OP_NOT_LIKE; break;
         default: fail(DFGPU_ERR_EXECUTION, std::string("operator: ") + operator_debug(e.op));  // expression.rs:494-497
       }
       out.push_back(in);

@@ -210,6 +210,18 @@ def check_program(schema_dtypes, expr):
     return out.value
 
 
+def utf8_like_host(s, pattern):
+    """dfgpu_utf8_like_host: (match, pattern class) of `s LIKE pattern` (bytes or str) by the engine's own pattern
+    compiler and matcher, on the host.  Classes: 0 exact, 1 prefix, 2 suffix, 3 contains, 4 general."""
+    s = s.encode("utf-8") if isinstance(s, str) else bytes(s)
+    pattern = pattern.encode("utf-8") if isinstance(pattern, str) else bytes(pattern)
+    m, cls = C.c_int32(), C.c_int32()
+    L = lib()
+    L.dfgpu_utf8_like_host.argtypes = [C.c_char_p, C.c_int64, C.c_char_p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    check(L.dfgpu_utf8_like_host(s, len(s), pattern, len(pattern), C.byref(m), C.byref(cls)))
+    return bool(m.value), cls.value
+
+
 class Batch:
     def __init__(self, ctx, handle, schema):
         self.ctx, self.h, self.schema = ctx, handle, schema

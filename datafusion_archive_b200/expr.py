@@ -5,15 +5,17 @@ The production host layer is the C++ mirror under csrc/host/ (the reference is c
 this module only exists so tests read like the reference's own tests, which build `Expr` by hand
 (src/execution/aggregate.rs:971-988).
 """
+import ctypes as C
 import struct
 
 from . import _abi as A
 
 _CMP = {A.OP_EQ, A.OP_NE, A.OP_LT, A.OP_LE, A.OP_GT, A.OP_GE}
-_BOOLOP = {A.OP_AND, A.OP_OR}
+_BOOLOP = {A.OP_AND, A.OP_OR, A.OP_LIKE, A.OP_NOT_LIKE}
 _OPNAME = {
     A.OP_ADD: "Plus", A.OP_SUB: "Minus", A.OP_MUL: "Multiply", A.OP_DIV: "Divide", A.OP_EQ: "Eq", A.OP_NE: "NotEq",
     A.OP_LT: "Lt", A.OP_LE: "LtEq", A.OP_GT: "Gt", A.OP_GE: "GtEq", A.OP_AND: "And", A.OP_OR: "Or",
+    A.OP_LIKE: "Like", A.OP_NOT_LIKE: "NotLike",
 }
 
 
@@ -33,6 +35,8 @@ class Expr:
     def not_eq(self, o): return self._bin(A.OP_NE, o)
     def __and__(self, o): return self._bin(A.OP_AND, o)
     def __or__(self, o): return self._bin(A.OP_OR, o)
+    def like(self, pattern): return self._bin(A.OP_LIKE, pattern)
+    def not_like(self, pattern): return self._bin(A.OP_NOT_LIKE, pattern)
 
     def cast(self, dtype):
         return Cast(self, dtype)
@@ -62,12 +66,17 @@ class Column(Expr):
 
 class Literal(Expr):
     """Expr::Literal(ScalarValue); default typing follows the planner: Python int -> Int64,
-    float -> Float64 (src/sqlplanner.rs:214-218)."""
+    float -> Float64, str -> Utf8 (src/sqlplanner.rs:214-218).  A Utf8 literal (str or bytes) is emitted as
+    DFGPU_OP_LIT_UTF8 pointing at an encoded copy that every emitted instruction keeps alive."""
 
     def __init__(self, value, dtype=None):
         if dtype is None:
-            dtype = A.FLOAT64 if isinstance(value, float) else A.INT64
+            dtype = A.UTF8 if isinstance(value, (str, bytes)) else A.FLOAT64 if isinstance(value, float) else A.INT64
         self.value, self.dtype = value, dtype
+        if dtype == A.UTF8:
+            raw = value.encode("utf-8") if isinstance(value, str) else bytes(value)
+            self._bytes = C.create_string_buffer(raw, max(1, len(raw)))
+            self._len = len(raw)
 
     def get_type(self, schema):
         return self.dtype
@@ -75,7 +84,11 @@ class Literal(Expr):
     def _emit(self, schema, out):
         i = A.Insn()
         i.op, i.dtype = A.OP_LIT, self.dtype
-        if self.dtype == A.FLOAT64:
+        if self.dtype == A.UTF8:
+            i.op, i.col = A.OP_LIT_UTF8, self._len
+            i.lit.str = C.addressof(self._bytes)
+            i._keep = self._bytes  # the program borrows the bytes: they live as long as the instruction
+        elif self.dtype == A.FLOAT64:
             i.lit.f64 = float(self.value)
         elif self.dtype == A.FLOAT32:
             i.lit.u64 = 0

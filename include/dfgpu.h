@@ -86,6 +86,11 @@ enum {
   DFGPU_OP_COL = 1,  /* Expr::Column(col)                         expression.rs:311-315 */
   DFGPU_OP_LIT = 2,  /* Expr::Literal(ScalarValue)                expression.rs:226-243 */
   DFGPU_OP_CAST = 3, /* Expr::Cast{expr,data_type}                expression.rs:246-280,316-378 */
+  DFGPU_OP_LIT_UTF8 = 4, /* Expr::Literal(ScalarValue::Utf8): `lit.str` = address of the bytes, `col` = byte length (>= 0;
+                            0 = ''), `dtype` = DFGPU_UTF8.  The bytes are borrowed for the call; a program the library keeps
+                            past the call (dfgpu_aggregate_create / _set_predicate) owns a copy.  A negative length or a
+                            null address with a nonzero length is DFGPU_ERR_GENERAL "malformed expression program".
+                            DFGPU_OP_LIT with dtype DFGPU_UTF8 stays "No support for literal type Utf8".  Additive. */
   DFGPU_OP_ADD = 10, /* Operator::Plus     → array_ops::add       expression.rs:466 */
   DFGPU_OP_SUB = 11, /* Operator::Minus    → array_ops::subtract  expression.rs:473 */
   DFGPU_OP_MUL = 12, /* Operator::Multiply → array_ops::multiply  expression.rs:480 */
@@ -96,6 +101,8 @@ enum {
   DFGPU_OP_LE = 23,  /* array_ops::lt_eq   expression.rs:431 */
   DFGPU_OP_GT = 24,  /* array_ops::gt      expression.rs:438 */
   DFGPU_OP_GE = 25,  /* array_ops::gt_eq   expression.rs:445 */
+  DFGPU_OP_LIKE = 26,     /* Operator::Like    (sqlparser.rs / logicalplan.rs Operator), postfix `x p`; see Utf8 predicates */
+  DFGPU_OP_NOT_LIKE = 27, /* Operator::NotLike */
   DFGPU_OP_AND = 30, /* array_ops::and     expression.rs:452 */
   DFGPU_OP_OR = 31,  /* array_ops::or      expression.rs:459 */
   DFGPU_OP_FN = 40   /* Expr::ScalarFunction{name,args,return_type} logicalplan.rs:156-160: `col` = DFGPU_FN_* code,
@@ -131,9 +138,26 @@ enum {
   DFGPU_FN_ATAN2 = 19  /* f64::atan2(y, x), two arguments */
 };
 
+/* Utf8 predicates (the reference plans them but executes neither: comparison_ops! has no Utf8 arm,
+ * expression.rs:171-209, and literals other than numbers are refused, :306-309).
+ *   - DFGPU_OP_EQ .. DFGPU_OP_GE between two Utf8 operands: a column against a DFGPU_OP_LIT_UTF8 literal (on either
+ *     side) or against another Utf8 column.  Byte-wise lexicographic order, a proper prefix first (Rust's [u8] Ord;
+ *     for valid UTF-8 this is code-point order).  The bytes are never validated.  Nulls as for every numeric
+ *     comparison: null equals null, null orders below every string including '', and the result has no nulls.
+ *   - DFGPU_OP_LIKE / DFGPU_OP_NOT_LIKE: `x` a Utf8 column, `p` a Utf8 literal.  `%` matches any run of characters
+ *     (possibly empty), `_` exactly one; a character is one UTF-8 code point: a byte that is not 10xxxxxx starts one.
+ *     Case-sensitive, no escape character (`\` is an ordinary byte).  A null `x` satisfies neither LIKE nor NOT LIKE;
+ *     the result has no nulls.
+ *   - They may appear wherever a Boolean may: WHERE, a Boolean projection, the aggregate's fused WHERE, under AND / OR.
+ *   - Refused: a non-literal pattern and literal against literal (DFGPU_ERR_NOT_IMPLEMENTED); non-Utf8 LIKE operands
+ *     (DFGPU_ERR_EXECUTION naming the operator); Utf8 against a number ("comparison_ops"); a Utf8 literal anywhere
+ *     else (DFGPU_ERR_EXECUTION "No support for literal type Utf8(..)"); a literal or pattern longer than
+ *     DFGPU_UTF8_LITERAL_MAX bytes (DFGPU_ERR_NOT_IMPLEMENTED). */
+#define DFGPU_UTF8_LITERAL_MAX 4096
+
 typedef struct dfgpu_insn {
   int32_t op;
-  int32_t col;   /* COL: column index; CAST: source dtype */
+  int32_t col;   /* COL: column index; CAST: source dtype; LIT_UTF8: byte length */
   int32_t dtype; /* see above */
   int32_t _pad;
   union {
@@ -141,6 +165,7 @@ typedef struct dfgpu_insn {
     int64_t i64;
     uint64_t u64;
     float f32;
+    const char* str; /* LIT_UTF8: address of the literal's bytes */
   } lit;
 } dfgpu_insn;
 
@@ -219,6 +244,10 @@ int dfgpu_batch_free(dfgpu_batch* b);
  * rules, Float64 arguments and the arity of DFGPU_OP_FN, column indices.  `out_dtype` receives the result
  * type.  Usable on a machine with no device. */
 int dfgpu_check_program(const int32_t* col_dtypes, int ncols, const dfgpu_insn* prog, int prog_len, int32_t* out_dtype);
+/* The LIKE matcher alone, on the host, for one string: compiles `pattern` exactly as the operators do and matches
+ * `s` with the matcher of the pattern's class.  *match = 1 / 0; *pattern_class = 0 exact, 1 prefix `abc%`, 2 suffix
+ * `%abc`, 3 contains `%abc%`, 4 general.  Usable on a machine with no device. */
+int dfgpu_utf8_like_host(const char* s, int64_t s_len, const char* pattern, int64_t pattern_len, int32_t* match, int32_t* pattern_class);
 
 /* ---- FilterRelation + ProjectRelation fused (src/execution/filter.rs:46-110,
  *      src/execution/projection.rs:46-66, wiring at src/execution/context.rs:126-161) ----

@@ -29,6 +29,8 @@ pub const DT_UTF8: i32 = 12;
 pub const OP_COL: i32 = 1;
 pub const OP_LIT: i32 = 2;
 pub const OP_CAST: i32 = 3;
+/// Expr::Literal(ScalarValue::Utf8): `lit` = address of the bytes (borrowed for the call), `col` = byte length.
+pub const OP_LIT_UTF8: i32 = 4;
 pub const OP_ADD: i32 = 10;
 pub const OP_SUB: i32 = 11;
 pub const OP_MUL: i32 = 12;
@@ -39,6 +41,9 @@ pub const OP_LT: i32 = 22;
 pub const OP_LE: i32 = 23;
 pub const OP_GT: i32 = 24;
 pub const OP_GE: i32 = 25;
+/// Operator::Like / NotLike: `x p`, x a Utf8 column, p a Utf8 literal
+pub const OP_LIKE: i32 = 26;
+pub const OP_NOT_LIKE: i32 = 27;
 pub const OP_AND: i32 = 30;
 pub const OP_OR: i32 = 31;
 /// Expr::ScalarFunction of a built-in function: `col` = FN_* code, `dtype` = Float64, arguments first.
@@ -89,7 +94,8 @@ pub struct dfgpu_col {
     pub values_bytes: i64,
 }
 
-/// One postfix instruction of an expression program (dfgpu_insn; `lit` carries f64 / i64 / u64 / f32 bits).
+/// One postfix instruction of an expression program (dfgpu_insn; `lit` carries f64 / i64 / u64 / f32 bits, or for
+/// OP_LIT_UTF8 the address of the literal's bytes, which the caller keeps alive for the call).
 #[repr(C)]
 #[derive(Clone, Copy)]
 pub struct dfgpu_insn {
@@ -164,6 +170,8 @@ extern "C" {
     pub fn dfgpu_batch_rows(b: *const dfgpu_batch, nrows: *mut i64) -> c_int;
     /// type check of one expression program without a device (the checks compile_scalar_expr makes: expression.rs:136-290)
     pub fn dfgpu_check_program(col_dtypes: *const i32, ncols: c_int, prog: *const dfgpu_insn, prog_len: c_int, out_dtype: *mut i32) -> c_int;
+    /// the LIKE pattern compiler and matcher on the host, for one string
+    pub fn dfgpu_utf8_like_host(s: *const c_char, s_len: i64, pattern: *const c_char, pattern_len: i64, is_match: *mut i32, pattern_class: *mut i32) -> c_int;
     pub fn dfgpu_result_col_device_ptr(r: *const dfgpu_result, i: c_int, dptr: *mut *const c_void) -> c_int;
 }
 

@@ -61,6 +61,8 @@ fn op_code(op: &Operator) -> Result<i32> {
         Operator::Minus => OP_SUB,
         Operator::Multiply => OP_MUL,
         Operator::Divide => OP_DIV,
+        Operator::Like => OP_LIKE,
+        Operator::NotLike => OP_NOT_LIKE,
         other => return Err(ExecutionError::ExecutionError(format!("operator: {:?}", other))), // expression.rs:494-497
     })
 }
@@ -84,6 +86,14 @@ pub fn lower(e: &Expr, schema: &Schema, remap: &[Option<usize>], out: &mut Vec<d
         Expr::Column(i) => {
             let at = remap.get(*i).and_then(|x| *x).ok_or_else(|| ExecutionError::InvalidColumn(format!("column index {} out of range", i)))?;
             out.push(insn(OP_COL, at as i32, dtype_code(schema.field(*i).data_type())?, 0));
+        }
+        // a Utf8 literal: `lit` = address of the bytes, `col` = their length.  The plan's ScalarValue outlives the call,
+        // and the engine copies the bytes of any program it keeps (dfgpu_aggregate_create / _set_predicate).
+        Expr::Literal(ScalarValue::Utf8(s)) => {
+            if s.len() > i32::MAX as usize {
+                return Err(ExecutionError::NotImplemented("Utf8 literal longer than 2^31 bytes".to_string()));
+            }
+            out.push(insn(OP_LIT_UTF8, s.len() as i32, DT_UTF8, s.as_ptr() as usize as u64));
         }
         Expr::Literal(v) => {
             let (dt, bits) = literal(v)?;
