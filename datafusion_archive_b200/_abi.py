@@ -47,6 +47,15 @@ FN_CODES = {
 }
 FN_ARITY = {code: (2 if code in (FN_POWER, FN_ATAN2) else 1) for code in FN_CODES.values()}
 
+# Utf8 functions (DFGPU_OP_UTF8_FN: `col` = code, `dtype` = result type); the Utf8 operand first, then Int64 literals
+OP_UTF8_FN = 41
+UTF8FN_UPPER, UTF8FN_LOWER, UTF8FN_TRIM, UTF8FN_LTRIM, UTF8FN_RTRIM = 1, 2, 3, 4, 5
+UTF8FN_SUBSTR_FROM, UTF8FN_SUBSTR, UTF8FN_LENGTH, UTF8FN_OCTET_LENGTH = 6, 7, 8, 9
+UTF8_FN_CODES = {
+    "upper": UTF8FN_UPPER, "lower": UTF8FN_LOWER, "trim": UTF8FN_TRIM, "ltrim": UTF8FN_LTRIM, "rtrim": UTF8FN_RTRIM,
+    "substr": UTF8FN_SUBSTR, "length": UTF8FN_LENGTH, "char_length": UTF8FN_LENGTH, "octet_length": UTF8FN_OCTET_LENGTH,
+}
+
 AGG_MIN, AGG_MAX, AGG_SUM, AGG_COUNT, AGG_COUNT_DISTINCT, AGG_AVG = 1, 2, 3, 4, 5, 6
 
 

@@ -1,6 +1,7 @@
 // expr_compile.cu — host half of the expression VM: type-check a postfix program the way
 // compile_scalar_expr would (src/execution/expression.rs:283-505), fold right-hand leaves into the
 // consuming instruction, and emit the device bytecode of expr_vm.cuh.
+#include <climits>
 #include <memory>
 
 #include "expr_vm.cuh"
@@ -21,14 +22,18 @@ MType mtype_of(int dt) {
 namespace {
 
 struct Node {
-  enum Kind { COL, LIT, CAST, BIN, FN } kind = COL;
-  int col = 0;               // COL: batch column, or -1 - k for synthetic column k (a recognised Utf8 predicate)
+  enum Kind { COL, LIT, CAST, BIN, FN, UFN } kind = COL;
+  int col = 0;               // COL: batch column, or -1 - k for synthetic column k (a recognised Utf8 predicate or
+                             // function); kViewCol for a Utf8 view that no program reads
+  int view = -1;             // COL of a Utf8 view: its index
   int dtype = 0;             // result dtype
-  unsigned long long imm = 0;  // LIT payload, widened to the machine representation
-  int op = 0;                // DFGPU_OP_* for BIN, DFGPU_FN_* for FN
+  unsigned long long imm = 0;  // LIT payload, widened to the machine representation; UFN: start
+  long long count = 0;       // UFN: count
+  int op = 0;                // DFGPU_OP_* for BIN, DFGPU_FN_* for FN, DFGPU_UTF8FN_* for UFN
   std::string str;           // LIT of dtype Utf8: the bytes
-  std::unique_ptr<Node> l, r;  // FN: the arguments (r: second argument of a two-argument function, else null)
+  std::unique_ptr<Node> l, r;  // FN: the arguments (r: second argument of a two-argument function, else null); UFN: l
 };
+constexpr int kViewCol = INT_MIN;
 
 bool is_utf8_lit(const Node* nd) { return nd->kind == Node::LIT && nd->dtype == DFGPU_UTF8; }
 
@@ -75,6 +80,13 @@ const char* fn_name(int code) {
   return code >= 1 && code <= DFGPU_FN_ATAN2 ? names[code] : nullptr;
 }
 int fn_arity(int code) { return code == DFGPU_FN_POWER || code == DFGPU_FN_ATAN2 ? 2 : 1; }
+
+// DFGPU_UTF8FN_* code -> SQL name, nullptr for an unknown code; the number of Int64 literal arguments after the string
+const char* utf8_fn_name(int code) {
+  static const char* const names[] = {nullptr, "upper", "lower", "trim", "ltrim", "rtrim", "substr", "substr", "length", "octet_length"};
+  return code >= 1 && code <= DFGPU_UTF8FN_OCTET_LENGTH ? names[code] : nullptr;
+}
+int utf8_fn_nlits(int code) { return code == DFGPU_UTF8FN_SUBSTR ? 2 : code == DFGPU_UTF8FN_SUBSTR_FROM ? 1 : 0; }
 
 VOp vop_of(int op) {
   switch (op) {
@@ -131,8 +143,49 @@ int ProgramBuilder::slot_of_column(int col) {
   return int(slots_.size()) - 1;
 }
 
-int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
+int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what, int* utf8_view) {
+  if (utf8_view) *utf8_view = -1;
   if (n <= 0 || !p) fail(DFGPU_ERR_GENERAL, std::string("empty expression program for ") + what);
+  // A maximal nest of Utf8 functions becomes one Utf8View when something other than a Utf8 function consumes it: an
+  // Int64 result is a synthetic column, a Utf8 one a COL node naming the view (read by Utf8 predicates only)
+  auto lower_view = [&](std::unique_ptr<Node>& x) {
+    if (!x || x->kind != Node::UFN) return;
+    std::vector<const Node*> nest;  // outermost first
+    const Node* q = x.get();
+    for (; q->kind == Node::UFN; q = q->l.get()) nest.push_back(q);
+    Utf8View v;
+    memset(&v.spec, 0, sizeof(v.spec));
+    v.src = q->col;
+    v.synth = -1;
+    v.projection = false;
+    for (auto it = nest.rbegin(); it != nest.rend(); ++it) {
+      const int code = (*it)->op;
+      if (code == DFGPU_UTF8FN_UPPER || code == DFGPU_UTF8FN_LOWER) {
+        v.spec.case_map = code;  // the outermost one wins
+      } else if (code == DFGPU_UTF8FN_LENGTH || code == DFGPU_UTF8FN_OCTET_LENGTH) {
+        v.spec.result = code;  // Int64: always the outermost function
+      } else {
+        if (v.spec.nsteps == kMaxUtf8Steps)
+          fail(DFGPU_ERR_NOT_IMPLEMENTED, "more than " + std::to_string(kMaxUtf8Steps) + " nested trim / substr calls");
+        Utf8Step& s = v.spec.step[v.spec.nsteps++];
+        s.op = code == DFGPU_UTF8FN_SUBSTR_FROM ? DFGPU_UTF8FN_SUBSTR : code;
+        s.start = (long long)(*it)->imm;
+        s.count = code == DFGPU_UTF8FN_SUBSTR_FROM ? -1 : (*it)->count;
+      }
+    }
+    const int dtype = x->dtype;
+    utf8_views_.push_back(v);
+    x = std::make_unique<Node>();
+    x->kind = Node::COL;
+    x->dtype = dtype;
+    x->view = int(utf8_views_.size()) - 1;
+    if (dtype == DFGPU_INT64) {
+      utf8_views_.back().synth = new_synth(nullptr, DFGPU_INT64, v.src);
+      x->col = -1 - utf8_views_.back().synth;
+    } else {
+      x->col = kViewCol;
+    }
+  };
   // 1. postfix -> tree, with the reference's type rules
   std::vector<std::unique_ptr<Node>> st;
   for (int i = 0; i < n; i++) {
@@ -168,6 +221,7 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
         if (st.empty()) fail(DFGPU_ERR_GENERAL, "malformed expression program");
         auto inner = std::move(st.back());
         st.pop_back();
+        lower_view(inner);
         refuse_utf8_literal(inner.get());
         if (inner->kind == Node::LIT) {
           // only Literal Int64 -> Float64 exists in the reference (expression.rs:345-373)
@@ -209,12 +263,43 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
         }
         nd->l = std::move(st.back());
         st.pop_back();
+        lower_view(nd->l);
+        lower_view(nd->r);
         refuse_utf8_literal(nd->l.get());
         refuse_utf8_literal(nd->r.get());
         // monomorphic over Float64: the caller casts, as the planner does (sqlplanner.rs:343-365)
         for (const Node* a : {nd->l.get(), nd->r.get()})
           if (a && a->dtype != DFGPU_FLOAT64)
             fail(DFGPU_ERR_EXECUTION, std::string("function '") + name + "' takes Float64 arguments, not " + dtype_name(a->dtype));
+        break;
+      }
+      case DFGPU_OP_UTF8_FN: {  // Expr::ScalarFunction of a Utf8 function (see "Utf8 functions" in dfgpu.h)
+        const char* name = utf8_fn_name(in.col);
+        if (!name) fail(DFGPU_ERR_EXECUTION, "unknown Utf8 function code " + std::to_string(in.col));
+        const int nlits = utf8_fn_nlits(in.col);
+        const bool is_len = in.col == DFGPU_UTF8FN_LENGTH || in.col == DFGPU_UTF8FN_OCTET_LENGTH;
+        if (in.dtype != (is_len ? DFGPU_INT64 : DFGPU_UTF8)) fail(DFGPU_ERR_GENERAL, "malformed expression program");
+        if (int(st.size()) < 1 + nlits)
+          fail(DFGPU_ERR_EXECUTION, std::string("function '") + name + "' takes " + std::to_string(1 + nlits) + (nlits ? " arguments" : " argument"));
+        long long arg[2] = {0, 0};
+        for (int k = nlits - 1; k >= 0; k--) {
+          const auto& a = st.back();
+          if (a->kind != Node::LIT || a->dtype != DFGPU_INT64)
+            fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string("function '") + name + "': start and count must be Int64 literals");
+          arg[k] = (long long)a->imm;
+          st.pop_back();
+        }
+        nd->kind = Node::UFN;
+        nd->op = in.col;
+        nd->dtype = in.dtype;
+        nd->l = std::move(st.back());
+        st.pop_back();
+        if (is_utf8_lit(nd->l.get())) fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string("function '") + name + "' over a Utf8 literal");
+        if (nd->l->dtype != DFGPU_UTF8 || (nd->l->kind != Node::COL && nd->l->kind != Node::UFN))
+          fail(DFGPU_ERR_EXECUTION, std::string("function '") + name + "' takes a Utf8 argument, not " + dtype_name(nd->l->dtype));
+        if (nlits == 2 && arg[1] < 0) fail(DFGPU_ERR_EXECUTION, "negative substring length not allowed");
+        nd->imm = (unsigned long long)arg[0];
+        nd->count = arg[1];
         break;
       }
       default: {
@@ -231,6 +316,8 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
         st.pop_back();
         nd->l = std::move(st.back());
         st.pop_back();
+        lower_view(nd->l);
+        lower_view(nd->r);
         int lt = nd->l->dtype, rt = nd->r->dtype;
         if (!is_cmp && !is_like) {
           refuse_utf8_literal(nd->l.get());
@@ -251,8 +338,9 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
             sp.op = op == DFGPU_OP_LT ? DFGPU_OP_GT : op == DFGPU_OP_LE ? DFGPU_OP_GE : op == DFGPU_OP_GT ? DFGPU_OP_LT : op == DFGPU_OP_GE ? DFGPU_OP_LE : op;
             std::swap(nd->l, nd->r);
           }
-          sp.a = nd->l->col;
-          sp.b = nd->r->kind == Node::COL ? nd->r->col : -1;
+          auto ref = [](const Node* x) { return x->view >= 0 ? -2 - x->view : x->col; };
+          sp.a = ref(nd->l.get());
+          sp.b = nd->r->kind == Node::COL ? ref(nd->r.get()) : -1;
           if (sp.b < 0) sp.lit = nd->r->str;
           sp.synth = new_synth(nullptr, DFGPU_BOOL);
           utf8_preds_.push_back(std::move(sp));
@@ -277,6 +365,17 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
   }
   if (st.size() != 1) fail(DFGPU_ERR_GENERAL, "malformed expression program");
   refuse_utf8_literal(st[0].get());
+  lower_view(st[0]);
+  if (st[0]->kind == Node::COL && st[0]->col == kViewCol) {  // the program's value is a Utf8 function nest
+    Utf8View& v = utf8_views_[size_t(st[0]->view)];
+    if (utf8_view) {
+      v.projection = true;
+      *utf8_view = st[0]->view;
+      return -1;
+    }
+    v.synth = new_synth(nullptr, DFGPU_UTF8, v.src);  // typed as Utf8; every operator refuses a Utf8 program value
+    st[0]->col = -1 - v.synth;
+  }
 
   // 2. tree -> bytecode with right-hand leaf folding; track the live register-stack depth
   CompiledProgram cp;
@@ -285,9 +384,12 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
     // comparisons never produce nulls)
     struct N {
       const dfgpu_batch* b;
+      const ProgramBuilder* pb;
       bool go(const Node* nd) const {
         switch (nd->kind) {
-          case Node::COL: return nd->col >= 0 && b->cols[size_t(nd->col)].null_count > 0;  // synthetic: never null
+          case Node::COL:
+            if (nd->col == kViewCol) return false;  // read by a Utf8 predicate only, whose result is never null
+            return nd->col >= 0 ? b->cols[size_t(nd->col)].null_count > 0 : pb->synth_nullable(-1 - nd->col);
           case Node::LIT: return false;
           case Node::CAST: return go(nd->l.get());
           case Node::FN: return go(nd->l.get()) || (nd->r && go(nd->r.get()));  // like arithmetic
@@ -297,7 +399,7 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what) {
           }
         }
       }
-    } nn{batch_};
+    } nn{batch_, this};
     cp.nullable = nn.go(st[0].get());
   }
   int depth = 0;
@@ -442,11 +544,17 @@ int ProgramBuilder::add_rowid_plus(unsigned long long bias) {
   return int(progs_.size()) - 1;
 }
 
-int ProgramBuilder::new_synth(const void* dptr, int dtype) {
+int ProgramBuilder::new_synth(const void* dptr, int dtype, int src) {
   if (int(slots_.size()) >= kMaxCols) fail(DFGPU_ERR_NOT_IMPLEMENTED, "too many distinct columns");
-  synth_.push_back(Synth{dptr, dtype});
+  synth_.push_back(Synth{dptr, dtype, src});
   slots_.push_back(-int(synth_.size()));  // -1 - k
   return int(synth_.size()) - 1;
+}
+
+// A Utf8 predicate's bitmap is never null; a Utf8 function's result is null where its source column is
+bool ProgramBuilder::synth_nullable(int k) const {
+  const int src = synth_[size_t(k)].src;
+  return src >= 0 && batch_->cols[size_t(src)].null_count > 0;
 }
 
 int ProgramBuilder::add_synthetic_column(const void* dptr, int dtype) {
@@ -467,7 +575,8 @@ int ProgramBuilder::add_synthetic_column(const void* dptr, int dtype) {
 
 void ProgramBuilder::finish(ProgramSet* out) const {
   memset(out, 0, sizeof(*out));
-  if (!utf8_preds_.empty() && !utf8_evaluated_ && batch_->ctx) fail(DFGPU_ERR_INTERNAL, "Utf8 predicates not evaluated before the scan");
+  if ((!utf8_preds_.empty() || !utf8_views_.empty()) && !utf8_evaluated_ && batch_->ctx)
+    fail(DFGPU_ERR_INTERNAL, "Utf8 predicates not evaluated before the scan");
   if (int(progs_.size()) > kMaxProgs)
     fail(DFGPU_ERR_NOT_IMPLEMENTED, "more than " + std::to_string(kMaxProgs) + " expressions in one operator");
   int pc = 0, maxd = 1;
@@ -491,9 +600,11 @@ void ProgramBuilder::finish(ProgramSet* out) const {
   out->max_depth = maxd;
   for (size_t s = 0; s < slots_.size(); s++) {
     if (slots_[s] < 0) {
-      const Synth& sy = synth_[size_t(-1 - slots_[s])];
+      const int k = -1 - slots_[s];
+      const Synth& sy = synth_[size_t(k)];
       out->cols[s].ptr = sy.ptr;
-      out->cols[s].validity = nullptr;
+      out->cols[s].validity = synth_nullable(k) ? batch_->cols[size_t(sy.src)].validity : nullptr;
+      if (out->cols[s].validity) out->has_nulls = 1;
       out->cols[s].dtype = sy.dtype;
       continue;
     }

@@ -108,9 +108,32 @@ struct CompiledProgram {
 // `synth`.  No string code runs inside the scan kernels.
 struct Utf8Pred {
   int op;           // DFGPU_OP_EQ .. DFGPU_OP_GE (a literal on the left already mirrored), DFGPU_OP_LIKE, DFGPU_OP_NOT_LIKE
-  int a, b;         // batch columns: a op b, or a op lit when b < 0
+  int a, b;         // operands: a batch column c >= 0, or Utf8 view v as -2 - v; b == -1: a op lit
   std::string lit;  // the literal, or the LIKE pattern (a copy: the program's bytes are borrowed)
   int synth;        // synthetic column index
+};
+
+// A nest of Utf8 functions (DFGPU_OP_UTF8_FN) over one Utf8 column, reduced to one view of each string: the range steps
+// in order, innermost first, then the outermost case map.  The ASCII case maps keep the length and the character
+// boundaries, so they commute with every range step.  utf8_function.cu evaluates it.
+constexpr int kMaxUtf8Steps = 16;
+struct Utf8Step {
+  int op;           // DFGPU_UTF8FN_TRIM / _LTRIM / _RTRIM / _SUBSTR (SUBSTR_FROM is SUBSTR with count -1)
+  long long start;  // SUBSTR: 1-based first character
+  long long count;  // SUBSTR: characters; -1: to the end
+};
+struct Utf8ViewSpec {
+  int nsteps;
+  int case_map;     // 0 none, DFGPU_UTF8FN_UPPER, DFGPU_UTF8FN_LOWER
+  int result;       // 0: the Utf8 string; DFGPU_UTF8FN_LENGTH / _OCTET_LENGTH: its length as Int64
+  Utf8Step step[kMaxUtf8Steps];
+};
+struct Utf8View {
+  int src;            // batch column (Utf8)
+  Utf8ViewSpec spec;
+  int synth;          // synthetic column the programs read (Int64 results, a Utf8 program result), else -1
+  bool projection;    // a Utf8 projection: filter/project evaluates it over the selected rows, not before the scan
+  DevColumn out;      // Utf8 result of eval_utf8_predicates (offsets from 0, bytes in whole 16-byte words)
 };
 
 class ProgramBuilder {
@@ -118,9 +141,11 @@ class ProgramBuilder {
   explicit ProgramBuilder(const dfgpu_batch* batch) : batch_(batch) {}
   ProgramBuilder(const ProgramBuilder&) = delete;
   ProgramBuilder& operator=(const ProgramBuilder&) = delete;
-  ~ProgramBuilder();  // returns the predicate bitmaps to the ctx pool
-  // Type-check + lower one postfix program; appends to the set and returns its index.
-  int add(const dfgpu_insn* p, int n, const char* what);
+  ~ProgramBuilder();  // returns the predicate bitmaps and view columns to the ctx pool
+  // Type-check + lower one postfix program; appends to the set and returns its index.  With `utf8_view`, a program whose
+  // value is a Utf8 function nest is not appended: it is recorded as a projection view, *utf8_view receives its index
+  // and -1 is returned (else *utf8_view = -1).
+  int add(const dfgpu_insn* p, int n, const char* what, int* utf8_view = nullptr);
   // Program yielding the global row number (UInt64): the gather index for variable-width columns.
   int add_rowid();
   // Program yielding `bias + global row number` (UInt64).
@@ -135,19 +160,28 @@ class ProgramBuilder {
   int slot_of_column(int col);
   // Evaluate the recognised Utf8 predicates over the batch on ctx->stream and point their synthetic columns at the
   // bitmaps (utf8_predicate.cu).  Every operator calls it once per batch, after the last add() and before finish().
+  // The Utf8 function views are evaluated first (utf8_function.cu), the predicates after, so a predicate may read a view.
   void eval_utf8_predicates(dfgpu_ctx* ctx);
   const std::vector<Utf8Pred>& utf8_preds() const { return utf8_preds_; }
+  const std::vector<Utf8View>& utf8_views() const { return utf8_views_; }
+  // Evaluate projection view `v` over the rows `rows[0..n)` of the batch (all n rows when `rows` is null) into *out,
+  // a column the caller owns (utf8_function.cu).
+  void eval_utf8_view_rows(dfgpu_ctx* ctx, int v, const unsigned long long* rows, long long n, DevColumn* out) const;
 
  private:
-  int new_synth(const void* dptr, int dtype);  // a synthetic column slot; returns the synthetic index
+  int new_synth(const void* dptr, int dtype, int src = -1);  // a synthetic column slot; returns the synthetic index
+  bool synth_nullable(int k) const;
+  void eval_utf8_views(dfgpu_ctx* ctx);  // every view but the projections, before the predicates (utf8_function.cu)
   const dfgpu_batch* batch_;
   std::vector<Utf8Pred> utf8_preds_;
+  std::vector<Utf8View> utf8_views_;
   bool utf8_evaluated_ = false;
   dfgpu_ctx* ctx_ = nullptr;  // of owned_
-  std::vector<void*> owned_;  // device bitmaps and literals of utf8_preds_
+  std::vector<void*> owned_;  // device bitmaps and literals of utf8_preds_, columns of utf8_views_
   std::vector<CompiledProgram> progs_;
   std::vector<int> slots_;  // slot -> batch column index, or -1 - k for synthetic column k
-  struct Synth { const void* ptr; int dtype; };
+  // src >= 0: the synthetic column is null where batch column `src` is (a Utf8 function's result)
+  struct Synth { const void* ptr; int dtype; int src; };
   std::vector<Synth> synth_;
 };
 

@@ -263,8 +263,10 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
       proj_len = plen.data();
     }
     // Projections that are a plain Utf8 column are gathered by row number after the fused kernel
-    // (utf8_gather.cu); everything else is evaluated inside it.
+    // (utf8_gather.cu), and projections of a Utf8 function are evaluated over those row numbers (utf8_function.cu);
+    // everything else is evaluated inside it.
     std::vector<int> out_kind;  // per output column: >= 0 kernel program slot, -1 - c = Utf8 gather of input column c
+    std::vector<int> out_view(size_t(nproj), -1);  // per output column: the Utf8 view it is, or -1
     int nkern = 0;
     bool any_utf8 = false;
     for (int i = 0; i < nproj; i++) {
@@ -274,7 +276,12 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
         any_utf8 = true;
         continue;
       }
-      int pi = pb.add(proj[i], proj_len[i], "projection");
+      int pi = pb.add(proj[i], proj_len[i], "projection", &out_view[size_t(i)]);
+      if (out_view[size_t(i)] >= 0) {
+        out_kind.push_back(INT32_MIN);
+        any_utf8 = true;
+        continue;
+      }
       int dt = pb.out_dtype(pi);
       if (!is_numeric(dt) && dt != DFGPU_BOOL)
         fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string("filter/projection output of type ") + dtype_name(dt) +
@@ -438,13 +445,18 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
         any_utf8 = true;  // synchronise before the byte buffers are released
       }
     for (int i = 0; i < nproj; i++)
-      if (out_kind[size_t(i)] < 0)
+      if (out_view[size_t(i)] >= 0)  // without a WHERE every row, in order: no row numbers needed
+        pb.eval_utf8_view_rows(ctx, out_view[size_t(i)], has_pred ? (const unsigned long long*)scratch.cols[0].values : nullptr, res->nrows,
+                               &res->cols[size_t(i)]);
+      else if (out_kind[size_t(i)] < 0)
         gather_utf8(ctx, batch->cols[size_t(-1 - out_kind[size_t(i)])], (const unsigned long long*)scratch.cols[0].values, res->nrows,
                     &res->cols[size_t(i)]);
     if (!has_pred)
       for (int i = 0; i < nproj; i++)
         if (out_kind[size_t(i)] < 0) {  // Utf8 column passed through untouched keeps its validity (expression.rs:313)
-          const DevColumn& srcc = batch->cols[size_t(-1 - out_kind[size_t(i)])];
+          // and so does a Utf8 function of one
+          const int src = out_view[size_t(i)] >= 0 ? pb.utf8_views()[size_t(out_view[size_t(i)])].src : -1 - out_kind[size_t(i)];
+          const DevColumn& srcc = batch->cols[size_t(src)];
           if (srcc.null_count > 0) {
             const size_t vb = size_t(n + 7) / 8;
             res->cols[size_t(i)].validity = (uint8_t*)ctx->alloc(vb);

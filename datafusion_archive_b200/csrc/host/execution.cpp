@@ -200,16 +200,26 @@ std::optional<RecordBatch> MemoryDataSource::next() {
 // ---- built-in scalar functions ---------------------------------------------------------------------------
 const std::vector<BuiltinFunction>& builtin_functions() {
   static const std::vector<BuiltinFunction> table = {
-      {"sqrt", DFGPU_FN_SQRT, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},     {"abs", DFGPU_FN_ABS, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
-      {"floor", DFGPU_FN_FLOOR, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},   {"ceil", DFGPU_FN_CEIL, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
-      {"trunc", DFGPU_FN_TRUNC, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},   {"round", DFGPU_FN_ROUND, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
-      {"signum", DFGPU_FN_SIGNUM, 1, DFGPU_FLOAT64, DFGPU_FLOAT64}, {"exp", DFGPU_FN_EXP, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
-      {"ln", DFGPU_FN_LN, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},         {"log2", DFGPU_FN_LOG2, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
-      {"log10", DFGPU_FN_LOG10, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},   {"sin", DFGPU_FN_SIN, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
-      {"cos", DFGPU_FN_COS, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},       {"tan", DFGPU_FN_TAN, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
-      {"asin", DFGPU_FN_ASIN, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},     {"acos", DFGPU_FN_ACOS, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},
-      {"atan", DFGPU_FN_ATAN, 1, DFGPU_FLOAT64, DFGPU_FLOAT64},     {"power", DFGPU_FN_POWER, 2, DFGPU_FLOAT64, DFGPU_FLOAT64},
-      {"atan2", DFGPU_FN_ATAN2, 2, DFGPU_FLOAT64, DFGPU_FLOAT64},
+      {"sqrt", DFGPU_OP_FN, DFGPU_FN_SQRT, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},  {"abs", DFGPU_OP_FN, DFGPU_FN_ABS, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},
+      {"floor", DFGPU_OP_FN, DFGPU_FN_FLOOR, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},  {"ceil", DFGPU_OP_FN, DFGPU_FN_CEIL, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},
+      {"trunc", DFGPU_OP_FN, DFGPU_FN_TRUNC, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},  {"round", DFGPU_OP_FN, DFGPU_FN_ROUND, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},
+      {"signum", DFGPU_OP_FN, DFGPU_FN_SIGNUM, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},  {"exp", DFGPU_OP_FN, DFGPU_FN_EXP, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},
+      {"ln", DFGPU_OP_FN, DFGPU_FN_LN, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},  {"log2", DFGPU_OP_FN, DFGPU_FN_LOG2, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},
+      {"log10", DFGPU_OP_FN, DFGPU_FN_LOG10, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},  {"sin", DFGPU_OP_FN, DFGPU_FN_SIN, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},
+      {"cos", DFGPU_OP_FN, DFGPU_FN_COS, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},  {"tan", DFGPU_OP_FN, DFGPU_FN_TAN, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},
+      {"asin", DFGPU_OP_FN, DFGPU_FN_ASIN, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},  {"acos", DFGPU_OP_FN, DFGPU_FN_ACOS, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},
+      {"atan", DFGPU_OP_FN, DFGPU_FN_ATAN, 1, 1, {DFGPU_FLOAT64}, DFGPU_FLOAT64},  {"power", DFGPU_OP_FN, DFGPU_FN_POWER, 2, 2, {DFGPU_FLOAT64, DFGPU_FLOAT64}, DFGPU_FLOAT64},
+      {"atan2", DFGPU_OP_FN, DFGPU_FN_ATAN2, 2, 2, {DFGPU_FLOAT64, DFGPU_FLOAT64}, DFGPU_FLOAT64},
+      // Utf8 functions (DFGPU_OP_UTF8_FN); substr(s, start) is DFGPU_UTF8FN_SUBSTR_FROM
+      {"upper", DFGPU_OP_UTF8_FN, DFGPU_UTF8FN_UPPER, 1, 1, {DFGPU_UTF8}, DFGPU_UTF8},
+      {"lower", DFGPU_OP_UTF8_FN, DFGPU_UTF8FN_LOWER, 1, 1, {DFGPU_UTF8}, DFGPU_UTF8},
+      {"trim", DFGPU_OP_UTF8_FN, DFGPU_UTF8FN_TRIM, 1, 1, {DFGPU_UTF8}, DFGPU_UTF8},
+      {"ltrim", DFGPU_OP_UTF8_FN, DFGPU_UTF8FN_LTRIM, 1, 1, {DFGPU_UTF8}, DFGPU_UTF8},
+      {"rtrim", DFGPU_OP_UTF8_FN, DFGPU_UTF8FN_RTRIM, 1, 1, {DFGPU_UTF8}, DFGPU_UTF8},
+      {"substr", DFGPU_OP_UTF8_FN, DFGPU_UTF8FN_SUBSTR, 2, 3, {DFGPU_UTF8, DFGPU_INT64, DFGPU_INT64}, DFGPU_UTF8},
+      {"length", DFGPU_OP_UTF8_FN, DFGPU_UTF8FN_LENGTH, 1, 1, {DFGPU_UTF8}, DFGPU_INT64},
+      {"char_length", DFGPU_OP_UTF8_FN, DFGPU_UTF8FN_LENGTH, 1, 1, {DFGPU_UTF8}, DFGPU_INT64},
+      {"octet_length", DFGPU_OP_UTF8_FN, DFGPU_UTF8FN_OCTET_LENGTH, 1, 1, {DFGPU_UTF8}, DFGPU_INT64},
   };
   return table;
 }
@@ -227,7 +237,7 @@ std::shared_ptr<FunctionMeta> builtin_function_meta(const std::string& name) {
   if (!f) return nullptr;
   auto fm = std::make_shared<FunctionMeta>();
   fm->name = f->name;
-  for (int i = 0; i < f->arity; i++) fm->args.push_back(Field{"n", f->arg_type, false});
+  for (int i = 0; i < f->arity; i++) fm->args.push_back(Field{"n", f->arg_types[i], false});
   fm->return_type = f->return_type;
   return fm;
 }
@@ -314,12 +324,13 @@ void lower(const Expr& e, const Schema& schema, const std::map<size_t, int>& rem
       const BuiltinFunction* f = find_builtin_function(e.name);
       if (!f) fail(DFGPU_ERR_GENERAL, "Invalid function '" + e.name + "'");
       // the planner rejects extra arguments but not missing ones
-      if (e.args.size() != size_t(f->arity))
-        fail(DFGPU_ERR_EXECUTION, "function '" + e.name + "' takes " + std::to_string(f->arity) + (f->arity == 1 ? " argument" : " arguments") +
-                                      ", got " + std::to_string(e.args.size()));
+      if (e.args.size() < size_t(f->min_arity) || e.args.size() > size_t(f->arity))
+        fail(DFGPU_ERR_EXECUTION, "function '" + e.name + "' takes " +
+                                      (f->min_arity < f->arity ? std::to_string(f->min_arity) + " or " : std::string()) + std::to_string(f->arity) +
+                                      (f->arity == 1 ? " argument" : " arguments") + ", got " + std::to_string(e.args.size()));
       for (auto& a : e.args) lower(*a, schema, remap, out);
-      in.op = DFGPU_OP_FN;
-      in.col = f->code;
+      in.op = f->op;
+      in.col = f->code == DFGPU_UTF8FN_SUBSTR && e.args.size() == 2 ? DFGPU_UTF8FN_SUBSTR_FROM : f->code;
       in.dtype = f->return_type;
       out.push_back(in);
       return;

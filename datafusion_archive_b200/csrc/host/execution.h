@@ -165,9 +165,10 @@ class ExecutionContext {
 // can be registered by the user: the GPU cannot run an arbitrary closure.
 struct BuiltinFunction {
   const char* name;  // lower case; SQL names match in any letter case
-  int code;          // DFGPU_FN_*
-  int arity;
-  DataType arg_type, return_type;
+  int op;            // DFGPU_OP_FN (Float64 math) or DFGPU_OP_UTF8_FN
+  int code;          // DFGPU_FN_* or DFGPU_UTF8FN_*
+  int min_arity, arity;  // arguments: min_arity .. arity (the planner's extra-argument check uses arity)
+  DataType arg_types[3], return_type;
 };
 const std::vector<BuiltinFunction>& builtin_functions();
 const BuiltinFunction* find_builtin_function(const std::string& name);      // nullptr for an unknown name

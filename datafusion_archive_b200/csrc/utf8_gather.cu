@@ -143,6 +143,26 @@ void utf8_hash(dfgpu_ctx* ctx, const DevColumn& src, long long n, unsigned long 
   ctx->launches++;
 }
 
+// offsets[1..n] hold n string lengths: turn them into the end offsets (offsets[0] = 0 is the caller's) and return the
+// total, which must fit the i32 offsets.  Synchronises the stream.
+long long scan_utf8_lengths(dfgpu_ctx* ctx, int* offsets, long long n) {
+  const long long nblocks = (n + SC_TILE - 1) / SC_TILE;
+  long long* sums = (long long*)ctx->alloc(size_t(nblocks) * 8);
+  k_scan_block<<<(unsigned)nblocks, SC_THREADS, 0, ctx->stream>>>(offsets + 1, n, sums);
+  DF_CUDA(cudaGetLastError());
+  k_scan_sums<<<1, 32, 0, ctx->stream>>>(sums, nblocks);
+  DF_CUDA(cudaGetLastError());
+  k_scan_add<<<(unsigned)nblocks, SC_THREADS, 0, ctx->stream>>>(offsets + 1, n, sums);
+  DF_CUDA(cudaGetLastError());
+  ctx->launches += 3;
+  DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 24, sums + (nblocks - 1), 8, cudaMemcpyDeviceToHost, ctx->stream));
+  DF_CUDA(cudaStreamSynchronize(ctx->stream));
+  ctx->free(sums);
+  const long long total = (long long)ctx->h_scratch[24];
+  if (total >= (1ll << 31)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "Utf8 output larger than 2 GiB (i32 offsets)");
+  return total;
+}
+
 void gather_utf8_multi(dfgpu_ctx* ctx, const Utf8Source* d_srcs, const unsigned long long* d_idx, long long nsel, DevColumn* out) {
   out->dtype = DFGPU_UTF8;
   out->offsets = (int32_t*)ctx->alloc(size_t(nsel + 1) * 4);
@@ -152,20 +172,8 @@ void gather_utf8_multi(dfgpu_ctx* ctx, const Utf8Source* d_srcs, const unsigned 
     const int grid = (int)std::min<long long>((nsel + 255) / 256, (long long)ctx->sm_count * 8);
     k_utf8_lengths<<<grid, 256, 0, ctx->stream>>>(d_idx, d_srcs, nsel, out->offsets);
     DF_CUDA(cudaGetLastError());
-    const long long nblocks = (nsel + SC_TILE - 1) / SC_TILE;
-    long long* sums = (long long*)ctx->alloc(size_t(nblocks) * 8);
-    k_scan_block<<<(unsigned)nblocks, SC_THREADS, 0, ctx->stream>>>(out->offsets + 1, nsel, sums);
-    DF_CUDA(cudaGetLastError());
-    k_scan_sums<<<1, 32, 0, ctx->stream>>>(sums, nblocks);
-    DF_CUDA(cudaGetLastError());
-    k_scan_add<<<(unsigned)nblocks, SC_THREADS, 0, ctx->stream>>>(out->offsets + 1, nsel, sums);
-    DF_CUDA(cudaGetLastError());
-    ctx->launches += 4;
-    DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 24, sums + (nblocks - 1), 8, cudaMemcpyDeviceToHost, ctx->stream));
-    DF_CUDA(cudaStreamSynchronize(ctx->stream));
-    ctx->free(sums);
-    total = (long long)ctx->h_scratch[24];
-    if (total >= (1ll << 31)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "Utf8 output larger than 2 GiB (i32 offsets)");
+    ctx->launches++;
+    total = scan_utf8_lengths(ctx, out->offsets, nsel);
   }
   out->values_bytes = size_t(total);
   out->values = ctx->alloc(size_t(total > 0 ? total : 1));

@@ -298,6 +298,7 @@ void ProgramBuilder::eval_utf8_predicates(dfgpu_ctx* ctx) {
   utf8_evaluated_ = true;
   ctx_ = ctx;
   const long long n = batch_->nrows;
+  eval_utf8_views(ctx);  // a predicate may read a view
   for (const Utf8Pred& sp : utf8_preds_) {
     const size_t words = size_t((n + 31) / 32);
     unsigned* bits = (unsigned*)ctx->alloc((words ? words : 1) * 4);
@@ -308,26 +309,26 @@ void ProgramBuilder::eval_utf8_predicates(dfgpu_ctx* ctx) {
     const LikePattern lp = like ? compile_like(sp.lit) : LikePattern{LIKE_EXACT, sp.lit};
     Utf8PredParams p;
     memset(&p, 0, sizeof(p));
-    auto bind = [&](int col, const int** off, const unsigned char** bytes, const unsigned char** valid) {
-      const DevColumn& c = batch_->cols[size_t(col)];
+    auto bind = [&](int ref, const int** off, const unsigned char** bytes, const unsigned char** valid) {
+      const DevColumn& c = ref >= 0 ? batch_->cols[size_t(ref)] : utf8_views_[size_t(-2 - ref)].out;
       if (reinterpret_cast<uintptr_t>(c.values) & 15) fail(DFGPU_ERR_INTERNAL, "Utf8 byte buffer not 16-byte aligned");
       *off = c.offsets;
       *bytes = (const unsigned char*)c.values;
       *valid = c.null_count > 0 ? c.validity : nullptr;
     };
     bind(sp.a, &p.aoff, &p.abytes, &p.avalid);
-    if (sp.b >= 0) bind(sp.b, &p.boff, &p.bbytes, &p.bvalid);
+    const bool rcol = sp.b != -1;
+    if (rcol) bind(sp.b, &p.boff, &p.bbytes, &p.bvalid);
     p.op = sp.op;
     p.n = n;
     p.out = bits;
-    if (sp.b < 0) {
+    if (!rcol) {
       p.lit_len = int(lp.lit.size());
       unsigned char* d = (unsigned char*)ctx->alloc(lp.lit.size() + 16);
       owned_.push_back(d);
       if (!lp.lit.empty()) DF_CUDA(cudaMemcpyAsync(d, lp.lit.data(), lp.lit.size(), cudaMemcpyHostToDevice, ctx->stream));
       p.lit = d;
     }
-    const bool rcol = sp.b >= 0;
     if (like && lp.cls != LIKE_EXACT) {
       const std::string name = std::string("k_utf8_like<") + kLikeClassName[lp.cls] + ">";
       switch (lp.cls) {

@@ -222,6 +222,21 @@ def utf8_like_host(s, pattern):
     return bool(m.value), cls.value
 
 
+def utf8_fn_host(s, expr):
+    """dfgpu_utf8_fn_host: the value of `expr`, a Utf8 function nest over column 0, for the one string `s` (bytes or str),
+    by the engine's own per-row code on the host: bytes for a Utf8 result, int for an Int64 one."""
+    s = s.encode("utf-8") if isinstance(s, str) else bytes(s)
+    prog = expr.program([A.UTF8])
+    arr = (A.Insn * len(prog))(*prog)
+    out = C.create_string_buffer(max(1, len(s)))
+    out_len, out_int, out_dtype = C.c_int64(), C.c_int64(), C.c_int32()
+    L = lib()
+    L.dfgpu_utf8_fn_host.argtypes = [C.c_char_p, C.c_int64, C.POINTER(A.Insn), C.c_int, C.c_char_p, C.POINTER(C.c_int64),
+                                     C.POINTER(C.c_int64), C.POINTER(C.c_int32)]
+    check(L.dfgpu_utf8_fn_host(s, len(s), arr, len(prog), out, C.byref(out_len), C.byref(out_int), C.byref(out_dtype)))
+    return out.raw[:out_len.value] if out_dtype.value == A.UTF8 else out_int.value
+
+
 class Batch:
     def __init__(self, ctx, handle, schema):
         self.ctx, self.h, self.schema = ctx, handle, schema

@@ -163,6 +163,32 @@ class ScalarFunction(Expr):
         return "%s(%s)" % (self.name, ", ".join(repr(a) for a in self.args))
 
 
+class Utf8Function(Expr):
+    """Expr::ScalarFunction of a Utf8 function (DFGPU_OP_UTF8_FN): upper, lower, trim, ltrim, rtrim, substr(s, start
+    [, count]), length / char_length, octet_length.  The first argument is the Utf8 operand, the others Int64 literals;
+    length and octet_length return Int64, the others Utf8."""
+
+    def __init__(self, name, *args):
+        self.name, self.args = name, [_wrap(a) for a in args]
+        self.code = A.UTF8_FN_CODES[name.lower()]
+        if self.code == A.UTF8FN_SUBSTR and len(self.args) == 2:
+            self.code = A.UTF8FN_SUBSTR_FROM
+        self.dtype = A.INT64 if self.code in (A.UTF8FN_LENGTH, A.UTF8FN_OCTET_LENGTH) else A.UTF8
+
+    def get_type(self, schema):
+        return self.dtype
+
+    def _emit(self, schema, out):
+        for a in self.args:
+            a._emit(schema, out)
+        i = A.Insn()
+        i.op, i.col, i.dtype = A.OP_UTF8_FN, self.code, self.dtype
+        out.append(i)
+
+    def __repr__(self):
+        return "%s(%s)" % (self.name, ", ".join(repr(a) for a in self.args))
+
+
 class AggregateFunction:
     """Expr::AggregateFunction{name,args,return_type} (src/logicalplan.rs:162-166)."""
 
@@ -201,6 +227,10 @@ def lit(v, dtype=None):
 
 def fn(name, *args):
     return ScalarFunction(name, *args)
+
+
+def utf8_fn(name, *args):
+    return Utf8Function(name, *args)
 
 
 def f64_bits(x):

@@ -105,9 +105,13 @@ enum {
   DFGPU_OP_NOT_LIKE = 27, /* Operator::NotLike */
   DFGPU_OP_AND = 30, /* array_ops::and     expression.rs:452 */
   DFGPU_OP_OR = 31,  /* array_ops::or      expression.rs:459 */
-  DFGPU_OP_FN = 40   /* Expr::ScalarFunction{name,args,return_type} logicalplan.rs:156-160: `col` = DFGPU_FN_* code,
+  DFGPU_OP_FN = 40,  /* Expr::ScalarFunction{name,args,return_type} logicalplan.rs:156-160: `col` = DFGPU_FN_* code,
                         `dtype` = Float64; the arguments come first, in order.  Additive: libraries older than it
                         reject it with "operator: 40". */
+  DFGPU_OP_UTF8_FN = 41 /* Expr::ScalarFunction of a Utf8 function: `col` = DFGPU_UTF8FN_* code, `dtype` = the result
+                           type (DFGPU_UTF8, or DFGPU_INT64 for LENGTH / OCTET_LENGTH).  The arguments come first: the
+                           Utf8 operand (a column or another DFGPU_OP_UTF8_FN), then the function's DFGPU_OP_LIT Int64
+                           values.  See "Utf8 functions" below.  Additive. */
 };
 
 /* Built-in scalar functions (DFGPU_OP_FN).  The reference declares Expr::ScalarFunction and plans it
@@ -154,6 +158,29 @@ enum {
  *     else (DFGPU_ERR_EXECUTION "No support for literal type Utf8(..)"); a literal or pattern longer than
  *     DFGPU_UTF8_LITERAL_MAX bytes (DFGPU_ERR_NOT_IMPLEMENTED). */
 #define DFGPU_UTF8_LITERAL_MAX 4096
+
+/* Utf8 functions (DFGPU_OP_UTF8_FN).  PostgreSQL's, under the C locale, defined for any bytes (never validated).  A
+ * character is one UTF-8 code point as LIKE's `_` counts them: the first byte of a string and every later byte that is
+ * not 10xxxxxx start one.  A null argument gives a null; a Utf8 result keeps the source's validity, with length 0 on
+ * null rows.  Any nesting over one Utf8 column is allowed, e.g. upper(trim(substr(s, 2))), length(lower(s)).
+ *   - Utf8 results may be projected, and compared or LIKE-matched wherever Utf8 predicates may appear.  Int64 results
+ *     may appear wherever an Int64 column may, aggregate arguments and GROUP BY keys included.
+ *   - Refused: a Utf8 result as a GROUP BY key ("Utf8 GROUP BY keys must be plain columns") or aggregate argument (as for
+ *     a Utf8 column); a Utf8 literal argument (DFGPU_ERR_NOT_IMPLEMENTED); a non-Utf8 argument (DFGPU_ERR_EXECUTION
+ *     "function 'upper' takes a Utf8 argument, not Int32"); a start or count that is not a DFGPU_OP_LIT Int64
+ *     (DFGPU_ERR_NOT_IMPLEMENTED); a negative count (DFGPU_ERR_EXECUTION "negative substring length not allowed"). */
+enum {
+  DFGPU_UTF8FN_UPPER = 1,        /* ASCII a-z -> A-Z, every other byte unchanged (no Unicode case mapping) */
+  DFGPU_UTF8FN_LOWER = 2,        /* ASCII A-Z -> a-z, every other byte unchanged */
+  DFGPU_UTF8FN_TRIM = 3,         /* remove spaces (0x20 only) at both ends */
+  DFGPU_UTF8FN_LTRIM = 4,        /* ... at the start */
+  DFGPU_UTF8FN_RTRIM = 5,        /* ... at the end */
+  DFGPU_UTF8FN_SUBSTR_FROM = 6,  /* substr(s, start): the characters from position `start` (1-based) on */
+  DFGPU_UTF8FN_SUBSTR = 7,       /* substr(s, start, count): positions [start, start + count) clipped to [1, n];
+                                    start may be <= 0 or past the end; the sum saturates */
+  DFGPU_UTF8FN_LENGTH = 8,       /* number of characters, Int64 (SQL length / char_length) */
+  DFGPU_UTF8FN_OCTET_LENGTH = 9  /* number of bytes, Int64 */
+};
 
 typedef struct dfgpu_insn {
   int32_t op;
@@ -248,6 +275,12 @@ int dfgpu_check_program(const int32_t* col_dtypes, int ncols, const dfgpu_insn* 
  * `s` with the matcher of the pattern's class.  *match = 1 / 0; *pattern_class = 0 exact, 1 prefix `abc%`, 2 suffix
  * `%abc`, 3 contains `%abc%`, 4 general.  Usable on a machine with no device. */
 int dfgpu_utf8_like_host(const char* s, int64_t s_len, const char* pattern, int64_t pattern_len, int32_t* match, int32_t* pattern_class);
+/* One Utf8 function nest alone, on the host, for one string: `prog` is a DFGPU_OP_UTF8_FN program over column 0 (Utf8),
+ * compiled and evaluated by the same per-row code as the kernels.  *out_dtype receives DFGPU_UTF8 or DFGPU_INT64.  A
+ * Utf8 result is written to out[0 .. *out_len) (`out` holds at least s_len bytes: no result is longer than its source),
+ * an Int64 result to *out_int.  Usable on a machine with no device. */
+int dfgpu_utf8_fn_host(const char* s, int64_t s_len, const dfgpu_insn* prog, int prog_len, char* out, int64_t* out_len,
+                       int64_t* out_int, int32_t* out_dtype);
 
 /* ---- FilterRelation + ProjectRelation fused (src/execution/filter.rs:46-110,
  *      src/execution/projection.rs:46-66, wiring at src/execution/context.rs:126-161) ----

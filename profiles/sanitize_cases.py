@@ -143,5 +143,21 @@ assert len(got[0]) == len(np.unique(ka))
 got = agg([va], [], [AggregateFunction("avg", col(0))])
 assert float(got[0][0]) == float(np.float64(va.astype(np.int64).sum()) / len(va))
 print("avg ok", flush=True)
+
+# 9. Utf8 functions: k_utf8_view_len / k_utf8_view_copy over every row, over selected rows, the case-only path, a
+# predicate over a view, and an Int64 length as a GROUP BY key (strings straddle 16-byte words; one is > 4 KiB)
+from datafusion_archive_b200.expr import utf8_fn  # noqa: E402
+sv = [None if i % 11 == 0 else (b" " * (i % 3) + b"ab\xc3\xa9Xy" * (i % 7) + b" " * (i % 2)) for i in range(200_003)] + [b"q" * 5000]
+sa = pa.array(sv, type=pa.binary())
+sx = rng.random(len(sv))
+o = fp([sa, sx], col(1) > lit(0.5), [utf8_fn("upper", utf8_fn("trim", utf8_fn("substr", col(0), 2))), utf8_fn("length", col(0))])
+assert len(o[0]) == int((sx > 0.5).sum())
+o = fp([pa.array([v or b"" for v in sv], type=pa.binary())], None, [utf8_fn("lower", col(0))])
+assert o[0][5] == sv[5].lower().decode()
+o = fp([sa, sx], utf8_fn("lower", col(0)).like(lit(b"%abx%")), [col(1)])
+assert len(o[0]) == sum(1 for v in sv if v is not None and b"abx" in v.strip(b" ").lower())
+got = agg([sa, sx], [utf8_fn("length", col(0))], [AggregateFunction("count", col(1))])
+assert int(np.asarray(got[1]).sum()) == len(sv)
+print("utf8 functions ok", flush=True)
 ctx.close()
 print("SANITIZE_CASES_OK")

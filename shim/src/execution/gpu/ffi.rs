@@ -69,6 +69,20 @@ pub const FN_ACOS: i32 = 16;
 pub const FN_ATAN: i32 = 17;
 pub const FN_POWER: i32 = 18;
 pub const FN_ATAN2: i32 = 19;
+/// Expr::ScalarFunction of a Utf8 function: `col` = UTF8FN_* code, `dtype` = Utf8 or Int64 (length / octet_length);
+/// the Utf8 operand (a column or another OP_UTF8_FN) first, then the function's OP_LIT Int64 arguments.
+pub const OP_UTF8_FN: i32 = 41;
+
+// Utf8 functions (DFGPU_UTF8FN_*): ASCII case maps, space trims, substr by 1-based characters, lengths
+pub const UTF8FN_UPPER: i32 = 1;
+pub const UTF8FN_LOWER: i32 = 2;
+pub const UTF8FN_TRIM: i32 = 3;
+pub const UTF8FN_LTRIM: i32 = 4;
+pub const UTF8FN_RTRIM: i32 = 5;
+pub const UTF8FN_SUBSTR_FROM: i32 = 6;
+pub const UTF8FN_SUBSTR: i32 = 7;
+pub const UTF8FN_LENGTH: i32 = 8;
+pub const UTF8FN_OCTET_LENGTH: i32 = 9;
 
 // aggregate functions (src/execution/expression.rs:32-39 AggregateType)
 pub const AGG_MIN: i32 = 1;
@@ -172,6 +186,9 @@ extern "C" {
     pub fn dfgpu_check_program(col_dtypes: *const i32, ncols: c_int, prog: *const dfgpu_insn, prog_len: c_int, out_dtype: *mut i32) -> c_int;
     /// the LIKE pattern compiler and matcher on the host, for one string
     pub fn dfgpu_utf8_like_host(s: *const c_char, s_len: i64, pattern: *const c_char, pattern_len: i64, is_match: *mut i32, pattern_class: *mut i32) -> c_int;
+    /// one Utf8 function nest over column 0 on the host, for one string
+    pub fn dfgpu_utf8_fn_host(s: *const c_char, s_len: i64, prog: *const dfgpu_insn, prog_len: c_int, out: *mut c_char, out_len: *mut i64,
+                              out_int: *mut i64, out_dtype: *mut i32) -> c_int;
     pub fn dfgpu_result_col_device_ptr(r: *const dfgpu_result, i: c_int, dptr: *mut *const c_void) -> c_int;
 }
 

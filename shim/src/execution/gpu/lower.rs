@@ -80,6 +80,15 @@ pub fn builtin_function(name: &str) -> Option<(i32, usize)> {
     BUILTIN_FUNCTIONS.iter().find(|f| f.0.eq_ignore_ascii_case(name)).map(|f| (f.1, f.2))
 }
 
+/// The Utf8 functions: (name, UTF8FN_* code, minimum and maximum arity, result dtype).  substr with two arguments is
+/// UTF8FN_SUBSTR_FROM.
+pub const UTF8_FUNCTIONS: &[(&str, i32, usize, usize, i32)] = &[
+    ("upper", UTF8FN_UPPER, 1, 1, DT_UTF8), ("lower", UTF8FN_LOWER, 1, 1, DT_UTF8), ("trim", UTF8FN_TRIM, 1, 1, DT_UTF8),
+    ("ltrim", UTF8FN_LTRIM, 1, 1, DT_UTF8), ("rtrim", UTF8FN_RTRIM, 1, 1, DT_UTF8), ("substr", UTF8FN_SUBSTR, 2, 3, DT_UTF8),
+    ("length", UTF8FN_LENGTH, 1, 1, DT_INT64), ("char_length", UTF8FN_LENGTH, 1, 1, DT_INT64),
+    ("octet_length", UTF8FN_OCTET_LENGTH, 1, 1, DT_INT64),
+];
+
 /// `remap[i]` = index of input column i among the columns actually uploaded (pruned to the referenced ones).
 pub fn lower(e: &Expr, schema: &Schema, remap: &[Option<usize>], out: &mut Vec<dfgpu_insn>) -> Result<()> {
     match e {
@@ -108,6 +117,17 @@ pub fn lower(e: &Expr, schema: &Schema, remap: &[Option<usize>], out: &mut Vec<d
             lower(left, schema, remap, out)?;
             lower(right, schema, remap, out)?;
             out.push(insn(op_code(op)?, 0, dtype_code(&left.get_type(schema)).unwrap_or(0), 0));
+        }
+        Expr::ScalarFunction { name, args, .. } if UTF8_FUNCTIONS.iter().any(|f| f.0.eq_ignore_ascii_case(name)) => {
+            let &(_, code, min, max, dt) = UTF8_FUNCTIONS.iter().find(|f| f.0.eq_ignore_ascii_case(name)).unwrap();
+            if args.len() < min || args.len() > max {
+                return Err(ExecutionError::ExecutionError(format!("function '{}' takes {} to {} argument(s), got {}", name, min, max, args.len())));
+            }
+            for a in args {
+                lower(a, schema, remap, out)?;
+            }
+            let code = if code == UTF8FN_SUBSTR && args.len() == 2 { UTF8FN_SUBSTR_FROM } else { code };
+            out.push(insn(OP_UTF8_FN, code, dt, 0));
         }
         Expr::ScalarFunction { name, args, .. } => {
             let (code, arity) = builtin_function(name).ok_or_else(|| ExecutionError::General(format!("Invalid function '{}'", name)))?;
