@@ -1639,42 +1639,43 @@ int grid_for(dfgpu_ctx* ctx, long long work_items, int per_block, int blocks_per
   return int(g);
 }
 
-// Launch one of the kernels that are neither a scan nor a reduce: 256 threads per CTA, one CTA per `per_block` work
-// items, at most blocks_per_sm CTAs per SM.
-template <class P>
-void launch_kernel(dfgpu_ctx* ctx, void (*kern)(P), const char* name, const P& p, long long work_items, int per_block, int blocks_per_sm) {
-  kern<<<grid_for(ctx, work_items, per_block, blocks_per_sm), 256, 0, ctx->stream>>>(p);
+// The operator's one launch path: AG_THREADS threads per CTA, one CTA per `per_block` work items, at most `per_sm` CTAs per
+// SM (0: as many as the occupancy calculator fits with `smem` bytes of dynamic shared memory).  bind(grid) runs first and
+// sets what depends on the grid in the caller's objects that `args` refer to.  Profiled launches, the scans, reduces and
+// COUNT(DISTINCT) inserts, are also timed in the profile ring (dfgpu_profile_get), where the benchmark's kernel times come from.
+constexpr bool PROFILED = true;
+template <class... P, class Bind>
+void launch(dfgpu_ctx* ctx, void (*kern)(P...), const char* name, long long work_items, int per_block, int per_sm, size_t smem,
+            bool profiled, Bind&& bind, const P&... args) {
+  if (per_sm == 0) {
+    DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, AG_THREADS, smem));
+    per_sm = std::max(per_sm, 1);
+  }
+  const int grid = grid_for(ctx, work_items, per_block, per_sm);
+  bind(grid);
+  const int ps = profiled ? ctx->prof_begin() : -1;
+  kern<<<grid, AG_THREADS, smem, ctx->stream>>>(args...);
   DF_CUDA(cudaGetLastError());
   trace_launch(name);
-  ctx->launches++;
-}
-
-// One scan kernel instantiation.  FRONT kernels route rows through the shared-memory front table.
-struct ScanKernel {
-  void (*fn)(AggParams);
-  const char* name;
-  bool front;
-};
-
-// Launch one scan kernel.  FRONT launches admit the keys of every CTA's front table unconditionally when
-// the CTA retires, so the fill limit of the global path is lowered by what they can add (grid x front
-// slots): the table stays at most half full and the front merge always finds a slot.
-void launch_scan(dfgpu_ctx* ctx, const ScanKernel& k, AggParams& p, long long n) {
-  const size_t smem = k.front ? size_t(AG_FRONT_SLOTS) * 8 * size_t(1 + p.naggs) : 0;
-  if (k.front && ctx->first_use((const void*)k.fn))
-    DF_CUDA(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, AG_FRONT_SLOTS * 8 * (1 + kMaxAggs)));
-  int per_sm = 0;
-  DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k.fn, AG_THREADS, smem));
-  if (per_sm < 1) per_sm = 1;
-  const int grid = grid_for(ctx, n, AG_TILE, per_sm);
-  if (k.front) p.max_groups = std::max<long long>(0, p.max_groups - (long long)grid * AG_FRONT_SLOTS);
-  const int ps = ctx->prof_begin();
-  k.fn<<<grid, AG_THREADS, smem, ctx->stream>>>(p);
-  DF_CUDA(cudaGetLastError());
-  trace_launch(k.name);
   ctx->prof_end(ps);
   ctx->launches++;
 }
+// A launch whose arguments do not depend on the grid.
+template <class P>
+void launch_kernel(dfgpu_ctx* ctx, void (*kern)(P), const char* name, const P& p, long long work_items, int per_block, int per_sm,
+                   bool profiled = false) {
+  launch(ctx, kern, name, work_items, per_block, per_sm, 0, profiled, [](int) {}, p);
+}
+
+// A kernel instantiation and its trace name.  FRONT scan kernels route rows through the shared-memory front table.
+template <class... P>
+struct Kernel {
+  void (*fn)(P...);
+  const char* name;
+  bool front = false;
+};
+using ScanKernel = Kernel<AggParams>;
+
 template <int DEPTH>
 ScanKernel hash_agg_kernel(bool front) {
   static const std::string with_front = "k_hash_agg<" + depth_arg(DEPTH) + ", true, false>";
@@ -1701,17 +1702,9 @@ ScanKernel lean_kernel(int mask, int mt) {
   }
 }
 template <int DEPTH, bool NULLS = false>
-void launch_reduce(dfgpu_ctx* ctx, const AggParams& p, long long n) {
-  int per_sm = 0;
-  DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_reduce<DEPTH, NULLS>, AG_THREADS, 0));
-  if (per_sm < 1) per_sm = 1;
-  const int ps = ctx->prof_begin();
-  k_reduce<DEPTH, NULLS><<<grid_for(ctx, n, RD_TILE, per_sm), AG_THREADS, 0, ctx->stream>>>(p);
-  DF_CUDA(cudaGetLastError());
+Kernel<AggParams> reduce_kernel() {
   static const std::string name = "k_reduce<" + depth_arg(DEPTH) + (NULLS ? ", true>" : ", false>");
-  trace_launch(name.c_str());
-  ctx->prof_end(ps);
-  ctx->launches++;
+  return {k_reduce<DEPTH, NULLS>, name.c_str()};
 }
 
 // groups x (1 + naggs) sectors is what the SoA layout keeps hot in L2; beyond this many bytes the
@@ -2307,97 +2300,70 @@ void set_grow(dfgpu_aggstate* st, int s, long long new_cap) {
   st->sets[size_t(s)] = mp.to;
 }
 
-// Insert the pairs of rows [begin, begin + count) of the batch into every set: after the group scan of the same rows.
-// Rows that a full set refused are replayed after the sets that reached their fill limit grew x4, like
-// group_by_update's loop.  `prefix_of` > 0: these rows are the prefix sample of a first batch of that many rows, and
-// each set is then sized for the number of pairs estimated from it.
-void distinct_update(dfgpu_aggstate* st, const BatchPrograms& bp, const AggParams& scan, long long begin, long long count, long long prefix_of) {
-  dfgpu_ctx* ctx = st->ctx;
-  const int nsets = int(st->dist_progs.size());
+// The parameters of a batch's COUNT(DISTINCT) insert, which puts the (group key, argument) pairs of the batch's rows into
+// every set after the group scan of the same rows: its own program set (WHERE, keys, set arguments), the keys packed
+// exactly as the scan packs them.  *plain: p.plain describes the programs for k_distinct_insert_plain.
+AggParams plan_insert(const dfgpu_aggstate* st, const BatchPrograms& bp, bool* plain) {
   AggParams p;
   memset(&p, 0, sizeof(p));
   bp.dpb.finish(&p.ps);
   if (p.ps.max_depth > 8) fail(DFGPU_ERR_NOT_IMPLEMENTED, "expression too deep (register stack depth > 8)");
   p.has_pred = bp.has_pred;
   p.nkeys = st->nkeys;
-  p.nargs = nsets;
+  p.nargs = int(st->dist_progs.size());
   for (int k = 0; k < st->nkeys; k++) {
-    p.key_mask[k] = scan.key_mask[k];
-    p.key_shift[k] = scan.key_shift[k];
+    p.key_mask[k] = st->key_mask[size_t(k)];
+    p.key_shift[k] = st->key_shift[size_t(k)];
   }
   p.counters = st->d_dctr;
-  const bool plain = plain_spec(bp.dpb, p.ps, bp.has_pred, st->nkeys, nsets, &p.plain);
-  DevBufs lists(ctx);
-  unsigned* ovf[2] = {lists.alloc<unsigned>(size_t(count) * 4), nullptr};
-  int cur = 0;
-  const unsigned* list = nullptr;
-  long long nlist = 0;
-  for (int round = 0;; round++) {
-    if (round > 60) fail(DFGPU_ERR_INTERNAL, "COUNT(DISTINCT) set growth did not converge");
-    p.row_begin = begin;
-    p.nrows = count;
-    p.row_list = list;
-    p.nlist = nlist;
-    p.ovf_rows = ovf[cur];
-    DF_CUDA(cudaMemsetAsync(st->d_dctr + DCTR_OVERFLOW, 0, 8, ctx->stream));
-    void (*fn)(AggParams, SetParams);
-    const char* name;
-    const int d = p.ps.max_depth;
-    if (has_fn(p.ps) && p.ps.has_nulls) fn = k_distinct_insert<kFnDepth, true>, name = "k_distinct_insert<kFnDepth, true>";
-    else if (has_fn(p.ps)) fn = k_distinct_insert<kFnDepth, false>, name = "k_distinct_insert<kFnDepth, false>";
-    else if (p.ps.has_nulls) fn = k_distinct_insert<8, true>, name = "k_distinct_insert<8, true>";
-    else if (plain && !list && (begin & 1) == 0 && p.ps.ncols <= 2) fn = k_distinct_insert_plain<2>, name = "k_distinct_insert_plain<2>";
-    else if (plain && !list && (begin & 1) == 0) fn = k_distinct_insert_plain<4>, name = "k_distinct_insert_plain<4>";
-    else if (d <= 2) fn = k_distinct_insert<2, false>, name = "k_distinct_insert<2, false>";
-    else fn = k_distinct_insert<8, false>, name = "k_distinct_insert<8, false>";
-    int per_sm = 0;
-    DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, AG_THREADS, 0));
-    const int grid = grid_for(ctx, list ? nlist : count, AG_TILE, std::max(per_sm, 1));
-    // A warp reads the fill once per tile and adds its tile's pairs after it, so up to one tile per warp of the grid
-    // (grid x AG_TILE pairs per set) is inserted past what the others read: the fill limit is lowered by that much,
-    // which keeps every set at most half full.
-    SetParams sp;
-    memset(&sp, 0, sizeof(sp));
-    for (int s = 0; s < nsets; s++) {
-      sp.set[s] = st->sets[size_t(s)];
-      sp.max_fill[s] = std::max<long long>(0, fill_limit(sp.set[s].cap) - (long long)grid * AG_TILE);
-      sp.mt[s] = mtype_of(st->dist_dtypes[size_t(s)]);
-    }
-    const int ps = ctx->prof_begin();
-    fn<<<grid, AG_THREADS, 0, ctx->stream>>>(p, sp);
-    DF_CUDA(cudaGetLastError());
-    trace_launch(name);
-    ctx->prof_end(ps);
-    ctx->launches++;
-    unsigned long long c[DCTR_SLOTS];
-    read_dctr(st, c);
-    if (c[DCTR_ERROR]) fail(DFGPU_ERR_ARROW, "DivideByZero");
-    const long long novf = (long long)c[DCTR_OVERFLOW];
-    bool grew = false;
-    for (int s = 0; s < nsets; s++) {
-      const long long n = (long long)c[DCTR_SET + 2 * s];
-      const bool refused = novf > 0 && n >= sp.max_fill[s];  // at the fill limit: this set refused new pairs
-      if (!refused && n <= fill_limit(sp.set[s].cap)) continue;
-      set_grow(st, s, grown_cap(sp.set[s].cap));
-      grew = true;
-    }
-    if (novf == 0) break;
-    if (!grew)  // refused at the probe limit below the fill limit: grow every set
-      for (int s = 0; s < nsets; s++) set_grow(st, s, grown_cap(sp.set[s].cap));
-    list = ovf[cur];
-    nlist = novf;
-    cur ^= 1;
-    if (!ovf[cur]) ovf[cur] = lists.alloc<unsigned>(size_t(count) * 4);
+  *plain = plain_spec(bp.dpb, p.ps, bp.has_pred, st->nkeys, p.nargs, &p.plain);
+  return p;
+}
+
+// The insert kernel of one round.  Replays read a row list and the plain kernels start on an even row, so both take the
+// interpreter.
+Kernel<AggParams, SetParams> choose_insert(const AggParams& p, bool plain_ok) {
+  const bool fn = has_fn(p.ps), plain = plain_ok && !p.row_list && (p.row_begin & 1) == 0;
+  if (fn && p.ps.has_nulls) return {k_distinct_insert<kFnDepth, true>, "k_distinct_insert<kFnDepth, true>"};
+  if (fn) return {k_distinct_insert<kFnDepth, false>, "k_distinct_insert<kFnDepth, false>"};
+  if (p.ps.has_nulls) return {k_distinct_insert<8, true>, "k_distinct_insert<8, true>"};
+  if (plain && p.ps.ncols <= 2) return {k_distinct_insert_plain<2>, "k_distinct_insert_plain<2>"};
+  if (plain) return {k_distinct_insert_plain<4>, "k_distinct_insert_plain<4>"};
+  if (p.ps.max_depth <= 2) return {k_distinct_insert<2, false>, "k_distinct_insert<2, false>"};
+  return {k_distinct_insert<8, false>, "k_distinct_insert<8, false>"};
+}
+
+// One round of the insert over the rows p describes, then the growth rule of the sets: each set that refused pairs at
+// its fill limit, or went past it, grows x4; when rows were refused and no set grew, the probe limit refused them below
+// the fill limit, and every set grows.  Returns the number of rows refused.
+long long insert_round(dfgpu_aggstate* st, AggParams& p, bool plain) {
+  const int nsets = int(st->dist_progs.size());
+  const Kernel<AggParams, SetParams> k = choose_insert(p, plain);
+  SetParams sp;
+  memset(&sp, 0, sizeof(sp));
+  for (int s = 0; s < nsets; s++) {
+    sp.set[s] = st->sets[size_t(s)];
+    sp.mt[s] = mtype_of(st->dist_dtypes[size_t(s)]);
   }
-  if (prefix_of > 0) {
-    unsigned long long c[DCTR_SLOTS];
-    read_dctr(st, c);
-    for (int s = 0; s < nsets; s++) {
-      const long long cur_cap = st->sets[size_t(s)].cap;
-      const long long want = prefix_cap(ctx, (long long)c[DCTR_SET + 2 * s], count, prefix_of, 16, cur_cap, AG_SET_MIN_CAP);
-      if (want > cur_cap) set_grow(st, s, want);
-    }
+  // A warp reads the fill once per tile and adds its tile's pairs after it, so up to one tile per warp of the grid
+  // (grid x AG_TILE pairs per set) is inserted past what the others read: the fill limit is lowered by that much,
+  // which keeps every set at most half full.
+  launch(st->ctx, k.fn, k.name, p.row_list ? p.nlist : p.nrows, AG_TILE, 0, 0, PROFILED, [&](int grid) {
+    for (int s = 0; s < nsets; s++) sp.max_fill[s] = std::max<long long>(0, fill_limit(sp.set[s].cap) - (long long)grid * AG_TILE);
+  }, p, sp);
+  unsigned long long c[DCTR_SLOTS];
+  read_dctr(st, c);
+  if (c[DCTR_ERROR]) fail(DFGPU_ERR_ARROW, "DivideByZero");
+  const long long novf = (long long)c[DCTR_OVERFLOW];
+  bool grow[kMaxAggs], any = false;
+  for (int s = 0; s < nsets; s++) {
+    const long long n = (long long)c[DCTR_SET + 2 * s];
+    grow[s] = (novf > 0 && n >= sp.max_fill[s]) || n > fill_limit(sp.set[s].cap);  // refused pairs at its fill limit, or past it
+    any = any || grow[s];
   }
+  for (int s = 0; s < nsets; s++)
+    if (grow[s] || (novf > 0 && !any)) set_grow(st, s, grown_cap(sp.set[s].cap));
+  return novf;
 }
 
 // GROUP BY at finish: add each set's pairs to the COUNT(DISTINCT) words of their groups.
@@ -2442,10 +2408,10 @@ void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
   if (bp.has_pred) DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_PASSED, 0, 8, ctx->stream));
   const int d = p.ps.max_depth;
   const bool fn = has_fn(p.ps);
+  Kernel<AggParams> k{};
   if (p.ps.has_nulls) {
     st->saw_nulls = true;
-    if (fn) launch_reduce<kFnDepth, true>(ctx, p, p.nrows);
-    else launch_reduce<8, true>(ctx, p, p.nrows);
+    k = fn ? reduce_kernel<kFnDepth, true>() : reduce_kernel<8, true>();
   } else {
     if (!bp.has_pred)
       for (int a = 0; a < st->naggs; a++) st->nonnull_host[size_t(a)] += p.nrows;
@@ -2464,15 +2430,14 @@ void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
       rp.naggs = p.naggs;
       for (int a = 0; a < p.naggs; a++) { rp.aggs[a] = p.aggs[a]; rp.agg_arg[a] = p.agg_arg[a]; }
       rp.t = st->t;
-      const int ps = ctx->prof_begin();
-      launch_kernel(ctx, k_reduce_f64, "k_reduce_f64", rp, p.nrows, 256 * 8, 8);
-      ctx->prof_end(ps);
-    } else if (fn) launch_reduce<kFnDepth>(ctx, p, p.nrows);
-    else if (d <= 1) launch_reduce<1>(ctx, p, p.nrows);
-    else if (d <= 2) launch_reduce<2>(ctx, p, p.nrows);
-    else if (d <= 4) launch_reduce<4>(ctx, p, p.nrows);
-    else launch_reduce<8>(ctx, p, p.nrows);
+      launch_kernel(ctx, k_reduce_f64, "k_reduce_f64", rp, p.nrows, 256 * 8, 8, PROFILED);
+    } else if (fn) k = reduce_kernel<kFnDepth>();
+    else if (d <= 1) k = reduce_kernel<1>();
+    else if (d <= 2) k = reduce_kernel<2>();
+    else if (d <= 4) k = reduce_kernel<4>();
+    else k = reduce_kernel<8>();
   }
+  if (k.fn) launch_kernel(ctx, k.fn, k.name, p, p.nrows, RD_TILE, 0, PROFILED);
   unsigned long long c[CTR_NONNULL];
   read_counters(st, c);
   if (c[CTR_ERROR]) fail(DFGPU_ERR_ARROW, "DivideByZero");
@@ -2586,102 +2551,106 @@ void verify_utf8_groups(dfgpu_aggstate* st, const BatchPrograms& bp, long long n
   if (flag) fail(DFGPU_ERR_INTERNAL, "Utf8 GROUP BY verification could not find a group");
 }
 
-// GROUP BY: scan the batch into the table.  Rows that find no slot go to an overflow list and are replayed in the next
-// round, after the table grew x4 -- or as they are, when each of them only met a slot that was still being published
-// (counter CTR_DEFERRED, which only wide scans set).
-void group_by_update(dfgpu_aggstate* st, const dfgpu_batch* batch, const BatchPrograms& bp, AggParams& p, Trace& tr) {
+// The grow-and-replay loop of the group table and of the COUNT(DISTINCT) sets.  run() passes rows [begin, begin + count)
+// of the batch through round(), then the rows it refused through it again, until a round refuses none.  round() launches
+// one kernel over the rows p describes, the range or the last round's overflow list, applies the growth rule of its
+// table or sets and returns the number of rows it appended to p.ovf_rows (counted in `overflow`).  The batch's two
+// overflow lists alternate; the second is allocated when a round first needs it.
+struct GrowAndReplay {
+  DevBufs bufs;
+  size_t bytes;
+  unsigned* list[2];
+  GrowAndReplay(dfgpu_ctx* ctx, long long nrows) : bufs(ctx), bytes(size_t(nrows) * 4), list{bufs.alloc<unsigned>(bytes), nullptr} {}
+  template <class Round>
+  void run(AggParams& p, unsigned long long* overflow, long long begin, long long count, const char* no_convergence, Round&& round) {
+    p.row_begin = begin;
+    p.nrows = count;
+    p.row_list = nullptr;
+    p.nlist = 0;
+    for (int i = 0, cur = 0;; i++, cur ^= 1) {
+      if (i > 60) fail(DFGPU_ERR_INTERNAL, no_convergence);
+      if (!list[cur]) list[cur] = bufs.alloc<unsigned>(bytes);
+      p.ovf_rows = list[cur];
+      DF_CUDA(cudaMemsetAsync(overflow, 0, 8, bufs.ctx->stream));
+      const long long novf = round();
+      if (novf == 0) return;
+      p.row_list = list[cur];
+      p.nlist = novf;
+    }
+  }
+};
+
+// One round of the group scan over the rows p describes, then the growth rule of the table: x4 when it went past its
+// fill limit, or when it refused rows -- except when each of them only met a slot that was still being published
+// (counter CTR_DEFERRED, which only wide scans set): those are replayed as they are.  Returns the number of rows refused.
+long long scan_round(dfgpu_aggstate* st, AggParams& p, const ScanPlan& plan, Trace& tr, bool prefix) {
   dfgpu_ctx* ctx = st->ctx;
-  if (st->wide) {
-    // retain this batch's Utf8 key columns: a group's string lives in the batch whose row created it
-    p.wide.kw = st->nkeys;
-    bool new_src = false;
-    for (int k = 0; k < st->nkeys; k++) {
-      p.wide.is_utf8[k] = st->key_is_utf8[size_t(k)];
-      const DevColumn* uc = bp.key_utf8[size_t(k)];
-      if (!uc) continue;
-      if (st->utf8_srcs.size() >= (1u << 20)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "more than 2^20 retained Utf8 GROUP BY key columns");
-      p.wide.ref_base[k] = retain_utf8(st, *uc, batch->nrows) << UTF8_SRC_SHIFT;
-      p.wide.off[k] = st->utf8_srcs.back().off;
-      p.wide.bytes[k] = st->utf8_srcs.back().bytes;
-      new_src = true;
-    }
-    if (new_src) upload_utf8_srcs(st);
-    p.wide.srcs = st->d_utf8_srcs;
+  const bool replay = p.row_list != nullptr;
+  p.t = st->t;
+  p.max_groups = fill_limit(st->t.cap);
+  // <= 64 groups: one private 256-slot table per warp (same shared-memory footprint as the
+  // CTA-wide 2048-slot table); otherwise one table per CTA
+  p.front_per_warp = st->ngroups <= 64 ? 1 : 0;
+  p.front_slots = p.front_per_warp ? AG_FRONT_SLOTS / (AG_THREADS / 32) : AG_FRONT_SLOTS;
+  // (A persisting-L2 access-policy window over the table was tried and removed: it slowed the scan
+  // several-fold at 1e5 and 1e6 groups.)
+  const ScanKernel k = choose_scan(st, p, plan, replay, st->use_front && !replay);
+  const size_t smem = k.front ? size_t(AG_FRONT_SLOTS) * 8 * size_t(1 + p.naggs) : 0;
+  if (k.front && ctx->first_use((const void*)k.fn))
+    DF_CUDA(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, AG_FRONT_SLOTS * 8 * (1 + kMaxAggs)));
+  // FRONT launches admit the keys of every CTA's front table unconditionally when the CTA retires, so the fill limit of
+  // the global path is lowered by what they can add (grid x front slots): the table stays at most half full and the
+  // front merge always finds a slot.
+  launch(ctx, k.fn, k.name, replay ? p.nlist : p.nrows, AG_TILE, 0, smem, PROFILED, [&](int grid) {
+    if (k.front) p.max_groups = std::max<long long>(0, p.max_groups - (long long)grid * AG_FRONT_SLOTS);
+  }, p);
+  unsigned long long c[CTR_NONNULL];
+  read_counters(st, c);
+  if (c[CTR_ERROR] == 2) fail(DFGPU_ERR_INTERNAL, "front-table merge could not find a slot");
+  if (c[CTR_ERROR]) fail(DFGPU_ERR_ARROW, "DivideByZero");
+  st->ngroups = (long long)c[CTR_GROUPS];
+  st->sentinel_used = c[CTR_SENTINEL] != 0;
+  const long long novf = (long long)c[CTR_OVERFLOW], deferred = (long long)c[CTR_DEFERRED];
+  if (deferred) DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_DEFERRED, 0, 8, ctx->stream));
+  tr.mark(prefix ? "scan kernel (prefix)" : "scan kernel");
+  if (st->ngroups > fill_limit(st->t.cap) || (novf > 0 && novf != deferred)) {
+    table_grow(st, grown_cap(st->t.cap));
+    if (novf == 0) tr.mark("table_grow (load factor)");
   }
-  const ScanPlan plan = st->wide ? ScanPlan{} : plan_scan(st, bp, p);
-  DevBufs lists(ctx);
-  unsigned* ovf[2] = {lists.alloc<unsigned>(size_t(batch->nrows) * 4), nullptr};
-  tr.mark("overflow list alloc");
-  // First big batch with no cardinality hint: a 1 Mi-row prefix is aggregated first; the number of groups it
-  // produces decides the table layout (SoA while the hot sectors fit L2, AoS beyond) before the bulk of the batch
-  // is touched.  Wide tables are AoS from the start.
-  const long long kPrefix = AG_PREFIX_ROWS;
-  const bool sample = st->rows_seen == batch->nrows && st->expected == 0 && !st->aos && batch->nrows >= 4 * kPrefix;
-  std::vector<std::pair<long long, long long>> ranges;  // (begin, count)
-  if (sample) {
-    ranges.push_back({0, kPrefix});
-    ranges.push_back({kPrefix, batch->nrows - kPrefix});
-  } else {
-    ranges.push_back({0, batch->nrows});
-  }
-  for (size_t ri = 0; ri < ranges.size(); ri++) {
-    int cur = 0;
-    const unsigned* list = nullptr;
-    long long nlist = 0;
-    for (int round = 0;; round++) {
-      if (round > 60) fail(DFGPU_ERR_INTERNAL, "hash table growth did not converge");
-      p.t = st->t;
-      p.max_groups = fill_limit(st->t.cap);
-      p.row_begin = ranges[ri].first;
-      p.nrows = ranges[ri].second;
-      p.row_list = list;
-      p.nlist = nlist;
-      p.ovf_rows = ovf[cur];
-      DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_OVERFLOW, 0, 8, ctx->stream));
-      // <= 64 groups: one private 256-slot table per warp (same shared-memory footprint as the
-      // CTA-wide 2048-slot table); otherwise one table per CTA
-      p.front_per_warp = st->ngroups <= 64 ? 1 : 0;
-      p.front_slots = p.front_per_warp ? AG_FRONT_SLOTS / (AG_THREADS / 32) : AG_FRONT_SLOTS;
-      // (A persisting-L2 access-policy window over the table was tried and removed: it slowed the scan
-      // several-fold at 1e5 and 1e6 groups.)
-      launch_scan(ctx, choose_scan(st, p, plan, list != nullptr, st->use_front && !list), p, list ? nlist : p.nrows);
-      unsigned long long c[CTR_NONNULL];
-      read_counters(st, c);
-      if (c[CTR_ERROR] == 2) fail(DFGPU_ERR_INTERNAL, "front-table merge could not find a slot");
-      if (c[CTR_ERROR]) fail(DFGPU_ERR_ARROW, "DivideByZero");
-      st->ngroups = (long long)c[CTR_GROUPS];
-      st->sentinel_used = c[CTR_SENTINEL] != 0;
-      const long long novf = (long long)c[CTR_OVERFLOW], deferred = (long long)c[CTR_DEFERRED];
-      if (deferred) DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_DEFERRED, 0, 8, ctx->stream));
-      tr.mark(ri == 0 && ranges.size() > 1 ? "scan kernel (prefix)" : "scan kernel");
-      if (novf == 0) {
-        if (st->ngroups > fill_limit(st->t.cap)) { table_grow(st, grown_cap(st->t.cap)); tr.mark("table_grow (load factor)"); }
-        break;
-      }
-      // rows that only met a slot still being published need no bigger table: replay them as they are
-      if (!(novf == deferred && st->ngroups <= fill_limit(st->t.cap))) table_grow(st, grown_cap(st->t.cap));
-      list = ovf[cur];
-      nlist = novf;
-      cur ^= 1;
-      if (!ovf[cur]) ovf[cur] = lists.alloc<unsigned>(size_t(batch->nrows) * 4);
-    }
-    if (!st->dist_progs.empty()) distinct_update(st, bp, p, ranges[ri].first, ranges[ri].second, sample && ri == 0 ? batch->nrows : 0);
-    // few groups so far: later rows of this stream go through the shared-memory front table
-    st->use_front = st->ngroups <= AG_FRONT_MAX_GROUPS && st->rows_seen >= (1ll << 20);
-    if (sample && ri == 0) {
-      // size (and lay out) the table for the estimated number of groups before the bulk of the batch
-      // is touched: one rebuild of a ~1 Mi-entry table instead of repeated 4x growth + replays
-      long long est = 0;
-      const long long want_cap = prefix_cap(ctx, st->ngroups, kPrefix, batch->nrows, 32 * (1 + st->naggs), st->t.cap, AG_MIN_CAP, &est);
-      const bool to_aos = !st->aos && want_aos(est, st->descs, st->naggs);
-      if (to_aos || want_cap > st->t.cap) {
-        st->aos = st->aos || to_aos;
-        table_grow(st, want_cap);
-        tr.mark("table_grow (prefix estimate)");
-      }
+  return novf;
+}
+
+// The row ranges, (begin, count), that a batch goes through the table and the sets in.  A first big batch with no
+// cardinality hint is cut after a 1 Mi-row prefix: what the prefix produces sizes the sets and decides the table's
+// capacity and layout (hybrid while the hot sectors fit L2, line beyond) before the rest of the batch is touched.  Wide
+// tables are line-laid-out from the start.
+std::vector<std::pair<long long, long long>> batch_ranges(const dfgpu_aggstate* st, long long nrows) {
+  if (st->rows_seen == nrows && st->expected == 0 && !st->aos && nrows >= 4 * AG_PREFIX_ROWS)
+    return {{0, AG_PREFIX_ROWS}, {AG_PREFIX_ROWS, nrows - AG_PREFIX_ROWS}};
+  return {{0, nrows}};
+}
+
+// After the prefix of a first batch of `batch_rows` rows: size each set, then the table, for the number of entries
+// estimated from the prefix -- one rebuild of a ~1 Mi-entry table or set instead of repeated x4 growth and replays.
+void size_from_prefix(dfgpu_aggstate* st, long long batch_rows, Trace& tr) {
+  if (!st->dist_progs.empty()) {
+    unsigned long long c[DCTR_SLOTS];
+    read_dctr(st, c);
+    for (size_t s = 0; s < st->dist_progs.size(); s++) {
+      const long long cur_cap = st->sets[s].cap;
+      const long long want = prefix_cap(st->ctx, (long long)c[DCTR_SET + 2 * s], AG_PREFIX_ROWS, batch_rows, 16, cur_cap, AG_SET_MIN_CAP);
+      if (want > cur_cap) set_grow(st, int(s), want);
     }
   }
-  if (bp.ukey) verify_utf8_groups(st, bp, batch->nrows);
+  if (st->nkeys == 0) return;
+  long long est = 0;
+  const long long want_cap = prefix_cap(st->ctx, st->ngroups, AG_PREFIX_ROWS, batch_rows, 32 * (1 + st->naggs), st->t.cap, AG_MIN_CAP, &est);
+  const bool to_aos = !st->aos && want_aos(est, st->descs, st->naggs);
+  if (to_aos || want_cap > st->t.cap) {
+    st->aos = st->aos || to_aos;
+    table_grow(st, want_cap);
+    tr.mark("table_grow (prefix estimate)");
+  }
 }
 
 void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
@@ -2718,18 +2687,48 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
   p.nrows = batch->nrows;
   p.counters = st->d_counters;
   p.has_pred = bp.has_pred;
-  if (st->nkeys > 0) {
-    group_by_update(st, batch, bp, p, tr);
-    return;
+  const bool group_by = st->nkeys > 0, distinct = !st->dist_progs.empty();
+  if (!group_by) {
+    reduce_update(st, bp, p);  // one launch over the whole batch
+    if (!distinct) return;
+  } else if (st->wide) {
+    // retain this batch's Utf8 key columns: a group's string lives in the batch whose row created it
+    p.wide.kw = st->nkeys;
+    bool new_src = false;
+    for (int k = 0; k < st->nkeys; k++) {
+      p.wide.is_utf8[k] = st->key_is_utf8[size_t(k)];
+      const DevColumn* uc = bp.key_utf8[size_t(k)];
+      if (!uc) continue;
+      if (st->utf8_srcs.size() >= (1u << 20)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "more than 2^20 retained Utf8 GROUP BY key columns");
+      p.wide.ref_base[k] = retain_utf8(st, *uc, batch->nrows) << UTF8_SRC_SHIFT;
+      p.wide.off[k] = st->utf8_srcs.back().off;
+      p.wide.bytes[k] = st->utf8_srcs.back().bytes;
+      new_src = true;
+    }
+    if (new_src) upload_utf8_srcs(st);
+    p.wide.srcs = st->d_utf8_srcs;
   }
-  reduce_update(st, bp, p);
-  if (st->dist_progs.empty()) return;
-  if (st->rows_seen == batch->nrows && st->expected == 0 && batch->nrows >= 4 * AG_PREFIX_ROWS) {  // size the sets from a prefix
-    distinct_update(st, bp, p, 0, AG_PREFIX_ROWS, batch->nrows);
-    distinct_update(st, bp, p, AG_PREFIX_ROWS, batch->nrows - AG_PREFIX_ROWS, 0);
-  } else {
-    distinct_update(st, bp, p, 0, batch->nrows, 0);
+  const ScanPlan plan = group_by && !st->wide ? plan_scan(st, bp, p) : ScanPlan{};
+  bool ins_plain = false;
+  AggParams ins = distinct ? plan_insert(st, bp, &ins_plain) : AggParams{};
+  GrowAndReplay loop(ctx, batch->nrows);
+  tr.mark("overflow list alloc");
+  const auto ranges = batch_ranges(st, batch->nrows);
+  for (size_t ri = 0; ri < ranges.size(); ri++) {
+    const long long begin = ranges[ri].first, count = ranges[ri].second;
+    const bool prefix = ranges.size() > 1 && ri == 0;
+    if (group_by)
+      loop.run(p, st->d_counters + CTR_OVERFLOW, begin, count, "hash table growth did not converge",
+               [&] { return scan_round(st, p, plan, tr, prefix); });
+    // after the group scan of the same rows: every key the insert packs is in the table
+    if (distinct)
+      loop.run(ins, st->d_dctr + DCTR_OVERFLOW, begin, count, "COUNT(DISTINCT) set growth did not converge",
+               [&] { return insert_round(st, ins, ins_plain); });
+    // few groups so far: later rows of this stream go through the shared-memory front table
+    if (group_by) st->use_front = st->ngroups <= AG_FRONT_MAX_GROUPS && st->rows_seen >= (1ll << 20);
+    if (prefix) size_from_prefix(st, batch->nrows, tr);
   }
+  if (bp.ukey) verify_utf8_groups(st, bp, batch->nrows);
 }
 }  // namespace
 
