@@ -12,6 +12,7 @@
 #include <memory>
 
 #include "expr_vm.cuh"
+#include "hash_table.cuh"
 
 namespace dfgpu {
 
@@ -24,7 +25,6 @@ constexpr int AG_R = 2;  // rows per thread per tile: the kernel is bound by sca
 constexpr int AG_TILE = AG_THREADS * AG_R;
 constexpr int kMaxAggs = 8;
 constexpr int kMaxKeys = 4;
-constexpr unsigned long long EMPTY_KEY = ~0ull;
 constexpr int AG_MAX_PROBE = 1 << 14;
 constexpr long long AG_MIN_CAP = 1ll << 22;
 constexpr long long AG_SET_MIN_CAP = 1ll << 20;  // COUNT(DISTINCT) pair sets: 16-byte slots
@@ -41,29 +41,6 @@ struct AggDesc {
   uint8_t mtype;  // machine type of the argument
   uint8_t dtype;  // Arrow dtype of the argument
   uint8_t out_dtype;
-};
-
-__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
-  x ^= x >> 33; x *= 0xff51afd7ed558ccdull;
-  x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull;
-  x ^= x >> 33;
-  return x;
-}
-
-// Capacity and probe sequence of the group table and of the COUNT(DISTINCT) pair sets: cap slots (a power of two), a
-// hash's home slot is its TOP log2(cap) bits, and probing steps linearly, wrapping at cap.  The host fills both fields
-// (set_cap); every kernel that places or looks up a key goes through home() and next().
-struct ProbeRule {
-  long long cap;
-  int hshift;  // 64 - log2(cap)
-  __host__ void set_cap(long long c) {
-    int lg = 0;
-    while ((1ll << lg) < c) lg++;
-    cap = c;
-    hshift = 64 - lg;
-  }
-  __device__ __forceinline__ unsigned long long home(unsigned long long hash) const { return hshift >= 64 ? 0ull : hash >> hshift; }
-  __device__ __forceinline__ unsigned long long next(unsigned long long slot) const { return (slot + 1ull) & ((unsigned long long)cap - 1ull); }
 };
 
 // Table addressing.  A slot is a LINE of lw 64-bit words (lw a power of two; word 0 = the packed key) plus
@@ -1619,15 +1596,8 @@ struct DevBufs {
   }
 };
 
-long long next_pow2(long long x) {
-  long long p = 1;
-  while (p < x) p <<= 1;
-  return p;
-}
-
-// Sizing policy of the group table and the pair sets: a table for n entries has at least min_cap slots and at least twice
-// n, rounded up to a power of two; it takes new entries up to half full and grows x4.
-long long table_cap(long long n, long long min_cap) { return std::max(min_cap, next_pow2(2 * n)); }
+// Growth policy of the group table and the pair sets (sized by table_cap, hash_table.cuh): a table takes new entries up
+// to half full and grows x4.
 long long fill_limit(long long cap) { return cap / 2; }
 long long grown_cap(long long cap) { return cap * 4; }
 

@@ -245,18 +245,6 @@ std::shared_ptr<FunctionMeta> builtin_function_meta(const std::string& name) {
 // ---- Expr -> postfix program of the C ABI -------------------------------------------------------------
 namespace {
 
-void collect_columns(const Expr& e, std::set<size_t>& acc) {  // collect_expr, sqlplanner.rs:435-458
-  switch (e.kind) {
-    case Expr::Column: acc.insert(e.index); break;
-    case Expr::BinaryExpr: collect_columns(*e.left, acc); collect_columns(*e.right, acc); break;
-    case Expr::Cast: case Expr::IsNull: case Expr::IsNotNull: case Expr::Sort: collect_columns(*e.left, acc); break;
-    case Expr::ScalarFunction: case Expr::AggregateFunction:
-      for (auto& a : e.args) collect_columns(*a, acc);
-      break;
-    default: break;
-  }
-}
-
 void lower(const Expr& e, const Schema& schema, const std::map<size_t, int>& remap, std::vector<dfgpu_insn>& out) {
   dfgpu_insn in;
   memset(&in, 0, sizeof(in));
@@ -536,6 +524,156 @@ RecordBatch GpuFilterProjectRelation::process(const RecordBatch& in_batch, const
   return download(r.r, out_schema);
 }
 
+// ---- join -------------------------------------------------------------------------------------------------
+namespace {
+
+// the same expression with every column index lowered by `by` (a right-input key over the joined schema -> over the
+// right input's own schema)
+ExprRef shift_columns(const ExprRef& e, size_t by) {
+  auto c = std::make_shared<Expr>(*e);
+  if (c->kind == Expr::Column) c->index -= by;
+  if (c->left) c->left = shift_columns(c->left, by);
+  if (c->right) c->right = shift_columns(c->right, by);
+  for (auto& a : c->args) a = shift_columns(a, by);
+  return c;
+}
+
+void set_bit(std::vector<uint8_t>& bits, int64_t i, bool v) {
+  if (v) bits[size_t(i >> 3)] |= uint8_t(1u << (i & 7));
+}
+bool get_bit(const uint8_t* bits, int64_t i) { return (bits[i >> 3] >> (i & 7)) & 1; }
+
+// One owned array holding column `c` of every batch, in order (Utf8 offsets rebased, bitmaps re-packed).
+ArrayRef concat_column(const std::vector<RecordBatch>& batches, size_t c, DataType dt) {
+  auto out = std::make_shared<Array>();
+  out->data_type = dt;
+  int64_t n = 0, nulls = 0;
+  for (auto& b : batches) {
+    n += b.columns[c]->len;
+    nulls += b.columns[c]->null_count;
+  }
+  out->len = n;
+  out->null_count = nulls;
+  if (nulls > 0) out->own_validity.assign(size_t((n + 7) / 8), 0);
+  const int w = datatype_width(dt);
+  if (dt == DFGPU_BOOL) out->own_values.assign(size_t((n + 7) / 8), 0);
+  else if (w > 0) out->own_values.resize(size_t(n) * size_t(w));
+  if (dt == DFGPU_UTF8) out->own_offsets.assign(1, 0);
+  int64_t row = 0;
+  for (auto& b : batches) {
+    const Array& a = *b.columns[c];
+    for (int64_t r = 0; r < a.len && nulls > 0; r++)
+      set_bit(out->own_validity, row + r, a.null_count == 0 || !a.validity || get_bit(a.validity, a.offset + r));
+    if (dt == DFGPU_BOOL) {
+      for (int64_t r = 0; r < a.len; r++) set_bit(out->own_values, row + r, get_bit(static_cast<const uint8_t*>(a.values), a.offset + r));
+    } else if (w > 0) {
+      if (a.len > 0) memcpy(out->own_values.data() + size_t(row) * size_t(w), static_cast<const uint8_t*>(a.values) + size_t(a.offset) * size_t(w), size_t(a.len) * size_t(w));
+    } else if (dt == DFGPU_UTF8) {
+      const int32_t lo = a.offsets[a.offset], base = out->own_offsets.back();
+      if (int64_t(base) + a.offsets[a.offset + a.len] - lo >= (int64_t(1) << 31)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "JOIN build column of more than 2 GiB of Utf8");
+      const uint8_t* bytes = static_cast<const uint8_t*>(a.values);
+      out->own_values.insert(out->own_values.end(), bytes + lo, bytes + a.offsets[a.offset + a.len]);
+      for (int64_t r = 1; r <= a.len; r++) out->own_offsets.push_back(base + (a.offsets[a.offset + r] - lo));
+    }
+    row += a.len;
+  }
+  out->values = out->own_values.data();
+  out->values_bytes = int64_t(out->own_values.size());
+  out->validity = nulls > 0 ? out->own_validity.data() : nullptr;
+  out->offsets = dt == DFGPU_UTF8 ? out->own_offsets.data() : nullptr;
+  return out;
+}
+
+std::vector<ExprRef> column_exprs(const std::vector<size_t>& cols) {
+  std::vector<ExprRef> v;
+  for (size_t c : cols) v.push_back(Expr::column(c));
+  return v;
+}
+
+struct Programs {
+  std::vector<std::vector<dfgpu_insn>> progs;
+  std::vector<const dfgpu_insn*> ptr;
+  std::vector<int> len;
+  Programs(const std::vector<ExprRef>& exprs, const Schema& schema, const Pruned& pr) : progs(exprs.size()) {
+    for (size_t i = 0; i < exprs.size(); i++) {
+      lower(*exprs[i], schema, pr.remap, progs[i]);
+      ptr.push_back(progs[i].data());
+      len.push_back(int(progs[i].size()));
+    }
+  }
+};
+
+}  // namespace
+
+GpuHashJoinRelation::GpuHashJoinRelation(dfgpu_ctx* gpu, SchemaRef schema, RelationRef left, RelationRef right, std::vector<ExprRef> left_keys,
+                                         std::vector<ExprRef> right_keys, std::vector<size_t> left_cols, std::vector<size_t> right_cols)
+    : gpu_(gpu), schema_(std::move(schema)), left_(std::move(left)), right_(std::move(right)), left_keys_(std::move(left_keys)),
+      right_keys_(std::move(right_keys)), left_cols_(std::move(left_cols)), right_cols_(std::move(right_cols)) {}
+
+GpuHashJoinRelation::~GpuHashJoinRelation() { release(); }
+
+void GpuHashJoinRelation::release() {
+  if (join_) dfgpu_join_free(join_);
+  join_ = nullptr;
+  released_ = true;
+}
+
+void GpuHashJoinRelation::build() {
+  std::vector<RecordBatch> batches;
+  while (auto b = right_->next()) batches.push_back(std::move(*b));
+  const Schema& rs = *right_->schema();
+  std::vector<ExprRef> all = right_keys_;
+  for (auto& e : column_exprs(right_cols_)) all.push_back(e);
+  Pruned pr = prune(all, rs.fields.size(), false);
+  RecordBatch whole;  // the referenced columns of every batch, concatenated (the build table is built once)
+  whole.columns.resize(rs.fields.size());
+  for (size_t c : pr.cols) whole.columns[c] = concat_column(batches, c, rs.fields[c].data_type);
+  BatchGuard b;
+  b.b = upload(gpu_, whole, pr);
+  batches.clear();
+  Programs keys(right_keys_, rs, pr);
+  std::vector<int> keep;
+  for (size_t c : right_cols_) keep.push_back(pr.remap.at(c));
+  GPU_CHECK(dfgpu_join_build(gpu_, b.b, keys.ptr.data(), keys.len.data(), int(keys.ptr.size()), keep.data(), int(keep.size()), &join_));
+  build_out_ = keep;
+}
+
+std::optional<RecordBatch> GpuHashJoinRelation::next() {
+  if (released_) return std::nullopt;
+  if (!join_) build();
+  auto batch = left_->next();
+  if (!batch) {  // probe side exhausted: the table is not needed any more
+    release();
+    return std::nullopt;
+  }
+  const Schema& ls = *left_->schema();
+  std::vector<ExprRef> all = left_keys_;
+  for (auto& e : column_exprs(left_cols_)) all.push_back(e);
+  Pruned pr = prune(all, batch->columns.size(), false);
+  BatchGuard b;
+  b.b = upload(gpu_, *batch, pr);
+  Programs keys(left_keys_, ls, pr);
+  std::vector<int> probe_cols;
+  for (size_t c : left_cols_) probe_cols.push_back(pr.remap.at(c));
+  ResultGuard r;
+  GPU_CHECK(dfgpu_join_probe(join_, b.b, keys.ptr.data(), keys.len.data(), int(keys.ptr.size()), probe_cols.data(), int(probe_cols.size()),
+                             build_out_.data(), int(build_out_.size()), &r.r));
+  RecordBatch got = download(r.r, schema_);
+  RecordBatch out;
+  out.schema = schema_;
+  out.num_rows = got.num_rows;
+  for (auto& f : schema_->fields) {  // placeholders: dtype and length only
+    auto a = std::make_shared<Array>();
+    a->data_type = f.data_type;
+    a->len = got.num_rows;
+    out.columns.push_back(a);
+  }
+  const size_t nl = ls.fields.size();
+  for (size_t i = 0; i < left_cols_.size(); i++) out.columns[left_cols_[i]] = got.columns[i];
+  for (size_t i = 0; i < right_cols_.size(); i++) out.columns[nl + right_cols_[i]] = got.columns[left_cols_.size() + i];
+  return out;
+}
+
 GpuAggregateRelation::GpuAggregateRelation(dfgpu_ctx* gpu, SchemaRef schema, RelationRef input, std::vector<ExprRef> group_expr,
                                            std::vector<ExprRef> aggr_expr, ExprRef predicate)
     : gpu_(gpu), schema_(std::move(schema)), input_(std::move(input)), group_expr_(std::move(group_expr)), aggr_expr_(std::move(aggr_expr)),
@@ -695,6 +833,8 @@ ExecutionContext::ExecutionContext(int device) : datasources_(std::make_shared<s
   GPU_CHECK(dfgpu_init(device, &gpu_));
 }
 ExecutionContext::~ExecutionContext() {
+  for (auto& w : joins_)
+    if (auto j = w.lock()) j->release();
   if (gpu_) dfgpu_shutdown(gpu_);
 }
 
@@ -715,18 +855,43 @@ PlanRef ExecutionContext::plan(const std::string& sql) {
 
 RelationRef ExecutionContext::sql(const std::string& sql) { return execute(plan(sql)); }
 
-RelationRef ExecutionContext::execute(const PlanRef& plan) {
+RelationRef ExecutionContext::execute(const PlanRef& plan) { return execute_node(plan, nullptr, true); }
+
+RelationRef ExecutionContext::execute_node(const PlanRef& plan, const std::set<size_t>* needed, bool shard) {
   if (verbose) printf("Logical plan: %s\n", plan->debug().c_str());
   switch (plan->kind) {
     case LogicalPlan::TableScan: {
       auto it = datasources_->find(plan->table_name);
       if (it == datasources_->end()) fail(DFGPU_ERR_GENERAL, "No table registered as '" + plan->table_name + "'");
       RelationRef scan = std::make_shared<DataSourceRelation>(it->second);
-      if (world_ > 1) return std::make_shared<ShardRelation>(scan, rank_, world_);  // this rank's row range of every batch
+      if (world_ > 1 && shard) return std::make_shared<ShardRelation>(scan, rank_, world_);  // this rank's row range of every batch
       return scan;
     }
+    case LogicalPlan::Join: {
+      // Broadcast join across ranks: the probe (left) side keeps the sharding of its leftmost table, the build (right)
+      // side is the whole table on every rank, so every output pair is produced by exactly one rank.
+      const size_t nl = plan->input->schema()->fields.size(), n = plan->schema()->fields.size();
+      std::vector<size_t> lcols, rcols;
+      for (size_t c = 0; c < n; c++)
+        if (!needed || needed->count(c)) (c < nl ? lcols : rcols).push_back(c < nl ? c : c - nl);
+      std::vector<ExprRef> lkeys, rkeys;
+      std::set<size_t> lneed(lcols.begin(), lcols.end());
+      for (auto& k : plan->on_keys) {
+        lkeys.push_back(k.first);
+        rkeys.push_back(shift_columns(k.second, nl));
+        collect_columns(*k.first, lneed);
+      }
+      RelationRef l = execute_node(plan->input, &lneed, shard);
+      RelationRef r = execute_node(plan->right, nullptr, false);
+      auto j = std::make_shared<GpuHashJoinRelation>(gpu_, plan->schema(), l, r, lkeys, rkeys, lcols, rcols);
+      joins_.push_back(j);
+      return j;
+    }
     case LogicalPlan::Selection: {  // context.rs:126-139 -> FilterRelation
-      RelationRef input_rel = execute(plan->input);
+      // FilterRelation alone passes every input column on, so every column is needed (nullptr): a Join below then
+      // materialises all its columns and leaves no placeholder.  (The planner fuses a Selection into the Projection or
+      // Aggregate above it, which prune instead.)
+      RelationRef input_rel = execute_node(plan->input, nullptr, shard);
       return std::make_shared<GpuFilterProjectRelation>(gpu_, input_rel, plan->expr[0], std::vector<ExprRef>{}, input_rel->schema());
     }
     case LogicalPlan::Projection: {  // context.rs:140-161 -> ProjectRelation (fused with a Selection below it)
@@ -736,7 +901,10 @@ RelationRef ExecutionContext::execute(const PlanRef& plan) {
         pred = src->expr[0];
         src = src->input;
       }
-      RelationRef input_rel = execute(src);
+      std::set<size_t> used;
+      for (auto& e : plan->expr) collect_columns(*e, used);
+      if (pred) collect_columns(*pred, used);
+      RelationRef input_rel = execute_node(src, &used, shard);
       const Schema& in_schema = *input_rel->schema();
       auto schema = std::make_shared<Schema>();
       for (auto& e : plan->expr)  // projection.rs:52-57: (name, type, nullable = true)
@@ -753,7 +921,11 @@ RelationRef ExecutionContext::execute(const PlanRef& plan) {
         pred = src->expr[0];
         src = src->input;
       }
-      RelationRef input_rel = execute(src);
+      std::set<size_t> used;
+      for (auto& e : plan->group_expr) collect_columns(*e, used);
+      for (auto& e : plan->aggr_expr) collect_columns(*e, used);
+      if (pred) collect_columns(*pred, used);
+      RelationRef input_rel = execute_node(src, &used, shard);
       return std::make_shared<GpuAggregateRelation>(gpu_, plan->schema(), input_rel, plan->group_expr, plan->aggr_expr, pred);
     }
     default:

@@ -8,6 +8,7 @@
 #include <fstream>
 #include <map>
 #include <optional>
+#include <set>
 
 #include "sqlplanner.h"
 
@@ -135,6 +136,36 @@ class GpuAggregateRelation : public Relation {
   bool end_of_results_ = false;
 };
 
+// Inner equi-join (LogicalPlan::Join; the reference has no join relation).  On the first next() it drains the build
+// (right) relation, concatenates its batches on the host and builds the GPU hash table (dfgpu_join_build); then each
+// batch of the probe (left) relation gives one output batch (dfgpu_join_probe).  `left_keys` are over the left schema,
+// `right_keys` over the right schema.
+// Output batches have the joined schema's column positions, but only the columns in `left_cols` / `right_cols` (the ones
+// the plan above references) are materialised: every other column is an empty placeholder (its dtype and length, no
+// buffers), which no relation above reads.  So no unreferenced column is ever gathered or copied.
+// The join's device state lives from the first next() until the probe side is exhausted.  A relation dropped before
+// that holds it until release(): ExecutionContext releases every join it created before it shuts the GPU context
+// down, so a relation that outlives its context never touches a freed one (its next() then returns nothing).
+class GpuHashJoinRelation : public Relation {
+ public:
+  GpuHashJoinRelation(dfgpu_ctx* gpu, SchemaRef schema, RelationRef left, RelationRef right, std::vector<ExprRef> left_keys,
+                      std::vector<ExprRef> right_keys, std::vector<size_t> left_cols, std::vector<size_t> right_cols);
+  ~GpuHashJoinRelation() override;
+  std::optional<RecordBatch> next() override;
+  const SchemaRef& schema() const override { return schema_; }
+  void release();  // frees the device state; next() returns nothing afterwards
+ private:
+  void build();
+  dfgpu_ctx* gpu_;
+  SchemaRef schema_;
+  RelationRef left_, right_;
+  std::vector<ExprRef> left_keys_, right_keys_;
+  std::vector<size_t> left_cols_, right_cols_;
+  dfgpu_join* join_ = nullptr;
+  bool released_ = false;
+  std::vector<int> build_out_;  // right_cols_ as columns of the uploaded build batch
+};
+
 class ExecutionContext {
  public:
   explicit ExecutionContext(int device);  // ExecutionContext::new() + dfgpu_init
@@ -154,7 +185,11 @@ class ExecutionContext {
   int world() const { return world_; }
   bool verbose = false;  // the reference prints "Logical plan: ..." on every execute (context.rs:105)
  private:
+  // `needed`: the columns of the plan's output that the relations above read (null: all).  `shard`: whether a
+  // TableScan is cut to this rank's row range (not under a join's build side: every rank builds from the whole table).
+  RelationRef execute_node(const PlanRef& plan, const std::set<size_t>* needed, bool shard);
   std::shared_ptr<std::map<std::string, DataSourceRef>> datasources_;
+  std::vector<std::weak_ptr<GpuHashJoinRelation>> joins_;  // released before gpu_ is shut down
   dfgpu_ctx* gpu_ = nullptr;
   int rank_ = 0, world_ = 1;
 };

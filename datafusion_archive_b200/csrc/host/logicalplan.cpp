@@ -205,6 +205,18 @@ std::string Expr::debug() const {
   return "?";
 }
 
+void collect_columns(const Expr& e, std::set<size_t>& acc) {
+  switch (e.kind) {
+    case Expr::Column: acc.insert(e.index); break;
+    case Expr::BinaryExpr: collect_columns(*e.left, acc); collect_columns(*e.right, acc); break;
+    case Expr::Cast: case Expr::IsNull: case Expr::IsNotNull: case Expr::Sort: collect_columns(*e.left, acc); break;
+    case Expr::ScalarFunction: case Expr::AggregateFunction:
+      for (auto& a : e.args) collect_columns(*a, acc);
+      break;
+    default: break;
+  }
+}
+
 // ---- LogicalPlan -------------------------------------------------------------------------------------
 const SchemaRef& LogicalPlan::schema() const {
   if (kind == Selection) return input->schema();
@@ -256,6 +268,14 @@ static void fmt_with_indent(const LogicalPlan& p, std::string& f, int indent) {
     case LogicalPlan::Limit:
       f += "Limit: " + std::to_string(p.limit);
       fmt_with_indent(*p.input, f, indent + 1);
+      break;
+    case LogicalPlan::Join:
+      f += "Join: on=[";
+      for (size_t i = 0; i < p.on_keys.size(); i++)
+        f += (i ? ", " : "") + p.on_keys[i].first->debug() + " Eq " + p.on_keys[i].second->debug();
+      f += "]";
+      fmt_with_indent(*p.input, f, indent + 1);
+      fmt_with_indent(*p.right, f, indent + 1);
       break;
   }
 }

@@ -7,6 +7,7 @@
 #pragma once
 #include <cstdint>
 #include <memory>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -30,6 +31,7 @@ struct Field {
   std::string name;
   DataType data_type = 0;
   bool nullable = false;
+  std::string qualifier = {};  // the table (or its alias) a scanned column belongs to; `q.c` resolves by it.  Not printed.
 };
 struct Schema {
   std::vector<Field> fields;
@@ -87,12 +89,17 @@ struct Expr {
 struct LogicalPlan;
 using PlanRef = std::shared_ptr<const LogicalPlan>;
 struct LogicalPlan {
-  enum Kind { Limit, Projection, Selection, Aggregate, Sort, TableScan, EmptyRelation } kind = EmptyRelation;
+  // Join (no reference counterpart: ROADMAP.md 0.7.0): inner equi-join of `input` (left, probe side) and `right` (build
+  // side, always one TableScan) on on_keys (left expr, right expr), both over the joined schema = left fields ++ right
+  // fields.  Chains are left-deep.
+  enum Kind { Limit, Projection, Selection, Aggregate, Sort, TableScan, EmptyRelation, Join } kind = EmptyRelation;
   size_t limit = 0;
   std::vector<ExprRef> expr;        // Projection / Sort exprs; Selection: expr[0]
   std::vector<ExprRef> group_expr;  // Aggregate
   std::vector<ExprRef> aggr_expr;   // Aggregate
   PlanRef input;
+  PlanRef right;                                    // Join
+  std::vector<std::pair<ExprRef, ExprRef>> on_keys;  // Join
   SchemaRef schema_;
   std::string schema_name, table_name;
   bool has_projection = false;
@@ -101,6 +108,9 @@ struct LogicalPlan {
   const SchemaRef& schema() const;  // logicalplan.rs:352-362
   std::string debug() const;        // logicalplan.rs:365-442
 };
+
+// The column indices an expression reads (collect_expr, sqlplanner.rs:435-458), added to `acc`.
+void collect_columns(const Expr& e, std::set<size_t>& acc);
 
 // ---- type coercion lattice -------------------------------------------------------------------------
 bool get_supertype(DataType l, DataType r, DataType* out);  // logicalplan.rs:446-554

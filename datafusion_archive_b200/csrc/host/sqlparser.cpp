@@ -53,6 +53,9 @@ std::vector<Token> tokenize(const std::string& s) {
       if ((c == '<' && i + 1 < s.size() && (s[i + 1] == '=' || s[i + 1] == '>')) || (c == '>' && i + 1 < s.size() && s[i + 1] == '=') ||
           (c == '!' && i + 1 < s.size() && s[i + 1] == '=')) {
         t.text = s.substr(i, 2); i += 2;
+      } else if (c == '.' && !out.empty() && out.back().kind == Token::Ident && i + 1 < s.size() &&
+                 (isalpha((unsigned char)s[i + 1]) || s[i + 1] == '_' || s[i + 1] == '"')) {  // qualifier.name
+        t.text = "."; i++;
       } else if (std::string("=<>+-*/%(),;").find(c) != std::string::npos) {
         t.text = std::string(1, c); i++;
       } else {
@@ -77,7 +80,9 @@ struct Parser {
   void expect_kw(const char* s) { if (!accept_kw(s)) perr(std::string("Expected ") + s + ", found: " + peek().text); }
 
   static bool reserved(const std::string& u) {
-    static const char* kws[] = {"SELECT", "FROM", "WHERE", "GROUP", "BY", "HAVING", "ORDER", "LIMIT", "AND", "OR", "NOT", "AS", "ASC", "DESC", "IS", "NULL", "LIKE", "CAST"};
+    static const char* kws[] = {"SELECT", "FROM", "WHERE", "GROUP", "BY", "HAVING", "ORDER", "LIMIT", "AND", "OR", "NOT", "AS", "ASC", "DESC", "IS", "NULL", "LIKE", "CAST",
+                                 // joins: reserved so that `FROM a LEFT JOIN b` cannot read LEFT as an alias of a
+                                 "JOIN", "INNER", "ON", "LEFT", "RIGHT", "FULL", "OUTER", "CROSS", "NATURAL", "USING"};
     for (auto k : kws) if (u == k) return true;
     return false;
   }
@@ -194,6 +199,12 @@ struct Parser {
         }
         n->kind = ASTNode::SQLIdentifier;
         n->id = t.text;
+        if (accept_sym(".")) {  // qualifier.name
+          Token c = next();
+          if (c.kind != Token::Ident) perr("Expected a column name after " + t.text + ".");
+          n->qualifier = t.text;
+          n->id = c.text;
+        }
         return n;
       }
       default: perr("Unexpected end of input");
@@ -241,18 +252,38 @@ struct Parser {
     return n;
   }
 
+  // name [ [AS] alias ]
+  ASTRef parse_table_ref(const char* after) {
+    Token t = next();
+    if (t.kind != Token::Ident || reserved(upper(t.text))) perr(std::string("Expected a table name after ") + after);
+    auto r = std::make_shared<ASTNode>();
+    r->kind = ASTNode::SQLIdentifier;
+    r->id = t.text;
+    const bool as = accept_kw("AS");
+    if (peek().kind == Token::Ident && !reserved(upper(peek().text))) r->qualifier = next().text;
+    else if (as) perr("Expected an alias after AS");
+    return r;
+  }
+
   ASTRef parse_select() {
     expect_kw("SELECT");
     auto n = std::make_shared<ASTNode>();
     n->kind = ASTNode::SQLSelect;
     do { n->projection.push_back(parse_expr()); } while (accept_sym(","));
     if (accept_kw("FROM")) {
-      Token t = next();
-      if (t.kind != Token::Ident || reserved(upper(t.text))) perr("Expected a table name after FROM");
-      auto r = std::make_shared<ASTNode>();
-      r->kind = ASTNode::SQLIdentifier;
-      r->id = t.text;
-      n->relation = r;
+      n->relation = parse_table_ref("FROM");
+      for (;;) {
+        for (const char* kind : {"LEFT", "RIGHT", "FULL", "OUTER", "CROSS", "NATURAL"})
+          if (is_kw(kind)) fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string(kind) + " JOIN is not supported: only [INNER] JOIN .. ON");
+        if (accept_kw("INNER")) expect_kw("JOIN");
+        else if (!accept_kw("JOIN")) break;
+        JoinClause j;
+        j.relation = parse_table_ref("JOIN");
+        if (is_kw("USING")) perr("JOIN .. USING is not supported: use JOIN .. ON");
+        expect_kw("ON");
+        j.on = parse_expr();
+        n->joins.push_back(j);
+      }
     }
     if (accept_kw("WHERE")) n->selection = parse_expr();
     if (accept_kw("GROUP")) {

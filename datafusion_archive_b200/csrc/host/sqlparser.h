@@ -1,7 +1,11 @@
 // sqlparser.h — SQL subset front-end.  The reference delegates parsing to crate sqlparser 0.2.1
 // (Cargo.toml:34, wrapped by src/dfparser.rs:74); that crate is not in the reference repository, so this
 // is a restatement of the grammar subset the planner consumes (src/sqlplanner.rs:46-375): one
-// SELECT [list] [FROM ident] [WHERE e] [GROUP BY e,..] [HAVING e] [ORDER BY e [ASC|DESC],..] [LIMIT n].
+// SELECT [list] [FROM ident] [WHERE e] [GROUP BY e,..] [HAVING e] [ORDER BY e [ASC|DESC],..] [LIMIT n].  Beyond it, FROM
+// takes inner joins (the reference has none; its ROADMAP.md 0.7.0 plans them):
+//   from      := table_ref { [INNER] JOIN table_ref ON expr }
+//   table_ref := name [ [AS] alias ]
+//   column    := name | qualifier '.' name        -- qualifier = the alias if given, else the table name
 #pragma once
 #include <memory>
 #include <string>
@@ -15,10 +19,12 @@ enum class SQLType { Boolean, SmallInt, Int, BigInt, Float, Real, Double, Char, 
 struct ASTNode;
 using ASTRef = std::shared_ptr<ASTNode>;
 struct OrderByExpr { ASTRef expr; bool asc = true; };
+struct JoinClause { ASTRef relation; ASTRef on; };  // INNER JOIN relation ON on
 
 struct ASTNode {
   enum Kind { SQLIdentifier, SQLWildcard, SQLLong, SQLDouble, SQLString, SQLBinaryExpr, SQLCast, SQLIsNull, SQLIsNotNull, SQLFunction, SQLSelect } kind = SQLIdentifier;
   std::string id;       // identifier / function name / string literal / unknown type name
+  std::string qualifier;  // SQLIdentifier: `q` of a column `q.c`; of a table after FROM / JOIN: its alias, or empty
   long long lval = 0;   // SQLLong
   double dval = 0;      // SQLDouble
   ASTRef left, right;   // binary; `left` = operand of cast / is-null
@@ -32,6 +38,7 @@ struct ASTNode {
   bool has_group_by = false, has_order_by = false;
   std::vector<ASTRef> group_by;
   std::vector<OrderByExpr> order_by;
+  std::vector<JoinClause> joins;  // after `relation`, left-deep
   std::string debug() const;
 };
 

@@ -55,7 +55,8 @@ PlanRef SqlToRel::sql_to_rel(const ASTRef& sql) const {
     case ASTNode::SQLSelect: {
       // parse the input relation so we have access to the row type
       PlanRef input;
-      if (sql->relation) input = sql_to_rel(sql->relation);
+      ExprRef residual;  // the ON terms of the joins that are not keys
+      if (sql->relation) input = plan_from(*sql, &residual);
       else {
         auto e = std::make_shared<LogicalPlan>();
         e->kind = LogicalPlan::EmptyRelation;
@@ -66,10 +67,15 @@ PlanRef SqlToRel::sql_to_rel(const ASTRef& sql) const {
 
       // selection first
       PlanRef selection_plan;
-      if (sql->selection) {
+      if (sql->selection || residual) {  // the join residual first, then the WHERE clause
+        ExprRef pred = residual;
+        if (sql->selection) {
+          ExprRef where = sql_to_rex(sql->selection, *input_schema);
+          pred = pred ? Expr::binary(pred, Operator::And, where) : where;
+        }
         auto s = std::make_shared<LogicalPlan>();
         s->kind = LogicalPlan::Selection;
-        s->expr.push_back(sql_to_rex(sql->selection, *input_schema));
+        s->expr.push_back(pred);
         s->input = input;
         selection_plan = s;
       }
@@ -138,11 +144,72 @@ PlanRef SqlToRel::sql_to_rel(const ASTRef& sql) const {
       t->kind = LogicalPlan::TableScan;
       t->schema_name = "default";
       t->table_name = sql->id;
-      t->schema_ = schema;
+      auto qualified = std::make_shared<Schema>(*schema);  // each field knows its table, for `q.c`
+      for (auto& f : qualified->fields) f.qualifier = sql->qualifier.empty() ? sql->id : sql->qualifier;
+      t->schema_ = qualified;
       return t;
     }
     default: fail(DFGPU_ERR_EXECUTION, "sql_to_rel does not support this relation: " + sql->debug());
   }
+}
+
+namespace {
+// 1: every column of `e` is below `split` (at least one); 2: every one at or above it; 0: otherwise
+int side_of(const Expr& e, size_t split) {
+  std::set<size_t> cols;
+  collect_columns(e, cols);
+  if (cols.empty()) return 0;
+  bool l = false, r = false;
+  for (size_t c : cols) (c < split ? l : r) = true;
+  return l && r ? 0 : (l ? 1 : 2);
+}
+void and_terms(const ExprRef& e, std::vector<ExprRef>& out) {
+  if (e->kind == Expr::BinaryExpr && e->op == Operator::And) {
+    and_terms(e->left, out);
+    and_terms(e->right, out);
+  } else {
+    out.push_back(e);
+  }
+}
+}  // namespace
+
+// FROM table_ref { JOIN table_ref ON expr }: a left-deep chain of Join nodes.  Each ON clause is planned like a WHERE
+// clause over the joined schema; its top-level AND terms `l Eq r` with l over the left input only and r over the right
+// input only (or the reverse) are the keys, every other term is returned in *residual (AND-ed, in order) for the
+// Selection above the joins.
+PlanRef SqlToRel::plan_from(const ASTNode& select, ExprRef* residual) const {
+  PlanRef plan = sql_to_rel(select.relation);
+  std::vector<std::string> names{select.relation->qualifier.empty() ? select.relation->id : select.relation->qualifier};
+  for (const JoinClause& jc : select.joins) {
+    PlanRef right = sql_to_rel(jc.relation);
+    const std::string q = jc.relation->qualifier.empty() ? jc.relation->id : jc.relation->qualifier;
+    if (std::find(names.begin(), names.end(), q) != names.end())
+      fail(DFGPU_ERR_GENERAL, "Table '" + q + "' appears more than once in FROM: give each occurrence an alias");
+    names.push_back(q);
+    auto schema = std::make_shared<Schema>(*plan->schema());
+    const size_t split = schema->fields.size();
+    for (auto& f : right->schema()->fields) schema->fields.push_back(f);
+    ExprRef on = sql_to_rex(jc.on, *schema);
+    if (on->get_type(*schema) != DFGPU_BOOL) fail(DFGPU_ERR_GENERAL, "JOIN ON expression did not evaluate to boolean");
+    std::vector<ExprRef> terms;
+    and_terms(on, terms);
+    auto j = std::make_shared<LogicalPlan>();
+    j->kind = LogicalPlan::Join;
+    j->input = plan;
+    j->right = right;
+    j->schema_ = schema;
+    for (auto& t : terms) {
+      if (t->kind == Expr::BinaryExpr && t->op == Operator::Eq) {
+        const int l = side_of(*t->left, split), r = side_of(*t->right, split);
+        if (l == 1 && r == 2) { j->on_keys.emplace_back(t->left, t->right); continue; }
+        if (l == 2 && r == 1) { j->on_keys.emplace_back(t->right, t->left); continue; }
+      }
+      *residual = *residual ? Expr::binary(*residual, Operator::And, t) : t;
+    }
+    if (j->on_keys.empty()) fail(DFGPU_ERR_NOT_IMPLEMENTED, "JOIN needs at least one equality between the two inputs");
+    plan = j;
+  }
+  return plan;
 }
 
 ExprRef SqlToRel::sql_to_rex(const ASTRef& sql, const Schema& schema) const {
@@ -151,9 +218,19 @@ ExprRef SqlToRel::sql_to_rex(const ASTRef& sql, const Schema& schema) const {
     case ASTNode::SQLDouble: return Expr::literal(ScalarValue::Float64(sql->dval));
     case ASTNode::SQLString: return Expr::literal(ScalarValue::Utf8(sql->id));
     case ASTNode::SQLIdentifier: {
-      for (size_t i = 0; i < schema.fields.size(); i++)
-        if (schema.fields[i].name == sql->id) return Expr::column(i);
-      fail(DFGPU_ERR_EXECUTION, "Invalid identifier '" + sql->id + "' for schema " + schema.to_string());
+      // `q.c`: the field of that table (or alias) and name.  `c`: the first field of that name, unless fields of that
+      // name come from more than one table.
+      long long found = -1;
+      for (size_t i = 0; i < schema.fields.size(); i++) {
+        const Field& f = schema.fields[i];
+        if (f.name != sql->id || (!sql->qualifier.empty() && f.qualifier != sql->qualifier)) continue;
+        if (found < 0) found = (long long)i;
+        else if (schema.fields[size_t(found)].qualifier != f.qualifier)
+          fail(DFGPU_ERR_GENERAL, "Ambiguous reference to column '" + sql->id + "'");
+      }
+      if (found >= 0) return Expr::column(size_t(found));
+      fail(DFGPU_ERR_EXECUTION, "Invalid identifier '" + (sql->qualifier.empty() ? "" : sql->qualifier + ".") + sql->id + "' for schema " +
+                                    schema.to_string());
     }
     case ASTNode::SQLWildcard:
       fail(DFGPU_ERR_NOT_IMPLEMENTED, "SQL wildcard operator is not supported in projection - please use explicit column names");

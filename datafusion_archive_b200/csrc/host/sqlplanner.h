@@ -25,6 +25,7 @@ class SqlToRel {
   PlanRef sql_to_rel(const ASTRef& sql) const;                     // sqlplanner.rs:46-209
   ExprRef sql_to_rex(const ASTRef& sql, const Schema& schema) const;  // sqlplanner.rs:212-375
  private:
+  PlanRef plan_from(const ASTNode& select, ExprRef* residual) const;  // FROM with joins (no reference counterpart)
   std::shared_ptr<SchemaProvider> schema_provider_;
 };
 

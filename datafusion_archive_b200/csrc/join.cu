@@ -1,0 +1,564 @@
+// join.cu — inner equi-join on integer keys: a hash table built over the build (right) input, a two-pass probe of each
+// probe (left) batch, and a gather of the output columns by row index.  The reference has no join (its ROADMAP.md
+// lists "JOIN support (hash join ...)" for 0.7.0); include/dfgpu.h documents the semantics.
+//
+// Build (dfgpu_join_build), for n build rows:
+//   k_join_build    one thread per row packs the key, claims the key's slot (atomicCAS on the key word, the key equal
+//                   to EMPTY_KEY takes slot cap) and records the row's slot; each warp counts its rows per slot with one
+//                   atomic per distinct slot
+//   scan            the counts of the cap + 1 slots become each slot's start (scan_counts, three launches)
+//   k_join_scatter  every row writes its row number into its slot's range: the build rows of one key are contiguous
+// Probe (dfgpu_join_probe), for n probe rows:
+//   k_join_count    per row: the number of build rows with its key (0 for a null key or a miss) and their start
+//   scan            64-bit offsets of each row's output range; the total is the output row count
+//   k_join_emit     per OUTPUT position: the probe row owning it (a search of the offsets restricted to the rows of the
+//                   CTA's tile) and its build row.  The work is spread by output, so a probe row with millions of
+//                   matches is written by as many threads as rows with one match each.
+//   gathers         k_join_gather<T> (1, 2, 4, 8 bytes), k_join_gather_bits (validity and Boolean values), and
+//                   gather_utf8 (utf8_gather.cu) for Utf8 columns
+#include <memory>
+
+#include "hash_table.cuh"
+
+namespace dfgpu {
+
+void gather_utf8(dfgpu_ctx* ctx, const DevColumn& src, const unsigned long long* d_idx, long long nsel, DevColumn* out);
+
+constexpr int kMaxJoinKeys = 4;
+constexpr long long JN_MIN_CAP = 1024;  // the build table never grows: no floor beyond a small minimum
+constexpr int JN_THREADS = 256;
+constexpr int SCAN_ITEMS = 8;
+constexpr int SCAN_TILE = JN_THREADS * SCAN_ITEMS;
+constexpr int EMIT_TILE = 2048;  // output positions per CTA tile of k_join_emit
+
+// The key columns of one input: each part is read as its raw integer, sign- or zero-extended to 64 bits, masked to its
+// width and shifted into place (the aggregate's packing: the last key in the low bits, a single key keeps its 64-bit
+// value).  A row with a null part has no key.
+struct JoinKeys {
+  const void* vals[kMaxJoinKeys];
+  const unsigned char* valid[kMaxJoinKeys];  // null: no nulls
+  unsigned long long mask[kMaxJoinKeys];
+  int width[kMaxJoinKeys];
+  int is_signed[kMaxJoinKeys];
+  int shift[kMaxJoinKeys];
+  int nkeys;
+};
+
+__device__ __forceinline__ bool join_key(const JoinKeys& k, long long r, unsigned long long* out) {
+  unsigned long long key = 0;
+#pragma unroll
+  for (int i = 0; i < kMaxJoinKeys; i++) {
+    if (i >= k.nkeys) break;
+    if (k.valid[i] && !((k.valid[i][r >> 3] >> (r & 7)) & 1)) return false;
+    unsigned long long v;
+    switch (k.width[i]) {
+      case 1: v = k.is_signed[i] ? (unsigned long long)(long long)((const signed char*)k.vals[i])[r] : (unsigned long long)((const unsigned char*)k.vals[i])[r]; break;
+      case 2: v = k.is_signed[i] ? (unsigned long long)(long long)((const short*)k.vals[i])[r] : (unsigned long long)((const unsigned short*)k.vals[i])[r]; break;
+      case 4: v = k.is_signed[i] ? (unsigned long long)(long long)((const int*)k.vals[i])[r] : (unsigned long long)((const unsigned*)k.vals[i])[r]; break;
+      default: v = ((const unsigned long long*)k.vals[i])[r]; break;
+    }
+    key |= (v & k.mask[i]) << k.shift[i];
+  }
+  *out = key;
+  return true;
+}
+
+// ---- build -------------------------------------------------------------------------------------------------------
+// Both build kernels walk the rows a warp at a time (all lanes together, so that the warp can combine its rows) and
+// aggregate the slot counters per warp: the lanes whose rows share a slot (__match_any_sync) make ONE atomic, so a key
+// repeated millions of times costs one atomic per 32 rows instead of one per row.
+constexpr unsigned long long NO_SLOT = ~0ull;
+
+__global__ void __launch_bounds__(JN_THREADS) k_join_build(JoinKeys k, long long n, ProbeRule t, unsigned long long* __restrict__ keys,
+                                                          unsigned* __restrict__ counts, unsigned long long* __restrict__ row_slot) {
+  const int lane = threadIdx.x & 31;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long base = (long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31); base < n; base += stride) {
+    const long long r = base + lane;
+    unsigned long long key, h = NO_SLOT;
+    if (r < n && join_key(k, r, &key)) {
+      h = (unsigned long long)t.cap;  // the key that equals the empty marker
+      if (key != EMPTY_KEY) {
+        h = t.home(mix64(key));
+        for (;;) {  // at most n distinct keys in at least 2n slots: an empty slot is always found
+          unsigned long long cur = __ldcg(keys + h);
+          if (cur == EMPTY_KEY) cur = atomicCAS(keys + h, EMPTY_KEY, key);
+          if (cur == EMPTY_KEY || cur == key) break;
+          h = t.next(h);
+        }
+      }
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, h);
+    if (h != NO_SLOT && lane == __ffs(peers) - 1) atomicAdd(counts + h, (unsigned)__popc(peers));
+    if (r < n) row_slot[r] = h;
+  }
+}
+
+// counts[s] still holds the slot's row count: the rows of a slot take its places from the end of its range, a warp's
+// rows of one slot with one atomic
+__global__ void __launch_bounds__(JN_THREADS) k_join_scatter(const unsigned long long* __restrict__ row_slot, long long n,
+                                                            const unsigned long long* __restrict__ start, unsigned* __restrict__ counts,
+                                                            unsigned* __restrict__ rows) {
+  const int lane = threadIdx.x & 31;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long base = (long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31); base < n; base += stride) {
+    const long long r = base + lane;
+    const unsigned long long s = r < n ? row_slot[r] : NO_SLOT;
+    const unsigned peers = __match_any_sync(0xffffffffu, s);
+    const int leader = __ffs(peers) - 1;
+    unsigned end = 0;
+    if (s != NO_SLOT && lane == leader) end = atomicSub(counts + s, (unsigned)__popc(peers));
+    end = __shfl_sync(0xffffffffu, end, leader);
+    if (s == NO_SLOT) continue;
+    const unsigned k = end - (unsigned)__popc(peers) + (unsigned)__popc(peers & ((1u << lane) - 1u));
+    rows[start[s] + k] = (unsigned)r;
+  }
+}
+
+// ---- exclusive scan of u32 counts into u64 offsets: out[i] = sum of in[0..i), out[n] = the total ------------------------
+__global__ void __launch_bounds__(JN_THREADS) k_scan_counts(const unsigned* __restrict__ in, long long n, unsigned long long* __restrict__ out,
+                                                           unsigned long long* __restrict__ sums) {
+  __shared__ unsigned long long s_warp[JN_THREADS / 32];
+  const long long base = (long long)blockIdx.x * SCAN_TILE + (long long)threadIdx.x * SCAN_ITEMS;
+  unsigned long long v[SCAN_ITEMS];
+  unsigned long long run = 0;
+#pragma unroll
+  for (int i = 0; i < SCAN_ITEMS; i++) {
+    v[i] = run;  // exclusive within the thread
+    run += base + i < n ? in[base + i] : 0u;
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned long long incl = run;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long x = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += x;
+  }
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  unsigned long long excl = incl - run;
+  for (int w = 0; w < warp; w++) excl += s_warp[w];
+#pragma unroll
+  for (int i = 0; i < SCAN_ITEMS; i++)
+    if (base + i < n) out[base + i] = v[i] + excl;  // block-local; k_scan_add finishes it
+  if (threadIdx.x == JN_THREADS - 1) sums[blockIdx.x] = excl + run;
+}
+// one CTA: exclusive scan of the nb block totals in place; the grand total goes to *total
+__global__ void __launch_bounds__(1024) k_scan_totals(unsigned long long* __restrict__ sums, long long nb, unsigned long long* __restrict__ total) {
+  __shared__ unsigned long long s_part[1024];
+  const long long per = (nb + 1023) / 1024, lo = (long long)threadIdx.x * per, hi = min(nb, lo + per);
+  unsigned long long acc = 0;
+  for (long long b = lo; b < hi; b++) acc += sums[b];
+  s_part[threadIdx.x] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long run = 0;
+    for (int i = 0; i < 1024; i++) {
+      const unsigned long long x = s_part[i];
+      s_part[i] = run;
+      run += x;
+    }
+    *total = run;
+  }
+  __syncthreads();
+  unsigned long long run = s_part[threadIdx.x];
+  for (long long b = lo; b < hi; b++) {
+    const unsigned long long x = sums[b];
+    sums[b] = run;
+    run += x;
+  }
+}
+__global__ void __launch_bounds__(JN_THREADS) k_scan_add(unsigned long long* __restrict__ out, long long n, const unsigned long long* __restrict__ sums) {
+  const unsigned long long add = sums[blockIdx.x];
+  const long long base = (long long)blockIdx.x * SCAN_TILE;
+  for (int i = threadIdx.x; i < SCAN_TILE; i += JN_THREADS)
+    if (base + i < n) out[base + i] += add;
+}
+
+// ---- probe -----------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(JN_THREADS) k_join_count(JoinKeys k, long long n, ProbeRule t, const unsigned long long* __restrict__ keys,
+                                                          const unsigned long long* __restrict__ start, unsigned* __restrict__ cnt,
+                                                          unsigned* __restrict__ bpos) {
+  for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (long long)gridDim.x * blockDim.x) {
+    unsigned long long key;
+    unsigned c = 0, b = 0;
+    if (join_key(k, r, &key)) {
+      long long s = -1;
+      if (key == EMPTY_KEY) {
+        s = t.cap;
+      } else {
+        unsigned long long h = t.home(mix64(key));
+        for (long long probes = 0; probes < t.cap; probes++) {
+          const unsigned long long cur = keys[h];
+          if (cur == key) { s = (long long)h; break; }
+          if (cur == EMPTY_KEY) break;
+          h = t.next(h);
+        }
+      }
+      if (s >= 0) {
+        const unsigned long long s0 = start[s];
+        c = (unsigned)(start[s + 1] - s0);
+        b = (unsigned)s0;
+      }
+    }
+    cnt[r] = c;
+    bpos[r] = b;
+  }
+}
+
+// the last row p in [lo, hi] with off[p] <= o: the probe row whose output range holds position o
+__device__ __forceinline__ long long owner_row(const unsigned long long* __restrict__ off, unsigned long long o, long long lo, long long hi) {
+  while (lo < hi) {
+    const long long mid = lo + (hi - lo + 1) / 2;
+    if (off[mid] <= o) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+__global__ void __launch_bounds__(JN_THREADS) k_join_emit(const unsigned long long* __restrict__ off, long long n, const unsigned* __restrict__ bpos,
+                                                         const unsigned* __restrict__ rows, unsigned long long total,
+                                                         unsigned* __restrict__ out_probe, unsigned* __restrict__ out_build) {
+  __shared__ long long s_range[2];
+  for (unsigned long long o0 = (unsigned long long)blockIdx.x * EMIT_TILE; o0 < total; o0 += (unsigned long long)gridDim.x * EMIT_TILE) {
+    const unsigned long long o1 = min(total, o0 + EMIT_TILE) - 1ull;
+    if (threadIdx.x == 0) s_range[0] = owner_row(off, o0, 0, n - 1);
+    if (threadIdx.x == 32) s_range[1] = owner_row(off, o1, 0, n - 1);
+    __syncthreads();
+    const long long lo = s_range[0], hi = s_range[1];
+    for (unsigned long long o = o0 + threadIdx.x; o <= o1; o += JN_THREADS) {
+      const long long p = owner_row(off, o, lo, hi);
+      out_probe[o] = (unsigned)p;
+      out_build[o] = rows[bpos[p] + (unsigned)(o - off[p])];
+    }
+    __syncthreads();
+  }
+}
+
+// ---- gathers -----------------------------------------------------------------------------------------------------------
+template <class T>
+__global__ void __launch_bounds__(JN_THREADS) k_join_gather(const T* __restrict__ src, const unsigned* __restrict__ idx, long long n, T* __restrict__ out) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) out[i] = src[idx[i]];
+}
+// bit i of the output = bit idx[i] of src, written as whole 32-bit words; `zeros` (may be null) counts the zero bits
+__global__ void __launch_bounds__(JN_THREADS) k_join_gather_bits(const unsigned char* __restrict__ src, const unsigned* __restrict__ idx, long long n,
+                                                                unsigned* __restrict__ out, unsigned long long* __restrict__ zeros) {
+  const long long padded = (n + 31) & ~31ll;
+  unsigned long long z = 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < padded; i += (long long)gridDim.x * blockDim.x) {
+    bool bit = false;
+    if (i < n) {
+      const unsigned j = idx[i];
+      bit = (src[j >> 3] >> (j & 7)) & 1;
+    }
+    const unsigned w = __ballot_sync(0xffffffffu, bit);
+    if ((threadIdx.x & 31) == 0) {
+      out[i >> 5] = w;
+      const long long valid = min(32ll, n - i);
+      z += (unsigned long long)(valid - __popc(w));
+    }
+  }
+  if (zeros && z) atomicAdd(zeros, z);
+}
+__global__ void __launch_bounds__(JN_THREADS) k_join_widen(const unsigned* __restrict__ idx, long long n, unsigned long long* __restrict__ out) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) out[i] = idx[i];
+}
+
+// ---- host side ---------------------------------------------------------------------------------------------------------
+namespace {
+
+int grid_of(dfgpu_ctx* ctx, long long work) {
+  long long g = (work + JN_THREADS - 1) / JN_THREADS;
+  const long long most = (long long)ctx->sm_count * 16;
+  return int(g < 1 ? 1 : (g > most ? most : g));
+}
+
+// every launch: trace, profile ring, launch counter
+template <class Kernel, class... Args>
+void launch(dfgpu_ctx* ctx, const char* name, Kernel kernel, int grid, int block, Args... args) {
+  const int ps = ctx->prof_begin();
+  kernel<<<grid, block, 0, ctx->stream>>>(args...);
+  DF_CUDA(cudaGetLastError());
+  trace_launch(name);
+  ctx->prof_end(ps);
+  ctx->launches++;
+}
+
+// out[0..n] = exclusive scan of in[0..n) with out[n] = the total, which is returned.  Synchronises the stream.
+unsigned long long scan_counts(dfgpu_ctx* ctx, const unsigned* in, long long n, unsigned long long* out) {
+  const long long nb = std::max(1ll, (n + SCAN_TILE - 1) / SCAN_TILE);
+  unsigned long long* sums = (unsigned long long*)ctx->alloc(size_t(nb) * 8);
+  launch(ctx, "k_scan_counts", k_scan_counts, int(nb), JN_THREADS, in, n, out, sums);
+  launch(ctx, "k_scan_totals", k_scan_totals, 1, 1024, sums, nb, out + n);
+  launch(ctx, "k_scan_add", k_scan_add, int(nb), JN_THREADS, out, n, (const unsigned long long*)sums);
+  DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 56, out + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  DF_CUDA(cudaStreamSynchronize(ctx->stream));
+  ctx->free(sums);
+  return ctx->h_scratch[56];
+}
+
+// Device buffers freed at scope exit (stream-ordered, see dfgpu_ctx::free)
+struct Bufs {
+  dfgpu_ctx* ctx;
+  std::vector<void*> blocks;
+  explicit Bufs(dfgpu_ctx* c) : ctx(c) {}
+  Bufs(const Bufs&) = delete;
+  Bufs& operator=(const Bufs&) = delete;
+  ~Bufs() {
+    for (void* q : blocks) ctx->free(q);
+  }
+  template <class T>
+  T* alloc(size_t count) {
+    void* q = ctx->alloc(count * sizeof(T));
+    blocks.push_back(q);
+    return static_cast<T*>(q);
+  }
+};
+
+// The key columns of one batch.  A key program that is a plain integer column is read in place; any other program is
+// evaluated by the projection operator (no predicate), so its values are exactly the expression VM's.
+struct KeyColumns {
+  JoinKeys k{};
+  int dtypes[kMaxJoinKeys] = {};
+  std::vector<std::unique_ptr<dfgpu_result, int (*)(dfgpu_result*)>> evaluated;
+};
+
+void key_columns(dfgpu_ctx* ctx, const dfgpu_batch* b, const dfgpu_insn* const* keys, const int* key_len, int nkeys, KeyColumns* out) {
+  if (nkeys < 1 || !keys || !key_len) fail(DFGPU_ERR_GENERAL, "JOIN needs at least one key");
+  if (nkeys > kMaxJoinKeys) fail(DFGPU_ERR_NOT_IMPLEMENTED, "JOIN on more than " + std::to_string(kMaxJoinKeys) + " keys");
+  std::vector<int32_t> col_dtypes;
+  for (const DevColumn& c : b->cols) col_dtypes.push_back(c.dtype);
+  int bits = 0;
+  std::string widths;
+  for (int i = 0; i < nkeys; i++) {
+    int32_t dt = 0;
+    const int rc = dfgpu_check_program(col_dtypes.empty() ? nullptr : col_dtypes.data(), int(col_dtypes.size()), keys[i], key_len[i], &dt);
+    if (rc != DFGPU_OK) fail(rc, dfgpu_last_error());
+    if (!is_int(dt)) fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string("JOIN keys of type ") + dtype_name(dt) + " are not supported (integer keys only)");
+    out->dtypes[i] = dt;
+    bits += dtype_width(dt) * 8;
+    widths += (i ? " + " : "") + std::string(dtype_name(dt));
+  }
+  if (bits > 64) fail(DFGPU_ERR_NOT_IMPLEMENTED, "JOIN keys wider than 64 bits (" + widths + ")");
+  JoinKeys& k = out->k;
+  k.nkeys = nkeys;
+  int shift = 0;
+  for (int i = nkeys - 1; i >= 0; i--) {
+    const int w = dtype_width(out->dtypes[i]);
+    k.width[i] = w;
+    k.is_signed[i] = is_signed_int(out->dtypes[i]) ? 1 : 0;
+    k.shift[i] = shift;
+    k.mask[i] = w == 8 ? ~0ull : ((1ull << (8 * w)) - 1ull);
+    shift += 8 * w;
+  }
+  if (nkeys == 1) k.mask[0] = ~0ull;  // a single key keeps its sign- or zero-extended 64-bit value
+  for (int i = 0; i < nkeys; i++) {
+    const DevColumn* c = nullptr;
+    if (key_len[i] == 1 && keys[i][0].op == DFGPU_OP_COL) {
+      c = &b->cols[size_t(keys[i][0].col)];
+    } else {
+      dfgpu_result* r = nullptr;
+      const int rc = dfgpu_filter_project(ctx, b, nullptr, 0, &keys[i], &key_len[i], 1, &r);
+      if (rc != DFGPU_OK) fail(rc, dfgpu_last_error());
+      out->evaluated.emplace_back(r, dfgpu_result_free);
+      c = &r->cols[0];
+    }
+    k.vals[i] = c->values;
+    k.valid[i] = c->null_count > 0 ? c->validity : nullptr;
+  }
+}
+
+// Gather one column by a row-index list.  `idx64` is filled on first use (Utf8 columns take 64-bit indices).
+void gather_column(dfgpu_ctx* ctx, const DevColumn& src, const unsigned* idx, long long n, Bufs& scratch, unsigned long long*& idx64,
+                   unsigned long long* d_nulls, DevColumn* out) {
+  out->dtype = src.dtype;
+  const int grid = grid_of(ctx, n);
+  if (src.dtype == DFGPU_UTF8) {
+    if (!idx64) {
+      idx64 = scratch.alloc<unsigned long long>(size_t(std::max(1ll, n)));
+      if (n > 0) launch(ctx, "k_join_widen", k_join_widen, grid, JN_THREADS, idx, n, idx64);
+    }
+    gather_utf8(ctx, src, idx64, n, out);
+  } else if (src.dtype == DFGPU_BOOL) {
+    out->values_bytes = size_t((n + 31) / 32) * 4 + 4;
+    out->values = ctx->alloc(out->values_bytes);
+    if (n > 0)
+      launch(ctx, "k_join_gather_bits", k_join_gather_bits, grid, JN_THREADS, (const unsigned char*)src.values, idx, n, (unsigned*)out->values,
+             (unsigned long long*)nullptr);
+    out->values_bytes = size_t(n + 7) / 8;
+  } else {
+    const int w = dtype_width(src.dtype);
+    out->values_bytes = size_t(std::max(1ll, n)) * size_t(w);
+    out->values = ctx->alloc(out->values_bytes);
+    if (n > 0) {
+      switch (w) {
+        case 1: launch(ctx, "k_join_gather<1>", k_join_gather<unsigned char>, grid, JN_THREADS, (const unsigned char*)src.values, idx, n, (unsigned char*)out->values); break;
+        case 2: launch(ctx, "k_join_gather<2>", k_join_gather<unsigned short>, grid, JN_THREADS, (const unsigned short*)src.values, idx, n, (unsigned short*)out->values); break;
+        case 4: launch(ctx, "k_join_gather<4>", k_join_gather<unsigned>, grid, JN_THREADS, (const unsigned*)src.values, idx, n, (unsigned*)out->values); break;
+        default: launch(ctx, "k_join_gather<8>", k_join_gather<unsigned long long>, grid, JN_THREADS, (const unsigned long long*)src.values, idx, n, (unsigned long long*)out->values); break;
+      }
+    }
+  }
+  if (src.null_count > 0 && src.validity && n > 0) {
+    out->validity = (uint8_t*)ctx->alloc(size_t((n + 31) / 32) * 4);
+    DF_CUDA(cudaMemsetAsync(d_nulls, 0, 8, ctx->stream));
+    launch(ctx, "k_join_gather_bits", k_join_gather_bits, grid, JN_THREADS, (const unsigned char*)src.validity, idx, n, (unsigned*)out->validity, d_nulls);
+    DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 57, d_nulls, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    DF_CUDA(cudaStreamSynchronize(ctx->stream));
+    out->null_count = (int64_t)ctx->h_scratch[57];
+    if (out->null_count == 0) {
+      ctx->free(out->validity);
+      out->validity = nullptr;
+    }
+  }
+}
+
+}  // namespace
+}  // namespace dfgpu
+
+using namespace dfgpu;
+
+struct dfgpu_join {
+  dfgpu_ctx* ctx = nullptr;
+  int nkeys = 0;
+  int key_dtypes[kMaxJoinKeys] = {};
+  ProbeRule t{};
+  unsigned long long* keys = nullptr;   // cap + 1 key words, EMPTY_KEY when free; slot cap is the key EMPTY_KEY
+  unsigned long long* start = nullptr;  // cap + 2: the first entry of each slot's rows, then the number of rows with a key
+  unsigned* rows = nullptr;             // build row numbers, grouped by slot
+  long long nrows = 0;
+  std::vector<int> keep;           // build column numbers kept
+  std::vector<DevColumn> cols;     // their device copies, in the order of `keep`
+  ~dfgpu_join() {
+    if (!ctx) return;
+    cudaSetDevice(ctx->device);
+    ctx->free(keys);
+    ctx->free(start);
+    ctx->free(rows);
+    for (auto& c : cols) {
+      ctx->free(c.values);
+      ctx->free(c.validity);
+      ctx->free(c.offsets);
+    }
+  }
+};
+
+extern "C" int dfgpu_join_build(dfgpu_ctx* ctx, const dfgpu_batch* build, const dfgpu_insn* const* keys, const int* key_len, int nkeys,
+                                const int* keep_cols, int n_keep, dfgpu_join** out) {
+  return guarded([&] {
+    if (!ctx || !build || !out || (n_keep > 0 && !keep_cols) || n_keep < 0) fail(DFGPU_ERR_GENERAL, "dfgpu_join_build: null argument");
+    ctx->use();
+    const long long n = build->nrows;
+    if (n >= (1ll << 32)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "JOIN build side of 2^32 rows or more");
+    for (int i = 0; i < n_keep; i++)
+      if (keep_cols[i] < 0 || size_t(keep_cols[i]) >= build->cols.size()) fail(DFGPU_ERR_INVALID_COLUMN, "keep column " + std::to_string(keep_cols[i]) + " out of range");
+    KeyColumns kc;
+    key_columns(ctx, build, keys, key_len, nkeys, &kc);
+    auto j = std::make_unique<dfgpu_join>();
+    j->ctx = ctx;
+    j->nkeys = nkeys;
+    for (int i = 0; i < nkeys; i++) j->key_dtypes[i] = kc.dtypes[i];
+    j->nrows = n;
+    j->t.set_cap(table_cap(n, JN_MIN_CAP));
+    const long long cap = j->t.cap;
+    j->keys = (unsigned long long*)ctx->alloc(size_t(cap + 1) * 8);
+    j->start = (unsigned long long*)ctx->alloc(size_t(cap + 2) * 8);
+    j->rows = (unsigned*)ctx->alloc(size_t(std::max(1ll, n)) * 4);
+    Bufs scratch(ctx);
+    unsigned* counts = scratch.alloc<unsigned>(size_t(cap + 1));
+    unsigned long long* row_slot = scratch.alloc<unsigned long long>(size_t(std::max(1ll, n)));
+    DF_CUDA(cudaMemsetAsync(j->keys, 0xff, size_t(cap + 1) * 8, ctx->stream));
+    DF_CUDA(cudaMemsetAsync(counts, 0, size_t(cap + 1) * 4, ctx->stream));
+    if (n > 0) launch(ctx, "k_join_build", k_join_build, grid_of(ctx, n), JN_THREADS, kc.k, n, (ProbeRule)j->t, j->keys, counts, row_slot);
+    scan_counts(ctx, counts, cap + 1, j->start);
+    if (n > 0)
+      launch(ctx, "k_join_scatter", k_join_scatter, grid_of(ctx, n), JN_THREADS, (const unsigned long long*)row_slot, n,
+             (const unsigned long long*)j->start, counts, j->rows);
+    // the join's own copy of the kept columns: the caller may free the batch
+    for (int i = 0; i < n_keep; i++) {
+      const DevColumn& s = build->cols[size_t(keep_cols[i])];
+      DevColumn d;
+      d.dtype = s.dtype;
+      d.values_bytes = s.values_bytes;
+      d.null_count = s.null_count;
+      const size_t vb = s.dtype == DFGPU_UTF8 ? (s.values_bytes + 15) & ~size_t(15) : s.values_bytes;
+      d.values = ctx->alloc(vb);
+      if (vb) DF_CUDA(cudaMemcpyAsync(d.values, s.values, vb, cudaMemcpyDeviceToDevice, ctx->stream));
+      if (s.validity && s.null_count > 0) {
+        d.validity = (uint8_t*)ctx->alloc(size_t(n + 7) / 8);
+        DF_CUDA(cudaMemcpyAsync(d.validity, s.validity, size_t(n + 7) / 8, cudaMemcpyDeviceToDevice, ctx->stream));
+      }
+      if (s.offsets) {
+        d.offsets = (int32_t*)ctx->alloc(size_t(n + 1) * 4);
+        DF_CUDA(cudaMemcpyAsync(d.offsets, s.offsets, size_t(n + 1) * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+      }
+      j->keep.push_back(keep_cols[i]);
+      j->cols.push_back(d);
+    }
+    DF_CUDA(cudaStreamSynchronize(ctx->stream));
+    *out = j.release();
+  });
+}
+
+extern "C" int dfgpu_join_probe(dfgpu_join* j, const dfgpu_batch* probe, const dfgpu_insn* const* keys, const int* key_len, int nkeys,
+                                const int* probe_cols, int n_probe_cols, const int* build_cols, int n_build_cols, dfgpu_result** out) {
+  return guarded([&] {
+    if (!j || !probe || !out || (n_probe_cols > 0 && !probe_cols) || (n_build_cols > 0 && !build_cols) || n_probe_cols < 0 || n_build_cols < 0)
+      fail(DFGPU_ERR_GENERAL, "dfgpu_join_probe: null argument");
+    dfgpu_ctx* ctx = j->ctx;
+    ctx->use();
+    const long long n = probe->nrows;
+    if (n >= (1ll << 32)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "JOIN probe batch of 2^32 rows or more");
+    for (int i = 0; i < n_probe_cols; i++)
+      if (probe_cols[i] < 0 || size_t(probe_cols[i]) >= probe->cols.size()) fail(DFGPU_ERR_INVALID_COLUMN, "probe column " + std::to_string(probe_cols[i]) + " out of range");
+    std::vector<const DevColumn*> bsrc;
+    for (int i = 0; i < n_build_cols; i++) {
+      auto it = std::find(j->keep.begin(), j->keep.end(), build_cols[i]);
+      if (it == j->keep.end()) fail(DFGPU_ERR_GENERAL, "build column " + std::to_string(build_cols[i]) + " was not kept by dfgpu_join_build");
+      bsrc.push_back(&j->cols[size_t(it - j->keep.begin())]);
+    }
+    if (nkeys != j->nkeys) fail(DFGPU_ERR_GENERAL, "JOIN probe has " + std::to_string(nkeys) + " keys, the build side " + std::to_string(j->nkeys));
+    KeyColumns kc;
+    key_columns(ctx, probe, keys, key_len, nkeys, &kc);
+    for (int i = 0; i < nkeys; i++)
+      if (kc.dtypes[i] != j->key_dtypes[i])
+        fail(DFGPU_ERR_EXECUTION, std::string("JOIN key types differ: ") + dtype_name(kc.dtypes[i]) + " and " + dtype_name(j->key_dtypes[i]));
+    Bufs scratch(ctx);
+    unsigned* cnt = scratch.alloc<unsigned>(size_t(std::max(1ll, n)));
+    unsigned* bpos = scratch.alloc<unsigned>(size_t(std::max(1ll, n)));
+    unsigned long long* off = scratch.alloc<unsigned long long>(size_t(n + 1));
+    if (n > 0)
+      launch(ctx, "k_join_count", k_join_count, grid_of(ctx, n), JN_THREADS, kc.k, n, (ProbeRule)j->t, (const unsigned long long*)j->keys,
+             (const unsigned long long*)j->start, cnt, bpos);
+    const unsigned long long total = n > 0 ? scan_counts(ctx, cnt, n, off) : 0ull;
+    if (total >= (1ull << 32)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "JOIN probe batch producing 2^32 or more output rows");
+    const long long m = (long long)total;
+    unsigned* pidx = scratch.alloc<unsigned>(size_t(std::max(1ll, m)));
+    unsigned* bidx = scratch.alloc<unsigned>(size_t(std::max(1ll, m)));
+    if (m > 0) {
+      const long long tiles = (m + EMIT_TILE - 1) / EMIT_TILE;
+      const int grid = int(std::min<long long>(tiles, (long long)ctx->sm_count * 8));
+      launch(ctx, "k_join_emit", k_join_emit, grid, JN_THREADS, (const unsigned long long*)off, n, (const unsigned*)bpos, (const unsigned*)j->rows,
+             total, pidx, bidx);
+    }
+    auto res = std::make_unique<dfgpu_result>();
+    res->ctx = ctx;
+    res->nrows = m;
+    unsigned long long* d_nulls = scratch.alloc<unsigned long long>(1);
+    unsigned long long *p64 = nullptr, *b64 = nullptr;
+    for (int i = 0; i < n_probe_cols; i++) {
+      res->cols.emplace_back();
+      gather_column(ctx, probe->cols[size_t(probe_cols[i])], pidx, m, scratch, p64, d_nulls, &res->cols.back());
+    }
+    for (int i = 0; i < n_build_cols; i++) {
+      res->cols.emplace_back();
+      gather_column(ctx, *bsrc[size_t(i)], bidx, m, scratch, b64, d_nulls, &res->cols.back());
+    }
+    DF_CUDA(cudaStreamSynchronize(ctx->stream));
+    *out = res.release();
+  });
+}
+
+extern "C" int dfgpu_join_free(dfgpu_join* j) {
+  return guarded([&] { delete j; });
+}

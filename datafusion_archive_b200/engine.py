@@ -85,6 +85,10 @@ def lib():
     L.dfgpu_comm_unique_id.argtypes = [C.c_char_p]
     L.dfgpu_comm_init.argtypes = [vp, C.c_int, C.c_int, C.c_char_p]
     L.dfgpu_comm_destroy.argtypes = [vp]
+    PC = C.POINTER(C.c_int)
+    L.dfgpu_join_build.argtypes = [vp, vp, C.POINTER(PI), PC, C.c_int, PC, C.c_int, C.POINTER(vp)]
+    L.dfgpu_join_probe.argtypes = [vp, vp, C.POINTER(PI), PC, C.c_int, PC, C.c_int, PC, C.c_int, C.POINTER(vp)]
+    L.dfgpu_join_free.argtypes = [vp]
     if L.dfgpu_abi_version() != A.ABI_VERSION:
         raise RuntimeError("libdfgpu.so ABI version mismatch")
     _LIB = L
@@ -341,6 +345,18 @@ class GpuContext:
         finally:
             lib().dfgpu_aggregate_free(st)
 
+    # -- inner equi-join ---------------------------------------------------------------------------
+    def join_build(self, batch, keys, keep_cols=None):
+        """dfgpu_join_build: the hash table over `batch` (the right input) on the integer key expressions `keys`.
+        `keep_cols` (default: every column) are the columns later probes may return; the batch may be freed after."""
+        keep = []
+        kptrs, klens, nk = A.make_programs([k.program(batch.schema) for k in keys], keep)
+        cols = list(range(len(batch.schema))) if keep_cols is None else list(keep_cols)
+        carr = (C.c_int * max(1, len(cols)))(*cols)
+        out = C.c_void_p()
+        check(lib().dfgpu_join_build(self.h, batch.h, kptrs, klens, nk, carr, len(cols), C.byref(out)))
+        return Join(self, out, keep_cols=cols)
+
     # -- utilities ------------------------------------------------------------------------------
     def sync(self):
         check(lib().dfgpu_sync(self.h))
@@ -376,6 +392,38 @@ class GpuContext:
         if self.h:
             check(lib().dfgpu_shutdown(self.h))
             self.h = None
+
+
+class Join:
+    """A built join (dfgpu_join): probe it with any number of batches of the left input."""
+
+    def __init__(self, ctx, handle, keep_cols):
+        self.ctx, self.h, self.keep_cols = ctx, handle, keep_cols
+
+    def probe(self, batch, keys, probe_cols=None, build_cols=None):
+        """dfgpu_join_probe: one row per matching (probe row, build row) pair, the `probe_cols` of `batch` (default:
+        all) followed by the `build_cols` of the build batch (default: every kept column)."""
+        keep = []
+        kptrs, klens, nk = A.make_programs([k.program(batch.schema) for k in keys], keep)
+        pc = list(range(len(batch.schema))) if probe_cols is None else list(probe_cols)
+        bc = list(self.keep_cols) if build_cols is None else list(build_cols)
+        parr = (C.c_int * max(1, len(pc)))(*pc)
+        barr = (C.c_int * max(1, len(bc)))(*bc)
+        out = C.c_void_p()
+        check(lib().dfgpu_join_probe(self.h, batch.h, kptrs, klens, nk, parr, len(pc), barr, len(bc), C.byref(out)))
+        return Result(self.ctx, out)
+
+    def free(self):
+        if self.h:
+            if self.ctx.h:
+                check(lib().dfgpu_join_free(self.h))
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
 
 
 def comm_unique_id():

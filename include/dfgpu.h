@@ -329,6 +329,34 @@ int dfgpu_aggregate_update_host(dfgpu_aggstate* st, const dfgpu_col* cols, int n
 int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out);
 int dfgpu_aggregate_free(dfgpu_aggstate* st);
 
+/* ---- inner equi-join on integer keys ----
+ * The reference has no join: its planner plans none and its `Relation` trait (src/execution/relation.rs:27-32) has
+ * no join relation; "JOIN support (hash join ...)" is the headline of its next milestone (ROADMAP.md, 0.7.0).  These
+ * entry points are what a GpuHashJoinRelation implementing that trait calls: build once over the right input, then
+ * probe once per batch of the left input.
+ *   - A pair (probe row p, build row b) is output when every key is non-null on both sides and the keys are equal.
+ *     Null keys never match (SQL join semantics; unlike DFGPU_OP_EQ, under which a null equals a null).
+ *   - Output rows keep probe-row order; the order of one probe row's matches is unspecified.
+ *   - Keys are postfix programs of any of the 8 integer types, 1 to 4 of them, whose widths sum to at most 64 bits.
+ *     They are packed as GROUP BY keys are (the last key in the low bits; a single key keeps its sign- or
+ *     zero-extended 64-bit value).  A key program that is not a plain column is evaluated exactly as a projection
+ *     (a CAST(UInt32 AS Int32) wraps).  Probe key i must have the type of build key i (DFGPU_ERR_EXECUTION "JOIN key
+ *     types differ: Int32 and Int64").  Float, Boolean and Utf8 keys and keys wider than 64 bits are
+ *     DFGPU_ERR_NOT_IMPLEMENTED naming the types; a key raising DivideByZero is DFGPU_ERR_ARROW.
+ *   - Output columns keep their dtype and validity: fixed-width, Boolean (bit-packed) and Utf8.
+ *   - A build side of 2^32 rows or more, a probe batch of 2^32 rows or more and a probe batch producing 2^32 or more
+ *     output rows are DFGPU_ERR_NOT_IMPLEMENTED. */
+typedef struct dfgpu_join dfgpu_join; /* the build side's hash table and its kept columns */
+/* Build the table over `build` (borrowed for the call only).  The join keeps its own device copy of the columns
+ * `keep_cols` (build-batch column numbers), so the caller may free the batch afterwards. */
+int dfgpu_join_build(dfgpu_ctx* ctx, const dfgpu_batch* build, const dfgpu_insn* const* keys, const int* key_len, int nkeys,
+                     const int* keep_cols, int n_keep, dfgpu_join** out);
+/* Probe with one batch: the result is the `probe_cols` of `probe` followed by the `build_cols` of the build batch
+ * (its column numbering; each must be among `keep_cols`, else DFGPU_ERR_GENERAL), one row per matching pair. */
+int dfgpu_join_probe(dfgpu_join* j, const dfgpu_batch* probe, const dfgpu_insn* const* keys, const int* key_len, int nkeys,
+                     const int* probe_cols, int n_probe_cols, const int* build_cols, int n_build_cols, dfgpu_result** out);
+int dfgpu_join_free(dfgpu_join* j);
+
 /* ---- results ---- */
 int dfgpu_result_shape(const dfgpu_result* r, int64_t* nrows, int* ncols);
 int dfgpu_result_col_dtype(const dfgpu_result* r, int i, int32_t* dtype);

@@ -6,7 +6,8 @@ protocol of the engine at sizes a sanitizer finishes in minutes, each result che
 Covers: the mbarrier / cp.async.bulk pipeline of k_filter_project_tma (full, ragged and single tiles, lagged
 scan, dual ring), the direct filter kernel, the CAS / RED table of k_hash_agg_lean / _plain / interpreter, table
 growth with overflow replay, the shared-memory front tables, wide-key slots (busy / ready publication) and the
-chunked host pipelines."""
+chunked host pipelines, and the
+join's build, probe and gathers."""
 import os
 import sys
 
@@ -159,5 +160,27 @@ assert len(o[0]) == sum(1 for v in sv if v is not None and b"abx" in v.strip(b" 
 got = agg([sa, sx], [utf8_fn("length", col(0))], [AggregateFunction("count", col(1))])
 assert int(np.asarray(got[1]).sum()) == len(sv)
 print("utf8 functions ok", flush=True)
+# 10. Inner join: k_join_build's CAS claims and warp-aggregated counts (a hot key, the key that equals the empty marker,
+# null keys), k_join_scatter, the u32 -> u64 scan, k_join_count, k_join_emit's per-tile search (a skewed key and
+# one-match rows), and every gather: fixed width, the ballot-based bit gather (validity, Boolean) and Utf8
+jn = 50_003
+jbk = np.concatenate([np.full(5000, 3, np.int64), np.full(7, -1, np.int64), rng.integers(0, 20_000, jn - 5007)])
+jbv = rng.random(jn) > 0.05
+jbool = pa.array(rng.random(jn) > 0.5, mask=rng.random(jn) < 0.1)
+jpk = np.concatenate([np.array([3, -1, 3], np.int64), rng.integers(0, 40_000, 70_000)])
+jps = pa.array(["r%d" % (i % 97) * (i % 5) for i in range(len(jpk))], mask=rng.random(len(jpk)) < 0.1)
+jbb = ctx.upload([pa.array(jbk, mask=~jbv), np.arange(jn, dtype=np.int32), jbool])
+jpb = ctx.upload([jpk, jps, rng.random(len(jpk))])
+jj = ctx.join_build(jbb, [col(0)], keep_cols=[1, 2])
+jbb.free()
+jr = jj.probe(jpb, [col(0)], probe_cols=[1, 2], build_cols=[1, 2])
+jo = jr.columns()
+jcnt = {}
+for k, v in zip(jbk.tolist(), jbv.tolist()):
+    if v:
+        jcnt[k] = jcnt.get(k, 0) + 1
+assert jr.nrows == sum(jcnt.get(k, 0) for k in jpk.tolist())
+jr.free(); jj.free(); jpb.free()
+print("join ok", flush=True)
 ctx.close()
 print("SANITIZE_CASES_OK")

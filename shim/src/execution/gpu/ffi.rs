@@ -10,6 +10,7 @@ use super::super::error::{ExecutionError, Result};
 #[repr(C)] pub struct dfgpu_batch { _p: [u8; 0] }
 #[repr(C)] pub struct dfgpu_result { _p: [u8; 0] }
 #[repr(C)] pub struct dfgpu_aggstate { _p: [u8; 0] }
+#[repr(C)] pub struct dfgpu_join { _p: [u8; 0] }
 
 // dfgpu dtype codes (arrow::datatypes::DataType)
 pub const DT_BOOL: i32 = 1;
@@ -158,6 +159,18 @@ extern "C" {
     pub fn dfgpu_aggregate_update_host(st: *mut dfgpu_aggstate, cols: *const dfgpu_col, ncols: c_int, chunk_rows: i64) -> c_int;
     pub fn dfgpu_aggregate_finish(st: *mut dfgpu_aggstate, out: *mut *mut dfgpu_result) -> c_int;
     pub fn dfgpu_aggregate_free(st: *mut dfgpu_aggstate) -> c_int;
+    /// inner equi-join on integer keys (ROADMAP.md 0.7.0 "JOIN support"; no reference relation): build over the right
+    /// input once, keeping a device copy of `keep_cols`
+    pub fn dfgpu_join_build(
+        ctx: *mut dfgpu_ctx, build: *const dfgpu_batch, keys: *const *const dfgpu_insn, key_len: *const c_int, nkeys: c_int,
+        keep_cols: *const c_int, n_keep: c_int, out: *mut *mut dfgpu_join,
+    ) -> c_int;
+    /// one probe batch: its `probe_cols`, then the kept `build_cols`, one row per matching pair
+    pub fn dfgpu_join_probe(
+        j: *mut dfgpu_join, probe: *const dfgpu_batch, keys: *const *const dfgpu_insn, key_len: *const c_int, nkeys: c_int,
+        probe_cols: *const c_int, n_probe_cols: c_int, build_cols: *const c_int, n_build_cols: c_int, out: *mut *mut dfgpu_result,
+    ) -> c_int;
+    pub fn dfgpu_join_free(j: *mut dfgpu_join) -> c_int;
     pub fn dfgpu_result_shape(r: *const dfgpu_result, nrows: *mut i64, ncols: *mut c_int) -> c_int;
     pub fn dfgpu_result_col_dtype(r: *const dfgpu_result, i: c_int, dtype: *mut i32) -> c_int;
     pub fn dfgpu_result_col_bytes(r: *const dfgpu_result, i: c_int, nbytes: *mut i64) -> c_int;
