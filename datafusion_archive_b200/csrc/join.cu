@@ -1,4 +1,4 @@
-// join.cu — inner equi-join on integer keys: a hash table built over the build (right) input, a two-pass probe of each
+// join.cu — inner equi-join on integer and Utf8 keys: a hash table built over the build (right) input, a two-pass probe of each
 // probe (left) batch, and a gather of the output columns by row index.  The reference has no join (its ROADMAP.md
 // lists "JOIN support (hash join ...)" for 0.7.0); include/dfgpu.h documents the semantics.
 //
@@ -16,9 +16,22 @@
 //                   matches is written by as many threads as rows with one match each.
 //   gathers         k_join_gather<T> (1, 2, 4, 8 bytes), k_join_gather_bits (validity and Boolean values), and
 //                   gather_utf8 (utf8_gather.cu) for Utf8 columns
+//
+// A key with Utf8 parts takes its own build and count kernels; the scan, k_join_scatter, k_join_emit and the gathers
+// are shared.  Each row has a 64-bit tag (the packed integer parts and the hash of each Utf8 part), and a slot holds
+// one distinct KEY, not one tag: its tag, its integer word and a representative build row, the smallest with the key.
+//   k_join_utf8_place   one round over the rows not yet placed: a row stops at the first slot of this round with its
+//                       tag, or claims an empty one (atomicCAS on the tag), and atomicMin's its row into the slot's
+//                       representative
+//   k_join_utf8_verify  after the round: a row whose key equals its slot's representative is placed and counted (one
+//                       atomic per warp and slot); any other row goes to the next round, which starts past the slots
+//                       sealed here.  With 64-bit tags there is one round unless two keys collide.
+//   k_join_utf8_count   the probe: at a slot with the row's tag, the key is confirmed against the representative
+//                       (integer word, then each Utf8 part's length and bytes) before the slot counts as a match
 #include <memory>
 
 #include "hash_table.cuh"
+#include "utf8_words.cuh"
 
 namespace dfgpu {
 
@@ -115,6 +128,126 @@ __global__ void __launch_bounds__(JN_THREADS) k_join_scatter(const unsigned long
   }
 }
 
+// ---- Utf8 keys ---------------------------------------------------------------------------------------------------
+// The Utf8 parts of a key, in key order.  The integer parts stay in a JoinKeys, packed as above (with no integer part
+// the word is 0).  Byte buffers are 16-byte aligned and allocated in whole 16-byte words, so that load16 may read the
+// aligned word that holds a string's last byte.
+struct Utf8Keys {
+  const int* off[kMaxJoinKeys];
+  const unsigned char* bytes[kMaxJoinKeys];
+  const unsigned char* valid[kMaxJoinKeys];  // null: no nulls
+  int n;
+};
+
+// A row's integer word and tag: mix64 over the word and each Utf8 part's utf8_hash_bytes, cut to the tag width (its
+// top bits, which home() reads) and never EMPTY_KEY.  False for a row with a null part.
+__device__ __forceinline__ bool utf8_tag(const JoinKeys& k, const Utf8Keys& u, unsigned long long tag_mask, long long r, unsigned long long* word,
+                                         unsigned long long* tag) {
+  if (!join_key(k, r, word)) return false;
+  unsigned long long h = mix64(*word);
+  for (int i = 0; i < kMaxJoinKeys; i++) {
+    if (i >= u.n) break;
+    if (u.valid[i] && !((u.valid[i][r >> 3] >> (r & 7)) & 1)) return false;
+    h = mix64(h ^ utf8_hash_bytes(u.bytes[i], __ldg(u.off[i] + r), __ldg(u.off[i] + r + 1)));
+  }
+  h &= tag_mask;
+  *tag = h == EMPTY_KEY ? EMPTY_KEY - 1ull : h;
+  return true;
+}
+
+// the low k bytes of a 32-bit word (k <= 0: none)
+__device__ __forceinline__ unsigned low_bytes(int k) { return k >= 4 ? ~0u : (k <= 0 ? 0u : (1u << (8 * k)) - 1u); }
+
+// bytes [a0, a0 + len) of a equal bytes [b0, b0 + len) of b, compared one 16-byte word of each side per step
+__device__ __forceinline__ bool bytes_equal(const unsigned char* a, long long a0, const unsigned char* b, long long b0, int len) {
+  for (int i = 0; i < len; i += 16) {
+    const uint4 x = load16(a, a0 + i, len - i), y = load16(b, b0 + i, len - i);
+    const int k = len - i;
+    if (((x.x ^ y.x) & low_bytes(k)) | ((x.y ^ y.y) & low_bytes(k - 4)) | ((x.z ^ y.z) & low_bytes(k - 8)) | ((x.w ^ y.w) & low_bytes(k - 12)))
+      return false;
+  }
+  return true;
+}
+
+// every Utf8 part of row ra of a equals that of row rb of b: the lengths, then the bytes
+__device__ __forceinline__ bool utf8_parts_equal(const Utf8Keys& a, long long ra, const Utf8Keys& b, long long rb) {
+  for (int i = 0; i < kMaxJoinKeys; i++) {
+    if (i >= a.n) break;
+    const int a0 = __ldg(a.off[i] + ra), la = __ldg(a.off[i] + ra + 1) - a0;
+    const int b0 = __ldg(b.off[i] + rb), lb = __ldg(b.off[i] + rb + 1) - b0;
+    if (la != lb || !bytes_equal(a.bytes[i], a0, b.bytes[i], b0, la)) return false;
+  }
+  return true;
+}
+
+// One build round over the rows of `list` (null: rows 0..n).  A slot sealed in an earlier round is passed over: every
+// row of one key stops at the same slot in a round (the first of that round with its tag, or the empty one they all
+// race for), so a key still unplaced has no sealed slot.  The row's slot goes to row_slot, NO_SLOT for a null key.
+__global__ void __launch_bounds__(JN_THREADS) k_join_utf8_place(JoinKeys k, Utf8Keys u, unsigned long long tag_mask, const unsigned* __restrict__ list,
+                                                               long long n, ProbeRule t, unsigned long long* __restrict__ tags,
+                                                               const unsigned char* __restrict__ sealed, unsigned* __restrict__ rep,
+                                                               unsigned long long* __restrict__ row_slot) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long r = list ? (long long)list[i] : i;
+    unsigned long long word, tag, h = NO_SLOT;
+    if (utf8_tag(k, u, tag_mask, r, &word, &tag)) {
+      h = t.home(tag);
+      for (;;) {  // at most n distinct keys in at least 2n slots, one key per slot: an empty slot is always found
+        unsigned long long cur = __ldcg(tags + h);
+        if (cur == EMPTY_KEY) cur = atomicCAS(tags + h, EMPTY_KEY, tag);
+        if ((cur == EMPTY_KEY || cur == tag) && !sealed[h]) break;
+        h = t.next(h);
+      }
+      atomicMin(rep + h, (unsigned)r);
+    }
+    row_slot[r] = h;
+  }
+}
+
+// After a round, when every representative is final: a row equal to its slot's representative is placed and counted,
+// a warp's rows of one slot with one atomic; any other row is appended to `next`.  The representative seals its slot
+// and records the slot's integer word.
+__global__ void __launch_bounds__(JN_THREADS) k_join_utf8_verify(JoinKeys k, Utf8Keys u, const unsigned* __restrict__ list, long long n,
+                                                                const unsigned* __restrict__ rep, unsigned char* __restrict__ sealed,
+                                                                unsigned long long* __restrict__ words, const unsigned long long* __restrict__ row_slot,
+                                                                unsigned* __restrict__ counts, unsigned* __restrict__ next,
+                                                                unsigned long long* __restrict__ n_next) {
+  const int lane = threadIdx.x & 31;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long base = (long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31); base < n; base += stride) {
+    const long long i = base + lane;
+    long long r = 0;
+    unsigned long long h = NO_SLOT;
+    bool retry = false;
+    if (i < n) {
+      r = list ? (long long)list[i] : i;
+      h = row_slot[r];
+      if (h != NO_SLOT) {
+        const unsigned q = rep[h];
+        unsigned long long w, wq;
+        join_key(k, r, &w);
+        if (q == (unsigned)r) {
+          sealed[h] = 1;
+          words[h] = w;
+        } else if (!join_key(k, q, &wq) || w != wq || !utf8_parts_equal(u, r, u, q)) {
+          retry = true;
+          h = NO_SLOT;
+        }
+      }
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, h);
+    if (h != NO_SLOT && lane == __ffs(peers) - 1) atomicAdd(counts + h, (unsigned)__popc(peers));
+    const unsigned again = __ballot_sync(0xffffffffu, retry);
+    if (again) {
+      const int leader = __ffs(again) - 1;
+      unsigned long long at = 0;
+      if (lane == leader) at = atomicAdd(n_next, (unsigned long long)__popc(again));
+      at = __shfl_sync(0xffffffffu, at, leader);
+      if (retry) next[at + (unsigned)__popc(again & ((1u << lane) - 1u))] = (unsigned)r;
+    }
+  }
+}
+
 // ---- exclusive scan of u32 counts into u64 offsets: out[i] = sum of in[0..i), out[n] = the total ------------------------
 __global__ void __launch_bounds__(JN_THREADS) k_scan_counts(const unsigned* __restrict__ in, long long n, unsigned long long* __restrict__ out,
                                                            unsigned long long* __restrict__ sums) {
@@ -203,6 +336,35 @@ __global__ void __launch_bounds__(JN_THREADS) k_join_count(JoinKeys k, long long
     }
     cnt[r] = c;
     bpos[r] = b;
+  }
+}
+
+// The probe of a key with Utf8 parts: at a slot with the row's tag, the key is confirmed against the slot's integer word
+// and its representative's Utf8 parts (`b`: the join's copy of the build key columns) before it counts as a match;
+// two keys with one tag never match.
+__global__ void __launch_bounds__(JN_THREADS) k_join_utf8_count(JoinKeys k, Utf8Keys u, unsigned long long tag_mask, long long n, ProbeRule t,
+                                                               const unsigned long long* __restrict__ tags, const unsigned long long* __restrict__ words,
+                                                               const unsigned* __restrict__ rep, Utf8Keys b, const unsigned long long* __restrict__ start,
+                                                               unsigned* __restrict__ cnt, unsigned* __restrict__ bpos) {
+  for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (long long)gridDim.x * blockDim.x) {
+    unsigned long long word, tag;
+    unsigned c = 0, bp = 0;
+    if (utf8_tag(k, u, tag_mask, r, &word, &tag)) {
+      unsigned long long h = t.home(tag);
+      for (long long probes = 0; probes < t.cap; probes++) {
+        const unsigned long long cur = tags[h];
+        if (cur == EMPTY_KEY) break;
+        if (cur == tag && words[h] == word && utf8_parts_equal(u, r, b, rep[h])) {
+          const unsigned long long s0 = start[h];
+          c = (unsigned)(start[h + 1] - s0);
+          bp = (unsigned)s0;
+          break;
+        }
+        h = t.next(h);
+      }
+    }
+    cnt[r] = c;
+    bpos[r] = bp;
   }
 }
 
@@ -315,10 +477,13 @@ struct Bufs {
   }
 };
 
-// The key columns of one batch.  A key program that is a plain integer column is read in place; any other program is
-// evaluated by the projection operator (no predicate), so its values are exactly the expression VM's.
+// The key columns of one batch.  A key program that is a plain column is read in place; any other program is
+// evaluated by the projection operator (no predicate), so its values are exactly the expression VM's.  The integer
+// parts go to `k`, the Utf8 parts to `u` (with their columns in `ucols`), each in key order.
 struct KeyColumns {
   JoinKeys k{};
+  Utf8Keys u{};
+  const DevColumn* ucols[kMaxJoinKeys] = {};
   int dtypes[kMaxJoinKeys] = {};
   std::vector<std::unique_ptr<dfgpu_result, int (*)(dfgpu_result*)>> evaluated;
 };
@@ -334,24 +499,31 @@ void key_columns(dfgpu_ctx* ctx, const dfgpu_batch* b, const dfgpu_insn* const* 
     int32_t dt = 0;
     const int rc = dfgpu_check_program(col_dtypes.empty() ? nullptr : col_dtypes.data(), int(col_dtypes.size()), keys[i], key_len[i], &dt);
     if (rc != DFGPU_OK) fail(rc, dfgpu_last_error());
-    if (!is_int(dt)) fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string("JOIN keys of type ") + dtype_name(dt) + " are not supported (integer keys only)");
+    if (!is_int(dt) && dt != DFGPU_UTF8)
+      fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string("JOIN keys of type ") + dtype_name(dt) + " are not supported (integer keys only)");
     out->dtypes[i] = dt;
+    if (dt == DFGPU_UTF8) continue;  // Utf8 parts are hashed, not packed: they do not count toward the 64 bits
     bits += dtype_width(dt) * 8;
-    widths += (i ? " + " : "") + std::string(dtype_name(dt));
+    widths += (widths.empty() ? "" : " + ") + std::string(dtype_name(dt));
   }
   if (bits > 64) fail(DFGPU_ERR_NOT_IMPLEMENTED, "JOIN keys wider than 64 bits (" + widths + ")");
+  // the integer parts, in key order; with no Utf8 part they are the key
+  std::vector<int> ints;
+  for (int i = 0; i < nkeys; i++)
+    if (out->dtypes[i] != DFGPU_UTF8) ints.push_back(i);
+  const int nints = int(ints.size());
   JoinKeys& k = out->k;
-  k.nkeys = nkeys;
+  k.nkeys = nints;
   int shift = 0;
-  for (int i = nkeys - 1; i >= 0; i--) {
-    const int w = dtype_width(out->dtypes[i]);
+  for (int i = nints - 1; i >= 0; i--) {
+    const int w = dtype_width(out->dtypes[ints[size_t(i)]]);
     k.width[i] = w;
-    k.is_signed[i] = is_signed_int(out->dtypes[i]) ? 1 : 0;
+    k.is_signed[i] = is_signed_int(out->dtypes[ints[size_t(i)]]) ? 1 : 0;
     k.shift[i] = shift;
     k.mask[i] = w == 8 ? ~0ull : ((1ull << (8 * w)) - 1ull);
     shift += 8 * w;
   }
-  if (nkeys == 1) k.mask[0] = ~0ull;  // a single key keeps its sign- or zero-extended 64-bit value
+  if (nints == 1) k.mask[0] = ~0ull;  // a single key keeps its sign- or zero-extended 64-bit value
   for (int i = 0; i < nkeys; i++) {
     const DevColumn* c = nullptr;
     if (key_len[i] == 1 && keys[i][0].op == DFGPU_OP_COL) {
@@ -363,9 +535,52 @@ void key_columns(dfgpu_ctx* ctx, const dfgpu_batch* b, const dfgpu_insn* const* 
       out->evaluated.emplace_back(r, dfgpu_result_free);
       c = &r->cols[0];
     }
-    k.vals[i] = c->values;
-    k.valid[i] = c->null_count > 0 ? c->validity : nullptr;
+    const unsigned char* valid = c->null_count > 0 ? c->validity : nullptr;
+    if (out->dtypes[i] == DFGPU_UTF8) {
+      // every Utf8 buffer of the engine is allocated in whole 16-byte words: uploads, gathers and function outputs
+      Utf8Keys& u = out->u;
+      out->ucols[u.n] = c;
+      u.off[u.n] = c->offsets;
+      u.bytes[u.n] = (const unsigned char*)c->values;
+      u.valid[u.n] = valid;
+      u.n++;
+    } else {
+      const int p = int(std::find(ints.begin(), ints.end(), i) - ints.begin());
+      k.vals[p] = c->values;
+      k.valid[p] = valid;
+    }
   }
+}
+
+// DFGPU_JOIN_TAG_BITS=n (1..64, default 64): keep only the top n bits of a Utf8 key's tag, so that distinct keys share
+// tags and the confirmation is exercised
+unsigned long long join_tag_mask() {
+  const char* e = getenv("DFGPU_JOIN_TAG_BITS");
+  if (!e || !*e) return ~0ull;
+  char* end = nullptr;
+  const long bits = strtol(e, &end, 10);
+  if (*end || bits < 1 || bits > 64) fail(DFGPU_ERR_GENERAL, std::string("DFGPU_JOIN_TAG_BITS must be 1 to 64, not '") + e + "'");
+  return ~0ull << (64 - bits);
+}
+
+// The join's own device copy of one build column of n rows (Utf8 bytes in whole 16-byte words, as in the source)
+DevColumn copy_column(dfgpu_ctx* ctx, const DevColumn& s, long long n) {
+  DevColumn d;
+  d.dtype = s.dtype;
+  d.values_bytes = s.values_bytes;
+  d.null_count = s.null_count;
+  const size_t vb = s.dtype == DFGPU_UTF8 ? (s.values_bytes + 15) & ~size_t(15) : s.values_bytes;
+  d.values = ctx->alloc(vb);
+  if (vb) DF_CUDA(cudaMemcpyAsync(d.values, s.values, vb, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (s.validity && s.null_count > 0) {
+    d.validity = (uint8_t*)ctx->alloc(size_t(n + 7) / 8);
+    DF_CUDA(cudaMemcpyAsync(d.validity, s.validity, size_t(n + 7) / 8, cudaMemcpyDeviceToDevice, ctx->stream));
+  }
+  if (s.offsets) {
+    d.offsets = (int32_t*)ctx->alloc(size_t(n + 1) * 4);
+    DF_CUDA(cudaMemcpyAsync(d.offsets, s.offsets, size_t(n + 1) * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+  }
+  return d;
 }
 
 // Gather one column by a row-index list.  `idx64` is filled on first use (Utf8 columns take 64-bit indices).
@@ -429,12 +644,24 @@ struct dfgpu_join {
   long long nrows = 0;
   std::vector<int> keep;           // build column numbers kept
   std::vector<DevColumn> cols;     // their device copies, in the order of `keep`
+  // a key with Utf8 parts: `keys` holds each slot's tag, and a slot one distinct key
+  unsigned long long tag_mask = ~0ull;  // DFGPU_JOIN_TAG_BITS at build time
+  unsigned long long* words = nullptr;  // cap: each slot's packed integer word
+  unsigned* rep = nullptr;              // cap: each slot's representative build row
+  std::vector<DevColumn> ukeys;         // device copies of the build side's Utf8 key columns, in key order
   ~dfgpu_join() {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     ctx->free(keys);
     ctx->free(start);
     ctx->free(rows);
+    ctx->free(words);
+    ctx->free(rep);
+    for (auto& c : ukeys) {
+      ctx->free(c.values);
+      ctx->free(c.validity);
+      ctx->free(c.offsets);
+    }
     for (auto& c : cols) {
       ctx->free(c.values);
       ctx->free(c.validity);
@@ -442,6 +669,42 @@ struct dfgpu_join {
     }
   }
 };
+
+// The table of a key with Utf8 parts: rounds of k_join_utf8_place and k_join_utf8_verify until every row with a key is
+// placed, leaving each slot's row count in `counts` and each row's slot in `row_slot`, as k_join_build does.  Each
+// round seals at least one slot, the one of its smallest pending row.  Keeps a copy of the Utf8 key columns for the
+// probe's confirmation.
+static void build_utf8(dfgpu_ctx* ctx, const KeyColumns& kc, long long n, dfgpu_join* j, Bufs& scratch, unsigned* counts,
+                       unsigned long long* row_slot) {
+  const long long cap = j->t.cap;
+  j->words = (unsigned long long*)ctx->alloc(size_t(cap) * 8);
+  j->rep = (unsigned*)ctx->alloc(size_t(cap) * 4);
+  for (int i = 0; i < kc.u.n; i++) j->ukeys.push_back(copy_column(ctx, *kc.ucols[i], n));
+  DF_CUDA(cudaMemsetAsync(j->rep, 0xff, size_t(cap) * 4, ctx->stream));
+  if (n == 0) return;
+  unsigned char* sealed = scratch.alloc<unsigned char>(size_t(cap));
+  unsigned long long* d_next = scratch.alloc<unsigned long long>(1);
+  unsigned* lists[2] = {scratch.alloc<unsigned>(size_t(n)), nullptr};
+  DF_CUDA(cudaMemsetAsync(sealed, 0, size_t(cap), ctx->stream));
+  const unsigned* list = nullptr;  // the first round takes every row
+  long long pending = n;
+  for (int round = 0;; round++) {
+    unsigned* next = lists[round & 1];
+    if (!next) next = lists[1] = scratch.alloc<unsigned>(size_t(n));
+    DF_CUDA(cudaMemsetAsync(d_next, 0, 8, ctx->stream));
+    launch(ctx, "k_join_utf8_place", k_join_utf8_place, grid_of(ctx, pending), JN_THREADS, kc.k, kc.u, j->tag_mask, list, pending, (ProbeRule)j->t,
+           j->keys, (const unsigned char*)sealed, j->rep, row_slot);
+    launch(ctx, "k_join_utf8_verify", k_join_utf8_verify, grid_of(ctx, pending), JN_THREADS, kc.k, kc.u, list, pending, (const unsigned*)j->rep,
+           sealed, j->words, (const unsigned long long*)row_slot, counts, next, d_next);
+    DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 58, d_next, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    DF_CUDA(cudaStreamSynchronize(ctx->stream));
+    const long long left = (long long)ctx->h_scratch[58];
+    if (left == 0) return;
+    if (left >= pending) fail(DFGPU_ERR_INTERNAL, "JOIN build: a Utf8 key round placed no row");
+    list = next;
+    pending = left;
+  }
+}
 
 extern "C" int dfgpu_join_build(dfgpu_ctx* ctx, const dfgpu_batch* build, const dfgpu_insn* const* keys, const int* key_len, int nkeys,
                                 const int* keep_cols, int n_keep, dfgpu_join** out) {
@@ -469,31 +732,20 @@ extern "C" int dfgpu_join_build(dfgpu_ctx* ctx, const dfgpu_batch* build, const 
     unsigned long long* row_slot = scratch.alloc<unsigned long long>(size_t(std::max(1ll, n)));
     DF_CUDA(cudaMemsetAsync(j->keys, 0xff, size_t(cap + 1) * 8, ctx->stream));
     DF_CUDA(cudaMemsetAsync(counts, 0, size_t(cap + 1) * 4, ctx->stream));
-    if (n > 0) launch(ctx, "k_join_build", k_join_build, grid_of(ctx, n), JN_THREADS, kc.k, n, (ProbeRule)j->t, j->keys, counts, row_slot);
+    if (kc.u.n == 0) {
+      if (n > 0) launch(ctx, "k_join_build", k_join_build, grid_of(ctx, n), JN_THREADS, kc.k, n, (ProbeRule)j->t, j->keys, counts, row_slot);
+    } else {
+      j->tag_mask = join_tag_mask();
+      build_utf8(ctx, kc, n, j.get(), scratch, counts, row_slot);
+    }
     scan_counts(ctx, counts, cap + 1, j->start);
     if (n > 0)
       launch(ctx, "k_join_scatter", k_join_scatter, grid_of(ctx, n), JN_THREADS, (const unsigned long long*)row_slot, n,
              (const unsigned long long*)j->start, counts, j->rows);
     // the join's own copy of the kept columns: the caller may free the batch
     for (int i = 0; i < n_keep; i++) {
-      const DevColumn& s = build->cols[size_t(keep_cols[i])];
-      DevColumn d;
-      d.dtype = s.dtype;
-      d.values_bytes = s.values_bytes;
-      d.null_count = s.null_count;
-      const size_t vb = s.dtype == DFGPU_UTF8 ? (s.values_bytes + 15) & ~size_t(15) : s.values_bytes;
-      d.values = ctx->alloc(vb);
-      if (vb) DF_CUDA(cudaMemcpyAsync(d.values, s.values, vb, cudaMemcpyDeviceToDevice, ctx->stream));
-      if (s.validity && s.null_count > 0) {
-        d.validity = (uint8_t*)ctx->alloc(size_t(n + 7) / 8);
-        DF_CUDA(cudaMemcpyAsync(d.validity, s.validity, size_t(n + 7) / 8, cudaMemcpyDeviceToDevice, ctx->stream));
-      }
-      if (s.offsets) {
-        d.offsets = (int32_t*)ctx->alloc(size_t(n + 1) * 4);
-        DF_CUDA(cudaMemcpyAsync(d.offsets, s.offsets, size_t(n + 1) * 4, cudaMemcpyDeviceToDevice, ctx->stream));
-      }
       j->keep.push_back(keep_cols[i]);
-      j->cols.push_back(d);
+      j->cols.push_back(copy_column(ctx, build->cols[size_t(keep_cols[i])], n));
     }
     DF_CUDA(cudaStreamSynchronize(ctx->stream));
     *out = j.release();
@@ -527,9 +779,20 @@ extern "C" int dfgpu_join_probe(dfgpu_join* j, const dfgpu_batch* probe, const d
     unsigned* cnt = scratch.alloc<unsigned>(size_t(std::max(1ll, n)));
     unsigned* bpos = scratch.alloc<unsigned>(size_t(std::max(1ll, n)));
     unsigned long long* off = scratch.alloc<unsigned long long>(size_t(n + 1));
-    if (n > 0)
+    if (n > 0 && kc.u.n == 0)
       launch(ctx, "k_join_count", k_join_count, grid_of(ctx, n), JN_THREADS, kc.k, n, (ProbeRule)j->t, (const unsigned long long*)j->keys,
              (const unsigned long long*)j->start, cnt, bpos);
+    if (n > 0 && kc.u.n > 0) {
+      Utf8Keys b{};
+      for (const DevColumn& c : j->ukeys) {
+        b.off[b.n] = c.offsets;
+        b.bytes[b.n] = (const unsigned char*)c.values;
+        b.n++;
+      }
+      launch(ctx, "k_join_utf8_count", k_join_utf8_count, grid_of(ctx, n), JN_THREADS, kc.k, kc.u, j->tag_mask, n, (ProbeRule)j->t,
+             (const unsigned long long*)j->keys, (const unsigned long long*)j->words, (const unsigned*)j->rep, b, (const unsigned long long*)j->start,
+             cnt, bpos);
+    }
     const unsigned long long total = n > 0 ? scan_counts(ctx, cnt, n, off) : 0ull;
     if (total >= (1ull << 32)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "JOIN probe batch producing 2^32 or more output rows");
     const long long m = (long long)total;

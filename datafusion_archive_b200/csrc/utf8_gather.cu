@@ -2,7 +2,7 @@
 // column by a list of selected row numbers.  Replaces the Utf8 arm of `fn filter`
 // (src/execution/filter.rs:93-103: per-row String allocation + BinaryArray::from(Vec<&str>)).
 // The row numbers come out of the fused filter kernel as one more projected column (V_PUSH_ROWID).
-#include "common.cuh"
+#include "utf8_words.cuh"
 
 namespace dfgpu {
 
@@ -89,11 +89,8 @@ __global__ void k_utf8_copy(const unsigned long long* __restrict__ idx, const Ut
 // 64-bit FNV-1a over each string, finalised with a 64-bit mixer: the GROUP BY key of a Utf8 column
 __global__ void k_utf8_hash(const int* __restrict__ off, const unsigned char* __restrict__ bytes, long long n, unsigned long long* __restrict__ out) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    unsigned long long h = 0xcbf29ce484222325ull;
     const int e = off[i + 1];
-    for (int b = off[i]; b < e; b++) { h ^= bytes[b]; h *= 0x100000001b3ull; }
-    h ^= h >> 32; h *= 0xd6e8feb86659fd93ull; h ^= h >> 32;
-    out[i] = h;
+    out[i] = utf8_hash_bytes(bytes, off[i], e);
   }
 }
 
@@ -176,7 +173,7 @@ void gather_utf8_multi(dfgpu_ctx* ctx, const Utf8Source* d_srcs, const unsigned 
     total = scan_utf8_lengths(ctx, out->offsets, nsel);
   }
   out->values_bytes = size_t(total);
-  out->values = ctx->alloc(size_t(total > 0 ? total : 1));
+  out->values = ctx->alloc(std::max<size_t>(16, (size_t(total) + 15) & ~size_t(15)));  // whole 16-byte words
   if (total > 0) {
     const int grid = (int)std::min<long long>((nsel * 32 + 255) / 256, (long long)ctx->sm_count * 16);
     k_utf8_copy<<<grid, 256, 0, ctx->stream>>>(d_idx, d_srcs, nsel, out->offsets, (unsigned char*)out->values);

@@ -11,6 +11,7 @@
 // (dfgpu_batch_upload), so a string that ends at the buffer's end is read safely.  The literal (or LIKE segment) is
 // copied to the device once per call and staged in shared memory by each CTA, zero-padded to whole 16-byte words.
 #include "expr_vm.cuh"
+#include "utf8_words.cuh"
 
 namespace dfgpu {
 
@@ -111,25 +112,6 @@ struct Utf8PredParams {
 
 __device__ __forceinline__ bool valid_bit(const unsigned char* v, long long row) {
   return !v || ((__ldg(v + (row >> 3)) >> (row & 7)) & 1u);
-}
-
-__device__ __forceinline__ unsigned fsr(unsigned lo, unsigned hi, int bits) { return __funnelshift_r(lo, hi, bits); }
-
-// 16 bytes of a string, starting at byte q of a 16-byte aligned buffer, as four little-endian words.  `avail` >= 1 bytes
-// from q belong to the string: the next aligned word is read only when those bytes reach into it.
-__device__ __forceinline__ uint4 load16(const unsigned char* base, long long q, int avail) {
-  const uint4* w = reinterpret_cast<const uint4*>(base + (q & ~15ll));
-  const int sh = int(q & 15);
-  const uint4 lo = __ldg(w);
-  if (sh == 0) return lo;
-  const uint4 hi = sh + min(avail, 16) > 16 ? __ldg(w + 1) : make_uint4(0u, 0u, 0u, 0u);
-  const int b = (sh & 3) * 8;
-  switch (sh >> 2) {
-    case 0: return make_uint4(fsr(lo.x, lo.y, b), fsr(lo.y, lo.z, b), fsr(lo.z, lo.w, b), fsr(lo.w, hi.x, b));
-    case 1: return make_uint4(fsr(lo.y, lo.z, b), fsr(lo.z, lo.w, b), fsr(lo.w, hi.x, b), fsr(hi.x, hi.y, b));
-    case 2: return make_uint4(fsr(lo.z, lo.w, b), fsr(lo.w, hi.x, b), fsr(hi.x, hi.y, b), fsr(hi.y, hi.z, b));
-    default: return make_uint4(fsr(lo.w, hi.x, b), fsr(hi.x, hi.y, b), fsr(hi.y, hi.z, b), fsr(hi.z, hi.w, b));
-  }
 }
 
 // A string in global memory: `len` bytes from byte `start` of `base`

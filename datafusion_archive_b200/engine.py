@@ -347,8 +347,9 @@ class GpuContext:
 
     # -- inner equi-join ---------------------------------------------------------------------------
     def join_build(self, batch, keys, keep_cols=None):
-        """dfgpu_join_build: the hash table over `batch` (the right input) on the integer key expressions `keys`.
-        `keep_cols` (default: every column) are the columns later probes may return; the batch may be freed after."""
+        """dfgpu_join_build: the hash table over `batch` (the right input) on the integer or Utf8 key
+        expressions `keys`.  `keep_cols` (default: every column) are the columns later probes may return; the batch may
+        be freed after."""
         keep = []
         kptrs, klens, nk = A.make_programs([k.program(batch.schema) for k in keys], keep)
         cols = list(range(len(batch.schema))) if keep_cols is None else list(keep_cols)

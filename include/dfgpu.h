@@ -329,7 +329,7 @@ int dfgpu_aggregate_update_host(dfgpu_aggstate* st, const dfgpu_col* cols, int n
 int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out);
 int dfgpu_aggregate_free(dfgpu_aggstate* st);
 
-/* ---- inner equi-join on integer keys ----
+/* ---- inner equi-join on integer and Utf8 keys ----
  * The reference has no join: its planner plans none and its `Relation` trait (src/execution/relation.rs:27-32) has
  * no join relation; "JOIN support (hash join ...)" is the headline of its next milestone (ROADMAP.md, 0.7.0).  These
  * entry points are what a GpuHashJoinRelation implementing that trait calls: build once over the right input, then
@@ -337,18 +337,22 @@ int dfgpu_aggregate_free(dfgpu_aggstate* st);
  *   - A pair (probe row p, build row b) is output when every key is non-null on both sides and the keys are equal.
  *     Null keys never match (SQL join semantics; unlike DFGPU_OP_EQ, under which a null equals a null).
  *   - Output rows keep probe-row order; the order of one probe row's matches is unspecified.
- *   - Keys are postfix programs of any of the 8 integer types, 1 to 4 of them, whose widths sum to at most 64 bits.
- *     They are packed as GROUP BY keys are (the last key in the low bits; a single key keeps its sign- or
- *     zero-extended 64-bit value).  A key program that is not a plain column is evaluated exactly as a projection
- *     (a CAST(UInt32 AS Int32) wraps).  Probe key i must have the type of build key i (DFGPU_ERR_EXECUTION "JOIN key
- *     types differ: Int32 and Int64").  Float, Boolean and Utf8 keys and keys wider than 64 bits are
- *     DFGPU_ERR_NOT_IMPLEMENTED naming the types; a key raising DivideByZero is DFGPU_ERR_ARROW.
+ *   - Keys are postfix programs, 1 to 4 of them, each of any of the 8 integer types or Utf8.  The integer parts'
+ *     widths sum to at most 64 bits (Utf8 parts do not count); they are packed as GROUP BY keys are (the last integer
+ *     part in the low bits; a single one keeps its sign- or zero-extended 64-bit value).  Utf8 parts compare byte for
+ *     byte ('a' is not 'a ', '' equals ''; no collation, trimming or UTF-8 validation), and keys that share a hash
+ *     never match unless equal.  A key program that is not a plain column is evaluated exactly as a projection
+ *     (a CAST(UInt32 AS Int32) wraps; lower(s) and substr(s, 1, 3) are Utf8 keys).  Probe key i must have the type of
+ *     build key i (DFGPU_ERR_EXECUTION "JOIN key types differ: Utf8 and Int64").  Float and Boolean keys and integer
+ *     parts wider than 64 bits are DFGPU_ERR_NOT_IMPLEMENTED naming the types; a key raising DivideByZero is
+ *     DFGPU_ERR_ARROW.
  *   - Output columns keep their dtype and validity: fixed-width, Boolean (bit-packed) and Utf8.
  *   - A build side of 2^32 rows or more, a probe batch of 2^32 rows or more and a probe batch producing 2^32 or more
  *     output rows are DFGPU_ERR_NOT_IMPLEMENTED. */
 typedef struct dfgpu_join dfgpu_join; /* the build side's hash table and its kept columns */
 /* Build the table over `build` (borrowed for the call only).  The join keeps its own device copy of the columns
- * `keep_cols` (build-batch column numbers), so the caller may free the batch afterwards. */
+ * `keep_cols` (build-batch column numbers) and of its Utf8 key columns, so the caller may free the batch afterwards.
+ * DFGPU_JOIN_TAG_BITS (1 to 64, default 64) cuts a Utf8 key's hash tag for tests of the collision handling. */
 int dfgpu_join_build(dfgpu_ctx* ctx, const dfgpu_batch* build, const dfgpu_insn* const* keys, const int* key_len, int nkeys,
                      const int* keep_cols, int n_keep, dfgpu_join** out);
 /* Probe with one batch: the result is the `probe_cols` of `probe` followed by the `build_cols` of the build batch

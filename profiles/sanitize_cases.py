@@ -182,5 +182,29 @@ for k, v in zip(jbk.tolist(), jbv.tolist()):
 assert jr.nrows == sum(jcnt.get(k, 0) for k in jpk.tolist())
 jr.free(); jj.free(); jpb.free()
 print("join ok", flush=True)
+# 11. Inner join on Utf8 keys: k_join_utf8_place's claims, k_join_utf8_verify's byte compare of each row against its
+# slot's representative and its list of rows for the next round, and k_join_utf8_count's confirmation against the
+# join's copy of the build keys (strings at every alignment, a string ending at its buffer's end, a lower() key); then
+# the same under 2-bit tags, where many distinct strings share a tag and the build runs many rounds
+jwords = ["w%d" % i * (1 + i % 7) for i in range(400)] + ["", "x" * 40]
+jus = pa.array([jwords[i] for i in rng.integers(0, len(jwords), 20_000)], mask=rng.random(20_000) < 0.05)
+jup = pa.array([jwords[i].upper() for i in rng.integers(0, len(jwords), 30_000)] + ["X" * 40])
+jcount = {}
+for v in jus.to_pylist():
+    if v is not None:
+        jcount[v] = jcount.get(v, 0) + 1
+for bits in (None, "2"):
+    if bits:
+        os.environ["DFGPU_JOIN_TAG_BITS"] = bits
+    jbb = ctx.upload([jus, np.arange(20_000, dtype=np.int32)])
+    jpb = ctx.upload([jup])
+    jj = ctx.join_build(jbb, [col(0)], keep_cols=[0, 1])
+    jbb.free()
+    jr = jj.probe(jpb, [utf8_fn("lower", col(0))], probe_cols=[0], build_cols=[0, 1])
+    jr.columns()
+    assert jr.nrows == sum(jcount.get(v.lower(), 0) for v in jup.to_pylist())
+    jr.free(); jj.free(); jpb.free()
+    os.environ.pop("DFGPU_JOIN_TAG_BITS", None)
+print("utf8 join ok", flush=True)
 ctx.close()
 print("SANITIZE_CASES_OK")
