@@ -347,7 +347,16 @@ constexpr int AG_FRONT_MAX_GROUPS = 1024;
 // NULLS: like the reference, keys and MIN/MAX/SUM arguments are read ignoring the validity bitmap
 // (`array.value(row)`, aggregate.rs:561-601, 807-852; a null produced by arithmetic reads as the
 // builder's default 0); only COUNT and AVG (extensions, §DESIGN) honour nulls.  A predicate that evaluates to
-// null reads as its value false (filter.rs:86 `filter.value(i)`).
+// null reads as its value false (filter.rs:86 `filter.value(i)`).  Under a WHERE the reference aggregates
+// FilterRelation's output, whose arrays carry no bitmap (filter.rs:83-91): keys and arguments are then
+// evaluated as over null-free arrays (the rule of filter_project.cu), so every surviving row counts.
+template <int DEPTH, int R, bool NULLS, class Rows>
+__device__ __forceinline__ unsigned eval_after_where(const AggParams& p, int prog, const Rows& g,
+                                                     unsigned long long (&v)[R], unsigned& valid) {
+  if (NULLS && !p.has_pred) return eval_program_n<DEPTH, R, false, true>(p.ps, prog, g, v, valid);
+  return eval_program_n<DEPTH, R, false, false>(p.ps, prog, g, v, valid);
+}
+
 template <int DEPTH, bool NULLS>
 struct InterpSrc {
   static constexpr int R = AG_R;
@@ -379,11 +388,11 @@ struct InterpSrc {
   }
   __device__ __forceinline__ void key(const AggParams& p, int k, unsigned long long (&v)[R]) {
     unsigned kv;
-    bad |= eval_program_n<DEPTH, R, false, NULLS>(p.ps, p.has_pred + k, g, v, kv) & mask;
+    bad |= eval_after_where<DEPTH, R, NULLS>(p, p.has_pred + k, g, v, kv) & mask;
   }
   // returns the DivideByZero bits of the rows; av = validity bits of the argument values
   __device__ __forceinline__ unsigned arg(const AggParams& p, int gi, unsigned long long (&v)[R], unsigned& av) {
-    return eval_program_n<DEPTH, R, false, NULLS>(p.ps, p.has_pred + p.nkeys + gi, g, v, av);
+    return eval_after_where<DEPTH, R, NULLS>(p, p.has_pred + p.nkeys + gi, g, v, av);
   }
   __device__ __forceinline__ unsigned rowid(int r) const { return (unsigned)g.rows[r]; }
 };
@@ -912,7 +921,9 @@ constexpr int RD_TILE = AG_THREADS * RD_R;
 
 // NULLS: array_ops::{min,max,sum} skip nulls and report None when nothing was non-null
 // (restated from arrow 0.12; call sites aggregate.rs:347-541): the number of non-null inputs per
-// aggregate is accumulated in counter CTR_NONNULL + a so finish can emit a null.
+// aggregate is accumulated in counter CTR_NONNULL + a so finish can emit a null.  Under a WHERE the
+// arguments are read as over FilterRelation's bitmap-free output (eval_after_where): nothing is skipped and
+// an aggregate is null only when no row passed.
 template <int DEPTH, bool NULLS>
 __global__ void __launch_bounds__(AG_THREADS) k_reduce(const __grid_constant__ AggParams p) {
   __shared__ unsigned long long s_acc[kMaxAggs][AG_THREADS];
@@ -949,7 +960,7 @@ __global__ void __launch_bounds__(AG_THREADS) k_reduce(const __grid_constant__ A
     for (int g = 0; g < p.nargs; g++) {
       unsigned long long v[RD_R];
       unsigned av;
-      const unsigned b = eval_program_n<DEPTH, RD_R, false, NULLS>(p.ps, p.has_pred + g, src, v, av);
+      const unsigned b = eval_after_where<DEPTH, RD_R, NULLS>(p, p.has_pred + g, src, v, av);
       bad = bad || ((b & rmask) != 0);
 #pragma unroll
       for (int a = 0; a < kMaxAggs; a++) {
@@ -960,7 +971,7 @@ __global__ void __launch_bounds__(AG_THREADS) k_reduce(const __grid_constant__ A
         for (int r = 0; r < RD_R; r++)
           if (((rmask >> r) & 1u) && (!NULLS || ((av >> r) & 1u))) acc = acc_fold(func, mt, acc, v[r]);
         s_acc[a][tid] = acc;
-        if (NULLS) nn[a] += __popc(av & rmask);
+        if (NULLS && !p.has_pred) nn[a] += __popc(av & rmask);  // under a WHERE the host counts CTR_PASSED instead
       }
     }
   }
@@ -1383,7 +1394,8 @@ __device__ __forceinline__ int set_insert(const SetView& set, unsigned long long
 
 // Insert the (group key, argument) pairs of a batch into the sets, one set per argument program p.ps[has_pred +
 // nkeys + s].  Runs after the group scan over the same rows: every key it packs (exactly as the scan packs it) is
-// already in the group table.  Rows that fail the WHERE clause and null arguments are skipped.  A row that some set
+// already in the group table.  Rows that fail the WHERE clause are skipped, and so are null arguments when there is
+// no WHERE (under one, InterpSrc reads the arguments as over null-free arrays).  A row that some set
 // refused goes to the overflow list and is replayed into every set after growth (inserting a pair twice is harmless).
 template <class Src, bool NULLS>
 __device__ __forceinline__ void distinct_insert_body(const AggParams& p, const SetParams& sp) {
@@ -2411,7 +2423,7 @@ void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
   unsigned long long c[CTR_NONNULL];
   read_counters(st, c);
   if (c[CTR_ERROR]) fail(DFGPU_ERR_ARROW, "DivideByZero");
-  if (bp.has_pred && !p.ps.has_nulls)  // null-free inputs: every row that passed the predicate is a non-null input
+  if (bp.has_pred)  // the arguments are read as over FilterRelation's null-free output: every row that passed is an input
     for (int a = 0; a < st->naggs; a++) st->nonnull_host[size_t(a)] += (long long)c[CTR_PASSED];
 }
 

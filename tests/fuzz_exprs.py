@@ -3,7 +3,7 @@ compare, boolean operands for And / Or), for GPU-vs-oracle fuzzing."""
 import numpy as np
 
 from datafusion_archive_b200 import _abi as A
-from datafusion_archive_b200.expr import BinaryExpr, col, lit
+from datafusion_archive_b200.expr import AggregateFunction, BinaryExpr, col, lit
 
 MATH = [A.OP_ADD, A.OP_SUB, A.OP_MUL, A.OP_DIV]
 CMP = [A.OP_EQ, A.OP_NE, A.OP_LT, A.OP_LE, A.OP_GT, A.OP_GE]
@@ -53,3 +53,277 @@ def references_column(e):
     if isinstance(e, Cast):
         return references_column(e.expr)
     return False
+
+
+# ---- nullable tables over all ten numeric dtypes and Boolean columns ---------------------------------------------
+# gen_table writes every column with pa.Array.from_buffers over our own buffers and puts deliberate garbage under
+# each null slot (type extremes, NaN, -0.0, infinities; bit 1 under a Boolean null), so that a kernel that reads 0
+# there, skips the row, or reads the hidden value gives a different answer each way.  Integer division is the one
+# operation that can fail: its divisors are plain columns made for it ("safe": zeros only under nulls; "gated": every
+# zero, null or not, in a row where the gate column is 0) or nonzero literals, and never -1, so MIN / -1 cannot occur.
+NUMERIC = [A.INT8, A.INT16, A.INT32, A.INT64, A.UINT8, A.UINT16, A.UINT32, A.UINT64, A.FLOAT32, A.FLOAT64]
+FLOATS = (A.FLOAT32, A.FLOAT64)
+PROFILES = ("bitmap", "nulls", "allnull", "nobitmap")  # null fraction 0 with a bitmap, ~30 %, all null, no bitmap
+
+
+def garbage(dtype):
+    """Values written under null slots (Float32: no subnormal, and sums of them cannot overflow at the test sizes)."""
+    if dtype == A.FLOAT64:
+        return np.array([np.nan, -0.0, np.inf, -np.inf, 1e200, -1e200], dtype=np.float64)
+    if dtype == A.FLOAT32:
+        return np.array([np.nan, -0.0, np.inf, -np.inf, 1e15, -1e15], dtype=np.float32)
+    info = np.iinfo(A.NP_OF[dtype])
+    return np.array(sorted({info.min, info.max, info.max - 1, info.min + 1 if info.min else 7}), dtype=A.NP_OF[dtype])
+
+
+def _values(rng, dtype, n, divisor):
+    """Valid-slot values: small magnitudes with a few type extremes; Float32 clear of subnormals; a divisor column
+    never holds 0 or -1."""
+    npd = A.NP_OF[dtype]
+    if dtype in FLOATS:
+        v = (rng.random(n) * 3.75 + 0.25) * rng.choice([-1.0, 1.0], n)
+        if not divisor:
+            v[rng.random(n) < 0.02] = -0.0
+        return v.astype(npd)
+    info = np.iinfo(npd)
+    lo = max(info.min, -20)
+    v = rng.integers(lo, 21, n, dtype=np.int64).astype(npd)
+    edge = rng.random(n) < 0.01
+    v[edge] = rng.choice(garbage(dtype), int(edge.sum()))
+    if divisor:
+        v[(v == 0) | ((v == -1) if info.min < 0 else False)] = 3
+    return v
+
+
+def column(values, valid):
+    """Arrow array over our buffers; valid=None: no bitmap.  Boolean values are packed LSB first."""
+    import pyarrow as pa
+    n = len(values)
+    bits = None if valid is None else pa.py_buffer(np.packbits(np.asarray(valid, dtype=bool), bitorder="little").tobytes())
+    if values.dtype == np.bool_:
+        return pa.Array.from_buffers(pa.bool_(), n, [bits, pa.py_buffer(np.packbits(values, bitorder="little").tobytes())])
+    return pa.Array.from_buffers(pa.from_numpy_dtype(values.dtype), n, [bits, pa.py_buffer(np.ascontiguousarray(values).tobytes())])
+
+
+def validity(rng, n, profile):
+    if profile == "nobitmap":
+        return None
+    if profile == "bitmap":
+        return np.ones(n, dtype=bool)
+    if profile == "allnull":
+        return np.zeros(n, dtype=bool)
+    return rng.random(n) >= 0.3
+
+
+class Table:
+    """Columns (pyarrow arrays) with their roles.  dtype[i]: the column's dtype code; valid[i]: its validity (None: no
+    bitmap); hidden[i]: its raw values.  gate: an Int32 column of 0 / 1 without nulls; a WHERE of a generated query
+    is `gate > 0 AND ...`, so the rows with gate 0 are the ones every WHERE drops.  safe[d] / gated[d]: the divisor
+    columns of dtype d."""
+
+    def __init__(self):
+        self.arrays, self.dtype, self.valid, self.hidden, self.profile = [], [], [], [], []
+        self.values, self.bools, self.safe, self.gated, self.gate = {}, [], {}, {}, None
+
+    def add(self, values, valid, profile):
+        self.arrays.append(column(values, valid))
+        self.dtype.append(A.BOOL if values.dtype == np.bool_ else A.DTYPE_OF_NP[values.dtype])
+        self.valid.append(valid)
+        self.hidden.append(values)
+        self.profile.append(profile)
+        return len(self.arrays) - 1
+
+
+def gen_table(rng, n, profiles=None, gate_frac=0.8, surviving_zero=False, dtypes=NUMERIC):
+    """A table of n rows: the gate, per dtype a value column, a safe and a gated divisor column, and two Boolean
+    columns.  profiles: a profile for every nullable column (default: random).  surviving_zero: also put zeros under
+    the nulls of the safe divisors in rows that pass the gate (a WHERE evaluates its keys and arguments as over
+    bitmap-free arrays, so such a row must raise DivideByZero)."""
+    pick = (lambda: profiles) if isinstance(profiles, str) else (lambda: PROFILES[int(rng.integers(0, len(PROFILES)))] if profiles is None else profiles)
+    t = Table()
+    gate = (rng.random(n) < gate_frac).astype(np.int32)
+    t.gate = t.add(gate, None, "nobitmap")
+    for d in dtypes:
+        g = garbage(d)
+        for role in ("values", "safe", "gated"):
+            prof = pick()
+            valid = validity(rng, n, prof)
+            v = _values(rng, d, n, role != "values")
+            nulls = np.zeros(n, dtype=bool) if valid is None else ~valid
+            hidden = g[rng.integers(0, len(g), n)]
+            if role != "values":  # a divisor's zeros are placed below, and it never holds -1
+                hidden = np.where((hidden == -1) | (hidden == 0), hidden.dtype.type(7), hidden)
+            v = np.where(nulls, hidden, v).astype(A.NP_OF[d])
+            if role == "safe":
+                zero = nulls & (rng.random(n) < 0.5) & ((gate == 0) | surviving_zero)
+                v[zero] = 0
+            elif role == "gated":
+                zero = (gate == 0) & (rng.random(n) < 0.5)
+                v[zero] = 0
+            i = t.add(v, valid, prof)
+            getattr(t, role)[d] = i
+    for _ in range(2):
+        prof = pick()
+        valid = validity(rng, n, prof)
+        v = rng.random(n) < 0.5
+        if valid is not None:
+            v[~valid] = True  # hidden bit 1 under every null
+        t.bools.append(t.add(v, valid, prof))
+    return t
+
+
+def _cap(e):
+    """(instructions, tree depth) of an expression."""
+    from datafusion_archive_b200.expr import Cast
+    if isinstance(e, BinaryExpr):
+        (a, da), (b, db) = _cap(e.left), _cap(e.right)
+        return a + b + 1, 1 + max(da, db)
+    if isinstance(e, Cast):
+        a, d = _cap(e.expr)
+        return a + 1, d + 1
+    return 1, 0
+
+
+class QueryGen:
+    """Random expressions over a Table, typed as the reference types them (identical operand dtypes, Boolean operands
+    of And / Or), with CAST only where the oracle implements it: a column to Int16 / Int32, an Int64 literal to
+    Float64.  `cols`: the columns a query may read (the engine reads at most 12 distinct columns per query)."""
+
+    def __init__(self, rng, table, cols, max_depth=8):
+        self.rng, self.t, self.max_depth = rng, table, max_depth
+        self.cols = set(cols)
+        self.divisor_role = "safe"
+
+    def _lit(self, d, nonzero=False):
+        r = self.rng
+        if d in FLOATS:
+            return lit(float(r.choice([0.5, 2.0, -3.0, 7.25, 1.5])), d)
+        lo = 0 if d in (A.UINT8, A.UINT16, A.UINT32, A.UINT64) else -5
+        x = int(r.integers(lo, 6))
+        if nonzero and x in (0, -1):
+            x = 3
+        return lit(x, d)
+
+    def _leaf(self, d):
+        r = self.rng
+        if d in (A.INT16, A.INT32) and r.random() < 0.2:  # CAST(column AS Int16 / Int32) from any numeric column
+            src = [c for c in self.cols if self.t.dtype[c] in NUMERIC]
+            if src:
+                return col(int(r.choice(sorted(src)))).cast(d)
+        if d == A.FLOAT64 and r.random() < 0.1:
+            return lit(int(r.integers(-5, 6)), A.INT64).cast(A.FLOAT64)
+        own = [c for c in self.cols if self.t.dtype[c] == d and c != self.t.gate]
+        if own and r.random() < 0.8:
+            return col(int(r.choice(sorted(own))))
+        return self._lit(d)
+
+    def numeric(self, d, depth):
+        r = self.rng
+        if depth <= 0 or r.random() < 0.25:
+            return self._leaf(d)
+        op = int(r.choice(MATH))
+        left = self.numeric(d, depth - 1)
+        if op == A.OP_DIV:
+            role = getattr(self.t, self.divisor_role)
+            if d in role and role[d] in self.cols and r.random() < 0.7:
+                right = col(role[d])
+            else:
+                right = self._lit(d, nonzero=True)
+        elif r.random() < 0.5:  # right-nested subtrees push the evaluator's register stack deep
+            right = self.numeric(d, depth - 1)
+        else:
+            right = self._leaf(d)
+        return BinaryExpr(left, op, right)
+
+    def boolean(self, depth):
+        r = self.rng
+        bools = [c for c in self.cols if self.t.dtype[c] == A.BOOL]
+        if depth <= 0 or r.random() < 0.35:
+            if bools and r.random() < 0.3:
+                return col(int(r.choice(sorted(bools))))
+            ds = sorted({self.t.dtype[c] for c in self.cols if self.t.dtype[c] in NUMERIC})
+            d = int(r.choice(ds))
+            sub = max(0, depth - 1)
+            return BinaryExpr(self.numeric(d, int(r.integers(0, sub + 1))), int(r.choice(CMP)), self.numeric(d, int(r.integers(0, sub + 1))))
+        return BinaryExpr(self.boolean(depth - 1), int(r.choice([A.OP_AND, A.OP_OR])), self.boolean(depth - 1))
+
+    def predicate(self):
+        """`gate > 0 AND <random Boolean>` (the predicate is null-aware: its divisors are the safe columns)."""
+        self.divisor_role = "safe"
+        b = self.boolean(int(self.rng.integers(0, self.max_depth + 1)))
+        return BinaryExpr(col(self.t.gate) > lit(0, A.INT32), A.OP_AND, b)
+
+    def value(self, d, under_where):
+        """A numeric expression of dtype d for a projection or an aggregate argument.  Under a WHERE the gated
+        divisors apply (their zeros sit only in rows the WHERE drops), else the safe ones."""
+        self.divisor_role = "gated" if under_where else "safe"
+        return self.numeric(d, int(self.rng.integers(0, self.max_depth + 1)))
+
+
+def fits(exprs, schema):
+    """Whether a query of these programs fits the engine's program-set limits (96 instructions, 12 columns)."""
+    n, cols = 0, set()
+    for e in exprs:
+        prog = e.program(schema)
+        n += len(prog)
+        cols |= {i.col for i in prog if i.op == A.OP_COL}
+    return n <= 96 and len(cols) <= 12
+
+
+def gen_fp_query(rng, table, ncols=8, with_pred=True):
+    """(pred, projections) for filter / project over a random subset of the table's columns (gate always included):
+    1-3 numeric projections and sometimes a Boolean one.  Retries until the query fits the engine's limits."""
+    schema = table.dtype
+    while True:
+        others = [i for i in range(len(schema)) if i != table.gate]
+        cols = set(rng.choice(others, size=min(ncols, len(others)), replace=False).tolist()) | {table.gate}
+        g = QueryGen(rng, table, cols)
+        pred = g.predicate() if with_pred else None
+        ds = sorted({schema[c] for c in cols if schema[c] in NUMERIC})
+        proj = [g.value(int(rng.choice(ds)), with_pred) for _ in range(int(rng.integers(1, 4)))]
+        if rng.random() < 0.2:
+            g.divisor_role = "safe" if not with_pred else "gated"
+            proj.append(g.boolean(2))
+        if fits(proj + ([pred] if pred is not None else []), schema) and any(references_column(e) for e in proj):
+            return pred, proj
+
+
+def add_keys(rng, t, key_dtypes, n):
+    """Integer key columns with few distinct values, garbage under their nulls (the bytes under a null key are its
+    value), appended to the table; returns their indices."""
+    out = []
+    for d in key_dtypes:
+        prof = PROFILES[int(rng.integers(0, len(PROFILES)))]
+        valid = validity(rng, n, prof)
+        v = rng.integers(0, 6, n).astype(A.NP_OF[d])
+        if valid is not None:
+            g = garbage(d)
+            v = np.where(valid, v, g[rng.integers(0, len(g), n)]).astype(A.NP_OF[d])
+        out.append(t.add(v, valid, prof))
+    return out
+
+
+def gen_agg_query(rng, t, key_cols, with_pred, plain_args, distinct_avg=False):
+    """(pred, keys, aggs): the keys are the key columns or expressions of them; 1-4 of MIN / MAX / SUM / COUNT (and
+    AVG / COUNT(DISTINCT) when asked) over plain columns or random expressions."""
+    while True:
+        others = [i for i in range(len(t.dtype)) if i != t.gate and i not in key_cols and t.dtype[i] != A.BOOL]
+        cols = set(rng.choice(others, size=min(6, len(others)), replace=False).tolist()) | {t.gate} | set(t.bools)
+        g = QueryGen(rng, t, cols, max_depth=8 if not plain_args else 4)
+        pred = g.predicate() if with_pred else None
+        keys = []
+        for k in key_cols:
+            e = col(k)
+            if rng.random() < 0.4:
+                e = e + lit(int(rng.integers(1, 9)), t.dtype[k]) if rng.random() < 0.5 else e * lit(3, t.dtype[k])
+            keys.append(e)
+        funcs = ["min", "max", "sum", "count"] + (["avg", "distinct"] if distinct_avg else [])
+        aggs = []
+        for _ in range(int(rng.integers(1, 5))):
+            c = int(rng.choice(sorted(cols - {t.gate} - set(t.bools))))
+            arg = col(c) if plain_args else g.value(t.dtype[c], with_pred)
+            f = str(rng.choice(funcs))
+            aggs.append(AggregateFunction("count", arg, distinct=True) if f == "distinct" else AggregateFunction(f, arg))
+        exprs = keys + [a.arg for a in aggs] + ([pred] if pred is not None else [])
+        if fits(exprs, t.dtype):
+            return pred, keys, aggs

@@ -20,7 +20,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import oracle_lib as O  # noqa: E402
 from datafusion_archive_b200 import _abi as A, parallel, workloads  # noqa: E402
-from datafusion_archive_b200.expr import AggregateFunction, col  # noqa: E402
+from datafusion_archive_b200.expr import AggregateFunction, col, lit  # noqa: E402
 
 
 def sort_by_key(cols):
@@ -141,6 +141,21 @@ def main():
             assert np.array_equal(gm, em), "validity of aggregate %d differs: %r vs %r" % (j, gm, em)
             if em[0]:
                 assert gv[0] == ev[0] or abs(gv[0] - ev[0]) <= 1e-9 * abs(ev[0]), (j, gv, ev)
+        # the same nullable columns under a fused WHERE that passes rows on rank 0 only: the aggregate sees the
+        # filter's bitmap-free output, so every surviving row counts (values under nulls included) and the merged
+        # scalars are non-null although rank 1 passed nothing
+        w = (np.arange(n) < n // (4 * world)).astype(np.int32)
+        wpred = col(2) > lit(0, A.INT32)
+        wb = ctx.upload([nullable(v[lo:hi], valid_some[lo:hi]), nullable(v[lo:hi], valid_none[lo:hi]), w[lo:hi]])
+        got = ctx.aggregate(wb, [], naggs, pred=wpred).columns()
+        keep = w > 0
+        exp = O.aggregate([v[keep], v[keep]], [], naggs)
+        assert int(unp(got[2])[0][0]) == int(keep.sum()) and int(unp(got[4])[0][0]) == int(keep.sum())
+        for j, (g, e) in enumerate(zip(got, exp)):
+            (gv, gm), (ev, em) = unp(g), unp(e)
+            assert gm[0] and em[0], "aggregate %d under the WHERE is null" % j
+            assert gv[0] == ev[0] or abs(gv[0] - ev[0]) <= 1e-9 * abs(ev[0]), (j, gv, ev)
+        wb.free()
         # every rank must hold bit-identical columns (same rows decoded in the same order)
         import hashlib
         digest = hashlib.sha256(b"".join(np.ascontiguousarray(c).tobytes() for c in merged)).hexdigest()
@@ -155,7 +170,6 @@ def main():
         np.testing.assert_allclose(got0[3], exp0[3], rtol=1e-9)
         assert np.array_equal(got0[4], exp0[4])
         # fused WHERE under the communicator
-        from datafusion_archive_b200.expr import lit
         pred = col(1) < lit(0.5)
         gotp = sort_by_key(ctx.aggregate(b, keys, aggs, pred=pred).columns())
         keep = arrays[1] < 0.5
