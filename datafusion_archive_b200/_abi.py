@@ -58,6 +58,9 @@ UTF8_FN_CODES = {
 
 AGG_MIN, AGG_MAX, AGG_SUM, AGG_COUNT, AGG_COUNT_DISTINCT, AGG_AVG = 1, 2, 3, 4, 5, 6
 
+# dfgpu_join_semi kinds
+JOIN_SEMI, JOIN_ANTI, JOIN_ANTI_NULL_AWARE = 1, 2, 3
+
 
 class Col(C.Structure):
     _fields_ = [

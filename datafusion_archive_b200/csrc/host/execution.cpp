@@ -527,17 +527,6 @@ RecordBatch GpuFilterProjectRelation::process(const RecordBatch& in_batch, const
 // ---- join -------------------------------------------------------------------------------------------------
 namespace {
 
-// the same expression with every column index lowered by `by` (a right-input key over the joined schema -> over the
-// right input's own schema)
-ExprRef shift_columns(const ExprRef& e, size_t by) {
-  auto c = std::make_shared<Expr>(*e);
-  if (c->kind == Expr::Column) c->index -= by;
-  if (c->left) c->left = shift_columns(c->left, by);
-  if (c->right) c->right = shift_columns(c->right, by);
-  for (auto& a : c->args) a = shift_columns(a, by);
-  return c;
-}
-
 void set_bit(std::vector<uint8_t>& bits, int64_t i, bool v) {
   if (v) bits[size_t(i >> 3)] |= uint8_t(1u << (i & 7));
 }
@@ -606,9 +595,10 @@ struct Programs {
 }  // namespace
 
 GpuHashJoinRelation::GpuHashJoinRelation(dfgpu_ctx* gpu, SchemaRef schema, RelationRef left, RelationRef right, std::vector<ExprRef> left_keys,
-                                         std::vector<ExprRef> right_keys, std::vector<size_t> left_cols, std::vector<size_t> right_cols)
+                                         std::vector<ExprRef> right_keys, std::vector<size_t> left_cols, std::vector<size_t> right_cols,
+                                         LogicalPlan::JoinKind kind)
     : gpu_(gpu), schema_(std::move(schema)), left_(std::move(left)), right_(std::move(right)), left_keys_(std::move(left_keys)),
-      right_keys_(std::move(right_keys)), left_cols_(std::move(left_cols)), right_cols_(std::move(right_cols)) {}
+      right_keys_(std::move(right_keys)), left_cols_(std::move(left_cols)), right_cols_(std::move(right_cols)), kind_(kind) {}
 
 GpuHashJoinRelation::~GpuHashJoinRelation() { release(); }
 
@@ -656,8 +646,13 @@ std::optional<RecordBatch> GpuHashJoinRelation::next() {
   std::vector<int> probe_cols;
   for (size_t c : left_cols_) probe_cols.push_back(pr.remap.at(c));
   ResultGuard r;
-  GPU_CHECK(dfgpu_join_probe(join_, b.b, keys.ptr.data(), keys.len.data(), int(keys.ptr.size()), probe_cols.data(), int(probe_cols.size()),
-                             build_out_.data(), int(build_out_.size()), &r.r));
+  if (kind_ == LogicalPlan::JoinKind::Inner) {
+    GPU_CHECK(dfgpu_join_probe(join_, b.b, keys.ptr.data(), keys.len.data(), int(keys.ptr.size()), probe_cols.data(), int(probe_cols.size()),
+                               build_out_.data(), int(build_out_.size()), &r.r));
+  } else {
+    const int kind = kind_ == LogicalPlan::JoinKind::Semi ? DFGPU_JOIN_SEMI : kind_ == LogicalPlan::JoinKind::Anti ? DFGPU_JOIN_ANTI : DFGPU_JOIN_ANTI_NULL_AWARE;
+    GPU_CHECK(dfgpu_join_semi(join_, b.b, keys.ptr.data(), keys.len.data(), int(keys.ptr.size()), kind, probe_cols.data(), int(probe_cols.size()), &r.r));
+  }
   RecordBatch got = download(r.r, schema_);
   RecordBatch out;
   out.schema = schema_;
@@ -672,6 +667,20 @@ std::optional<RecordBatch> GpuHashJoinRelation::next() {
   for (size_t i = 0; i < left_cols_.size(); i++) out.columns[left_cols_[i]] = got.columns[i];
   for (size_t i = 0; i < right_cols_.size(); i++) out.columns[nl + right_cols_[i]] = got.columns[left_cols_.size() + i];
   return out;
+}
+
+const std::vector<RecordBatch>& SharedScan::batches() {
+  if (!drained_) {
+    while (auto b = ds_->next()) batches_.push_back(std::move(*b));
+    drained_ = true;
+  }
+  return batches_;
+}
+
+std::optional<RecordBatch> SharedScanRelation::next() {
+  const auto& all = scan_->batches();
+  if (pos_ >= all.size()) return std::nullopt;
+  return all[pos_++];
 }
 
 GpuAggregateRelation::GpuAggregateRelation(dfgpu_ctx* gpu, SchemaRef schema, RelationRef input, std::vector<ExprRef> group_expr,
@@ -855,7 +864,27 @@ PlanRef ExecutionContext::plan(const std::string& sql) {
 
 RelationRef ExecutionContext::sql(const std::string& sql) { return execute(plan(sql)); }
 
-RelationRef ExecutionContext::execute(const PlanRef& plan) { return execute_node(plan, nullptr, true); }
+namespace {
+void count_scans(const LogicalPlan& p, std::map<std::string, int>& n) {
+  if (p.kind == LogicalPlan::TableScan) n[p.table_name]++;
+  if (p.input) count_scans(*p.input, n);
+  if (p.right) count_scans(*p.right, n);
+}
+}  // namespace
+
+RelationRef ExecutionContext::execute(const PlanRef& plan) {
+  // a table the plan scans more than once is drained once and replayed to each scan; a table scanned once is read as is
+  std::map<std::string, int> scans;
+  count_scans(*plan, scans);
+  shared_.clear();
+  for (auto& [name, n] : scans) {
+    auto it = datasources_->find(name);
+    if (n > 1 && it != datasources_->end()) shared_[name] = std::make_shared<SharedScan>(it->second);
+  }
+  RelationRef r = execute_node(plan, nullptr, true);
+  shared_.clear();
+  return r;
+}
 
 RelationRef ExecutionContext::execute_node(const PlanRef& plan, const std::set<size_t>* needed, bool shard) {
   if (verbose) printf("Logical plan: %s\n", plan->debug().c_str());
@@ -863,13 +892,18 @@ RelationRef ExecutionContext::execute_node(const PlanRef& plan, const std::set<s
     case LogicalPlan::TableScan: {
       auto it = datasources_->find(plan->table_name);
       if (it == datasources_->end()) fail(DFGPU_ERR_GENERAL, "No table registered as '" + plan->table_name + "'");
-      RelationRef scan = std::make_shared<DataSourceRelation>(it->second);
+      auto sh = shared_.find(plan->table_name);
+      RelationRef scan;
+      if (sh != shared_.end()) scan = std::make_shared<SharedScanRelation>(sh->second);
+      else scan = std::make_shared<DataSourceRelation>(it->second);
       if (world_ > 1 && shard) return std::make_shared<ShardRelation>(scan, rank_, world_);  // this rank's row range of every batch
       return scan;
     }
     case LogicalPlan::Join: {
       // Broadcast join across ranks: the probe (left) side keeps the sharding of its leftmost table, the build (right)
-      // side is the whole table on every rank, so every output pair is produced by exactly one rank.
+      // side is the whole table on every rank, so every output pair is produced by exactly one rank.  A semi / anti join
+      // (a subquery: its plan is the build side) decides each probe row on exactly one rank; its schema is the left
+      // schema, so it has no right columns.
       const size_t nl = plan->input->schema()->fields.size(), n = plan->schema()->fields.size();
       std::vector<size_t> lcols, rcols;
       for (size_t c = 0; c < n; c++)
@@ -883,7 +917,7 @@ RelationRef ExecutionContext::execute_node(const PlanRef& plan, const std::set<s
       }
       RelationRef l = execute_node(plan->input, &lneed, shard);
       RelationRef r = execute_node(plan->right, nullptr, false);
-      auto j = std::make_shared<GpuHashJoinRelation>(gpu_, plan->schema(), l, r, lkeys, rkeys, lcols, rcols);
+      auto j = std::make_shared<GpuHashJoinRelation>(gpu_, plan->schema(), l, r, lkeys, rkeys, lcols, rcols, plan->join_kind);
       joins_.push_back(j);
       return j;
     }

@@ -140,6 +140,8 @@ class GpuAggregateRelation : public Relation {
 // (right) relation, concatenates its batches on the host and builds the GPU hash table (dfgpu_join_build); then each
 // batch of the probe (left) relation gives one output batch (dfgpu_join_probe).  `left_keys` are over the left schema,
 // `right_keys` over the right schema.
+// A semi / anti join (`kind`) keeps the probe rows that pass (dfgpu_join_semi): its schema is the left schema, and
+// `right_cols` is empty.
 // Output batches have the joined schema's column positions, but only the columns in `left_cols` / `right_cols` (the ones
 // the plan above references) are materialised: every other column is an empty placeholder (its dtype and length, no
 // buffers), which no relation above reads.  So no unreferenced column is ever gathered or copied.
@@ -149,7 +151,8 @@ class GpuAggregateRelation : public Relation {
 class GpuHashJoinRelation : public Relation {
  public:
   GpuHashJoinRelation(dfgpu_ctx* gpu, SchemaRef schema, RelationRef left, RelationRef right, std::vector<ExprRef> left_keys,
-                      std::vector<ExprRef> right_keys, std::vector<size_t> left_cols, std::vector<size_t> right_cols);
+                      std::vector<ExprRef> right_keys, std::vector<size_t> left_cols, std::vector<size_t> right_cols,
+                      LogicalPlan::JoinKind kind = LogicalPlan::JoinKind::Inner);
   ~GpuHashJoinRelation() override;
   std::optional<RecordBatch> next() override;
   const SchemaRef& schema() const override { return schema_; }
@@ -161,9 +164,34 @@ class GpuHashJoinRelation : public Relation {
   RelationRef left_, right_;
   std::vector<ExprRef> left_keys_, right_keys_;
   std::vector<size_t> left_cols_, right_cols_;
+  LogicalPlan::JoinKind kind_;
   dfgpu_join* join_ = nullptr;
   bool released_ = false;
   std::vector<int> build_out_;  // right_cols_ as columns of the uploaded build batch
+};
+
+// The batches of one DataSource, drained on first use and replayed to each scan of a query that reads the table more
+// than once (a self-join, a subquery over an outer table): a DataSource is one-pass.
+class SharedScan {
+ public:
+  explicit SharedScan(DataSourceRef ds) : ds_(std::move(ds)) {}
+  const SchemaRef& schema() const { return ds_->schema(); }
+  const std::vector<RecordBatch>& batches();
+ private:
+  DataSourceRef ds_;
+  std::vector<RecordBatch> batches_;
+  bool drained_ = false;
+};
+
+// One scan of a SharedScan, with its own cursor
+class SharedScanRelation : public Relation {
+ public:
+  explicit SharedScanRelation(std::shared_ptr<SharedScan> scan) : scan_(std::move(scan)) {}
+  std::optional<RecordBatch> next() override;
+  const SchemaRef& schema() const override { return scan_->schema(); }
+ private:
+  std::shared_ptr<SharedScan> scan_;
+  size_t pos_ = 0;
 };
 
 class ExecutionContext {
@@ -190,6 +218,7 @@ class ExecutionContext {
   RelationRef execute_node(const PlanRef& plan, const std::set<size_t>* needed, bool shard);
   std::shared_ptr<std::map<std::string, DataSourceRef>> datasources_;
   std::vector<std::weak_ptr<GpuHashJoinRelation>> joins_;  // released before gpu_ is shut down
+  std::map<std::string, std::shared_ptr<SharedScan>> shared_;  // the tables the query being executed scans more than once
   dfgpu_ctx* gpu_ = nullptr;
   int rank_ = 0, world_ = 1;
 };

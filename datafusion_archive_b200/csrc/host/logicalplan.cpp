@@ -217,6 +217,15 @@ void collect_columns(const Expr& e, std::set<size_t>& acc) {
   }
 }
 
+ExprRef shift_columns(const ExprRef& e, size_t by) {
+  auto c = std::make_shared<Expr>(*e);
+  if (c->kind == Expr::Column) c->index -= by;
+  if (c->left) c->left = shift_columns(c->left, by);
+  if (c->right) c->right = shift_columns(c->right, by);
+  for (auto& a : c->args) a = shift_columns(a, by);
+  return c;
+}
+
 // ---- LogicalPlan -------------------------------------------------------------------------------------
 const SchemaRef& LogicalPlan::schema() const {
   if (kind == Selection) return input->schema();
@@ -270,7 +279,11 @@ static void fmt_with_indent(const LogicalPlan& p, std::string& f, int indent) {
       fmt_with_indent(*p.input, f, indent + 1);
       break;
     case LogicalPlan::Join:
-      f += "Join: on=[";
+      f += p.join_kind == LogicalPlan::JoinKind::Inner ? "Join"
+           : p.join_kind == LogicalPlan::JoinKind::Semi ? "SemiJoin"
+           : p.join_kind == LogicalPlan::JoinKind::Anti ? "AntiJoin"
+                                                        : "AntiJoin (null-aware)";
+      f += ": on=[";
       for (size_t i = 0; i < p.on_keys.size(); i++)
         f += (i ? ", " : "") + p.on_keys[i].first->debug() + " Eq " + p.on_keys[i].second->debug();
       f += "]";

@@ -90,9 +90,14 @@ struct LogicalPlan;
 using PlanRef = std::shared_ptr<const LogicalPlan>;
 struct LogicalPlan {
   // Join (no reference counterpart: ROADMAP.md 0.7.0): inner equi-join of `input` (left, probe side) and `right` (build
-  // side, always one TableScan) on on_keys (left expr, right expr), both over the joined schema = left fields ++ right
+  // side, one TableScan) on on_keys (left expr, right expr), both over the joined schema = left fields ++ right
   // fields.  Chains are left-deep.
+  // A semi / anti join (join_kind) keeps the rows of `input` that have a match in `right` (Semi), that have none (Anti),
+  // or that have none under NOT IN's three-valued logic (AntiNullAware, one key); its schema is `input`'s, and `right`
+  // is a Projection whose columns are the build keys.  The right keys of on_keys are numbered over the left fields
+  // followed by `right`'s, as for an inner join.
   enum Kind { Limit, Projection, Selection, Aggregate, Sort, TableScan, EmptyRelation, Join } kind = EmptyRelation;
+  enum class JoinKind { Inner, Semi, Anti, AntiNullAware } join_kind = JoinKind::Inner;  // Join
   size_t limit = 0;
   std::vector<ExprRef> expr;        // Projection / Sort exprs; Selection: expr[0]
   std::vector<ExprRef> group_expr;  // Aggregate
@@ -111,6 +116,9 @@ struct LogicalPlan {
 
 // The column indices an expression reads (collect_expr, sqlplanner.rs:435-458), added to `acc`.
 void collect_columns(const Expr& e, std::set<size_t>& acc);
+
+// The same expression with every column index lowered by `by` (a key over a joined schema -> over its right input).
+ExprRef shift_columns(const ExprRef& e, size_t by);
 
 // ---- type coercion lattice -------------------------------------------------------------------------
 bool get_supertype(DataType l, DataType r, DataType* out);  // logicalplan.rs:446-554

@@ -95,7 +95,7 @@ struct Parser {
       if (u == "AND") return 10;
       if (u == "NOT") return 15;
       if (u == "IS") return 17;
-      if (u == "LIKE") return 20;
+      if (u == "LIKE" || u == "IN") return 20;
       return 0;
     }
     if (t.kind == Token::Sym) {
@@ -172,6 +172,15 @@ struct Parser {
       case Token::Ident: {
         std::string u = upper(t.text);
         if (u == "SELECT") { pos--; return parse_select(); }
+        // EXISTS (SELECT ..) and NOT EXISTS (SELECT ..); EXISTS followed by anything else is an identifier or function
+        const bool not_exists = u == "NOT" && is_kw("EXISTS") && subquery_at(pos + 1);
+        if (not_exists || (u == "EXISTS" && subquery_at(pos))) {
+          if (not_exists) pos++;
+          n->kind = ASTNode::SQLExists;
+          n->negated = not_exists;
+          n->subquery = parse_subquery();
+          return n;
+        }
         if (u == "CAST") {
           expect_sym("(");
           n->kind = ASTNode::SQLCast;
@@ -223,12 +232,29 @@ struct Parser {
         n->left = left;
         return n;
       }
+      const bool not_in = u == "NOT" && is_kw("IN");
+      if (u == "IN" || not_in) {  // x [NOT] IN (SELECT ..)
+        if (not_in) pos++;
+        if (!subquery_at(pos)) {
+          if (peek().kind == Token::Sym && peek().text == "(")
+            fail(DFGPU_ERR_NOT_IMPLEMENTED, "IN over a list of values is not supported: only IN (SELECT ..)");
+          perr("Expected ( after IN, found: " + peek().text);
+        }
+        n->kind = ASTNode::SQLInSubquery;
+        n->left = left;
+        n->negated = not_in;
+        n->subquery = parse_subquery();
+        return n;
+      }
       n->kind = ASTNode::SQLBinaryExpr;
       n->left = left;
       if (u == "AND") n->op = SQLOperator::And;
       else if (u == "OR") n->op = SQLOperator::Or;
       else if (u == "LIKE") n->op = SQLOperator::Like;
-      else if (u == "NOT") { expect_kw("LIKE"); n->op = SQLOperator::NotLike; }
+      else if (u == "NOT") {
+        if (!accept_kw("LIKE")) perr("Expected LIKE or IN after NOT, found: " + peek().text);
+        n->op = SQLOperator::NotLike;
+      }
       else perr("No infix parser for token " + t.text);
       n->right = parse_expr(precedence);
       return n;
@@ -250,6 +276,18 @@ struct Parser {
     else perr("No infix parser for token " + s);
     n->right = parse_expr(precedence);
     return n;
+  }
+
+  // tokens i, i + 1 are `(` SELECT
+  bool subquery_at(size_t i) const {
+    return i + 1 < toks.size() && toks[i].kind == Token::Sym && toks[i].text == "(" && toks[i + 1].kind == Token::Ident &&
+           upper(toks[i + 1].text) == "SELECT";
+  }
+  ASTRef parse_subquery() {
+    expect_sym("(");
+    ASTRef q = parse_select();
+    expect_sym(")");
+    return q;
   }
 
   // name [ [AS] alias ]
@@ -323,6 +361,8 @@ std::string ASTNode::debug() const {
     case SQLIsNotNull: return "SQLIsNotNull(..)";
     case SQLFunction: return "SQLFunction { id: \"" + id + "\", .. }";
     case SQLSelect: return "SQLSelect { .. }";
+    case SQLInSubquery: return negated ? "SQLInSubquery { negated: true, .. }" : "SQLInSubquery { .. }";
+    case SQLExists: return negated ? "SQLExists { negated: true, .. }" : "SQLExists { .. }";
   }
   return "?";
 }

@@ -6,6 +6,8 @@
 //   from      := table_ref { [INNER] JOIN table_ref ON expr }
 //   table_ref := name [ [AS] alias ]
 //   column    := name | qualifier '.' name        -- qualifier = the alias if given, else the table name
+// and WHERE takes subqueries (planned as semi / anti joins, only as top-level AND terms):
+//   expr [NOT] IN ( select )  |  [NOT] EXISTS ( select )
 #pragma once
 #include <memory>
 #include <string>
@@ -22,7 +24,8 @@ struct OrderByExpr { ASTRef expr; bool asc = true; };
 struct JoinClause { ASTRef relation; ASTRef on; };  // INNER JOIN relation ON on
 
 struct ASTNode {
-  enum Kind { SQLIdentifier, SQLWildcard, SQLLong, SQLDouble, SQLString, SQLBinaryExpr, SQLCast, SQLIsNull, SQLIsNotNull, SQLFunction, SQLSelect } kind = SQLIdentifier;
+  enum Kind { SQLIdentifier, SQLWildcard, SQLLong, SQLDouble, SQLString, SQLBinaryExpr, SQLCast, SQLIsNull, SQLIsNotNull, SQLFunction, SQLSelect,
+              SQLInSubquery, SQLExists } kind = SQLIdentifier;
   std::string id;       // identifier / function name / string literal / unknown type name
   std::string qualifier;  // SQLIdentifier: `q` of a column `q.c`; of a table after FROM / JOIN: its alias, or empty
   long long lval = 0;   // SQLLong
@@ -32,6 +35,9 @@ struct ASTNode {
   SQLType sql_type = SQLType::Other;
   std::vector<ASTRef> args;
   bool distinct = false;  // SQLFunction: COUNT(DISTINCT expr)
+  // SQLInSubquery: `left` [NOT] IN (`subquery`); SQLExists: [NOT] EXISTS (`subquery`)
+  ASTRef subquery;
+  bool negated = false;
   // SQLSelect
   std::vector<ASTRef> projection;
   ASTRef relation, selection, having, limit;

@@ -63,16 +63,14 @@ PlanRef SqlToRel::sql_to_rel(const ASTRef& sql) const {
         e->schema_ = std::make_shared<Schema>();
         input = e;
       }
-      const SchemaRef& input_schema = input->schema();
+      const SchemaRef input_schema = input->schema();  // semi / anti joins of the WHERE clause keep it
 
       // selection first
       PlanRef selection_plan;
-      if (sql->selection || residual) {  // the join residual first, then the WHERE clause
+      ExprRef where = sql->selection ? plan_where(sql->selection, *input_schema, &input) : nullptr;
+      if (where || residual) {  // the join residual first, then the WHERE clause
         ExprRef pred = residual;
-        if (sql->selection) {
-          ExprRef where = sql_to_rex(sql->selection, *input_schema);
-          pred = pred ? Expr::binary(pred, Operator::And, where) : where;
-        }
+        if (where) pred = pred ? Expr::binary(pred, Operator::And, where) : where;
         auto s = std::make_shared<LogicalPlan>();
         s->kind = LogicalPlan::Selection;
         s->expr.push_back(pred);
@@ -163,6 +161,25 @@ int side_of(const Expr& e, size_t split) {
   for (size_t c : cols) (c < split ? l : r) = true;
   return l && r ? 0 : (l ? 1 : 2);
 }
+void ast_and_terms(const ASTRef& e, std::vector<ASTRef>& out) {
+  if (e->kind == ASTNode::SQLBinaryExpr && e->op == SQLOperator::And) {
+    ast_and_terms(e->left, out);
+    ast_and_terms(e->right, out);
+  } else {
+    out.push_back(e);
+  }
+}
+bool is_subquery_term(const ASTNode& e) { return e.kind == ASTNode::SQLInSubquery || e.kind == ASTNode::SQLExists; }
+bool contains_aggregate(const ASTRef& e) {
+  if (!e) return false;
+  if (e->kind == ASTNode::SQLFunction) {
+    const std::string l = lower(e->id);
+    if (l == "min" || l == "max" || l == "sum" || l == "avg" || l == "count") return true;
+  }
+  for (auto& a : e->args)
+    if (contains_aggregate(a)) return true;
+  return contains_aggregate(e->left) || contains_aggregate(e->right);
+}
 void and_terms(const ExprRef& e, std::vector<ExprRef>& out) {
   if (e->kind == Expr::BinaryExpr && e->op == Operator::And) {
     and_terms(e->left, out);
@@ -212,31 +229,161 @@ PlanRef SqlToRel::plan_from(const ASTNode& select, ExprRef* residual) const {
   return plan;
 }
 
-ExprRef SqlToRel::sql_to_rex(const ASTRef& sql, const Schema& schema) const {
+// The WHERE clause of a SELECT over *input: each top-level AND term that is an IN / EXISTS subquery becomes a semi or
+// anti join above *input, in order; the other terms are returned AND-ed, in order (null if there are none).
+ExprRef SqlToRel::plan_where(const ASTRef& where, const Schema& schema, PlanRef* input) const {
+  std::vector<ASTRef> terms;
+  ast_and_terms(where, terms);
+  if (std::none_of(terms.begin(), terms.end(), [](const ASTRef& t) { return is_subquery_term(*t); })) return sql_to_rex(where, schema);
+  ExprRef pred;
+  for (auto& t : terms) {
+    if (is_subquery_term(*t)) {
+      *input = plan_subquery(*t, *input, {});
+      continue;
+    }
+    ExprRef e = sql_to_rex(t, schema);
+    pred = pred ? Expr::binary(pred, Operator::And, e) : e;
+  }
+  return pred;
+}
+
+// `term` ([NOT] IN / [NOT] EXISTS) as a semi / anti join of `left` (the query's FROM plan) and the subquery.  The probe
+// keys are the IN operand and the outer side of each correlated equality, the build keys the subquery's column and the
+// inner sides; the subquery's other WHERE terms (over its own columns) and its ON residual are the build side's
+// Selection, under the Projection of the build keys.
+PlanRef SqlToRel::plan_subquery(const ASTNode& term, PlanRef left, const std::vector<SchemaRef>& far) const {
+  const ASTNode& q = *term.subquery;
+  const bool in = term.kind == ASTNode::SQLInSubquery;
+  const std::string form = std::string(term.negated ? "NOT " : "") + (in ? "IN" : "EXISTS");
+  if (q.has_group_by || q.having || q.has_order_by || q.limit)
+    fail(DFGPU_ERR_NOT_IMPLEMENTED, "GROUP BY, HAVING, ORDER BY and LIMIT are not supported in an " + form + " subquery");
+  for (auto& e : q.projection)
+    if (contains_aggregate(e)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "aggregates are not supported in an " + form + " subquery");
+  if (!q.relation) fail(DFGPU_ERR_NOT_IMPLEMENTED, "an " + form + " subquery needs a FROM clause");
+  if (in && q.projection.size() != 1) fail(DFGPU_ERR_GENERAL, "IN subquery must return exactly one column");
+  ExprRef pred;
+  PlanRef sub = plan_from(q, &pred);
+  const SchemaRef sub_schema = sub->schema(), outer_schema = left->schema();
+  const size_t ns = sub_schema->fields.size(), nl = outer_schema->fields.size();
+  Schema both = *sub_schema;  // the subquery's fields, then the outer query's
+  for (auto& f : outer_schema->fields) both.fields.push_back(f);
+  const Scope scope{ns, far};
+  std::vector<ExprRef> probe, build;
+  if (in) {
+    const Scope outer_scope{nl, far};
+    ExprRef x = rex(term.left, *outer_schema, &outer_scope);
+    ExprRef y = rex(q.projection[0], both, &scope);
+    std::set<size_t> ycols;
+    collect_columns(*y, ycols);
+    if (!ycols.empty() && *ycols.rbegin() >= ns) fail(DFGPU_ERR_NOT_IMPLEMENTED, "the column of an IN subquery must be over the subquery's own tables");
+    const DataType xt = x->get_type(*outer_schema), yt = y->get_type(*sub_schema);
+    DataType st;
+    if (!get_supertype(xt, yt, &st))
+      fail(DFGPU_ERR_GENERAL, std::string("No common supertype found for binary operator Eq with input types ") + datatype_debug(xt) + " and " +
+                                  datatype_debug(yt));
+    probe.push_back(x->cast_to(st, *outer_schema));
+    build.push_back(y->cast_to(st, *sub_schema));
+  }
+  if (q.selection) {
+    std::vector<SchemaRef> far_in{outer_schema};  // a nested subquery's far scopes
+    far_in.insert(far_in.end(), far.begin(), far.end());
+    std::vector<ASTRef> terms;
+    ast_and_terms(q.selection, terms);
+    for (auto& t : terms) {
+      if (is_subquery_term(*t)) {
+        sub = plan_subquery(*t, sub, far_in);
+        continue;
+      }
+      ExprRef e = rex(t, both, &scope);
+      std::set<size_t> cols;
+      collect_columns(*e, cols);
+      if (cols.empty() || *cols.rbegin() < ns) {  // over the subquery's columns only
+        pred = pred ? Expr::binary(pred, Operator::And, e) : e;
+        continue;
+      }
+      if (*cols.begin() >= ns) fail(DFGPU_ERR_NOT_IMPLEMENTED, "a subquery WHERE term over outer columns only is not supported");
+      if (e->kind == Expr::BinaryExpr && e->op == Operator::Eq) {
+        const int l = side_of(*e->left, ns), r = side_of(*e->right, ns);
+        if (l == 1 && r == 2) {
+          build.push_back(e->left);
+          probe.push_back(shift_columns(e->right, ns));
+          continue;
+        }
+        if (l == 2 && r == 1) {
+          build.push_back(e->right);
+          probe.push_back(shift_columns(e->left, ns));
+          continue;
+        }
+      }
+      fail(DFGPU_ERR_NOT_IMPLEMENTED, "a correlated subquery term must be an equality between an inner and an outer expression");
+    }
+  }
+  if (in && term.negated && probe.size() > 1) fail(DFGPU_ERR_NOT_IMPLEMENTED, "correlated NOT IN subqueries are not supported");
+  if (!in && probe.empty()) fail(DFGPU_ERR_NOT_IMPLEMENTED, form + " subquery without a correlated equality is not supported");
+  if (pred) {
+    auto s = std::make_shared<LogicalPlan>();
+    s->kind = LogicalPlan::Selection;
+    s->expr.push_back(pred);
+    s->input = sub;
+    sub = s;
+  }
+  auto proj = std::make_shared<LogicalPlan>();
+  proj->kind = LogicalPlan::Projection;
+  proj->expr = build;
+  proj->input = sub;
+  proj->schema_ = std::make_shared<Schema>();
+  proj->schema_->fields = exprlist_to_fields(build, *sub_schema);
+  auto j = std::make_shared<LogicalPlan>();
+  j->kind = LogicalPlan::Join;
+  j->join_kind = !term.negated ? LogicalPlan::JoinKind::Semi : in ? LogicalPlan::JoinKind::AntiNullAware : LogicalPlan::JoinKind::Anti;
+  j->input = left;
+  j->right = proj;
+  j->schema_ = outer_schema;
+  for (size_t i = 0; i < probe.size(); i++) j->on_keys.emplace_back(probe[i], Expr::column(nl + i));
+  return j;
+}
+
+ExprRef SqlToRel::sql_to_rex(const ASTRef& sql, const Schema& schema) const { return rex(sql, schema, nullptr); }
+
+ExprRef SqlToRel::rex(const ASTRef& sql, const Schema& schema, const Scope* scope) const {
   switch (sql->kind) {
     case ASTNode::SQLLong: return Expr::literal(ScalarValue::Int64(sql->lval));
     case ASTNode::SQLDouble: return Expr::literal(ScalarValue::Float64(sql->dval));
     case ASTNode::SQLString: return Expr::literal(ScalarValue::Utf8(sql->id));
     case ASTNode::SQLIdentifier: {
       // `q.c`: the field of that table (or alias) and name.  `c`: the first field of that name, unless fields of that
-      // name come from more than one table.
-      long long found = -1;
-      for (size_t i = 0; i < schema.fields.size(); i++) {
-        const Field& f = schema.fields[i];
-        if (f.name != sql->id || (!sql->qualifier.empty() && f.qualifier != sql->qualifier)) continue;
-        if (found < 0) found = (long long)i;
-        else if (schema.fields[size_t(found)].qualifier != f.qualifier)
-          fail(DFGPU_ERR_GENERAL, "Ambiguous reference to column '" + sql->id + "'");
-      }
+      // name come from more than one table.  In a subquery the fields of its own tables are searched first.
+      auto find = [&](const Schema& sch, size_t lo, size_t hi) {
+        long long found = -1;
+        for (size_t i = lo; i < hi; i++) {
+          const Field& f = sch.fields[i];
+          if (f.name != sql->id || (!sql->qualifier.empty() && f.qualifier != sql->qualifier)) continue;
+          if (found < 0) found = (long long)i;
+          else if (sch.fields[size_t(found)].qualifier != f.qualifier)
+            fail(DFGPU_ERR_GENERAL, "Ambiguous reference to column '" + sql->id + "'");
+        }
+        return found;
+      };
+      const size_t n = schema.fields.size(), inner = scope ? std::min(scope->inner, n) : n;
+      long long found = find(schema, 0, inner);
+      if (found < 0 && inner < n) found = find(schema, inner, n);
       if (found >= 0) return Expr::column(size_t(found));
+      if (scope)
+        for (auto& s : scope->far)
+          if (find(*s, 0, s->fields.size()) >= 0)
+            fail(DFGPU_ERR_NOT_IMPLEMENTED, "a subquery may only reference the query just outside it, not '" + sql->id +
+                                                "' of a query further out (correlation that skips a level)");
       fail(DFGPU_ERR_EXECUTION, "Invalid identifier '" + (sql->qualifier.empty() ? "" : sql->qualifier + ".") + sql->id + "' for schema " +
                                     schema.to_string());
     }
+    case ASTNode::SQLInSubquery:
+    case ASTNode::SQLExists:
+      fail(DFGPU_ERR_NOT_IMPLEMENTED, "IN / EXISTS subqueries are supported only as AND terms of WHERE");
     case ASTNode::SQLWildcard:
       fail(DFGPU_ERR_NOT_IMPLEMENTED, "SQL wildcard operator is not supported in projection - please use explicit column names");
-    case ASTNode::SQLCast: return Expr::cast(sql_to_rex(sql->left, schema), convert_data_type(*sql));
-    case ASTNode::SQLIsNull: return Expr::is_null(sql_to_rex(sql->left, schema), false);
-    case ASTNode::SQLIsNotNull: return Expr::is_null(sql_to_rex(sql->left, schema), true);
+    case ASTNode::SQLCast: return Expr::cast(rex(sql->left, schema, scope), convert_data_type(*sql));
+    case ASTNode::SQLIsNull: return Expr::is_null(rex(sql->left, schema, scope), false);
+    case ASTNode::SQLIsNotNull: return Expr::is_null(rex(sql->left, schema, scope), true);
     case ASTNode::SQLBinaryExpr: {
       Operator op;
       switch (sql->op) {
@@ -257,7 +404,7 @@ ExprRef SqlToRel::sql_to_rex(const ASTRef& sql, const Schema& schema) const {
         case SQLOperator::Like: op = Operator::Like; break;
         default: op = Operator::NotLike; break;
       }
-      ExprRef left_expr = sql_to_rex(sql->left, schema), right_expr = sql_to_rex(sql->right, schema);
+      ExprRef left_expr = rex(sql->left, schema, scope), right_expr = rex(sql->right, schema, scope);
       DataType lt = left_expr->get_type(schema), rt = right_expr->get_type(schema), st;
       if (!get_supertype(lt, rt, &st))
         fail(DFGPU_ERR_GENERAL, std::string("No common supertype found for binary operator ") + operator_debug(op) + " with input types " +
@@ -268,7 +415,7 @@ ExprRef SqlToRel::sql_to_rex(const ASTRef& sql, const Schema& schema) const {
       const std::string lid = lower(sql->id);
       if (lid == "min" || lid == "max" || lid == "sum" || lid == "avg") {
         std::vector<ExprRef> rex_args;
-        for (auto& a : sql->args) rex_args.push_back(sql_to_rex(a, schema));
+        for (auto& a : sql->args) rex_args.push_back(rex(a, schema, scope));
         if (rex_args.empty()) fail(DFGPU_ERR_INTERNAL, "aggregate function without arguments (reference: index panic at sqlplanner.rs:320)");
         // return type is same as the argument type for MIN / MAX / SUM; AVG is Float64 (the reference types it as
         // its argument too, but never executes it)
@@ -277,7 +424,7 @@ ExprRef SqlToRel::sql_to_rex(const ASTRef& sql, const Schema& schema) const {
       }
       if (lid == "count" && sql->distinct) {
         std::vector<ExprRef> rex_args;
-        for (auto& a : sql->args) rex_args.push_back(sql_to_rex(a, schema));
+        for (auto& a : sql->args) rex_args.push_back(rex(a, schema, scope));
         if (rex_args.size() != 1) fail(DFGPU_ERR_GENERAL, "COUNT(DISTINCT) takes exactly one argument");
         return Expr::aggregate(sql->id, rex_args, DFGPU_UINT64, true);
       }
@@ -286,7 +433,7 @@ ExprRef SqlToRel::sql_to_rex(const ASTRef& sql, const Schema& schema) const {
         for (auto& a : sql->args) {
           // COUNT(1) / COUNT(*) -> COUNT(first_column)
           if ((a->kind == ASTNode::SQLLong && a->lval == 1) || a->kind == ASTNode::SQLWildcard) rex_args.push_back(Expr::column(0));
-          else rex_args.push_back(sql_to_rex(a, schema));
+          else rex_args.push_back(rex(a, schema, scope));
         }
         return Expr::aggregate(sql->id, rex_args, DFGPU_UINT64);
       }
@@ -294,7 +441,7 @@ ExprRef SqlToRel::sql_to_rex(const ASTRef& sql, const Schema& schema) const {
       if (!fm) fail(DFGPU_ERR_GENERAL, "Invalid function '" + sql->id + "'");
       std::vector<ExprRef> safe_args;
       for (size_t i = 0; i < sql->args.size(); i++) {
-        ExprRef a = sql_to_rex(sql->args[i], schema);
+        ExprRef a = rex(sql->args[i], schema, scope);
         if (i >= fm->args.size()) fail(DFGPU_ERR_INTERNAL, "too many function arguments (reference: index panic at sqlplanner.rs:356)");
         safe_args.push_back(a->cast_to(fm->args[i].data_type, schema));
       }

@@ -26,6 +26,16 @@ class SqlToRel {
   ExprRef sql_to_rex(const ASTRef& sql, const Schema& schema) const;  // sqlplanner.rs:212-375
  private:
   PlanRef plan_from(const ASTNode& select, ExprRef* residual) const;  // FROM with joins (no reference counterpart)
+  // IN / EXISTS subqueries (no reference counterpart).  A subquery's expressions are planned over its own fields
+  // followed by the fields of the query just outside it: `inner` is the number of its own, and a name resolves in the
+  // innermost scope that has it.  `far` are the schemas of the queries further out, which it may not reference.
+  struct Scope {
+    size_t inner;
+    std::vector<SchemaRef> far;
+  };
+  ExprRef rex(const ASTRef& sql, const Schema& schema, const Scope* scope) const;
+  ExprRef plan_where(const ASTRef& where, const Schema& schema, PlanRef* input) const;
+  PlanRef plan_subquery(const ASTNode& term, PlanRef left, const std::vector<SchemaRef>& far) const;
   std::shared_ptr<SchemaProvider> schema_provider_;
 };
 

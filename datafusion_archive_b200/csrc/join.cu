@@ -17,6 +17,13 @@
 //   gathers         k_join_gather<T> (1, 2, 4, 8 bytes), k_join_gather_bits (validity and Boolean values), and
 //                   gather_utf8 (utf8_gather.cu) for Utf8 columns
 //
+// Semi / anti join (dfgpu_join_semi), on the same build:
+//   k_join_mark     per probe row: one pass bit (match for semi, no match for anti), written as 32-bit words with
+//                   __ballot_sync, and each tile's pass count (k_join_utf8_mark for a key with Utf8 parts)
+//   scan            the tile counts become each tile's output offset; the total is the output row count
+//   k_join_select   per tile: the passing row numbers in row order (a prefix over the mask words' popcounts)
+//   gathers         as above, for the probe columns only
+//
 // A key with Utf8 parts takes its own build and count kernels; the scan, k_join_scatter, k_join_emit and the gathers
 // are shared.  Each row has a 64-bit tag (the packed integer parts and the hash of each Utf8 part), and a slot holds
 // one distinct KEY, not one tag: its tag, its integer word and a representative build row, the smallest with the key.
@@ -309,6 +316,23 @@ __global__ void __launch_bounds__(JN_THREADS) k_scan_add(unsigned long long* __r
 }
 
 // ---- probe -----------------------------------------------------------------------------------------------------------
+// The slot of a packed integer key: slot cap for the key equal to EMPTY_KEY, -1 when the key is not in the table.
+__device__ __forceinline__ long long find_slot(const ProbeRule& t, const unsigned long long* __restrict__ keys, unsigned long long key) {
+  long long s = -1;
+  if (key == EMPTY_KEY) {
+    s = t.cap;
+  } else {
+    unsigned long long h = t.home(mix64(key));
+    for (long long probes = 0; probes < t.cap; probes++) {
+      const unsigned long long cur = keys[h];
+      if (cur == key) { s = (long long)h; break; }
+      if (cur == EMPTY_KEY) break;
+      h = t.next(h);
+    }
+  }
+  return s;
+}
+
 __global__ void __launch_bounds__(JN_THREADS) k_join_count(JoinKeys k, long long n, ProbeRule t, const unsigned long long* __restrict__ keys,
                                                           const unsigned long long* __restrict__ start, unsigned* __restrict__ cnt,
                                                           unsigned* __restrict__ bpos) {
@@ -316,18 +340,7 @@ __global__ void __launch_bounds__(JN_THREADS) k_join_count(JoinKeys k, long long
     unsigned long long key;
     unsigned c = 0, b = 0;
     if (join_key(k, r, &key)) {
-      long long s = -1;
-      if (key == EMPTY_KEY) {
-        s = t.cap;
-      } else {
-        unsigned long long h = t.home(mix64(key));
-        for (long long probes = 0; probes < t.cap; probes++) {
-          const unsigned long long cur = keys[h];
-          if (cur == key) { s = (long long)h; break; }
-          if (cur == EMPTY_KEY) break;
-          h = t.next(h);
-        }
-      }
+      const long long s = find_slot(t, keys, key);
       if (s >= 0) {
         const unsigned long long s0 = start[s];
         c = (unsigned)(start[s + 1] - s0);
@@ -339,32 +352,130 @@ __global__ void __launch_bounds__(JN_THREADS) k_join_count(JoinKeys k, long long
   }
 }
 
-// The probe of a key with Utf8 parts: at a slot with the row's tag, the key is confirmed against the slot's integer word
-// and its representative's Utf8 parts (`b`: the join's copy of the build key columns) before it counts as a match;
-// two keys with one tag never match.
+// The slot of a key with Utf8 parts (probe row r of `u`, its integer word and tag) in *slot: at a slot with the row's
+// tag, the key is confirmed against the slot's integer word and its representative's Utf8 parts (`b`: the join's copy of
+// the build key columns) before it counts as a match; two keys with one tag never match.  False when the key is not in
+// the table.
+__device__ __forceinline__ bool find_utf8_slot(const ProbeRule& t, const unsigned long long* __restrict__ tags,
+                                               const unsigned long long* __restrict__ words, const unsigned* __restrict__ rep,
+                                               const Utf8Keys& u, long long r, const Utf8Keys& b, unsigned long long word,
+                                               unsigned long long tag, unsigned long long* slot) {
+  unsigned long long h = t.home(tag);
+  for (long long probes = 0; probes < t.cap; probes++) {
+    const unsigned long long cur = tags[h];
+    if (cur == EMPTY_KEY) break;
+    if (cur == tag && words[h] == word && utf8_parts_equal(u, r, b, rep[h])) {
+      *slot = h;
+      return true;
+    }
+    h = t.next(h);
+  }
+  return false;
+}
+
 __global__ void __launch_bounds__(JN_THREADS) k_join_utf8_count(JoinKeys k, Utf8Keys u, unsigned long long tag_mask, long long n, ProbeRule t,
                                                                const unsigned long long* __restrict__ tags, const unsigned long long* __restrict__ words,
                                                                const unsigned* __restrict__ rep, Utf8Keys b, const unsigned long long* __restrict__ start,
                                                                unsigned* __restrict__ cnt, unsigned* __restrict__ bpos) {
   for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (long long)gridDim.x * blockDim.x) {
-    unsigned long long word, tag;
+    unsigned long long word, tag, h;
     unsigned c = 0, bp = 0;
-    if (utf8_tag(k, u, tag_mask, r, &word, &tag)) {
-      unsigned long long h = t.home(tag);
-      for (long long probes = 0; probes < t.cap; probes++) {
-        const unsigned long long cur = tags[h];
-        if (cur == EMPTY_KEY) break;
-        if (cur == tag && words[h] == word && utf8_parts_equal(u, r, b, rep[h])) {
-          const unsigned long long s0 = start[h];
-          c = (unsigned)(start[h + 1] - s0);
-          bp = (unsigned)s0;
-          break;
-        }
-        h = t.next(h);
-      }
+    if (utf8_tag(k, u, tag_mask, r, &word, &tag) && find_utf8_slot(t, tags, words, rep, u, r, b, word, tag, &h)) {
+      const unsigned long long s0 = start[h];
+      c = (unsigned)(start[h + 1] - s0);
+      bp = (unsigned)s0;
     }
     cnt[r] = c;
     bpos[r] = bp;
+  }
+}
+
+// ---- semi / anti join: one pass bit per probe row, then an order-preserving compaction ---------------------------------
+// A probe row passes when it has a match (semi) or has none (anti); a row with a null key part passes when `null_pass`
+// is set (anti; null-aware anti only over an empty build side).  The rows are cut into tiles of MARK_TILE: k_join_mark
+// writes the tile's MARK_TILE / 32 mask words (warp w of the CTA writes words i * 8 + w, one __ballot_sync each) and
+// its pass count; the counts are scanned into tile offsets; k_join_select writes the passing row numbers of each tile,
+// in row order, at its offset.
+constexpr int MARK_TILE = 2048;
+constexpr int MARK_WORDS = MARK_TILE / 32;
+constexpr int WARP_WORDS = MARK_WORDS / (JN_THREADS / 32);  // mask words per warp and tile: 8
+
+template <class Pass>
+__device__ __forceinline__ void mark_tiles(long long n, unsigned* __restrict__ mask, unsigned* __restrict__ tile_cnt, Pass pass) {
+  __shared__ unsigned s_cnt[JN_THREADS / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long ntiles = (n + MARK_TILE - 1) / MARK_TILE;
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    unsigned c = 0;
+#pragma unroll 1
+    for (int i = 0; i < MARK_TILE / JN_THREADS; i++) {
+      const long long r = tile * MARK_TILE + i * JN_THREADS + threadIdx.x;
+      const unsigned w = __ballot_sync(0xffffffffu, r < n && pass(r));
+      c += (unsigned)__popc(w);
+      if (lane == 0) mask[r >> 5] = w;
+    }
+    if (lane == 0) s_cnt[warp] = c;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      unsigned total = 0;
+      for (int w = 0; w < JN_THREADS / 32; w++) total += s_cnt[w];
+      tile_cnt[tile] = total;
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(JN_THREADS) k_join_mark(JoinKeys k, long long n, ProbeRule t, const unsigned long long* __restrict__ keys,
+                                                         const unsigned long long* __restrict__ start, int anti, int null_pass,
+                                                         unsigned* __restrict__ mask, unsigned* __restrict__ tile_cnt) {
+  mark_tiles(n, mask, tile_cnt, [&](long long r) {
+    unsigned long long key;
+    if (!join_key(k, r, &key)) return null_pass != 0;
+    const long long s = find_slot(t, keys, key);
+    const bool hit = s >= 0 && (s < t.cap || start[s + 1] != start[s]);  // slot cap holds rows only if the key occurs
+    return hit != (anti != 0);
+  });
+}
+
+__global__ void __launch_bounds__(JN_THREADS) k_join_utf8_mark(JoinKeys k, Utf8Keys u, unsigned long long tag_mask, long long n, ProbeRule t,
+                                                              const unsigned long long* __restrict__ tags, const unsigned long long* __restrict__ words,
+                                                              const unsigned* __restrict__ rep, Utf8Keys b, int anti, int null_pass,
+                                                              unsigned* __restrict__ mask, unsigned* __restrict__ tile_cnt) {
+  mark_tiles(n, mask, tile_cnt, [&](long long r) {
+    unsigned long long word, tag, h;
+    if (!utf8_tag(k, u, tag_mask, r, &word, &tag)) return null_pass != 0;
+    return find_utf8_slot(t, tags, words, rep, u, r, b, word, tag, &h) != (anti != 0);
+  });
+}
+
+// One tile per CTA iteration: each warp takes 8 of the tile's mask words; a prefix over the words' popcounts (within the
+// warp, then over the warps) places each word's rows, and the lanes of a word write its set bits' row numbers together.
+__global__ void __launch_bounds__(JN_THREADS) k_join_select(const unsigned* __restrict__ mask, long long ntiles,
+                                                           const unsigned long long* __restrict__ tile_off, unsigned* __restrict__ out) {
+  __shared__ unsigned s_warp[JN_THREADS / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned below = (1u << lane) - 1u;
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const long long w0 = tile * MARK_WORDS + warp * WARP_WORDS;
+    const unsigned word = lane < WARP_WORDS ? mask[w0 + lane] : 0u;
+    const unsigned c = (unsigned)__popc(word);
+    unsigned incl = c;
+#pragma unroll
+    for (int o = 1; o < WARP_WORDS; o <<= 1) {
+      const unsigned x = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += x;
+    }
+    if (lane == WARP_WORDS - 1) s_warp[warp] = incl;
+    __syncthreads();
+    unsigned before = 0;
+    for (int w = 0; w < warp; w++) before += s_warp[w];
+    const unsigned long long at = tile_off[tile] + before;
+#pragma unroll
+    for (int j = 0; j < WARP_WORDS; j++) {
+      const unsigned wj = __shfl_sync(0xffffffffu, word, j), ej = __shfl_sync(0xffffffffu, incl - c, j);
+      if ((wj >> lane) & 1u) out[at + ej + (unsigned)__popc(wj & below)] = (unsigned)((w0 + j) * 32 + lane);
+    }
+    __syncthreads();
   }
 }
 
@@ -642,6 +753,7 @@ struct dfgpu_join {
   unsigned long long* start = nullptr;  // cap + 2: the first entry of each slot's rows, then the number of rows with a key
   unsigned* rows = nullptr;             // build row numbers, grouped by slot
   long long nrows = 0;
+  long long null_rows = 0;         // build rows with a null key part (null-aware anti join)
   std::vector<int> keep;           // build column numbers kept
   std::vector<DevColumn> cols;     // their device copies, in the order of `keep`
   // a key with Utf8 parts: `keys` holds each slot's tag, and a slot one distinct key
@@ -738,7 +850,7 @@ extern "C" int dfgpu_join_build(dfgpu_ctx* ctx, const dfgpu_batch* build, const 
       j->tag_mask = join_tag_mask();
       build_utf8(ctx, kc, n, j.get(), scratch, counts, row_slot);
     }
-    scan_counts(ctx, counts, cap + 1, j->start);
+    j->null_rows = n - (long long)scan_counts(ctx, counts, cap + 1, j->start);  // start[cap + 1]: the rows with a key
     if (n > 0)
       launch(ctx, "k_join_scatter", k_join_scatter, grid_of(ctx, n), JN_THREADS, (const unsigned long long*)row_slot, n,
              (const unsigned long long*)j->start, counts, j->rows);
@@ -816,6 +928,70 @@ extern "C" int dfgpu_join_probe(dfgpu_join* j, const dfgpu_batch* probe, const d
     for (int i = 0; i < n_build_cols; i++) {
       res->cols.emplace_back();
       gather_column(ctx, *bsrc[size_t(i)], bidx, m, scratch, b64, d_nulls, &res->cols.back());
+    }
+    DF_CUDA(cudaStreamSynchronize(ctx->stream));
+    *out = res.release();
+  });
+}
+
+extern "C" int dfgpu_join_semi(dfgpu_join* j, const dfgpu_batch* probe, const dfgpu_insn* const* keys, const int* key_len, int nkeys, int kind,
+                               const int* probe_cols, int n_probe_cols, dfgpu_result** out) {
+  return guarded([&] {
+    if (!j || !probe || !out || (n_probe_cols > 0 && !probe_cols) || n_probe_cols < 0) fail(DFGPU_ERR_GENERAL, "dfgpu_join_semi: null argument");
+    if (kind != DFGPU_JOIN_SEMI && kind != DFGPU_JOIN_ANTI && kind != DFGPU_JOIN_ANTI_NULL_AWARE)
+      fail(DFGPU_ERR_GENERAL, "dfgpu_join_semi: unknown kind " + std::to_string(kind));
+    if (kind == DFGPU_JOIN_ANTI_NULL_AWARE && nkeys != 1) fail(DFGPU_ERR_GENERAL, "a null-aware anti join takes exactly one key");
+    dfgpu_ctx* ctx = j->ctx;
+    ctx->use();
+    const long long n = probe->nrows;
+    if (n >= (1ll << 32)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "JOIN probe batch of 2^32 rows or more");
+    for (int i = 0; i < n_probe_cols; i++)
+      if (probe_cols[i] < 0 || size_t(probe_cols[i]) >= probe->cols.size()) fail(DFGPU_ERR_INVALID_COLUMN, "probe column " + std::to_string(probe_cols[i]) + " out of range");
+    if (nkeys != j->nkeys) fail(DFGPU_ERR_GENERAL, "JOIN probe has " + std::to_string(nkeys) + " keys, the build side " + std::to_string(j->nkeys));
+    KeyColumns kc;
+    key_columns(ctx, probe, keys, key_len, nkeys, &kc);
+    for (int i = 0; i < nkeys; i++)
+      if (kc.dtypes[i] != j->key_dtypes[i])
+        fail(DFGPU_ERR_EXECUTION, std::string("JOIN key types differ: ") + dtype_name(kc.dtypes[i]) + " and " + dtype_name(j->key_dtypes[i]));
+    // NOT IN over a set holding a null is never true: no row passes, and nothing is launched
+    const bool none = kind == DFGPU_JOIN_ANTI_NULL_AWARE && j->null_rows > 0;
+    const int anti = kind != DFGPU_JOIN_SEMI;
+    const int null_pass = kind == DFGPU_JOIN_ANTI || (kind == DFGPU_JOIN_ANTI_NULL_AWARE && j->nrows == 0);
+    Bufs scratch(ctx);
+    const long long ntiles = (n + MARK_TILE - 1) / MARK_TILE;
+    long long m = 0;
+    unsigned* idx = nullptr;
+    if (n > 0 && !none) {
+      unsigned* mask = scratch.alloc<unsigned>(size_t(ntiles) * MARK_WORDS);
+      unsigned* tile_cnt = scratch.alloc<unsigned>(size_t(ntiles));
+      unsigned long long* tile_off = scratch.alloc<unsigned long long>(size_t(ntiles + 1));
+      const int grid = int(std::min<long long>(ntiles, (long long)ctx->sm_count * 8));
+      if (kc.u.n == 0) {
+        launch(ctx, "k_join_mark", k_join_mark, grid, JN_THREADS, kc.k, n, (ProbeRule)j->t, (const unsigned long long*)j->keys,
+               (const unsigned long long*)j->start, anti, null_pass, mask, tile_cnt);
+      } else {
+        Utf8Keys b{};
+        for (const DevColumn& c : j->ukeys) {
+          b.off[b.n] = c.offsets;
+          b.bytes[b.n] = (const unsigned char*)c.values;
+          b.n++;
+        }
+        launch(ctx, "k_join_utf8_mark", k_join_utf8_mark, grid, JN_THREADS, kc.k, kc.u, j->tag_mask, n, (ProbeRule)j->t,
+               (const unsigned long long*)j->keys, (const unsigned long long*)j->words, (const unsigned*)j->rep, b, anti, null_pass, mask, tile_cnt);
+      }
+      m = (long long)scan_counts(ctx, tile_cnt, ntiles, tile_off);
+      idx = scratch.alloc<unsigned>(size_t(std::max(1ll, m)));
+      if (m > 0)
+        launch(ctx, "k_join_select", k_join_select, grid, JN_THREADS, (const unsigned*)mask, ntiles, (const unsigned long long*)tile_off, idx);
+    }
+    auto res = std::make_unique<dfgpu_result>();
+    res->ctx = ctx;
+    res->nrows = m;
+    unsigned long long* d_nulls = scratch.alloc<unsigned long long>(1);
+    unsigned long long* idx64 = nullptr;
+    for (int i = 0; i < n_probe_cols; i++) {
+      res->cols.emplace_back();
+      gather_column(ctx, probe->cols[size_t(probe_cols[i])], idx, m, scratch, idx64, d_nulls, &res->cols.back());
     }
     DF_CUDA(cudaStreamSynchronize(ctx->stream));
     *out = res.release();

@@ -88,6 +88,7 @@ def lib():
     PC = C.POINTER(C.c_int)
     L.dfgpu_join_build.argtypes = [vp, vp, C.POINTER(PI), PC, C.c_int, PC, C.c_int, C.POINTER(vp)]
     L.dfgpu_join_probe.argtypes = [vp, vp, C.POINTER(PI), PC, C.c_int, PC, C.c_int, PC, C.c_int, C.POINTER(vp)]
+    L.dfgpu_join_semi.argtypes = [vp, vp, C.POINTER(PI), PC, C.c_int, C.c_int, PC, C.c_int, C.POINTER(vp)]
     L.dfgpu_join_free.argtypes = [vp]
     if L.dfgpu_abi_version() != A.ABI_VERSION:
         raise RuntimeError("libdfgpu.so ABI version mismatch")
@@ -412,6 +413,17 @@ class Join:
         barr = (C.c_int * max(1, len(bc)))(*bc)
         out = C.c_void_p()
         check(lib().dfgpu_join_probe(self.h, batch.h, kptrs, klens, nk, parr, len(pc), barr, len(bc), C.byref(out)))
+        return Result(self.ctx, out)
+
+    def semi(self, batch, keys, kind=A.JOIN_SEMI, probe_cols=None):
+        """dfgpu_join_semi: the `probe_cols` of `batch` (default: all) of the probe rows that pass, in probe order.
+        `kind` is A.JOIN_SEMI, A.JOIN_ANTI or A.JOIN_ANTI_NULL_AWARE (include/dfgpu.h has the rules)."""
+        keep = []
+        kptrs, klens, nk = A.make_programs([k.program(batch.schema) for k in keys], keep)
+        pc = list(range(len(batch.schema))) if probe_cols is None else list(probe_cols)
+        parr = (C.c_int * max(1, len(pc)))(*pc)
+        out = C.c_void_p()
+        check(lib().dfgpu_join_semi(self.h, batch.h, kptrs, klens, nk, kind, parr, len(pc), C.byref(out)))
         return Result(self.ctx, out)
 
     def free(self):

@@ -329,7 +329,7 @@ int dfgpu_aggregate_update_host(dfgpu_aggstate* st, const dfgpu_col* cols, int n
 int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out);
 int dfgpu_aggregate_free(dfgpu_aggstate* st);
 
-/* ---- inner equi-join on integer and Utf8 keys ----
+/* ---- inner, semi and anti equi-join on integer and Utf8 keys ----
  * The reference has no join: its planner plans none and its `Relation` trait (src/execution/relation.rs:27-32) has
  * no join relation; "JOIN support (hash join ...)" is the headline of its next milestone (ROADMAP.md, 0.7.0).  These
  * entry points are what a GpuHashJoinRelation implementing that trait calls: build once over the right input, then
@@ -350,6 +350,7 @@ int dfgpu_aggregate_free(dfgpu_aggstate* st);
  *   - A build side of 2^32 rows or more, a probe batch of 2^32 rows or more and a probe batch producing 2^32 or more
  *     output rows are DFGPU_ERR_NOT_IMPLEMENTED. */
 typedef struct dfgpu_join dfgpu_join; /* the build side's hash table and its kept columns */
+enum { DFGPU_JOIN_SEMI = 1, DFGPU_JOIN_ANTI = 2, DFGPU_JOIN_ANTI_NULL_AWARE = 3 }; /* dfgpu_join_semi kinds */
 /* Build the table over `build` (borrowed for the call only).  The join keeps its own device copy of the columns
  * `keep_cols` (build-batch column numbers) and of its Utf8 key columns, so the caller may free the batch afterwards.
  * DFGPU_JOIN_TAG_BITS (1 to 64, default 64) cuts a Utf8 key's hash tag for tests of the collision handling. */
@@ -359,6 +360,20 @@ int dfgpu_join_build(dfgpu_ctx* ctx, const dfgpu_batch* build, const dfgpu_insn*
  * (its column numbering; each must be among `keep_cols`, else DFGPU_ERR_GENERAL), one row per matching pair. */
 int dfgpu_join_probe(dfgpu_join* j, const dfgpu_batch* probe, const dfgpu_insn* const* keys, const int* key_len, int nkeys,
                      const int* probe_cols, int n_probe_cols, const int* build_cols, int n_build_cols, dfgpu_result** out);
+/* Semi and anti join with one probe batch: the `probe_cols` of the probe rows that pass, in probe-row order, each
+ * probe row at most once.  `kind`:
+ *   DFGPU_JOIN_SEMI             a row passes when every key part is non-null and some build row has an equal key
+ *                               (SQL `x IN (SELECT y ..)`, `EXISTS (.. WHERE u.a = t.a ..)`)
+ *   DFGPU_JOIN_ANTI             a row passes when no build row has an equal key; a row with a null key part passes
+ *                               (SQL `NOT EXISTS`)
+ *   DFGPU_JOIN_ANTI_NULL_AWARE  exactly one key (else DFGPU_ERR_GENERAL).  An empty build side: every row passes.
+ *                               A build row with a null key: no row passes (no kernel runs).  Otherwise a row passes
+ *                               when its key is non-null and no build row has an equal key (SQL `x NOT IN (SELECT y ..)`
+ *                               under three-valued logic, unknown read as false)
+ * Keys, key types and their refusals and the 2^32-row probe limit are those of dfgpu_join_probe.  A join built for
+ * semi / anti probes needs no kept columns (n_keep = 0). */
+int dfgpu_join_semi(dfgpu_join* j, const dfgpu_batch* probe, const dfgpu_insn* const* keys, const int* key_len, int nkeys, int kind,
+                    const int* probe_cols, int n_probe_cols, dfgpu_result** out);
 int dfgpu_join_free(dfgpu_join* j);
 
 /* ---- results ---- */

@@ -14,6 +14,7 @@ import sys
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from datafusion_archive_b200 import _abi as A  # noqa: E402
 from datafusion_archive_b200 import engine, workloads  # noqa: E402
 from datafusion_archive_b200.expr import AggregateFunction, col, lit  # noqa: E402
 
@@ -206,5 +207,32 @@ for bits in (None, "2"):
     jr.free(); jj.free(); jpb.free()
     os.environ.pop("DFGPU_JOIN_TAG_BITS", None)
 print("utf8 join ok", flush=True)
+# 12. Semi / anti join: k_join_mark's ballots and tile counts, k_join_select's prefix over the mask words (a ragged last
+# tile, every kind, nulls on both sides), and k_join_utf8_mark's confirmation under 2-bit tags
+spk = pa.array(rng.integers(0, 300, 9_001), mask=rng.random(9_001) < 0.05)
+sbk = pa.array(rng.integers(0, 600, 200), mask=rng.random(200) < 0.01)
+sset = {v for v in sbk.to_pylist() if v is not None}
+for kind in (A.JOIN_SEMI, A.JOIN_ANTI, A.JOIN_ANTI_NULL_AWARE):
+    sbb, spb = ctx.upload([sbk]), ctx.upload([spk, np.arange(9_001, dtype=np.int64)])
+    sj = ctx.join_build(sbb, [col(0)], keep_cols=[])
+    sr = sj.semi(spb, [col(0)], kind, probe_cols=[1])
+    got = sr.columns()[0] if sr.nrows else np.zeros(0, np.int64)
+    pl = spk.to_pylist()
+    if kind == A.JOIN_SEMI:
+        exp = [i for i, v in enumerate(pl) if v is not None and v in sset]
+    elif kind == A.JOIN_ANTI:
+        exp = [i for i, v in enumerate(pl) if v is None or v not in sset]
+    else:
+        exp = [] if sbk.null_count else [i for i, v in enumerate(pl) if v is not None and v not in sset]
+    assert list(got) == exp, kind
+    sr.free(); sj.free(); sbb.free(); spb.free()
+os.environ["DFGPU_JOIN_TAG_BITS"] = "2"
+sbb, spb = ctx.upload([jus]), ctx.upload([jup, np.arange(len(jup), dtype=np.int64)])
+sj = ctx.join_build(sbb, [col(0)], keep_cols=[])
+sr = sj.semi(spb, [utf8_fn("lower", col(0))], A.JOIN_SEMI, probe_cols=[1])
+assert sr.nrows == sum(1 for v in jup.to_pylist() if v.lower() in jcount)
+sr.free(); sj.free(); sbb.free(); spb.free()
+os.environ.pop("DFGPU_JOIN_TAG_BITS", None)
+print("semi join ok", flush=True)
 ctx.close()
 print("SANITIZE_CASES_OK")

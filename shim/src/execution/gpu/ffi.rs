@@ -170,6 +170,12 @@ extern "C" {
         j: *mut dfgpu_join, probe: *const dfgpu_batch, keys: *const *const dfgpu_insn, key_len: *const c_int, nkeys: c_int,
         probe_cols: *const c_int, n_probe_cols: c_int, build_cols: *const c_int, n_build_cols: c_int, out: *mut *mut dfgpu_result,
     ) -> c_int;
+    /// semi / anti join (kind: DFGPU_JOIN_SEMI, _ANTI, _ANTI_NULL_AWARE = 1, 2, 3): the `probe_cols` of the passing
+    /// probe rows, in probe order
+    pub fn dfgpu_join_semi(
+        j: *mut dfgpu_join, probe: *const dfgpu_batch, keys: *const *const dfgpu_insn, key_len: *const c_int, nkeys: c_int, kind: c_int,
+        probe_cols: *const c_int, n_probe_cols: c_int, out: *mut *mut dfgpu_result,
+    ) -> c_int;
     pub fn dfgpu_join_free(j: *mut dfgpu_join) -> c_int;
     pub fn dfgpu_result_shape(r: *const dfgpu_result, nrows: *mut i64, ncols: *mut c_int) -> c_int;
     pub fn dfgpu_result_col_dtype(r: *const dfgpu_result, i: c_int, dtype: *mut i32) -> c_int;

@@ -1,0 +1,21 @@
+"""Semi and anti joins across two ranks (NCCL, two H100s): IN, NOT IN with and without a null in the subquery, EXISTS
+and NOT EXISTS under aggregates and projections give every rank the one-GPU result, including with an empty rank."""
+import os
+import subprocess
+import sys
+
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+@pytest.mark.gpu
+def test_nccl_world2_semi_join():
+    from datafusion_archive_b200 import engine
+    if engine.device_count() < 2:
+        pytest.skip("needs 2 GPUs")
+    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
+           "--master-port", "29663", os.path.join(ROOT, "tests", "semi_join_mp_worker.py")]
+    p = subprocess.run(cmd, capture_output=True, text=True, timeout=600, cwd=ROOT)
+    assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-4000:]
+    assert "MP_SEMI_JOIN_OK world=2" in p.stdout
