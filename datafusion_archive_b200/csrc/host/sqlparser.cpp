@@ -2,6 +2,7 @@
 #include "sqlparser.h"
 
 #include <cctype>
+#include <cerrno>
 #include <cstdlib>
 
 #include "logicalplan.h"
@@ -157,7 +158,14 @@ struct Parser {
     switch (t.kind) {
       case Token::Number:
         if (t.text.find('.') != std::string::npos) { n->kind = ASTNode::SQLDouble; n->dval = strtod(t.text.c_str(), nullptr); }
-        else { n->kind = ASTNode::SQLLong; n->lval = strtoll(t.text.c_str(), nullptr, 10); }
+        else {
+          // digits beyond i64 are refused, not saturated: `-9223372036854775808` is the prefix `-` applied to
+          // 9223372036854775808, which does not fit, so INT64_MIN is written `-9223372036854775807 - 1`
+          errno = 0;
+          n->kind = ASTNode::SQLLong;
+          n->lval = strtoll(t.text.c_str(), nullptr, 10);
+          if (errno == ERANGE) perr("Could not parse '" + t.text + "' as i64: number too large to fit in target type");
+        }
         return n;
       case Token::String: n->kind = ASTNode::SQLString; n->id = t.text; return n;
       case Token::Sym:

@@ -95,6 +95,11 @@ enum {
   DFGPU_OP_SUB = 11, /* Operator::Minus    → array_ops::subtract  expression.rs:473 */
   DFGPU_OP_MUL = 12, /* Operator::Multiply → array_ops::multiply  expression.rs:480 */
   DFGPU_OP_DIV = 13, /* Operator::Divide   → array_ops::divide    expression.rs:487 */
+  /* + - * /: both operands of one dtype, which is the result's.  Integers wrap at the operand width (Rust release
+     semantics), `/` truncates toward zero and MIN / -1 = MIN.  Floats are IEEE, each result rounded once to nearest
+     (no FTZ, no fused multiply-add).  A zero divisor of any type, -0.0 included, is DFGPU_ERR_ARROW "DivideByZero",
+     raised only for a row that survives the WHERE (a WHERE reads every row); without a WHERE a null row does not
+     raise it, while under a WHERE a surviving row's null slot is divided like any other value. */
   DFGPU_OP_EQ = 20,  /* array_ops::eq      expression.rs:410 */
   DFGPU_OP_NE = 21,  /* array_ops::neq     expression.rs:417 */
   DFGPU_OP_LT = 22,  /* array_ops::lt      expression.rs:424 */

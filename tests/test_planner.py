@@ -58,6 +58,10 @@ def test_more_planner_rules(mock):
     assert mock.plan("SELECT salary + age, salary * 2 FROM person WHERE age < 30") == (
         "Projection: #5 Plus CAST(#3 AS Float64), #5 Multiply CAST(Int64(2) AS Float64)\n"
         "  Selection: CAST(#3 AS Int64) Lt Int64(30)\n    TableScan: person projection=None")
+    # the i64 extremes are literals as written; INT64_MIN is `-9223372036854775807 - 1`
+    assert mock.plan("SELECT age FROM person WHERE age < 9223372036854775807 AND age > -9223372036854775807 - 1") == (
+        "Projection: #3\n  Selection: CAST(#3 AS Int64) Lt Int64(9223372036854775807) And "
+        "CAST(#3 AS Int64) Gt Int64(-9223372036854775807) Minus Int64(1)\n    TableScan: person projection=None")
 
 
 def test_planner_errors(mock):
@@ -73,6 +77,11 @@ def test_planner_errors(mock):
         # get_supertype(Int32, UInt32) = Int32 but can_coerce_from(Int32, UInt32) is false: the reference's
         # own lattice inconsistency (logicalplan.rs:474 vs :565-568), reproduced
         ("SELECT id FROM person WHERE age < id", "Cannot automatically convert UInt32 to Int32"),
+        # integer literals whose digits do not fit i64 are refused, not saturated (the prefix `-` is not part of
+        # the literal, so INT64_MIN itself is refused too)
+        ("SELECT id FROM person WHERE id > 9223372036854775808", "9223372036854775808"),
+        ("SELECT id FROM person WHERE id > -9223372036854775808", "9223372036854775808"),
+        ("SELECT id + 99999999999999999999999 FROM person", "99999999999999999999999"),
     ]:
         with pytest.raises(host.ExecutionError) as e:
             mock.plan(sql)
