@@ -192,6 +192,71 @@ extern "C" int dfgpu_profile_get(dfgpu_ctx* ctx, double* kernel_ms, int64_t* lau
   });
 }
 
+int dfgpu_ctx::fp_acquire(dfgpu_result* owner) {
+  if (fp_free.empty()) {  // take back the retired slots whose kernel has completed
+    for (size_t i = 0; i < fp_retired.size();) {
+      const cudaError_t e = cudaEventQuery(fp_slots[size_t(fp_retired[i])].done);
+      if (e == cudaErrorNotReady) {
+        cudaGetLastError();  // not an error: keep it out of the next launch check
+        i++;
+        continue;
+      }
+      DF_CUDA(e);
+      fp_free.push_back(fp_retired[i]);
+      fp_retired[i] = fp_retired.back();
+      fp_retired.pop_back();
+    }
+  }
+  if (fp_free.empty()) {  // all slots in flight: grow rather than wait
+    unsigned long long* words = nullptr;
+    DF_CUDA(cudaMallocHost(&words, size_t(kFpSlab) * 2 * 8));
+    fp_slabs.push_back(words);
+    for (int i = 0; i < kFpSlab; i++) {
+      FpSlot s;
+      s.words = words + 2 * i;
+      DF_CUDA(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
+      fp_free.push_back(int(fp_slots.size()));
+      fp_slots.push_back(s);
+    }
+  }
+  const int s = fp_free.back();
+  fp_free.pop_back();
+  FpSlot& slot = fp_slots[size_t(s)];
+  slot.words[0] = 0;
+  slot.words[1] = 0;
+  slot.owner = owner;
+  return s;
+}
+
+void dfgpu_ctx::fp_retire(int s) {
+  fp_slots[size_t(s)].owner = nullptr;
+  fp_retired.push_back(s);
+}
+
+namespace dfgpu {
+
+// A pending result's kernel has completed (or is waited for here): take its row count and flag, free its slot.
+static void settle(const dfgpu_result* r) {
+  dfgpu_ctx* ctx = r->ctx;
+  dfgpu_ctx::FpSlot& s = ctx->fp_slots[size_t(r->pending)];
+  DF_CUDA(cudaEventSynchronize(s.done));
+  r->nrows = (int64_t)s.words[0];
+  r->div_by_zero = s.words[1] != 0;
+  s.owner = nullptr;
+  ctx->fp_free.push_back(r->pending);
+  r->pending = -1;
+}
+
+void resolve(const dfgpu_result* r) {
+  if (r->pending >= 0) {
+    r->ctx->use();
+    settle(r);
+  }
+  if (r->div_by_zero) fail(DFGPU_ERR_ARROW, "DivideByZero");
+}
+
+}  // namespace dfgpu
+
 dfgpu_batch::~dfgpu_batch() {
   if (!ctx || !owns) return;
   cudaSetDevice(ctx->device);
@@ -223,6 +288,8 @@ void dfgpu_ctx::host_release(void* p) {
 dfgpu_result::~dfgpu_result() {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
+  // never waits: the slot returns once its kernel is seen complete, the buffers below go back in stream order
+  if (pending >= 0) ctx->fp_retire(pending);
   if (on_host) {
     for (auto& c : cols) ctx->host_release(c.values);
     return;
@@ -343,6 +410,11 @@ extern "C" int dfgpu_shutdown(dfgpu_ctx* ctx) {
     if (!ctx) return;
     ctx->use();
     cudaStreamSynchronize(ctx->stream);
+    // results still pending keep their row count: they outlive the slots that hold it
+    for (auto& s : ctx->fp_slots)
+      if (s.owner) settle(s.owner);
+    for (auto& s : ctx->fp_slots) cudaEventDestroy(s.done);
+    for (void* w : ctx->fp_slabs) cudaFreeHost(w);
     dfgpu_comm_destroy(ctx);
     ctx->release_cached();
     if (ctx->flush_buf) cudaFree(ctx->flush_buf);
@@ -548,9 +620,11 @@ extern "C" int dfgpu_batch_free(dfgpu_batch* b) {
 // results
 // ---------------------------------------------------------------------------------------------
 extern "C" int dfgpu_result_shape(const dfgpu_result* r, int64_t* nrows, int* ncols) {
-  *nrows = r->nrows;
-  *ncols = int(r->cols.size());
-  return 0;
+  return guarded([&] {
+    resolve(r);
+    *nrows = r->nrows;
+    *ncols = int(r->cols.size());
+  });
 }
 extern "C" int dfgpu_result_col_dtype(const dfgpu_result* r, int i, int32_t* dtype) {
   return guarded([&] {
@@ -561,6 +635,7 @@ extern "C" int dfgpu_result_col_dtype(const dfgpu_result* r, int i, int32_t* dty
 extern "C" int dfgpu_result_col_bytes(const dfgpu_result* r, int i, int64_t* nbytes) {
   return guarded([&] {
     if (i < 0 || size_t(i) >= r->cols.size()) fail(DFGPU_ERR_INVALID_COLUMN, "result column out of range");
+    resolve(r);
     const DevColumn& c = r->cols[size_t(i)];
     const int w = dtype_width(c.dtype);
     *nbytes = w ? r->nrows * w : int64_t(c.values_bytes);
@@ -569,12 +644,14 @@ extern "C" int dfgpu_result_col_bytes(const dfgpu_result* r, int i, int64_t* nby
 extern "C" int dfgpu_result_col_nulls(const dfgpu_result* r, int i, int64_t* nulls) {
   return guarded([&] {
     if (i < 0 || size_t(i) >= r->cols.size()) fail(DFGPU_ERR_INVALID_COLUMN, "result column out of range");
+    resolve(r);
     *nulls = r->cols[size_t(i)].null_count;
   });
 }
 extern "C" int dfgpu_result_copy_col(const dfgpu_result* r, int i, void* dst_values, uint8_t* dst_validity, int32_t* dst_offsets) {
   return guarded([&] {
     if (i < 0 || size_t(i) >= r->cols.size()) fail(DFGPU_ERR_INVALID_COLUMN, "result column out of range");
+    resolve(r);
     dfgpu_ctx* ctx = r->ctx;
     ctx->use();
     const DevColumn& c = r->cols[size_t(i)];
@@ -600,6 +677,7 @@ extern "C" int dfgpu_result_col_device_ptr(const dfgpu_result* r, int i, const v
   return guarded([&] {
     if (i < 0 || size_t(i) >= r->cols.size()) fail(DFGPU_ERR_INVALID_COLUMN, "result column out of range");
     if (r->on_host) fail(DFGPU_ERR_GENERAL, "result lives in host memory: use dfgpu_result_col_host_ptr");
+    resolve(r);
     *dptr = r->cols[size_t(i)].values;
   });
 }
@@ -613,6 +691,7 @@ extern "C" int dfgpu_result_col_host_ptr(const dfgpu_result* r, int i, const voi
   return guarded([&] {
     if (i < 0 || size_t(i) >= r->cols.size()) fail(DFGPU_ERR_INVALID_COLUMN, "result column out of range");
     if (!r->on_host) fail(DFGPU_ERR_GENERAL, "result lives in device memory: use dfgpu_result_copy_col");
+    resolve(r);
     *hptr = r->cols[size_t(i)].values;
   });
 }

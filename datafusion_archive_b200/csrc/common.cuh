@@ -102,6 +102,22 @@ struct dfgpu_ctx {
   int rank = 0, world = 1;
   void* nccl_comm = nullptr;
 
+  // Stream-ordered filter/project results (filter_project.cu): each result whose row count is not read yet owns one
+  // slot, a pinned [row count, DivideByZero flag] word pair its kernel writes and an event recorded after that kernel.
+  // A slot is handed out again only after its event has been observed complete; the slab grows instead of waiting.
+  struct FpSlot {
+    unsigned long long* words = nullptr;
+    cudaEvent_t done = nullptr;
+    dfgpu_result* owner = nullptr;  // the pending result, or null
+  };
+  static constexpr int kFpSlab = 64;  // slots added per growth
+  std::vector<FpSlot> fp_slots;
+  std::vector<void*> fp_slabs;  // pinned blocks behind fp_slots[].words
+  std::vector<int> fp_free;     // slots ready for a new result
+  std::vector<int> fp_retired;  // slots of results freed while their kernel could still be running
+  int fp_acquire(dfgpu_result* owner);
+  void fp_retire(int slot);
+
   // kernels whose per-device function attributes (dynamic shared memory limit) were set through this
   // ctx: the attribute belongs to the device, so it is tracked per ctx and not per process
   std::vector<const void*> configured_kernels;
@@ -171,8 +187,18 @@ struct dfgpu_batch {
 
 struct dfgpu_result {
   dfgpu_ctx* ctx = nullptr;
-  int64_t nrows = 0;
+  // A stream-ordered filter/project result learns its row count when its kernel has completed: until
+  // dfgpu::resolve has run, `pending` is its ctx->fp_slots index and nrows is not valid.
+  mutable int64_t nrows = 0;
+  mutable int pending = -1;
+  mutable bool div_by_zero = false;
   std::vector<DevColumn> cols;
   bool on_host = false;  // columns live in pinned host memory (dfgpu_filter_project_host)
   ~dfgpu_result();
 };
+
+namespace dfgpu {
+// Makes a result's shape readable: waits for a pending result's kernel, reads its row count, and fails with
+// DivideByZero when the kernel raised it (api.cu).  Every entry point that reports a result's shape or data calls it.
+void resolve(const dfgpu_result* r);
+}  // namespace dfgpu

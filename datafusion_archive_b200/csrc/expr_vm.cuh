@@ -71,6 +71,13 @@ inline bool has_fn(const ProgramSet& ps) {
     if (ps.insn[pc].op >= V_FN) return true;
   return false;
 }
+// Some program of the set divides: the only instruction whose kernels can raise an error (DivideByZero, for integers and
+// floats alike).  A set without one cannot fail once its kernel is launched.
+inline bool has_div(const ProgramSet& ps) {
+  for (int pc = 0; pc < ps.start[ps.nprog]; pc++)
+    if (ps.insn[pc].op == V_DIV || ps.insn[pc].op == V_RDIV) return true;
+  return false;
+}
 
 // Interpreter-free shapes.  ProgramBuilder::add recognises them; the operators pass them to kernels that evaluate them
 // with straight-line code (same arithmetic as the interpreter, no decode in the inner loop).

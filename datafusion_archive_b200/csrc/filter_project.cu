@@ -371,16 +371,28 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
     // tile_status is sized for the smallest tile either kernel uses (1024 rows)
     const size_t max_tiles = size_t((n + 1023) / 1024) + 1;
     // one allocation, one memset: [ticket, pad..] then the tile words.  The row count and the error
-    // flag are written by the kernel straight into pinned host memory (zero-copy), so the step ends
-    // with a stream synchronise and no device-to-host copy.
+    // flag are written by the kernel straight into pinned host memory (zero-copy), so no device-to-host
+    // copy follows the kernel.
     unsigned long long* status = (unsigned long long*)ctx->alloc((max_tiles + 8) * 8);
     DF_CUDA(cudaMemsetAsync(status, 0, (max_tiles + 8) * 8, ctx->stream));
-    ctx->h_scratch[0] = 0;
-    ctx->h_scratch[2] = 0;
     p.tile_status = status + 8;
     p.ticket = (unsigned*)(status + 0);
-    p.out_count = ctx->h_scratch + 0;
-    p.err_flag = (unsigned*)(ctx->h_scratch + 2);
+    // Stream-ordered: when nothing after the kernel needs the row count on the host (no Boolean packing, no Utf8
+    // gather, no validity outputs) and no program can raise, the call returns once the kernel is queued.  The kernel
+    // writes the count into a word pair the result owns, read when the result is first used (resolve, api.cu).
+    bool any_bool = false;
+    for (int i = 0; i < nproj; i++) any_bool = any_bool || bool_of_out[size_t(i)] >= 0;
+    const bool stream_ordered = has_pred && !p.ps.has_nulls && !any_utf8 && !any_bool && !has_div(p.ps);
+    if (stream_ordered) {
+      res->pending = ctx->fp_acquire(res.get());
+      p.out_count = ctx->fp_slots[size_t(res->pending)].words;
+      p.err_flag = (unsigned*)(p.out_count + 1);
+    } else {
+      ctx->h_scratch[0] = 0;
+      ctx->h_scratch[2] = 0;
+      p.out_count = ctx->h_scratch + 0;
+      p.err_flag = (unsigned*)(ctx->h_scratch + 2);
+    }
     // validity outputs: only a query WITHOUT a predicate can emit nulls (see k_filter_project)
     memset(p.out_valid, 0, sizeof(p.out_valid));
     p.null_counts = ctx->d_scratch + 32;
@@ -414,6 +426,13 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
       else if (d <= 2) launch_fp<2>(ctx, p);
       else if (d <= 4) launch_fp<4>(ctx, p);
       else launch_fp<8>(ctx, p);
+    }
+    if (stream_ordered) {
+      DF_CUDA(cudaEventRecord(ctx->fp_slots[size_t(res->pending)].done, ctx->stream));
+      ctx->free(status);
+      if (getenv("DFGPU_TRACE")) fprintf(stderr, "[dfgpu trace] filter_project returns stream-ordered\n");
+      *out = res.release();
+      return;
     }
     if (p.ps.has_nulls && !has_pred)
       DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 32, ctx->d_scratch + 32, kMaxProgs * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -633,7 +652,8 @@ extern "C" int dfgpu_filter_project_host(dfgpu_ctx* ctx, const dfgpu_col* cols, 
         }
       }
       if (resident) break;
-      // the kernel of this chunk has completed (dfgpu_filter_project synchronised ctx->stream)
+      // waits for the kernel of this chunk: its row count sizes the copies, and stream_out reads what it wrote
+      resolve(ch.res);
       for (int q = 0; q < nproj; q++) {
         const int w = dtype_width(res->cols[size_t(q)].dtype);
         if (ch.res->nrows > 0)

@@ -120,11 +120,32 @@ class PinnedBuffer:
 
 
 class Result:
-    def __init__(self, ctx, handle):
+    """An operator's output.  `shape_on_first_use`: the operator may have returned before its kernel finished
+    (dfgpu_filter_project), so the shape is read, waiting for the kernel, when nrows / ncols is first asked for;
+    other results read it here, so that it stays available after free()."""
+
+    def __init__(self, ctx, handle, shape_on_first_use=False):
         self.ctx, self.h = ctx, handle
-        nrows, ncols = C.c_int64(), C.c_int()
-        lib().dfgpu_result_shape(self.h, C.byref(nrows), C.byref(ncols))
-        self.nrows, self.ncols = nrows.value, ncols.value
+        self._shape = None
+        if not shape_on_first_use:
+            self._read_shape()
+
+    def _read_shape(self):
+        if self._shape is None:
+            if not self.h:
+                raise RuntimeError("the result was freed before its shape was read")
+            nrows, ncols = C.c_int64(), C.c_int()
+            check(lib().dfgpu_result_shape(self.h, C.byref(nrows), C.byref(ncols)))
+            self._shape = (nrows.value, ncols.value)
+        return self._shape
+
+    @property
+    def nrows(self):
+        return self._read_shape()[0]
+
+    @property
+    def ncols(self):
+        return self._read_shape()[1]
 
     def dtype(self, i):
         dt = C.c_int32()
@@ -170,7 +191,7 @@ class Result:
 
 def _fetch_result(L, handle):
     nrows, ncols = C.c_int64(), C.c_int()
-    L.dfgpu_result_shape(handle, C.byref(nrows), C.byref(ncols))
+    check(L.dfgpu_result_shape(handle, C.byref(nrows), C.byref(ncols)))
     n = nrows.value
     cols = []
     for i in range(ncols.value):
@@ -287,7 +308,7 @@ class GpuContext:
         ptrs, lens, n = A.make_programs([e.program(schema) for e in proj], keep)
         out = C.c_void_p()
         check(lib().dfgpu_filter_project(self.h, batch.h, parr, len(pprog), ptrs, lens, n, C.byref(out)))
-        return Result(self, out)
+        return Result(self, out, shape_on_first_use=True)
 
     def filter_project_host(self, arrays, pred=None, proj=(), chunk_rows=0):
         """Host buffers in, host (pinned) buffers out; upload / kernel / download pipelined by chunk."""

@@ -292,7 +292,13 @@ int dfgpu_utf8_fn_host(const char* s, int64_t s_len, const dfgpu_insn* prog, int
  * pred_len == 0: no WHERE clause.  nproj == 0: emit every input column (what FilterRelation alone
  * does: filter.rs:55-57).  Output rows keep input order (filter.rs:86-90).  A projection whose type is
  * Boolean (a comparison or AND / OR: expression.rs:212-224,236-290) comes back as a DFGPU_BOOL column,
- * bit-packed LSB first like arrow's BooleanArray; dfgpu_result_col_bytes reports (nrows + 7) / 8. */
+ * bit-packed LSB first like arrow's BooleanArray; dfgpu_result_col_bytes reports (nrows + 7) / 8.
+ * Stream-ordered calls: a query with a WHERE clause whose referenced columns have no nulls, whose outputs are all
+ * numeric (no Boolean, no Utf8) and which divides nowhere returns once its work is queued, before the kernel has
+ * finished.  Every other call returns finished, and reports DivideByZero itself.  The accessors below
+ * (dfgpu_result_shape, _col_bytes, _col_nulls, _copy_col, _col_device_ptr, _col_host_ptr) wait for the kernel
+ * before they answer; dfgpu_result_col_dtype and dfgpu_result_free never wait.  dfgpu_shutdown waits for every
+ * call still running, and the shape of a result that outlives its ctx stays readable. */
 int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, const dfgpu_insn* pred, int pred_len,
                          const dfgpu_insn* const* proj, const int* proj_len, int nproj, dfgpu_result** out);
 
