@@ -1584,69 +1584,31 @@ struct dfgpu_aggstate {
 
 namespace {
 
-// Words of the pinned ctx->h_scratch that the operator stages through.
-constexpr int HS_COUNTERS = 8;  // counter slots [0, CTR_NONNULL)
-constexpr int HS_HEADER = 16;   // multi-GPU header record (up to 16 words)
-constexpr int HS_NONNULL = 40;  // the CTR_NONNULL block (kMaxAggs words)
-constexpr int HS_ROWS = 48;     // CTR_ROWS
-
-// Device blocks that go back to the ctx pool at scope exit.
-struct DevBufs {
-  dfgpu_ctx* ctx;
-  std::vector<void*> blocks;
-  explicit DevBufs(dfgpu_ctx* c) : ctx(c) {}
-  DevBufs(const DevBufs&) = delete;
-  DevBufs& operator=(const DevBufs&) = delete;
-  ~DevBufs() {
-    for (void* q : blocks) ctx->free(q);
-  }
-  template <class T = unsigned long long>
-  T* alloc(size_t bytes) {
-    void* q = ctx->alloc(bytes);
-    blocks.push_back(q);
-    return static_cast<T*>(q);
-  }
-};
-
 // Growth policy of the group table and the pair sets (sized by table_cap, hash_table.cuh): a table takes new entries up
 // to half full and grows x4.
 long long fill_limit(long long cap) { return cap / 2; }
 long long grown_cap(long long cap) { return cap * 4; }
 
-int grid_for(dfgpu_ctx* ctx, long long work_items, int per_block, int blocks_per_sm) {
-  long long g = (work_items + per_block - 1) / per_block;
-  long long cap = (long long)ctx->sm_count * blocks_per_sm;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return int(g);
-}
-
-// The operator's one launch path: AG_THREADS threads per CTA, one CTA per `per_block` work items, at most `per_sm` CTAs per
-// SM (0: as many as the occupancy calculator fits with `smem` bytes of dynamic shared memory).  bind(grid) runs first and
-// sets what depends on the grid in the caller's objects that `args` refer to.  Profiled launches, the scans, reduces and
-// COUNT(DISTINCT) inserts, are also timed in the profile ring (dfgpu_profile_get), where the benchmark's kernel times come from.
-constexpr bool PROFILED = true;
+// The operator's launches: AG_THREADS threads per CTA, one CTA per `per_block` work items, at most `per_sm` CTAs per SM (0: as
+// many as the occupancy calculator fits with opts.smem bytes of dynamic shared memory).  bind(grid) runs first and sets
+// what depends on the grid in the caller's objects that `args` refer to.  Profiled launches are the scans, reduces and
+// COUNT(DISTINCT) inserts.
 template <class... P, class Bind>
-void launch(dfgpu_ctx* ctx, void (*kern)(P...), const char* name, long long work_items, int per_block, int per_sm, size_t smem,
-            bool profiled, Bind&& bind, const P&... args) {
+void launch_ag(dfgpu_ctx* ctx, void (*kern)(P...), const char* name, long long work_items, int per_block, int per_sm, const LaunchOpts& opts,
+               Bind&& bind, const P&... args) {
   if (per_sm == 0) {
-    DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, AG_THREADS, smem));
+    DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, AG_THREADS, opts.smem));
     per_sm = std::max(per_sm, 1);
   }
   const int grid = grid_for(ctx, work_items, per_block, per_sm);
   bind(grid);
-  const int ps = profiled ? ctx->prof_begin() : -1;
-  kern<<<grid, AG_THREADS, smem, ctx->stream>>>(args...);
-  DF_CUDA(cudaGetLastError());
-  trace_launch(name);
-  ctx->prof_end(ps);
-  ctx->launches++;
+  launch(ctx, name, kern, grid, AG_THREADS, opts, args...);
 }
 // A launch whose arguments do not depend on the grid.
 template <class P>
 void launch_kernel(dfgpu_ctx* ctx, void (*kern)(P), const char* name, const P& p, long long work_items, int per_block, int per_sm,
-                   bool profiled = false) {
-  launch(ctx, kern, name, work_items, per_block, per_sm, 0, profiled, [](int) {}, p);
+                   const LaunchOpts& opts = {}) {
+  launch_ag(ctx, kern, name, work_items, per_block, per_sm, opts, [](int) {}, p);
 }
 
 // A kernel instantiation and its trace name.  FRONT scan kernels route rows through the shared-memory front table.
@@ -1774,19 +1736,9 @@ TableLayout table_alloc(dfgpu_ctx* ctx, int naggs, int nkeys, const std::vector<
 }
 
 // counter slots [0, CTR_NONNULL) -> host8 (synchronises the stream)
-void read_counters(dfgpu_aggstate* st, unsigned long long* host8) {
-  dfgpu_ctx* ctx = st->ctx;
-  DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + HS_COUNTERS, st->d_counters, CTR_NONNULL * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  DF_CUDA(cudaStreamSynchronize(ctx->stream));
-  for (int i = 0; i < CTR_NONNULL; i++) host8[i] = ctx->h_scratch[HS_COUNTERS + i];
-}
+void read_counters(dfgpu_aggstate* st, unsigned long long* host8) { read_words(st->ctx, st->d_counters, CTR_NONNULL * 8, host8); }
 // one counter slot (synchronises the stream)
-unsigned long long read_counter(dfgpu_aggstate* st, int slot) {
-  dfgpu_ctx* ctx = st->ctx;
-  DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + HS_COUNTERS + slot, st->d_counters + slot, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  DF_CUDA(cudaStreamSynchronize(ctx->stream));
-  return ctx->h_scratch[HS_COUNTERS + slot];
-}
+unsigned long long read_counter(dfgpu_aggstate* st, int slot) { return read_word(st->ctx, st->d_counters + slot); }
 
 // Raw compaction (k_compact, raw = 1) of table t: the occupied slots as (packed key, accumulators) entries.  Entry i's
 // key goes to keys[i * stride] and accumulator a to vals[a * val_step + i * stride] (stride 0 = 1); the number of
@@ -2261,11 +2213,7 @@ SetView set_alloc(dfgpu_ctx* ctx, long long cap) {
 }
 
 // DCTR_* slots -> host (synchronises the stream)
-void read_dctr(dfgpu_aggstate* st, unsigned long long* host) {
-  dfgpu_ctx* ctx = st->ctx;
-  DF_CUDA(cudaMemcpyAsync(host, st->d_dctr, DCTR_SLOTS * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  DF_CUDA(cudaStreamSynchronize(ctx->stream));
-}
+void read_dctr(dfgpu_aggstate* st, unsigned long long* host) { read_words(st->ctx, st->d_dctr, DCTR_SLOTS * 8, host); }
 
 // Grow set s to new_cap by re-inserting its pairs (their number does not change).
 void set_grow(dfgpu_aggstate* st, int s, long long new_cap) {
@@ -2330,7 +2278,7 @@ long long insert_round(dfgpu_aggstate* st, AggParams& p, bool plain) {
   // A warp reads the fill once per tile and adds its tile's pairs after it, so up to one tile per warp of the grid
   // (grid x AG_TILE pairs per set) is inserted past what the others read: the fill limit is lowered by that much,
   // which keeps every set at most half full.
-  launch(st->ctx, k.fn, k.name, p.row_list ? p.nlist : p.nrows, AG_TILE, 0, 0, PROFILED, [&](int grid) {
+  launch_ag(st->ctx, k.fn, k.name, p.row_list ? p.nlist : p.nrows, AG_TILE, 0, PROFILED, [&](int grid) {
     for (int s = 0; s < nsets; s++) sp.max_fill[s] = std::max<long long>(0, fill_limit(sp.set[s].cap) - (long long)grid * AG_TILE);
   }, p, sp);
   unsigned long long c[DCTR_SLOTS];
@@ -2583,7 +2531,7 @@ long long scan_round(dfgpu_aggstate* st, AggParams& p, const ScanPlan& plan, Tra
   // FRONT launches admit the keys of every CTA's front table unconditionally when the CTA retires, so the fill limit of
   // the global path is lowered by what they can add (grid x front slots): the table stays at most half full and the
   // front merge always finds a slot.
-  launch(ctx, k.fn, k.name, replay ? p.nlist : p.nrows, AG_TILE, 0, smem, PROFILED, [&](int grid) {
+  launch_ag(ctx, k.fn, k.name, replay ? p.nlist : p.nrows, AG_TILE, 0, LaunchOpts{smem, true}, [&](int grid) {
     if (k.front) p.max_groups = std::max<long long>(0, p.max_groups - (long long)grid * AG_FRONT_SLOTS);
   }, p);
   unsigned long long c[CTR_NONNULL];
@@ -2748,15 +2696,17 @@ void agg_exchange_scalars(dfgpu_ctx* ctx, dfgpu_aggstate* st) {
   }
   // per-aggregate non-null input counts travel with the accumulators: fold the host-side counts of the
   // null-free batches into the device counters, which the exchange sums over ranks
-  DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + HS_NONNULL, st->d_counters + CTR_NONNULL, kMaxAggs * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  DF_CUDA(cudaStreamSynchronize(ctx->stream));
+  static_assert(kMaxAggs <= SCR_AGG_NONNULL.words, "a non-null count per aggregate");
+  unsigned long long* nonnull = ctx->h_scratch + SCR_AGG_NONNULL.at;  // pinned: uploaded below
+  unsigned long long* rows = ctx->h_scratch + SCR_AGG_ROWS.at;
+  read_words(ctx, st->d_counters + CTR_NONNULL, kMaxAggs * 8, nonnull);
   for (int a = 0; a < kMaxAggs; a++) {
-    if (a < st->naggs) ctx->h_scratch[HS_NONNULL + a] += (unsigned long long)st->nonnull_host[size_t(a)];
+    if (a < st->naggs) nonnull[a] += (unsigned long long)st->nonnull_host[size_t(a)];
     if (a < st->naggs) st->nonnull_host[size_t(a)] = 0;
   }
-  ctx->h_scratch[HS_ROWS] = (unsigned long long)st->rows_seen;
-  DF_CUDA(cudaMemcpyAsync(st->d_counters + CTR_NONNULL, ctx->h_scratch + HS_NONNULL, kMaxAggs * 8, cudaMemcpyHostToDevice, ctx->stream));
-  DF_CUDA(cudaMemcpyAsync(st->d_counters + CTR_ROWS, ctx->h_scratch + HS_ROWS, 8, cudaMemcpyHostToDevice, ctx->stream));
+  *rows = (unsigned long long)st->rows_seen;
+  DF_CUDA(cudaMemcpyAsync(st->d_counters + CTR_NONNULL, nonnull, kMaxAggs * 8, cudaMemcpyHostToDevice, ctx->stream));
+  DF_CUDA(cudaMemcpyAsync(st->d_counters + CTR_ROWS, rows, 8, cudaMemcpyHostToDevice, ctx->stream));
   st->saw_nulls = true;
   // slot 0's accumulators (cap = 0: every accumulator in its own one-word array, contiguous)
   comm_allreduce_aggs(ctx, st->naggs, funcs, mtypes, st->t.val(0, 0), st->d_counters + CTR_NONNULL, st->d_counters + CTR_ROWS);
@@ -2796,7 +2746,8 @@ void agg_exchange_groups(dfgpu_ctx* ctx, dfgpu_aggstate* st, DevBufs& rows_buf, 
   op.naggs = st->naggs;
   op.counts = d_rec + HDR;
   if (n_local > 0) launch_kernel(ctx, k_owner_count, "k_owner_count", op, n_local, 256 * 4, 8);
-  unsigned long long* hh = ctx->h_scratch + HS_HEADER;  // pinned
+  static_assert(HDR <= SCR_AGG_HEADER.words, "the header record fits its scratch range");
+  unsigned long long* hh = ctx->h_scratch + SCR_AGG_HEADER.at;  // pinned
   memset(hh, 0, HDR * 8);
   hh[0] = st->typed ? 1 : 0;
   hh[1] = (unsigned long long)st->nkeys;
@@ -3007,7 +2958,8 @@ std::unique_ptr<dfgpu_result> finish_regroup(dfgpu_ctx* ctx, dfgpu_aggstate* st)
   const int NH = 1 + kMaxKeys;
   DevBufs tmp(ctx);
   unsigned long long* d_h = tmp.alloc(size_t(NH) * 8 * size_t(W + 1));
-  unsigned long long* hh = ctx->h_scratch + HS_HEADER;
+  static_assert(NH <= SCR_AGG_HEADER.words, "the size record fits its scratch range");
+  unsigned long long* hh = ctx->h_scratch + SCR_AGG_HEADER.at;  // pinned
   memset(hh, 0, size_t(NH) * 8);
   hh[0] = (unsigned long long)local->nrows;
   for (int k = 0; k < st->nkeys; k++)
@@ -3161,9 +3113,8 @@ void assemble_outputs(dfgpu_aggstate* st, dfgpu_result* res) {
     ap.nulls = d_nulls + i;
     launch_kernel(ctx, k_avg_finish, "k_avg_finish", ap, n, 256 * 4, 8);
   }
-  unsigned long long* h = ctx->h_scratch + HS_NONNULL;  // pinned
-  DF_CUDA(cudaMemcpyAsync(h, d_nulls, kMaxAggs * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  DF_CUDA(cudaStreamSynchronize(ctx->stream));
+  unsigned long long h[kMaxAggs];
+  read_words(ctx, d_nulls, sizeof(h), h);
   for (size_t i = 0; i < st->out_word.size(); i++) {
     DevColumn& c = res->cols[nk + i];
     if (!st->out_is_avg[i]) continue;
@@ -3321,9 +3272,9 @@ extern "C" int dfgpu_aggregate_finish(dfgpu_aggstate* st, dfgpu_result** out) {
       // an aggregate that saw no non-null input is null (array_from_scalar!, aggregate.rs:641-643)
       std::vector<long long> nonnull = st->nonnull_host;
       if (st->saw_nulls) {
-        DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + HS_NONNULL, st->d_counters + CTR_NONNULL, kMaxAggs * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        DF_CUDA(cudaStreamSynchronize(ctx->stream));
-        for (int a = 0; a < st->naggs; a++) nonnull[size_t(a)] += (long long)ctx->h_scratch[HS_NONNULL + a];
+        unsigned long long d[kMaxAggs];
+        read_words(ctx, st->d_counters + CTR_NONNULL, sizeof(d), d);
+        for (int a = 0; a < st->naggs; a++) nonnull[size_t(a)] += (long long)d[a];
       }
       std::vector<char> avg_word(size_t(st->naggs), 0);  // an AVG's validity comes from its count word (k_avg_finish)
       for (size_t i = 0; i < st->out_word.size(); i++)

@@ -66,6 +66,34 @@ void trace_launch(const char* kernel) {
   if (getenv("DFGPU_TRACE")) fprintf(stderr, "[dfgpu trace] launch %s\n", kernel);
 }
 
+int grid_for(const dfgpu_ctx* ctx, long long work_items, int per_block, int per_sm) {
+  const long long g = (work_items + per_block - 1) / per_block;
+  return int(std::max(1ll, std::min(g, (long long)ctx->sm_count * per_sm)));
+}
+
+void read_words(dfgpu_ctx* ctx, const void* dev, size_t bytes, void* host) {
+  if (bytes > size_t(SCR_STAGE.words) * 8) fail(DFGPU_ERR_INTERNAL, "read_words: " + std::to_string(bytes) + " bytes exceed the staging range");
+  unsigned long long* stage = ctx->h_scratch + SCR_STAGE.at;
+  DF_CUDA(cudaMemcpyAsync(stage, dev, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  DF_CUDA(cudaStreamSynchronize(ctx->stream));
+  memcpy(host, stage, bytes);
+}
+
+unsigned long long read_word(dfgpu_ctx* ctx, const unsigned long long* dev) {
+  unsigned long long v = 0;
+  read_words(ctx, dev, 8, &v);
+  return v;
+}
+
+void free_column(dfgpu_ctx* ctx, DevColumn& c) {
+  ctx->free(c.values);
+  ctx->free(c.validity);
+  ctx->free(c.offsets);
+  c.values = nullptr;
+  c.validity = nullptr;
+  c.offsets = nullptr;
+}
+
 }  // namespace dfgpu
 
 using namespace dfgpu;
@@ -260,11 +288,7 @@ void resolve(const dfgpu_result* r) {
 dfgpu_batch::~dfgpu_batch() {
   if (!ctx || !owns) return;
   cudaSetDevice(ctx->device);
-  for (auto& c : cols) {
-    ctx->free(c.values);
-    ctx->free(c.validity);
-    ctx->free(c.offsets);
-  }
+  for (auto& c : cols) free_column(ctx, c);
 }
 void* dfgpu_ctx::host_alloc(size_t bytes) {
   if (bytes == 0) bytes = 8;
@@ -294,11 +318,7 @@ dfgpu_result::~dfgpu_result() {
     for (auto& c : cols) ctx->host_release(c.values);
     return;
   }
-  for (auto& c : cols) {
-    ctx->free(c.values);
-    ctx->free(c.validity);
-    ctx->free(c.offsets);
-  }
+  for (auto& c : cols) free_column(ctx, c);
 }
 
 extern "C" int dfgpu_abi_version(void) { return DFGPU_ABI_VERSION; }
@@ -396,9 +416,9 @@ extern "C" int dfgpu_init(int device, dfgpu_ctx** out) {
     DF_CUDA(cudaDeviceGetDefaultMemPool(&pool, device));
     uint64_t thresh = ~0ull;
     DF_CUDA(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thresh));
-    DF_CUDA(cudaMalloc(&ctx->d_scratch, 64 * 8));
-    DF_CUDA(cudaMemset(ctx->d_scratch, 0, 64 * 8));
-    DF_CUDA(cudaMallocHost(&ctx->h_scratch, 64 * 8));
+    DF_CUDA(cudaMalloc(&ctx->d_scratch, kScratchWords * 8));
+    DF_CUDA(cudaMemset(ctx->d_scratch, 0, kScratchWords * 8));
+    DF_CUDA(cudaMallocHost(&ctx->h_scratch, kScratchWords * 8));
     *out = ctx.release();
   });
 }

@@ -74,9 +74,9 @@ struct dfgpu_ctx {
   bool force_direct_kernel = false;  // DFGPU_FP_KERNEL=direct: bypass the TMA pipeline (A/B testing)
   void* flush_buf = nullptr;
   size_t flush_bytes = 0;
-  // device scratch shared by operators (error flags, counters); 64 x u64
+  // scratch words shared by the operators, laid out by the SCR_* ranges below
   unsigned long long* d_scratch = nullptr;
-  unsigned long long* h_scratch = nullptr;  // pinned mirror
+  unsigned long long* h_scratch = nullptr;  // pinned
   // pinned staging ring for uploads from pageable memory
   void* stage[2] = {nullptr, nullptr};
   cudaEvent_t stage_ev[2] = {nullptr, nullptr};
@@ -175,6 +175,83 @@ struct Trace {
 // DFGPU_TRACE: name each kernel as it is launched, template arguments included, so that a run shows which
 // instantiation the dispatch chose (the kernel tests assert it)
 void trace_launch(const char* kernel);
+
+// ceil(work_items / per_block) CTAs, at least 1 and at most per_sm per SM
+int grid_for(const dfgpu_ctx* ctx, long long work_items, int per_block, int per_sm);
+
+struct LaunchOpts {
+  size_t smem = 0;           // dynamic shared memory bytes
+  bool profiled = false;     // timed in the profile ring (dfgpu_profile_get), where the benchmark's kernel times come from
+  bool cooperative = false;  // cudaLaunchCooperativeKernel: every CTA of the grid resident at once
+};
+constexpr LaunchOpts PROFILED{0, true, false};
+
+// Every kernel launch of the library: on ctx->stream, checked, named under DFGPU_TRACE, timed when opts.profiled and
+// counted in ctx->launches (dfgpu_kernel_launches).  The arguments must have the kernel's exact parameter types.
+template <class... P>
+void launch(dfgpu_ctx* ctx, const char* name, void (*kernel)(P...), int grid, int block, const LaunchOpts& opts, const P&... args) {
+  const int ps = opts.profiled ? ctx->prof_begin() : -1;
+  if (opts.cooperative) {
+    void* argv[] = {(void*)&args...};
+    DF_CUDA(cudaLaunchCooperativeKernel((const void*)kernel, dim3(grid), dim3(block), argv, opts.smem, ctx->stream));
+  } else {
+    kernel<<<grid, block, opts.smem, ctx->stream>>>(args...);
+  }
+  DF_CUDA(cudaGetLastError());
+  trace_launch(name);
+  ctx->prof_end(ps);
+  ctx->launches++;
+}
+
+// The words of ctx->h_scratch (pinned) and ctx->d_scratch (device), kScratchWords u64 each, as ranges of one user each,
+// so that no user overwrites words another's copy or kernel may still read.
+struct ScratchRange {
+  int at, words;
+};
+constexpr ScratchRange SCR_FP_ROWS{0, 1};       // filter/project: the row count its kernel writes to h_scratch (zero-copy)
+constexpr ScratchRange SCR_FP_DIV0{1, 1};       // filter/project: its DivideByZero flag, likewise
+constexpr ScratchRange SCR_FP_NULLS{2, 24};     // filter/project: null count per program, in d_scratch, copied to h_scratch
+constexpr ScratchRange SCR_AGG_HEADER{26, 16};  // aggregate: multi-GPU header record, built in h_scratch and uploaded
+constexpr ScratchRange SCR_AGG_NONNULL{42, 8};  // aggregate: the CTR_NONNULL counters, written in h_scratch and uploaded
+constexpr ScratchRange SCR_AGG_ROWS{50, 1};     // aggregate: CTR_ROWS, likewise
+constexpr ScratchRange SCR_STAGE{64, 64};       // read_words: staging of one synchronous read, free again when it returns
+constexpr int kScratchWords = 128;
+constexpr ScratchRange kScratchLayout[] = {SCR_FP_ROWS, SCR_FP_DIV0, SCR_FP_NULLS, SCR_AGG_HEADER, SCR_AGG_NONNULL, SCR_AGG_ROWS, SCR_STAGE};
+constexpr bool scratch_layout_ok() {
+  int end = 0;
+  for (const ScratchRange& r : kScratchLayout) {
+    if (r.at < end || r.words < 1) return false;
+    end = r.at + r.words;
+  }
+  return end <= kScratchWords;
+}
+static_assert(scratch_layout_ok(), "the scratch ranges overlap or overflow the scratch buffers");
+
+// Synchronous device -> host copy of `bytes` (at most SCR_STAGE's) through the pinned staging range: copies on ctx->stream,
+// synchronises it and copies the words out to `host`.
+void read_words(dfgpu_ctx* ctx, const void* dev, size_t bytes, void* host);
+unsigned long long read_word(dfgpu_ctx* ctx, const unsigned long long* dev);
+
+// Device blocks that go back to the ctx pool at scope exit (stream-ordered, see dfgpu_ctx::free).
+struct DevBufs {
+  dfgpu_ctx* ctx;
+  std::vector<void*> blocks;
+  explicit DevBufs(dfgpu_ctx* c) : ctx(c) {}
+  DevBufs(const DevBufs&) = delete;
+  DevBufs& operator=(const DevBufs&) = delete;
+  ~DevBufs() {
+    for (void* q : blocks) ctx->free(q);
+  }
+  template <class T = unsigned long long>
+  T* alloc(size_t bytes) {
+    void* q = ctx->alloc(bytes);
+    blocks.push_back(q);
+    return static_cast<T*>(q);
+  }
+};
+
+// Returns a column's values, validity and offsets to the ctx pool and nulls them.
+void free_column(dfgpu_ctx* ctx, DevColumn& c);
 }  // namespace dfgpu
 
 struct dfgpu_batch {

@@ -182,26 +182,13 @@ __global__ void __launch_bounds__(256) k_pack_bits(const unsigned char* __restri
     if ((threadIdx.x & 31) == 0) words[i >> 5] = m;
   }
 }
-static int grid_for_rows(dfgpu_ctx* ctx, long long rows) {
-  long long g = (rows + 255) / 256;
-  const long long cap = (long long)ctx->sm_count * 8;
-  return int(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 template <int DEPTH, bool NULLS = false>
 static void launch_fp(dfgpu_ctx* ctx, const FPParams& p) {
   int per_sm = 0;
   DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_filter_project<DEPTH, NULLS>, FP_THREADS, 0));
   if (per_sm < 1) per_sm = 1;
-  long long grid = (long long)ctx->sm_count * per_sm;
-  if (grid > p.ntiles) grid = p.ntiles;
-  const int ps = ctx->prof_begin();
-  k_filter_project<DEPTH, NULLS><<<(unsigned)grid, FP_THREADS, 0, ctx->stream>>>(p);
-  DF_CUDA(cudaGetLastError());
   static const std::string name = "k_filter_project<" + depth_arg(DEPTH) + (NULLS ? ", true>" : ", false>");
-  trace_launch(name.c_str());
-  ctx->prof_end(ps);
-  ctx->launches++;
+  launch(ctx, name.c_str(), k_filter_project<DEPTH, NULLS>, grid_for(ctx, p.ntiles, 1, per_sm), FP_THREADS, PROFILED, p);
 }
 
 }  // namespace dfgpu
@@ -388,17 +375,18 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
       p.out_count = ctx->fp_slots[size_t(res->pending)].words;
       p.err_flag = (unsigned*)(p.out_count + 1);
     } else {
-      ctx->h_scratch[0] = 0;
-      ctx->h_scratch[2] = 0;
-      p.out_count = ctx->h_scratch + 0;
-      p.err_flag = (unsigned*)(ctx->h_scratch + 2);
+      p.out_count = ctx->h_scratch + SCR_FP_ROWS.at;
+      p.err_flag = (unsigned*)(ctx->h_scratch + SCR_FP_DIV0.at);
+      *p.out_count = 0;
+      *p.err_flag = 0;
     }
     // validity outputs: only a query WITHOUT a predicate can emit nulls (see k_filter_project)
     memset(p.out_valid, 0, sizeof(p.out_valid));
-    p.null_counts = ctx->d_scratch + 32;
+    static_assert(kMaxProgs <= SCR_FP_NULLS.words, "a null count per program");
+    p.null_counts = ctx->d_scratch + SCR_FP_NULLS.at;
     std::vector<int> valid_of_out(size_t(nproj), -1);  // result column -> kernel program with a validity buffer
     if (p.ps.has_nulls && !has_pred) {
-      DF_CUDA(cudaMemsetAsync(ctx->d_scratch + 32, 0, kMaxProgs * 8, ctx->stream));
+      DF_CUDA(cudaMemsetAsync(p.null_counts, 0, kMaxProgs * 8, ctx->stream));
       for (int i = 0; i < nproj; i++) {
         const int k = out_kind[size_t(i)];
         if (k >= 0 && p.ps.nullable[k]) {
@@ -435,31 +423,28 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
       return;
     }
     if (p.ps.has_nulls && !has_pred)
-      DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 32, ctx->d_scratch + 32, kMaxProgs * 8, cudaMemcpyDeviceToHost, ctx->stream));
+      DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + SCR_FP_NULLS.at, p.null_counts, kMaxProgs * 8, cudaMemcpyDeviceToHost, ctx->stream));
     DF_CUDA(cudaStreamSynchronize(ctx->stream));
     ctx->free(status);
     for (int i = 0; i < nproj; i++) {
       DevColumn& c = res->cols[size_t(i)];
       if (valid_of_out[size_t(i)] >= 0) {
-        c.null_count = (int64_t)ctx->h_scratch[32 + valid_of_out[size_t(i)]];
+        c.null_count = (int64_t)ctx->h_scratch[SCR_FP_NULLS.at + valid_of_out[size_t(i)]];
         if (c.null_count == 0) {
           ctx->free(c.validity);
           c.validity = nullptr;
         }
       }
     }
-    if ((unsigned)ctx->h_scratch[2] != 0) fail(DFGPU_ERR_ARROW, "DivideByZero");
-    res->nrows = has_pred ? (int64_t)ctx->h_scratch[0] : n;
+    if (*p.err_flag != 0) fail(DFGPU_ERR_ARROW, "DivideByZero");
+    res->nrows = has_pred ? (int64_t)*p.out_count : n;
     for (int i = 0; i < nproj; i++)
       if (bool_of_out[size_t(i)] >= 0) {
         DevColumn& c = res->cols[size_t(i)];
         const long long words = (res->nrows + 31) / 32;
-        if (words > 0) {
-          k_pack_bits<<<grid_for_rows(ctx, words * 32), 256, 0, ctx->stream>>>(
-              (const unsigned char*)bool_bytes.cols[size_t(bool_of_out[size_t(i)])].values, res->nrows, (unsigned*)c.values);
-          DF_CUDA(cudaGetLastError());
-          ctx->launches++;
-        }
+        if (words > 0)
+          launch(ctx, "k_pack_bits", k_pack_bits, grid_for(ctx, words * 32, 256, 8), 256, {},
+                 (const unsigned char*)bool_bytes.cols[size_t(bool_of_out[size_t(i)])].values, (long long)res->nrows, (unsigned*)c.values);
         c.values_bytes = size_t(res->nrows + 7) / 8;
         any_utf8 = true;  // synchronise before the byte buffers are released
       }

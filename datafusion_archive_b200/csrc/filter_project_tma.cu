@@ -772,17 +772,11 @@ static void launch_one(dfgpu_ctx* ctx, const FPParams& p, size_t smem) {
   auto kern = k_filter_project_tma<DEPTH, K, F64ONLY, FAST, LEAN>;
   if (ctx->first_use((const void*)kern))
     DF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TM_SMEM_BUDGET + 16384 + TM_HDR_BYTES));
-  long long grid = std::min(ctx->sm_count, TM_MAX_GRID);  // one persistent CTA per SM
-  if (grid > p.ntiles) grid = p.ntiles;
-  const int ps = ctx->prof_begin();
-  // cooperative launch: the wave-synchronous scan needs every CTA of the grid resident at once
-  void* args[] = {(void*)&p};
-  DF_CUDA(cudaLaunchCooperativeKernel((const void*)kern, dim3((unsigned)grid), dim3(TM_THREADS), args, smem, ctx->stream));
+  const int grid = std::min(std::min(ctx->sm_count, TM_MAX_GRID), p.ntiles);  // one persistent CTA per SM
   static const std::string name = "k_filter_project_tma<" + depth_arg(DEPTH) + ", " + std::to_string(K) + (F64ONLY ? ", true" : ", false") +
                                   (FAST ? ", true, " : ", false, ") + std::to_string(LEAN) + ">";
-  trace_launch(name.c_str());
-  ctx->prof_end(ps);
-  ctx->launches++;
+  // cooperative launch: the wave-synchronous scan needs every CTA of the grid resident at once
+  launch(ctx, name.c_str(), kern, grid, TM_THREADS, LaunchOpts{smem, true, true}, p);
 }
 
 template <int DEPTH, int K>

@@ -6,7 +6,7 @@
 //   k_join_build    one thread per row packs the key, claims the key's slot (atomicCAS on the key word, the key equal
 //                   to EMPTY_KEY takes slot cap) and records the row's slot; each warp counts its rows per slot with one
 //                   atomic per distinct slot
-//   scan            the counts of the cap + 1 slots become each slot's start (scan_counts, three launches)
+//   scan            the counts of the cap + 1 slots become each slot's start (scan_exclusive, scan.cuh)
 //   k_join_scatter  every row writes its row number into its slot's range: the build rows of one key are contiguous
 // Probe (dfgpu_join_probe), for n probe rows:
 //   k_join_count    per row: the number of build rows with its key (0 for a null key or a miss) and their start
@@ -38,6 +38,7 @@
 #include <memory>
 
 #include "hash_table.cuh"
+#include "scan.cuh"
 #include "utf8_words.cuh"
 
 namespace dfgpu {
@@ -47,8 +48,6 @@ void gather_utf8(dfgpu_ctx* ctx, const DevColumn& src, const unsigned long long*
 constexpr int kMaxJoinKeys = 4;
 constexpr long long JN_MIN_CAP = 1024;  // the build table never grows: no floor beyond a small minimum
 constexpr int JN_THREADS = 256;
-constexpr int SCAN_ITEMS = 8;
-constexpr int SCAN_TILE = JN_THREADS * SCAN_ITEMS;
 constexpr int EMIT_TILE = 2048;  // output positions per CTA tile of k_join_emit
 
 // The key columns of one input: each part is read as its raw integer, sign- or zero-extended to 64 bits, masked to its
@@ -253,66 +252,6 @@ __global__ void __launch_bounds__(JN_THREADS) k_join_utf8_verify(JoinKeys k, Utf
       if (retry) next[at + (unsigned)__popc(again & ((1u << lane) - 1u))] = (unsigned)r;
     }
   }
-}
-
-// ---- exclusive scan of u32 counts into u64 offsets: out[i] = sum of in[0..i), out[n] = the total ------------------------
-__global__ void __launch_bounds__(JN_THREADS) k_scan_counts(const unsigned* __restrict__ in, long long n, unsigned long long* __restrict__ out,
-                                                           unsigned long long* __restrict__ sums) {
-  __shared__ unsigned long long s_warp[JN_THREADS / 32];
-  const long long base = (long long)blockIdx.x * SCAN_TILE + (long long)threadIdx.x * SCAN_ITEMS;
-  unsigned long long v[SCAN_ITEMS];
-  unsigned long long run = 0;
-#pragma unroll
-  for (int i = 0; i < SCAN_ITEMS; i++) {
-    v[i] = run;  // exclusive within the thread
-    run += base + i < n ? in[base + i] : 0u;
-  }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  unsigned long long incl = run;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const unsigned long long x = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += x;
-  }
-  if (lane == 31) s_warp[warp] = incl;
-  __syncthreads();
-  unsigned long long excl = incl - run;
-  for (int w = 0; w < warp; w++) excl += s_warp[w];
-#pragma unroll
-  for (int i = 0; i < SCAN_ITEMS; i++)
-    if (base + i < n) out[base + i] = v[i] + excl;  // block-local; k_scan_add finishes it
-  if (threadIdx.x == JN_THREADS - 1) sums[blockIdx.x] = excl + run;
-}
-// one CTA: exclusive scan of the nb block totals in place; the grand total goes to *total
-__global__ void __launch_bounds__(1024) k_scan_totals(unsigned long long* __restrict__ sums, long long nb, unsigned long long* __restrict__ total) {
-  __shared__ unsigned long long s_part[1024];
-  const long long per = (nb + 1023) / 1024, lo = (long long)threadIdx.x * per, hi = min(nb, lo + per);
-  unsigned long long acc = 0;
-  for (long long b = lo; b < hi; b++) acc += sums[b];
-  s_part[threadIdx.x] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned long long run = 0;
-    for (int i = 0; i < 1024; i++) {
-      const unsigned long long x = s_part[i];
-      s_part[i] = run;
-      run += x;
-    }
-    *total = run;
-  }
-  __syncthreads();
-  unsigned long long run = s_part[threadIdx.x];
-  for (long long b = lo; b < hi; b++) {
-    const unsigned long long x = sums[b];
-    sums[b] = run;
-    run += x;
-  }
-}
-__global__ void __launch_bounds__(JN_THREADS) k_scan_add(unsigned long long* __restrict__ out, long long n, const unsigned long long* __restrict__ sums) {
-  const unsigned long long add = sums[blockIdx.x];
-  const long long base = (long long)blockIdx.x * SCAN_TILE;
-  for (int i = threadIdx.x; i < SCAN_TILE; i += JN_THREADS)
-    if (base + i < n) out[base + i] += add;
 }
 
 // ---- probe -----------------------------------------------------------------------------------------------------------
@@ -540,54 +479,6 @@ __global__ void __launch_bounds__(JN_THREADS) k_join_widen(const unsigned* __res
 // ---- host side ---------------------------------------------------------------------------------------------------------
 namespace {
 
-int grid_of(dfgpu_ctx* ctx, long long work) {
-  long long g = (work + JN_THREADS - 1) / JN_THREADS;
-  const long long most = (long long)ctx->sm_count * 16;
-  return int(g < 1 ? 1 : (g > most ? most : g));
-}
-
-// every launch: trace, profile ring, launch counter
-template <class Kernel, class... Args>
-void launch(dfgpu_ctx* ctx, const char* name, Kernel kernel, int grid, int block, Args... args) {
-  const int ps = ctx->prof_begin();
-  kernel<<<grid, block, 0, ctx->stream>>>(args...);
-  DF_CUDA(cudaGetLastError());
-  trace_launch(name);
-  ctx->prof_end(ps);
-  ctx->launches++;
-}
-
-// out[0..n] = exclusive scan of in[0..n) with out[n] = the total, which is returned.  Synchronises the stream.
-unsigned long long scan_counts(dfgpu_ctx* ctx, const unsigned* in, long long n, unsigned long long* out) {
-  const long long nb = std::max(1ll, (n + SCAN_TILE - 1) / SCAN_TILE);
-  unsigned long long* sums = (unsigned long long*)ctx->alloc(size_t(nb) * 8);
-  launch(ctx, "k_scan_counts", k_scan_counts, int(nb), JN_THREADS, in, n, out, sums);
-  launch(ctx, "k_scan_totals", k_scan_totals, 1, 1024, sums, nb, out + n);
-  launch(ctx, "k_scan_add", k_scan_add, int(nb), JN_THREADS, out, n, (const unsigned long long*)sums);
-  DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 56, out + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  DF_CUDA(cudaStreamSynchronize(ctx->stream));
-  ctx->free(sums);
-  return ctx->h_scratch[56];
-}
-
-// Device buffers freed at scope exit (stream-ordered, see dfgpu_ctx::free)
-struct Bufs {
-  dfgpu_ctx* ctx;
-  std::vector<void*> blocks;
-  explicit Bufs(dfgpu_ctx* c) : ctx(c) {}
-  Bufs(const Bufs&) = delete;
-  Bufs& operator=(const Bufs&) = delete;
-  ~Bufs() {
-    for (void* q : blocks) ctx->free(q);
-  }
-  template <class T>
-  T* alloc(size_t count) {
-    void* q = ctx->alloc(count * sizeof(T));
-    blocks.push_back(q);
-    return static_cast<T*>(q);
-  }
-};
-
 // The key columns of one batch.  A key program that is a plain column is read in place; any other program is
 // evaluated by the projection operator (no predicate), so its values are exactly the expression VM's.  The integer
 // parts go to `k`, the Utf8 parts to `u` (with their columns in `ucols`), each in key order.
@@ -695,21 +586,21 @@ DevColumn copy_column(dfgpu_ctx* ctx, const DevColumn& s, long long n) {
 }
 
 // Gather one column by a row-index list.  `idx64` is filled on first use (Utf8 columns take 64-bit indices).
-void gather_column(dfgpu_ctx* ctx, const DevColumn& src, const unsigned* idx, long long n, Bufs& scratch, unsigned long long*& idx64,
+void gather_column(dfgpu_ctx* ctx, const DevColumn& src, const unsigned* idx, long long n, DevBufs& scratch, unsigned long long*& idx64,
                    unsigned long long* d_nulls, DevColumn* out) {
   out->dtype = src.dtype;
-  const int grid = grid_of(ctx, n);
+  const int grid = grid_for(ctx, n, JN_THREADS, 16);
   if (src.dtype == DFGPU_UTF8) {
     if (!idx64) {
-      idx64 = scratch.alloc<unsigned long long>(size_t(std::max(1ll, n)));
-      if (n > 0) launch(ctx, "k_join_widen", k_join_widen, grid, JN_THREADS, idx, n, idx64);
+      idx64 = scratch.alloc<unsigned long long>(size_t(std::max(1ll, n)) * sizeof(unsigned long long));
+      if (n > 0) launch(ctx, "k_join_widen", k_join_widen, grid, JN_THREADS, PROFILED, idx, n, idx64);
     }
     gather_utf8(ctx, src, idx64, n, out);
   } else if (src.dtype == DFGPU_BOOL) {
     out->values_bytes = size_t((n + 31) / 32) * 4 + 4;
     out->values = ctx->alloc(out->values_bytes);
     if (n > 0)
-      launch(ctx, "k_join_gather_bits", k_join_gather_bits, grid, JN_THREADS, (const unsigned char*)src.values, idx, n, (unsigned*)out->values,
+      launch(ctx, "k_join_gather_bits", k_join_gather_bits, grid, JN_THREADS, PROFILED, (const unsigned char*)src.values, idx, n, (unsigned*)out->values,
              (unsigned long long*)nullptr);
     out->values_bytes = size_t(n + 7) / 8;
   } else {
@@ -718,20 +609,18 @@ void gather_column(dfgpu_ctx* ctx, const DevColumn& src, const unsigned* idx, lo
     out->values = ctx->alloc(out->values_bytes);
     if (n > 0) {
       switch (w) {
-        case 1: launch(ctx, "k_join_gather<1>", k_join_gather<unsigned char>, grid, JN_THREADS, (const unsigned char*)src.values, idx, n, (unsigned char*)out->values); break;
-        case 2: launch(ctx, "k_join_gather<2>", k_join_gather<unsigned short>, grid, JN_THREADS, (const unsigned short*)src.values, idx, n, (unsigned short*)out->values); break;
-        case 4: launch(ctx, "k_join_gather<4>", k_join_gather<unsigned>, grid, JN_THREADS, (const unsigned*)src.values, idx, n, (unsigned*)out->values); break;
-        default: launch(ctx, "k_join_gather<8>", k_join_gather<unsigned long long>, grid, JN_THREADS, (const unsigned long long*)src.values, idx, n, (unsigned long long*)out->values); break;
+        case 1: launch(ctx, "k_join_gather<1>", k_join_gather<unsigned char>, grid, JN_THREADS, PROFILED, (const unsigned char*)src.values, idx, n, (unsigned char*)out->values); break;
+        case 2: launch(ctx, "k_join_gather<2>", k_join_gather<unsigned short>, grid, JN_THREADS, PROFILED, (const unsigned short*)src.values, idx, n, (unsigned short*)out->values); break;
+        case 4: launch(ctx, "k_join_gather<4>", k_join_gather<unsigned>, grid, JN_THREADS, PROFILED, (const unsigned*)src.values, idx, n, (unsigned*)out->values); break;
+        default: launch(ctx, "k_join_gather<8>", k_join_gather<unsigned long long>, grid, JN_THREADS, PROFILED, (const unsigned long long*)src.values, idx, n, (unsigned long long*)out->values); break;
       }
     }
   }
   if (src.null_count > 0 && src.validity && n > 0) {
     out->validity = (uint8_t*)ctx->alloc(size_t((n + 31) / 32) * 4);
     DF_CUDA(cudaMemsetAsync(d_nulls, 0, 8, ctx->stream));
-    launch(ctx, "k_join_gather_bits", k_join_gather_bits, grid, JN_THREADS, (const unsigned char*)src.validity, idx, n, (unsigned*)out->validity, d_nulls);
-    DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 57, d_nulls, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    DF_CUDA(cudaStreamSynchronize(ctx->stream));
-    out->null_count = (int64_t)ctx->h_scratch[57];
+    launch(ctx, "k_join_gather_bits", k_join_gather_bits, grid, JN_THREADS, PROFILED, (const unsigned char*)src.validity, idx, n, (unsigned*)out->validity, d_nulls);
+    out->null_count = (int64_t)read_word(ctx, d_nulls);
     if (out->null_count == 0) {
       ctx->free(out->validity);
       out->validity = nullptr;
@@ -769,16 +658,8 @@ struct dfgpu_join {
     ctx->free(rows);
     ctx->free(words);
     ctx->free(rep);
-    for (auto& c : ukeys) {
-      ctx->free(c.values);
-      ctx->free(c.validity);
-      ctx->free(c.offsets);
-    }
-    for (auto& c : cols) {
-      ctx->free(c.values);
-      ctx->free(c.validity);
-      ctx->free(c.offsets);
-    }
+    for (auto& c : ukeys) free_column(ctx, c);
+    for (auto& c : cols) free_column(ctx, c);
   }
 };
 
@@ -786,7 +667,7 @@ struct dfgpu_join {
 // placed, leaving each slot's row count in `counts` and each row's slot in `row_slot`, as k_join_build does.  Each
 // round seals at least one slot, the one of its smallest pending row.  Keeps a copy of the Utf8 key columns for the
 // probe's confirmation.
-static void build_utf8(dfgpu_ctx* ctx, const KeyColumns& kc, long long n, dfgpu_join* j, Bufs& scratch, unsigned* counts,
+static void build_utf8(dfgpu_ctx* ctx, const KeyColumns& kc, long long n, dfgpu_join* j, DevBufs& scratch, unsigned* counts,
                        unsigned long long* row_slot) {
   const long long cap = j->t.cap;
   j->words = (unsigned long long*)ctx->alloc(size_t(cap) * 8);
@@ -795,22 +676,20 @@ static void build_utf8(dfgpu_ctx* ctx, const KeyColumns& kc, long long n, dfgpu_
   DF_CUDA(cudaMemsetAsync(j->rep, 0xff, size_t(cap) * 4, ctx->stream));
   if (n == 0) return;
   unsigned char* sealed = scratch.alloc<unsigned char>(size_t(cap));
-  unsigned long long* d_next = scratch.alloc<unsigned long long>(1);
-  unsigned* lists[2] = {scratch.alloc<unsigned>(size_t(n)), nullptr};
+  unsigned long long* d_next = scratch.alloc<unsigned long long>(sizeof(unsigned long long));
+  unsigned* lists[2] = {scratch.alloc<unsigned>(size_t(n) * sizeof(unsigned)), nullptr};
   DF_CUDA(cudaMemsetAsync(sealed, 0, size_t(cap), ctx->stream));
   const unsigned* list = nullptr;  // the first round takes every row
   long long pending = n;
   for (int round = 0;; round++) {
     unsigned* next = lists[round & 1];
-    if (!next) next = lists[1] = scratch.alloc<unsigned>(size_t(n));
+    if (!next) next = lists[1] = scratch.alloc<unsigned>(size_t(n) * sizeof(unsigned));
     DF_CUDA(cudaMemsetAsync(d_next, 0, 8, ctx->stream));
-    launch(ctx, "k_join_utf8_place", k_join_utf8_place, grid_of(ctx, pending), JN_THREADS, kc.k, kc.u, j->tag_mask, list, pending, (ProbeRule)j->t,
+    launch(ctx, "k_join_utf8_place", k_join_utf8_place, grid_for(ctx, pending, JN_THREADS, 16), JN_THREADS, PROFILED, kc.k, kc.u, j->tag_mask, list, pending, (ProbeRule)j->t,
            j->keys, (const unsigned char*)sealed, j->rep, row_slot);
-    launch(ctx, "k_join_utf8_verify", k_join_utf8_verify, grid_of(ctx, pending), JN_THREADS, kc.k, kc.u, list, pending, (const unsigned*)j->rep,
+    launch(ctx, "k_join_utf8_verify", k_join_utf8_verify, grid_for(ctx, pending, JN_THREADS, 16), JN_THREADS, PROFILED, kc.k, kc.u, list, pending, (const unsigned*)j->rep,
            sealed, j->words, (const unsigned long long*)row_slot, counts, next, d_next);
-    DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 58, d_next, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    DF_CUDA(cudaStreamSynchronize(ctx->stream));
-    const long long left = (long long)ctx->h_scratch[58];
+    const long long left = (long long)read_word(ctx, d_next);
     if (left == 0) return;
     if (left >= pending) fail(DFGPU_ERR_INTERNAL, "JOIN build: a Utf8 key round placed no row");
     list = next;
@@ -839,20 +718,20 @@ extern "C" int dfgpu_join_build(dfgpu_ctx* ctx, const dfgpu_batch* build, const 
     j->keys = (unsigned long long*)ctx->alloc(size_t(cap + 1) * 8);
     j->start = (unsigned long long*)ctx->alloc(size_t(cap + 2) * 8);
     j->rows = (unsigned*)ctx->alloc(size_t(std::max(1ll, n)) * 4);
-    Bufs scratch(ctx);
-    unsigned* counts = scratch.alloc<unsigned>(size_t(cap + 1));
-    unsigned long long* row_slot = scratch.alloc<unsigned long long>(size_t(std::max(1ll, n)));
+    DevBufs scratch(ctx);
+    unsigned* counts = scratch.alloc<unsigned>(size_t(cap + 1) * sizeof(unsigned));
+    unsigned long long* row_slot = scratch.alloc<unsigned long long>(size_t(std::max(1ll, n)) * sizeof(unsigned long long));
     DF_CUDA(cudaMemsetAsync(j->keys, 0xff, size_t(cap + 1) * 8, ctx->stream));
     DF_CUDA(cudaMemsetAsync(counts, 0, size_t(cap + 1) * 4, ctx->stream));
     if (kc.u.n == 0) {
-      if (n > 0) launch(ctx, "k_join_build", k_join_build, grid_of(ctx, n), JN_THREADS, kc.k, n, (ProbeRule)j->t, j->keys, counts, row_slot);
+      if (n > 0) launch(ctx, "k_join_build", k_join_build, grid_for(ctx, n, JN_THREADS, 16), JN_THREADS, PROFILED, kc.k, n, (ProbeRule)j->t, j->keys, counts, row_slot);
     } else {
       j->tag_mask = join_tag_mask();
       build_utf8(ctx, kc, n, j.get(), scratch, counts, row_slot);
     }
-    j->null_rows = n - (long long)scan_counts(ctx, counts, cap + 1, j->start);  // start[cap + 1]: the rows with a key
+    j->null_rows = n - (long long)scan_exclusive<unsigned, unsigned long long>(ctx, counts, j->start, cap + 1, true);  // start[cap + 1]: the rows with a key
     if (n > 0)
-      launch(ctx, "k_join_scatter", k_join_scatter, grid_of(ctx, n), JN_THREADS, (const unsigned long long*)row_slot, n,
+      launch(ctx, "k_join_scatter", k_join_scatter, grid_for(ctx, n, JN_THREADS, 16), JN_THREADS, PROFILED, (const unsigned long long*)row_slot, n,
              (const unsigned long long*)j->start, counts, j->rows);
     // the join's own copy of the kept columns: the caller may free the batch
     for (int i = 0; i < n_keep; i++) {
@@ -887,12 +766,12 @@ extern "C" int dfgpu_join_probe(dfgpu_join* j, const dfgpu_batch* probe, const d
     for (int i = 0; i < nkeys; i++)
       if (kc.dtypes[i] != j->key_dtypes[i])
         fail(DFGPU_ERR_EXECUTION, std::string("JOIN key types differ: ") + dtype_name(kc.dtypes[i]) + " and " + dtype_name(j->key_dtypes[i]));
-    Bufs scratch(ctx);
-    unsigned* cnt = scratch.alloc<unsigned>(size_t(std::max(1ll, n)));
-    unsigned* bpos = scratch.alloc<unsigned>(size_t(std::max(1ll, n)));
-    unsigned long long* off = scratch.alloc<unsigned long long>(size_t(n + 1));
+    DevBufs scratch(ctx);
+    unsigned* cnt = scratch.alloc<unsigned>(size_t(std::max(1ll, n)) * sizeof(unsigned));
+    unsigned* bpos = scratch.alloc<unsigned>(size_t(std::max(1ll, n)) * sizeof(unsigned));
+    unsigned long long* off = scratch.alloc<unsigned long long>(size_t(n + 1) * sizeof(unsigned long long));
     if (n > 0 && kc.u.n == 0)
-      launch(ctx, "k_join_count", k_join_count, grid_of(ctx, n), JN_THREADS, kc.k, n, (ProbeRule)j->t, (const unsigned long long*)j->keys,
+      launch(ctx, "k_join_count", k_join_count, grid_for(ctx, n, JN_THREADS, 16), JN_THREADS, PROFILED, kc.k, n, (ProbeRule)j->t, (const unsigned long long*)j->keys,
              (const unsigned long long*)j->start, cnt, bpos);
     if (n > 0 && kc.u.n > 0) {
       Utf8Keys b{};
@@ -901,25 +780,24 @@ extern "C" int dfgpu_join_probe(dfgpu_join* j, const dfgpu_batch* probe, const d
         b.bytes[b.n] = (const unsigned char*)c.values;
         b.n++;
       }
-      launch(ctx, "k_join_utf8_count", k_join_utf8_count, grid_of(ctx, n), JN_THREADS, kc.k, kc.u, j->tag_mask, n, (ProbeRule)j->t,
+      launch(ctx, "k_join_utf8_count", k_join_utf8_count, grid_for(ctx, n, JN_THREADS, 16), JN_THREADS, PROFILED, kc.k, kc.u, j->tag_mask, n, (ProbeRule)j->t,
              (const unsigned long long*)j->keys, (const unsigned long long*)j->words, (const unsigned*)j->rep, b, (const unsigned long long*)j->start,
              cnt, bpos);
     }
-    const unsigned long long total = n > 0 ? scan_counts(ctx, cnt, n, off) : 0ull;
+    const unsigned long long total = n > 0 ? scan_exclusive<unsigned, unsigned long long>(ctx, cnt, off, n, true) : 0ull;
     if (total >= (1ull << 32)) fail(DFGPU_ERR_NOT_IMPLEMENTED, "JOIN probe batch producing 2^32 or more output rows");
     const long long m = (long long)total;
-    unsigned* pidx = scratch.alloc<unsigned>(size_t(std::max(1ll, m)));
-    unsigned* bidx = scratch.alloc<unsigned>(size_t(std::max(1ll, m)));
+    unsigned* pidx = scratch.alloc<unsigned>(size_t(std::max(1ll, m)) * sizeof(unsigned));
+    unsigned* bidx = scratch.alloc<unsigned>(size_t(std::max(1ll, m)) * sizeof(unsigned));
     if (m > 0) {
-      const long long tiles = (m + EMIT_TILE - 1) / EMIT_TILE;
-      const int grid = int(std::min<long long>(tiles, (long long)ctx->sm_count * 8));
-      launch(ctx, "k_join_emit", k_join_emit, grid, JN_THREADS, (const unsigned long long*)off, n, (const unsigned*)bpos, (const unsigned*)j->rows,
+      const int grid = grid_for(ctx, m, EMIT_TILE, 8);
+      launch(ctx, "k_join_emit", k_join_emit, grid, JN_THREADS, PROFILED, (const unsigned long long*)off, n, (const unsigned*)bpos, (const unsigned*)j->rows,
              total, pidx, bidx);
     }
     auto res = std::make_unique<dfgpu_result>();
     res->ctx = ctx;
     res->nrows = m;
-    unsigned long long* d_nulls = scratch.alloc<unsigned long long>(1);
+    unsigned long long* d_nulls = scratch.alloc<unsigned long long>(sizeof(unsigned long long));
     unsigned long long *p64 = nullptr, *b64 = nullptr;
     for (int i = 0; i < n_probe_cols; i++) {
       res->cols.emplace_back();
@@ -957,17 +835,17 @@ extern "C" int dfgpu_join_semi(dfgpu_join* j, const dfgpu_batch* probe, const df
     const bool none = kind == DFGPU_JOIN_ANTI_NULL_AWARE && j->null_rows > 0;
     const int anti = kind != DFGPU_JOIN_SEMI;
     const int null_pass = kind == DFGPU_JOIN_ANTI || (kind == DFGPU_JOIN_ANTI_NULL_AWARE && j->nrows == 0);
-    Bufs scratch(ctx);
+    DevBufs scratch(ctx);
     const long long ntiles = (n + MARK_TILE - 1) / MARK_TILE;
     long long m = 0;
     unsigned* idx = nullptr;
     if (n > 0 && !none) {
-      unsigned* mask = scratch.alloc<unsigned>(size_t(ntiles) * MARK_WORDS);
-      unsigned* tile_cnt = scratch.alloc<unsigned>(size_t(ntiles));
-      unsigned long long* tile_off = scratch.alloc<unsigned long long>(size_t(ntiles + 1));
-      const int grid = int(std::min<long long>(ntiles, (long long)ctx->sm_count * 8));
+      unsigned* mask = scratch.alloc<unsigned>(size_t(ntiles) * MARK_WORDS * sizeof(unsigned));
+      unsigned* tile_cnt = scratch.alloc<unsigned>(size_t(ntiles) * sizeof(unsigned));
+      unsigned long long* tile_off = scratch.alloc<unsigned long long>(size_t(ntiles + 1) * sizeof(unsigned long long));
+      const int grid = grid_for(ctx, n, MARK_TILE, 8);
       if (kc.u.n == 0) {
-        launch(ctx, "k_join_mark", k_join_mark, grid, JN_THREADS, kc.k, n, (ProbeRule)j->t, (const unsigned long long*)j->keys,
+        launch(ctx, "k_join_mark", k_join_mark, grid, JN_THREADS, PROFILED, kc.k, n, (ProbeRule)j->t, (const unsigned long long*)j->keys,
                (const unsigned long long*)j->start, anti, null_pass, mask, tile_cnt);
       } else {
         Utf8Keys b{};
@@ -976,18 +854,18 @@ extern "C" int dfgpu_join_semi(dfgpu_join* j, const dfgpu_batch* probe, const df
           b.bytes[b.n] = (const unsigned char*)c.values;
           b.n++;
         }
-        launch(ctx, "k_join_utf8_mark", k_join_utf8_mark, grid, JN_THREADS, kc.k, kc.u, j->tag_mask, n, (ProbeRule)j->t,
+        launch(ctx, "k_join_utf8_mark", k_join_utf8_mark, grid, JN_THREADS, PROFILED, kc.k, kc.u, j->tag_mask, n, (ProbeRule)j->t,
                (const unsigned long long*)j->keys, (const unsigned long long*)j->words, (const unsigned*)j->rep, b, anti, null_pass, mask, tile_cnt);
       }
-      m = (long long)scan_counts(ctx, tile_cnt, ntiles, tile_off);
-      idx = scratch.alloc<unsigned>(size_t(std::max(1ll, m)));
+      m = (long long)scan_exclusive<unsigned, unsigned long long>(ctx, tile_cnt, tile_off, ntiles, true);
+      idx = scratch.alloc<unsigned>(size_t(std::max(1ll, m)) * sizeof(unsigned));
       if (m > 0)
-        launch(ctx, "k_join_select", k_join_select, grid, JN_THREADS, (const unsigned*)mask, ntiles, (const unsigned long long*)tile_off, idx);
+        launch(ctx, "k_join_select", k_join_select, grid, JN_THREADS, PROFILED, (const unsigned*)mask, ntiles, (const unsigned long long*)tile_off, idx);
     }
     auto res = std::make_unique<dfgpu_result>();
     res->ctx = ctx;
     res->nrows = m;
-    unsigned long long* d_nulls = scratch.alloc<unsigned long long>(1);
+    unsigned long long* d_nulls = scratch.alloc<unsigned long long>(sizeof(unsigned long long));
     unsigned long long* idx64 = nullptr;
     for (int i = 0; i < n_probe_cols; i++) {
       res->cols.emplace_back();

@@ -6,7 +6,7 @@
 // depth is one pass over each string.  Evaluation:
 //   - k_utf8_view_len, one thread per row, resolves [b, e) and writes the Int64 result (length, octet_length), or the
 //     output length and b.  octet_length of a bare column reads the offsets only.
-//   - The lengths become offsets by the Utf8 gather's scan (scan_utf8_lengths, utf8_gather.cu).
+//   - The lengths become offsets by the Utf8 gather's scan (lengths_to_offsets, utf8_gather.cu).
 //   - k_utf8_view_copy, one warp per row like k_utf8_copy, copies [b, e) with the case map applied.  A view that only
 //     changes the case of every row of a column without nulls takes the source's offsets, rebased to 0, and skips the
 //     length pass and the scan.
@@ -23,7 +23,7 @@
 
 namespace dfgpu {
 
-long long scan_utf8_lengths(dfgpu_ctx* ctx, int* offsets, long long n);
+long long lengths_to_offsets(dfgpu_ctx* ctx, int* offsets, long long n);
 void shift_copy_i32(dfgpu_ctx* ctx, int* dst, const int* src, long long n, int add);
 
 namespace {
@@ -111,7 +111,7 @@ struct ViewParams {
   const unsigned long long* rows;  // the rows to evaluate, or null: rows 0 .. n-1
   long long n;
   long long* out_int;              // Int64 result per row, or null
-  int* out_len;                    // else: the length of row i at out_len[1 + i] ...
+  int* out_len;                    // else: the length of row i at out_len[i] ...
   int* begin;                      // ... and its first source byte at begin[i]
   Utf8ViewSpec spec;
 };
@@ -128,7 +128,7 @@ __global__ void __launch_bounds__(UF_THREADS) k_utf8_view_len(const __grid_const
     if (p.out_int) {
       p.out_int[i] = p.spec.result == DFGPU_UTF8FN_OCTET_LENGTH ? e - b : count_chars_words(p.bytes, b, e);
     } else {
-      p.out_len[i + 1] = e - b;
+      p.out_len[i] = e - b;
       p.begin[i] = b;
     }
   }
@@ -156,17 +156,6 @@ __global__ void __launch_bounds__(UF_THREADS) k_utf8_view_copy(const __grid_cons
   }
 }
 
-template <class K, class P>
-void launch_view(dfgpu_ctx* ctx, K kernel, const P& p, long long threads, const char* name) {
-  const int grid = (int)std::max<long long>(1, std::min<long long>((threads + UF_THREADS - 1) / UF_THREADS, (long long)ctx->sm_count * 16));
-  const int ps = ctx->prof_begin();
-  kernel<<<grid, UF_THREADS, 0, ctx->stream>>>(p);
-  DF_CUDA(cudaGetLastError());
-  trace_launch(name);
-  ctx->prof_end(ps);
-  ctx->launches++;
-}
-
 // Evaluate `spec` over rows[0..n) of `src` (rows 0..n-1 when `rows` is null): the Int64 results into out_int, or else the
 // Utf8 column into *out (offsets and bytes allocated here; validity is the caller's)
 void eval_view(dfgpu_ctx* ctx, const DevColumn& src, const Utf8ViewSpec& spec, const unsigned long long* rows, long long n,
@@ -182,38 +171,29 @@ void eval_view(dfgpu_ctx* ctx, const DevColumn& src, const Utf8ViewSpec& spec, c
   p.spec = spec;
   if (out_int) {
     p.out_int = out_int;
-    if (n > 0) launch_view(ctx, k_utf8_view_len, p, n, "k_utf8_view_len");
+    if (n > 0) launch(ctx, "k_utf8_view_len", k_utf8_view_len, grid_for(ctx, n, UF_THREADS, 16), UF_THREADS, PROFILED, p);
     return;
   }
   out->dtype = DFGPU_UTF8;
   out->offsets = (int32_t*)ctx->alloc(size_t(n + 1) * 4);
   long long total = 0;
   int* begin = nullptr;
-  struct Scratch {
-    dfgpu_ctx* ctx;
-    void* p;
-    ~Scratch() { ctx->free(p); }
-  } scratch{ctx, nullptr};
+  DevBufs scratch(ctx);
   if (n > 0 && spec.nsteps == 0 && !rows && !p.valid) {
     // only the case changes: the source's ranges, rebased to 0
-    DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 24, src.offsets, 4, cudaMemcpyDeviceToHost, ctx->stream));
-    DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + 25, src.offsets + n, 4, cudaMemcpyDeviceToHost, ctx->stream));
-    DF_CUDA(cudaStreamSynchronize(ctx->stream));
     int lo, hi;
-    memcpy(&lo, ctx->h_scratch + 24, 4);
-    memcpy(&hi, ctx->h_scratch + 25, 4);
+    read_words(ctx, src.offsets, 4, &lo);
+    read_words(ctx, src.offsets + n, 4, &hi);
     shift_copy_i32(ctx, out->offsets, src.offsets, n + 1, -lo);
     total = (long long)hi - lo;
+  } else if (n > 0) {
+    begin = scratch.alloc<int>(size_t(n) * 4);
+    p.out_len = out->offsets;
+    p.begin = begin;
+    launch(ctx, "k_utf8_view_len", k_utf8_view_len, grid_for(ctx, n, UF_THREADS, 16), UF_THREADS, PROFILED, p);
+    total = lengths_to_offsets(ctx, out->offsets, n);  // refuses more than 2 GiB
   } else {
     DF_CUDA(cudaMemsetAsync(out->offsets, 0, 4, ctx->stream));
-    if (n > 0) {
-      begin = (int*)ctx->alloc(size_t(n) * 4);
-      scratch.p = begin;
-      p.out_len = out->offsets;
-      p.begin = begin;
-      launch_view(ctx, k_utf8_view_len, p, n, "k_utf8_view_len");
-      total = scan_utf8_lengths(ctx, out->offsets, n);  // refuses more than 2 GiB
-    }
   }
   out->values_bytes = size_t(total);
   out->values = ctx->alloc(std::max<size_t>(16, (size_t(total) + 15) & ~size_t(15)));  // whole 16-byte words
@@ -226,7 +206,7 @@ void eval_view(dfgpu_ctx* ctx, const DevColumn& src, const Utf8ViewSpec& spec, c
     c.n = n;
     c.out = (unsigned char*)out->values;
     c.case_map = spec.case_map;
-    launch_view(ctx, k_utf8_view_copy, c, n * 32, "k_utf8_view_copy");
+    launch(ctx, "k_utf8_view_copy", k_utf8_view_copy, grid_for(ctx, n * 32, UF_THREADS, 16), UF_THREADS, PROFILED, c);
   }
 }
 

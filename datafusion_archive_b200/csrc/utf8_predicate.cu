@@ -249,18 +249,6 @@ __global__ void __launch_bounds__(UP_THREADS) k_utf8_like(const __grid_constant_
   });
 }
 
-template <class K>
-void launch_pred(dfgpu_ctx* ctx, K kernel, const Utf8PredParams& p, const std::string& name) {
-  const long long warps = (p.n + 31) / 32;
-  const int grid = (int)std::max<long long>(1, std::min<long long>((warps + UP_THREADS / 32 - 1) / (UP_THREADS / 32), (long long)ctx->sm_count * 16));
-  const int ps = ctx->prof_begin();
-  kernel<<<grid, UP_THREADS, 0, ctx->stream>>>(p);
-  DF_CUDA(cudaGetLastError());
-  trace_launch(name.c_str());
-  ctx->prof_end(ps);
-  ctx->launches++;
-}
-
 const char* cmp_name(int op) {
   switch (op) {
     case DFGPU_OP_LT: return "lt";
@@ -311,22 +299,23 @@ void ProgramBuilder::eval_utf8_predicates(dfgpu_ctx* ctx) {
       if (!lp.lit.empty()) DF_CUDA(cudaMemcpyAsync(d, lp.lit.data(), lp.lit.size(), cudaMemcpyHostToDevice, ctx->stream));
       p.lit = d;
     }
+    const int grid = grid_for(ctx, n, UP_THREADS, 16);
     if (like && lp.cls != LIKE_EXACT) {
       const std::string name = std::string("k_utf8_like<") + kLikeClassName[lp.cls] + ">";
       switch (lp.cls) {
-        case LIKE_PREFIX: launch_pred(ctx, k_utf8_like<LIKE_PREFIX>, p, name); break;
-        case LIKE_SUFFIX: launch_pred(ctx, k_utf8_like<LIKE_SUFFIX>, p, name); break;
-        case LIKE_CONTAINS: launch_pred(ctx, k_utf8_like<LIKE_CONTAINS>, p, name); break;
-        default: launch_pred(ctx, k_utf8_like<LIKE_GENERAL>, p, name); break;
+        case LIKE_PREFIX: launch(ctx, name.c_str(), k_utf8_like<LIKE_PREFIX>, grid, UP_THREADS, PROFILED, p); break;
+        case LIKE_SUFFIX: launch(ctx, name.c_str(), k_utf8_like<LIKE_SUFFIX>, grid, UP_THREADS, PROFILED, p); break;
+        case LIKE_CONTAINS: launch(ctx, name.c_str(), k_utf8_like<LIKE_CONTAINS>, grid, UP_THREADS, PROFILED, p); break;
+        default: launch(ctx, name.c_str(), k_utf8_like<LIKE_GENERAL>, grid, UP_THREADS, PROFILED, p); break;
       }
     } else if (like || sp.op == DFGPU_OP_EQ || sp.op == DFGPU_OP_NE) {
       const std::string name = std::string("k_utf8_cmp<eq, ") + (rcol ? "col>" : "lit>");
-      if (rcol) launch_pred(ctx, k_utf8_cmp<false, true>, p, name);
-      else launch_pred(ctx, k_utf8_cmp<false, false>, p, name);
+      if (rcol) launch(ctx, name.c_str(), k_utf8_cmp<false, true>, grid, UP_THREADS, PROFILED, p);
+      else launch(ctx, name.c_str(), k_utf8_cmp<false, false>, grid, UP_THREADS, PROFILED, p);
     } else {
       const std::string name = std::string("k_utf8_cmp<") + cmp_name(sp.op) + ", " + (rcol ? "col>" : "lit>");
-      if (rcol) launch_pred(ctx, k_utf8_cmp<true, true>, p, name);
-      else launch_pred(ctx, k_utf8_cmp<true, false>, p, name);
+      if (rcol) launch(ctx, name.c_str(), k_utf8_cmp<true, true>, grid, UP_THREADS, PROFILED, p);
+      else launch(ctx, name.c_str(), k_utf8_cmp<true, false>, grid, UP_THREADS, PROFILED, p);
     }
   }
 }

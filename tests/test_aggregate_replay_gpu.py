@@ -6,10 +6,6 @@ runs the updates of an aggregate under DFGPU_TRACE, compares the kernels they la
 operator produces for that input, and checks the result against numpy.  Every input is far from the fill limits it meets,
 so the number of replay rounds does not depend on how the CTAs of a launch interleave."""
 import ctypes as C
-import os
-import re
-import sys
-import tempfile
 
 import numpy as np
 import pytest
@@ -17,6 +13,7 @@ import pytest
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine
 from datafusion_archive_b200.expr import AggregateFunction, col
+from kernel_trace import traced
 
 pytestmark = pytest.mark.gpu
 
@@ -26,29 +23,6 @@ def ctx():
     c = engine.GpuContext(0)
     yield c
     c.close()
-
-
-def launched(fn):
-    """The names of the kernels launched while fn() ran, in launch order.  Under DFGPU_TRACE the library names every
-    kernel it launches on stderr; file descriptor 2 is redirected to a temporary file meanwhile."""
-    sys.stderr.flush()
-    saved = os.dup(2)
-    old_env = os.environ.get("DFGPU_TRACE")
-    with tempfile.TemporaryFile() as f:
-        os.dup2(f.fileno(), 2)
-        os.environ["DFGPU_TRACE"] = "1"
-        try:
-            fn()
-        finally:
-            os.dup2(saved, 2)
-            os.close(saved)
-            if old_env is None:
-                del os.environ["DFGPU_TRACE"]
-            else:
-                os.environ["DFGPU_TRACE"] = old_env
-        f.seek(0)
-        text = f.read().decode(errors="replace")
-    return re.findall(r"\[dfgpu trace\] launch (k_\w+(?:<[^>]*>)?)", text)
 
 
 def aggregate(ctx, arrays, keys, aggs, expected_groups=0, batches=1):
@@ -64,7 +38,7 @@ def aggregate(ctx, arrays, keys, aggs, expected_groups=0, batches=1):
         def update():
             for b in bs:
                 engine.check(engine.lib().dfgpu_aggregate_update(st, b.h))
-        names = launched(update)
+        _, names = traced(update)
         out = C.c_void_p()
         engine.check(engine.lib().dfgpu_aggregate_finish(st, C.byref(out)))
         r = engine.Result(ctx, out)

@@ -20,7 +20,8 @@ import groupby_ref as R
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
 from datafusion_archive_b200.expr import AggregateFunction, col, lit
-from test_cast_gpu import assert_same, launched, sql_batches, traced
+from kernel_trace import traced_set as traced
+from test_cast_gpu import assert_same, launched, sql_batches
 
 pytestmark = pytest.mark.gpu
 

@@ -3,9 +3,6 @@ so results must equal the numpy reference (f64 sum of the non-null values / thei
 compared with math.fsum at rtol 1e-12.  Under DFGPU_TRACE each dispatch case asserts the kernel that ran."""
 import math
 import os
-import re
-import sys
-import tempfile
 
 import numpy as np
 import pyarrow as pa
@@ -14,6 +11,7 @@ import pytest
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
 from datafusion_archive_b200.expr import AggregateFunction, col, lit
+from kernel_trace import traced_set as traced
 
 pytestmark = pytest.mark.gpu
 
@@ -31,36 +29,6 @@ def ctx():
 
 def avg(arg):
     return AggregateFunction("avg", arg)
-
-
-def canon(name):
-    """`k_hash_agg<8, false, true>` -> `k_hash_agg<8,0,1>`."""
-    m = re.match(r"(k_\w+)(<[^>]*>)?", name)
-    args = re.sub(r"\s", "", m.group(2) or "")
-    return m.group(1) + args.replace("true", "1").replace("false", "0")
-
-
-def traced(fn):
-    """(fn(), set of canonical names of the kernels launched while it ran).  Under DFGPU_TRACE the library names
-    every aggregate kernel it launches on stderr; file descriptor 2 is redirected to a temporary file meanwhile."""
-    sys.stderr.flush()
-    saved = os.dup(2)
-    old_env = os.environ.get("DFGPU_TRACE")
-    with tempfile.TemporaryFile() as f:
-        os.dup2(f.fileno(), 2)
-        os.environ["DFGPU_TRACE"] = "1"
-        try:
-            out = fn()
-        finally:
-            os.dup2(saved, 2)
-            os.close(saved)
-            if old_env is None:
-                del os.environ["DFGPU_TRACE"]
-            else:
-                os.environ["DFGPU_TRACE"] = old_env
-        f.seek(0)
-        text = f.read().decode(errors="replace")
-    return out, {canon(m) for m in re.findall(r"\[dfgpu trace\] launch (k_\w+(?:<[^>]*>)?)", text)}
 
 
 def gpu(ctx, batches, keys, aggs, pred=None, expected=0):

@@ -5,16 +5,13 @@ the SQL planner's implicit coercions.
 
 Bit for bit unless noted; NaNs compare as a class.  Each ABI case runs with DFGPU_TRACE set and asserts the kernel it
 is about, so a case cannot silently land on another instantiation."""
-import os
-import re
-import sys
-import tempfile
 
 import numpy as np
 import pytest
 
 import cast_ref as CR
 import groupby_ref as R
+from kernel_trace import traced_set as traced
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
 from datafusion_archive_b200.expr import AggregateFunction, col, lit, utf8_fn
@@ -36,30 +33,6 @@ def ctx():
     c = engine.GpuContext(0)
     yield c
     c.close()
-
-
-def traced(fn):
-    """(fn(), set of canonical kernel names launched while it ran: `k_x<8, true>` -> `k_x<8,1>`).  Under DFGPU_TRACE
-    the library names every kernel it launches on stderr; file descriptor 2 goes to a temporary file meanwhile."""
-    sys.stderr.flush()
-    saved = os.dup(2)
-    old = os.environ.get("DFGPU_TRACE")
-    with tempfile.TemporaryFile() as f:
-        os.dup2(f.fileno(), 2)
-        os.environ["DFGPU_TRACE"] = "1"
-        try:
-            out = fn()
-        finally:
-            os.dup2(saved, 2)
-            os.close(saved)
-            if old is None:
-                del os.environ["DFGPU_TRACE"]
-            else:
-                os.environ["DFGPU_TRACE"] = old
-        f.seek(0)
-        text = f.read().decode(errors="replace")
-    names = re.findall(r"\[dfgpu trace\] launch (k_\w+(?:<[^>]*>)?)", text)
-    return out, {re.sub(r"\s", "", m).replace("true", "1").replace("false", "0") for m in names}
 
 
 def launched(names, want):

@@ -4,7 +4,6 @@ Each case runs with DFGPU_TRACE set, reads the names of the kernels the library 
 `k_filter_project_tma<DEPTH, K, F64ONLY, FAST, LEAN>` or `k_filter_project<DEPTH, NULLS>` it expects, so a change in
 how expression shapes are recognised cannot silently move a query onto another kernel.  K follows from the bytes
 per row the predicate and the projections read (DESIGN §4.2): 8 rows per lane up to 16 bytes, 4 up to 32."""
-import re
 
 import numpy as np
 import pytest
@@ -12,6 +11,7 @@ import pytest
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine
 from datafusion_archive_b200.expr import col, lit
+from kernel_trace import capfd_launched
 
 pytestmark = pytest.mark.gpu
 
@@ -29,14 +29,7 @@ def ctx():
 def launched(monkeypatch, capfd):
     """Returns a function that yields the canonical names of the kernels launched since the last call:
     `k_filter_project_tma<1, 8, true, true, 1>` -> `k_filter_project_tma<1,8,1,1,1>`."""
-    monkeypatch.setenv("DFGPU_TRACE", "1")
-    capfd.readouterr()
-
-    def names():
-        text = capfd.readouterr().err
-        found = re.findall(r"\[dfgpu trace\] launch (k_\w+<[^>]*>)", text)
-        return {re.sub(r"\s", "", m).replace("true", "1").replace("false", "0") for m in found}
-    return names
+    return capfd_launched(monkeypatch, capfd)
 
 
 def f64s(rng, n, nan=True):

@@ -4,15 +4,12 @@ Each case runs with DFGPU_TRACE set, reads the names of the kernels the library 
 instantiation it is named for ran, so a change in the dispatch cannot silently move a case onto another kernel.
 Inputs carry the value edges where kernels go wrong: NaN, ±0.0, ±inf, subnormals, the integer extremes, UInt64 values with
 the top bit set, and the keys that pack to the table's empty marker."""
-import os
-import re
-import sys
-import tempfile
 
 import numpy as np
 import pytest
 
 import groupby_ref as R
+from kernel_trace import traced_set as traced
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine
 from datafusion_archive_b200.expr import AggregateFunction, col, lit
@@ -29,36 +26,6 @@ def ctx():
     c = engine.GpuContext(0)
     yield c
     c.close()
-
-
-def canon(name):
-    """`k_hash_agg<8, false, true>` -> `k_hash_agg<8,0,1>`."""
-    m = re.match(r"(k_\w+)(<[^>]*>)?", name)
-    args = re.sub(r"\s", "", m.group(2) or "")
-    return m.group(1) + args.replace("true", "1").replace("false", "0")
-
-
-def traced(fn):
-    """(fn(), set of canonical names of the kernels launched while it ran).  Under DFGPU_TRACE the library names
-    every aggregate kernel it launches on stderr; file descriptor 2 is redirected to a temporary file meanwhile."""
-    sys.stderr.flush()
-    saved = os.dup(2)
-    old_env = os.environ.get("DFGPU_TRACE")
-    with tempfile.TemporaryFile() as f:
-        os.dup2(f.fileno(), 2)
-        os.environ["DFGPU_TRACE"] = "1"
-        try:
-            out = fn()
-        finally:
-            os.dup2(saved, 2)
-            os.close(saved)
-            if old_env is None:
-                del os.environ["DFGPU_TRACE"]
-            else:
-                os.environ["DFGPU_TRACE"] = old_env
-        f.seek(0)
-        text = f.read().decode(errors="replace")
-    return out, {canon(m) for m in re.findall(r"\[dfgpu trace\] launch (k_\w+(?:<[^>]*>)?)", text)}
 
 
 def run_agg(ctx, batches, keys, aggs, expected=0, pred=None):

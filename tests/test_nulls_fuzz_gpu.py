@@ -8,7 +8,6 @@ NaN: the payload of a NaN produced by arithmetic is not pinned) except float SUM
 gamma bound around the exact sum of the rows the oracle evaluated.  Every case runs under DFGPU_TRACE and asserts that the
 NULLS instantiation it is about was launched."""
 import math
-import re
 
 import numpy as np
 import pyarrow as pa
@@ -17,6 +16,7 @@ import pytest
 import fuzz_exprs as F
 import groupby_ref as G
 import oracle_lib as O
+from kernel_trace import capfd_launched
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
 from datafusion_archive_b200.expr import AggregateFunction, col, lit
@@ -35,14 +35,7 @@ def ctx():
 def launched(monkeypatch, capfd):
     """Returns a function that yields the canonical names of the kernels launched since the last call:
     `k_hash_agg<8, false, true>` -> `k_hash_agg<8,0,1>`."""
-    monkeypatch.setenv("DFGPU_TRACE", "1")
-    capfd.readouterr()
-
-    def names():
-        text = capfd.readouterr().err
-        found = re.findall(r"\[dfgpu trace\] launch (k_\w+<[^>]*>)", text)
-        return {re.sub(r"\s", "", m).replace("true", "1").replace("false", "0") for m in found}
-    return names
+    return capfd_launched(monkeypatch, capfd)
 
 
 def unpack(c):

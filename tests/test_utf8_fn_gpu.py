@@ -13,7 +13,8 @@ import pytest
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
 from datafusion_archive_b200.expr import AggregateFunction, col, lit, utf8_fn
-from test_avg_gpu import rows, traced
+from kernel_trace import traced_set as traced
+from test_avg_gpu import rows
 from utf8_fn_ref import NESTS, build, ev, is_int, random_strings
 
 pytestmark = pytest.mark.gpu
