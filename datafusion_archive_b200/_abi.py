@@ -49,6 +49,9 @@ FN_ARITY = {code: (2 if code in (FN_POWER, FN_ATAN2) else 1) for code in FN_CODE
 
 # Utf8 functions (DFGPU_OP_UTF8_FN: `col` = code, `dtype` = result type); the Utf8 operand first, then Int64 literals
 OP_UTF8_FN = 41
+# CASE WHEN c1 THEN v1 .. [ELSE e] END (DFGPU_OP_CASE): operands c1 v1 .. cn vn [e] first, `col` = their number, `dtype` =
+# the result type
+OP_CASE = 42
 UTF8FN_UPPER, UTF8FN_LOWER, UTF8FN_TRIM, UTF8FN_LTRIM, UTF8FN_RTRIM = 1, 2, 3, 4, 5
 UTF8FN_SUBSTR_FROM, UTF8FN_SUBSTR, UTF8FN_LENGTH, UTF8FN_OCTET_LENGTH = 6, 7, 8, 9
 UTF8_FN_CODES = {

@@ -922,8 +922,8 @@ constexpr int RD_TILE = AG_THREADS * RD_R;
 // NULLS: array_ops::{min,max,sum} skip nulls and report None when nothing was non-null
 // (restated from arrow 0.12; call sites aggregate.rs:347-541): the number of non-null inputs per
 // aggregate is accumulated in counter CTR_NONNULL + a so finish can emit a null.  Under a WHERE the
-// arguments are read as over FilterRelation's bitmap-free output (eval_after_where): nothing is skipped and
-// an aggregate is null only when no row passed.
+// arguments are read as over FilterRelation's bitmap-free output (eval_after_where): only a CASE-made null
+// (extended interpreter) is skipped, and without one an aggregate is null only when no row passed.
 template <int DEPTH, bool NULLS>
 __global__ void __launch_bounds__(AG_THREADS) k_reduce(const __grid_constant__ AggParams p) {
   __shared__ unsigned long long s_acc[kMaxAggs][AG_THREADS];
@@ -971,7 +971,8 @@ __global__ void __launch_bounds__(AG_THREADS) k_reduce(const __grid_constant__ A
         for (int r = 0; r < RD_R; r++)
           if (((rmask >> r) & 1u) && (!NULLS || ((av >> r) & 1u))) acc = acc_fold(func, mt, acc, v[r]);
         s_acc[a][tid] = acc;
-        if (NULLS && !p.has_pred) nn[a] += __popc(av & rmask);  // under a WHERE the host counts CTR_PASSED instead
+        // under a WHERE the host counts CTR_PASSED instead, unless a CASE can make nulls (extended interpreter)
+        if (NULLS && (!p.has_pred || DEPTH == kCaseDepth)) nn[a] += __popc(av & rmask);
       }
     }
   }
@@ -2254,6 +2255,8 @@ AggParams plan_insert(const dfgpu_aggstate* st, const BatchPrograms& bp, bool* p
 // interpreter.
 Kernel<AggParams, SetParams> choose_insert(const AggParams& p, bool plain_ok) {
   const bool fn = has_fn(p.ps), plain = plain_ok && !p.row_list && (p.row_begin & 1) == 0;
+  if (has_case(p.ps) && p.ps.has_nulls) return {k_distinct_insert<kCaseDepth, true>, "k_distinct_insert<kCaseDepth, true>"};
+  if (has_case(p.ps)) return {k_distinct_insert<kCaseDepth, false>, "k_distinct_insert<kCaseDepth, false>"};
   if (fn && p.ps.has_nulls) return {k_distinct_insert<kFnDepth, true>, "k_distinct_insert<kFnDepth, true>"};
   if (fn) return {k_distinct_insert<kFnDepth, false>, "k_distinct_insert<kFnDepth, false>"};
   if (p.ps.has_nulls) return {k_distinct_insert<8, true>, "k_distinct_insert<8, true>"};
@@ -2341,7 +2344,7 @@ void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
   Kernel<AggParams> k{};
   if (p.ps.has_nulls) {
     st->saw_nulls = true;
-    k = fn ? reduce_kernel<kFnDepth, true>() : reduce_kernel<8, true>();
+    k = has_case(p.ps) ? reduce_kernel<kCaseDepth, true>() : fn ? reduce_kernel<kFnDepth, true>() : reduce_kernel<8, true>();
   } else {
     if (!bp.has_pred)
       for (int a = 0; a < st->naggs; a++) st->nonnull_host[size_t(a)] += p.nrows;
@@ -2361,7 +2364,8 @@ void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
       for (int a = 0; a < p.naggs; a++) { rp.aggs[a] = p.aggs[a]; rp.agg_arg[a] = p.agg_arg[a]; }
       rp.t = st->t;
       launch_kernel(ctx, k_reduce_f64, "k_reduce_f64", rp, p.nrows, 256 * 8, 8, PROFILED);
-    } else if (fn) k = reduce_kernel<kFnDepth>();
+    } else if (has_case(p.ps)) k = reduce_kernel<kCaseDepth>();
+    else if (fn) k = reduce_kernel<kFnDepth>();
     else if (d <= 1) k = reduce_kernel<1>();
     else if (d <= 2) k = reduce_kernel<2>();
     else if (d <= 4) k = reduce_kernel<4>();
@@ -2371,7 +2375,9 @@ void reduce_update(dfgpu_aggstate* st, const BatchPrograms& bp, AggParams& p) {
   unsigned long long c[CTR_NONNULL];
   read_counters(st, c);
   if (c[CTR_ERROR]) fail(DFGPU_ERR_ARROW, "DivideByZero");
-  if (bp.has_pred)  // the arguments are read as over FilterRelation's null-free output: every row that passed is an input
+  // the arguments are read as over FilterRelation's null-free output: every row that passed is an input, unless a CASE
+  // made a null (the kernel then counted the non-null inputs itself)
+  if (bp.has_pred && !(p.ps.has_nulls && has_case(p.ps)))
     for (int a = 0; a < st->naggs; a++) st->nonnull_host[size_t(a)] += (long long)c[CTR_PASSED];
 }
 
@@ -2412,13 +2418,16 @@ ScanPlan plan_scan(const dfgpu_aggstate* st, const BatchPrograms& bp, AggParams&
 // take the interpreter; FRONT routes rows through the shared-memory front table.  A lean launch gets its table
 // addresses in p.lean.
 ScanKernel choose_scan(const dfgpu_aggstate* st, AggParams& p, const ScanPlan& plan, bool replay, bool front) {
-  const bool fn = has_fn(p.ps);
+  const bool fn = has_fn(p.ps), cs = has_case(p.ps);
   if (st->wide) {
+    if (cs && p.ps.has_nulls) return {k_hash_agg_wide<kCaseDepth, true>, "k_hash_agg_wide<kCaseDepth, true>", false};
+    if (cs) return {k_hash_agg_wide<kCaseDepth, false>, "k_hash_agg_wide<kCaseDepth, false>", false};
     if (fn && p.ps.has_nulls) return {k_hash_agg_wide<kFnDepth, true>, "k_hash_agg_wide<kFnDepth, true>", false};
     if (fn) return {k_hash_agg_wide<kFnDepth, false>, "k_hash_agg_wide<kFnDepth, false>", false};
     if (p.ps.has_nulls) return {k_hash_agg_wide<8, true>, "k_hash_agg_wide<8, true>", false};
     return {k_hash_agg_wide<8, false>, "k_hash_agg_wide<8, false>", false};
   }
+  if (cs && p.ps.has_nulls) return {k_hash_agg<kCaseDepth, false, true>, "k_hash_agg<kCaseDepth, false, true>", false};
   if (fn && p.ps.has_nulls) return {k_hash_agg<kFnDepth, false, true>, "k_hash_agg<kFnDepth, false, true>", false};
   if (p.ps.has_nulls) return {k_hash_agg<8, false, true>, "k_hash_agg<8, false, true>", false};
   const bool even = (p.row_begin & 1) == 0;
@@ -2453,6 +2462,7 @@ ScanKernel choose_scan(const dfgpu_aggstate* st, AggParams& p, const ScanPlan& p
     return {k_hash_agg_plain<4, false>, "k_hash_agg_plain<4, false>", false};
   }
   const int d = p.ps.max_depth;
+  if (cs) return hash_agg_kernel<kCaseDepth>(front);
   if (fn) return hash_agg_kernel<kFnDepth>(front);
   if (d <= 1) return hash_agg_kernel<1>(front);
   if (d <= 2) return hash_agg_kernel<2>(front);

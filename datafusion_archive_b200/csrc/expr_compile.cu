@@ -22,7 +22,7 @@ MType mtype_of(int dt) {
 namespace {
 
 struct Node {
-  enum Kind { COL, LIT, CAST, BIN, FN, UFN } kind = COL;
+  enum Kind { COL, LIT, CAST, BIN, FN, UFN, CASE } kind = COL;
   int col = 0;               // COL: batch column, or -1 - k for synthetic column k (a recognised Utf8 predicate or
                              // function); kViewCol for a Utf8 view that no program reads
   int view = -1;             // COL of a Utf8 view: its index
@@ -32,6 +32,7 @@ struct Node {
   int op = 0;                // DFGPU_OP_* for BIN, DFGPU_FN_* for FN, DFGPU_UTF8FN_* for UFN
   std::string str;           // LIT of dtype Utf8: the bytes
   std::unique_ptr<Node> l, r;  // FN: the arguments (r: second argument of a two-argument function, else null); UFN: l
+  std::vector<std::unique_ptr<Node>> args;  // CASE: c1 v1 .. cn vn [e]
 };
 constexpr int kViewCol = INT_MIN;
 
@@ -302,6 +303,28 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what, int* utf8_
         nd->count = arg[1];
         break;
       }
+      case DFGPU_OP_CASE: {  // CASE WHEN c1 THEN v1 .. [ELSE e] END: `col` operands c1 v1 .. cn vn [e], `dtype` the result type
+        if (in.col < 2 || in.col > int(st.size())) fail(DFGPU_ERR_GENERAL, "malformed expression program");
+        nd->kind = Node::CASE;
+        for (auto it = st.end() - in.col; it != st.end(); ++it) nd->args.push_back(std::move(*it));
+        st.resize(st.size() - size_t(in.col));
+        int rt = 0;
+        for (size_t k = 0; k < nd->args.size(); k++) {
+          lower_view(nd->args[k]);
+          const Node* a = nd->args[k].get();
+          if (k % 2 == 0 && k + 1 < nd->args.size()) {
+            if (a->dtype != DFGPU_BOOL) fail(DFGPU_ERR_EXECUTION, "CASE WHEN condition did not evaluate to boolean");
+            continue;
+          }
+          if (a->dtype == DFGPU_UTF8) fail(DFGPU_ERR_NOT_IMPLEMENTED, "CASE with a Utf8 result");
+          if (rt && a->dtype != rt)
+            fail(DFGPU_ERR_EXECUTION, std::string("CASE branch types differ: ") + dtype_name(rt) + " and " + dtype_name(a->dtype));
+          rt = a->dtype;
+        }
+        if (in.dtype != rt) fail(DFGPU_ERR_GENERAL, "malformed expression program");
+        nd->dtype = rt;
+        break;
+      }
       default: {
         int op = in.op;
         bool is_math = op >= DFGPU_OP_ADD && op <= DFGPU_OP_DIV;
@@ -393,6 +416,13 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what, int* utf8_
           case Node::LIT: return false;
           case Node::CAST: return go(nd->l.get());
           case Node::FN: return go(nd->l.get()) || (nd->r && go(nd->r.get()));  // like arithmetic
+          case Node::CASE: {  // the chosen branch's validity; null when no WHEN is taken and there is no ELSE
+            const size_t n = nd->args.size();
+            if (n % 2 == 0) return true;
+            for (size_t k = 1; k < n; k += 2)
+              if (go(nd->args[k].get())) return true;
+            return go(nd->args[n - 1].get());
+          }
           default: {
             const bool cmp = nd->op >= DFGPU_OP_EQ && nd->op <= DFGPU_OP_GE;
             return !cmp && (go(nd->l.get()) || go(nd->r.get()));
@@ -439,6 +469,24 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what, int* utf8_
           di.mtype = mtype_of(nd->l->dtype);
           cp->code.push_back(di);
           break;
+        case Node::CASE: {
+          // a fold backward from the ELSE: e, then cn vn SEL, .., c1 v1 SEL, so that the stack holds at most the fold, one
+          // condition and the operand being evaluated, whatever the number of WHENs.  Without ELSE the last WHEN is SEL0.
+          const size_t n = nd->args.size();
+          const bool has_else = n % 2 == 1;
+          if (has_else) go(nd->args[n - 1].get());
+          for (size_t k = (n & ~size_t(1)); k >= 2; k -= 2) {
+            go(nd->args[k - 2].get());
+            go(nd->args[k - 1].get());
+            const bool sel0 = !has_else && k == (n & ~size_t(1));
+            di.op = sel0 ? V_SEL0 : V_SEL;
+            di.dtype = uint8_t(nd->dtype);
+            di.mtype = mtype_of(nd->dtype);
+            cp->code.push_back(di);
+            bump(sel0 ? -1 : -2);
+          }
+          break;
+        }
         case Node::FN:
           if (!nd->r) {  // one argument: applied to the accumulator, like CAST
             go(nd->l.get());
@@ -491,6 +539,7 @@ int ProgramBuilder::add(const dfgpu_insn* p, int n, const char* what, int* utf8_
   } em{this, &cp, &depth};
   em.go(st[0].get());
   cp.out_dtype = st[0]->dtype;
+  for (const DevInsn& di : cp.code) cp.makes_nulls = cp.makes_nulls || (cp.nullable && di.op == V_SEL0);
 
   // 3. interpreter-free shapes
   const Node* root = st[0].get();
@@ -587,6 +636,7 @@ void ProgramBuilder::finish(ProgramSet* out) const {
     for (const auto& di : progs_[i].code) out->insn[pc++] = di;
     out->out_dtype[i] = uint8_t(progs_[i].out_dtype);
     out->nullable[i] = progs_[i].nullable ? 1 : 0;
+    if (progs_[i].makes_nulls) out->has_nulls = 1;  // a CASE without ELSE can make a null from any input
     if (progs_[i].max_depth > maxd) maxd = progs_[i].max_depth;
   }
   out->f64_only = 1;

@@ -22,13 +22,24 @@ enum VOp : uint8_t {
   V_RSUB, V_RDIV,  // operands exchanged (emitted for stack-mode instructions only, see expr_compile.cu)
   // scalar functions (DFGPU_OP_FN), Float64 only, `aux` = DFGPU_FN_* code: V_FN applies a one-argument function to the
   // accumulator like V_CAST, V_FN2 / V_RFN2 a two-argument one in any RhsMode (V_RFN2: operands exchanged)
-  V_FN, V_FN2, V_RFN2
+  V_FN, V_FN2, V_RFN2,
+  // CASE (DFGPU_OP_CASE), lowered as a fold backward from the ELSE (expr_compile.cu).  Stack operands only, the
+  // accumulator holding the THEN value v, the entry below it the condition c:
+  //   V_SEL   pops c and the fold so far e below it: c ? v : e
+  //   V_SEL0  (the last WHEN of a CASE without ELSE) pops c: c ? v : null
+  // A condition is taken when it is true and valid.
+  V_SEL, V_SEL0
 };
-// The interpreter kernels' DEPTH template argument is the register-stack depth (1, 2, 4 or 8), or kFnDepth for a program
-// set that contains V_FN* (has_fn below): depth 8 with the scalar functions compiled in.  Only kFnDepth
-// instantiations contain them, so the kernels that run function-free queries keep their code.
+// The interpreter kernels' DEPTH template argument is the register-stack depth (1, 2, 4 or 8), kFnDepth for a program set
+// that contains V_FN* (has_fn below): depth 8 with the scalar functions compiled in, or kCaseDepth for a set that contains
+// V_SEL* (has_case): the extended interpreter, depth 8 with the scalar functions, CASE, validity tracking and per-entry
+// error bits.  Only those instantiations contain that code, so the kernels that run other queries keep theirs: CASE's
+// bookkeeping costs a function-only query nothing.
 constexpr int kFnDepth = 9;
-inline std::string depth_arg(int depth) { return depth == kFnDepth ? "kFnDepth" : std::to_string(depth); }
+constexpr int kCaseDepth = 10;
+inline std::string depth_arg(int depth) {
+  return depth == kFnDepth ? "kFnDepth" : depth == kCaseDepth ? "kCaseDepth" : std::to_string(depth);
+}
 enum RhsMode : uint8_t { RHS_STACK = 0, RHS_IMM = 1, RHS_COL = 2 };
 
 struct __align__(16) DevInsn {   // 16 bytes, lives in kernel parameter (constant) space
@@ -61,14 +72,21 @@ struct ProgramSet {
   int ncols;
   int max_depth;
   int f64_only;  // every operand Float64/Boolean and no CAST: the lean evaluator applies
-  int has_nulls; // some referenced column carries a validity bitmap: kernels use the NULLS evaluator
+  int has_nulls; // some referenced column carries a validity bitmap, or some program's result can be a CASE-made null
+                 // (CompiledProgram::makes_nulls): kernels use the NULLS evaluator
   uint8_t nullable[kMaxProgs];  // program result can be null (arrow 0.12 array_ops semantics)
 };
-// Some program of the set calls a scalar function (V_FN*): its kernels run with DEPTH = kFnDepth.  Read from the code rather
-// than stored, so that the kernel parameter blocks keep their layout.
+// Some program of the set calls a scalar function or has a CASE (V_FN*, V_SEL*): its kernels run with DEPTH = kFnDepth,
+// or kCaseDepth when has_case.  Read from the code rather than stored, so that the kernel parameter blocks keep their
+// layout.
 inline bool has_fn(const ProgramSet& ps) {
   for (int pc = 0; pc < ps.start[ps.nprog]; pc++)
     if (ps.insn[pc].op >= V_FN) return true;
+  return false;
+}
+inline bool has_case(const ProgramSet& ps) {
+  for (int pc = 0; pc < ps.start[ps.nprog]; pc++)
+    if (ps.insn[pc].op >= V_SEL) return true;
   return false;
 }
 // Some program of the set divides: the only instruction whose kernels can raise an error (DivideByZero, for integers and
@@ -103,6 +121,7 @@ static_assert(sizeof(Leaf) == 32 && sizeof(LeafChain) == 136, "FPParams and AggP
 struct CompiledProgram {
   std::vector<DevInsn> code;
   bool nullable = false;
+  bool makes_nulls = false;  // nullable, and has a CASE without ELSE: can be null even where every input column is valid
   int out_dtype = 0;
   int max_depth = 0;
   Leaf leaf{};        // kind 1: the program is exactly one column; 2 / 3: one + - * / (no integer division, no
@@ -460,6 +479,13 @@ static __device__ __noinline__ double scalar_fn(int fn, double x, double y) {
 // `filter.value(i)` (filter.rs:86) and update_accumulators' `z.value(row)` (aggregate.rs:561-601) read;
 // comparisons never yield null: nulls are ordered (lt/lt_eq: null on the left -> true; gt/gt_eq: null
 // on the right -> true; eq: both null).  `out_valid` receives the validity bits of the result.
+//
+// The extended interpreter (DEPTH == kCaseDepth) always tracks validity, so that the nulls a CASE without ELSE makes reach
+// the result; without NULLS it reads every column as valid (the input bitmaps are dropped, as under a WHERE).  It also
+// evaluates CASE lazily: each stack entry carries the DivideByZero bits of its rows (badmask for the accumulator, spille
+// for the spilled entries), an operation ORs its operands' bits and a select keeps err(c) | (taken ? err(v) : err(e)).
+// The result's bits are the top entry's.  For a program without CASE that is the OR over every operation, which is
+// what the other instantiations compute in badmask directly.
 template <int DEPTH, int R, bool F64ONLY, bool NULLS, class Src>
 __device__ __forceinline__ unsigned eval_program_n(const ProgramSet& ps, int prog, const Src& src,
                                                    unsigned long long (&out)[R], unsigned& out_valid) {
@@ -469,11 +495,14 @@ __device__ __forceinline__ unsigned eval_program_n(const ProgramSet& ps, int pro
   // stack-mode instruction R loads (its operands were exchanged at lowering so that the accumulator is
   // always the left input).
   constexpr unsigned ALL = (1u << R) - 1u;
-  constexpr bool FN = DEPTH == kFnDepth;  // the scalar-function cases are compiled in
+  constexpr bool FN = DEPTH >= kFnDepth;   // the scalar-function cases are compiled in
+  constexpr bool CS = DEPTH == kCaseDepth; // and the CASE cases, with their bookkeeping
+  constexpr bool TV = NULLS || CS;         // validity is tracked
   constexpr int D = FN ? 8 : DEPTH;
   constexpr int SPILL = D > 1 ? D - 1 : 1;
   unsigned long long spill[SPILL][R];
   unsigned spillv[SPILL];
+  unsigned spille[SPILL];  // CS: DivideByZero bits of the spilled entries
   unsigned accv = ALL;
   int depth = 0;
 #pragma unroll
@@ -489,7 +518,35 @@ __device__ __forceinline__ unsigned eval_program_n(const ProgramSet& ps, int pro
     const int dt = (raw.x >> 24) & 0xff;
     const int slot = (int)(short)(raw.y & 0xffff);
     const unsigned long long imm = ((unsigned long long)raw.w << 32) | raw.z;
-    if constexpr (FN) {  // discarded in every other instantiation, which therefore keeps its code
+    if constexpr (CS) {  // discarded in every other instantiation, which therefore keeps its code
+      if (op >= V_SEL) {
+        // pop the condition c (the entry below the accumulator v) and, for V_SEL, the fold e below it
+        depth--;
+        const int dc = depth - 1 < SPILL ? depth - 1 : SPILL - 1;
+        unsigned taken = 0;
+#pragma unroll
+        for (int r = 0; r < R; r++) taken |= (unsigned)(spill[dc][r] & 1ull) << r;
+        taken &= spillv[dc];  // a null condition is not taken
+        const unsigned errc = spille[dc];
+        if (op == V_SEL) {
+          depth--;
+          const int de = depth - 1 < SPILL ? depth - 1 : SPILL - 1;
+#pragma unroll
+          for (int r = 0; r < R; r++)
+            if (!((taken >> r) & 1u)) out[r] = spill[de][r];
+          accv = (accv & taken) | (spillv[de] & ~taken);
+          badmask = errc | (badmask & taken) | (spille[de] & ~taken);
+        } else {
+#pragma unroll
+          for (int r = 0; r < R; r++)
+            if (!((taken >> r) & 1u)) out[r] = 0ull;
+          accv &= taken;
+          badmask = errc | (badmask & taken);
+        }
+        continue;
+      }
+    }
+    if constexpr (FN) {
       if (op >= V_FN) {
         // scalar function: Float64 in, Float64 out; a row is null where an argument is, with value 0 (like arithmetic)
         const int fn = (int)(short)(raw.y >> 16);
@@ -510,13 +567,14 @@ __device__ __forceinline__ unsigned eval_program_n(const ProgramSet& ps, int pro
             const int d = depth - 1 >= 0 ? (depth - 1 < SPILL ? depth - 1 : SPILL - 1) : 0;
 #pragma unroll
             for (int r = 0; r < R; r++) y[r] = spill[d][r];
-            if (NULLS) valid &= spillv[d];
+            if (TV) valid &= spillv[d];
+            if constexpr (CS) badmask |= spille[d];
           }
           const bool swap = op == V_RFN2;
 #pragma unroll
           for (int r = 0; r < R; r++) out[r] = d2u(scalar_fn(fn, u2d(swap ? y[r] : out[r]), u2d(swap ? out[r] : y[r])));
         }
-        if (NULLS) {
+        if (TV) {
 #pragma unroll
           for (int r = 0; r < R; r++)
             if (!((valid >> r) & 1u)) out[r] = 0ull;
@@ -530,10 +588,12 @@ __device__ __forceinline__ unsigned eval_program_n(const ProgramSet& ps, int pro
         const int d = depth - 1 < SPILL ? depth - 1 : SPILL - 1;
 #pragma unroll
         for (int r = 0; r < R; r++) spill[d][r] = out[r];
-        if (NULLS) spillv[d] = accv;
+        if (TV) spillv[d] = accv;
+        if constexpr (CS) spille[d] = badmask;
       }
       depth++;
-      if (NULLS) accv = op == V_PUSH_COL ? src.col_valid(ps, slot) : ALL;
+      if constexpr (CS) badmask = 0;
+      if (TV) accv = NULLS && op == V_PUSH_COL ? src.col_valid(ps, slot) : ALL;
       if (op == V_PUSH_IMM) {
 #pragma unroll
         for (int r = 0; r < R; r++) out[r] = imm;
@@ -547,7 +607,7 @@ __device__ __forceinline__ unsigned eval_program_n(const ProgramSet& ps, int pro
       const int src_dt = (int)(short)(raw.y >> 16);
 #pragma unroll
       for (int r = 0; r < R; r++) out[r] = cast_value(out[r], mt, src_dt, dt);
-      if (NULLS) {
+      if (TV) {
 #pragma unroll
         for (int r = 0; r < R; r++)
           if (!((accv >> r) & 1u)) out[r] = 0ull;
@@ -568,14 +628,15 @@ __device__ __forceinline__ unsigned eval_program_n(const ProgramSet& ps, int pro
         const int d = depth - 1 >= 0 ? (depth - 1 < SPILL ? depth - 1 : SPILL - 1) : 0;
 #pragma unroll
         for (int r = 0; r < R; r++) y[r] = spill[d][r];
-        if (NULLS) vb = spillv[d];
+        if (TV) vb = spillv[d];
+        if constexpr (CS) badmask |= spille[d];
       }
       const unsigned both = va & vb;
       // The (machine type, op) dispatch is hoisted out of the per-row loop: it is warp-uniform and
       // paid once per R rows.  A zero divisor sets the row's bit in badmask (arrow 0.12
       // array_ops::divide returns ArrowError::DivideByZero for ints and floats alike).
 #define DF_ROWS(EXPR) _Pragma("unroll") for (int r = 0; r < R; r++) { const unsigned long long a = out[r], b = y[r]; (void)a; (void)b; out[r] = (EXPR); }
-#define DF_DIVCHK(WHICH, COND) _Pragma("unroll") for (int r = 0; r < R; r++) { const unsigned long long z = WHICH[r]; if ((COND) && (!NULLS || ((both >> r) & 1u))) badmask |= 1u << r; }
+#define DF_DIVCHK(WHICH, COND) _Pragma("unroll") for (int r = 0; r < R; r++) { const unsigned long long z = WHICH[r]; if ((COND) && (!TV || ((both >> r) & 1u))) badmask |= 1u << r; }
       switch (F64ONLY ? (op == V_AND || op == V_OR ? (int)MT_BOOL : (int)MT_F64) : mt) {
         case MT_F64:
           switch (op) {
@@ -654,7 +715,7 @@ __device__ __forceinline__ unsigned eval_program_n(const ProgramSet& ps, int pro
       }
 #undef DF_ROWS
 #undef DF_DIVCHK
-      if (NULLS) {
+      if (TV) {
         if (op >= V_EQ && op <= V_GE) {
           // comparisons: never null; a null operand is ordered, not propagated (a = accumulator = the
           // left input of the instruction as emitted, b = y = its right input)
@@ -683,7 +744,7 @@ __device__ __forceinline__ unsigned eval_program_n(const ProgramSet& ps, int pro
       }
     }
   }
-  out_valid = NULLS ? accv : ALL;
+  out_valid = TV ? accv : ALL;
   return badmask & src.valid;
 }
 

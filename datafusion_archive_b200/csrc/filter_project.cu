@@ -20,7 +20,9 @@ namespace dfgpu {
 // semantics (a null And/Or result reads as false, like `filter.value(i)` in filter.rs:86).  With a
 // predicate the projections then see null-free arrays, exactly like the reference: `fn filter` copies
 // values and drops the bitmap (filter.rs:83-91) before ProjectRelation runs.  Without a predicate the
-// projections run on the original arrays and their validity is written out (32 rows per ballot word).
+// projections run on the original arrays and their validity is written out (32 rows per ballot word).  A CASE-made null
+// is a null under a predicate too: the extended interpreter writes the validity of such a projection as one byte per
+// selected row (out_vbytes), packed after the kernel.
 template <int DEPTH, bool NULLS>
 __global__ void __launch_bounds__(FP_THREADS) k_filter_project(const __grid_constant__ FPParams p) {
   __shared__ int s_tile;
@@ -139,7 +141,7 @@ __global__ void __launch_bounds__(FP_THREADS) k_filter_project(const __grid_cons
         unsigned ov = (1u << FP_R) - 1u;
         unsigned b;
         if (NULLS && !p.has_pred) b = eval_program_n<DEPTH, FP_R, false, true>(p.ps, prog, src, v, ov);
-        else b = eval_program<DEPTH, FP_R, false>(p.ps, prog, src, v);
+        else b = eval_program_n<DEPTH, FP_R, false, false>(p.ps, prog, src, v, ov);
         if (NULLS && !p.has_pred && p.out_valid[q]) {
 #pragma unroll
           for (int r = 0; r < FP_R; r++) {
@@ -161,6 +163,8 @@ __global__ void __launch_bounds__(FP_THREADS) k_filter_project(const __grid_cons
           if (f) {
             const unsigned long long idx = prefix + s_woff[j * FP_WARPS + warp] + __popc(m & lt_mask);
             store_elem(o, odt, (long long)idx, v[r]);
+            if constexpr (DEPTH == kCaseDepth)
+              if (NULLS && p.out_vbytes[q]) p.out_vbytes[q][idx] = (unsigned char)((ov >> r) & 1u);
             // DivideByZero only counts for rows that survive the filter: ProjectRelation runs on
             // the filtered batch (src/execution/context.rs:140-161).
             if ((b >> r) & 1u) bad = true;
@@ -181,6 +185,22 @@ __global__ void __launch_bounds__(256) k_pack_bits(const unsigned char* __restri
     const unsigned m = __ballot_sync(0xffffffffu, i < n && bytes[i] != 0);
     if ((threadIdx.x & 31) == 0) words[i >> 5] = m;
   }
+}
+// same, for validity bytes: also adds the number of zero bytes (the nulls) to *zeros
+__global__ void __launch_bounds__(256) k_pack_valid(const unsigned char* __restrict__ bytes, long long n, unsigned* __restrict__ words,
+                                                    unsigned long long* __restrict__ zeros) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long padded = (n + 31) / 32 * 32;
+  unsigned z = 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < padded; i += stride) {
+    const unsigned m = __ballot_sync(0xffffffffu, i < n && bytes[i] != 0);
+    const unsigned in = __ballot_sync(0xffffffffu, i < n);
+    if ((threadIdx.x & 31) == 0) {
+      words[i >> 5] = m;
+      z += __popc(in & ~m);
+    }
+  }
+  if (z) atomicAdd(zeros, (unsigned long long)z);
 }
 template <int DEPTH, bool NULLS = false>
 static void launch_fp(dfgpu_ctx* ctx, const FPParams& p) {
@@ -385,6 +405,23 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
     static_assert(kMaxProgs <= SCR_FP_NULLS.words, "a null count per program");
     p.null_counts = ctx->d_scratch + SCR_FP_NULLS.at;
     std::vector<int> valid_of_out(size_t(nproj), -1);  // result column -> kernel program with a validity buffer
+    memset(p.out_vbytes, 0, sizeof(p.out_vbytes));
+    dfgpu_result vbytes;  // RAII for the validity bytes of CASE projections under a predicate
+    vbytes.ctx = ctx;
+    std::vector<int> vbytes_of_out(size_t(nproj), -1);
+    if (has_pred && has_case(p.ps)) {
+      for (int i = 0; i < nproj; i++) {
+        const int k = out_kind[size_t(i)];
+        if (k < 0 || !pb.prog(k + has_pred).makes_nulls) continue;
+        DevColumn b;
+        b.dtype = DFGPU_UINT8;
+        b.values_bytes = size_t(n);
+        b.values = ctx->alloc(b.values_bytes);
+        p.out_vbytes[k] = (unsigned char*)b.values;
+        vbytes_of_out[size_t(i)] = int(vbytes.cols.size());
+        vbytes.cols.push_back(b);
+      }
+    }
     if (p.ps.has_nulls && !has_pred) {
       DF_CUDA(cudaMemsetAsync(p.null_counts, 0, kMaxProgs * 8, ctx->stream));
       for (int i = 0; i < nproj; i++) {
@@ -404,12 +441,14 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
     if (p.ps.has_nulls) {
       p.ntiles = int((n + FP_TILE - 1) / FP_TILE);
       // the null-aware evaluator lives in the direct kernel only
-      if (fn) launch_fp<kFnDepth, true>(ctx, p);
+      if (has_case(p.ps)) launch_fp<kCaseDepth, true>(ctx, p);
+      else if (fn) launch_fp<kFnDepth, true>(ctx, p);
       else launch_fp<8, true>(ctx, p);
     } else if (ctx->force_direct_kernel || !launch_fp_tma(ctx, p)) {
       p.ntiles = int((n + FP_TILE - 1) / FP_TILE);
       const int d = p.ps.max_depth;
-      if (fn) launch_fp<kFnDepth>(ctx, p);
+      if (has_case(p.ps)) launch_fp<kCaseDepth>(ctx, p);
+      else if (fn) launch_fp<kFnDepth>(ctx, p);
       else if (d <= 1) launch_fp<1>(ctx, p);
       else if (d <= 2) launch_fp<2>(ctx, p);
       else if (d <= 4) launch_fp<4>(ctx, p);
@@ -438,6 +477,29 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
     }
     if (*p.err_flag != 0) fail(DFGPU_ERR_ARROW, "DivideByZero");
     res->nrows = has_pred ? (int64_t)*p.out_count : n;
+    if (!vbytes.cols.empty() && res->nrows > 0) {
+      DF_CUDA(cudaMemsetAsync(p.null_counts, 0, kMaxProgs * 8, ctx->stream));
+      const long long words = (res->nrows + 31) / 32;
+      for (int i = 0; i < nproj; i++)
+        if (vbytes_of_out[size_t(i)] >= 0) {
+          DevColumn& c = res->cols[size_t(i)];
+          c.validity = (uint8_t*)ctx->alloc(size_t(words) * 4);
+          launch(ctx, "k_pack_valid", k_pack_valid, grid_for(ctx, words * 32, 256, 8), 256, {},
+                 (const unsigned char*)vbytes.cols[size_t(vbytes_of_out[size_t(i)])].values, (long long)res->nrows, (unsigned*)c.validity,
+                 p.null_counts + out_kind[size_t(i)]);
+        }
+      DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + SCR_FP_NULLS.at, p.null_counts, kMaxProgs * 8, cudaMemcpyDeviceToHost, ctx->stream));
+      DF_CUDA(cudaStreamSynchronize(ctx->stream));
+      for (int i = 0; i < nproj; i++) {
+        DevColumn& c = res->cols[size_t(i)];
+        if (vbytes_of_out[size_t(i)] < 0) continue;
+        c.null_count = (int64_t)ctx->h_scratch[SCR_FP_NULLS.at + out_kind[size_t(i)]];
+        if (c.null_count == 0) {
+          ctx->free(c.validity);
+          c.validity = nullptr;
+        }
+      }
+    }
     for (int i = 0; i < nproj; i++)
       if (bool_of_out[size_t(i)] >= 0) {
         DevColumn& c = res->cols[size_t(i)];
@@ -521,10 +583,12 @@ extern "C" int dfgpu_filter_project_host(dfgpu_ctx* ctx, const dfgpu_col* cols, 
     if (pred_len > 0) scan(pred, pred_len);
     for (int q = 0; q < nproj; q++) scan(proj[q], proj_len[q]);
     if (used.empty()) fail(DFGPU_ERR_NOT_IMPLEMENTED, "queries that reference no column");
-    // Utf8 / Boolean / nullable inputs: not chunk-pipelined — the referenced columns are uploaded whole and the resident
-    // operator runs (same kernels, same results); the result then lives in DEVICE memory (dfgpu_result_on_host says
-    // which; dfgpu_result_copy_col works for both)
+    // Utf8 / Boolean / nullable inputs and projections that can hold a CASE-made null: not chunk-pipelined — the
+    // referenced columns are uploaded whole and the resident operator runs (same kernels, same results); the result then
+    // lives in DEVICE memory (dfgpu_result_on_host says which; dfgpu_result_copy_col works for both)
     bool resident = false;
+    for (int q = 0; q < nproj; q++)
+      for (int i = 0; i < proj_len[q]; i++) resident = resident || (proj[q][i].op == DFGPU_OP_CASE && proj[q][i].col % 2 == 0);
     for (int c : used) resident = resident || !is_numeric(cols[c].dtype) || cols[c].validity;
     auto rewrite = [&](const dfgpu_insn* p, int len) {
       std::vector<dfgpu_insn> v(p, p + len);

@@ -39,6 +39,9 @@ struct FPParams {
   // "fast shapes" (Leaf, as ProgramBuilder::add recognised them): the TMA kernel runs them without the interpreter
   LeafChain pred_fast;  // the predicate as a comparison chain
   Leaf proj_fast[kMaxProgs];
+  // queries with a predicate whose projection can hold a CASE-made null (direct kernel, extended interpreter only): one
+  // validity byte per selected row, in output order; null for every other projection
+  unsigned char* out_vbytes[kMaxProgs];
 };
 
 constexpr unsigned long long ST_AGG = 1ull << 62, ST_INCL = 2ull << 62, ST_MASK = (1ull << 62) - 1;

@@ -889,7 +889,10 @@ bool launch_fp_tma(dfgpu_ctx* ctx, FPParams& p) {
   p.ntiles = int((p.nrows + tile - 1) / tile);
   const size_t smem = TM_HDR_BYTES + (size_t)p.nstagesA * p.stage_bytesA + (size_t)p.nstagesB * p.stage_bytesB;
   const int d = p.ps.max_depth;
-  if (fn) {
+  if (has_case(p.ps)) {
+    if (p.ps.f64_only) launch_one<kCaseDepth, 4, true, false>(ctx, p, smem);
+    else launch_one<kCaseDepth, 4, false, false>(ctx, p, smem);
+  } else if (fn) {
     if (p.ps.f64_only) launch_one<kFnDepth, 4, true, false>(ctx, p, smem);
     else launch_one<kFnDepth, 4, false, false>(ctx, p, smem);
   } else if (K == 8) launch_k<2, 8>(ctx, p, smem);

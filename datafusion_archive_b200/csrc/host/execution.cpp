@@ -323,6 +323,13 @@ void lower(const Expr& e, const Schema& schema, const std::map<size_t, int>& rem
       out.push_back(in);
       return;
     }
+    case Expr::Case:
+      for (auto& a : e.args) lower(*a, schema, remap, out);
+      in.op = DFGPU_OP_CASE;
+      in.col = int(e.args.size());
+      in.dtype = e.get_type(schema);
+      out.push_back(in);
+      return;
     default: fail(DFGPU_ERR_EXECUTION, "expression " + e.debug());  // expression.rs:500-503
   }
 }

@@ -147,6 +147,7 @@ ExprRef Expr::scalar_fn(const std::string& name, std::vector<ExprRef> args, Data
   auto e = std::make_shared<Expr>(); e->kind = ScalarFunction; e->name = name; e->args = std::move(args); e->data_type = rt; return e;
 }
 ExprRef Expr::sort(ExprRef x, bool asc) { auto e = std::make_shared<Expr>(); e->kind = Sort; e->left = std::move(x); e->asc = asc; return e; }
+ExprRef Expr::case_when(std::vector<ExprRef> args) { auto e = std::make_shared<Expr>(); e->kind = Case; e->args = std::move(args); return e; }
 ExprRef Expr::is_null(ExprRef x, bool negated) {
   auto e = std::make_shared<Expr>(); e->kind = negated ? IsNotNull : IsNull; e->left = std::move(x); return e;
 }
@@ -162,6 +163,7 @@ DataType Expr::get_type(const Schema& schema) const {
     case Cast: case ScalarFunction: case AggregateFunction: return data_type;
     case IsNull: case IsNotNull: return DFGPU_BOOL;
     case Sort: return left->get_type(schema);
+    case Case: return args[1]->get_type(schema);
     case BinaryExpr:
       switch (op) {
         case Operator::Eq: case Operator::NotEq: case Operator::Lt: case Operator::LtEq: case Operator::Gt: case Operator::GtEq:
@@ -180,7 +182,22 @@ DataType Expr::get_type(const Schema& schema) const {
 ExprRef Expr::cast_to(DataType t, const Schema& schema) const {
   DataType this_type = get_type(schema);
   if (this_type == t) return std::make_shared<Expr>(*this);
-  if (can_coerce_from(t, this_type)) return Expr::cast(std::make_shared<Expr>(*this), t);
+  if (can_coerce_from(t, this_type)) {
+    if (kind == Case) {  // cast the THEN / ELSE values instead: the engine casts columns and literals, not expressions
+      std::vector<ExprRef> a = args;
+      auto recast = [&](ExprRef& v) {
+        // a value the planner already widened (CAST(#3 AS Int64)) is widened from its source in one step: the same
+        // value, since every coercion is exact or rounds once, and a CAST the engine can run
+        const bool widened = v->kind == Cast && (v->left->kind == Column || v->left->kind == Literal) &&
+                             can_coerce_from(v->data_type, v->left->get_type(schema));
+        v = (widened ? v->left : v)->cast_to(t, schema);
+      };
+      for (size_t k = 1; k < a.size(); k += 2) recast(a[k]);
+      if (a.size() % 2) recast(a.back());
+      return Expr::case_when(std::move(a));
+    }
+    return Expr::cast(std::make_shared<Expr>(*this), t);
+  }
   fail(DFGPU_ERR_GENERAL, std::string("Cannot automatically convert ") + datatype_debug(this_type) + " to " + datatype_debug(t));
 }
 
@@ -193,6 +210,12 @@ std::string Expr::debug() const {
     case IsNotNull: return left->debug() + " IS NOT NULL";
     case BinaryExpr: return left->debug() + " " + operator_debug(op) + " " + right->debug();
     case Sort: return left->debug() + (asc ? " ASC" : " DESC");
+    case Case: {
+      std::string s = "CASE";
+      for (size_t i = 0; i + 1 < args.size(); i += 2) s += " WHEN " + args[i]->debug() + " THEN " + args[i + 1]->debug();
+      if (args.size() % 2) s += " ELSE " + args.back()->debug();
+      return s + " END";
+    }
     case ScalarFunction: case AggregateFunction: {
       std::string s = name + (distinct ? "(DISTINCT " : "(");
       for (size_t i = 0; i < args.size(); i++) {
@@ -210,7 +233,7 @@ void collect_columns(const Expr& e, std::set<size_t>& acc) {
     case Expr::Column: acc.insert(e.index); break;
     case Expr::BinaryExpr: collect_columns(*e.left, acc); collect_columns(*e.right, acc); break;
     case Expr::Cast: case Expr::IsNull: case Expr::IsNotNull: case Expr::Sort: collect_columns(*e.left, acc); break;
-    case Expr::ScalarFunction: case Expr::AggregateFunction:
+    case Expr::ScalarFunction: case Expr::AggregateFunction: case Expr::Case:
       for (auto& a : e.args) collect_columns(*a, acc);
       break;
     default: break;

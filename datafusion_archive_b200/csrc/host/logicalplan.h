@@ -60,7 +60,8 @@ const char* operator_debug(Operator op);
 struct Expr;
 using ExprRef = std::shared_ptr<const Expr>;
 struct Expr {
-  enum Kind { Column, Literal, BinaryExpr, IsNotNull, IsNull, Cast, Sort, ScalarFunction, AggregateFunction } kind = Column;
+  // Case: args = c1 v1 .. cn vn [e], every v and e of one type (the planner casts them), as DFGPU_OP_CASE takes them
+  enum Kind { Column, Literal, BinaryExpr, IsNotNull, IsNull, Cast, Sort, ScalarFunction, AggregateFunction, Case } kind = Column;
   size_t index = 0;         // Column
   ScalarValue value;        // Literal
   ExprRef left, right;      // BinaryExpr; `left` is also the operand of IsNull/IsNotNull/Cast/Sort
@@ -79,6 +80,7 @@ struct Expr {
   static ExprRef scalar_fn(const std::string& name, std::vector<ExprRef> args, DataType rt);
   static ExprRef sort(ExprRef e, bool asc);
   static ExprRef is_null(ExprRef e, bool negated);
+  static ExprRef case_when(std::vector<ExprRef> args);
 
   DataType get_type(const Schema& schema) const;             // logicalplan.rs:170-198
   ExprRef cast_to(DataType t, const Schema& schema) const;   // logicalplan.rs:200-215

@@ -83,7 +83,8 @@ struct Parser {
   static bool reserved(const std::string& u) {
     static const char* kws[] = {"SELECT", "FROM", "WHERE", "GROUP", "BY", "HAVING", "ORDER", "LIMIT", "AND", "OR", "NOT", "AS", "ASC", "DESC", "IS", "NULL", "LIKE", "CAST",
                                  // joins: reserved so that `FROM a LEFT JOIN b` cannot read LEFT as an alias of a
-                                 "JOIN", "INNER", "ON", "LEFT", "RIGHT", "FULL", "OUTER", "CROSS", "NATURAL", "USING"};
+                                 "JOIN", "INNER", "ON", "LEFT", "RIGHT", "FULL", "OUTER", "CROSS", "NATURAL", "USING",
+                                 "CASE", "WHEN", "THEN", "ELSE", "END"};
     for (auto k : kws) if (u == k) return true;
     return false;
   }
@@ -189,6 +190,20 @@ struct Parser {
           n->subquery = parse_subquery();
           return n;
         }
+        if (u == "CASE") {  // CASE [x] WHEN c THEN v [WHEN ..] [ELSE e] END
+          n->kind = ASTNode::SQLCase;
+          if (!is_kw("WHEN") && !is_kw("END")) n->left = parse_expr();
+          while (accept_kw("WHEN")) {
+            n->args.push_back(parse_expr());
+            expect_kw("THEN");
+            n->args.push_back(parse_expr());
+          }
+          if (n->args.empty()) perr("Expected WHEN after CASE, found: " + peek().text);
+          if (accept_kw("ELSE")) n->right = parse_expr();
+          expect_kw("END");
+          return n;
+        }
+        if (u == "WHEN" || u == "THEN" || u == "ELSE" || u == "END") perr("Expected an expression, found: " + t.text);
         if (u == "CAST") {
           expect_sym("(");
           n->kind = ASTNode::SQLCast;
@@ -371,6 +386,7 @@ std::string ASTNode::debug() const {
     case SQLSelect: return "SQLSelect { .. }";
     case SQLInSubquery: return negated ? "SQLInSubquery { negated: true, .. }" : "SQLInSubquery { .. }";
     case SQLExists: return negated ? "SQLExists { negated: true, .. }" : "SQLExists { .. }";
+    case SQLCase: return "SQLCase { .. }";
   }
   return "?";
 }

@@ -25,12 +25,14 @@ struct JoinClause { ASTRef relation; ASTRef on; };  // INNER JOIN relation ON on
 
 struct ASTNode {
   enum Kind { SQLIdentifier, SQLWildcard, SQLLong, SQLDouble, SQLString, SQLBinaryExpr, SQLCast, SQLIsNull, SQLIsNotNull, SQLFunction, SQLSelect,
-              SQLInSubquery, SQLExists } kind = SQLIdentifier;
+              SQLInSubquery, SQLExists, SQLCase } kind = SQLIdentifier;
   std::string id;       // identifier / function name / string literal / unknown type name
   std::string qualifier;  // SQLIdentifier: `q` of a column `q.c`; of a table after FROM / JOIN: its alias, or empty
   long long lval = 0;   // SQLLong
   double dval = 0;      // SQLDouble
   ASTRef left, right;   // binary; `left` = operand of cast / is-null
+  // SQLCase: `left` = the operand of the simple form CASE x WHEN .. (else null), `args` = WHEN / THEN pairs, `right` = ELSE
+  // (or null)
   SQLOperator op = SQLOperator::Eq;
   SQLType sql_type = SQLType::Other;
   std::vector<ASTRef> args;

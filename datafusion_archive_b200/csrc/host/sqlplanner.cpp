@@ -34,6 +34,7 @@ Field expr_to_field(const Expr& e, const Schema& input_schema) {
     case Expr::Literal: return Field{"lit", e.value.get_datatype(), true};
     case Expr::ScalarFunction: case Expr::AggregateFunction: return Field{e.name, e.data_type, true};
     case Expr::Cast: return Field{"cast", e.data_type, true};
+    case Expr::Case: return Field{"case", e.get_type(input_schema), true};
     case Expr::BinaryExpr: {
       DataType st;
       if (!get_supertype(e.left->get_type(input_schema), e.right->get_type(input_schema), &st))
@@ -345,6 +346,15 @@ PlanRef SqlToRel::plan_subquery(const ASTNode& term, PlanRef left, const std::ve
 
 ExprRef SqlToRel::sql_to_rex(const ASTRef& sql, const Schema& schema) const { return rex(sql, schema, nullptr); }
 
+// l op r with both operands cast to their supertype (sqlplanner.rs:402-414)
+ExprRef SqlToRel::coerced_binary(const ExprRef& l, Operator op, const ExprRef& r, const Schema& schema) {
+  DataType lt = l->get_type(schema), rt = r->get_type(schema), st;
+  if (!get_supertype(lt, rt, &st))
+    fail(DFGPU_ERR_GENERAL, std::string("No common supertype found for binary operator ") + operator_debug(op) + " with input types " +
+                                datatype_debug(lt) + " and " + datatype_debug(rt));
+  return Expr::binary(l->cast_to(st, schema), op, r->cast_to(st, schema));
+}
+
 ExprRef SqlToRel::rex(const ASTRef& sql, const Schema& schema, const Scope* scope) const {
   switch (sql->kind) {
     case ASTNode::SQLLong: return Expr::literal(ScalarValue::Int64(sql->lval));
@@ -404,12 +414,30 @@ ExprRef SqlToRel::rex(const ASTRef& sql, const Schema& schema, const Scope* scop
         case SQLOperator::Like: op = Operator::Like; break;
         default: op = Operator::NotLike; break;
       }
-      ExprRef left_expr = rex(sql->left, schema, scope), right_expr = rex(sql->right, schema, scope);
-      DataType lt = left_expr->get_type(schema), rt = right_expr->get_type(schema), st;
-      if (!get_supertype(lt, rt, &st))
-        fail(DFGPU_ERR_GENERAL, std::string("No common supertype found for binary operator ") + operator_debug(op) + " with input types " +
-                                    datatype_debug(lt) + " and " + datatype_debug(rt));
-      return Expr::binary(left_expr->cast_to(st, schema), op, right_expr->cast_to(st, schema));
+      return coerced_binary(rex(sql->left, schema, scope), op, rex(sql->right, schema, scope), schema);
+    }
+    case ASTNode::SQLCase: {
+      // the simple form CASE x WHEN a THEN .. is the searched form with conditions x Eq a; the THEN / ELSE values are cast
+      // to their supertype, as the operands of a binary operator are
+      ExprRef x = sql->left ? rex(sql->left, schema, scope) : nullptr;
+      std::vector<ExprRef> args;
+      for (size_t i = 0; i < sql->args.size(); i++) {
+        ExprRef a = rex(sql->args[i], schema, scope);
+        args.push_back(x && i % 2 == 0 ? coerced_binary(x, Operator::Eq, a, schema) : a);
+      }
+      if (sql->right) args.push_back(rex(sql->right, schema, scope));
+      std::vector<size_t> vals;  // the THEN values, then the ELSE
+      for (size_t i = 1; i < args.size(); i += 2) vals.push_back(i);
+      if (args.size() % 2) vals.push_back(args.size() - 1);
+      DataType st = args[1]->get_type(schema);
+      for (size_t k : vals) {
+        const DataType t = args[k]->get_type(schema), prev = st;
+        if (!get_supertype(prev, t, &st))
+          fail(DFGPU_ERR_GENERAL, std::string("No common supertype found for CASE with input types ") + datatype_debug(prev) + " and " +
+                                      datatype_debug(t));
+      }
+      for (size_t k : vals) args[k] = args[k]->cast_to(st, schema);
+      return Expr::case_when(std::move(args));
     }
     case ASTNode::SQLFunction: {
       const std::string lid = lower(sql->id);

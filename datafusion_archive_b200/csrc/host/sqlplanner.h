@@ -34,6 +34,7 @@ class SqlToRel {
     std::vector<SchemaRef> far;
   };
   ExprRef rex(const ASTRef& sql, const Schema& schema, const Scope* scope) const;
+  static ExprRef coerced_binary(const ExprRef& l, Operator op, const ExprRef& r, const Schema& schema);
   ExprRef plan_where(const ASTRef& where, const Schema& schema, PlanRef* input) const;
   PlanRef plan_subquery(const ASTNode& term, PlanRef left, const std::vector<SchemaRef>& far) const;
   std::shared_ptr<SchemaProvider> schema_provider_;

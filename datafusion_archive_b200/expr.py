@@ -189,6 +189,32 @@ class Utf8Function(Expr):
         return "%s(%s)" % (self.name, ", ".join(repr(a) for a in self.args))
 
 
+class Case(Expr):
+    """CASE WHEN c1 THEN v1 [WHEN ..] [ELSE e] END (DFGPU_OP_CASE): `whens` is a list of (condition, value) pairs,
+    `else_` the ELSE value or None.  Like the C ABI, it casts nothing: every value has the result type."""
+
+    def __init__(self, whens, else_=None):
+        self.whens = [(c, _wrap(v)) for c, v in whens]
+        self.else_ = None if else_ is None else _wrap(else_)
+
+    def get_type(self, schema):
+        return self.whens[0][1].get_type(schema)
+
+    def _emit(self, schema, out):
+        for c, v in self.whens:
+            c._emit(schema, out)
+            v._emit(schema, out)
+        if self.else_ is not None:
+            self.else_._emit(schema, out)
+        i = A.Insn()
+        i.op, i.col, i.dtype = A.OP_CASE, 2 * len(self.whens) + (self.else_ is not None), self.get_type(schema)
+        out.append(i)
+
+    def __repr__(self):
+        s = "CASE" + "".join(" WHEN %r THEN %r" % w for w in self.whens)
+        return s + (" ELSE %r" % self.else_ if self.else_ is not None else "") + " END"
+
+
 class AggregateFunction:
     """Expr::AggregateFunction{name,args,return_type} (src/logicalplan.rs:162-166)."""
 
@@ -223,6 +249,10 @@ def col(i):
 
 def lit(v, dtype=None):
     return Literal(v, dtype)
+
+
+def case(whens, else_=None):
+    return Case(whens, else_)
 
 
 def fn(name, *args):

@@ -113,11 +113,31 @@ enum {
   DFGPU_OP_FN = 40,  /* Expr::ScalarFunction{name,args,return_type} logicalplan.rs:156-160: `col` = DFGPU_FN_* code,
                         `dtype` = Float64; the arguments come first, in order.  Additive: libraries older than it
                         reject it with "operator: 40". */
-  DFGPU_OP_UTF8_FN = 41 /* Expr::ScalarFunction of a Utf8 function: `col` = DFGPU_UTF8FN_* code, `dtype` = the result
+  DFGPU_OP_UTF8_FN = 41, /* Expr::ScalarFunction of a Utf8 function: `col` = DFGPU_UTF8FN_* code, `dtype` = the result
                            type (DFGPU_UTF8, or DFGPU_INT64 for LENGTH / OCTET_LENGTH).  The arguments come first: the
                            Utf8 operand (a column or another DFGPU_OP_UTF8_FN), then the function's DFGPU_OP_LIT Int64
                            values.  See "Utf8 functions" below.  Additive. */
+  DFGPU_OP_CASE = 42 /* CASE WHEN c1 THEN v1 [WHEN c2 THEN v2 ..] [ELSE e] END: the operands come first, in the order
+                        c1 v1 .. cn vn [e]; `col` = the number of operands, 2n, or 2n + 1 with an ELSE; `dtype` = the result
+                        type.  See "CASE" below.  Additive: libraries older than it reject it with "operator: 42". */
 };
+
+/* CASE (DFGPU_OP_CASE).
+ *   - Choice: the value of the first WHEN whose condition is true; a false or null condition is not taken.  When no WHEN
+ *     is taken, the ELSE value; without ELSE, null (with value 0 under the null, like every null an expression makes).
+ *     The result has the validity of the branch chosen.
+ *   - Laziness: a row raises DivideByZero only from the conditions up to and including the first true one and from the
+ *     value chosen; a branch not taken or a condition after the one taken never raises, in nested CASEs too.  The rule
+ *     of DFGPU_OP_DIV applies on top: only a row that survives the WHERE raises.
+ *   - Nulls: a CASE-made null is a null wherever a result can carry one, under a WHERE too (a projection then has a
+ *     validity bitmap, while the input columns' bitmaps are still dropped).  COUNT, AVG, COUNT(DISTINCT) and a reduction
+ *     without GROUP BY skip it; GROUP BY SUM / MIN / MAX and GROUP BY keys read its value 0.
+ *   - Types: every condition is Boolean (DFGPU_ERR_EXECUTION "CASE WHEN condition did not evaluate to boolean"); every
+ *     THEN / ELSE operand has one numeric or Boolean dtype, the result type (DFGPU_ERR_EXECUTION "CASE branch types
+ *     differ: Int64 and Float64"); a Utf8 result is DFGPU_ERR_NOT_IMPLEMENTED "CASE with a Utf8 result".  Utf8
+ *     predicates are conditions like any other.  An operand count below 2 or above the operands present, or a `dtype`
+ *     other than the result type, is DFGPU_ERR_GENERAL "malformed expression program".
+ *   - A CASE may appear wherever a numeric or Boolean expression may; its operands are any expressions, CASE included. */
 
 /* Built-in scalar functions (DFGPU_OP_FN).  The reference declares Expr::ScalarFunction and plans it
  * (sqlplanner.rs:343-365: every argument cast to the declared type) but never executes it

@@ -7,7 +7,8 @@ Covers: the mbarrier / cp.async.bulk pipeline of k_filter_project_tma (full, rag
 scan, dual ring), the direct filter kernel, the CAS / RED table of k_hash_agg_lean / _plain / interpreter, table
 growth with overflow replay, the shared-memory front tables, wide-key slots (busy / ready publication) and the
 chunked host pipelines, and the
-join's build, probe and gathers."""
+join's build, probe and gathers, and CASE in the extended interpreter: its validity bytes under a WHERE (out_vbytes,
+k_pack_valid), the null-aware reduce, the group scan and the TMA interpreter loop."""
 import os
 import sys
 
@@ -16,7 +17,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from datafusion_archive_b200 import _abi as A  # noqa: E402
 from datafusion_archive_b200 import engine, workloads  # noqa: E402
-from datafusion_archive_b200.expr import AggregateFunction, col, lit  # noqa: E402
+from datafusion_archive_b200.expr import AggregateFunction, case, col, lit  # noqa: E402
 
 ctx = engine.GpuContext(0)
 rng = np.random.default_rng(1)
@@ -234,5 +235,28 @@ assert sr.nrows == sum(1 for v in jup.to_pylist() if v.lower() in jcount)
 sr.free(); sj.free(); sbb.free(); spb.free()
 os.environ.pop("DFGPU_JOIN_TAG_BITS", None)
 print("semi join ok", flush=True)
+
+# 13. CASE: the direct kernel's validity bytes of a CASE without ELSE under a WHERE and k_pack_valid's ballots and zero
+# count (a ragged last word), the NULLS kernel without a WHERE, the TMA interpreter loop (CASE with ELSE), and the reduce
+# and group scan counting CASE-made nulls under a fused WHERE
+for n in [1, 31, 33, 300_001]:
+    a = rng.random(n)
+    nn = case([(col(0) > lit(0.5), col(0))])
+    v, ok = (lambda c: c if isinstance(c, tuple) else (c, np.ones(len(c), bool)))(fp([a], col(0) < lit(0.9), [nn])[0])
+    sel = a < 0.9
+    assert np.array_equal(ok, a[sel] > 0.5) and np.array_equal(v[ok], a[sel][a[sel] > 0.5]), n
+    c = fp([a], None, [nn])[0]
+    c = c if isinstance(c, tuple) else (c, np.ones(len(c), bool))
+    assert np.array_equal(c[1], a > 0.5), n
+    o = fp([a], None, [case([(col(0) > lit(0.5), col(0))], lit(0.0))])[0]
+    assert np.array_equal(o, np.where(a > 0.5, a, 0.0)), n
+kc = rng.integers(0, 1000, 300_001, dtype=np.int64)
+vc = rng.random(300_001)
+cnt = agg([kc, vc], [], [AggregateFunction("count", case([(col(1) > lit(0.5), col(1))]))], nb=2, pred=col(0) > lit(100))
+assert cnt[0][0] == np.count_nonzero((vc > 0.5) & (kc > 100))
+g = agg([kc, vc], [col(0)], [AggregateFunction("count", case([(col(1) > lit(0.5), col(1))]))], pred=col(0) > lit(100))
+exp = np.bincount(kc[(vc > 0.5) & (kc > 100)], minlength=1000)
+assert np.array_equal(np.asarray(g[1]), exp[np.asarray(g[0])])
+print("case ok", flush=True)
 ctx.close()
 print("SANITIZE_CASES_OK")
