@@ -384,12 +384,14 @@ dfgpu_batch* upload(dfgpu_ctx* gpu, const RecordBatch& batch, const Pruned& p) {
   return out;
 }
 
+// `schema`'s columns of `r`: its first schema->fields.size() columns, or all of them when it has no fields
 RecordBatch download(dfgpu_result* r, SchemaRef schema) {
   RecordBatch out;
   out.schema = std::move(schema);
   int64_t nrows = 0;
   int ncols = 0;
   GPU_CHECK(dfgpu_result_shape(r, &nrows, &ncols));
+  if (out.schema && !out.schema->fields.empty()) ncols = std::min(ncols, int(out.schema->fields.size()));
   out.num_rows = nrows;
   for (int i = 0; i < ncols; i++) {
     auto a = std::make_shared<Array>();
@@ -691,9 +693,38 @@ std::optional<RecordBatch> SharedScanRelation::next() {
 }
 
 GpuAggregateRelation::GpuAggregateRelation(dfgpu_ctx* gpu, SchemaRef schema, RelationRef input, std::vector<ExprRef> group_expr,
-                                           std::vector<ExprRef> aggr_expr, ExprRef predicate)
+                                           std::vector<ExprRef> aggr_expr, ExprRef predicate, std::optional<ResultStage> stage)
     : gpu_(gpu), schema_(std::move(schema)), input_(std::move(input)), group_expr_(std::move(group_expr)), aggr_expr_(std::move(aggr_expr)),
-      predicate_(std::move(predicate)) {}
+      predicate_(std::move(predicate)), stage_(std::move(stage)) {}
+
+RecordBatch GpuAggregateRelation::finish(dfgpu_aggstate* st) {
+  ResultGuard r;
+  GPU_CHECK(dfgpu_aggregate_finish(st, &r.r));
+  if (!stage_) return download(r.r, schema_);
+  // every rank holds the same global result, so each sorts it alike and no collective is needed
+  const Schema& as = *stage_->aggregate_schema;
+  BatchGuard view;  // freed before the result it views
+  GPU_CHECK(dfgpu_result_as_batch(r.r, &view.b));
+  const Pruned cols = prune({}, as.fields.size(), true);
+  std::vector<dfgpu_insn> keep;
+  if (stage_->keep) lower(*stage_->keep, as, cols.remap, keep);
+  std::vector<ExprRef> keys;
+  std::vector<int32_t> desc;
+  for (auto& s : stage_->sort) {
+    keys.push_back(s->left);
+    desc.push_back(s->asc ? 0 : 1);
+  }
+  if (stage_->ordered)
+    for (size_t k = 0; k < group_expr_.size(); k++) {
+      keys.push_back(Expr::column(k));
+      desc.push_back(0);
+    }
+  const Programs kp(keys, as, cols);
+  ResultGuard sorted;
+  GPU_CHECK(dfgpu_sort(gpu_, view.b, keep.data(), int(keep.size()), kp.ptr.data(), kp.len.data(), desc.data(), int(keys.size()), stage_->limit,
+                       &sorted.r));
+  return download(sorted.r, schema_);
+}
 
 std::optional<RecordBatch> ShardRelation::next() {
   auto batch = input_->next();
@@ -803,9 +834,7 @@ std::optional<RecordBatch> GpuAggregateRelation::next() {
         aggs[a]._pad = 0;
       }
       GPU_CHECK(dfgpu_aggregate_create(gpu_, kptr.data(), klen.data(), int(kptr.size()), aggs.data(), int(aggs.size()), 0, &st));
-      ResultGuard r;
-      GPU_CHECK(dfgpu_aggregate_finish(st, &r.r));
-      return download(r.r, schema_);
+      return finish(st);
     }
     if (!group_expr_.empty()) {
       RecordBatch out;
@@ -827,9 +856,7 @@ std::optional<RecordBatch> GpuAggregateRelation::next() {
     }
     GPU_CHECK(dfgpu_aggregate_create(gpu_, nullptr, nullptr, 0, aggs.data(), int(aggs.size()), 0, &st));
   }
-  ResultGuard r;
-  GPU_CHECK(dfgpu_aggregate_finish(st, &r.r));
-  return download(r.r, schema_);
+  return finish(st);
 }
 
 // ---- ExecutionContext ----------------------------------------------------------------------------------
@@ -872,6 +899,30 @@ PlanRef ExecutionContext::plan(const std::string& sql) {
 RelationRef ExecutionContext::sql(const std::string& sql) { return execute(plan(sql)); }
 
 namespace {
+// The Aggregate under the result stage `top` of an aggregate query (Projection? Limit? Sort? Selection? over it, at
+// least one of them), with the stage in *st; null when `top` is not one
+const LogicalPlan* aggregate_under(const LogicalPlan& top, GpuAggregateRelation::ResultStage* st) {
+  const LogicalPlan* p = &top;
+  if (p->kind == LogicalPlan::Projection) p = p->input.get();
+  if (p->kind == LogicalPlan::Limit) {
+    st->limit = int64_t(p->limit);
+    st->ordered = true;
+    p = p->input.get();
+  }
+  if (p->kind == LogicalPlan::Sort) {
+    st->sort = p->expr;
+    st->ordered = true;
+    p = p->input.get();
+  }
+  if (p->kind == LogicalPlan::Selection) {
+    st->keep = p->expr[0];
+    p = p->input.get();
+  }
+  if (p == &top || p->kind != LogicalPlan::Aggregate) return nullptr;
+  st->aggregate_schema = p->schema();
+  return p;
+}
+
 void count_scans(const LogicalPlan& p, std::map<std::string, int>& n) {
   if (p.kind == LogicalPlan::TableScan) n[p.table_name]++;
   if (p.input) count_scans(*p.input, n);
@@ -895,6 +946,28 @@ RelationRef ExecutionContext::execute(const PlanRef& plan) {
 
 RelationRef ExecutionContext::execute_node(const PlanRef& plan, const std::set<size_t>* needed, bool shard) {
   if (verbose) printf("Logical plan: %s\n", plan->debug().c_str());
+  GpuAggregateRelation::ResultStage stage;
+  const LogicalPlan* agg = aggregate_under(*plan, &stage);
+  if (agg || plan->kind == LogicalPlan::Aggregate) {  // context.rs:162-192 -> AggregateRelation
+    // Aggregate{input: Selection{expr, input}} (what `SELECT .. WHERE .. GROUP BY ..` plans to,
+    // sqlplanner.rs:93-96): the reference stacks FilterRelation under AggregateRelation; here the predicate is
+    // handed to the aggregate's scan kernel and only the columns it, the keys and the arguments read are uploaded
+    std::optional<GpuAggregateRelation::ResultStage> result_stage;
+    if (agg) result_stage = stage;
+    else agg = plan.get();
+    ExprRef pred;
+    PlanRef src = agg->input;
+    if (src->kind == LogicalPlan::Selection) {
+      pred = src->expr[0];
+      src = src->input;
+    }
+    std::set<size_t> used;
+    for (auto& e : agg->group_expr) collect_columns(*e, used);
+    for (auto& e : agg->aggr_expr) collect_columns(*e, used);
+    if (pred) collect_columns(*pred, used);
+    RelationRef input_rel = execute_node(src, &used, shard);
+    return std::make_shared<GpuAggregateRelation>(gpu_, plan->schema(), input_rel, agg->group_expr, agg->aggr_expr, pred, result_stage);
+  }
   switch (plan->kind) {
     case LogicalPlan::TableScan: {
       auto it = datasources_->find(plan->table_name);
@@ -951,23 +1024,6 @@ RelationRef ExecutionContext::execute_node(const PlanRef& plan, const std::set<s
       for (auto& e : plan->expr)  // projection.rs:52-57: (name, type, nullable = true)
         schema->fields.push_back(Field{runtime_expr_name(*e, in_schema), e->get_type(in_schema), true});
       return std::make_shared<GpuFilterProjectRelation>(gpu_, input_rel, pred, plan->expr, schema);
-    }
-    case LogicalPlan::Aggregate: {  // context.rs:162-192 -> AggregateRelation
-      // Aggregate{input: Selection{expr, input}} (what `SELECT .. WHERE .. GROUP BY ..` plans to,
-      // sqlplanner.rs:93-96): the reference stacks FilterRelation under AggregateRelation; here the predicate is
-      // handed to the aggregate's scan kernel and only the columns it, the keys and the arguments read are uploaded
-      ExprRef pred;
-      PlanRef src = plan->input;
-      if (src->kind == LogicalPlan::Selection) {
-        pred = src->expr[0];
-        src = src->input;
-      }
-      std::set<size_t> used;
-      for (auto& e : plan->group_expr) collect_columns(*e, used);
-      for (auto& e : plan->aggr_expr) collect_columns(*e, used);
-      if (pred) collect_columns(*pred, used);
-      RelationRef input_rel = execute_node(src, &used, shard);
-      return std::make_shared<GpuAggregateRelation>(gpu_, plan->schema(), input_rel, plan->group_expr, plan->aggr_expr, pred);
     }
     default:
       fail(DFGPU_ERR_NOT_IMPLEMENTED, "Limit / Sort / EmptyRelation plans are not executable (reference: unimplemented!() at context.rs:194)");

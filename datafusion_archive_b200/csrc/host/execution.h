@@ -121,18 +121,30 @@ class ShardRelation : public Relation {
 // AggregateRelation: src/execution/aggregate.rs:38-61, 615-631.  `predicate` (may be null) is the expression
 // of a Selection directly under the Aggregate (context.rs:126-139 builds FilterRelation there): it is fused
 // into the scan kernel instead of materialising the filtered batch.
+// A result stage (the Selection / Sort / Limit / Projection the planner puts over the Aggregate of a query with HAVING,
+// ORDER BY or LIMIT) runs on the aggregate's device result through dfgpu_sort: the rows where `keep` is true, ordered
+// by `sort`, then by the GROUP BY keys ascending when `ordered`, the first `limit`, and the first `visible` columns.
 class GpuAggregateRelation : public Relation {
  public:
+  struct ResultStage {
+    ExprRef keep;               // HAVING over the aggregate's output, or null
+    std::vector<ExprRef> sort;  // Expr::Sort over the aggregate's output
+    bool ordered = false;       // a Sort or a Limit: the GROUP BY keys break the remaining ties
+    int64_t limit = -1;         // < 0: no LIMIT
+    SchemaRef aggregate_schema;  // the aggregate's own output: GROUP BY keys, then every aggregate, hidden ones included
+  };
   GpuAggregateRelation(dfgpu_ctx* gpu, SchemaRef schema, RelationRef input, std::vector<ExprRef> group_expr, std::vector<ExprRef> aggr_expr,
-                       ExprRef predicate = nullptr);
+                       ExprRef predicate = nullptr, std::optional<ResultStage> stage = std::nullopt);
   std::optional<RecordBatch> next() override;
   const SchemaRef& schema() const override { return schema_; }
  private:
+  RecordBatch finish(dfgpu_aggstate* st);  // dfgpu_aggregate_finish, the result stage and the download
   dfgpu_ctx* gpu_;
   SchemaRef schema_;
   RelationRef input_;
   std::vector<ExprRef> group_expr_, aggr_expr_;
   ExprRef predicate_;
+  std::optional<ResultStage> stage_;
   bool end_of_results_ = false;
 };
 

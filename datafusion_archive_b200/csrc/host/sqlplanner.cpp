@@ -102,6 +102,7 @@ PlanRef SqlToRel::sql_to_rel(const ASTRef& sql) const {
         a->group_expr = group_expr;
         a->aggr_expr = aggr_expr;
         a->schema_ = aggr_schema;
+        if (sql->having || sql->has_order_by || sql->limit) return plan_aggregate_result(*sql, a, expr, *input_schema);
         return a;
       }
 
@@ -190,6 +191,97 @@ void and_terms(const ExprRef& e, std::vector<ExprRef>& out) {
   }
 }
 }  // namespace
+
+namespace {
+// `e` (over the aggregate's input) over the aggregate's output: a subtree equal to a GROUP BY expression (equal plan
+// text) becomes that column, an aggregate call the column of the equal aggregate, appended to `aggr` (hidden) when
+// there is none.  A column of the input left over is an error.
+ExprRef over_aggregate(const ExprRef& e, const std::vector<ExprRef>& group, std::vector<ExprRef>& aggr, const Schema& input) {
+  const std::string d = e->debug();
+  for (size_t k = 0; k < group.size(); k++)
+    if (group[k]->debug() == d) return Expr::column(k);
+  if (e->kind == Expr::AggregateFunction) {
+    size_t i = 0;
+    while (i < aggr.size() && aggr[i]->debug() != d) i++;
+    if (i == aggr.size()) aggr.push_back(e);
+    return Expr::column(group.size() + i);
+  }
+  if (e->kind == Expr::Column)
+    fail(DFGPU_ERR_GENERAL, "Column '" + input.fields[e->index].name + "' must appear in the GROUP BY clause or be used in an aggregate function");
+  auto c = std::make_shared<Expr>(*e);
+  if (c->left) c->left = over_aggregate(c->left, group, aggr, input);
+  if (c->right) c->right = over_aggregate(c->right, group, aggr, input);
+  for (auto& a : c->args) a = over_aggregate(a, group, aggr, input);
+  return c;
+}
+}  // namespace
+
+// Aggregate -> Selection (HAVING) -> Sort -> Limit -> Projection (only when HAVING or ORDER BY added hidden aggregates,
+// to drop them).  HAVING and the ORDER BY keys are planned over the input like the SELECT list, then rewritten over the
+// aggregate's output; an integer literal k in ORDER BY is the k-th SELECT-list item.
+PlanRef SqlToRel::plan_aggregate_result(const ASTNode& select, std::shared_ptr<LogicalPlan> a, const std::vector<ExprRef>& select_exprs,
+                                        const Schema& input_schema) const {
+  const size_t visible = a->group_expr.size() + a->aggr_expr.size();
+  std::vector<ExprRef> aggr = a->aggr_expr;
+  ExprRef having;
+  if (select.having) having = over_aggregate(sql_to_rex(select.having, input_schema), a->group_expr, aggr, input_schema);
+  std::vector<ExprRef> sort;
+  for (auto& o : select.order_by) {
+    ExprRef e;
+    if (o.expr->kind == ASTNode::SQLLong) {
+      const long long k = o.expr->lval;
+      if (k < 1 || size_t(k) > select_exprs.size()) fail(DFGPU_ERR_GENERAL, "ORDER BY position " + std::to_string(k) + " is not in select list");
+      e = select_exprs[size_t(k - 1)];
+    } else {
+      e = sql_to_rex(o.expr, input_schema);
+    }
+    sort.push_back(Expr::sort(over_aggregate(e, a->group_expr, aggr, input_schema), o.asc));
+  }
+  std::vector<ExprRef> all_fields = a->group_expr;
+  for (auto& x : aggr) all_fields.push_back(x);
+  auto schema = std::make_shared<Schema>();
+  schema->fields = exprlist_to_fields(all_fields, input_schema);
+  a->aggr_expr = aggr;
+  a->schema_ = schema;
+  if (having && having->get_type(*schema) != DFGPU_BOOL) fail(DFGPU_ERR_GENERAL, "HAVING expression did not evaluate to boolean");
+  for (auto& s : sort)
+    if (s->get_type(*schema) == DFGPU_BOOL) fail(DFGPU_ERR_NOT_IMPLEMENTED, "ORDER BY a Boolean expression is not supported: " + s->left->debug());
+  PlanRef plan = a;
+  if (having) {
+    auto s = std::make_shared<LogicalPlan>();
+    s->kind = LogicalPlan::Selection;
+    s->expr.push_back(having);
+    s->input = plan;
+    plan = s;
+  }
+  if (!sort.empty()) {
+    auto s = std::make_shared<LogicalPlan>();
+    s->kind = LogicalPlan::Sort;
+    s->expr = sort;
+    s->input = plan;
+    s->schema_ = schema;
+    plan = s;
+  }
+  if (select.limit) {
+    if (select.limit->kind != ASTNode::SQLLong) fail(DFGPU_ERR_GENERAL, "LIMIT parameter is not a number");
+    auto l = std::make_shared<LogicalPlan>();
+    l->kind = LogicalPlan::Limit;
+    l->limit = size_t(select.limit->lval);
+    l->schema_ = schema;
+    l->input = plan;
+    plan = l;
+  }
+  if (aggr.size() + a->group_expr.size() > visible) {
+    auto proj = std::make_shared<LogicalPlan>();
+    proj->kind = LogicalPlan::Projection;
+    for (size_t i = 0; i < visible; i++) proj->expr.push_back(Expr::column(i));
+    proj->input = plan;
+    proj->schema_ = std::make_shared<Schema>();
+    proj->schema_->fields.assign(schema->fields.begin(), schema->fields.begin() + long(visible));
+    plan = proj;
+  }
+  return plan;
+}
 
 // FROM table_ref { JOIN table_ref ON expr }: a left-deep chain of Join nodes.  Each ON clause is planned like a WHERE
 // clause over the joined schema; its top-level AND terms `l Eq r` with l over the left input only and r over the right

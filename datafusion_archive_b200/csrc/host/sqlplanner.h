@@ -37,6 +37,9 @@ class SqlToRel {
   static ExprRef coerced_binary(const ExprRef& l, Operator op, const ExprRef& r, const Schema& schema);
   ExprRef plan_where(const ASTRef& where, const Schema& schema, PlanRef* input) const;
   PlanRef plan_subquery(const ASTNode& term, PlanRef left, const std::vector<SchemaRef>& far) const;
+  // HAVING, ORDER BY and LIMIT of an aggregate query over its Aggregate (no reference counterpart: sqlplanner.rs:112)
+  PlanRef plan_aggregate_result(const ASTNode& select, std::shared_ptr<LogicalPlan> aggregate, const std::vector<ExprRef>& select_exprs,
+                                const Schema& input_schema) const;
   std::shared_ptr<SchemaProvider> schema_provider_;
 };
 

@@ -14,14 +14,13 @@
 //   k_join_emit     per OUTPUT position: the probe row owning it (a search of the offsets restricted to the rows of the
 //                   CTA's tile) and its build row.  The work is spread by output, so a probe row with millions of
 //                   matches is written by as many threads as rows with one match each.
-//   gathers         k_join_gather<T> (1, 2, 4, 8 bytes), k_join_gather_bits (validity and Boolean values), and
-//                   gather_utf8 (utf8_gather.cu) for Utf8 columns
+//   gathers         gather_column (gather.cuh)
 //
 // Semi / anti join (dfgpu_join_semi), on the same build:
 //   k_join_mark     per probe row: one pass bit (match for semi, no match for anti), written as 32-bit words with
 //                   __ballot_sync, and each tile's pass count (k_join_utf8_mark for a key with Utf8 parts)
 //   scan            the tile counts become each tile's output offset; the total is the output row count
-//   k_join_select   per tile: the passing row numbers in row order (a prefix over the mask words' popcounts)
+//   k_join_select   per tile: the passing row numbers in row order (select_rows, gather.cuh)
 //   gathers         as above, for the probe columns only
 //
 // A key with Utf8 parts takes its own build and count kernels; the scan, k_join_scatter, k_join_emit and the gathers
@@ -37,17 +36,16 @@
 //                       (integer word, then each Utf8 part's length and bytes) before the slot counts as a match
 #include <memory>
 
+#include "gather.cuh"
 #include "hash_table.cuh"
 #include "scan.cuh"
 #include "utf8_words.cuh"
 
 namespace dfgpu {
 
-void gather_utf8(dfgpu_ctx* ctx, const DevColumn& src, const unsigned long long* d_idx, long long nsel, DevColumn* out);
-
 constexpr int kMaxJoinKeys = 4;
 constexpr long long JN_MIN_CAP = 1024;  // the build table never grows: no floor beyond a small minimum
-constexpr int JN_THREADS = 256;
+constexpr int JN_THREADS = SEL_THREADS;
 constexpr int EMIT_TILE = 2048;  // output positions per CTA tile of k_join_emit
 
 // The key columns of one input: each part is read as its raw integer, sign- or zero-extended to 64 bits, masked to its
@@ -334,36 +332,7 @@ __global__ void __launch_bounds__(JN_THREADS) k_join_utf8_count(JoinKeys k, Utf8
 // is set (anti; null-aware anti only over an empty build side).  The rows are cut into tiles of MARK_TILE: k_join_mark
 // writes the tile's MARK_TILE / 32 mask words (warp w of the CTA writes words i * 8 + w, one __ballot_sync each) and
 // its pass count; the counts are scanned into tile offsets; k_join_select writes the passing row numbers of each tile,
-// in row order, at its offset.
-constexpr int MARK_TILE = 2048;
-constexpr int MARK_WORDS = MARK_TILE / 32;
-constexpr int WARP_WORDS = MARK_WORDS / (JN_THREADS / 32);  // mask words per warp and tile: 8
-
-template <class Pass>
-__device__ __forceinline__ void mark_tiles(long long n, unsigned* __restrict__ mask, unsigned* __restrict__ tile_cnt, Pass pass) {
-  __shared__ unsigned s_cnt[JN_THREADS / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const long long ntiles = (n + MARK_TILE - 1) / MARK_TILE;
-  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    unsigned c = 0;
-#pragma unroll 1
-    for (int i = 0; i < MARK_TILE / JN_THREADS; i++) {
-      const long long r = tile * MARK_TILE + i * JN_THREADS + threadIdx.x;
-      const unsigned w = __ballot_sync(0xffffffffu, r < n && pass(r));
-      c += (unsigned)__popc(w);
-      if (lane == 0) mask[r >> 5] = w;
-    }
-    if (lane == 0) s_cnt[warp] = c;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      unsigned total = 0;
-      for (int w = 0; w < JN_THREADS / 32; w++) total += s_cnt[w];
-      tile_cnt[tile] = total;
-    }
-    __syncthreads();
-  }
-}
-
+// in row order, at its offset (mark_tiles and select_rows: gather.cuh).
 __global__ void __launch_bounds__(JN_THREADS) k_join_mark(JoinKeys k, long long n, ProbeRule t, const unsigned long long* __restrict__ keys,
                                                          const unsigned long long* __restrict__ start, int anti, int null_pass,
                                                          unsigned* __restrict__ mask, unsigned* __restrict__ tile_cnt) {
@@ -385,37 +354,6 @@ __global__ void __launch_bounds__(JN_THREADS) k_join_utf8_mark(JoinKeys k, Utf8K
     if (!utf8_tag(k, u, tag_mask, r, &word, &tag)) return null_pass != 0;
     return find_utf8_slot(t, tags, words, rep, u, r, b, word, tag, &h) != (anti != 0);
   });
-}
-
-// One tile per CTA iteration: each warp takes 8 of the tile's mask words; a prefix over the words' popcounts (within the
-// warp, then over the warps) places each word's rows, and the lanes of a word write its set bits' row numbers together.
-__global__ void __launch_bounds__(JN_THREADS) k_join_select(const unsigned* __restrict__ mask, long long ntiles,
-                                                           const unsigned long long* __restrict__ tile_off, unsigned* __restrict__ out) {
-  __shared__ unsigned s_warp[JN_THREADS / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const unsigned below = (1u << lane) - 1u;
-  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const long long w0 = tile * MARK_WORDS + warp * WARP_WORDS;
-    const unsigned word = lane < WARP_WORDS ? mask[w0 + lane] : 0u;
-    const unsigned c = (unsigned)__popc(word);
-    unsigned incl = c;
-#pragma unroll
-    for (int o = 1; o < WARP_WORDS; o <<= 1) {
-      const unsigned x = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += x;
-    }
-    if (lane == WARP_WORDS - 1) s_warp[warp] = incl;
-    __syncthreads();
-    unsigned before = 0;
-    for (int w = 0; w < warp; w++) before += s_warp[w];
-    const unsigned long long at = tile_off[tile] + before;
-#pragma unroll
-    for (int j = 0; j < WARP_WORDS; j++) {
-      const unsigned wj = __shfl_sync(0xffffffffu, word, j), ej = __shfl_sync(0xffffffffu, incl - c, j);
-      if ((wj >> lane) & 1u) out[at + ej + (unsigned)__popc(wj & below)] = (unsigned)((w0 + j) * 32 + lane);
-    }
-    __syncthreads();
-  }
 }
 
 // the last row p in [lo, hi] with off[p] <= o: the probe row whose output range holds position o
@@ -445,35 +383,6 @@ __global__ void __launch_bounds__(JN_THREADS) k_join_emit(const unsigned long lo
     }
     __syncthreads();
   }
-}
-
-// ---- gathers -----------------------------------------------------------------------------------------------------------
-template <class T>
-__global__ void __launch_bounds__(JN_THREADS) k_join_gather(const T* __restrict__ src, const unsigned* __restrict__ idx, long long n, T* __restrict__ out) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) out[i] = src[idx[i]];
-}
-// bit i of the output = bit idx[i] of src, written as whole 32-bit words; `zeros` (may be null) counts the zero bits
-__global__ void __launch_bounds__(JN_THREADS) k_join_gather_bits(const unsigned char* __restrict__ src, const unsigned* __restrict__ idx, long long n,
-                                                                unsigned* __restrict__ out, unsigned long long* __restrict__ zeros) {
-  const long long padded = (n + 31) & ~31ll;
-  unsigned long long z = 0;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < padded; i += (long long)gridDim.x * blockDim.x) {
-    bool bit = false;
-    if (i < n) {
-      const unsigned j = idx[i];
-      bit = (src[j >> 3] >> (j & 7)) & 1;
-    }
-    const unsigned w = __ballot_sync(0xffffffffu, bit);
-    if ((threadIdx.x & 31) == 0) {
-      out[i >> 5] = w;
-      const long long valid = min(32ll, n - i);
-      z += (unsigned long long)(valid - __popc(w));
-    }
-  }
-  if (zeros && z) atomicAdd(zeros, z);
-}
-__global__ void __launch_bounds__(JN_THREADS) k_join_widen(const unsigned* __restrict__ idx, long long n, unsigned long long* __restrict__ out) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) out[i] = idx[i];
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------------------
@@ -583,49 +492,6 @@ DevColumn copy_column(dfgpu_ctx* ctx, const DevColumn& s, long long n) {
     DF_CUDA(cudaMemcpyAsync(d.offsets, s.offsets, size_t(n + 1) * 4, cudaMemcpyDeviceToDevice, ctx->stream));
   }
   return d;
-}
-
-// Gather one column by a row-index list.  `idx64` is filled on first use (Utf8 columns take 64-bit indices).
-void gather_column(dfgpu_ctx* ctx, const DevColumn& src, const unsigned* idx, long long n, DevBufs& scratch, unsigned long long*& idx64,
-                   unsigned long long* d_nulls, DevColumn* out) {
-  out->dtype = src.dtype;
-  const int grid = grid_for(ctx, n, JN_THREADS, 16);
-  if (src.dtype == DFGPU_UTF8) {
-    if (!idx64) {
-      idx64 = scratch.alloc<unsigned long long>(size_t(std::max(1ll, n)) * sizeof(unsigned long long));
-      if (n > 0) launch(ctx, "k_join_widen", k_join_widen, grid, JN_THREADS, PROFILED, idx, n, idx64);
-    }
-    gather_utf8(ctx, src, idx64, n, out);
-  } else if (src.dtype == DFGPU_BOOL) {
-    out->values_bytes = size_t((n + 31) / 32) * 4 + 4;
-    out->values = ctx->alloc(out->values_bytes);
-    if (n > 0)
-      launch(ctx, "k_join_gather_bits", k_join_gather_bits, grid, JN_THREADS, PROFILED, (const unsigned char*)src.values, idx, n, (unsigned*)out->values,
-             (unsigned long long*)nullptr);
-    out->values_bytes = size_t(n + 7) / 8;
-  } else {
-    const int w = dtype_width(src.dtype);
-    out->values_bytes = size_t(std::max(1ll, n)) * size_t(w);
-    out->values = ctx->alloc(out->values_bytes);
-    if (n > 0) {
-      switch (w) {
-        case 1: launch(ctx, "k_join_gather<1>", k_join_gather<unsigned char>, grid, JN_THREADS, PROFILED, (const unsigned char*)src.values, idx, n, (unsigned char*)out->values); break;
-        case 2: launch(ctx, "k_join_gather<2>", k_join_gather<unsigned short>, grid, JN_THREADS, PROFILED, (const unsigned short*)src.values, idx, n, (unsigned short*)out->values); break;
-        case 4: launch(ctx, "k_join_gather<4>", k_join_gather<unsigned>, grid, JN_THREADS, PROFILED, (const unsigned*)src.values, idx, n, (unsigned*)out->values); break;
-        default: launch(ctx, "k_join_gather<8>", k_join_gather<unsigned long long>, grid, JN_THREADS, PROFILED, (const unsigned long long*)src.values, idx, n, (unsigned long long*)out->values); break;
-      }
-    }
-  }
-  if (src.null_count > 0 && src.validity && n > 0) {
-    out->validity = (uint8_t*)ctx->alloc(size_t((n + 31) / 32) * 4);
-    DF_CUDA(cudaMemsetAsync(d_nulls, 0, 8, ctx->stream));
-    launch(ctx, "k_join_gather_bits", k_join_gather_bits, grid, JN_THREADS, PROFILED, (const unsigned char*)src.validity, idx, n, (unsigned*)out->validity, d_nulls);
-    out->null_count = (int64_t)read_word(ctx, d_nulls);
-    if (out->null_count == 0) {
-      ctx->free(out->validity);
-      out->validity = nullptr;
-    }
-  }
 }
 
 }  // namespace
@@ -860,7 +726,7 @@ extern "C" int dfgpu_join_semi(dfgpu_join* j, const dfgpu_batch* probe, const df
       m = (long long)scan_exclusive<unsigned, unsigned long long>(ctx, tile_cnt, tile_off, ntiles, true);
       idx = scratch.alloc<unsigned>(size_t(std::max(1ll, m)) * sizeof(unsigned));
       if (m > 0)
-        launch(ctx, "k_join_select", k_join_select, grid, JN_THREADS, PROFILED, (const unsigned*)mask, ntiles, (const unsigned long long*)tile_off, idx);
+        select_rows(ctx, grid, mask, ntiles, tile_off, idx);
     }
     auto res = std::make_unique<dfgpu_result>();
     res->ctx = ctx;

@@ -90,6 +90,8 @@ def lib():
     L.dfgpu_join_probe.argtypes = [vp, vp, C.POINTER(PI), PC, C.c_int, PC, C.c_int, PC, C.c_int, C.POINTER(vp)]
     L.dfgpu_join_semi.argtypes = [vp, vp, C.POINTER(PI), PC, C.c_int, C.c_int, PC, C.c_int, C.POINTER(vp)]
     L.dfgpu_join_free.argtypes = [vp]
+    L.dfgpu_sort.argtypes = [vp, vp, PI, C.c_int, C.POINTER(PI), PC, C.POINTER(C.c_int32), C.c_int, C.c_int64, C.POINTER(vp)]
+    L.dfgpu_result_as_batch.argtypes = [vp, C.POINTER(vp)]
     if L.dfgpu_abi_version() != A.ABI_VERSION:
         raise RuntimeError("libdfgpu.so ABI version mismatch")
     _LIB = L
@@ -379,6 +381,30 @@ class GpuContext:
         out = C.c_void_p()
         check(lib().dfgpu_join_build(self.h, batch.h, kptrs, klens, nk, carr, len(cols), C.byref(out)))
         return Join(self, out, keep_cols=cols)
+
+    # -- ORDER BY / LIMIT / HAVING ------------------------------------------------------------------
+    def sort(self, batch, keys=(), desc=None, keep=None, limit=-1):
+        """dfgpu_sort: every column of `batch` (a Batch, or a device Result viewed in place), the rows where `keep` is true,
+        stably ordered by the expressions `keys` (`desc[i]` true: descending), the first `limit` of them (< 0: all)."""
+        view = None
+        if isinstance(batch, Result):
+            h = C.c_void_p()
+            check(lib().dfgpu_result_as_batch(batch.h, C.byref(h)))
+            view = Batch(self, h, [batch.dtype(i) for i in range(batch.ncols)])
+            batch = view
+        try:
+            keep_alive = []
+            kptrs, klens, nk = A.make_programs([k.program(batch.schema) for k in keys], keep_alive)
+            kprog = keep.program(batch.schema) if keep is not None else []
+            karr = (A.Insn * max(1, len(kprog)))(*kprog)
+            d = list(desc) if desc is not None else [False] * nk
+            darr = (C.c_int32 * max(1, nk))(*[int(bool(x)) for x in d])
+            out = C.c_void_p()
+            check(lib().dfgpu_sort(self.h, batch.h, karr, len(kprog), kptrs, klens, darr, nk, limit, C.byref(out)))
+            return Result(self, out)
+        finally:
+            if view is not None:
+                view.free()
 
     # -- utilities ------------------------------------------------------------------------------
     def sync(self):

@@ -407,6 +407,29 @@ int dfgpu_join_semi(dfgpu_join* j, const dfgpu_batch* probe, const dfgpu_insn* c
                     const int* probe_cols, int n_probe_cols, dfgpu_result** out);
 int dfgpu_join_free(dfgpu_join* j);
 
+/* ---- ORDER BY / LIMIT / HAVING over a device result ----
+ * The reference plans LogicalPlan::Sort and LogicalPlan::Limit (src/sqlplanner.rs) but its ExecutionContext::execute
+ * leaves both unimplemented!() (src/execution/context.rs:113,194).  dfgpu_sort is what a Sort / Limit relation calls:
+ *   - Keep: the rows where `keep` (a Boolean postfix program over `in`) is true; a null or false row is dropped.
+ *     keep_len 0 keeps every row.  A program that is not Boolean is DFGPU_ERR_EXECUTION.
+ *   - Order: the kept rows, stably ordered by keys[0], then keys[1], ..; desc[i] != 0 orders key i descending (`desc`
+ *     may be NULL: all ascending).  Rows equal on every key keep their input order.  Integers order by value; floats
+ *     by the MIN / MAX accumulators' order (-0.0 before +0.0, every NaN equal and after +inf); Utf8 byte-wise
+ *     lexicographically, a proper prefix first, as Utf8 `<`.  A null is below every value: first ascending, last
+ *     descending.  A Boolean key is DFGPU_ERR_NOT_IMPLEMENTED.  nkeys 0 keeps the input order.
+ *   - Limit: the first `limit` rows of that order (limit < 0: all of them).
+ *   - Output: every column of `in`, with its dtype, validity and null count.  Key and keep programs that are not a
+ *     plain column are evaluated first exactly as a projection without a WHERE (dfgpu_filter_project).
+ *   - An input of 2^32 rows or more is DFGPU_ERR_NOT_IMPLEMENTED.
+ * The library knows nothing of GROUP BY: a caller wanting a total order over an aggregate's result appends its group
+ * key columns as the last, ascending keys. */
+int dfgpu_sort(dfgpu_ctx* ctx, const dfgpu_batch* in, const dfgpu_insn* keep, int keep_len, const dfgpu_insn* const* keys, const int* key_len,
+               const int32_t* desc, int nkeys, int64_t limit, dfgpu_result** out);
+/* A batch that views the columns of a device result without copying them (an aggregate's result goes into dfgpu_sort
+ * without a download and upload).  Free the view with dfgpu_batch_free before freeing the result.  A host-resident
+ * result is DFGPU_ERR_GENERAL. */
+int dfgpu_result_as_batch(const dfgpu_result* r, dfgpu_batch** out);
+
 /* ---- results ---- */
 int dfgpu_result_shape(const dfgpu_result* r, int64_t* nrows, int* ncols);
 int dfgpu_result_col_dtype(const dfgpu_result* r, int i, int32_t* dtype);

@@ -258,5 +258,16 @@ g = agg([kc, vc], [col(0)], [AggregateFunction("count", case([(col(1) > lit(0.5)
 exp = np.bincount(kc[(vc > 0.5) & (kc > 100)], minlength=1000)
 assert np.array_equal(np.asarray(g[1]), exp[np.asarray(g[0])])
 print("case ok", flush=True)
+# 14. ORDER BY / LIMIT / HAVING (dfgpu_sort): the keep mask's ragged last tile, a nullable Utf8 key's MSD rounds and
+# null pass, a skipped digit, the stable scatter's partial chunk and tile, and the gathers of a LIMIT inside a tile
+for n in [1, 33, 4097, 100_003]:
+    ks = pa.array(["k%d" % (i % 37) * (1 + i % 3) for i in range(n)], type=pa.string(), mask=np.arange(n) % 11 == 0)
+    kv = rng.integers(0, 300, n, dtype=np.int64)
+    keep = pa.array(np.arange(n) % 5 != 0, mask=np.arange(n) % 7 == 0)
+    b = ctx.upload([ks, kv, np.arange(n, dtype=np.int64), keep])
+    r = ctx.sort(b, keys=[col(0), col(1)], desc=[True, False], keep=col(3), limit=n // 2)
+    assert r.nrows == min(n // 2, int(np.count_nonzero((np.arange(n) % 5 != 0) & (np.arange(n) % 7 != 0)))), n
+    r.free(); b.free()
+print("sort ok", flush=True)
 ctx.close()
 print("SANITIZE_CASES_OK")

@@ -177,6 +177,15 @@ extern "C" {
         probe_cols: *const c_int, n_probe_cols: c_int, out: *mut *mut dfgpu_result,
     ) -> c_int;
     pub fn dfgpu_join_free(j: *mut dfgpu_join) -> c_int;
+    /// Sort / Limit over a device result (LogicalPlan::Sort / Limit, unimplemented!() at context.rs:113,194): keep the
+    /// rows where `keep` is true, order them stably by the keys (desc[i] != 0: descending), return the first `limit`
+    /// (< 0: all)
+    pub fn dfgpu_sort(
+        ctx: *mut dfgpu_ctx, input: *const dfgpu_batch, keep: *const dfgpu_insn, keep_len: c_int, keys: *const *const dfgpu_insn,
+        key_len: *const c_int, desc: *const i32, nkeys: c_int, limit: i64, out: *mut *mut dfgpu_result,
+    ) -> c_int;
+    /// a batch viewing a device result's columns (free it before the result)
+    pub fn dfgpu_result_as_batch(r: *const dfgpu_result, out: *mut *mut dfgpu_batch) -> c_int;
     pub fn dfgpu_result_shape(r: *const dfgpu_result, nrows: *mut i64, ncols: *mut c_int) -> c_int;
     pub fn dfgpu_result_col_dtype(r: *const dfgpu_result, i: c_int, dtype: *mut i32) -> c_int;
     pub fn dfgpu_result_col_bytes(r: *const dfgpu_result, i: c_int, nbytes: *mut i64) -> c_int;
