@@ -3126,13 +3126,7 @@ void assemble_outputs(dfgpu_aggstate* st, dfgpu_result* res) {
   unsigned long long h[kMaxAggs];
   read_words(ctx, d_nulls, sizeof(h), h);
   for (size_t i = 0; i < st->out_word.size(); i++) {
-    DevColumn& c = res->cols[nk + i];
-    if (!st->out_is_avg[i]) continue;
-    c.null_count = (int64_t)h[i];
-    if (c.null_count == 0) {  // no null: no bitmap, like every other aggregate column
-      ctx->free(c.validity);
-      c.validity = nullptr;
-    }
+    if (st->out_is_avg[i]) set_null_count(ctx, res->cols[nk + i], (int64_t)h[i]);
   }
 }
 }  // namespace

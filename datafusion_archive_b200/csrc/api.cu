@@ -94,6 +94,14 @@ void free_column(dfgpu_ctx* ctx, DevColumn& c) {
   c.offsets = nullptr;
 }
 
+void set_null_count(dfgpu_ctx* ctx, DevColumn& c, int64_t nulls) {
+  c.null_count = nulls;
+  if (nulls == 0) {
+    ctx->free(c.validity);
+    c.validity = nullptr;
+  }
+}
+
 }  // namespace dfgpu
 
 using namespace dfgpu;

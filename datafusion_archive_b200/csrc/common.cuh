@@ -252,6 +252,8 @@ struct DevBufs {
 
 // Returns a column's values, validity and offsets to the ctx pool and nulls them.
 void free_column(dfgpu_ctx* ctx, DevColumn& c);
+// Sets a column's null count, and frees its bitmap when it has no null: a column without nulls carries no bitmap.
+void set_null_count(dfgpu_ctx* ctx, DevColumn& c, int64_t nulls);
 }  // namespace dfgpu
 
 struct dfgpu_batch {

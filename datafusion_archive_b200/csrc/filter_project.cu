@@ -177,18 +177,10 @@ __global__ void __launch_bounds__(FP_THREADS) k_filter_project(const __grid_cons
   }
 }
 
-// one byte per row -> BooleanArray bits (LSB first); one warp packs 32 rows into one word
-__global__ void __launch_bounds__(256) k_pack_bits(const unsigned char* __restrict__ bytes, long long n, unsigned* __restrict__ words) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  const long long padded = (n + 31) / 32 * 32;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < padded; i += stride) {
-    const unsigned m = __ballot_sync(0xffffffffu, i < n && bytes[i] != 0);
-    if ((threadIdx.x & 31) == 0) words[i >> 5] = m;
-  }
-}
-// same, for validity bytes: also adds the number of zero bytes (the nulls) to *zeros
-__global__ void __launch_bounds__(256) k_pack_valid(const unsigned char* __restrict__ bytes, long long n, unsigned* __restrict__ words,
-                                                    unsigned long long* __restrict__ zeros) {
+// one byte per row -> bits (LSB first), one warp per 32 rows and output word; `zeros` (may be null) gains the number of
+// zero bytes: the nulls, when the bytes are validity
+__global__ void __launch_bounds__(256) k_pack_bits(const unsigned char* __restrict__ bytes, long long n, unsigned* __restrict__ words,
+                                                   unsigned long long* __restrict__ zeros) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   const long long padded = (n + 31) / 32 * 32;
   unsigned z = 0;
@@ -200,7 +192,10 @@ __global__ void __launch_bounds__(256) k_pack_valid(const unsigned char* __restr
       z += __popc(in & ~m);
     }
   }
-  if (z) atomicAdd(zeros, (unsigned long long)z);
+  if (zeros && z) atomicAdd(zeros, (unsigned long long)z);
+}
+static void pack_bits(dfgpu_ctx* ctx, const unsigned char* bytes, long long n, unsigned* words, unsigned long long* zeros) {
+  launch(ctx, "k_pack_bits", k_pack_bits, grid_for(ctx, (n + 31) / 32 * 32, 256, 8), 256, {}, bytes, n, words, zeros);
 }
 template <int DEPTH, bool NULLS = false>
 static void launch_fp(dfgpu_ctx* ctx, const FPParams& p) {
@@ -211,11 +206,71 @@ static void launch_fp(dfgpu_ctx* ctx, const FPParams& p) {
   launch(ctx, name.c_str(), k_filter_project<DEPTH, NULLS>, grid_for(ctx, p.ntiles, 1, per_sm), FP_THREADS, PROFILED, p);
 }
 
-}  // namespace dfgpu
-
-namespace dfgpu {
 void gather_utf8(dfgpu_ctx* ctx, const DevColumn& src, const unsigned long long* d_idx, long long nsel, DevColumn* out);
+
+// A batch of the given column types and no data, for typing programs without a device.  Its ctx is null: it owns
+// nothing and its destructor frees nothing.
+static dfgpu_batch schema_only(const int32_t* dtypes, int ncols) {
+  dfgpu_batch b;
+  for (int i = 0; i < ncols; i++) {
+    DevColumn c;
+    c.dtype = dtypes[i];
+    b.cols.push_back(c);
+  }
+  return b;
 }
+
+// nproj == 0: FilterRelation alone emits every input column (filter.rs:55-57).  Points proj / proj_len / nproj at one
+// column program per input column, held in `ident`.
+struct IdentityProjection {
+  std::vector<dfgpu_insn> insn;
+  std::vector<const dfgpu_insn*> ptr;
+  std::vector<int> len;
+};
+template <class DtypeOf>
+static void project_every_column(int ncols, DtypeOf dtype_of, IdentityProjection& ident, const dfgpu_insn* const*& proj,
+                                 const int*& proj_len, int& nproj) {
+  if (nproj != 0) return;
+  ident.insn.assign(size_t(ncols), dfgpu_insn{});
+  for (int i = 0; i < ncols; i++) {
+    ident.insn[size_t(i)].op = DFGPU_OP_COL;
+    ident.insn[size_t(i)].col = i;
+    ident.insn[size_t(i)].dtype = dtype_of(i);
+    ident.ptr.push_back(&ident.insn[size_t(i)]);
+    ident.len.push_back(1);
+  }
+  nproj = ncols;
+  proj = ident.ptr.data();
+  proj_len = ident.len.data();
+}
+
+// The WHERE program: program 0 of the set, and Boolean (filter.rs:64-66).
+static void add_predicate(ProgramBuilder& pb, const dfgpu_insn* pred, int pred_len) {
+  if (pb.out_dtype(pb.add(pred, pred_len, "predicate")) != DFGPU_BOOL)
+    fail(DFGPU_ERR_EXECUTION, "Filter expression did not evaluate to boolean");
+}
+
+// One output column of dfgpu_filter_project: how it is computed, and what the call allocates and settles for it.
+struct OutCol {
+  enum Kind {
+    VALUE,        // fixed-width value, written by the kernel
+    BOOL,         // Boolean: the kernel writes one byte per selected row, packed into bits afterwards
+    UTF8_GATHER,  // a Utf8 input column, gathered by the selected row numbers after the kernel (utf8_gather.cu)
+    UTF8_VIEW,    // a Utf8 function of one, evaluated over those row numbers (utf8_function.cu)
+  } kind = VALUE;
+  int slot = -1;  // VALUE / BOOL: the kernel's projection index (its program is slot + has_pred)
+  int src = -1;   // UTF8_*: the input column, whose validity the result keeps without a WHERE
+  int view = -1;  // UTF8_VIEW: the builder's Utf8 view
+  // Under a WHERE the kernel drops the input bitmaps, so only a CASE-made null is a null: the kernel writes such a
+  // projection's validity as one byte per selected row (vbytes), packed into the bitmap afterwards.
+  bool case_nulls = false;
+  bool kernel_validity = false;     // no WHERE, nullable: the kernel writes the bitmap and counts the nulls
+  unsigned char* bytes = nullptr;   // BOOL: the kernel's bytes
+  unsigned char* vbytes = nullptr;  // case_nulls: the validity bytes
+  bool utf8() const { return kind == UTF8_GATHER || kind == UTF8_VIEW; }
+};
+
+}  // namespace dfgpu
 using namespace dfgpu;
 
 // Host-only type check of one expression program (no ctx, no device): the same ProgramBuilder the
@@ -223,13 +278,8 @@ using namespace dfgpu;
 extern "C" int dfgpu_check_program(const int32_t* col_dtypes, int ncols, const dfgpu_insn* prog, int prog_len, int32_t* out_dtype) {
   return guarded([&] {
     if (!col_dtypes || ncols < 0 || !prog || prog_len <= 0 || !out_dtype) fail(DFGPU_ERR_GENERAL, "dfgpu_check_program: null argument");
-    dfgpu_batch schema_only;  // ctx == nullptr: owns nothing, its destructor frees nothing
-    for (int i = 0; i < ncols; i++) {
-      DevColumn c;
-      c.dtype = col_dtypes[i];
-      schema_only.cols.push_back(c);
-    }
-    ProgramBuilder pb(&schema_only);
+    const dfgpu_batch schema = schema_only(col_dtypes, ncols);
+    ProgramBuilder pb(&schema);
     const int pi = pb.add(prog, prog_len, "expression");
     ProgramSet ps;  // Utf8 predicates are typed, not evaluated
     pb.finish(&ps);  // instruction / column-slot limits
@@ -244,58 +294,41 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
     ctx->use();
     ProgramBuilder pb(batch);
     const int has_pred = pred_len > 0 ? 1 : 0;
-    if (has_pred) {
-      int pi = pb.add(pred, pred_len, "predicate");
-      if (pb.out_dtype(pi) != DFGPU_BOOL)  // filter.rs:64-66
-        fail(DFGPU_ERR_EXECUTION, "Filter expression did not evaluate to boolean");
-    }
-    // nproj == 0: FilterRelation alone emits every input column (filter.rs:55-57)
-    std::vector<dfgpu_insn> ident;
-    std::vector<const dfgpu_insn*> pptr;
-    std::vector<int> plen;
-    if (nproj == 0) {
-      ident.resize(batch->cols.size());
-      for (size_t i = 0; i < batch->cols.size(); i++) {
-        memset(&ident[i], 0, sizeof(dfgpu_insn));
-        ident[i].op = DFGPU_OP_COL;
-        ident[i].col = int(i);
-        ident[i].dtype = batch->cols[i].dtype;
-      }
-      for (size_t i = 0; i < batch->cols.size(); i++) {
-        pptr.push_back(&ident[i]);
-        plen.push_back(1);
-      }
-      nproj = int(batch->cols.size());
-      proj = pptr.data();
-      proj_len = plen.data();
-    }
-    // Projections that are a plain Utf8 column are gathered by row number after the fused kernel
-    // (utf8_gather.cu), and projections of a Utf8 function are evaluated over those row numbers (utf8_function.cu);
-    // everything else is evaluated inside it.
-    std::vector<int> out_kind;  // per output column: >= 0 kernel program slot, -1 - c = Utf8 gather of input column c
-    std::vector<int> out_view(size_t(nproj), -1);  // per output column: the Utf8 view it is, or -1
+    if (has_pred) add_predicate(pb, pred, pred_len);
+    IdentityProjection ident;
+    project_every_column(int(batch->cols.size()), [&](int i) { return batch->cols[size_t(i)].dtype; }, ident, proj, proj_len, nproj);
+
+    // ---- plan: one record per output column ----
+    std::vector<OutCol> outs((size_t)nproj);
     int nkern = 0;
-    bool any_utf8 = false;
+    bool any_utf8 = false, any_bool = false, any_case_nulls = false;
     for (int i = 0; i < nproj; i++) {
-      if (proj_len[i] == 1 && proj[i][0].op == DFGPU_OP_COL && proj[i][0].col >= 0 && size_t(proj[i][0].col) < batch->cols.size() &&
-          batch->cols[size_t(proj[i][0].col)].dtype == DFGPU_UTF8) {
-        out_kind.push_back(-1 - proj[i][0].col);
-        any_utf8 = true;
-        continue;
+      OutCol& o = outs[size_t(i)];
+      const dfgpu_insn* q = proj[i];
+      if (proj_len[i] == 1 && q[0].op == DFGPU_OP_COL && q[0].col >= 0 && size_t(q[0].col) < batch->cols.size() &&
+          batch->cols[size_t(q[0].col)].dtype == DFGPU_UTF8) {
+        o.kind = OutCol::UTF8_GATHER;
+        o.src = q[0].col;
+      } else {
+        const int pi = pb.add(q, proj_len[i], "projection", &o.view);
+        if (o.view >= 0) {
+          o.kind = OutCol::UTF8_VIEW;
+          o.src = pb.utf8_views()[size_t(o.view)].src;
+        } else {
+          const int dt = pb.out_dtype(pi);
+          if (!is_numeric(dt) && dt != DFGPU_BOOL)
+            fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string("filter/projection output of type ") + dtype_name(dt) +
+                                                " is not supported on the GPU path yet");
+          o.kind = dt == DFGPU_BOOL ? OutCol::BOOL : OutCol::VALUE;
+          o.slot = nkern++;
+          o.case_nulls = has_pred && pb.prog(pi).makes_nulls;
+        }
       }
-      int pi = pb.add(proj[i], proj_len[i], "projection", &out_view[size_t(i)]);
-      if (out_view[size_t(i)] >= 0) {
-        out_kind.push_back(INT32_MIN);
-        any_utf8 = true;
-        continue;
-      }
-      int dt = pb.out_dtype(pi);
-      if (!is_numeric(dt) && dt != DFGPU_BOOL)
-        fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string("filter/projection output of type ") + dtype_name(dt) +
-                                            " is not supported on the GPU path yet");
-      out_kind.push_back(nkern++);
+      any_utf8 = any_utf8 || o.utf8();
+      any_bool = any_bool || o.kind == OutCol::BOOL;
+      any_case_nulls = any_case_nulls || o.case_nulls;
     }
-    int rowid_slot = -1;
+    int rowid_slot = -1;  // the selected row numbers, which the Utf8 outputs are gathered by
     if (any_utf8) {
       pb.add_rowid();
       rowid_slot = nkern++;
@@ -310,85 +343,86 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
         fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string("expressions over ") + dtype_name(p.ps.cols[s].dtype) + " columns are not supported on the GPU path yet");
     }
     if (p.ps.max_depth > 8) fail(DFGPU_ERR_NOT_IMPLEMENTED, "expression too deep (register stack depth > 8)");
-    // Boolean projections (comparisons / AND / OR, expression.rs:212-224,236-290) leave the kernel as one
-    // byte per selected row and are bit-packed (BooleanArray layout) once the row count is known.
-    for (int k = 0; k < nkern; k++)
-      if (p.ps.out_dtype[k + has_pred] == DFGPU_BOOL) p.ps.out_dtype[k + has_pred] = DFGPU_UINT8;
+    // without a WHERE over nullable inputs the kernel writes the validity of the nullable projections and counts their nulls
+    const bool kernel_nulls = !has_pred && p.ps.has_nulls;
+    for (OutCol& o : outs) {
+      if (o.slot < 0) continue;
+      o.kernel_validity = kernel_nulls && p.ps.nullable[o.slot + has_pred];
+      // Boolean projections (comparisons / AND / OR, expression.rs:212-224,236-290) leave the kernel as bytes
+      if (o.kind == OutCol::BOOL) p.ps.out_dtype[o.slot + has_pred] = DFGPU_UINT8;
+    }
 
+    // ---- allocate and launch ----
     auto res = std::make_unique<dfgpu_result>();
     res->ctx = ctx;
     const long long n = batch->nrows;
-    dfgpu_result bool_bytes;  // RAII for the unpacked Boolean outputs
-    bool_bytes.ctx = ctx;
-    std::vector<int> bool_of_out(size_t(nproj), -1);
-    // kernel outputs (worst case n rows each); the row-number column is scratch, not a result column
-    dfgpu_result scratch;  // RAII for the row-number buffer
-    scratch.ctx = ctx;
-    std::vector<void*> kern_out(size_t(nkern), nullptr);
-    for (int i = 0; i < nproj; i++) {
+    const size_t rows = size_t(n > 0 ? n : 1);
+    for (const OutCol& o : outs) {
       DevColumn c;
-      if (out_kind[size_t(i)] >= 0) {
-        c.dtype = pb.out_dtype(out_kind[size_t(i)] + has_pred);
-        if (c.dtype == DFGPU_BOOL) {
-          DevColumn b;
-          b.dtype = DFGPU_UINT8;
-          b.values_bytes = size_t(n > 0 ? n : 1);
-          b.values = ctx->alloc(b.values_bytes);
-          bool_of_out[size_t(i)] = int(bool_bytes.cols.size());
-          bool_bytes.cols.push_back(b);
-          kern_out[size_t(out_kind[size_t(i)])] = b.values;
-          c.values_bytes = size_t((n + 31) / 32) * 4 + 4;  // packed, whole 32-bit words
-          c.values = ctx->alloc(c.values_bytes);
-        } else {
-          c.values_bytes = size_t(n > 0 ? n : 1) * size_t(dtype_width(c.dtype));
-          c.values = ctx->alloc(c.values_bytes);
-          kern_out[size_t(out_kind[size_t(i)])] = c.values;
-        }
-      } else {
-        c.dtype = DFGPU_UTF8;  // filled by the gather below
-      }
+      c.dtype = o.kind == OutCol::VALUE ? pb.out_dtype(o.slot + has_pred) : o.kind == OutCol::BOOL ? DFGPU_BOOL : DFGPU_UTF8;
+      if (o.kind == OutCol::VALUE) c.values_bytes = rows * size_t(dtype_width(c.dtype));
+      if (o.kind == OutCol::BOOL) c.values_bytes = size_t((n + 31) / 32) * 4 + 4;  // packed, whole 32-bit words
+      if (!o.utf8()) c.values = ctx->alloc(c.values_bytes);
       res->cols.push_back(c);
     }
-    if (rowid_slot >= 0) {
-      DevColumn c;
-      c.dtype = DFGPU_UINT64;
-      c.values_bytes = size_t(n > 0 ? n : 1) * 8;
-      c.values = ctx->alloc(c.values_bytes);
-      scratch.cols.push_back(c);
-      kern_out[size_t(rowid_slot)] = c.values;
-    }
     if (n == 0) {
-      for (auto& c : res->cols)
-        if (c.dtype == DFGPU_BOOL) c.values_bytes = 0;
-      for (auto& c : res->cols)
-        if (c.dtype == DFGPU_UTF8) {
+      for (size_t i = 0; i < outs.size(); i++) {
+        DevColumn& c = res->cols[i];
+        if (outs[i].kind == OutCol::BOOL) c.values_bytes = 0;
+        if (outs[i].utf8()) {
           c.offsets = (int32_t*)ctx->alloc(4);
           DF_CUDA(cudaMemsetAsync(c.offsets, 0, 4, ctx->stream));
           c.values = ctx->alloc(1);
         }
-      DF_CUDA(cudaStreamSynchronize(ctx->stream));
+      }
+      DF_CUDA(cudaStreamSynchronize(ctx->stream));  // a result that is not stream-ordered is complete when the call returns
       res->nrows = 0;
       *out = res.release();
       return;
     }
+    DevBufs tmp(ctx);  // the kernel's byte outputs, the row numbers and the tile status words
     p.nrows = n;
     p.has_pred = has_pred;
     p.nproj = nkern;
-    for (int i = 0; i < nkern; i++) p.out[i] = kern_out[size_t(i)];
+    memset(p.out_valid, 0, sizeof(p.out_valid));
+    memset(p.out_vbytes, 0, sizeof(p.out_vbytes));
+    static_assert(kMaxProgs <= SCR_FP_NULLS.words, "a null count per program");
+    p.null_counts = ctx->d_scratch + SCR_FP_NULLS.at;
+    if (kernel_nulls) DF_CUDA(cudaMemsetAsync(p.null_counts, 0, kMaxProgs * 8, ctx->stream));
+    for (size_t i = 0; i < outs.size(); i++) {
+      OutCol& o = outs[i];
+      DevColumn& c = res->cols[i];
+      if (o.slot < 0) continue;
+      if (o.kind == OutCol::BOOL) o.bytes = tmp.alloc<unsigned char>(rows);
+      p.out[o.slot] = o.kind == OutCol::BOOL ? o.bytes : c.values;
+      if (o.case_nulls) {
+        o.vbytes = tmp.alloc<unsigned char>(rows);
+        p.out_vbytes[o.slot] = o.vbytes;
+      }
+      if (o.kernel_validity) {
+        const size_t bitmap_bytes = size_t((n + 31) / 32) * 4;
+        c.validity = (uint8_t*)ctx->alloc(bitmap_bytes);
+        DF_CUDA(cudaMemsetAsync(c.validity, 0, bitmap_bytes, ctx->stream));
+        p.out_valid[o.slot] = (unsigned*)c.validity;
+      }
+    }
+    unsigned long long* row_numbers = nullptr;
+    if (rowid_slot >= 0) {
+      row_numbers = tmp.alloc(rows * 8);
+      p.out[rowid_slot] = row_numbers;
+    }
     // tile_status is sized for the smallest tile either kernel uses (1024 rows)
     const size_t max_tiles = size_t((n + 1023) / 1024) + 1;
     // one allocation, one memset: [ticket, pad..] then the tile words.  The row count and the error
     // flag are written by the kernel straight into pinned host memory (zero-copy), so no device-to-host
     // copy follows the kernel.
-    unsigned long long* status = (unsigned long long*)ctx->alloc((max_tiles + 8) * 8);
+    unsigned long long* status = tmp.alloc((max_tiles + 8) * 8);
     DF_CUDA(cudaMemsetAsync(status, 0, (max_tiles + 8) * 8, ctx->stream));
     p.tile_status = status + 8;
     p.ticket = (unsigned*)(status + 0);
     // Stream-ordered: when nothing after the kernel needs the row count on the host (no Boolean packing, no Utf8
     // gather, no validity outputs) and no program can raise, the call returns once the kernel is queued.  The kernel
     // writes the count into a word pair the result owns, read when the result is first used (resolve, api.cu).
-    bool any_bool = false;
-    for (int i = 0; i < nproj; i++) any_bool = any_bool || bool_of_out[size_t(i)] >= 0;
     const bool stream_ordered = has_pred && !p.ps.has_nulls && !any_utf8 && !any_bool && !has_div(p.ps);
     if (stream_ordered) {
       res->pending = ctx->fp_acquire(res.get());
@@ -399,41 +433,6 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
       p.err_flag = (unsigned*)(ctx->h_scratch + SCR_FP_DIV0.at);
       *p.out_count = 0;
       *p.err_flag = 0;
-    }
-    // validity outputs: only a query WITHOUT a predicate can emit nulls (see k_filter_project)
-    memset(p.out_valid, 0, sizeof(p.out_valid));
-    static_assert(kMaxProgs <= SCR_FP_NULLS.words, "a null count per program");
-    p.null_counts = ctx->d_scratch + SCR_FP_NULLS.at;
-    std::vector<int> valid_of_out(size_t(nproj), -1);  // result column -> kernel program with a validity buffer
-    memset(p.out_vbytes, 0, sizeof(p.out_vbytes));
-    dfgpu_result vbytes;  // RAII for the validity bytes of CASE projections under a predicate
-    vbytes.ctx = ctx;
-    std::vector<int> vbytes_of_out(size_t(nproj), -1);
-    if (has_pred && has_case(p.ps)) {
-      for (int i = 0; i < nproj; i++) {
-        const int k = out_kind[size_t(i)];
-        if (k < 0 || !pb.prog(k + has_pred).makes_nulls) continue;
-        DevColumn b;
-        b.dtype = DFGPU_UINT8;
-        b.values_bytes = size_t(n);
-        b.values = ctx->alloc(b.values_bytes);
-        p.out_vbytes[k] = (unsigned char*)b.values;
-        vbytes_of_out[size_t(i)] = int(vbytes.cols.size());
-        vbytes.cols.push_back(b);
-      }
-    }
-    if (p.ps.has_nulls && !has_pred) {
-      DF_CUDA(cudaMemsetAsync(p.null_counts, 0, kMaxProgs * 8, ctx->stream));
-      for (int i = 0; i < nproj; i++) {
-        const int k = out_kind[size_t(i)];
-        if (k >= 0 && p.ps.nullable[k]) {
-          const size_t vbytes = size_t((n + 31) / 32) * 4;
-          res->cols[size_t(i)].validity = (uint8_t*)ctx->alloc(vbytes);
-          DF_CUDA(cudaMemsetAsync(res->cols[size_t(i)].validity, 0, vbytes, ctx->stream));
-          p.out_valid[k] = (unsigned*)res->cols[size_t(i)].validity;
-          valid_of_out[size_t(i)] = k;
-        }
-      }
     }
     p.pred_fast = has_pred ? pb.prog(0).chain : LeafChain{};
     for (int i = 0; i < nkern; i++) p.proj_fast[i] = pb.prog(i + has_pred).leaf;
@@ -456,81 +455,56 @@ extern "C" int dfgpu_filter_project(dfgpu_ctx* ctx, const dfgpu_batch* batch, co
     }
     if (stream_ordered) {
       DF_CUDA(cudaEventRecord(ctx->fp_slots[size_t(res->pending)].done, ctx->stream));
-      ctx->free(status);
       if (getenv("DFGPU_TRACE")) fprintf(stderr, "[dfgpu trace] filter_project returns stream-ordered\n");
       *out = res.release();
       return;
     }
-    if (p.ps.has_nulls && !has_pred)
+
+    // ---- settle ----
+    if (kernel_nulls)
       DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + SCR_FP_NULLS.at, p.null_counts, kMaxProgs * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    DF_CUDA(cudaStreamSynchronize(ctx->stream));
-    ctx->free(status);
-    for (int i = 0; i < nproj; i++) {
-      DevColumn& c = res->cols[size_t(i)];
-      if (valid_of_out[size_t(i)] >= 0) {
-        c.null_count = (int64_t)ctx->h_scratch[SCR_FP_NULLS.at + valid_of_out[size_t(i)]];
-        if (c.null_count == 0) {
-          ctx->free(c.validity);
-          c.validity = nullptr;
-        }
-      }
-    }
+    DF_CUDA(cudaStreamSynchronize(ctx->stream));  // the host reads the row count, the DivideByZero flag and the null counts
+    for (size_t i = 0; i < outs.size(); i++)
+      if (outs[i].kernel_validity) set_null_count(ctx, res->cols[i], (int64_t)ctx->h_scratch[SCR_FP_NULLS.at + outs[i].slot]);
     if (*p.err_flag != 0) fail(DFGPU_ERR_ARROW, "DivideByZero");
     res->nrows = has_pred ? (int64_t)*p.out_count : n;
-    if (!vbytes.cols.empty() && res->nrows > 0) {
+    const long long words = (res->nrows + 31) / 32;
+    if (any_case_nulls && words > 0) {
       DF_CUDA(cudaMemsetAsync(p.null_counts, 0, kMaxProgs * 8, ctx->stream));
-      const long long words = (res->nrows + 31) / 32;
-      for (int i = 0; i < nproj; i++)
-        if (vbytes_of_out[size_t(i)] >= 0) {
-          DevColumn& c = res->cols[size_t(i)];
-          c.validity = (uint8_t*)ctx->alloc(size_t(words) * 4);
-          launch(ctx, "k_pack_valid", k_pack_valid, grid_for(ctx, words * 32, 256, 8), 256, {},
-                 (const unsigned char*)vbytes.cols[size_t(vbytes_of_out[size_t(i)])].values, (long long)res->nrows, (unsigned*)c.validity,
-                 p.null_counts + out_kind[size_t(i)]);
+      for (size_t i = 0; i < outs.size(); i++)
+        if (outs[i].case_nulls) {
+          res->cols[i].validity = (uint8_t*)ctx->alloc(size_t(words) * 4);
+          pack_bits(ctx, outs[i].vbytes, res->nrows, (unsigned*)res->cols[i].validity, p.null_counts + outs[i].slot);
         }
       DF_CUDA(cudaMemcpyAsync(ctx->h_scratch + SCR_FP_NULLS.at, p.null_counts, kMaxProgs * 8, cudaMemcpyDeviceToHost, ctx->stream));
-      DF_CUDA(cudaStreamSynchronize(ctx->stream));
-      for (int i = 0; i < nproj; i++) {
-        DevColumn& c = res->cols[size_t(i)];
-        if (vbytes_of_out[size_t(i)] < 0) continue;
-        c.null_count = (int64_t)ctx->h_scratch[SCR_FP_NULLS.at + out_kind[size_t(i)]];
-        if (c.null_count == 0) {
-          ctx->free(c.validity);
-          c.validity = nullptr;
-        }
+      DF_CUDA(cudaStreamSynchronize(ctx->stream));  // the host reads the packs' null counts
+      for (size_t i = 0; i < outs.size(); i++)
+        if (outs[i].case_nulls) set_null_count(ctx, res->cols[i], (int64_t)ctx->h_scratch[SCR_FP_NULLS.at + outs[i].slot]);
+    }
+    for (size_t i = 0; i < outs.size(); i++) {
+      const OutCol& o = outs[i];
+      DevColumn& c = res->cols[i];
+      if (o.kind == OutCol::BOOL) {
+        if (words > 0) pack_bits(ctx, o.bytes, res->nrows, (unsigned*)c.values, nullptr);
+        c.values_bytes = size_t(res->nrows + 7) / 8;
+      } else if (o.kind == OutCol::UTF8_VIEW) {  // without a WHERE every row, in order: no row numbers needed
+        pb.eval_utf8_view_rows(ctx, o.view, has_pred ? row_numbers : nullptr, res->nrows, &c);
+      } else if (o.kind == OutCol::UTF8_GATHER) {
+        gather_utf8(ctx, batch->cols[size_t(o.src)], row_numbers, res->nrows, &c);
+      }
+      // without a WHERE a Utf8 column passed through keeps its validity (expression.rs:313), and so does a Utf8 function of one
+      if (!has_pred && o.utf8() && batch->cols[size_t(o.src)].null_count > 0) {
+        const DevColumn& srcc = batch->cols[size_t(o.src)];
+        const size_t vb = size_t(n + 7) / 8;
+        c.validity = (uint8_t*)ctx->alloc(vb);
+        DF_CUDA(cudaMemcpyAsync(c.validity, srcc.validity, vb, cudaMemcpyDeviceToDevice, ctx->stream));
+        c.null_count = srcc.null_count;
       }
     }
-    for (int i = 0; i < nproj; i++)
-      if (bool_of_out[size_t(i)] >= 0) {
-        DevColumn& c = res->cols[size_t(i)];
-        const long long words = (res->nrows + 31) / 32;
-        if (words > 0)
-          launch(ctx, "k_pack_bits", k_pack_bits, grid_for(ctx, words * 32, 256, 8), 256, {},
-                 (const unsigned char*)bool_bytes.cols[size_t(bool_of_out[size_t(i)])].values, (long long)res->nrows, (unsigned*)c.values);
-        c.values_bytes = size_t(res->nrows + 7) / 8;
-        any_utf8 = true;  // synchronise before the byte buffers are released
-      }
-    for (int i = 0; i < nproj; i++)
-      if (out_view[size_t(i)] >= 0)  // without a WHERE every row, in order: no row numbers needed
-        pb.eval_utf8_view_rows(ctx, out_view[size_t(i)], has_pred ? (const unsigned long long*)scratch.cols[0].values : nullptr, res->nrows,
-                               &res->cols[size_t(i)]);
-      else if (out_kind[size_t(i)] < 0)
-        gather_utf8(ctx, batch->cols[size_t(-1 - out_kind[size_t(i)])], (const unsigned long long*)scratch.cols[0].values, res->nrows,
-                    &res->cols[size_t(i)]);
-    if (!has_pred)
-      for (int i = 0; i < nproj; i++)
-        if (out_kind[size_t(i)] < 0) {  // Utf8 column passed through untouched keeps its validity (expression.rs:313)
-          // and so does a Utf8 function of one
-          const int src = out_view[size_t(i)] >= 0 ? pb.utf8_views()[size_t(out_view[size_t(i)])].src : -1 - out_kind[size_t(i)];
-          const DevColumn& srcc = batch->cols[size_t(src)];
-          if (srcc.null_count > 0) {
-            const size_t vb = size_t(n + 7) / 8;
-            res->cols[size_t(i)].validity = (uint8_t*)ctx->alloc(vb);
-            DF_CUDA(cudaMemcpyAsync(res->cols[size_t(i)].validity, srcc.validity, vb, cudaMemcpyDeviceToDevice, ctx->stream));
-            res->cols[size_t(i)].null_count = srcc.null_count;
-          }
-        }
-    if (any_utf8) DF_CUDA(cudaStreamSynchronize(ctx->stream));
+    // a result that is not stream-ordered is complete when the call returns: wait for the packs, gathers and copies queued
+    // after the synchronisation above (its readers may use another stream, and the byte buffers go back to the pool)
+    const bool queued_after_sync = any_bool || any_utf8;
+    if (queued_after_sync) DF_CUDA(cudaStreamSynchronize(ctx->stream));
     *out = res.release();
   });
 }
@@ -550,24 +524,8 @@ extern "C" int dfgpu_filter_project_host(dfgpu_ctx* ctx, const dfgpu_col* cols, 
     for (int i = 0; i < ncols; i++) {
       if (cols[i].len != n) fail(DFGPU_ERR_GENERAL, "all columns of a RecordBatch must have the same length");
     }
-    // nproj == 0 -> every input column
-    std::vector<dfgpu_insn> ident;
-    std::vector<const dfgpu_insn*> pptr;
-    std::vector<int> plen;
-    if (nproj == 0) {
-      ident.resize(size_t(ncols));
-      for (int i = 0; i < ncols; i++) {
-        memset(&ident[size_t(i)], 0, sizeof(dfgpu_insn));
-        ident[size_t(i)].op = DFGPU_OP_COL;
-        ident[size_t(i)].col = i;
-        ident[size_t(i)].dtype = cols[i].dtype;
-        pptr.push_back(&ident[size_t(i)]);
-        plen.push_back(1);
-      }
-      nproj = ncols;
-      proj = pptr.data();
-      proj_len = plen.data();
-    }
+    IdentityProjection ident;
+    project_every_column(ncols, [&](int i) { return cols[i].dtype; }, ident, proj, proj_len, nproj);
     // referenced columns only (the reference uploads nothing, but gathers every column: filter.rs:55-57)
     std::vector<int> remap(size_t(ncols), -1), used;
     auto scan = [&](const dfgpu_insn* p, int len) {
@@ -583,13 +541,6 @@ extern "C" int dfgpu_filter_project_host(dfgpu_ctx* ctx, const dfgpu_col* cols, 
     if (pred_len > 0) scan(pred, pred_len);
     for (int q = 0; q < nproj; q++) scan(proj[q], proj_len[q]);
     if (used.empty()) fail(DFGPU_ERR_NOT_IMPLEMENTED, "queries that reference no column");
-    // Utf8 / Boolean / nullable inputs and projections that can hold a CASE-made null: not chunk-pipelined — the
-    // referenced columns are uploaded whole and the resident operator runs (same kernels, same results); the result then
-    // lives in DEVICE memory (dfgpu_result_on_host says which; dfgpu_result_copy_col works for both)
-    bool resident = false;
-    for (int q = 0; q < nproj; q++)
-      for (int i = 0; i < proj_len[q]; i++) resident = resident || (proj[q][i].op == DFGPU_OP_CASE && proj[q][i].col % 2 == 0);
-    for (int c : used) resident = resident || !is_numeric(cols[c].dtype) || cols[c].validity;
     auto rewrite = [&](const dfgpu_insn* p, int len) {
       std::vector<dfgpu_insn> v(p, p + len);
       for (auto& in : v)
@@ -607,7 +558,31 @@ extern "C" int dfgpu_filter_project_host(dfgpu_ctx* ctx, const dfgpu_col* cols, 
       proj2p.push_back(v.data());
       proj2l.push_back(int(v.size()));
     }
-    auto run_resident = [&] {
+    // The chunks carry fixed-width values only, and the result columns are pinned host arrays of fixed-width values.
+    // Everything else runs the resident operator on the whole batch (same kernels, same results; the result then lives
+    // in DEVICE memory: dfgpu_result_on_host says which, dfgpu_result_copy_col works for both).  That is decided here,
+    // before anything is uploaded: a referenced input that is not numeric or has a validity bitmap, a projection whose
+    // result is not numeric (Boolean), or one with a CASE without ELSE (V_SEL0: the postfix program does not tell a
+    // consumed null from a result one) takes the resident operator.
+    std::vector<int32_t> used_dtypes;
+    bool resident = false;
+    for (int c : used) {
+      resident = resident || !is_numeric(cols[c].dtype) || cols[c].validity;
+      used_dtypes.push_back(cols[c].dtype);
+    }
+    std::vector<int> out_dtype;
+    if (!resident) {  // typed by the front end of every chunk's call, on the same programs
+      const dfgpu_batch schema = schema_only(used_dtypes.data(), int(used_dtypes.size()));
+      ProgramBuilder pb(&schema);
+      if (pred_len > 0) add_predicate(pb, pred2.data(), int(pred2.size()));
+      for (int q = 0; q < nproj; q++) {
+        const int pi = pb.add(proj2p[size_t(q)], proj2l[size_t(q)], "projection");
+        out_dtype.push_back(pb.out_dtype(pi));
+        resident = resident || !is_numeric(pb.out_dtype(pi));
+        for (const DevInsn& di : pb.prog(pi).code) resident = resident || di.op == V_SEL0;
+      }
+    }
+    if (resident) {
       std::vector<dfgpu_col> sub;
       for (int c : used) sub.push_back(cols[c]);
       dfgpu_batch* b = nullptr;
@@ -616,9 +591,6 @@ extern "C" int dfgpu_filter_project_host(dfgpu_ctx* ctx, const dfgpu_col* cols, 
       struct G { dfgpu_batch* b; ~G() { dfgpu_batch_free(b); } } g{b};
       rc = dfgpu_filter_project(ctx, b, pred2.data(), int(pred2.size()), proj2p.data(), proj2l.data(), nproj, out);
       if (rc != DFGPU_OK) fail(rc, dfgpu_last_error());
-    };
-    if (resident) {
-      run_resident();
       return;
     }
 
@@ -681,26 +653,19 @@ extern "C" int dfgpu_filter_project_host(dfgpu_ctx* ctx, const dfgpu_col* cols, 
     auto res = std::make_unique<dfgpu_result>();
     res->ctx = ctx;
     res->on_host = true;
+    for (int dt : out_dtype) {
+      DevColumn hcol;
+      hcol.dtype = dt;
+      hcol.values_bytes = size_t(n > 0 ? n : 1) * size_t(dtype_width(dt));
+      hcol.values = ctx->host_alloc(hcol.values_bytes);
+      res->cols.push_back(hcol);
+    }
     long long off = 0;
     for (long long c = 0; c < nchunks; c++) {
       Chunk& ch = *chunks[size_t(c)];
       DF_CUDA(cudaStreamWaitEvent(ctx->stream, ch.ev, 0));
       int rc = dfgpu_filter_project(ctx, &ch.batch, pred2.data(), int(pred2.size()), proj2p.data(), proj2l.data(), nproj, &ch.res);
       if (rc != 0) fail(rc, dfgpu_last_error());
-      if (c == 0) {
-        for (int q = 0; q < nproj; q++) {
-          DevColumn hcol;
-          hcol.dtype = ch.res->cols[size_t(q)].dtype;
-          if (!is_numeric(hcol.dtype)) {  // Boolean projections (bit-packed): the resident operator handles the whole batch
-            resident = true;
-            break;
-          }
-          hcol.values_bytes = size_t(n > 0 ? n : 1) * size_t(dtype_width(hcol.dtype));
-          hcol.values = ctx->host_alloc(hcol.values_bytes);
-          res->cols.push_back(hcol);
-        }
-      }
-      if (resident) break;
       // waits for the kernel of this chunk: its row count sizes the copies, and stream_out reads what it wrote
       resolve(ch.res);
       for (int q = 0; q < nproj; q++) {
@@ -712,11 +677,6 @@ extern "C" int dfgpu_filter_project_host(dfgpu_ctx* ctx, const dfgpu_col* cols, 
       off += ch.res->nrows;
     }
     DF_CUDA(cudaStreamSynchronize(ctx->stream_out));
-    if (resident) {
-      res.reset();  // returns the pinned blocks of the projections before the Boolean one
-      run_resident();
-      return;
-    }
     res->nrows = off;
     *out = res.release();
   });

@@ -104,11 +104,7 @@ void gather_column(dfgpu_ctx* ctx, const DevColumn& src, const unsigned* idx, lo
     out->validity = (uint8_t*)ctx->alloc(size_t((n + 31) / 32) * 4);
     DF_CUDA(cudaMemsetAsync(d_nulls, 0, 8, ctx->stream));
     launch(ctx, "k_join_gather_bits", k_join_gather_bits, grid, SEL_THREADS, PROFILED, (const unsigned char*)src.validity, idx, n, (unsigned*)out->validity, d_nulls);
-    out->null_count = (int64_t)read_word(ctx, d_nulls);
-    if (out->null_count == 0) {
-      ctx->free(out->validity);
-      out->validity = nullptr;
-    }
+    set_null_count(ctx, *out, (int64_t)read_word(ctx, d_nulls));
   }
 }
 

@@ -493,17 +493,20 @@ RecordBatch GpuFilterProjectRelation::process(const RecordBatch& in_batch, const
   std::vector<const dfgpu_insn*> pp;
   std::vector<int> pl;
   for (auto& p : progs) { pp.push_back(p.data()); pl.push_back(int(p.size())); }
-  // Large all-numeric batches: host buffers in, pinned host buffers out, with upload / kernel /
-  // download overlapped by row-range chunk inside the library; the result columns are wrapped
-  // zero-copy (the pinned block lives as long as the RecordBatch).
-  bool numeric_only = batch->num_rows >= (4ll << 20);
-  for (size_t c : pr.cols) numeric_only = numeric_only && datatype_width(batch->columns[c]->data_type) > 0 && batch->columns[c]->null_count == 0;
-  for (auto& f : out_schema->fields) numeric_only = numeric_only && datatype_width(f.data_type) > 0;  // Boolean / Utf8 outputs: resident path
-  if (numeric_only) {
+  // Large batches: host buffers straight in.  The library overlaps upload, kernel and download by row-range chunk
+  // when it can and returns pinned host columns, wrapped zero-copy here (the pinned block lives as long as the
+  // RecordBatch); otherwise it runs the resident operator on the whole batch and the result is in device memory.
+  if (batch->num_rows >= (4ll << 20)) {
     std::vector<dfgpu_col> cols;
     for (size_t c : pr.cols) cols.push_back(batch->columns[c]->view());
-    dfgpu_result* raw = nullptr;
-    GPU_CHECK(dfgpu_filter_project_host(gpu_, cols.data(), int(cols.size()), pred.data(), int(pred.size()), pp.data(), pl.data(), int(pp.size()), 0, &raw));
+    if (cols.empty()) fail(DFGPU_ERR_NOT_IMPLEMENTED, "queries that reference no column");
+    ResultGuard r;
+    GPU_CHECK(dfgpu_filter_project_host(gpu_, cols.data(), int(cols.size()), pred.data(), int(pred.size()), pp.data(), pl.data(), int(pp.size()), 0, &r.r));
+    int on_host = 0;
+    GPU_CHECK(dfgpu_result_on_host(r.r, &on_host));
+    if (!on_host) return download(r.r, out_schema);
+    dfgpu_result* raw = r.r;
+    r.r = nullptr;
     std::shared_ptr<void> owner(raw, [](void* p) { dfgpu_result_free(static_cast<dfgpu_result*>(p)); });
     RecordBatch out;
     out.schema = out_schema;

@@ -8,7 +8,7 @@ scan, dual ring), the direct filter kernel, the CAS / RED table of k_hash_agg_le
 growth with overflow replay, the shared-memory front tables, wide-key slots (busy / ready publication) and the
 chunked host pipelines, and the
 join's build, probe and gathers, and CASE in the extended interpreter: its validity bytes under a WHERE (out_vbytes,
-k_pack_valid), the null-aware reduce, the group scan and the TMA interpreter loop."""
+k_pack_bits), the null-aware reduce, the group scan and the TMA interpreter loop."""
 import os
 import sys
 
@@ -236,7 +236,7 @@ sr.free(); sj.free(); sbb.free(); spb.free()
 os.environ.pop("DFGPU_JOIN_TAG_BITS", None)
 print("semi join ok", flush=True)
 
-# 13. CASE: the direct kernel's validity bytes of a CASE without ELSE under a WHERE and k_pack_valid's ballots and zero
+# 13. CASE: the direct kernel's validity bytes of a CASE without ELSE under a WHERE and k_pack_bits's ballots and zero
 # count (a ragged last word), the NULLS kernel without a WHERE, the TMA interpreter loop (CASE with ELSE), and the reduce
 # and group scan counting CASE-made nulls under a fused WHERE
 for n in [1, 31, 33, 300_001]:

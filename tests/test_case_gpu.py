@@ -217,7 +217,7 @@ def test_kernels(ctx):
     _, k = traced(lambda: project(ctx, [x], [case([(col(0) > 0.5, col(0))])]))
     assert k == {"k_filter_project<kCaseDepth,1>"}
     _, k = traced(lambda: project(ctx, [x], [case([(col(0) > 0.5, col(0))])], pred=col(0) < 0.7))
-    assert k == {"k_filter_project<kCaseDepth,1>", "k_pack_valid"}
+    assert k == {"k_filter_project<kCaseDepth,1>", "k_pack_bits"}
     (got,) = project(ctx, [x], [case([(col(0) > 0.5, col(0))])], pred=col(0) < 0.7)
     sel = x < 0.7
     assert_column(got, np.where(x[sel] > 0.5, x[sel], 0), x[sel] > 0.5)

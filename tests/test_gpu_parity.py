@@ -7,7 +7,8 @@ import pytest
 import oracle_lib as O
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, workloads
-from datafusion_archive_b200.expr import AggregateFunction, col, lit
+from datafusion_archive_b200.expr import AggregateFunction, case, col, lit
+from kernel_trace import traced
 
 pytestmark = pytest.mark.gpu
 
@@ -177,7 +178,8 @@ def test_host_pipelined_matches_resident_path(ctx):
     r = ctx.filter_project_host([np.array([], dtype=np.float64)], col(0) > lit(0.5), [col(0)])
     assert r.nrows == 0
     r.free()
-    # referenced Utf8 / nullable / Boolean columns: the same entry point runs the resident operator (device result)
+    # referenced Utf8 / nullable / Boolean columns, and a numeric projection with a CASE without ELSE: the same entry
+    # point runs the resident operator (device result)
     import pyarrow as pa
     rng = np.random.default_rng(5)
     m = 200_000
@@ -187,7 +189,8 @@ def test_host_pipelined_matches_resident_path(ctx):
     flag = rng.random(m) < 0.5
     for arrs, p_, pr in [([names, x], col(1) > lit(0.5), [col(0), col(1)]),
                          ([xn, x], col(1) < lit(0.25), [col(0), col(0) + col(1)]),
-                         ([flag, x], col(0) & (col(1) > lit(0.5)), [col(1)])]:
+                         ([flag, x], col(0) & (col(1) > lit(0.5)), [col(1)]),
+                         ([x], col(0) < lit(0.9), [col(0), case([(col(0) > lit(0.5), col(0) * lit(2.0))])])]:
         r = ctx.filter_project_host(arrs, p_, pr)
         assert not r.on_host
         got = r.columns()
@@ -204,8 +207,10 @@ def test_host_pipelined_matches_resident_path(ctx):
     r = ctx.filter_project_host(arrays, pred, proj)
     assert r.on_host
     r.free()
-    r = ctx.filter_project_host([x], col(0) > lit(0.5), [col(0), col(0) < lit(0.75)], chunk_rows=50_000)  # a Boolean projection
+    # a Boolean projection: the resident operator runs once, and no chunk runs before it
+    r, k = traced(lambda: ctx.filter_project_host([x], col(0) > lit(0.5), [col(0), col(0) < lit(0.75)], chunk_rows=50_000))
     assert not r.on_host
+    assert sum(n.startswith("k_filter_project") for n in k) == 1 and k.count("k_pack_bits") == 1
     got = r.columns()
     r.free()
     assert np.array_equal(got[0], x[x > 0.5]) and np.array_equal(got[1], x[x > 0.5] < 0.75)
