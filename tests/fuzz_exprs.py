@@ -3,7 +3,7 @@ compare, boolean operands for And / Or), for GPU-vs-oracle fuzzing."""
 import numpy as np
 
 from datafusion_archive_b200 import _abi as A
-from datafusion_archive_b200.expr import AggregateFunction, BinaryExpr, col, lit
+from datafusion_archive_b200.expr import AggregateFunction, BinaryExpr, Case, Literal, col, fn, lit, utf8_fn
 
 MATH = [A.OP_ADD, A.OP_SUB, A.OP_MUL, A.OP_DIV]
 CMP = [A.OP_EQ, A.OP_NE, A.OP_LT, A.OP_LE, A.OP_GT, A.OP_GE]
@@ -45,13 +45,17 @@ def gen_query(rng, schema, max_depth=3, has_literal_only_ok=False):
 
 
 def references_column(e):
-    from datafusion_archive_b200.expr import Column, Cast
+    from datafusion_archive_b200.expr import Column, Cast, ScalarFunction, Utf8Function
     if isinstance(e, Column):
         return True
     if isinstance(e, BinaryExpr):
         return references_column(e.left) or references_column(e.right)
     if isinstance(e, Cast):
         return references_column(e.expr)
+    if isinstance(e, (ScalarFunction, Utf8Function)):
+        return any(references_column(a) for a in e.args)
+    if isinstance(e, Case):
+        return any(references_column(x) for w in e.whens for x in w) or (e.else_ is not None and references_column(e.else_))
     return False
 
 
@@ -123,7 +127,7 @@ class Table:
 
     def __init__(self):
         self.arrays, self.dtype, self.valid, self.hidden, self.profile = [], [], [], [], []
-        self.values, self.bools, self.safe, self.gated, self.gate = {}, [], {}, {}, None
+        self.values, self.bools, self.safe, self.gated, self.gate, self.utf8 = {}, [], {}, {}, None, []
 
     def add(self, values, valid, profile):
         self.arrays.append(column(values, valid))
@@ -184,15 +188,51 @@ def _cap(e):
     return 1, 0
 
 
+def add_strings(rng, t, n, k=2):
+    """k nullable Utf8 columns of utf8_fn_ref.random_strings (multi-byte and invalid bytes, spaces at either end, '')
+    with a `\\0` put into about one string in twenty, appended to the table; returns their indices."""
+    import pyarrow as pa
+    import utf8_fn_ref
+    out = []
+    for _ in range(k):
+        vals = utf8_fn_ref.random_strings(n, int(rng.integers(0, 1 << 30)), null_frac=0.15)
+        zero = rng.random(n) < 0.05
+        vals = [v if v is None or not z else v[:len(v) // 2] + b"\0" + v[len(v) // 2:] for v, z in zip(vals, zero)]
+        t.arrays.append(pa.array(vals, type=pa.binary()))
+        t.dtype.append(A.UTF8)
+        t.valid.append(np.array([v is not None for v in vals]))
+        t.hidden.append(vals)
+        t.profile.append("nulls")
+        t.utf8.append(len(t.arrays) - 1)
+        out.append(len(t.arrays) - 1)
+    return out
+
+
+# The full language (QueryGen(full=True)): every node kind, typed as the C ABI types it (it casts nothing).
+FULL_KINDS = ("case", "fn", "cast", "utf8_cmp", "like", "utf8_fn", "length", "transcendental", "guarded_div", "unguarded_div")
+EXACT_FNS = ["sqrt", "abs", "floor", "ceil", "trunc", "round", "signum"]
+TRANSCENDENTAL = ["exp", "ln", "log2", "log10", "sin", "cos", "tan", "asin", "acos", "atan", "power", "atan2"]
+LIKE_PATTERNS = [b"%", b"a%", b"%a", b"%a%", b"_", b"__%", b"%_", b"Hello%", b"%\xc3\xa9%", b"_\xf0\x9f\x98\x80%", b"%  ", b" %",
+                 b"%0123%", b"a_c", b"", b"%\0%"]
+UTF8_LITERALS = [b"", b"a", b"Hello", b"abc", b" ", b"\xc3\xa9", b"Z", b"\0", b"\xff"]
+
+
 class QueryGen:
     """Random expressions over a Table, typed as the reference types them (identical operand dtypes, Boolean operands
     of And / Or), with CAST only where the oracle implements it: a column to Int16 / Int32, an Int64 literal to
-    Float64.  `cols`: the columns a query may read (the engine reads at most 12 distinct columns per query)."""
+    Float64.  `cols`: the columns a query may read (the engine reads at most 12 distinct columns per query).
 
-    def __init__(self, rng, table, cols, max_depth=8):
-        self.rng, self.t, self.max_depth = rng, table, max_depth
+    full=True: the whole language, typed as the C ABI requires: CASE (1-4 WHENs, with and without ELSE, nested, as a
+    value and as a Boolean), the exact scalar functions at any depth over Float64 (other dtypes cast to it), CASTs
+    between every numeric dtype, Utf8 comparisons and LIKE over Utf8 columns and nests of upper / lower / trim /
+    substr (Int64 literal bounds), length / octet_length as Int64 leaves, and divisions guarded by a CASE over their
+    zero divisor beside a share of unguarded ones.  `seen` collects the node kinds made."""
+
+    def __init__(self, rng, table, cols, max_depth=8, full=False):
+        self.rng, self.t, self.max_depth, self.full = rng, table, max_depth, full
         self.cols = set(cols)
         self.divisor_role = "safe"
+        self.seen = set()
 
     def _lit(self, d, nonzero=False):
         r = self.rng
@@ -217,8 +257,125 @@ class QueryGen:
             return col(int(r.choice(sorted(own))))
         return self._lit(d)
 
+    # ---- the full language ----------------------------------------------------------------------------------------
+    def _utf8_cols(self):
+        return sorted(c for c in self.cols if self.t.dtype[c] == A.UTF8)
+
+    def utf8(self, depth):
+        """A Utf8 column or a nest of upper / lower / trim / ltrim / rtrim / substr over one."""
+        r = self.rng
+        if depth <= 0 or r.random() < 0.4:
+            return col(int(r.choice(self._utf8_cols())))
+        self.seen.add("utf8_fn")
+        name = str(r.choice(["upper", "lower", "trim", "ltrim", "rtrim", "substr", "substr"]))
+        inner = self.utf8(depth - 1)
+        if name != "substr":
+            return utf8_fn(name, inner)
+        start = lit(int(r.choice([-3, -1, 0, 1, 2, 3, 5])), A.INT64)
+        if r.random() < 0.4:
+            return utf8_fn("substr", inner, start)
+        return utf8_fn("substr", inner, start, lit(int(r.choice([0, 1, 2, 4, 9])), A.INT64))
+
+    def utf8_predicate(self):
+        r = self.rng
+        s = self.utf8(int(r.integers(0, 4)))
+        if r.random() < 0.4:
+            self.seen.add("like")
+            return BinaryExpr(s, int(r.choice([A.OP_LIKE, A.OP_NOT_LIKE])), lit(bytes(r.choice(LIKE_PATTERNS)), A.UTF8))
+        self.seen.add("utf8_cmp")
+        op = int(r.choice(CMP))
+        other = self.utf8(1) if r.random() < 0.3 else lit(bytes(r.choice(UTF8_LITERALS)), A.UTF8)
+        if isinstance(other, Literal) and r.random() < 0.3:
+            return BinaryExpr(other, op, s)  # a literal on the left
+        return BinaryExpr(s, op, other)
+
+    def _case(self, depth, value):
+        """CASE with 1-4 WHENs, with or without ELSE, whose values are made by value(depth)."""
+        r = self.rng
+        self.seen.add("case")
+        whens = [(self.boolean(max(0, depth - 1)), value(depth - 1)) for _ in range(int(r.integers(1, 5)))]
+        if any(isinstance(e, Case) for _, e in whens):
+            self.seen.add("nested_case")
+        return Case(whens, value(depth - 1) if r.random() < 0.6 else None)
+
+    def _divide(self, d, depth):
+        """x / y over a divisor that may be zero: guarded by a CASE on `y <> 0` (never raises) or, rarely, unguarded over
+        a value column (raises when a zero lands in a row that is evaluated)."""
+        r = self.rng
+        x = self.numeric(d, depth - 1)
+        own = sorted(c for c in self.cols if self.t.dtype[c] == d and c != self.t.gate)
+        if not own:
+            return BinaryExpr(x, A.OP_DIV, self._lit(d, nonzero=True))
+        y = col(int(r.choice(own)))
+        if r.random() < 0.12:
+            self.seen.add("unguarded_div")
+            return BinaryExpr(x, A.OP_DIV, y)
+        self.seen.add("guarded_div")
+        zero = lit(0.0 if d in FLOATS else 0, d)
+        return Case([(y.not_eq(zero), BinaryExpr(x, A.OP_DIV, y))], self.numeric(d, depth - 1) if r.random() < 0.7 else None)
+
+    def _full_numeric(self, d, depth):
+        r = self.rng
+        src = sorted(c for c in self.cols if self.t.dtype[c] in NUMERIC and self.t.dtype[c] != d)
+        if depth <= 0 or r.random() < 0.2:
+            if d == A.INT64 and self._utf8_cols() and r.random() < 0.15:
+                self.seen.add("length")
+                return utf8_fn(str(r.choice(["length", "octet_length", "char_length"])), self.utf8(int(r.integers(0, 3))))
+            if src and r.random() < 0.2:  # the C ABI casts columns (and Int64 literals to Float64) only
+                self.seen.add("cast")
+                return col(int(r.choice(src))).cast(d)
+            return self._leaf(d)
+        k = r.random()
+        if k < 0.2:
+            return self._case(depth, lambda dd: self.numeric(d, dd))
+        if k < 0.3 and src:
+            self.seen.add("cast")
+            return BinaryExpr(col(int(r.choice(src))).cast(d), int(r.choice([A.OP_ADD, A.OP_SUB, A.OP_MUL])), self.numeric(d, depth - 1))
+        if k < 0.5 and d == A.FLOAT64:
+            self.seen.add("fn")
+            return fn(str(r.choice(EXACT_FNS)), self.numeric(A.FLOAT64, depth - 1))
+        if k < 0.56:
+            return self._divide(d, depth)
+        op = int(r.choice([A.OP_ADD, A.OP_SUB, A.OP_MUL]))
+        left = self.numeric(d, depth - 1)
+        right = self.numeric(d, depth - 1) if r.random() < 0.6 else self._leaf(d)
+        return BinaryExpr(left, op, right)
+
+    def _full_boolean(self, depth):
+        r = self.rng
+        k = r.random()
+        if self._utf8_cols() and k < 0.2:
+            return self.utf8_predicate()
+        if depth > 0 and k < 0.3:
+            self.seen.add("bool_case")
+            return self._case(depth, lambda dd: self.boolean(max(0, dd)))
+        return None
+
+    def deep(self, d):
+        """A right-nested chain `l1 op (l2 op (.. (CASE ..)))` whose stack depth is exactly 8, the limit: the entries
+        below the top are spilled, and their operands are small CASEs and guarded divisions, so the spilled entries
+        carry validity and DivideByZero bits."""
+        import expr_ref
+        r = self.rng
+        self.seen.add("deep")
+        small = lambda: self._case(1, lambda dd: self._leaf(d)) if r.random() < 0.4 else self._divide(d, 1) if r.random() < 0.4 else self._leaf(d)  # noqa: E731
+        e = self._case(1, lambda dd: self._leaf(d))
+        while expr_ref.stack_depth(e, self.t.dtype) < 8:
+            e = BinaryExpr(small(), int(r.choice([A.OP_ADD, A.OP_SUB, A.OP_MUL])), e)
+        return e
+
+    def transcendental(self):
+        """A transcendental function of Float64 operands: only ever the root of a projection."""
+        r = self.rng
+        self.seen.add("transcendental")
+        name = str(r.choice(TRANSCENDENTAL))
+        args = [self.numeric(A.FLOAT64, int(r.integers(0, 3))) for _ in range(2 if name in ("power", "atan2") else 1)]
+        return fn(name, *args)
+
     def numeric(self, d, depth):
         r = self.rng
+        if self.full:
+            return self._full_numeric(d, depth)
         if depth <= 0 or r.random() < 0.25:
             return self._leaf(d)
         op = int(r.choice(MATH))
@@ -237,6 +394,10 @@ class QueryGen:
 
     def boolean(self, depth):
         r = self.rng
+        if self.full:
+            b = self._full_boolean(depth)
+            if b is not None:
+                return b
         bools = [c for c in self.cols if self.t.dtype[c] == A.BOOL]
         if depth <= 0 or r.random() < 0.35:
             if bools and r.random() < 0.3:
@@ -260,31 +421,65 @@ class QueryGen:
         return self.numeric(d, int(self.rng.integers(0, self.max_depth + 1)))
 
 
+def _synthetic_slots(e, schema):
+    """The synthetic columns the compiler makes for `e`: one per Utf8 predicate and per Int64 Utf8 function nest."""
+    from datafusion_archive_b200.expr import Cast, ScalarFunction, Utf8Function
+    if isinstance(e, Utf8Function):
+        return 1 if e.dtype == A.INT64 else 0
+    if isinstance(e, BinaryExpr):
+        if e.op in (A.OP_LIKE, A.OP_NOT_LIKE) or e.left.get_type(schema) == A.UTF8:
+            return 1
+        return _synthetic_slots(e.left, schema) + _synthetic_slots(e.right, schema)
+    if isinstance(e, Cast):
+        return _synthetic_slots(e.expr, schema)
+    if isinstance(e, ScalarFunction):
+        return sum(_synthetic_slots(a, schema) for a in e.args)
+    if isinstance(e, Case):
+        return sum(_synthetic_slots(x, schema) for w in e.whens for x in w) + (_synthetic_slots(e.else_, schema) if e.else_ is not None else 0)
+    return 0
+
+
 def fits(exprs, schema):
-    """Whether a query of these programs fits the engine's program-set limits (96 instructions, 12 columns)."""
-    n, cols = 0, set()
+    """Whether a query of these programs fits the engine's program-set limits (96 instructions, 12 columns, synthetic
+    ones included, stack depth 8)."""
+    import expr_ref
+    n, cols, synth = 0, set(), 0
     for e in exprs:
         prog = e.program(schema)
         n += len(prog)
-        cols |= {i.col for i in prog if i.op == A.OP_COL}
-    return n <= 96 and len(cols) <= 12
+        cols |= {i.col for i in prog if i.op == A.OP_COL and schema[i.col] != A.UTF8}
+        synth += _synthetic_slots(e, schema)
+    return n <= 96 and len(cols) + synth <= 12 and all(expr_ref.stack_depth(e, schema) <= 8 for e in exprs)
 
 
-def gen_fp_query(rng, table, ncols=8, with_pred=True):
+def gen_fp_query(rng, table, ncols=8, with_pred=True, full=False, seen=None):
     """(pred, projections) for filter / project over a random subset of the table's columns (gate always included):
-    1-3 numeric projections and sometimes a Boolean one.  Retries until the query fits the engine's limits."""
+    1-3 numeric projections and sometimes a Boolean one.  Retries until the query fits the engine's limits.
+    full: the whole language (QueryGen(full=True)), every Utf8 column readable, and sometimes a transcendental
+    projection; `seen` (a set) collects the node kinds made."""
     schema = table.dtype
     while True:
-        others = [i for i in range(len(schema)) if i != table.gate]
+        others = [i for i in range(len(schema)) if i != table.gate and schema[i] != A.UTF8]
         cols = set(rng.choice(others, size=min(ncols, len(others)), replace=False).tolist()) | {table.gate}
-        g = QueryGen(rng, table, cols)
+        if full:
+            cols |= set(table.utf8)
+        g = QueryGen(rng, table, cols, full=full, max_depth=8 if not full else 6)
         pred = g.predicate() if with_pred else None
         ds = sorted({schema[c] for c in cols if schema[c] in NUMERIC})
         proj = [g.value(int(rng.choice(ds)), with_pred) for _ in range(int(rng.integers(1, 4)))]
         if rng.random() < 0.2:
             g.divisor_role = "safe" if not with_pred else "gated"
             proj.append(g.boolean(2))
+        if full and rng.random() < 0.25:
+            proj.append(g.transcendental())
+        if full and rng.random() < 0.25:
+            proj[0] = g.deep(int(rng.choice(ds)))
+        if full and pred is not None and rng.random() < 0.15:
+            d = int(rng.choice(ds))
+            pred = BinaryExpr(pred, A.OP_AND, BinaryExpr(g.deep(d), A.OP_GT, g._lit(d)))
         if fits(proj + ([pred] if pred is not None else []), schema) and any(references_column(e) for e in proj):
+            if seen is not None:
+                seen |= g.seen
             return pred, proj
 
 
@@ -303,27 +498,35 @@ def add_keys(rng, t, key_dtypes, n):
     return out
 
 
-def gen_agg_query(rng, t, key_cols, with_pred, plain_args, distinct_avg=False):
+def gen_agg_query(rng, t, key_cols, with_pred, plain_args, distinct_avg=False, full=False, seen=None):
     """(pred, keys, aggs): the keys are the key columns or expressions of them; 1-4 of MIN / MAX / SUM / COUNT (and
-    AVG / COUNT(DISTINCT) when asked) over plain columns or random expressions."""
+    AVG / COUNT(DISTINCT) when asked) over plain columns or random expressions.  full: the whole language in the
+    arguments and the WHERE, and keys that are sometimes a CASE over the key column."""
     while True:
-        others = [i for i in range(len(t.dtype)) if i != t.gate and i not in key_cols and t.dtype[i] != A.BOOL]
+        others = [i for i in range(len(t.dtype)) if i != t.gate and i not in key_cols and t.dtype[i] not in (A.BOOL, A.UTF8)]
         cols = set(rng.choice(others, size=min(6, len(others)), replace=False).tolist()) | {t.gate} | set(t.bools)
-        g = QueryGen(rng, t, cols, max_depth=8 if not plain_args else 4)
+        if full:
+            cols |= set(t.utf8)
+        g = QueryGen(rng, t, cols, max_depth=(8 if not full else 5) if not plain_args else 4, full=full)
         pred = g.predicate() if with_pred else None
         keys = []
         for k in key_cols:
             e = col(k)
-            if rng.random() < 0.4:
+            if full and rng.random() < 0.4:
+                g.seen.add("case")
+                e = Case([(g.boolean(1), e)], e + lit(1, t.dtype[k]) if rng.random() < 0.7 else None)
+            elif rng.random() < 0.4:
                 e = e + lit(int(rng.integers(1, 9)), t.dtype[k]) if rng.random() < 0.5 else e * lit(3, t.dtype[k])
             keys.append(e)
         funcs = ["min", "max", "sum", "count"] + (["avg", "distinct"] if distinct_avg else [])
         aggs = []
         for _ in range(int(rng.integers(1, 5))):
-            c = int(rng.choice(sorted(cols - {t.gate} - set(t.bools))))
-            arg = col(c) if plain_args else g.value(t.dtype[c], with_pred)
+            c = int(rng.choice(sorted(cols - {t.gate} - set(t.bools) - set(t.utf8))))
+            arg = col(c) if plain_args else g.deep(t.dtype[c]) if full and rng.random() < 0.2 else g.value(t.dtype[c], with_pred)
             f = str(rng.choice(funcs))
             aggs.append(AggregateFunction("count", arg, distinct=True) if f == "distinct" else AggregateFunction(f, arg))
         exprs = keys + [a.arg for a in aggs] + ([pred] if pred is not None else [])
         if fits(exprs, t.dtype):
+            if seen is not None:
+                seen |= g.seen
             return pred, keys, aggs

@@ -11,7 +11,9 @@ import pytest
 
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
-from datafusion_archive_b200.expr import AggregateFunction, BinaryExpr, Case, Cast, Column, Literal, case, col, lit
+from datafusion_archive_b200.expr import AggregateFunction, case, col, lit
+import expr_ref
+from groupby_ref import arrow_nullable
 from kernel_trace import traced_set as traced
 from test_avg_gpu import rows
 
@@ -48,78 +50,7 @@ def dctx():
 def ref(e, arrays, nulls):
     """(values, valid, err) of `e` per row, as the extended interpreter computes them.  `nulls`: the input columns'
     bitmaps are read (no WHERE above the expression); else every input slot reads as valid."""
-    n = len(_vals(arrays[0]))
-    if isinstance(e, Column):
-        a = arrays[e.index]
-        v = _vals(a)
-        valid = _valid(a) if nulls else np.ones(n, bool)
-        return v, valid, np.zeros(n, bool)
-    if isinstance(e, Cast):
-        v, valid, err = ref(e.expr, arrays, nulls)
-        return np.where(valid, v, 0).astype(A.NP_OF[e.dtype]), valid, err
-    if isinstance(e, Literal):
-        return np.full(n, e.value, dtype=A.NP_OF[e.dtype] if e.dtype != A.BOOL else bool), np.ones(n, bool), np.zeros(n, bool)
-    if isinstance(e, Case):
-        if e.else_ is not None:
-            v, valid, err = ref(e.else_, arrays, nulls)
-            v = v.copy()
-        else:
-            v0, _, _ = ref(e.whens[0][1], arrays, nulls)
-            v, valid, err = np.zeros(n, v0.dtype), np.zeros(n, bool), np.zeros(n, bool)
-        for c, x in reversed(e.whens):
-            cv, cvalid, cerr = ref(c, arrays, nulls)
-            xv, xvalid, xerr = ref(x, arrays, nulls)
-            taken = cv.astype(bool) & cvalid
-            v = np.where(taken, xv, v)
-            valid = np.where(taken, xvalid, valid)
-            err = cerr | np.where(taken, xerr, err)
-        v = np.where(valid, v, np.zeros_like(v))
-        return v, valid, err
-    assert isinstance(e, BinaryExpr)
-    a, va, ea = ref(e.left, arrays, nulls)
-    b, vb, eb = ref(e.right, arrays, nulls)
-    both = va & vb
-    err = ea | eb
-    op = e.op
-    if op in (A.OP_EQ, A.OP_NE, A.OP_LT, A.OP_LE, A.OP_GT, A.OP_GE):
-        f = {A.OP_EQ: np.equal, A.OP_NE: np.not_equal, A.OP_LT: np.less, A.OP_LE: np.less_equal, A.OP_GT: np.greater,
-             A.OP_GE: np.greater_equal}[op]
-        v = f(a, b)
-        ln, rn = ~va, ~vb  # nulls are ordered: eq both null, lt / le null on the left, gt / ge null on the right
-        nv = {A.OP_EQ: ln & rn, A.OP_NE: ~(ln & rn), A.OP_LT: ln, A.OP_LE: ln, A.OP_GT: rn, A.OP_GE: rn}[op]
-        return np.where(both, v, nv), np.ones(n, bool), err
-    with np.errstate(all="ignore"):
-        if op == A.OP_AND:
-            v = a.astype(bool) & b.astype(bool)
-        elif op == A.OP_OR:
-            v = a.astype(bool) | b.astype(bool)
-        elif op == A.OP_ADD:
-            v = a + b
-        elif op == A.OP_SUB:
-            v = a - b
-        elif op == A.OP_MUL:
-            v = a * b
-        else:
-            err = err | ((b == 0) & both)
-            if np.issubdtype(a.dtype, np.integer):
-                q = np.where(b == 0, 0, np.abs(a) // np.where(b == 0, 1, np.abs(b)))
-                v = (q * np.sign(a) * np.sign(b)).astype(a.dtype)
-            else:
-                v = a / b
-    v = np.where(both, v, np.zeros_like(v))
-    return v, both, err
-
-
-def _vals(a):
-    if isinstance(a, pa.Array):
-        return np.asarray(a.fill_null(0 if not pa.types.is_boolean(a.type) else False).to_numpy(zero_copy_only=False))
-    return np.asarray(a)
-
-
-def _valid(a):
-    if isinstance(a, pa.Array):
-        return ~np.asarray(a.is_null().to_numpy(zero_copy_only=False))
-    return np.ones(len(a), bool)
+    return expr_ref.evaluate(e, arrays, read_bitmaps=nulls)
 
 
 def project(c, arrays, exprs, pred=None):
@@ -387,6 +318,24 @@ def test_aggregate_arguments(ctx, with_pred):
                     assert np.isclose(gv, ev, rtol=1e-12), (f, kk, gv, ev)
                 else:
                     assert gv == ev, (f, kk, gv, ev)
+
+
+def test_a_case_passes_the_value_stored_under_a_selected_null_through(ctx):
+    """GROUP BY SUM / MIN / MAX and a GROUP BY key read the value stored under a null that a CASE selects, as they read
+    a null column's own; COUNT skips the null."""
+    n = 1_000
+    v = np.arange(n, dtype=np.int64) + 100
+    valid = np.arange(n) % 3 != 0
+    y = arrow_nullable(v, valid)  # the stored values stay under the nulls
+    k = (np.arange(n) % 4).astype(np.int64)
+    x = np.linspace(0, 1, n)
+    e = case([(col(2) < 2.0, col(0))], lit(0))  # always taken
+    got = run_agg(ctx, [y, k, x], [col(1)], [AggregateFunction(f, e) for f in ("sum", "min", "max", "count")])
+    for g, s, mn, mx, c in zip(*[split(c_)[0] for c_ in got]):
+        sel = k == g
+        assert (s, mn, mx, c) == (v[sel].sum(), v[sel].min(), v[sel].max(), valid[sel].sum()), g
+    got = run_agg(ctx, [y, k, x], [case([(col(2) < 2.0, col(0))])], [AggregateFunction("count", col(2))])
+    assert sorted(got[0].tolist()) == v.tolist() and (got[1] == 1).all()
 
 
 def test_group_by_keys(ctx):

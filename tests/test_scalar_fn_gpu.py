@@ -14,6 +14,7 @@ import pytest
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
 from datafusion_archive_b200.expr import AggregateFunction, col, fn
+from expr_ref import EXACT_REF, LONG, LONG2, rust_abs, rust_round, rust_signum
 from kernel_trace import traced_set as traced
 from test_avg_gpu import rows
 
@@ -28,29 +29,6 @@ def ctx():
     c = engine.GpuContext(0)
     yield c
     c.close()
-
-
-# ---- numpy restatements of the Rust f64 methods ------------------------------------------------------------------
-def rust_round(x):
-    """f64::round: half away from zero.  x - trunc(x) is exact, so 0.49999999999999994 is not a half."""
-    t = np.trunc(x)
-    with np.errstate(invalid="ignore"):
-        return np.where(np.abs(x - t) >= 0.5, t + np.copysign(1.0, x), t)
-
-
-def rust_signum(x):
-    return np.where(np.isnan(x), np.nan, np.copysign(1.0, x))
-
-
-def rust_abs(x):
-    return (x.view(np.uint64) & np.uint64(0x7FFFFFFFFFFFFFFF)).view(np.float64)
-
-
-EXACT_REF = {"sqrt": np.sqrt, "abs": rust_abs, "floor": np.floor, "ceil": np.ceil, "trunc": np.trunc, "round": rust_round,
-             "signum": rust_signum}
-LONG = {"exp": np.exp, "ln": np.log, "log2": np.log2, "log10": np.log10, "sin": np.sin, "cos": np.cos, "tan": np.tan,
-        "asin": np.arcsin, "acos": np.arccos, "atan": np.arctan}
-LONG2 = {"power": np.power, "atan2": np.arctan2}
 
 
 def bits_equal(got, exp):

@@ -6,7 +6,6 @@ numeric comparisons, as Boolean projections, in the aggregate's fused WHERE, aft
 SQL and at 1e7 rows through the host paths.  Under DFGPU_TRACE the pre-pass kernel of each pattern class is asserted."""
 import ctypes as C
 import os
-import re
 
 import numpy as np
 import pyarrow as pa
@@ -15,6 +14,7 @@ import pytest
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
 from datafusion_archive_b200.expr import AggregateFunction, col, lit
+from expr_ref import cmp3, like_ref
 from kernel_trace import traced_set as traced
 from test_avg_gpu import rows
 
@@ -31,23 +31,6 @@ def ctx():
     c = engine.GpuContext(0)
     yield c
     c.close()
-
-
-# ---- Python reference ----------------------------------------------------------------------------------------------
-def cmp3(a, b):
-    if a is None or b is None:
-        return (a is not None) - (b is not None)
-    return (a > b) - (a < b)
-
-
-def py_like(s, p):
-    rx = b"".join(b"[\\x00-\\xff]*" if ch == 0x25 else b"[\\x00-\\xff][\\x80-\\xbf]*+" if ch == 0x5F else re.escape(bytes([ch]))
-                  for ch in p)
-    return re.fullmatch(rx, s, re.DOTALL) is not None
-
-
-def like_ref(vals, p, neg=False):
-    return np.array([v is not None and (py_like(v, p) != neg) for v in vals], bool)
 
 
 def strings(n, seed, null_frac=0.1):
