@@ -1,4 +1,5 @@
-"""Exact CPU reference of the GROUP BY / reduce operator (numpy only), for checking every kernel instantiation.
+"""Exact CPU reference of the GROUP BY / reduce operator (numpy only), for checking every kernel instantiation and every
+aggregate function the operator accepts: MIN, MAX, SUM, COUNT, AVG and COUNT(DISTINCT).
 
 The semantics are those DESIGN §7 states for the GPU path:
 * keys are grouped by value and keep their own dtype; the bytes under a null key slot are the key;
@@ -7,14 +8,35 @@ The semantics are those DESIGN §7 states for the GPU path:
 * integer SUM is exact and wraps at the width of its output dtype, which is the argument dtype;
 * COUNT counts the valid values, as uint64;
 * float SUM: NaN if a NaN or both infinities are present, else the infinity present, else within
-  gamma(n) * sum|v| of the exact sum, gamma(n) = n u / (1 - n u): a bound that holds for any summation order;
-* GROUP BY reads MIN / MAX / SUM arguments ignoring the validity bitmap (arrow 0.12 `value(row)`), while a
-  reduction without GROUP BY skips null values and is null when no value is valid.
+  gamma(n) * sum|v| of the exact sum, gamma(n) = n u / (1 - n u): a bound that holds for any summation order.  The
+  bound is 0 (the sum is exact) when every value is a multiple of a power of two q >= the dtype's smallest normal and
+  sum|v| < 2^p q (p = 53, or 24 for Float32): then every partial sum in any order is exactly representable and no
+  partial sum is subnormal, so Float32's flush to zero cannot apply;
+* AVG: Float64, the mean of the valid values, each first rounded to f64 (integers beyond 2^53 round to nearest).  Null
+  when the group has no valid value.  NaN if a NaN or both infinities are present, else the infinity present, else
+  within the f64 SUM bound above divided by the count, plus the rounding of that one division; when the sum is exact,
+  it is exactly the f64 quotient sum / count;
+* COUNT(DISTINCT): the number of distinct valid values, as uint64; +0.0 and -0.0 are one value, and all NaNs are one
+  value;
+* GROUP BY reads MIN / MAX / SUM arguments ignoring the validity bitmap (arrow 0.12 `value(row)`), while COUNT, AVG and
+  COUNT(DISTINCT) skip null values, so a group whose values are all null counts 0 and its AVG is null;
+* without GROUP BY every aggregate skips null values and the result is one row, also over zero rows: COUNT and
+  COUNT(DISTINCT) are 0 there, and MIN / MAX / SUM / AVG are null when no value is valid;
+* WHERE: `where` is the per-row pass mask, and only the rows it passes are aggregated.  The keys and arguments of those
+  rows are read as over FilterRelation's output, which has no bitmaps: the value under a null slot of a column is an
+  ordinary valid value there, and only an expression such as a CASE without ELSE can still be null.  The caller passes
+  keys and arguments evaluated that way.  With the rules above, a COUNT under a WHERE that passes nothing is 0
+  without GROUP BY, and the other aggregates are null.
 """
 import numpy as np
 
-MIN, MAX, SUM, COUNT = "min", "max", "sum", "count"
-_U = {np.dtype(np.float64): 2.0 ** -53, np.dtype(np.float32): 2.0 ** -24}
+MIN, MAX, SUM, COUNT, AVG, COUNT_DISTINCT = "min", "max", "sum", "count", "avg", "count_distinct"
+_P = {np.dtype(np.float64): 53, np.dtype(np.float32): 24}  # significand bits; the unit roundoff u is 2^-p
+
+
+def func_of(agg):
+    """The reference's name for an expr.AggregateFunction."""
+    return COUNT_DISTINCT if agg.distinct else agg.name
 
 
 def _vm(x):
@@ -30,13 +52,11 @@ class Expected:
 
     def __init__(self, keys, aggs):
         self.keys = keys   # list of arrays, one per key column, sorted by key tuple
-        self.aggs = aggs   # list of dicts, see _agg
+        self.aggs = aggs   # list of dicts, see aggregate
 
 
 def _segments(keys, n):
     """Row order that sorts by the key tuple, segment starts of equal keys, and the keys of each segment."""
-    if not keys:
-        return np.arange(n), (np.zeros(1, dtype=np.int64) if n else np.zeros(0, dtype=np.int64)), []
     order = np.lexsort([k for k in reversed(keys)])
     sk = [k[order] for k in keys]
     change = np.zeros(n, dtype=bool)
@@ -48,85 +68,122 @@ def _segments(keys, n):
     return order, starts, [k[starts] for k in sk]
 
 
-def _reduceat(ufunc, x, starts, empty):
-    """ufunc.reduceat over segments, where an empty segment (possible only without GROUP BY) yields `empty`."""
-    if len(x) == 0:
-        return np.full(len(starts), empty, dtype=x.dtype)
-    return ufunc.reduceat(x, starts)
+def _reduce(ufunc, x, seg, nseg, empty):
+    """ufunc over the elements of each segment (seg: the sorted segment id of each element); `empty` for a segment
+    without element."""
+    out = np.full(nseg, empty, dtype=x.dtype)
+    if len(x):
+        present, starts = np.unique(seg, return_index=True)
+        out[present] = ufunc.reduceat(x, starts)
+    return out
 
 
-def _min_max(func, v, starts, counts):
+def _min_max(func, v, seg, nseg):
     dt = v.dtype
     if not np.issubdtype(dt, np.floating):
         ufunc, empty = (np.minimum, np.iinfo(dt).max) if func == MIN else (np.maximum, np.iinfo(dt).min)
-        return {"values": _reduceat(ufunc, v, starts, empty), "isnan": np.zeros(len(starts), dtype=bool)}
+        return {"values": _reduce(ufunc, v, seg, nseg, empty), "isnan": np.zeros(nseg, dtype=bool)}
     nan = np.isnan(v)
     fill = np.inf if func == MIN else -np.inf
     w = np.where(nan, dt.type(fill), v)
     ufunc = np.minimum if func == MIN else np.maximum
-    r = _reduceat(ufunc, w, starts, fill).astype(dt)
-    seg = np.repeat(np.arange(len(starts)), counts)
-    all_nan = np.bincount(seg, weights=~nan, minlength=len(starts)) == 0
+    r = _reduce(ufunc, w, seg, nseg, fill).astype(dt)
+    all_nan = np.bincount(seg, weights=~nan, minlength=nseg) == 0
     # the total order puts -0.0 below +0.0: a zero extremum is -0.0 for MIN when the group holds a -0.0,
     # and +0.0 for MAX when it holds a +0.0
     want_sign = func == MIN
-    has = np.bincount(seg, weights=(w == 0) & (np.signbit(w) == want_sign), minlength=len(starts)) > 0
+    has = np.bincount(seg, weights=(w == 0) & (np.signbit(w) == want_sign), minlength=nseg) > 0
     zero = r == 0
     r[zero & has] = dt.type(-0.0 if want_sign else 0.0)
     r[zero & ~has] = dt.type(0.0 if want_sign else -0.0)
     return {"values": r, "isnan": all_nan}
 
 
-def _float_sum(v, starts, counts):
+def _lowest_bit(x):
+    """The value of the lowest set significand bit of each nonzero finite x, a power of two."""
+    m, e = np.frexp(x.astype(np.float64))  # x = m 2^e, 0.5 <= |m| < 1, and m 2^53 is an integer
+    sig = np.abs(np.ldexp(m, 53)).astype(np.uint64)
+    return np.ldexp((sig & (~sig + np.uint64(1))).astype(np.float64), e - 53)
+
+
+def _float_sum(v, seg, nseg):
     dt = v.dtype
-    u = _U[dt]
-    nseg = len(starts)
-    seg = np.repeat(np.arange(nseg), counts)
+    u = 2.0 ** -_P[dt]
     flags = lambda m: np.bincount(seg, weights=m, minlength=nseg) > 0  # noqa: E731
     nan, pinf, ninf = flags(np.isnan(v)), flags(v == np.inf), flags(v == -np.inf)
-    fin = np.where(np.isfinite(v), v, dt.type(0)).astype(np.longdouble)
-    exact = _reduceat(np.add, fin, starts, 0).astype(np.longdouble) if nseg else np.zeros(0, dtype=np.longdouble)
-    absum = _reduceat(np.add, np.abs(fin), starts, 0).astype(np.float64) if nseg else np.zeros(0)
+    fin = np.where(np.isfinite(v), v, dt.type(0))
+    exact = _reduce(np.add, fin.astype(np.longdouble), seg, nseg, 0)
+    absum = _reduce(np.add, np.abs(fin).astype(np.longdouble), seg, nseg, 0)
+    counts = np.bincount(seg, minlength=nseg)
     nu = counts.astype(np.float64) * u
     gamma = nu / (1.0 - nu)
     # the long-double reference sum has an error bound of its own (64-bit significand), well below gamma
-    bound = (gamma + counts * 2.0 ** -63) * absum
+    bound = (gamma + counts * 2.0 ** -63) * absum.astype(np.float64)
+    q = _reduce(np.minimum, np.where(fin != 0, _lowest_bit(fin), np.inf), seg, nseg, np.inf)
+    bound[(absum < np.ldexp(q, _P[dt]).astype(np.longdouble)) & (q >= np.finfo(dt).tiny)] = 0.0
     special = np.where(nan | (pinf & ninf), 1, np.where(pinf, 2, np.where(ninf, 3, 0)))
     return {"exact": exact, "bound": bound, "special": special}
 
 
-def aggregate(keys, aggs):
-    """keys: list of key columns; aggs: list of (func, column) with func in MIN / MAX / SUM / COUNT.  A column is
-    an array or a (values, valid) pair.  Returns an Expected, keys sorted by tuple (numpy order of each dtype)."""
+def _avg(x, seg, nseg, nvalid):
+    """AVG of the f64 values x: the SUM rule above, divided by the count."""
+    s = _float_sum(x, seg, nseg)
+    c = np.maximum(nvalid, 1).astype(np.float64)
+    exact, bound = s["exact"], s["bound"]
+    s["exact"] = np.where(bound == 0, (exact.astype(np.float64) / c).astype(np.longdouble), exact / c)
+    s["bound"] = np.where(bound == 0, 0.0, (bound + 2.0 ** -53 * (np.abs(exact).astype(np.float64) + bound)) / c)
+    return s
+
+
+def _count_distinct(v, seg, nseg):
+    if v.dtype.kind == "f":
+        w = v.astype(np.float64) + 0.0  # -0.0 + 0.0 is +0.0
+        v = w.view(np.uint64).copy()
+        v[np.isnan(w)] = 0x7FF8000000000000
+    order = np.lexsort((v, seg))
+    s, x = seg[order], v[order]
+    first = np.ones(len(order), dtype=bool)
+    first[1:] = (s[1:] != s[:-1]) | (x[1:] != x[:-1])
+    return np.bincount(s[first], minlength=nseg).astype(np.uint64)
+
+
+def aggregate(keys, aggs, where=None):
+    """keys: list of key columns, none without GROUP BY; aggs: list of (func, column) with func one of MIN / MAX / SUM /
+    COUNT / AVG / COUNT_DISTINCT; where: the per-row pass mask of a WHERE, or None.  A column is an array or a (values,
+    valid) pair.  Returns an Expected, keys sorted by tuple (numpy order of each dtype)."""
     kv = [_vm(k)[0] for k in keys]
     n = len(_vm(aggs[0][1])[0]) if aggs else len(kv[0])
-    order, starts, ukeys = _segments(kv, n)
+    take = np.ones(n, dtype=bool) if where is None else np.asarray(where, dtype=bool)
+    kv = [k[take] for k in kv]
+    n = int(take.sum())
     grouped = len(keys) > 0
+    order, starts, ukeys = _segments(kv, n) if grouped else (np.arange(n), np.zeros(1, dtype=np.int64), [])
+    nseg = len(starts)
+    seg = np.repeat(np.arange(nseg), np.diff(np.append(starts, n)))
     out = []
     for func, c in aggs:
         v, valid = _vm(c)
-        v = v[order]
-        valid = np.ones(n, dtype=bool) if valid is None else valid[order]
-        if grouped:
-            counts = np.diff(np.append(starts, n))
-            nvalid = np.add.reduceat(valid.astype(np.uint64), starts) if n else np.zeros(0, dtype=np.uint64)
-            sel, sstarts, scounts = v, starts, counts
-        else:
-            # no GROUP BY: null values are skipped, and an aggregate over no valid value is null
-            sel = v[valid]
-            nvalid = np.array([valid.sum()], dtype=np.uint64)
-            sstarts, scounts = np.zeros(1, dtype=np.int64), np.array([len(sel)])
-        d = {"func": func, "null": (nvalid == 0) if not grouped and func != COUNT else np.zeros(len(starts), dtype=bool)}
+        v = v[take][order]
+        valid = np.ones(n, dtype=bool) if valid is None else valid[take][order]
+        nvalid = np.bincount(seg[valid], minlength=nseg).astype(np.uint64)
+        d = {"func": func, "null": np.zeros(nseg, dtype=bool)}
         if func == COUNT:
-            d.update(values=nvalid.astype(np.uint64), dtype=np.dtype(np.uint64))
-        elif func in (MIN, MAX):
-            d.update(_min_max(func, sel, sstarts, scounts), dtype=v.dtype)
-        elif np.issubdtype(v.dtype, np.floating):
-            d.update(_float_sum(sel, sstarts, scounts), dtype=v.dtype)
+            d.update(values=nvalid, dtype=np.dtype(np.uint64))
+        elif func == COUNT_DISTINCT:
+            d.update(values=_count_distinct(v[valid], seg[valid], nseg), dtype=np.dtype(np.uint64))
+        elif func == AVG:
+            d.update(_avg(v[valid].astype(np.float64), seg[valid], nseg, nvalid), dtype=np.dtype(np.float64), null=nvalid == 0)
         else:
-            wide = sel.astype(np.int64).view(np.uint64) if np.issubdtype(v.dtype, np.signedinteger) else sel.astype(np.uint64)
-            s = _reduceat(np.add, wide, sstarts, 0)
-            d.update(values=s.astype(v.dtype), dtype=v.dtype)  # wraps at the output width
+            sel, sseg = (v, seg) if grouped else (v[valid], seg[valid])
+            if not grouped:
+                d["null"] = nvalid == 0
+            if func in (MIN, MAX):
+                d.update(_min_max(func, sel, sseg, nseg), dtype=v.dtype)
+            elif np.issubdtype(v.dtype, np.floating):
+                d.update(_float_sum(sel, sseg, nseg), dtype=v.dtype)
+            else:
+                wide = sel.astype(np.int64).view(np.uint64) if np.issubdtype(v.dtype, np.signedinteger) else sel.astype(np.uint64)
+                d.update(values=_reduce(np.add, wide, sseg, nseg, 0).astype(v.dtype), dtype=v.dtype)  # wraps at the output width
         out.append(d)
     return Expected(ukeys, out)
 

@@ -8,6 +8,7 @@ import subprocess
 import numpy as np
 
 from datafusion_archive_b200 import _abi as A
+from datafusion_archive_b200.expr import col
 
 _ROOT = A.repo_root()
 _LIB = None
@@ -129,3 +130,21 @@ def aggregate(arrays, keys=(), aggs=(), batch_size=0, schema=None):
         return fetch_result(L, "oracle", out)
     finally:
         L.oracle_result_free(out)
+
+
+def rows(arrays, pred, exprs):
+    """FilterRelation + ProjectRelation: the value of each expression on each row that passes `pred`.  Filter gathers
+    every fixed-width column, which the reference's filter() does for Float64 / Utf8 only (filter.rs:82-108)."""
+    set_extensions(filter_all_primitives=True)
+    try:
+        return filter_project(arrays, pred, exprs)
+    finally:
+        set_extensions(filter_all_primitives=False)
+
+
+def filtered_aggregate(arrays, pred, keys, aggs):
+    """The reference's wiring of a WHERE under an aggregate: FilterRelation (gathers every column, dropping the bitmaps)
+    feeding AggregateRelation (context.rs:126-139, 162-192)."""
+    if pred is None:
+        return aggregate(arrays, keys, aggs)
+    return aggregate(rows(arrays, pred, [col(i) for i in range(len(arrays))]), keys, aggs)

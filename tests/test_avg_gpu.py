@@ -1,6 +1,7 @@
-"""AVG(x) on the GPU.  Inputs are integers or multiples of 1/8 small enough that every f64 sum is exact in any order,
-so results must equal the numpy reference (f64 sum of the non-null values / their count) bit for bit; random floats are
-compared with math.fsum at rtol 1e-12.  Under DFGPU_TRACE each dispatch case asserts the kernel that ran."""
+"""AVG(x) on the GPU against the exact reference of tests/groupby_ref.py.  Inputs are integers or multiples of 1/8 small
+enough that every f64 sum is exact in any order, so results must equal the f64 quotient of the sum of the non-null values
+and their count; random floats are compared with math.fsum at rtol 1e-12.  Under DFGPU_TRACE each dispatch case asserts
+the kernel that ran."""
 import math
 import os
 
@@ -8,6 +9,7 @@ import numpy as np
 import pyarrow as pa
 import pytest
 
+import groupby_ref as G
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
 from datafusion_archive_b200.expr import AggregateFunction, col, lit
@@ -49,40 +51,9 @@ def run(ctx, batches, keys, aggs, pred=None, expected=0):
     return traced(lambda: gpu(ctx, batches, keys, aggs, pred, expected))
 
 
-def ref_fast(keys, v, valid=None):
-    """{key tuple: AVG of the valid values, None when there are none}, for inputs whose f64 sums are exact in any order."""
-    kc = [np.asarray(k).astype(np.int64) for k in keys]
-    ok = np.ones(len(v), bool) if valid is None else np.asarray(valid, bool)
-    uniq, inv = np.unique(np.stack(kc, axis=1), axis=0, return_inverse=True)
-    inv = inv.reshape(-1)
-    s = np.bincount(inv[ok], weights=np.asarray(v, np.float64)[ok], minlength=len(uniq))
-    c = np.bincount(inv[ok], minlength=len(uniq))
-    return {tuple(int(x) for x in u): (float(s[i] / c[i]) if c[i] else None) for i, u in enumerate(uniq)}
-
-
-def as_dict(cols, nkeys, which=0):
-    """{key tuple: value or None} of aggregate column `which`."""
-    keys = [np.asarray(c) for c in cols[:nkeys]]
-    keys = [k.astype(np.int64) if k.dtype.kind in "iu" else k for k in keys]
-    v = cols[nkeys + which]
-    vals, valid = (v if isinstance(v, tuple) else (v, None))
-    assert np.asarray(vals).dtype == np.float64
-    out = {}
-    for i in range(len(vals)):
-        g = tuple(k[i].item() if hasattr(k[i], "item") else k[i] for k in keys)
-        out[g] = None if valid is not None and not valid[i] else float(vals[i])
-    return out
-
-
-def same(a, b):
-    """Dict equality where NaN equals NaN and values are compared bit for bit."""
-    assert a.keys() == b.keys()
-    for g in a:
-        x, y = a[g], b[g]
-        if x is None or y is None:
-            assert x is None and y is None, (g, x, y)
-        else:
-            assert np.float64(x).view(np.uint64) == np.float64(y).view(np.uint64) or (math.isnan(x) and math.isnan(y)), (g, x, y)
+def check(got, keys, v, where=None):
+    """`got` (the keys, then AVG(v)) against groupby_ref."""
+    G.assert_matches(got, G.aggregate(keys, [(G.AVG, v)], where=where))
 
 
 def values(dt, n, rng):
@@ -107,7 +78,7 @@ def test_key_by_argument_dtype(ctx, kdt, vdt):
     k = rng.integers(0, 60, n).astype(kdt)
     v = values(vdt, n, rng)
     got, _ = run(ctx, [[k, v]], [col(0)], [avg(col(1))])
-    same(as_dict(got, 1), ref_fast([k], v))
+    check(got, [k], v)
 
 
 def test_lean_equals_sum_over_count(ctx):
@@ -120,19 +91,16 @@ def test_lean_equals_sum_over_count(ctx):
     assert "k_avg_finish" in names
     sc, names2 = run(ctx, [[k, v]], [col(0)], [AggregateFunction("sum", col(1)), AggregateFunction("count", col(1))])
     assert "k_hash_agg_lean<12,1>" in names2
-    a, b = as_dict(got, 1), as_dict([sc[0], sc[1], sc[2].astype(np.float64)], 1, 0)
-    cnt = {g: c for g, c in zip(sc[0].tolist(), sc[2].tolist())}
-    for g in a:
-        exp = b[g] / cnt[g[0]]
-        assert a[g] == pytest.approx(exp, rel=1e-12)
+    o, so = np.argsort(got[0]), np.argsort(sc[0])
+    assert np.array_equal(got[0][o], sc[0][so])
+    assert got[1][o] == pytest.approx(sc[1][so] / sc[2][so], rel=1e-12)
     # exact data: the two queries agree bit for bit
     w = (rng.integers(-800, 800, n) / 8).astype(np.float64)
     got, _ = run(ctx, [[k, w]], [col(0)], [avg(col(1))])
     sc, _ = run(ctx, [[k, w]], [col(0)], [AggregateFunction("sum", col(1)), AggregateFunction("count", col(1))])
-    mine = as_dict(got, 1)
-    for g, s, c in zip(sc[0].tolist(), sc[1].tolist(), sc[2].tolist()):
-        assert mine[(g,)] == s / c
-    same(mine, ref_fast([k], w))
+    o, so = np.argsort(got[0]), np.argsort(sc[0])
+    assert np.array_equal(got[0][o], sc[0][so]) and np.array_equal(got[1][o], sc[1][so] / sc[2][so])
+    check(got, [k], w)
 
 
 @pytest.mark.parametrize("vdt", [np.int32, np.int64, np.float32], ids=lambda d: np.dtype(d).name)
@@ -143,7 +111,7 @@ def test_plain_kernel(ctx, vdt):
     v = values(vdt, n, rng)
     got, names = run(ctx, [[k, v]], [col(0)], [avg(col(1))])
     assert "k_hash_agg_plain<2,0>" in names and not any(x.startswith("k_hash_agg_lean") for x in names), sorted(names)
-    same(as_dict(got, 1), ref_fast([k], v))
+    check(got, [k], v)
 
 
 def test_interpreter_expression_argument(ctx):
@@ -154,7 +122,7 @@ def test_interpreter_expression_argument(ctx):
     b = rng.integers(-1000, 1000, n).astype(np.int64)
     got, names = run(ctx, [[k, a, b]], [col(0)], [avg(col(1) * lit(3, A.INT64) + col(2))])
     assert any(x.startswith("k_hash_agg<") and x.endswith(",0,0>") for x in names), sorted(names)
-    same(as_dict(got, 1), ref_fast([k], a * 3 + b))
+    check(got, [k], a * 3 + b)
 
 
 def test_nulls_kernel_and_all_null_group(ctx):
@@ -167,11 +135,9 @@ def test_nulls_kernel_and_all_null_group(ctx):
     arr = pa.array(v, mask=~valid)
     got, names = run(ctx, [[k, arr]], [col(0)], [avg(col(1)), AggregateFunction("count", col(1))])
     assert "k_hash_agg<8,0,1>" in names, sorted(names)
-    d = as_dict(got, 1)
-    same(d, ref_fast([k], v, valid))
-    assert d[(7,)] is None
-    cnt = dict(zip(got[0].tolist(), np.asarray(got[2]).tolist()))
-    assert cnt[7] == 0
+    G.assert_matches(got, G.aggregate([k], [(G.AVG, (v, valid)), (G.COUNT, (v, valid))]))
+    g7 = np.flatnonzero(got[0] == 7)[0]
+    assert not got[1][1][g7] and got[2][g7] == 0
     # the result reports its null count
     bs = [ctx.upload([k, arr])]
     r = ctx.aggregate(bs, [col(0)], [avg(col(1))])
@@ -199,7 +165,7 @@ def test_front_table(ctx):
     assert "k_hash_agg_plain<2,1>" in names, sorted(names)
     k = np.concatenate([b[0] for b in batches])
     v = np.concatenate([b[1] for b in batches])
-    same(as_dict(got, 1), ref_fast([k], v))
+    check(got, [k], v)
 
 
 def test_wide_composite_key(ctx):
@@ -210,7 +176,7 @@ def test_wide_composite_key(ctx):
     v = (rng.integers(-800, 800, n) / 8).astype(np.float32)
     got, names = run(ctx, [[k1, k2, v]], [col(0), col(1)], [avg(col(2))])
     assert "k_hash_agg_wide<8,0>" in names, sorted(names)
-    same(as_dict(got, 2), ref_fast([k1, k2], v))
+    check(got, [k1, k2], v)
 
 
 def test_utf8_key(ctx):
@@ -222,9 +188,8 @@ def test_utf8_key(ctx):
     v = rng.integers(-1000, 1000, n).astype(np.int16)
     got, names = run(ctx, [[s, v]], [col(0)], [avg(col(1))])
     assert "k_utf8_group_verify" in names
-    d = as_dict(got, 1)
-    exp = ref_fast([idx], v)
-    same(d, {(words[g[0]],): x for g, x in exp.items()})
+    index = {w: i for i, w in enumerate(words)}
+    check([np.array([index[w] for w in got[0]])] + got[1:], [idx], v)
 
 
 def test_table_growth_with_replay(ctx):
@@ -303,12 +268,10 @@ def test_float_edges(ctx):
     v = np.array([x for xs in groups.values() for x in xs], dtype=np.float64)
     for keys, arrays in (([col(0)], [k, v]), ([col(0)], [k.astype(np.int32), v])):
         got, _ = run(ctx, [arrays], keys, [avg(col(1))])
-        d = as_dict(got, 1)
-        assert math.isnan(d[(0,)]) and math.isnan(d[(1,)]) and d[(2,)] == inf and d[(3,)] == -inf and d[(4,)] == 0.375
-    whole, _ = run(ctx, [[v[k == 2]]], [], [avg(col(0))])
-    assert float(whole[0][0]) == inf
-    whole, _ = run(ctx, [[v[k == 1]]], [], [avg(col(0))])
-    assert math.isnan(float(whole[0][0]))
+        check(got, arrays[:1], v)
+    for g in (1, 2):
+        whole, _ = run(ctx, [[v[k == g]]], [], [avg(col(0))])
+        check(whole, [], v[k == g])
 
 
 def test_float32_subnormals_are_kept(ctx):
@@ -316,12 +279,13 @@ def test_float32_subnormals_are_kept(ctx):
     v = np.array([tiny, 3 * tiny, tiny * 2, tiny], dtype=np.float32)
     k = np.zeros(len(v), np.int64)
     got, _ = run(ctx, [[k, v]], [col(0)], [avg(col(1))])
-    exp = float(np.float64(tiny) * 7 / 4)
-    assert as_dict(got, 1)[(0,)] == exp != 0.0
+    assert got[1][0] == np.float64(tiny) * 7 / 4 != 0.0
+    check(got, [k], v)
     whole, _ = run(ctx, [[v]], [], [avg(col(0))])
-    assert float(whole[0][0]) == exp
-    nul, _ = run(ctx, [[k, pa.array(v, mask=np.array([0, 0, 1, 0], bool))]], [col(0)], [avg(col(1))])
-    assert as_dict(nul, 1)[(0,)] == float(np.float64(tiny) * 5 / 3)
+    check(whole, [], v)
+    valid = np.array([1, 1, 0, 1], bool)
+    nul, _ = run(ctx, [[k, pa.array(v, mask=~valid)]], [col(0)], [avg(col(1))])
+    check(nul, [k], (v, valid))
 
 
 def test_int64_extremes(ctx):
@@ -329,11 +293,10 @@ def test_int64_extremes(ctx):
     k = np.array([0, 0, 0, 1, 1, 2, 3], dtype=np.int64)
     v = np.array([hi, hi, lo, lo, lo, hi, (1 << 53) + 1], dtype=np.int64)
     got, _ = run(ctx, [[k, v]], [col(0)], [avg(col(1))])
-    d = as_dict(got, 1)
-    assert d == {(0,): 2.0 ** 63 / 3, (1,): -(2.0 ** 63), (2,): 2.0 ** 63, (3,): 2.0 ** 53}  # rounded when widened
+    check(got, [k], v)  # each value rounded when widened: 2^63 / 3, -2^63, 2^63, 2^53
     u = np.array([np.iinfo(np.uint64).max, 1], dtype=np.uint64)
     whole, _ = run(ctx, [[u]], [], [avg(col(0))])
-    assert float(whole[0][0]) == 2.0 ** 63
+    assert float(whole[0][0]) == 2.0 ** 63  # 2^64 - 1 widens to 2^64, and 2^64 + 1 rounds to 2^64
 
 
 def test_batches_where_and_mixed(ctx):
@@ -347,7 +310,7 @@ def test_batches_where_and_mixed(ctx):
     vv = np.concatenate([b[1] for b in batches])
     ww = np.concatenate([b[2] for b in batches])
     got, _ = run(ctx, batches, [col(0)], [avg(col(2))], pred=col(1) > lit(10, A.INT32))
-    same(as_dict(got, 1), {g: x for g, x in ref_fast([kk[vv > 10]], ww[vv > 10]).items()})
+    check(got, [kk], ww, where=vv > 10)
     mixed = [AggregateFunction("sum", col(1)), avg(col(1)), AggregateFunction("count", col(1), distinct=True), avg(col(2)),
              AggregateFunction("min", col(2))]
     got, _ = run(ctx, batches, [col(0)], mixed)
@@ -355,11 +318,10 @@ def test_batches_where_and_mixed(ctx):
     o, ob = np.argsort(got[0]), np.argsort(base[0])
     for i, j in ((1, 1), (3, 2), (5, 3)):
         assert np.array_equal(np.asarray(got[i])[o], np.asarray(base[j])[ob])
-    same(as_dict(got, 1, 1), ref_fast([kk], vv))
-    same(as_dict(got, 1, 3), ref_fast([kk], ww))
+    exp = [(G.SUM, vv), (G.AVG, vv), (G.COUNT_DISTINCT, vv), (G.AVG, ww), (G.MIN, ww)]
+    G.assert_matches(got, G.aggregate([kk], exp))
     whole, _ = run(ctx, batches, [], mixed)
-    assert float(whole[1][0]) == float(np.float64(vv.sum()) / n) and float(whole[3][0]) == float(np.float64(ww.sum()) / n)
-    assert int(whole[0][0]) == int(vv.sum()) and int(whole[2][0]) == len(np.unique(vv))
+    G.assert_matches(whole, G.aggregate([], exp))
 
 
 def test_update_host_chunks(ctx):
@@ -370,7 +332,7 @@ def test_update_host_chunks(ctx):
     r = ctx.aggregate_host([k, v], keys=[col(0)], aggs=[avg(col(1))], chunk_rows=4 << 20)
     chunked = r.columns()
     r.free()
-    same(as_dict(chunked, 1), ref_fast([k], v))
+    check(chunked, [k], v)
 
 
 def test_errors(ctx):
@@ -394,7 +356,7 @@ def test_errors(ctx):
         gpu(ctx, [[k, k.astype(np.float64)]], [col(0)], [avg(col(1))] * 4 + [AggregateFunction("sum", col(1))])
     assert e.value.code == A.ERR_NOT_IMPLEMENTED and "accumulator words" in e.value.msg
     got = gpu(ctx, [[k, k.astype(np.float64)]], [col(0)], [avg(col(1))] * 4)
-    assert as_dict(got, 1, 3) == {(1,): 1.0, (2,): 2.0}
+    G.assert_matches(got, G.aggregate([k], [(G.AVG, k.astype(np.float64))] * 4))
 
 
 def rows(rel):
@@ -435,8 +397,7 @@ def test_sql(ctx):
         hctx.register_memory("t", [("k", k), ("v", v)], batch_size=30_000)
         rel = hctx.sql("SELECT k, AVG(v) FROM t WHERE v > 3 GROUP BY k")
         assert [dt for _, dt in rel.schema()] == [A.INT64, A.FLOAT64]
-        got = {(int(a),): float(m) for a, m in rows(rel)}
-        same(got, ref_fast([k[v > 3]], v[v > 3]))
+        check([np.concatenate(c) for c in zip(*rel.collect())], [k], v, where=v > 3)
         hctx.register_memory("u", [("k", k), ("v", v)], batch_size=30_000)
         rel = hctx.sql("SELECT AVG(v), COUNT(v) FROM u WHERE v > 100")
         assert rows(rel) == [(None, 0)]

@@ -1,11 +1,12 @@
-"""COUNT(DISTINCT x) on the GPU, exact against a numpy reference that de-duplicates (group key, normalised value) pairs,
-where the normalised value makes +0.0 and -0.0 one value and every NaN one value, and nulls are skipped."""
+"""COUNT(DISTINCT x) on the GPU, exact against the reference of tests/groupby_ref.py: +0.0 and -0.0 are one value,
+every NaN is one value, and nulls are skipped."""
 import os
 
 import numpy as np
 import pyarrow as pa
 import pytest
 
+import groupby_ref as G
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
 from datafusion_archive_b200.expr import AggregateFunction, col
@@ -28,40 +29,9 @@ def cd(arg):
     return AggregateFunction("count", arg, distinct=True)
 
 
-def norm(v):
-    """The 64-bit word distinctness is decided on (numpy side)."""
-    v = np.asarray(v)
-    if v.dtype.kind == "f":
-        d = v.astype(np.float64) + 0.0  # -0.0 + 0.0 == +0.0
-        bits = d.view(np.uint64).copy()
-        bits[np.isnan(d)] = 0x7FF8000000000000
-        return bits
-    return v.astype(np.int64).view(np.uint64)
-
-
-def ref(keys, v, valid=None, where=None):
-    """{key tuple: COUNT(DISTINCT v)} over rows passing `where`; groups whose values are all null count 0."""
-    n = len(v)
-    take = np.ones(n, bool) if where is None else np.asarray(where, bool)
-    ok = take if valid is None else take & np.asarray(valid, bool)
-    kcols = [np.asarray(k).astype(np.int64) for k in keys] or [np.zeros(n, np.int64)]
-    out = {g: 0 for g in zip(*[k[take].tolist() for k in kcols])}
-    cols = [k[ok] for k in kcols] + [norm(v)[ok]]
-    if len(cols[0]):
-        order = np.lexsort(cols[::-1])
-        cols = [c[order] for c in cols]
-        first = np.ones(len(order), bool)  # first row of each distinct (key, value) pair
-        first[1:] = np.any([c[1:] != c[:-1] for c in cols], axis=0)
-        for g in zip(*[k[first].tolist() for k in cols[:-1]]):
-            out[g] += 1
-    return out
-
-
-def as_dict(cols, nkeys):
-    keys = [np.asarray(c).astype(np.int64) for c in cols[:nkeys]]
-    vals = cols[nkeys:]
-    n = len(vals[0])
-    return [{tuple(int(k[i]) for k in keys): int(v[i]) for i in range(n)} for v in vals]
+def check(got, keys, v, where=None):
+    """`got` (the keys, then COUNT(DISTINCT v)) against groupby_ref."""
+    G.assert_matches(got, G.aggregate(keys, [(G.COUNT_DISTINCT, v)], where=where))
 
 
 def gpu(ctx, arrays, keys, aggs, pred=None, batches=1):
@@ -95,7 +65,7 @@ def test_key_by_argument_dtype(ctx, kdt, vdt):
     k = values(kdt, n, rng, distinct=40)
     v = values(vdt, n, rng, distinct=60)
     got = gpu(ctx, [k, v], [col(0)], [cd(col(1))])
-    assert as_dict(got, 1)[0] == ref([k], v)
+    check(got, [k], v)
 
 
 @pytest.mark.parametrize("vdt", [np.float32, np.float64], ids=lambda d: np.dtype(d).name)
@@ -108,9 +78,9 @@ def test_float_edges(ctx, vdt):
     v = np.concatenate([v, nans])
     k = np.arange(len(v), dtype=np.int64) % 3
     got = gpu(ctx, [k, v], [col(0)], [cd(col(1))])
-    assert as_dict(got, 1)[0] == ref([k], v)
+    check(got, [k], v)
     # +0.0 and -0.0 are one value, and every NaN payload is one more
-    assert as_dict(got, 1)[0][(0,)] == len(specials)
+    assert got[1][np.flatnonzero(got[0] == 0)[0]] == len(specials)
     whole = gpu(ctx, [v], [], [cd(col(0))])
     assert int(whole[0][0]) == len(specials)
 
@@ -124,9 +94,9 @@ def test_nulls(ctx):
     valid[k == 5] = False  # a group whose values are all null: present, count 0
     arr = pa.array(v, mask=~valid)
     got = gpu(ctx, [k, arr], [col(0)], [cd(col(1)), AggregateFunction("count", col(1))])
-    d = as_dict(got, 1)
-    assert d[0] == ref([k], v, valid)
-    assert d[0][(5,)] == 0 and d[1][(5,)] == 0
+    G.assert_matches(got, G.aggregate([k], [(G.COUNT_DISTINCT, (v, valid)), (G.COUNT, (v, valid))]))
+    g5 = np.flatnonzero(got[0] == 5)[0]
+    assert got[1][g5] == 0 and got[2][g5] == 0
     whole = gpu(ctx, [arr], [], [cd(col(0))])
     assert int(whole[0][0]) == len(np.unique(v[valid]))
 
@@ -189,9 +159,9 @@ def test_empty_marker_key_and_pair(ctx):
     k = np.array([-1, -1, -1, -1, 0, 0, 7, -1], dtype=np.int64)
     v = np.array([-1, -1, 3, 4, -1, -1, -1, 3], dtype=np.int64)
     got = gpu(ctx, [k, v], [col(0)], [cd(col(1))])
-    assert as_dict(got, 1)[0] == ref([k], v) == {(-1,): 3, (0,): 1, (7,): 1}
-    got = gpu(ctx, [k, v], [col(0)], [cd(col(1))], batches=3)
-    assert as_dict(got, 1)[0] == ref([k], v)
+    check(got, [k], v)
+    assert sorted(zip(got[0].tolist(), got[1].tolist())) == [(-1, 3), (0, 1), (7, 1)]
+    check(gpu(ctx, [k, v], [col(0)], [cd(col(1))], batches=3), [k], v)
 
 
 def test_three_batches(ctx):
@@ -200,7 +170,8 @@ def test_three_batches(ctx):
     v = rng.integers(0, 100, 300_000).astype(np.int64)
     one = gpu(ctx, [k, v], [col(0)], [cd(col(1))])
     three = gpu(ctx, [k, v], [col(0)], [cd(col(1))], batches=3)
-    assert as_dict(one, 1)[0] == as_dict(three, 1)[0] == ref([k], v)
+    check(one, [k], v)
+    check(three, [k], v)
 
 
 def test_set_growth(ctx, capfd, monkeypatch):
@@ -213,8 +184,7 @@ def test_set_growth(ctx, capfd, monkeypatch):
     got = gpu(ctx, [k, v], [col(0)], [cd(col(1))], batches=5)
     err = capfd.readouterr().err
     assert err.count("launch k_set_move") >= 2
-    d = as_dict(got, 1)[0]
-    assert d == {(g,): int(c) for g, c in enumerate(np.bincount(k))}  # every value is distinct
+    check(got, [k], v)  # every value is distinct: each group counts its rows
     monkeypatch.delenv("DFGPU_TRACE")
     whole = gpu(ctx, [v], [], [cd(col(0))])  # one big first batch: the prefix sizes the set
     assert int(whole[0][0]) == n
@@ -236,7 +206,7 @@ def test_front_and_line_tables(ctx, ngroups):
     for a in (1, 2, 4):
         assert np.array_equal(got[a][o], base[a][ob])
     np.testing.assert_allclose(got[3][o], base[3][ob], rtol=1e-9)
-    assert as_dict([got[0], got[5]], 1)[0] == ref([k], v)
+    check([got[0], got[5]], [k], v)
 
 
 def test_where_and_expression_argument(ctx):
@@ -246,9 +216,9 @@ def test_where_and_expression_argument(ctx):
     a = rng.integers(0, 40, n).astype(np.int64)
     b = rng.integers(0, 40, n).astype(np.int64)
     got = gpu(ctx, [k, a, b], [col(0)], [cd(col(1) + col(2))], pred=col(1) > 10)
-    assert as_dict(got, 1)[0] == ref([k], a + b, where=a > 10)
+    check(got, [k], a + b, where=a > 10)
     whole = gpu(ctx, [k, a, b], [], [cd(col(1) + col(2))], pred=col(1) > 10)
-    assert int(whole[0][0]) == len(np.unique((a + b)[a > 10]))
+    check(whole, [], a + b, where=a > 10)
 
 
 def test_several_distinct_and_mixed(ctx):
@@ -266,9 +236,8 @@ def test_several_distinct_and_mixed(ctx):
     o, ob = np.lexsort((got[1], got[0])), np.lexsort((base[1], base[0]))
     for i, j in ((2, 2), (4, 3), (7, 4)):
         assert np.array_equal(got[i][o], base[j][ob])
-    d = as_dict(got, 2)
-    assert d[1] == d[4] == ref([k1, k2], a)
-    assert d[3] == ref([k1, k2], b)
+    G.assert_matches(got, G.aggregate([k1, k2], [(G.SUM, a), (G.COUNT_DISTINCT, a), (G.MAX, b), (G.COUNT_DISTINCT, b),
+                                                  (G.COUNT_DISTINCT, a), (G.COUNT, a)]))
 
 
 def test_update_host_chunks(ctx):
@@ -281,8 +250,9 @@ def test_update_host_chunks(ctx):
     chunked = r.columns()
     r.free()
     resident = gpu(ctx, [k, v], [col(0)], aggs)
-    assert as_dict(chunked, 1) == as_dict(resident, 1)
-    assert as_dict(chunked, 1)[1] == ref([k], v)
+    exp = G.aggregate([k], [(G.SUM, v), (G.COUNT_DISTINCT, v)])
+    G.assert_matches(chunked, exp, "chunked")
+    G.assert_matches(resident, exp, "resident")
 
 
 def test_not_implemented_shapes(ctx):
@@ -319,8 +289,8 @@ def test_sql(ctx):
         k = rng.integers(0, 50, 100_000).astype(np.int64)
         v = rng.integers(0, 20, 100_000).astype(np.int32)
         hctx.register_memory("t", [("k", k), ("v", v)], batch_size=30_000)
-        got = rows(hctx.sql("SELECT k, COUNT(DISTINCT v) FROM t WHERE v > 3 GROUP BY k"))
-        assert {(int(a),): int(c) for a, c in got} == ref([k], v, where=v > 3)
+        rel = hctx.sql("SELECT k, COUNT(DISTINCT v) FROM t WHERE v > 3 GROUP BY k")
+        check([np.concatenate(c) for c in zip(*rel.collect())], [k], v, where=v > 3)
         hctx.register_memory("u", [("k", k), ("v", v)], batch_size=30_000)
         got = rows(hctx.sql("SELECT COUNT(DISTINCT v + v), COUNT(v) FROM u"))
         assert [(int(a), int(b)) for a, b in got] == [(len(np.unique(v + v)), len(v))]

@@ -224,17 +224,9 @@ def test_chunked_host_call(ctx):
 
 
 # ---- aggregates ------------------------------------------------------------------------------------------------------
-FN = {"min": G.MIN, "max": G.MAX, "sum": G.SUM, "count": G.COUNT}
-
-
-def distinct_count(v):
-    v = np.where(v == 0, v.dtype.type(0), v) if v.dtype.kind == "f" else v  # +0.0 and -0.0 are one value
-    return len(np.unique(v))
-
-
 def check_agg(c, batches, T, pred, keys, aggs, msg):
-    """The engine's GROUP BY / reduce against groupby_ref fed with the reference's keys and arguments (AVG and
-    COUNT(DISTINCT) computed here).  Returns whether the call raised."""
+    """The engine's GROUP BY / reduce against groupby_ref fed with the reference's keys and arguments.  Returns whether
+    the call raised."""
     rb = pred is None
     bad, keep = R.raises(T, pred, keys + [a.arg for a in aggs])
     run = lambda: c.aggregate(batches, keys, aggs, 0, pred=pred).columns()  # noqa: E731
@@ -242,56 +234,12 @@ def check_agg(c, batches, T, pred, keys, aggs, msg):
         expect_raise(run, msg)
         return True
     got = traced(run)
-    kv = [R.evaluate(k, T, rb).values[keep] for k in keys]
-    args = []
-    for a in aggs:
-        v = R.evaluate(a.arg, T, rb)
-        args.append((v.values[keep], v.valid[keep]))
-    plain = [i for i, a in enumerate(aggs) if a.name in FN and not a.distinct]
-    nk = len(keys)
-    if not nk and pred is not None and not keep.any():
-        return False  # nothing passed: COUNT's 0 against the reference's null (test_nulls_fuzz_gpu covers that case)
-    if plain:
-        try:
-            G.assert_matches(got[:nk] + [got[nk + i] for i in plain], G.aggregate(kv, [(FN[aggs[i].name], args[i]) for i in plain]))
-        except AssertionError as err:
-            raise AssertionError("%s: %s" % (msg, err)) from None
-    # AVG and COUNT(DISTINCT): per group over the valid values
-    if nk:
-        gk = [unpack(x)[0] for x in got[:nk]]
-        order = np.lexsort(gk[::-1])
-        gk = [x[order] for x in gk]
-        rows_of = {}
-        ids = np.lexsort(kv[::-1])
-        for r in ids:
-            rows_of.setdefault(tuple(x[r].item() for x in kv), []).append(r)
-        groups = [np.array(rows_of[tuple(x[i].item() for x in gk)]) for i in range(len(gk[0]))]
-    else:
-        order = np.arange(1)
-        groups = [np.flatnonzero(np.ones(int(keep.sum()), bool))]
-    for i, a in enumerate(aggs):
-        if i in plain:
-            continue
-        gv, gm = unpack(got[nk + i])
-        gv, gm = gv[order], gm[order]
-        v, valid = args[i]
-        for j, rows in enumerate(groups):
-            sel = rows[valid[rows]] if len(rows) else rows
-            where = "%s: aggregate %d, group %d" % (msg, i, j)
-            if a.distinct:
-                assert gm[j] and gv[j] == distinct_count(v[sel]), "%s: COUNT(DISTINCT) %s, expected %d" % (where, gv[j], distinct_count(v[sel]))
-                continue
-            if len(sel) == 0:
-                assert not gm[j], "%s: AVG over no value is not null" % where
-                continue
-            x = v[sel].astype(np.float64)
-            with np.errstate(all="ignore"):
-                ex = np.sum(x.astype(np.longdouble)) / len(sel)
-            assert gm[j], "%s: AVG is null" % where
-            if np.isfinite(ex) and np.isfinite(np.abs(x).sum()):
-                assert abs(gv[j] - float(ex)) <= 1e-9 * np.abs(x).sum() / len(sel) + 1e-300, "%s: AVG %r, expected %r" % (where, gv[j], ex)
-            else:
-                assert np.isnan(gv[j]) == np.isnan(float(ex)) or not np.isfinite(gv[j]), "%s: AVG %r, expected %r" % (where, gv[j], ex)
+    kv = [R.evaluate(k, T, rb).values for k in keys]
+    args = [(v.values, v.valid) for v in (R.evaluate(a.arg, T, rb) for a in aggs)]
+    try:
+        G.assert_matches(got, G.aggregate(kv, [(G.func_of(a), x) for a, x in zip(aggs, args)], where=keep))
+    except AssertionError as err:
+        raise AssertionError("%s: %s" % (msg, err)) from None
     return False
 
 

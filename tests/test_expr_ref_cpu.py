@@ -18,14 +18,6 @@ from datafusion_archive_b200 import engine
 from datafusion_archive_b200.expr import BinaryExpr, Case, Cast, ScalarFunction, Utf8Function, case, col, fn, lit, utf8_fn
 
 
-def oracle_rows(arrays, pred, exprs):
-    O.set_extensions(filter_all_primitives=True)
-    try:
-        return O.filter_project(arrays, pred, exprs)
-    finally:
-        O.set_extensions(filter_all_primitives=False)
-
-
 def unpack(c):
     if isinstance(c, tuple):
         return np.asarray(c[0]), np.asarray(c[1], dtype=bool)
@@ -62,7 +54,7 @@ def test_reference_matches_the_oracle_on_its_subset(profile):
         pred, proj = F.gen_fp_query(rng, t, with_pred=q % 3 != 0)
         bad, keep = R.raises(T, pred, proj)
         try:
-            exp = oracle_rows(t.arrays, pred, proj)
+            exp = O.rows(t.arrays, pred, proj)
         except O.OracleError as e:
             assert "DivideByZero" in e.msg and bad, (q, pred, proj, e.msg)
             raised += 1

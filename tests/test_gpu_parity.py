@@ -1,9 +1,11 @@
 """GPU parity tests: the sm_90a path through the C ABI vs the CPU oracle on the same seeded inputs
-(bit-exact for integer/index/ordering work and every non-reduced f64, 1e-9 relative for f64 SUM),
-the reference's golden vectors, edge cases, and size-independent properties at BASELINE sizes."""
+(bit-exact for integer/index/ordering work and every non-reduced f64, 1e-9 relative for f64 SUM) or vs the exact
+GROUP BY reference of tests/groupby_ref.py, the reference's golden vectors, edge cases, and size-independent properties
+at BASELINE sizes."""
 import numpy as np
 import pytest
 
+import groupby_ref as G
 import oracle_lib as O
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, workloads
@@ -271,11 +273,7 @@ def test_boolean_input_columns(ctx):
             if n == 0:  # (the oracle's relation yields no batch at all for an empty input)
                 assert all(len(x) == 0 for x in got)
                 continue
-            O.set_extensions(filter_all_primitives=True)  # FilterRelation gathers every input column; the reference's
-            try:                                          # filter() only knows Float64 / Utf8 (filter.rs:82-108)
-                exp = O.filter_project([a, f, g], pred, proj)
-            finally:
-                O.set_extensions(filter_all_primitives=False)
+            exp = O.rows([a, f, g], pred, proj)
             assert len(got) == len(exp)
             for x, y in zip(got, exp):
                 assert np.array_equal(np.asarray(x), np.asarray(y))
@@ -285,15 +283,11 @@ def test_boolean_input_columns(ctx):
     f = rng.random(n) < 0.5
     fa = pa.array(f, mask=rng.random(n) < 0.2)
     na = pa.array(a, mask=rng.random(n) < 0.1)
-    O.set_extensions(filter_all_primitives=True)
-    try:
-        for pred, proj in [(col(1) & (col(0) > lit(0.3)), [col(0), col(1)]), (None, [col(1) | (col(0) < lit(0.5))])]:
-            assert_nullable_equal(gpu_fp(ctx, [na, fa], pred, proj), O.filter_project([na, fa], pred, proj))
-    finally:
-        O.set_extensions(filter_all_primitives=False)
+    for pred, proj in [(col(1) & (col(0) > lit(0.3)), [col(0), col(1)]), (None, [col(1) | (col(0) < lit(0.5))])]:
+        assert_nullable_equal(gpu_fp(ctx, [na, fa], pred, proj), O.rows([na, fa], pred, proj))
     # fused WHERE with a Boolean column under an aggregate
     k = rng.integers(0, 50, n, dtype=np.int64)
-    exp = oracle_filtered_aggregate([k, a, f], col(2) & (col(1) < lit(0.8)), [col(0)], [AggregateFunction("max", col(1)), AggregateFunction("count", col(1))])
+    exp = O.filtered_aggregate([k, a, f], col(2) & (col(1) < lit(0.8)), [col(0)], [AggregateFunction("max", col(1)), AggregateFunction("count", col(1))])
     got = gpu_agg(ctx, [k, a, f], [col(0)], [AggregateFunction("max", col(1)), AggregateFunction("count", col(1))], pred=col(2) & (col(1) < lit(0.8)))
     check_groupby(got, exp, 1, exact_cols={0, 1, 2}, sum_cols=set())
     with pytest.raises(engine.DfGpuError) as ei:  # aggregate.rs:848-850
@@ -330,22 +324,12 @@ def test_all_numeric_dtypes(ctx, np_dt):
     arrays = [x, y]
     pred = (col(0) < col(1)) | (col(0).eq(col(1)))
     proj = [col(0) + col(1), col(0) - col(1), col(0) * col(1), col(0) / col(1), col(0)]
-    O.set_extensions(filter_all_primitives=True)
-    try:
-        exp = O.filter_project(arrays, pred, proj)
-    finally:
-        O.set_extensions(filter_all_primitives=False)
+    exp = O.rows(arrays, pred, proj)
     got = gpu_fp(ctx, arrays, pred, proj)
     assert_cols_bit_equal(got, exp)
     lt = lit(int(x[5]) if np.issubdtype(np_dt, np.integer) else float(x[5]), dt)
     for p in [col(0) >= lt, col(0).not_eq(lt), col(0) > lt, col(0) <= lt]:
-        got = gpu_fp(ctx, arrays, p, [col(1)])
-        O.set_extensions(filter_all_primitives=True)
-        try:
-            exp = O.filter_project(arrays, p, [col(1)])
-        finally:
-            O.set_extensions(filter_all_primitives=False)
-        assert_cols_bit_equal(got, exp)
+        assert_cols_bit_equal(gpu_fp(ctx, arrays, p, [col(1)]), O.rows(arrays, p, [col(1)]))
 
 
 def test_lean_filter_shapes_all_operators(ctx):
@@ -407,13 +391,9 @@ def test_lean_filter_shapes_integer_operands(ctx, np_dt):
         preds += [col(0) < rhs, col(0) <= rhs, col(0) > rhs, col(0) >= rhs, col(0).eq(rhs), col(0).not_eq(rhs)]
     projs = [[col(0)], [col(2), col(1)], [col(0) + col(1), col(0) * col(1)], [col(0) - col(1)], [col(1) * lit(3, dt), col(2) * lit(0.5)],
              [col(0) + lit(7, dt)]]
-    O.set_extensions(filter_all_primitives=True)  # the reference's filter() gathers Float64 / Utf8 only (filter.rs:82-108)
-    try:
-        for i, p in enumerate(preds):
-            pr = projs[i % len(projs)]
-            assert_cols_bit_equal(gpu_fp(ctx, [a, b, f], p, pr), O.filter_project([a, b, f], p, pr))
-    finally:
-        O.set_extensions(filter_all_primitives=False)
+    for i, p in enumerate(preds):
+        pr = projs[i % len(projs)]
+        assert_cols_bit_equal(gpu_fp(ctx, [a, b, f], p, pr), O.rows([a, b, f], p, pr))
 
 
 def test_nan_and_signed_zero_compare(ctx):
@@ -507,15 +487,8 @@ def test_groupby_low_cardinality_front_table(ctx):
         iv = rng.integers(-50, 50, n, dtype=np.int64)
         aggs = [AggregateFunction("sum", col(1)), AggregateFunction("count", col(1)), AggregateFunction("min", col(1)),
                 AggregateFunction("max", col(1)), AggregateFunction("sum", col(2))]
-        got = sort_by_key(gpu_agg(ctx, [k, v, iv], [col(0)], aggs))
-        uk, inv = np.unique(k, return_inverse=True)
-        assert np.array_equal(got[0], uk)
-        np.testing.assert_allclose(got[1], np.bincount(inv, weights=v), rtol=SUM_RTOL)
-        assert np.array_equal(got[2], np.bincount(inv).astype(np.uint64))
-        mn = np.full(len(uk), np.inf); np.minimum.at(mn, inv, v)
-        mx = np.full(len(uk), -np.inf); np.maximum.at(mx, inv, v)
-        assert np.array_equal(got[3], mn) and np.array_equal(got[4], mx)
-        assert np.array_equal(got[5], np.bincount(inv, weights=iv).astype(np.int64))
+        got = gpu_agg(ctx, [k, v, iv], [col(0)], aggs)
+        G.assert_matches(got, G.aggregate([k], [(G.SUM, v), (G.COUNT, v), (G.MIN, v), (G.MAX, v), (G.SUM, iv)]), ngroups)
 
 
 def test_groupby_high_cardinality_layouts(ctx):
@@ -525,30 +498,11 @@ def test_groupby_high_cardinality_layouts(ctx):
     k = workloads.mix_keys(rng.integers(0, 1_500_000, n, dtype=np.int64))
     v = rng.random(n)
     aggs = [AggregateFunction("min", col(1)), AggregateFunction("max", col(1)), AggregateFunction("sum", col(1)), AggregateFunction("count", col(1))]
-    uk, inv = np.unique(k, return_inverse=True)
-    mn = np.full(len(uk), np.inf); np.minimum.at(mn, inv, v)
-    mx = np.full(len(uk), -np.inf); np.maximum.at(mx, inv, v)
+    exp = G.aggregate([k], [(G.MIN, v), (G.MAX, v), (G.SUM, v), (G.COUNT, v)])
     for hint in [2_000_000, 0]:
-        got = sort_by_key(gpu_agg(ctx, [k, v], [col(0)], aggs, expected=hint))
-        assert np.array_equal(got[0], uk) and np.array_equal(got[1], mn) and np.array_equal(got[2], mx)
-        np.testing.assert_allclose(got[3], np.bincount(inv, weights=v), rtol=SUM_RTOL)
-        assert np.array_equal(got[4], np.bincount(inv).astype(np.uint64))
+        G.assert_matches(gpu_agg(ctx, [k, v], [col(0)], aggs, expected=hint), exp, hint)
     # two batches: the second one finds the table already converted
-    got = sort_by_key(gpu_agg(ctx, [k, v], [col(0)], aggs, nbatches=2))
-    assert np.array_equal(got[0], uk) and np.array_equal(got[4], np.bincount(inv).astype(np.uint64))
-
-
-def oracle_filtered_aggregate(arrays, pred, keys, aggs):
-    """The reference's wiring for WHERE + GROUP BY: FilterRelation (gathers every column) feeding
-    AggregateRelation (context.rs:126-139, 162-192)."""
-    # (the reference's filter() gathers Float64 / Utf8 only, filter.rs:82-108; integer columns need the
-    # oracle's all-primitives extension, as everywhere in this file)
-    O.set_extensions(filter_all_primitives=True)
-    try:
-        kept = O.filter_project(arrays, pred, [col(i) for i in range(len(arrays))])
-    finally:
-        O.set_extensions(filter_all_primitives=False)
-    return O.aggregate(kept, keys, aggs)
+    G.assert_matches(gpu_agg(ctx, [k, v], [col(0)], aggs, nbatches=2), exp, "two batches")
 
 
 def test_groupby_fused_where_vs_oracle(ctx):
@@ -563,7 +517,7 @@ def test_groupby_fused_where_vs_oracle(ctx):
              (col(1) * lit(2.0)) < lit(0.5),
              col(1) < lit(-1.0)]  # nothing passes: empty result
     for pred in preds:
-        exp = oracle_filtered_aggregate(arrays, pred, keys, aggs)
+        exp = O.filtered_aggregate(arrays, pred, keys, aggs)
         for nb in [1, 3]:
             got = gpu_agg(ctx, arrays, keys, aggs, nbatches=nb, pred=pred)
             check_groupby(got, exp, 1, exact_cols={0, 1, 2, 4}, sum_cols={3})
@@ -578,7 +532,7 @@ def test_groupby_fused_where_vs_oracle(ctx):
     keys2 = [col(0) + lit(7)]
     aggs2 = [AggregateFunction("sum", col(2) * lit(3.0)), AggregateFunction("max", col(1)), AggregateFunction("count", col(2))]
     pred2 = (col(1) > lit(-20)) & (col(2) < lit(0.75))
-    exp = oracle_filtered_aggregate([k, w, v], pred2, keys2, aggs2)
+    exp = O.filtered_aggregate([k, w, v], pred2, keys2, aggs2)
     got = gpu_agg(ctx, [k, w, v], keys2, aggs2, pred=pred2)
     check_groupby(got, exp, 1, exact_cols={0, 2, 3}, sum_cols={1})
     # Int32 keys / Float32 arguments through the plain kernel's 4-byte loads, odd row count
@@ -586,7 +540,7 @@ def test_groupby_fused_where_vs_oracle(ctx):
     v32 = rng.random(n - 1).astype(np.float32)
     aggs3 = [AggregateFunction("min", col(1)), AggregateFunction("max", col(1)), AggregateFunction("count", col(1))]
     pred3 = col(1) >= lit(0.5, A.FLOAT32)
-    exp = oracle_filtered_aggregate([k32, v32], pred3, [col(0)], aggs3)
+    exp = O.filtered_aggregate([k32, v32], pred3, [col(0)], aggs3)
     got = gpu_agg(ctx, [k32, v32], [col(0)], aggs3, pred=pred3)
     check_groupby(got, exp, 1, exact_cols={0, 1, 2, 3}, sum_cols=set())
 
@@ -599,7 +553,7 @@ def test_no_groupby_fused_where_vs_oracle(ctx):
     aggs = [AggregateFunction("min", col(0)), AggregateFunction("max", col(0)), AggregateFunction("sum", col(0)), AggregateFunction("count", col(0)),
             AggregateFunction("sum", col(1))]
     for pred in [col(0) < lit(0.3), (col(1) >= lit(500)) & (col(0) > lit(0.5))]:
-        exp = oracle_filtered_aggregate([v, w], pred, [], aggs)
+        exp = O.filtered_aggregate([v, w], pred, [], aggs)
         got = gpu_agg(ctx, [v, w], [], aggs, nbatches=2, pred=pred)
         for i, (g, e) in enumerate(zip(got, exp)):
             if i == 2:
@@ -608,7 +562,7 @@ def test_no_groupby_fused_where_vs_oracle(ctx):
                 assert np.array_equal(g, e), i
     # nothing passes: MIN / MAX / SUM are null, exactly as over an empty input
     got = gpu_agg(ctx, [v, w], [], aggs[:3], pred=col(0) < lit(-1.0))
-    exp = oracle_filtered_aggregate([v, w], col(0) < lit(-1.0), [], aggs[:3])
+    exp = O.filtered_aggregate([v, w], col(0) < lit(-1.0), [], aggs[:3])
     for g, e in zip(got, exp):
         assert isinstance(g, tuple) == isinstance(e, tuple)
         if isinstance(g, tuple):
@@ -692,7 +646,7 @@ def test_groupby_wide_composite_keys(ctx):
             check_wide(got, exp, nk, sum_cols={nk + 4})
     # fused WHERE with wide keys
     pred = col(2) < lit(0.5)
-    exp = oracle_filtered_aggregate([k1, k2, v, iv], pred, [col(0), col(1)], aggs(2, 3))
+    exp = O.filtered_aggregate([k1, k2, v, iv], pred, [col(0), col(1)], aggs(2, 3))
     check_wide(gpu_agg(ctx, [k1, k2, v, iv], [col(0), col(1)], aggs(2, 3), pred=pred), exp, 2, sum_cols={6})
 
 
@@ -758,16 +712,8 @@ def test_groupby_two_keys_and_expression_args(ctx):
     got_small = gpu_agg(ctx, [k1[:m], k2[:m], a[:m], b[:m]], [col(0), col(1)], aggs)
     exp_small = O.aggregate([k1[:m], k2[:m], a[:m], b[:m]], [col(0), col(1)], aggs)
     check_groupby(got_small, exp_small, 2, set(), {2})
-    # full size against numpy
-    got = sort_by_key(got, 2)
-    comp = k1.astype(np.int64) * 100000 + k2.astype(np.int64)
-    uk, inv = np.unique(comp, return_inverse=True)
-    assert len(got[0]) == len(uk)
-    np.testing.assert_allclose(got[2], np.bincount(inv, weights=a * b), rtol=SUM_RTOL)
-    mx = np.full(len(uk), -np.inf)
-    np.maximum.at(mx, inv, a + b)
-    assert np.array_equal(got[3], mx)
-    assert np.array_equal(got[4], np.bincount(inv).astype(np.uint64))
+    # full size against the exact reference
+    G.assert_matches(got, G.aggregate([k1, k2], [(G.SUM, a * b), (G.MAX, a + b), (G.COUNT, a)]), "full size")
 
 
 @pytest.mark.parametrize("np_dt", [np.int32, np.int64, np.uint16, np.float32, np.float64])

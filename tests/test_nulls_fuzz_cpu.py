@@ -11,20 +11,6 @@ from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200.expr import AggregateFunction, col, lit
 
 
-def rows(arrays, pred, exprs):
-    O.set_extensions(filter_all_primitives=True)
-    try:
-        return O.filter_project(arrays, pred, exprs)
-    finally:
-        O.set_extensions(filter_all_primitives=False)
-
-
-def filtered_aggregate(arrays, pred, keys, aggs):
-    if pred is None:
-        return O.aggregate(arrays, keys, aggs)
-    return O.aggregate(rows(arrays, pred, [col(i) for i in range(len(arrays))]), keys, aggs)
-
-
 def test_table_invariants():
     rng = np.random.default_rng(1)
     n = 5_000
@@ -99,7 +85,7 @@ def test_generated_queries_run_on_the_oracle():
     depth8 = casts = bool_leaves = 0
     for q in range(120):
         pred, proj = F.gen_fp_query(rng, t, with_pred=q % 2 == 0)
-        rows(t.arrays, pred, proj)
+        O.rows(t.arrays, pred, proj)
         progs = [e.program(t.dtype) for e in proj + ([pred] if pred is not None else [])]
         casts += any(i.op == A.OP_CAST for p in progs for i in p)
         bool_leaves += any(i.op == A.OP_COL and t.dtype[i.col] == A.BOOL for p in progs for i in p)
@@ -112,9 +98,9 @@ def test_surviving_zero_divisor_raises_on_the_oracle():
     t = F.gen_table(rng, 2_000, profiles="nulls", surviving_zero=True, dtypes=[A.INT32])
     gate = col(t.gate) > lit(0, A.INT32)
     e = col(t.values[A.INT32]) / col(t.safe[A.INT32])
-    rows(t.arrays, None, [e])  # null-aware without a predicate: no error
+    O.rows(t.arrays, None, [e])  # null-aware without a predicate: no error
     try:
-        rows(t.arrays, gate, [e])
+        O.rows(t.arrays, gate, [e])
         raise AssertionError("a zero divisor in a surviving row must raise")
     except O.OracleError as err:
         assert "DivideByZero" in err.msg
@@ -124,7 +110,6 @@ def test_oracle_filtered_aggregate_vs_groupby_ref():
     """The oracle's filter-then-aggregate equals groupby_ref over the rows the oracle evaluated, the comparison the GPU
     fuzz makes (without GROUP BY float MIN / MAX are left out: arrow 0.12 returns NaN when a batch starts with NaN)."""
     rng = np.random.default_rng(5)
-    fn = {"min": G.MIN, "max": G.MAX, "sum": G.SUM, "count": G.COUNT}
     for qi in range(12):
         n = 2_000
         t = F.gen_table(rng, n)
@@ -134,11 +119,11 @@ def test_oracle_filtered_aggregate_vs_groupby_ref():
             aggs = [a for a in aggs if not (a.name in ("min", "max") and A.NP_OF.get(a.arg.get_type(t.dtype), np.int8)().dtype.kind == "f")]
             if not aggs:
                 continue
-        got = filtered_aggregate(t.arrays, pred, keys, aggs)
-        r = rows(t.arrays, pred, keys + [a.arg for a in aggs])
+        got = O.filtered_aggregate(t.arrays, pred, keys, aggs)
+        r = O.rows(t.arrays, pred, keys + [a.arg for a in aggs])
         if not keys and pred is not None and len(np.asarray(r[0][0] if isinstance(r[0], tuple) else r[0])) == 0:
             continue  # nothing passed: the oracle's COUNT is null, the engine's 0 (the GPU fuzz compares that case)
-        G.assert_matches(got, G.aggregate(r[:len(keys)], [(fn[a.name], r[len(keys) + i]) for i, a in enumerate(aggs)]), ctx=str(qi))
+        G.assert_matches(got, G.aggregate(r[:len(keys)], [(G.func_of(a), r[len(keys) + i]) for i, a in enumerate(aggs)]), ctx=str(qi))
 
 
 def test_worked_example_on_the_oracle():
@@ -147,9 +132,9 @@ def test_worked_example_on_the_oracle():
     k = np.array([0, 0, 1, 1], dtype=np.int64)
     w = np.array([1.0, 1.0, 1.0, 1.0])
     pred = col(2) > lit(0.0)
-    out = filtered_aggregate([v, k, w], pred, [], [AggregateFunction(f, col(0)) for f in ("min", "max", "sum", "count")])
+    out = O.filtered_aggregate([v, k, w], pred, [], [AggregateFunction(f, col(0)) for f in ("min", "max", "sum", "count")])
     assert [float(np.asarray(c)[0]) for c in out] == [-50.0, 100.0, 54.0, 4.0]
-    out = filtered_aggregate([v, k, w], pred, [col(1)], [AggregateFunction("count", col(0)), AggregateFunction("sum", col(0) * lit(2.0))])
+    out = O.filtered_aggregate([v, k, w], pred, [col(1)], [AggregateFunction("count", col(0)), AggregateFunction("sum", col(0) * lit(2.0))])
     order = np.argsort(out[0])
     assert out[1][order].tolist() == [2, 2] and out[2][order].tolist() == [202.0, -94.0]
     # without the WHERE: no-GROUP-BY reductions skip the nulls

@@ -3,12 +3,9 @@ Boolean columns, with deliberate garbage under every null slot (tests/fuzz_exprs
 (narrow and wide keys), the reduction without GROUP BY, COUNT(DISTINCT) and AVG, with and without a fused WHERE.
 
 A WHERE under an aggregate is compared with filter-then-aggregate, the reference's wiring: FilterRelation copies values
-and drops the bitmaps, so the aggregate sees the surviving rows with no nulls.  Comparisons are exact (any NaN equals any
-NaN: the payload of a NaN produced by arithmetic is not pinned) except float SUM, which is held to the `groupby_ref`
-gamma bound around the exact sum of the rows the oracle evaluated.  Every case runs under DFGPU_TRACE and asserts that the
-NULLS instantiation it is about was launched."""
-import math
-
+and drops the bitmaps, so the aggregate sees the surviving rows with no nulls.  Every aggregate result is checked by
+`groupby_ref` over the rows the oracle evaluated; MIN / MAX / SUM / COUNT are compared with the oracle's own aggregate
+too.  Every case runs under DFGPU_TRACE and asserts that the NULLS instantiation it is about was launched."""
 import numpy as np
 import pyarrow as pa
 import pytest
@@ -78,22 +75,6 @@ def concat(batches):
     return [pa.concat_arrays([arrow(b[i]) for b in batches]) if len(batches) > 1 else batches[0][i] for i in range(len(batches[0]))]
 
 
-def oracle_rows(arrays, pred, exprs):
-    """The oracle's FilterRelation + ProjectRelation: the value of each expression on each surviving row."""
-    O.set_extensions(filter_all_primitives=True)
-    try:
-        return O.filter_project(arrays, pred, exprs)
-    finally:
-        O.set_extensions(filter_all_primitives=False)
-
-
-def oracle_filtered_aggregate(arrays, pred, keys, aggs):
-    """FilterRelation (gathers every column, dropping the bitmaps) feeding AggregateRelation (context.rs:126-139)."""
-    if pred is None:
-        return O.aggregate(arrays, keys, aggs)
-    return O.aggregate(oracle_rows(arrays, pred, [col(i) for i in range(len(arrays))]), keys, aggs)
-
-
 def both(oracle_fn, gpu_fn):
     """(expected, got), or (None, None) when the oracle raises: then the engine must raise the same Arrow error."""
     try:
@@ -147,7 +128,7 @@ def test_fuzz_filter_project_nullable(ctx, launched):
             for q in range(30):
                 with_pred = q % 3 != 0
                 pred, proj = F.gen_fp_query(rng, t, with_pred=with_pred)
-                exp, got = both(lambda: oracle_rows(t.arrays, pred, proj), lambda: gpu_fp(ctx, b, pred, proj))
+                exp, got = both(lambda: O.rows(t.arrays, pred, proj), lambda: gpu_fp(ctx, b, pred, proj))
                 if exp is None:
                     raised += 1
                     continue
@@ -169,9 +150,9 @@ def test_filter_project_zero_divisor_in_surviving_row(ctx):
         gate = col(t.gate) > lit(0, A.INT32)
         b = ctx.upload(t.arrays)
         try:
-            assert_fp_equal(gpu_fp(ctx, b, None, [num / safe]), oracle_rows(t.arrays, None, [num / safe]), d)
-            assert_fp_equal(gpu_fp(ctx, b, gate, [num / gated]), oracle_rows(t.arrays, gate, [num / gated]), d)
-            exp, got = both(lambda: oracle_rows(t.arrays, gate, [num / safe]), lambda: gpu_fp(ctx, b, gate, [num / safe]))
+            assert_fp_equal(gpu_fp(ctx, b, None, [num / safe]), O.rows(t.arrays, None, [num / safe]), d)
+            assert_fp_equal(gpu_fp(ctx, b, gate, [num / gated]), O.rows(t.arrays, gate, [num / gated]), d)
+            exp, got = both(lambda: O.rows(t.arrays, gate, [num / safe]), lambda: gpu_fp(ctx, b, gate, [num / safe]))
             assert exp is None, d
         finally:
             b.free()
@@ -180,21 +161,10 @@ def test_filter_project_zero_divisor_in_surviving_row(ctx):
 # ---------------------------------------------------------------------------------------------------------------
 # aggregates
 # ---------------------------------------------------------------------------------------------------------------
-def expected_groupby_ref(rows, nkeys, aggs, pred):
+def expected(rows, nkeys, aggs):
     """groupby_ref's expectation from the per-row values the oracle evaluated (keys first, then one column per
-    aggregate argument).  Without GROUP BY, a COUNT under a WHERE that passes nothing is 0, not null: the batches
-    were not empty."""
-    fn = {"min": G.MIN, "max": G.MAX, "sum": G.SUM, "count": G.COUNT}
-    exp = G.aggregate(rows[:nkeys], [(fn[a.name], rows[nkeys + i]) for i, a in enumerate(aggs)])
-    if nothing_passed(rows, nkeys, pred):
-        for d in exp.aggs:
-            if d["func"] == G.COUNT:
-                d["null"] = np.zeros(1, dtype=bool)
-    return exp
-
-
-def nothing_passed(rows, nkeys, pred):
-    return nkeys == 0 and pred is not None and len(unpack(rows[0])[0]) == 0
+    aggregate argument)."""
+    return G.aggregate(rows[:nkeys], [(G.func_of(a), rows[nkeys + i]) for i, a in enumerate(aggs)])
 
 
 def sorted_result(cols, nkeys):
@@ -211,17 +181,16 @@ def check_aggregate(arrays, pred, keys, aggs, got_fn, what):
     GROUP BY, float MIN / MAX come from groupby_ref too: arrow 0.12's scan returns NaN when the first value of a batch
     is NaN while the engine skips NaN, a documented deviation (DESIGN §7)."""
     nk = len(keys)
-    exp, got = both(lambda: oracle_filtered_aggregate(arrays, pred, keys, aggs), got_fn)
+    exp, got = both(lambda: O.filtered_aggregate(arrays, pred, keys, aggs), got_fn)
     if exp is None:
         return "raised"
-    rows = oracle_rows(arrays, pred, keys + [a.arg for a in aggs])
-    G.assert_matches(got, expected_groupby_ref(rows, nk, aggs, pred), ctx=str(what))
+    rows = O.rows(arrays, pred, keys + [a.arg for a in aggs])
+    G.assert_matches(got, expected(rows, nk, aggs), ctx=str(what))
     g, e = sorted_result(got, nk), sorted_result(exp, nk)
     assert len(g) == len(e) and len(g[0][0]) == len(e[0][0]), what
     for i, ((gv, gm), (ev, em)) in enumerate(zip(g, e)):
-        if i >= nk and aggs[i - nk].name == "count" and nothing_passed(rows, nk, pred):
-            assert gm[0] and int(gv[0]) == 0, what  # the oracle's COUNT over no surviving row is null
-            continue
+        if i >= nk and aggs[i - nk].name == "count" and not len(unpack(rows[0])[0]):
+            continue  # the oracle's COUNT over no row is null; groupby_ref's 0 was checked above
         assert np.array_equal(gm, em), (what, i, "validity")
         if i >= nk:
             a = aggs[i - nk]
@@ -371,7 +340,7 @@ def test_aggregate_zero_divisor_in_surviving_row(ctx, launched, kernel):
             if kernel == "k_distinct_insert<8,1>":
                 # the oracle has no COUNT(DISTINCT): its filter-then-project raises for the same argument
                 distinct = lambda e: [AggregateFunction("count", e, distinct=True)]  # noqa: E731
-                exp, _ = both(lambda: oracle_rows(t.arrays, gate, [bad]), lambda: gpu_agg(ctx, b, keys, distinct(bad), gate))
+                exp, _ = both(lambda: O.rows(t.arrays, gate, [bad]), lambda: gpu_agg(ctx, b, keys, distinct(bad), gate))
                 assert exp is None, d
                 raised += 1
                 gpu_agg(ctx, b, keys, distinct(good), gate)
@@ -444,47 +413,6 @@ def test_where_over_nulls_worked_example(ctx):
             x.free()
 
 
-# ---------------------------------------------------------------------------------------------------------------
-# AVG and COUNT(DISTINCT): a numpy reference over the rows the oracle evaluated
-# ---------------------------------------------------------------------------------------------------------------
-def ref_avg_distinct(rows, nkeys, funcs):
-    """{key tuple: [value per aggregate]}: AVG = (exact sum / count of the valid values as f64, the error bound of an
-    f64 sum in any order), NaN if a NaN or both infinities are present; COUNT(DISTINCT) = distinct valid values (+0.0
-    equals -0.0, every NaN one value)."""
-    kv = [unpack(c)[0] for c in rows[:nkeys]]
-    n = len(unpack(rows[nkeys])[0])
-    groups = {}
-    for r in range(n):
-        groups.setdefault(tuple(k[r].item() for k in kv), []).append(r)
-    if not nkeys and not groups:
-        groups[()] = []
-    out = {}
-    for key, idx in groups.items():
-        res = []
-        for j, f in enumerate(funcs):
-            v, m = unpack(rows[nkeys + j])
-            x = v[np.array(idx, dtype=np.int64)][m[np.array(idx, dtype=np.int64)]]
-            if f == "distinct":
-                if np.issubdtype(x.dtype, np.floating):
-                    x = np.where(x == 0, 0.0, x.astype(np.float64))
-                    res.append(len(np.unique(x[~np.isnan(x)])) + int(np.isnan(x).any()))
-                else:
-                    res.append(len(np.unique(x)))
-            else:
-                f64 = x.astype(np.float64)
-                if len(f64) == 0:
-                    res.append(None)
-                elif np.isnan(f64).any() or (np.isposinf(f64).any() and np.isneginf(f64).any()):
-                    res.append(math.nan)
-                elif np.isinf(f64).any():
-                    res.append(float(f64[np.isinf(f64)][0]))
-                else:
-                    bound = len(f64) * 2.0 ** -52 * math.fsum(np.abs(f64).tolist()) / len(f64)
-                    res.append((math.fsum(f64.tolist()) / len(f64), bound))
-        out[key] = res
-    return out
-
-
 def test_avg_count_distinct_nullable(ctx, launched):
     """AVG and COUNT(DISTINCT) with and without GROUP BY and WHERE: without a WHERE the nulls are skipped, under one
     every surviving row counts, its value being the one under the null."""
@@ -513,23 +441,7 @@ def test_avg_count_distinct_nullable(ctx, launched):
             for x in b:
                 x.free()
         seen |= launched()
-        rows = oracle_rows(t.arrays, pred, keys + args)
-        exp = ref_avg_distinct(rows, len(keys), funcs)
-        gcols = [unpack(c) for c in got]
-        assert len(gcols[0][0]) == len(exp), qi
-        for r in range(len(gcols[0][0])):
-            key = tuple(gcols[k][0][r].item() for k in range(len(keys)))
-            for j, f in enumerate(funcs):
-                gv, gm = gcols[len(keys) + j]
-                e = exp[key][j]
-                if f == "distinct":
-                    assert gm[r] and int(gv[r]) == e, (qi, key, j)
-                elif e is None:
-                    assert not gm[r], (qi, key, j)
-                elif isinstance(e, float):
-                    assert gm[r] and (gv[r] == e or (math.isnan(e) and math.isnan(gv[r]))), (qi, key, j, gv[r], e)
-                else:
-                    assert gm[r] and abs(gv[r] - e[0]) <= e[1] + 1e-12 * abs(e[0]), (qi, key, j, gv[r], e)
+        G.assert_matches(got, expected(O.rows(t.arrays, pred, keys + args), len(keys), aggs), ctx=str(qi))
     assert "k_distinct_insert<8,1>" in seen, sorted(seen)
 
 
