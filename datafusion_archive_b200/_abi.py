@@ -60,6 +60,8 @@ UTF8_FN_CODES = {
 }
 
 AGG_MIN, AGG_MAX, AGG_SUM, AGG_COUNT, AGG_COUNT_DISTINCT, AGG_AVG = 1, 2, 3, 4, 5, 6
+# dfgpu_window's rank functions (the aggregates above are its other functions)
+WIN_ROW_NUMBER, WIN_RANK, WIN_DENSE_RANK = 16, 17, 18
 
 # dfgpu_join_semi kinds
 JOIN_SEMI, JOIN_ANTI, JOIN_ANTI_NULL_AWARE = 1, 2, 3

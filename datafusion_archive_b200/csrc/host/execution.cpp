@@ -681,6 +681,94 @@ std::optional<RecordBatch> GpuHashJoinRelation::next() {
   return out;
 }
 
+GpuWindowRelation::GpuWindowRelation(dfgpu_ctx* gpu, SchemaRef schema, RelationRef input, std::vector<size_t> cols, bool projected,
+                                     std::vector<ExprRef> window_expr)
+    : gpu_(gpu), schema_(std::move(schema)), input_(std::move(input)), cols_(std::move(cols)), projected_(projected), window_expr_(std::move(window_expr)) {}
+
+std::optional<RecordBatch> GpuWindowRelation::next() {
+  if (done_) return std::nullopt;
+  done_ = true;
+  std::vector<RecordBatch> batches;
+  while (auto b = input_->next()) batches.push_back(std::move(*b));
+  const size_t nin = schema_->fields.size() - window_expr_.size();
+  RecordBatch whole;  // the window's input: the columns in cols_, concatenated; placeholders elsewhere
+  whole.schema = schema_;
+  for (auto& b : batches) whole.num_rows += b.num_rows;
+  for (size_t c = 0; c < nin; c++) {
+    auto a = std::make_shared<Array>();
+    a->data_type = schema_->fields[c].data_type;
+    a->len = whole.num_rows;
+    whole.columns.push_back(a);
+  }
+  for (size_t k = 0; k < cols_.size(); k++)
+    whole.columns[cols_[k]] = concat_column(batches, projected_ ? k : cols_[k], schema_->fields[cols_[k]].data_type);
+  batches.clear();
+  int64_t world = 1;
+  dfgpu_comm_world(gpu_, &world);
+  if (whole.num_rows == 0 && world == 1) return std::nullopt;
+  // the columns every call reads, uploaded once
+  std::vector<ExprRef> all;
+  for (auto& w : window_expr_) all.push_back(w);
+  Pruned pr = prune(all, nin, false);
+  if (pr.cols.empty()) {  // only ranks over no key: any column carries the row count
+    pr.remap[cols_[0]] = 0;
+    pr.cols.push_back(cols_[0]);
+  }
+  const Schema& in_schema = *schema_;
+  BatchGuard b;
+  b.b = upload(gpu_, whole, pr);
+  std::vector<ArrayRef> out(window_expr_.size());
+  std::vector<bool> done(window_expr_.size(), false);
+  for (size_t i = 0; i < window_expr_.size(); i++) {
+    if (done[i]) continue;
+    // every call of this OVER specification
+    const Expr& w = *window_expr_[i];
+    auto spec = [](const Expr& e) {
+      std::string s;
+      for (auto& p : e.partition_by) s += p->debug() + ",";
+      s += "|";
+      for (auto& o : e.order_by) s += o->debug() + ",";
+      return s;
+    };
+    std::vector<size_t> calls;
+    for (size_t j = i; j < window_expr_.size(); j++)
+      if (!done[j] && spec(*window_expr_[j]) == spec(w)) calls.push_back(j);
+    std::vector<ExprRef> okeys;
+    std::vector<int32_t> desc;
+    for (auto& o : w.order_by) {
+      okeys.push_back(o->left);
+      desc.push_back(o->asc ? 0 : 1);
+    }
+    const Programs part(w.partition_by, in_schema, pr), order(okeys, in_schema, pr);
+    std::vector<std::vector<dfgpu_insn>> args(calls.size());
+    std::vector<dfgpu_agg> fns(calls.size());
+    for (size_t k = 0; k < calls.size(); k++) {
+      const Expr& e = *window_expr_[calls[k]];
+      std::string n = e.name;
+      for (auto& c : n) c = char(tolower((unsigned char)c));
+      int f = n == "row_number" ? DFGPU_WIN_ROW_NUMBER : n == "rank" ? DFGPU_WIN_RANK : n == "dense_rank" ? DFGPU_WIN_DENSE_RANK : 0;
+      if (!f) f = n == "min" ? DFGPU_AGG_MIN : n == "max" ? DFGPU_AGG_MAX : n == "sum" ? DFGPU_AGG_SUM : n == "count" ? DFGPU_AGG_COUNT : DFGPU_AGG_AVG;
+      if (!e.args.empty()) lower(*e.args[0], in_schema, pr.remap, args[k]);
+      memset(&fns[k], 0, sizeof(dfgpu_agg));
+      fns[k].func = f;
+      fns[k].arg = args[k].empty() ? nullptr : args[k].data();
+      fns[k].arg_len = int(args[k].size());
+      fns[k].out_dtype = e.data_type;
+    }
+    ResultGuard r;
+    GPU_CHECK(dfgpu_window(gpu_, b.b, part.ptr.data(), part.len.data(), int(part.ptr.size()), order.ptr.data(), order.len.data(), desc.data(),
+                           int(order.ptr.size()), fns.data(), int(fns.size()), &r.r));
+    RecordBatch got = download(r.r, nullptr);
+    for (size_t k = 0; k < calls.size(); k++) {
+      out[calls[k]] = got.columns[k];
+      done[calls[k]] = true;
+    }
+  }
+  if (whole.num_rows == 0) return std::nullopt;  // this rank had no rows: it joined the exchange only
+  for (auto& a : out) whole.columns.push_back(a);
+  return whole;
+}
+
 const std::vector<RecordBatch>& SharedScan::batches() {
   if (!drained_) {
     while (auto b = ds_->next()) batches_.push_back(std::move(*b));
@@ -1027,6 +1115,32 @@ RelationRef ExecutionContext::execute_node(const PlanRef& plan, const std::set<s
       for (auto& e : plan->expr)  // projection.rs:52-57: (name, type, nullable = true)
         schema->fields.push_back(Field{runtime_expr_name(*e, in_schema), e->get_type(in_schema), true});
       return std::make_shared<GpuFilterProjectRelation>(gpu_, input_rel, pred, plan->expr, schema);
+    }
+    case LogicalPlan::Window: {
+      // the window sees exactly what `SELECT <the columns it and the plan above read> FROM .. WHERE ..` returns: a
+      // Selection under it runs as a filter / project of those columns
+      ExprRef pred;
+      PlanRef src = plan->input;
+      if (src->kind == LogicalPlan::Selection) {
+        pred = src->expr[0];
+        src = src->input;
+      }
+      const size_t nin = src->schema()->fields.size();
+      std::set<size_t> cols;
+      for (size_t c = 0; c < nin; c++)
+        if (!needed || needed->count(c)) cols.insert(c);
+      for (auto& w : plan->window_expr) collect_columns(*w, cols);
+      if (cols.empty() && nin > 0) cols.insert(0);  // the row count
+      std::set<size_t> used = cols;
+      if (pred) collect_columns(*pred, used);
+      RelationRef input_rel = execute_node(src, &used, shard);
+      std::vector<size_t> colv(cols.begin(), cols.end());
+      if (pred) {
+        auto schema = std::make_shared<Schema>();
+        for (size_t c : colv) schema->fields.push_back(src->schema()->fields[c]);
+        input_rel = std::make_shared<GpuFilterProjectRelation>(gpu_, input_rel, pred, column_exprs(colv), schema);
+      }
+      return std::make_shared<GpuWindowRelation>(gpu_, plan->schema(), input_rel, colv, pred != nullptr, plan->window_expr);
     }
     default:
       fail(DFGPU_ERR_NOT_IMPLEMENTED, "Limit / Sort / EmptyRelation plans are not executable (reference: unimplemented!() at context.rs:194)");

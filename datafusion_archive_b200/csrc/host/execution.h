@@ -148,6 +148,27 @@ class GpuAggregateRelation : public Relation {
   bool end_of_results_ = false;
 };
 
+// Window (LogicalPlan::Window; the reference has no window functions).  On the first next() it drains its input and
+// concatenates the batches on the host, uploads the columns the window calls read once and calls dfgpu_window once per
+// distinct OVER specification; it returns one batch: the input columns in `cols` (the input's batches hold exactly those,
+// in that order, when `projected`; else they hold every input column), every other input column as an empty placeholder,
+// then one column per window call.  With a communicator attached every rank calls dfgpu_window, a rank without rows with
+// an empty batch, and gets its own rows back.
+class GpuWindowRelation : public Relation {
+ public:
+  GpuWindowRelation(dfgpu_ctx* gpu, SchemaRef schema, RelationRef input, std::vector<size_t> cols, bool projected, std::vector<ExprRef> window_expr);
+  std::optional<RecordBatch> next() override;
+  const SchemaRef& schema() const override { return schema_; }
+ private:
+  dfgpu_ctx* gpu_;
+  SchemaRef schema_;
+  RelationRef input_;
+  std::vector<size_t> cols_;
+  bool projected_;
+  std::vector<ExprRef> window_expr_;
+  bool done_ = false;
+};
+
 // Inner equi-join (LogicalPlan::Join; the reference has no join relation).  On the first next() it drains the build
 // (right) relation, concatenates its batches on the host and builds the GPU hash table (dfgpu_join_build); then each
 // batch of the probe (left) relation gives one output batch (dfgpu_join_probe).  `left_keys` are over the left schema,

@@ -148,6 +148,10 @@ ExprRef Expr::scalar_fn(const std::string& name, std::vector<ExprRef> args, Data
 }
 ExprRef Expr::sort(ExprRef x, bool asc) { auto e = std::make_shared<Expr>(); e->kind = Sort; e->left = std::move(x); e->asc = asc; return e; }
 ExprRef Expr::case_when(std::vector<ExprRef> args) { auto e = std::make_shared<Expr>(); e->kind = Case; e->args = std::move(args); return e; }
+ExprRef Expr::window(const std::string& name, std::vector<ExprRef> args, std::vector<ExprRef> partition_by, std::vector<ExprRef> order_by, DataType rt) {
+  auto e = std::make_shared<Expr>(); e->kind = WindowFunction; e->name = name; e->args = std::move(args); e->partition_by = std::move(partition_by);
+  e->order_by = std::move(order_by); e->data_type = rt; return e;
+}
 ExprRef Expr::is_null(ExprRef x, bool negated) {
   auto e = std::make_shared<Expr>(); e->kind = negated ? IsNotNull : IsNull; e->left = std::move(x); return e;
 }
@@ -160,7 +164,7 @@ DataType Expr::get_type(const Schema& schema) const {
     case Literal:
       if (value.dtype == 0) fail(DFGPU_ERR_NOT_IMPLEMENTED, "ScalarValue::Null has no data type (reference: unimplemented!())");
       return value.get_datatype();
-    case Cast: case ScalarFunction: case AggregateFunction: return data_type;
+    case Cast: case ScalarFunction: case AggregateFunction: case WindowFunction: return data_type;
     case IsNull: case IsNotNull: return DFGPU_BOOL;
     case Sort: return left->get_type(schema);
     case Case: return args[1]->get_type(schema);
@@ -216,12 +220,17 @@ std::string Expr::debug() const {
       if (args.size() % 2) s += " ELSE " + args.back()->debug();
       return s + " END";
     }
-    case ScalarFunction: case AggregateFunction: {
+    case ScalarFunction: case AggregateFunction: case WindowFunction: {
       std::string s = name + (distinct ? "(DISTINCT " : "(");
       for (size_t i = 0; i < args.size(); i++) {
         if (i) s += ", ";
         s += args[i]->debug();
       }
+      s += ")";
+      if (kind != WindowFunction) return s;
+      s += " OVER (";
+      for (size_t i = 0; i < partition_by.size(); i++) s += (i ? ", " : "PARTITION BY ") + partition_by[i]->debug();
+      for (size_t i = 0; i < order_by.size(); i++) s += (i ? ", " : partition_by.empty() ? "ORDER BY " : " ORDER BY ") + order_by[i]->debug();
       return s + ")";
     }
   }
@@ -236,8 +245,21 @@ void collect_columns(const Expr& e, std::set<size_t>& acc) {
     case Expr::ScalarFunction: case Expr::AggregateFunction: case Expr::Case:
       for (auto& a : e.args) collect_columns(*a, acc);
       break;
+    case Expr::WindowFunction:
+      for (auto& a : e.args) collect_columns(*a, acc);
+      for (auto& a : e.partition_by) collect_columns(*a, acc);
+      for (auto& a : e.order_by) collect_columns(*a, acc);
+      break;
     default: break;
   }
+}
+
+bool contains_window(const Expr& e) {
+  if (e.kind == Expr::WindowFunction) return true;
+  if ((e.left && contains_window(*e.left)) || (e.right && contains_window(*e.right))) return true;
+  for (auto& a : e.args)
+    if (contains_window(*a)) return true;
+  return false;
 }
 
 ExprRef shift_columns(const ExprRef& e, size_t by) {
@@ -246,6 +268,8 @@ ExprRef shift_columns(const ExprRef& e, size_t by) {
   if (c->left) c->left = shift_columns(c->left, by);
   if (c->right) c->right = shift_columns(c->right, by);
   for (auto& a : c->args) a = shift_columns(a, by);
+  for (auto& a : c->partition_by) a = shift_columns(a, by);
+  for (auto& a : c->order_by) a = shift_columns(a, by);
   return c;
 }
 
@@ -299,6 +323,10 @@ static void fmt_with_indent(const LogicalPlan& p, std::string& f, int indent) {
       break;
     case LogicalPlan::Limit:
       f += "Limit: " + std::to_string(p.limit);
+      fmt_with_indent(*p.input, f, indent + 1);
+      break;
+    case LogicalPlan::Window:
+      f += "Window: windowExpr=[[" + exprs_debug(p.window_expr) + "]]";
       fmt_with_indent(*p.input, f, indent + 1);
       break;
     case LogicalPlan::Join:

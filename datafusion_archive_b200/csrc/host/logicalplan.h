@@ -61,7 +61,9 @@ struct Expr;
 using ExprRef = std::shared_ptr<const Expr>;
 struct Expr {
   // Case: args = c1 v1 .. cn vn [e], every v and e of one type (the planner casts them), as DFGPU_OP_CASE takes them
-  enum Kind { Column, Literal, BinaryExpr, IsNotNull, IsNull, Cast, Sort, ScalarFunction, AggregateFunction, Case } kind = Column;
+  // WindowFunction: name(args) OVER (PARTITION BY partition_by ORDER BY order_by), order_by being Sort exprs; data_type is
+  // the result type
+  enum Kind { Column, Literal, BinaryExpr, IsNotNull, IsNull, Cast, Sort, ScalarFunction, AggregateFunction, Case, WindowFunction } kind = Column;
   size_t index = 0;         // Column
   ScalarValue value;        // Literal
   ExprRef left, right;      // BinaryExpr; `left` is also the operand of IsNull/IsNotNull/Cast/Sort
@@ -71,6 +73,7 @@ struct Expr {
   std::string name;         // functions
   std::vector<ExprRef> args;
   bool distinct = false;    // AggregateFunction: COUNT(DISTINCT ..)
+  std::vector<ExprRef> partition_by, order_by;  // WindowFunction
 
   static ExprRef column(size_t i);
   static ExprRef literal(const ScalarValue& v);
@@ -81,6 +84,8 @@ struct Expr {
   static ExprRef sort(ExprRef e, bool asc);
   static ExprRef is_null(ExprRef e, bool negated);
   static ExprRef case_when(std::vector<ExprRef> args);
+  static ExprRef window(const std::string& name, std::vector<ExprRef> args, std::vector<ExprRef> partition_by, std::vector<ExprRef> order_by,
+                        DataType rt);
 
   DataType get_type(const Schema& schema) const;             // logicalplan.rs:170-198
   ExprRef cast_to(DataType t, const Schema& schema) const;   // logicalplan.rs:200-215
@@ -98,12 +103,15 @@ struct LogicalPlan {
   // or that have none under NOT IN's three-valued logic (AntiNullAware, one key); its schema is `input`'s, and `right`
   // is a Projection whose columns are the build keys.  The right keys of on_keys are numbered over the left fields
   // followed by `right`'s, as for an inner join.
-  enum Kind { Limit, Projection, Selection, Aggregate, Sort, TableScan, EmptyRelation, Join } kind = EmptyRelation;
+  // Window (no reference counterpart): the rows of `input` with one more column per window_expr (Expr::WindowFunction over
+  // `input`'s schema); its schema is input's fields followed by one field per window call, named by the function.
+  enum Kind { Limit, Projection, Selection, Aggregate, Sort, TableScan, EmptyRelation, Join, Window } kind = EmptyRelation;
   enum class JoinKind { Inner, Semi, Anti, AntiNullAware } join_kind = JoinKind::Inner;  // Join
   size_t limit = 0;
   std::vector<ExprRef> expr;        // Projection / Sort exprs; Selection: expr[0]
   std::vector<ExprRef> group_expr;  // Aggregate
   std::vector<ExprRef> aggr_expr;   // Aggregate
+  std::vector<ExprRef> window_expr;  // Window
   PlanRef input;
   PlanRef right;                                    // Join
   std::vector<std::pair<ExprRef, ExprRef>> on_keys;  // Join
@@ -118,6 +126,9 @@ struct LogicalPlan {
 
 // The column indices an expression reads (collect_expr, sqlplanner.rs:435-458), added to `acc`.
 void collect_columns(const Expr& e, std::set<size_t>& acc);
+
+// Whether an expression holds a window function call
+bool contains_window(const Expr& e);
 
 // The same expression with every column index lowered by `by` (a key over a joined schema -> over its right input).
 ExprRef shift_columns(const ExprRef& e, size_t by);

@@ -227,6 +227,8 @@ struct Parser {
             do { n->args.push_back(parse_expr()); } while (accept_sym(","));
             expect_sym(")");
           }
+          if (is_kw("OVER") && toks[pos + 1].kind == Token::Sym && toks[pos + 1].text == "(") parse_window(*n);
+          else if (is_kw("OVER") && toks[pos + 1].kind == Token::Ident) perr("named windows are not supported: write OVER (..)");
           return n;
         }
         n->kind = ASTNode::SQLIdentifier;
@@ -299,6 +301,29 @@ struct Parser {
     else perr("No infix parser for token " + s);
     n->right = parse_expr(precedence);
     return n;
+  }
+
+  // OVER ( [PARTITION BY e, ..] [ORDER BY e [ASC|DESC], ..] ) after a function call
+  void parse_window(ASTNode& f) {
+    expect_kw("OVER");
+    expect_sym("(");
+    f.over = true;
+    if (is_kw("PARTITION") && toks[pos + 1].kind == Token::Ident && upper(toks[pos + 1].text) == "BY") {
+      pos += 2;
+      do { f.partition_by.push_back(parse_expr()); } while (accept_sym(","));
+    }
+    if (accept_kw("ORDER")) {
+      expect_kw("BY");
+      do {
+        OrderByExpr o;
+        o.expr = parse_expr();
+        if (accept_kw("DESC")) o.asc = false;
+        else accept_kw("ASC");
+        f.window_order.push_back(o);
+      } while (accept_sym(","));
+    }
+    if (is_kw("ROWS") || is_kw("RANGE") || is_kw("GROUPS")) fail(DFGPU_ERR_NOT_IMPLEMENTED, "window frame clauses are not supported");
+    expect_sym(")");
   }
 
   // tokens i, i + 1 are `(` SELECT
@@ -382,7 +407,7 @@ std::string ASTNode::debug() const {
     case SQLCast: return "SQLCast { .. }";
     case SQLIsNull: return "SQLIsNull(..)";
     case SQLIsNotNull: return "SQLIsNotNull(..)";
-    case SQLFunction: return "SQLFunction { id: \"" + id + "\", .. }";
+    case SQLFunction: return "SQLFunction { id: \"" + id + "\"" + (over ? ", over: Some(..)" : "") + ", .. }";
     case SQLSelect: return "SQLSelect { .. }";
     case SQLInSubquery: return negated ? "SQLInSubquery { negated: true, .. }" : "SQLInSubquery { .. }";
     case SQLExists: return negated ? "SQLExists { negated: true, .. }" : "SQLExists { .. }";

@@ -8,6 +8,9 @@
 //   column    := name | qualifier '.' name        -- qualifier = the alias if given, else the table name
 // and WHERE takes subqueries (planned as semi / anti joins, only as top-level AND terms):
 //   expr [NOT] IN ( select )  |  [NOT] EXISTS ( select )
+// and a function call takes a window (no reserved word is added: OVER is read only right after a call's closing
+// parenthesis when `(` follows, PARTITION BY only inside that parenthesis):
+//   name ( args ) OVER ( [PARTITION BY expr, ..] [ORDER BY expr [ASC|DESC], ..] )
 #pragma once
 #include <memory>
 #include <string>
@@ -37,6 +40,10 @@ struct ASTNode {
   SQLType sql_type = SQLType::Other;
   std::vector<ASTRef> args;
   bool distinct = false;  // SQLFunction: COUNT(DISTINCT expr)
+  // SQLFunction with a window: f(..) OVER (PARTITION BY `partition_by` ORDER BY `window_order`)
+  bool over = false;
+  std::vector<ASTRef> partition_by;
+  std::vector<OrderByExpr> window_order;
   // SQLInSubquery: `left` [NOT] IN (`subquery`); SQLExists: [NOT] EXISTS (`subquery`)
   ASTRef subquery;
   bool negated = false;

@@ -32,7 +32,7 @@ Field expr_to_field(const Expr& e, const Schema& input_schema) {
       if (e.index >= input_schema.fields.size()) fail(DFGPU_ERR_INVALID_COLUMN, "column index out of range");
       return input_schema.fields[e.index];
     case Expr::Literal: return Field{"lit", e.value.get_datatype(), true};
-    case Expr::ScalarFunction: case Expr::AggregateFunction: return Field{e.name, e.data_type, true};
+    case Expr::ScalarFunction: case Expr::AggregateFunction: case Expr::WindowFunction: return Field{e.name, e.data_type, true};
     case Expr::Cast: return Field{"cast", e.data_type, true};
     case Expr::Case: return Field{"case", e.get_type(input_schema), true};
     case Expr::BinaryExpr: {
@@ -51,9 +51,15 @@ std::vector<Field> exprlist_to_fields(const std::vector<ExprRef>& expr, const Sc
   return out;
 }
 
+namespace {
+void refuse_windows(const ASTNode& select);
+ExprRef over_window(const ExprRef& e, size_t ninput, std::vector<ExprRef>& calls);
+}  // namespace
+
 PlanRef SqlToRel::sql_to_rel(const ASTRef& sql) const {
   switch (sql->kind) {
     case ASTNode::SQLSelect: {
+      refuse_windows(*sql);
       // parse the input relation so we have access to the row type
       PlanRef input;
       ExprRef residual;  // the ON terms of the joins that are not keys
@@ -86,6 +92,9 @@ PlanRef SqlToRel::sql_to_rel(const ASTRef& sql) const {
       std::vector<ExprRef> aggr_expr;
       for (auto& e : expr)
         if (e->kind == Expr::AggregateFunction) aggr_expr.push_back(e);
+      const bool windowed = std::any_of(expr.begin(), expr.end(), [](const ExprRef& e) { return contains_window(*e); });
+      if (windowed && (!aggr_expr.empty() || sql->has_group_by))
+        fail(DFGPU_ERR_NOT_IMPLEMENTED, "window functions are not supported in an aggregate query");
 
       if (!aggr_expr.empty()) {
         PlanRef aggregate_input = selection_plan ? selection_plan : input;
@@ -107,8 +116,19 @@ PlanRef SqlToRel::sql_to_rel(const ASTRef& sql) const {
       }
 
       PlanRef projection_input = selection_plan ? selection_plan : input;
+      const Schema* projection_input_schema = input_schema.get();
+      if (windowed) {  // Projection <- Window <- [Selection] <- input: each window call becomes a column of the Window
+        auto w = std::make_shared<LogicalPlan>();
+        w->kind = LogicalPlan::Window;
+        w->input = projection_input;
+        for (auto& e : expr) e = over_window(e, input_schema->fields.size(), w->window_expr);
+        w->schema_ = std::make_shared<Schema>(*input_schema);
+        for (auto& x : w->window_expr) w->schema_->fields.push_back(expr_to_field(*x, *input_schema));
+        projection_input = w;
+        projection_input_schema = w->schema_.get();
+      }
       auto projection_schema = std::make_shared<Schema>();
-      projection_schema->fields = exprlist_to_fields(expr, *input_schema);
+      projection_schema->fields = exprlist_to_fields(expr, *projection_input_schema);
       auto proj = std::make_shared<LogicalPlan>();
       proj->kind = LogicalPlan::Projection;
       proj->expr = expr;
@@ -189,6 +209,55 @@ void and_terms(const ExprRef& e, std::vector<ExprRef>& out) {
   } else {
     out.push_back(e);
   }
+}
+// Whether an AST holds a window call, subqueries included
+bool ast_has_window(const ASTRef& e) {
+  if (!e) return false;
+  if (e->kind == ASTNode::SQLFunction && e->over) return true;
+  for (auto* v : {&e->args, &e->partition_by, &e->projection, &e->group_by})
+    for (auto& a : *v)
+      if (ast_has_window(a)) return true;
+  for (auto& o : e->window_order)
+    if (ast_has_window(o.expr)) return true;
+  for (auto& o : e->order_by)
+    if (ast_has_window(o.expr)) return true;
+  for (auto& j : e->joins)
+    if (ast_has_window(j.on)) return true;
+  return ast_has_window(e->left) || ast_has_window(e->right) || ast_has_window(e->subquery) || ast_has_window(e->selection) ||
+         ast_has_window(e->having);
+}
+// A window call is allowed in the SELECT list of a non-aggregate query only
+void refuse_windows(const ASTNode& select) {
+  auto refuse = [](const char* where) { fail(DFGPU_ERR_GENERAL, std::string("window functions are not allowed in ") + where); };
+  for (auto& j : select.joins)
+    if (ast_has_window(j.on)) refuse("ON");
+  if (select.selection) {
+    std::vector<ASTRef> terms;
+    ast_and_terms(select.selection, terms);
+    for (auto& t : terms)
+      if (is_subquery_term(*t) && ast_has_window(t->subquery)) refuse("an IN / EXISTS subquery");
+    if (ast_has_window(select.selection)) refuse("WHERE");
+  }
+  for (auto& g : select.group_by)
+    if (ast_has_window(g)) refuse("GROUP BY");
+  if (ast_has_window(select.having)) refuse("HAVING");
+}
+// `e` over the Window's output: each window call becomes the column of the equal call (equal plan text) in `calls`,
+// appended when there is none
+ExprRef over_window(const ExprRef& e, size_t ninput, std::vector<ExprRef>& calls) {
+  if (e->kind == Expr::WindowFunction) {
+    const std::string d = e->debug();
+    size_t i = 0;
+    while (i < calls.size() && calls[i]->debug() != d) i++;
+    if (i == calls.size()) calls.push_back(e);
+    return Expr::column(ninput + i);
+  }
+  if (!contains_window(*e)) return e;
+  auto c = std::make_shared<Expr>(*e);
+  if (c->left) c->left = over_window(c->left, ninput, calls);
+  if (c->right) c->right = over_window(c->right, ninput, calls);
+  for (auto& a : c->args) a = over_window(a, ninput, calls);
+  return c;
 }
 }  // namespace
 
@@ -533,6 +602,36 @@ ExprRef SqlToRel::rex(const ASTRef& sql, const Schema& schema, const Scope* scop
     }
     case ASTNode::SQLFunction: {
       const std::string lid = lower(sql->id);
+      if (sql->over) {
+        std::vector<ExprRef> args, part, order;
+        DataType rt = DFGPU_UINT64;
+        if (lid == "row_number" || lid == "rank" || lid == "dense_rank") {
+          if (!sql->args.empty()) fail(DFGPU_ERR_GENERAL, sql->id + "() takes no arguments");
+        } else if (lid == "min" || lid == "max" || lid == "sum" || lid == "avg" || lid == "count") {
+          if (sql->distinct) fail(DFGPU_ERR_NOT_IMPLEMENTED, "COUNT(DISTINCT x) OVER (..) is not supported");
+          if (sql->args.size() != 1) fail(DFGPU_ERR_GENERAL, sql->id + "() OVER (..) takes exactly one argument");
+          const ASTRef& a = sql->args[0];
+          // COUNT(1) / COUNT(*) -> COUNT(first_column), as for the aggregate
+          if (lid == "count" && ((a->kind == ASTNode::SQLLong && a->lval == 1) || a->kind == ASTNode::SQLWildcard)) args.push_back(Expr::column(0));
+          else args.push_back(rex(a, schema, scope));
+          rt = lid == "count" ? DFGPU_UINT64 : lid == "avg" ? DFGPU_FLOAT64 : args[0]->get_type(schema);
+        } else {
+          fail(DFGPU_ERR_GENERAL, "Invalid function '" + sql->id + "'");
+        }
+        for (auto& p : sql->partition_by) part.push_back(rex(p, schema, scope));
+        for (auto& o : sql->window_order) order.push_back(Expr::sort(rex(o.expr, schema, scope), o.asc));
+        for (auto* v : {&args, &part, &order})
+          for (auto& x : *v)
+            if (contains_window(*x)) fail(DFGPU_ERR_GENERAL, "window functions cannot be nested");
+        for (auto* v : {&part, &order})
+          for (auto& x : *v)
+            if (x->get_type(schema) == DFGPU_BOOL)
+              fail(DFGPU_ERR_NOT_IMPLEMENTED, std::string(v == &part ? "PARTITION BY" : "ORDER BY") + " a Boolean key is not supported");
+        return Expr::window(sql->id, args, part, order, rt);
+      }
+      for (auto& a : sql->args)
+        if ((lid == "min" || lid == "max" || lid == "sum" || lid == "avg" || lid == "count") && ast_has_window(a))
+          fail(DFGPU_ERR_GENERAL, "window functions are not allowed in an aggregate argument");
       if (lid == "min" || lid == "max" || lid == "sum" || lid == "avg") {
         std::vector<ExprRef> rex_args;
         for (auto& a : sql->args) rex_args.push_back(rex(a, schema, scope));

@@ -92,6 +92,8 @@ def lib():
     L.dfgpu_join_free.argtypes = [vp]
     L.dfgpu_sort.argtypes = [vp, vp, PI, C.c_int, C.POINTER(PI), PC, C.POINTER(C.c_int32), C.c_int, C.c_int64, C.POINTER(vp)]
     L.dfgpu_result_as_batch.argtypes = [vp, C.POINTER(vp)]
+    L.dfgpu_window.argtypes = [vp, vp, C.POINTER(PI), PC, C.c_int, C.POINTER(PI), PC, C.POINTER(C.c_int32), C.c_int, C.POINTER(A.Agg), C.c_int,
+                               C.POINTER(vp)]
     if L.dfgpu_abi_version() != A.ABI_VERSION:
         raise RuntimeError("libdfgpu.so ABI version mismatch")
     _LIB = L
@@ -405,6 +407,22 @@ class GpuContext:
         finally:
             if view is not None:
                 view.free()
+
+    # -- window functions ----------------------------------------------------------------------------
+    def window(self, batch, fns, partition=(), order=(), desc=None):
+        """dfgpu_window: one column per function of `fns`, each (func, arg expression or None, out_dtype or 0) with func
+        one of A.WIN_ROW_NUMBER / WIN_RANK / WIN_DENSE_RANK (arg None) or A.AGG_MIN / MAX / SUM / COUNT / AVG, over the
+        rows of `batch` partitioned by the expressions `partition` and ordered by `order` (`desc[i]` true: descending),
+        in the batch's row order."""
+        keep = []
+        pptrs, plens, npart = A.make_programs([k.program(batch.schema) for k in partition], keep)
+        optrs, olens, nord = A.make_programs([k.program(batch.schema) for k in order], keep)
+        d = list(desc) if desc is not None else [False] * nord
+        darr = (C.c_int32 * max(1, nord))(*[int(bool(x)) for x in d])
+        farr = A.make_aggs([(f, a.program(batch.schema) if a is not None else [], dt) for f, a, dt in fns], keep)
+        out = C.c_void_p()
+        check(lib().dfgpu_window(self.h, batch.h, pptrs, plens, npart, optrs, olens, darr, nord, farr, len(fns), C.byref(out)))
+        return Result(self, out)
 
     # -- utilities ------------------------------------------------------------------------------
     def sync(self):

@@ -430,6 +430,34 @@ int dfgpu_sort(dfgpu_ctx* ctx, const dfgpu_batch* in, const dfgpu_insn* keep, in
  * result is DFGPU_ERR_GENERAL. */
 int dfgpu_result_as_batch(const dfgpu_result* r, dfgpu_batch** out);
 
+/* ---- window functions: f(args) OVER (PARTITION BY .. ORDER BY ..) ----
+ * The reference has no window functions.  dfgpu_window evaluates the functions of one window specification:
+ *   - Order: rows are ordered by the partition keys `part` (ascending), then by the ORDER BY keys `order` (desc[i] != 0:
+ *     descending; `desc` may be NULL), under dfgpu_sort's rules: nulls first ascending, -0.0 before +0.0, every NaN after
+ *     +inf, Utf8 byte-wise.  Rows that tie keep their input order.  A Boolean key is DFGPU_ERR_NOT_IMPLEMENTED.
+ *   - Partition: rows whose partition keys have equal sort encodings (two nulls share one, all NaNs share one, -0.0 and
+ *     +0.0 do not).  npart 0: the whole input is one partition.  Peers: rows of one partition equal on every ORDER BY key.
+ *   - Frame: with ORDER BY, the partition's rows through the row's last peer (RANGE BETWEEN UNBOUNDED PRECEDING AND
+ *     CURRENT ROW); without, the whole partition.
+ *   - Functions (`fns[k].func`, result column k): DFGPU_WIN_ROW_NUMBER (1 + the row's position in its partition),
+ *     DFGPU_WIN_RANK (1 + the rows of the partition before the row's first peer), DFGPU_WIN_DENSE_RANK (1 + the peer groups
+ *     before the row's), all UInt64 with `arg` unused; DFGPU_AGG_COUNT (UInt64, the valid values of the frame) and
+ *     DFGPU_AGG_SUM / MIN / MAX (the argument's type) / AVG (Float64) over the valid values of the frame, with the
+ *     aggregates' value rules (integer SUM wraps at its width; MIN / MAX with -0.0 < +0.0, NaN skipped unless every value
+ *     is NaN).  A frame without a valid value is null, except for COUNT (0).  Float SUM / AVG add in an order fixed by
+ *     the input alone, so they give the same bits on every run and on any number of ranks.  DFGPU_AGG_COUNT_DISTINCT
+ *     is DFGPU_ERR_NOT_IMPLEMENTED; a non-numeric argument and `out_dtype` are refused as dfgpu_aggregate_create does.
+ *   - Output: one column per function, one row per input row, in `in`'s row order.  Key and argument programs that are
+ *     not a plain column are evaluated first exactly as a projection without a WHERE (dfgpu_filter_project).
+ *   - An input of 2^32 rows or more is DFGPU_ERR_NOT_IMPLEMENTED.
+ * With a communicator attached the specification runs over the rank-ordered concatenation of every rank's `in` (each
+ * rank all-gathers the key and argument columns), and the result holds this rank's rows only.  Every rank must call it,
+ * a rank without rows with an empty batch of the same columns. */
+enum { DFGPU_WIN_ROW_NUMBER = 16, DFGPU_WIN_RANK = 17, DFGPU_WIN_DENSE_RANK = 18 };
+int dfgpu_window(dfgpu_ctx* ctx, const dfgpu_batch* in, const dfgpu_insn* const* part, const int* part_len, int npart,
+                 const dfgpu_insn* const* order, const int* order_len, const int32_t* desc, int norder,
+                 const dfgpu_agg* fns, int nfns, dfgpu_result** out);
+
 /* ---- results ---- */
 int dfgpu_result_shape(const dfgpu_result* r, int64_t* nrows, int* ncols);
 int dfgpu_result_col_dtype(const dfgpu_result* r, int i, int32_t* dtype);

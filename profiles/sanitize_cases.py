@@ -269,5 +269,15 @@ for n in [1, 33, 4097, 100_003]:
     assert r.nrows == min(n // 2, int(np.count_nonzero((np.arange(n) % 5 != 0) & (np.arange(n) % 7 != 0)))), n
     r.free(); b.free()
 print("sort ok", flush=True)
+# 15. window functions (dfgpu_window): the segmented scan's ragged last tile, a nullable Utf8 partition key, one row,
+# and the rank, MIN / AVG and integer SUM outputs of a partial validity word
+for n in [1, 33, 2049, 100_003]:
+    ks = pa.array(["k%d" % (i % 37) for i in range(n)], type=pa.string(), mask=np.arange(n) % 11 == 0)
+    b = ctx.upload([ks, rng.integers(0, 300, n, dtype=np.int64), pa.array(rng.standard_normal(n), mask=np.arange(n) % 5 == 0)])
+    r = ctx.window(b, [(A.WIN_RANK, None, 0), (A.AGG_MIN, col(2), 0), (A.AGG_AVG, col(2), 0), (A.AGG_SUM, col(1), 0)], partition=[col(0)],
+                   order=[col(1)], desc=[True])
+    assert r.nrows == n, n
+    r.free(); b.free()
+print("window ok", flush=True)
 ctx.close()
 print("SANITIZE_CASES_OK")

@@ -184,6 +184,14 @@ extern "C" {
         ctx: *mut dfgpu_ctx, input: *const dfgpu_batch, keep: *const dfgpu_insn, keep_len: c_int, keys: *const *const dfgpu_insn,
         key_len: *const c_int, desc: *const i32, nkeys: c_int, limit: i64, out: *mut *mut dfgpu_result,
     ) -> c_int;
+    /// window functions of one specification (no reference counterpart): rows partitioned by `part`, ordered by `order`
+    /// (desc[i] != 0: descending); one result column per `fns` entry (func = DFGPU_WIN_* or DFGPU_AGG_*), in input row
+    /// order; with a communicator, over every rank's rows in rank order, returning this rank's rows
+    pub fn dfgpu_window(
+        ctx: *mut dfgpu_ctx, input: *const dfgpu_batch, part: *const *const dfgpu_insn, part_len: *const c_int, npart: c_int,
+        order: *const *const dfgpu_insn, order_len: *const c_int, desc: *const i32, norder: c_int, fns: *const dfgpu_agg, nfns: c_int,
+        out: *mut *mut dfgpu_result,
+    ) -> c_int;
     /// a batch viewing a device result's columns (free it before the result)
     pub fn dfgpu_result_as_batch(r: *const dfgpu_result, out: *mut *mut dfgpu_batch) -> c_int;
     pub fn dfgpu_result_shape(r: *const dfgpu_result, nrows: *mut i64, ncols: *mut c_int) -> c_int;
