@@ -2268,8 +2268,10 @@ Kernel<AggParams, SetParams> choose_insert(const AggParams& p, bool plain_ok) {
 
 // One round of the insert over the rows p describes, then the growth rule of the sets: each set that refused pairs at
 // its fill limit, or went past it, grows x4; when rows were refused and no set grew, the probe limit refused them below
-// the fill limit, and every set grows.  Returns the number of rows refused.
-long long insert_round(dfgpu_aggstate* st, AggParams& p, bool plain) {
+// the fill limit, and every set grows.  As for the group table (scan_round), that happens at most once per batch
+// (*probe_grown): pairs whose hashes share their top bits share a home at every capacity.  Returns the number of rows
+// refused.
+long long insert_round(dfgpu_aggstate* st, AggParams& p, bool plain, bool* probe_grown) {
   const int nsets = int(st->dist_progs.size());
   const Kernel<AggParams, SetParams> k = choose_insert(p, plain);
   SetParams sp;
@@ -2293,6 +2295,12 @@ long long insert_round(dfgpu_aggstate* st, AggParams& p, bool plain) {
     const long long n = (long long)c[DCTR_SET + 2 * s];
     grow[s] = (novf > 0 && n >= sp.max_fill[s]) || n > fill_limit(sp.set[s].cap);  // refused pairs at its fill limit, or past it
     any = any || grow[s];
+  }
+  if (novf > 0 && !any) {
+    if (*probe_grown)
+      fail(DFGPU_ERR_NOT_IMPLEMENTED, "COUNT(DISTINCT) pairs whose hashes share one home slot: more than the probe limit of " +
+                                          std::to_string(AG_MAX_PROBE) + " pairs on one probe chain");
+    *probe_grown = true;
   }
   for (int s = 0; s < nsets; s++)
     if (grow[s] || (novf > 0 && !any)) set_grow(st, s, grown_cap(sp.set[s].cap));
@@ -2523,7 +2531,12 @@ struct GrowAndReplay {
 // One round of the group scan over the rows p describes, then the growth rule of the table: x4 when it went past its
 // fill limit, or when it refused rows -- except when each of them only met a slot that was still being published
 // (counter CTR_DEFERRED, which only wide scans set): those are replayed as they are.  Returns the number of rows refused.
-long long scan_round(dfgpu_aggstate* st, AggParams& p, const ScanPlan& plan, Trace& tr, bool prefix) {
+//
+// Rows refused while the table is below the round's own fill limit met the probe limit: AG_MAX_PROBE occupied slots
+// after their home.  Growth spreads a cluster of ordinary keys, but keys whose hashes share their top bits share a
+// home at every capacity, and growing again would only multiply the table until allocation fails.  So a batch grows
+// at most once for that reason (*probe_grown); the next such round fails.
+long long scan_round(dfgpu_aggstate* st, AggParams& p, const ScanPlan& plan, Trace& tr, bool prefix, bool* probe_grown) {
   dfgpu_ctx* ctx = st->ctx;
   const bool replay = p.row_list != nullptr;
   p.t = st->t;
@@ -2553,6 +2566,13 @@ long long scan_round(dfgpu_aggstate* st, AggParams& p, const ScanPlan& plan, Tra
   const long long novf = (long long)c[CTR_OVERFLOW], deferred = (long long)c[CTR_DEFERRED];
   if (deferred) DF_CUDA(cudaMemsetAsync(st->d_counters + CTR_DEFERRED, 0, 8, ctx->stream));
   tr.mark(prefix ? "scan kernel (prefix)" : "scan kernel");
+  // a row refused for the fill limit read a group count >= max_groups, which only grows: below it, no row was
+  if (novf > deferred && st->ngroups < p.max_groups) {
+    if (*probe_grown)
+      fail(DFGPU_ERR_NOT_IMPLEMENTED, "GROUP BY keys whose hashes share one home slot: more than the probe limit of " +
+                                          std::to_string(AG_MAX_PROBE) + " keys on one probe chain");
+    *probe_grown = true;
+  }
   if (st->ngroups > fill_limit(st->t.cap) || (novf > 0 && novf != deferred)) {
     table_grow(st, grown_cap(st->t.cap));
     if (novf == 0) tr.mark("table_grow (load factor)");
@@ -2654,16 +2674,17 @@ void agg_update(dfgpu_aggstate* st, const dfgpu_batch* batch) {
   GrowAndReplay loop(ctx, batch->nrows);
   tr.mark("overflow list alloc");
   const auto ranges = batch_ranges(st, batch->nrows);
+  bool table_probe_grown = false, set_probe_grown = false;  // growth for the probe limit, once per batch
   for (size_t ri = 0; ri < ranges.size(); ri++) {
     const long long begin = ranges[ri].first, count = ranges[ri].second;
     const bool prefix = ranges.size() > 1 && ri == 0;
     if (group_by)
       loop.run(p, st->d_counters + CTR_OVERFLOW, begin, count, "hash table growth did not converge",
-               [&] { return scan_round(st, p, plan, tr, prefix); });
+               [&] { return scan_round(st, p, plan, tr, prefix, &table_probe_grown); });
     // after the group scan of the same rows: every key the insert packs is in the table
     if (distinct)
       loop.run(ins, st->d_dctr + DCTR_OVERFLOW, begin, count, "COUNT(DISTINCT) set growth did not converge",
-               [&] { return insert_round(st, ins, ins_plain); });
+               [&] { return insert_round(st, ins, ins_plain, &set_probe_grown); });
     // few groups so far: later rows of this stream go through the shared-memory front table
     if (group_by) st->use_front = st->ngroups <= AG_FRONT_MAX_GROUPS && st->rows_seen >= (1ll << 20);
     if (prefix) size_from_prefix(st, batch->nrows, tr);

@@ -67,10 +67,11 @@ def mix64(x):
 
 
 def owner_of(keys, world):
-    """Owner rank of every packed 64-bit group key (aggregate.cu owner_of): hash bits the table slot does
-    not use; the key that equals the empty marker belongs to rank 0."""
+    """Owner rank of every packed 64-bit group key, as aggregate.cu owner_of computes it: the low 32 bits of
+    mix64(key), which a table of up to 2^32 slots does not use for the home slot, modulo the world size; the key that
+    equals the empty marker belongs to rank 0."""
     k = np.asarray(keys).view(np.uint64) if np.asarray(keys).dtype.itemsize == 8 else np.asarray(keys).astype(np.int64).view(np.uint64)
-    own = ((mix64(k) >> np.uint64(44)) % np.uint64(world)).astype(np.int64)
+    own = ((mix64(k) & np.uint64(0xffffffff)) % np.uint64(world)).astype(np.int64)
     own[k == np.uint64(0xFFFFFFFFFFFFFFFF)] = 0
     return own
 

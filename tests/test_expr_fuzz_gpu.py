@@ -25,7 +25,8 @@ from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine
 from datafusion_archive_b200.expr import AggregateFunction, Case, col, fn, lit
 from kernel_trace import traced_set
-from test_join_gpu import gpu_pairs, ref_join, same_pairs
+from join_ref import inner as ref_join, same_pairs
+from test_join_gpu import gpu_pairs
 from test_scalar_fn_gpu import within_ulps
 
 pytestmark = pytest.mark.gpu

@@ -1,5 +1,5 @@
-"""Inner equi-join on the GPU (dfgpu_join_build / dfgpu_join_probe and JOIN through ctx.sql()), compared with an
-exact numpy join written here.  Rows are compared as sorted multisets: the order of one probe row's matches is
+"""Inner equi-join on the GPU (dfgpu_join_build / dfgpu_join_probe and JOIN through ctx.sql()), compared with the
+exact join of tests/join_ref.py.  Rows are compared as sorted multisets: the order of one probe row's matches is
 unspecified."""
 import numpy as np
 import pyarrow as pa
@@ -8,6 +8,7 @@ import pytest
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
 from datafusion_archive_b200.expr import col, lit
+from join_ref import inner as ref_join, same_pairs
 
 pytestmark = pytest.mark.gpu
 
@@ -33,33 +34,6 @@ def values_of(a, dtype=None):
     return np.asarray(a, dtype=dtype)
 
 
-def ref_join(pkeys, bkeys):
-    """(probe rows, build rows) of every matching pair: keys equal part by part, null keys never match."""
-    n_p, n_b = len(pkeys[0]), len(bkeys[0])
-    pv = np.logical_and.reduce([valid_of(k) for k in pkeys]) if n_p else np.zeros(0, bool)
-    bv = np.logical_and.reduce([valid_of(k) for k in bkeys]) if n_b else np.zeros(0, bool)
-    parts = []
-    for pk, bk in zip(pkeys, bkeys):
-        parts.append(np.concatenate([values_of(pk, np.int64 if values_of(pk).dtype.kind == "i" else np.uint64),
-                                     values_of(bk, np.int64 if values_of(bk).dtype.kind == "i" else np.uint64)]))
-    rec = np.rec.fromarrays(parts) if parts[0].size else None
-    if rec is None:
-        return np.zeros(0, np.int64), np.zeros(0, np.int64)
-    _, ids = np.unique(rec, return_inverse=True)
-    ids = ids.reshape(-1)
-    pid, bid = ids[:n_p], ids[n_p:]
-    brows = np.nonzero(bv)[0]
-    order = np.argsort(bid[brows], kind="stable")
-    sorted_ids, sorted_rows = bid[brows][order], brows[order]
-    lo = np.searchsorted(sorted_ids, pid, "left")
-    hi = np.searchsorted(sorted_ids, pid, "right")
-    cnt = np.where(pv, hi - lo, 0)
-    total = int(cnt.sum())
-    prow = np.repeat(np.arange(n_p), cnt)
-    first = np.repeat(lo, cnt) + (np.arange(total) - np.repeat(np.cumsum(cnt) - cnt, cnt))
-    return prow, sorted_rows[first]
-
-
 def gpu_pairs(ctx, probe_arrays, pkeys, build_arrays, bkeys):
     """Join with a row-number column appended to each side; returns (probe rows, build rows)."""
     pa_ = list(probe_arrays) + [np.arange(len(values_of(probe_arrays[0])), dtype=np.int64)]
@@ -71,14 +45,6 @@ def gpu_pairs(ctx, probe_arrays, pkeys, build_arrays, bkeys):
     got = r.columns()
     r.free(); j.free(); pb.free()
     return got[0], got[1]
-
-
-def same_pairs(got, exp):
-    g = np.lexsort((got[1], got[0]))
-    e = np.lexsort((exp[1], exp[0]))
-    assert len(got[0]) == len(exp[0])
-    assert np.array_equal(np.asarray(got[0])[g], np.asarray(exp[0])[e])
-    assert np.array_equal(np.asarray(got[1])[g], np.asarray(exp[1])[e])
 
 
 def nullable(vals, valid, dtype):

@@ -1,5 +1,5 @@
 """Inner equi-join on keys with Utf8 parts, alone or mixed with integer parts (dfgpu_join_build / dfgpu_join_probe and
-JOIN through ctx.sql()), compared with an exact numpy join written here.  Utf8 parts compare byte for byte, a null part
+JOIN through ctx.sql()), compared with the exact join of tests/join_ref.py.  Utf8 parts compare byte for byte, a null part
 never matches, and two keys that share a hash tag must not match: DFGPU_JOIN_TAG_BITS cuts the tag to force that.
 Rows are compared as sorted multisets: the order of one probe row's matches is unspecified."""
 import time
@@ -12,6 +12,7 @@ import pytest
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
 from datafusion_archive_b200.expr import col, utf8_fn
+from join_ref import inner as ref_join, same_pairs
 
 pytestmark = pytest.mark.gpu
 
@@ -27,43 +28,6 @@ def as_arrow(a):
     return a if isinstance(a, pa.Array) else pa.array(a)
 
 
-def codes(p, b):
-    """Equal values of a key part get equal int64 codes across both sides; (probe codes, probe valid, build codes, build valid)."""
-    p, b = as_arrow(p), as_arrow(b)
-    both = pa.chunked_array([p, b], type=p.type).combine_chunks()
-    enc = pc.dictionary_encode(both)
-    idx = np.asarray(enc.indices.fill_null(0).to_numpy(zero_copy_only=False), dtype=np.int64)
-    valid = np.asarray(both.is_valid())
-    return idx[:len(p)], valid[:len(p)], idx[len(p):], valid[len(p):]
-
-
-def ref_join(pkeys, bkeys):
-    """(probe rows, build rows) of every matching pair: every part equal, null parts never match."""
-    n_p, n_b = len(pkeys[0]), len(bkeys[0])
-    pv, bv = np.ones(n_p, bool), np.ones(n_b, bool)
-    parts = []
-    for pk, bk in zip(pkeys, bkeys):
-        pcode, pval, bcode, bval = codes(pk, bk)
-        pv &= pval
-        bv &= bval
-        parts.append(np.concatenate([pcode, bcode]))
-    if n_p == 0 or n_b == 0:
-        return np.zeros(0, np.int64), np.zeros(0, np.int64)
-    _, ids = np.unique(np.rec.fromarrays(parts), return_inverse=True)
-    ids = ids.reshape(-1)
-    pid, bid = ids[:n_p], ids[n_p:]
-    brows = np.nonzero(bv)[0]
-    order = np.argsort(bid[brows], kind="stable")
-    sorted_ids, sorted_rows = bid[brows][order], brows[order]
-    lo = np.searchsorted(sorted_ids, pid, "left")
-    hi = np.searchsorted(sorted_ids, pid, "right")
-    cnt = np.where(pv, hi - lo, 0)
-    total = int(cnt.sum())
-    prow = np.repeat(np.arange(n_p), cnt)
-    first = np.repeat(lo, cnt) + (np.arange(total) - np.repeat(np.cumsum(cnt) - cnt, cnt))
-    return prow, sorted_rows[first]
-
-
 def gpu_pairs(ctx, probe_arrays, pkeys, build_arrays, bkeys):
     """Join with a row-number column appended to each side; returns (probe rows, build rows)."""
     pa_ = list(probe_arrays) + [np.arange(len(probe_arrays[0]), dtype=np.int64)]
@@ -75,14 +39,6 @@ def gpu_pairs(ctx, probe_arrays, pkeys, build_arrays, bkeys):
     got = r.columns()
     r.free(); j.free(); pb.free()
     return got[0], got[1]
-
-
-def same_pairs(got, exp):
-    g = np.lexsort((got[1], got[0]))
-    e = np.lexsort((exp[1], exp[0]))
-    assert len(got[0]) == len(exp[0])
-    assert np.array_equal(np.asarray(got[0])[g], np.asarray(exp[0])[e])
-    assert np.array_equal(np.asarray(got[1])[g], np.asarray(exp[1])[e])
 
 
 def check(ctx, probe, pkeys, build, bkeys, ref_p=None, ref_b=None):

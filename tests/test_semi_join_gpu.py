@@ -1,5 +1,5 @@
 """Semi and anti joins on the GPU (dfgpu_join_semi, and [NOT] IN / [NOT] EXISTS subqueries through ctx.sql()), compared
-exactly with a Python reference of include/dfgpu.h's table: the passing probe rows, in probe order."""
+exactly with tests/join_ref.py, the reference of include/dfgpu.h's table: the passing probe rows, in probe order."""
 import os
 
 import numpy as np
@@ -9,6 +9,7 @@ import pytest
 from datafusion_archive_b200 import _abi as A
 from datafusion_archive_b200 import engine, host
 from datafusion_archive_b200.expr import col, lit
+from join_ref import passing
 
 pytestmark = pytest.mark.gpu
 
@@ -21,31 +22,6 @@ def ctx():
     c = engine.GpuContext(0)
     yield c
     c.close()
-
-
-def py_rows(arrays):
-    """the key tuples of each row, None for a null part"""
-    cols = [a.to_pylist() if isinstance(a, (pa.Array, pa.ChunkedArray)) else np.asarray(a).tolist() for a in arrays]
-    return list(zip(*cols)) if cols and len(cols[0]) else []
-
-
-def ref_pass(kind, pkeys, bkeys, n_probe):
-    """the probe rows that pass, per the semantics table of dfgpu_join_semi"""
-    build = py_rows(bkeys)
-    keys = {r for r in build if None not in r}
-    has_null = any(None in r for r in build)
-    out = []
-    for i, r in enumerate(py_rows(pkeys) if n_probe else []):
-        null = None in r
-        if kind == A.JOIN_SEMI:
-            ok = not null and r in keys
-        elif kind == A.JOIN_ANTI:
-            ok = null or r not in keys
-        else:
-            ok = not build or (not has_null and not null and r not in keys)
-        if ok:
-            out.append(i)
-    return np.array(out, dtype=np.int64)
 
 
 def gpu_pass(ctx, kind, probe_arrays, pkeys, build_arrays, bkeys):
@@ -62,7 +38,7 @@ def gpu_pass(ctx, kind, probe_arrays, pkeys, build_arrays, bkeys):
 
 
 def check(ctx, kind, probe, pkeys, build, bkeys, pref=None, bref=None):
-    exp = ref_pass(kind, pref if pref is not None else probe, bref if bref is not None else build, len(probe[0]))
+    exp = passing(kind, pref if pref is not None else probe, bref if bref is not None else build)
     got = gpu_pass(ctx, kind, probe, pkeys, build, bkeys)
     assert np.array_equal(got, exp), (len(got), len(exp))
 
@@ -164,7 +140,7 @@ def test_payload_columns_keep_validity(ctx):
         r = j.semi(pb, [col(0)], kind, probe_cols=[3, 1, 2, 0])
         got = r.columns()
         r.free()
-        sel = ref_pass(kind, [pk], [bk], n)
+        sel = passing(kind, [pk], [bk])
         assert np.array_equal(got[3], pk[sel])
         for g, a in zip(got[:3], (strs, f64, bools)):
             vals, valid = g if isinstance(g, tuple) else (g, np.ones(len(sel), bool))
